@@ -1,4 +1,4 @@
-"""diffusiondepth_b200 — B200-native (sm_100a) engine for the DiffusionDepth hot path.
+"""diffusiondepth_b200 — H100-native (sm_90a) engine for the DiffusionDepth hot path.
 
 Hot path = the T-step DDIM denoising loop over the 16-channel depth latent + the depth-latent decoder
 (reference: duanyiqun/DiffusionDepth src/model/head/ddim_depth_estimate_res_swin_addHAHI.py:254-303,

@@ -83,7 +83,7 @@ def load_library():
     if not os.path.exists(path):
         raise EngineError(
             f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU/PyTorch fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU/PyTorch fallback.")
     lib = C.CDLL(path)
     for name, (res, args) in SIGNATURES.items():
         try:

@@ -1,122 +1,82 @@
-// 3x3 / stride 1 / pad 1 convolution on tcgen05 with ROW-HALO REUSE of the activation operand.
+// 3x3 / stride 1 / pad 1 convolution as an implicit GEMM on Hopper's warpgroup MMA (wgmma), with ROW-HALO REUSE of
+// the activation operand.
 //
-// Measurement (profiles/README.md, round 1): every conv of the DDIM loop moves ~48 KB of operands from L2 into
-// shared memory per pipeline stage and all of them run at the same ~0.7-0.9 us per stage, i.e. they sit on the
-// chip's L2->SM (TMA) bandwidth, not on the tensor pipe.  conv3x3_umma_kernel re-fetches the 128-pixel activation
-// patch once per tap (9x).  Here the output tile is 16 rows x 8 columns and, per 32-channel chunk, the producer
-// fetches three [18 rows][8 cols] column-shifted strips (dx = -1, 0, +1).  For tap (dy, dx) the A operand is strip
-// dx starting dy rows down: its 8-pixel row groups are dense and aligned to the swizzle repeat, so the canonical
-// K-major UMMA descriptor (SBO = 8 rows) addresses it with no copy.  A traffic drops 9 x 128 -> 3 x 144 pixel rows
-// per chunk (2.67x), total L2->SM bytes by 20 % (256->256) to 41 % (256->64).
+//   M = 128 output pixels (a 16-row x 8-column patch of one image), N = COUT, K = 9 taps x CIN.
 //
-// Two TMA rings: A strips (one slot per channel chunk, consumed by 9 taps) and B weight tiles (one slot per
-// (chunk, tap)).  Everything else (3-pass fp16 split, TMEM double buffer, warp roles, epilogues) is as in
-// conv_umma.cuh.  Replaces the same reference lines (ScheduledCNNRefine convs, head :339-359, :321-333).
+// Operands are fp16 hi/lo planes of the fp32 tensors (x = hi + lo, each scaled by a power of two), and every K step
+// issues three MMAs  D += A_lo*B_hi ; D += A_hi*B_hi ; D += A_hi*B_lo  so the fp32 accumulator carries ~22
+// significant bits per product (SURVEY.md §7.2-1: a single fp16/tf32 pass misses the 1e-3 parity bar after 20 DDIM
+// steps, the 3-pass split matches fp32).
+//
+// Row-halo reuse: per channel chunk the producer fetches three [18 rows][8 cols] column-shifted strips (dx = -1, 0,
+// +1) with one 4-D TMA tensor map {C, W, H, B} (TMA's out-of-bounds zero fill *is* the conv's zero padding).  For tap
+// (dy, dx) the A operand is strip dx starting dy rows down: its 8-pixel row groups are dense and aligned to the
+// swizzle atom, so the canonical K-major wgmma descriptor (SBO = 8 rows) addresses it with no copy.  The activation
+// bytes moved per chunk drop from 9 x 128 to 3 x 144 pixel rows.  Weights are pre-packed [tap][COUT][CIN] fp16 hi/lo
+// and fetched by a 3-D map with box {BK, COUT, 1}.
+//
+// Roles: warpgroup 0 = producers (warp 0: A strips, warp 1: B weight tiles; one elected lane issues the copies),
+// warpgroups 1 .. NWG = consumers.  Consumer warpgroup w owns all 128 pixels of the tile and output channels
+// [w NW, (w + 1) NW) as two 64-row wgmma accumulators in registers; after the K loop it drains them chunk by chunk
+// through a shared-memory staging tile so that thread t holds row (pixel) t of the chunk for the epilogue (bias,
+// GroupNorm partial sums, fp32 / split-plane stores).
+// Replaces: the nn.Conv2d calls inside ScheduledCNNRefine (reference
+// src/model/head/ddim_depth_estimate_res_swin_addHAHI.py:339-359, UpSample_add :321-333).
 #pragma once
-#include "conv_umma.cuh"
+#include "conv_common.cuh"
 
 namespace dd {
 
 constexpr int HALO_TH = 16;  // output tile: 16 rows x 8 columns = 128 pixels
 constexpr int HALO_TW = 8;
 
-// PAIR = true: two CTAs of one cluster (one TPC) run ONE tcgen05.mma.cta_group::2 with M = 256: each CTA stages its own
-// 128-pixel strips (A) and HALF of the weight tile (COUT/2 rows of B); the hardware feeds both tensor cores from the two
-// halves, so per SM the weight tile is written to and read from shared memory half as often.  Measured motivation
-// (profiles/README.md): the single-CTA kernel moves ~110 KB through each SM's shared-memory port per (chunk, tap) stage
-// = ~860 cycles at 128 B/clk, above the 768 cycles of tensor work -> it is shared-memory-port bound.
-// F8 = true (PAIR only): FP8 CORRECTION PRODUCTS.  The operand planes are hi = fp16(s x), a8 = e4m3(s x / 4) and
-// l8 = e4m3((s x - hi) * 512) (weights: hi = fp16(t w), w8 = e4m3(t w / 512), lw8 = e4m3((t w - hi) * 4)), and per
-// 32 channels the issuer sends  D += l8 * w8 ; D += a8 * lw8  (kind::f8f6f4, K = 32 each; the power-of-two scales
-// cancel: 512 / 512 = 1, 4 / 4 = 1)  and  D += hi * hi  (kind::f16, 2 x K = 16)  into the ONE fp32 accumulator: 4 MMAs
-// of 2 pass-equivalents instead of 6 MMAs of 3.  The F8 mainloop works on 64-CHANNEL chunks (BK = 64): fp16 rows of
-// 128 B (128-byte swizzle), e4m3 rows of 64 B (64-byte swizzle) — with 32-channel chunks the e4m3 rows are 32 B and both
-// TMA and the MMA operand fetch run well below their rate on such rows (first version: 816 us, this layout's probe:
-// 629 us) — and its A ring is dx-granular: a unit = the three planes of ONE column-shifted strip (36 KB), consumed by
-// that dx's three taps, so three units and three 32 KB weight stages fit beside each other.  Measured (profiles/README.md round 2): on CTA pairs a K = 32 e4m3 MMA
-// costs ~175 cycles against 2 x 128 for the same K in fp16 (single CTA: 260 — it needs cta_group::2), and under the
-// 1 kW power cap the clock rises with the lighter MMA mix: 256->256 at C3 629 us vs 948 us (3 fp16 passes on pairs)
-// vs 1119 us (round 1).  Parity cost (oracle/probe_fp8_static.py, real C3 case vs the reference golden): max |dz|
-// 3.4e-4 / rms 7e-5 instead of 2.3e-5 / 4.5e-6, tolerance 1e-3.  Same bytes per element in HBM (2 + 1 + 1).
-template <int CIN, int COUT, int BK, bool PAIR = false, bool F8 = false>
+template <int CIN, int COUT, int BK>
 struct HaloCfg {
-  static_assert(!F8 || (PAIR && BK == 64 && COUT == 256 && CIN % 64 == 0), "fp8 corrections: pair kernel, 64-channel chunks, wide layers");
-  static_assert(F8 || BK == 16 || BK == 32, "bad K chunk");
+  static_assert(BK == 16 || BK == 32, "bad K chunk");
   static_assert((CIN % BK == 0 || CIN < BK) && CIN % 16 == 0, "bad K chunk");
-  // CIN < BK (16-channel latent, BK = 32) is supported — the box is wider than the channel extent, TMA zero-fills the
-  // rest and only CIN / 16 K-steps are issued — but measured slower on 16->64 (110 vs 82 us), so the engine keeps BK = 16.
   static constexpr int KC = (CIN + BK - 1) / BK;
   static constexpr int KSTEPS = (CIN < BK ? CIN : BK) / 16;
   static constexpr int ROW_BYTES = BK * 2;
   static constexpr int STRIP_ROWS = (HALO_TH + 2) * HALO_TW;        // 144 pixel rows
   static constexpr int STRIP_BYTES = STRIP_ROWS * ROW_BYTES;        // one plane, one dx
   static constexpr int STRIP_PAD = (STRIP_BYTES + 1023) / 1024 * 1024;
-  static constexpr int STRIP8_BYTES = STRIP_ROWS * BK;              // e4m3 plane: one byte per channel
-  static constexpr int STRIP8_PAD = (STRIP8_BYTES + 1023) / 1024 * 1024;
-  static constexpr int DX_STRIDE = F8 ? STRIP_PAD + 2 * STRIP8_PAD : 2 * STRIP_PAD;  // planes of one dx: hi, lo | hi, a8, l8
-  static constexpr int A_SLOT = F8 ? DX_STRIDE : 3 * DX_STRIDE;       // F8: one dx per ring unit
-  static constexpr int B_ROWS = PAIR ? COUT / 2 : COUT;             // weight rows this CTA stages
-  static constexpr int B_TILE = B_ROWS * ROW_BYTES;                 // one plane, one tap, one chunk
+  static constexpr int DX_STRIDE = 2 * STRIP_PAD;                   // planes of one dx: hi, lo
+  static constexpr int A_SLOT = 3 * DX_STRIDE;
+  static constexpr int A_SLOTS = 2;
+  static constexpr int B_TILE = COUT * ROW_BYTES;                   // one plane, one tap, one chunk
   static constexpr int B_TILE_PAD = (B_TILE + 1023) / 1024 * 1024;
-  static constexpr int B8_TILE = B_ROWS * BK;
-  static constexpr int B8_TILE_PAD = (B8_TILE + 1023) / 1024 * 1024;
-  static constexpr int B_SLOT = F8 ? B_TILE_PAD + 2 * B8_TILE_PAD : 2 * B_TILE_PAD;
-  // F8 with ONE chunk per tile (64 -> 256, K = 576: the epilogue is on the critical path, so it keeps the transposed
-  // coalesced fp32 store and its staging tiles): two strip units instead of three make room for them
-  static constexpr bool F8_NARROW_K = F8 && CIN == 64;
-  static constexpr int A_SLOTS = F8 ? (F8_NARROW_K ? 2 : 3) : 2;
-  // Two sets of four epilogue warps where the epilogue is on the critical path: Cout = 64 (two chunks, one per set; each
-  // set then owns two GroupNorm groups) and the pair kernel's 64->256 layer (K = 576: 18 stages per tile, so draining a
-  // 128 x 256 fp32 tile with one warp per scheduler took as long as the mainloop; the sets take alternate chunks and
-  // each holds partial sums of all four groups).
-  // F8_NARROW_K (64 -> 256 with fp8 corrections: nine stages of 2 pass-equivalents per tile): FOUR sets on 16-column
-  // chunks (16 epilogue warps, <= 96 registers).  ncu with two sets: tensor pipe 62 % active, issue-active 41 % with two
-  // epilogue warps per scheduler stalled on their own TMEM / shared-memory latencies — the drain of a 128 x 256 fp32
-  // tile, not the mainloop, set the tile rate.
-#ifdef DD_NE3_EPI8  // A/B build of profiles/README.md (session 2): the two-set epilogue on 32-column chunks
-  static constexpr bool F8_EPI16 = false;
-#else
-  static constexpr bool F8_EPI16 = F8_NARROW_K;
-#endif
-  static constexpr int EPI_SETS = F8_EPI16 ? 4 : ((COUT == 64 || PAIR) ? 2 : 1);
-  static constexpr bool STATS_LOCAL = (COUT == 64);  // a set's chunk(s) cover whole groups of their own
-  static constexpr int EPI_WARPS = 4 * EPI_SETS;
-  static constexpr int THREADS = 128 + 32 * EPI_WARPS;
-  static constexpr int CH = COUT < 32 ? COUT : (F8_EPI16 ? 16 : 32);  // accumulator columns per epilogue chunk
-  static constexpr int XPOSE_BYTES = (F8 && !F8_NARROW_K) ? 0 : EPI_WARPS * 32 * CH * 4;  // F8 256 -> 256: fp32 outputs (tests) store row-wise
-  static constexpr int CTRL_BYTES = EPI_WARPS > 8 ? 2048 : 1024;  // barriers, TMEM slot, GroupNorm partials [2][EPI_WARPS][4][2]
-  static constexpr int BUDGET = 227 * 1024 - 1024 - CTRL_BYTES - XPOSE_BYTES - A_SLOTS * A_SLOT;
+  static constexpr int B_SLOT = 2 * B_TILE_PAD;
+  // consumer warpgroups: a 64 x NW fp32 accumulator takes NW / 2 registers per thread, two of them (128 rows) NW
+  static constexpr int NWG = COUT > 128 ? 2 : 1;
+  static constexpr int NW = COUT / NWG;
+  static constexpr int THREADS = 128 * (1 + NWG);
+  static constexpr int CH = NW < 32 ? NW : 32;           // accumulator columns per epilogue chunk
+  static constexpr int LD = CH + 1;                                  // staging row stride (floats): conflict-free rows
+  static constexpr int STAGE_BYTES = NWG * 128 * LD * 4;
+  static constexpr int CTRL_BYTES = 1024;  // barriers, GroupNorm partials [2][4 NWG][4][2]
+  static constexpr int BUDGET = 227 * 1024 - 1024 - CTRL_BYTES - STAGE_BYTES - A_SLOTS * A_SLOT;
   static constexpr int B_SLOTS_RAW = BUDGET / B_SLOT;
-  // Small layers (16->64, 64->16): all 9 x KC weight tiles fit in shared memory -> fetch them ONCE per CTA instead of once
-  // per tile.  Each cp.async.bulk.tensor costs its issuing thread ~160 ns, and 18 weight copies per 128-pixel tile were
-  // the whole tile time of the 16->64 layer (tensor pipe 12.5 % active).
-  static constexpr bool B_RESIDENT = !PAIR && (9 * KC * B_SLOT <= 40 * 1024) && (9 * KC <= B_SLOTS_RAW);
-  static constexpr int B_SLOTS = B_RESIDENT ? 9 * KC : (F8 ? 3 : (B_SLOTS_RAW > 8 ? 8 : B_SLOTS_RAW));
-  static_assert(!F8 || B_SLOTS_RAW >= 3, "fp8 layout does not fit");
+  // Small layers (16->64, 64->16): all 9 x KC weight tiles fit in shared memory -> fetch them ONCE per CTA instead of
+  // once per tile.
+  static constexpr bool B_RESIDENT = (9 * KC * B_SLOT <= 40 * 1024) && (9 * KC <= B_SLOTS_RAW);
+  static constexpr int B_SLOTS = B_RESIDENT ? 9 * KC : (B_SLOTS_RAW > 8 ? 8 : B_SLOTS_RAW);
   static_assert(B_SLOTS >= 2, "B ring too small");
-  static constexpr int SMEM_BYTES = A_SLOTS * A_SLOT + B_SLOTS * B_SLOT + 1024 + CTRL_BYTES + XPOSE_BYTES;
-  static constexpr int A_TX = F8 ? STRIP_BYTES + 2 * STRIP8_BYTES : 6 * STRIP_BYTES;
-  static constexpr int B_TX = F8 ? B_TILE + 2 * B8_TILE : 2 * B_TILE;
-  // Narrow-N layers: back-to-back MMAs into ONE accumulator serialise on its read-modify-write latency (~105 cycles
-  // per MMA measured for N = 64 / 16, vs 32-48 cycles of work).  Give each of the three split passes its own TMEM
-  // accumulator (three independent chains, summed in the epilogue; the small terms also add up separately).
-  static constexpr int NACC = COUT <= 64 ? 3 : 1;
-  static constexpr int ACC_COLS = NACC * COUT;  // TMEM columns per accumulator buffer
-  static constexpr int TMEM_COLS_RAW = 2 * ACC_COLS;
-  static constexpr int TMEM_COLS = TMEM_COLS_RAW <= 32 ? 32 : (TMEM_COLS_RAW <= 64 ? 64 : (TMEM_COLS_RAW <= 128 ? 128 : (TMEM_COLS_RAW <= 256 ? 256 : 512)));
-  static constexpr int GROUP_CH = COUT / 4;
+  static constexpr int SMEM_BYTES = A_SLOTS * A_SLOT + B_SLOTS * B_SLOT + 1024 + CTRL_BYTES + STAGE_BYTES;
+  static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB dynamic shared memory limit");
+  static constexpr int A_TX = 6 * STRIP_BYTES;
+  static constexpr int B_TX = 2 * B_TILE;
+  static constexpr int GROUP_CH = COUT / 4;  // GroupNorm(4, COUT)
+  static constexpr int GPW = NW >= GROUP_CH ? NW / GROUP_CH : 1;  // groups per consumer warpgroup
+  static_assert(NW % GROUP_CH == 0, "a warpgroup's columns cover whole GroupNorm groups");
 };
 
-// F8: tmA_lo / tmB_lo are the maps of the activation a8 / the weight w8 planes, tmA_x / tmB_x those of l8 / lw8 (uint8 maps,
-// 32-byte swizzle); without F8 the two extra maps are unused copies.
-template <int CIN, int COUT, int BK, int EPI, bool PAIR = false, bool F8 = false>
-__global__ void __launch_bounds__((HaloCfg<CIN, COUT, BK, PAIR, F8>::THREADS), 1)
+template <int CIN, int COUT, int BK, int EPI>
+__global__ void __launch_bounds__((HaloCfg<CIN, COUT, BK>::THREADS), 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                    const __grid_constant__ CUtensorMap tmA_x, const __grid_constant__ CUtensorMap tmB_x,
                     const ConvArgs p) {
-  using C = HaloCfg<CIN, COUT, BK, PAIR, F8>;
-  static_assert(!PAIR || C::NACC == 1, "pair mode is for the wide layers");
+  using C = HaloCfg<CIN, COUT, BK>;
+  constexpr int NW = C::NW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_ring = smem;
@@ -126,113 +86,52 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   uint64_t* a_empty = a_full + C::A_SLOTS;
   uint64_t* b_full = a_empty + C::A_SLOTS;
   uint64_t* b_empty = b_full + C::B_SLOTS;
-  uint64_t* tfull_bar = b_empty + C::B_SLOTS;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  float* red = reinterpret_cast<float*>(tmem_slot + 2);  // [2][4][4][2]
-  float* xpose = reinterpret_cast<float*>(ctrl + C::CTRL_BYTES);
+  float* red = reinterpret_cast<float*>(b_empty + C::B_SLOTS);  // [2][4 NWG][4][2]
+  float* stage = reinterpret_cast<float*>(ctrl + C::CTRL_BYTES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;  // cluster dims (2,1,1): rank == blockIdx.x & 1
-  // Both CTAs of a pair walk the same number of tiles (tile = pair base + rank); a tile past the end is computed on
-  // zero-filled (out-of-bounds) strips and never stored.
-#define DD_TILE_LOOP for (int tile = blockIdx.x; (PAIR ? (tile & ~1) : tile) < p.num_tiles; tile += gridDim.x)
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA_hi);
     tma_prefetch_desc(&tmA_lo);
     tma_prefetch_desc(&tmB_hi);
     tma_prefetch_desc(&tmB_lo);
-    if constexpr (F8) {
-      tma_prefetch_desc(&tmA_x);
-      tma_prefetch_desc(&tmB_x);
-    }
-    // pair mode: the leader's full barriers take one arrive.expect_tx from each CTA's producer; its tempty barriers take
-    // the four epilogue warps of both CTAs; empty / tfull barriers live in each CTA and are hit by multicast commits
+    // full: one arrive.expect_tx by the producer; empty: one arrive per consumer warpgroup
     for (int s = 0; s < C::A_SLOTS; ++s) {
-      mbar_init(&a_full[s], PAIR ? 2 : 1);
-      mbar_init(&a_empty[s], 1);
+      mbar_init(&a_full[s], 1);
+      mbar_init(&a_empty[s], C::NWG);
     }
     for (int s = 0; s < C::B_SLOTS; ++s) {
-      mbar_init(&b_full[s], PAIR ? 2 : 1);
-      mbar_init(&b_empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], PAIR ? 2 * C::EPI_WARPS : C::EPI_WARPS);
+      mbar_init(&b_full[s], 1);
+      mbar_init(&b_empty[s], C::NWG);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (PAIR) {
-      tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
+  if constexpr (C::NWG > 1) {
+    if (warp < 4) setmaxnreg_dec<40>();
+    else setmaxnreg_inc<232>();
+  }
   if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (A strips).  Like the MMA issuer
-    // below, the WHOLE warp walks the loop (barrier waits and coordinates stay warp-uniform) and one elected lane issues
-    // the copies: with a lone `lane == 0` thread in a divergent region every cp.async.bulk.tensor was wrapped in an
-    // ELECT / BRA.U.ANY loop (cuobjdump), now the six copies of a chunk are consecutive UTMALDGs.
+    // ------------------------------------------------------------------ TMA producer (A strips).  The WHOLE warp walks
+    // the loop (barrier waits and coordinates stay warp-uniform) and one elected lane issues the copies.
     const bool leader = elect_one();
     int sa = 0;
     uint32_t pa = 0;
-    if constexpr (F8) {
-      DD_TILE_LOOP {
-        const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
-        const int x0 = tx * HALO_TW, y0 = ty * HALO_TH;
-        for (int kc = 0; kc < C::KC; ++kc) {
-          for (int dx = 0; dx < 3; ++dx) {  // one ring unit per column-shifted strip: hi, a8, l8
-            mbar_wait(&a_empty[sa], pa ^ 1);
-            uint8_t* d = a_ring + sa * C::A_SLOT;
-            if (leader) {
-              const uint32_t lead = mapa_u32(smem_u32(&a_full[sa]), 0);
-              mbar_arrive_expect_tx_cluster(lead, C::A_TX);
-              tma_load_4d_pair(d, &tmA_hi, lead, kc * BK, x0 + dx - 1, y0 - 1, img);
-              tma_load_4d_pair(d + C::STRIP_PAD, &tmA_lo, lead, kc * BK, x0 + dx - 1, y0 - 1, img);
-              tma_load_4d_pair(d + C::STRIP_PAD + C::STRIP8_PAD, &tmA_x, lead, kc * BK, x0 + dx - 1, y0 - 1, img);
-            }
-            __syncwarp();
-            if (++sa == C::A_SLOTS) {
-              sa = 0;
-              pa ^= 1;
-            }
-          }
-        }
-      }
-    } else
-    DD_TILE_LOOP {
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
       const int x0 = tx * HALO_TW, y0 = ty * HALO_TH;
       for (int kc = 0; kc < C::KC; ++kc) {
         mbar_wait(&a_empty[sa], pa ^ 1);
         uint8_t* s = a_ring + sa * C::A_SLOT;
         if (leader) {
-          if constexpr (PAIR) {
-            const uint32_t lead = mapa_u32(smem_u32(&a_full[sa]), 0);
-            mbar_arrive_expect_tx_cluster(lead, C::A_TX);
+          mbar_arrive_expect_tx(&a_full[sa], C::A_TX);
 #pragma unroll
-            for (int dx = 0; dx < 3; ++dx) {
-              uint8_t* d = s + dx * C::DX_STRIDE;
-              tma_load_4d_pair(d, &tmA_hi, lead, kc * BK, x0 + dx - 1, y0 - 1, img);
-              tma_load_4d_pair(d + C::STRIP_PAD, &tmA_lo, lead, kc * BK, x0 + dx - 1, y0 - 1, img);
-            }
-          } else {
-            mbar_arrive_expect_tx(&a_full[sa], C::A_TX);
-#pragma unroll
-            for (int dx = 0; dx < 3; ++dx) {
-              tma_load_4d(s + (2 * dx) * C::STRIP_PAD, &tmA_hi, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
-              tma_load_4d(s + (2 * dx + 1) * C::STRIP_PAD, &tmA_lo, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
-            }
+          for (int dx = 0; dx < 3; ++dx) {
+            tma_load_4d(s + (2 * dx) * C::STRIP_PAD, &tmA_hi, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
+            tma_load_4d(s + (2 * dx + 1) * C::STRIP_PAD, &tmA_lo, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
           }
         }
         __syncwarp();
@@ -242,31 +141,21 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         }
       }
     }
-  } else if (warp == 3) {
+  } else if (warp == 1) {
     // ------------------------------------------------------------------ TMA producer (B weight tiles), same structure
     const bool leader = elect_one();
     int sb = 0;
     uint32_t pb = 0;
-    DD_TILE_LOOP {
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       if (C::B_RESIDENT && tile != static_cast<int>(blockIdx.x)) break;  // weights stay in their slots after the first tile
       for (int kc = 0; kc < C::KC; ++kc) {
-        for (int it = 0; it < 9; ++it) {
-          const int tap = F8 ? (it % 3) * 3 + it / 3 : it;  // F8 walks the taps dx-major (dx = it / 3, dy = it % 3)
+        for (int tap = 0; tap < 9; ++tap) {
           mbar_wait(&b_empty[sb], pb ^ 1);
           uint8_t* s = b_ring + sb * C::B_SLOT;
           if (leader) {
-            if constexpr (PAIR) {  // this CTA's half of the output channels
-              const uint32_t lead = mapa_u32(smem_u32(&b_full[sb]), 0);
-              mbar_arrive_expect_tx_cluster(lead, C::B_TX);
-              tma_load_3d_pair(s, &tmB_hi, lead, kc * BK, static_cast<int>(rank) * C::B_ROWS, tap);
-              tma_load_3d_pair(s + C::B_TILE_PAD, &tmB_lo, lead, kc * BK, static_cast<int>(rank) * C::B_ROWS, tap);
-              if constexpr (F8)
-                tma_load_3d_pair(s + C::B_TILE_PAD + C::B8_TILE_PAD, &tmB_x, lead, kc * BK, static_cast<int>(rank) * C::B_ROWS, tap);
-            } else {
-              mbar_arrive_expect_tx(&b_full[sb], C::B_TX);
-              tma_load_3d(s, &tmB_hi, &b_full[sb], kc * BK, 0, tap);
-              tma_load_3d(s + C::B_TILE_PAD, &tmB_lo, &b_full[sb], kc * BK, 0, tap);
-            }
+            mbar_arrive_expect_tx(&b_full[sb], C::B_TX);
+            tma_load_3d(s, &tmB_hi, &b_full[sb], kc * BK, 0, tap);
+            tma_load_3d(s + C::B_TILE_PAD, &tmB_lo, &b_full[sb], kc * BK, 0, tap);
           }
           __syncwarp();
           if (++sb == C::B_SLOTS) {
@@ -275,314 +164,134 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
           }
         }
       }
-    }
-  } else if (warp == 1 && rank == 0) {
-    // ------------------------------------------------------------------ MMA issuer (pair mode: the leader CTA only).
-    // The WHOLE warp walks the loop (barrier waits, operand addresses: warp-uniform, so the compiler keeps them in
-    // uniform registers) and one elected lane issues the MMAs and commits.  With a lone `lane == 0` thread in a
-    // divergent region every tcgen05.mma was wrapped in an elect/branch loop with R2UR moves (~16 SASS instructions per
-    // MMA), and the issue stream, not the tensor pipe, set the pace.
-    const bool leader = elect_one();
-    constexpr uint32_t idesc = umma_idesc_f16(PAIR ? 2 * TILE_M : TILE_M, COUT);
-    int sa = 0, sb = 0, buf = 0;
-    uint32_t pa = 0, pb = 0, acc_phase = 0;
-    if constexpr (F8) {
-      // 64-channel chunks; per (chunk, dx) one A unit {hi: 128-byte rows, a8 / l8: 64-byte rows}, per (chunk, dx, dy) one
-      // weight stage {hi, w8, lw8}.  Tap (dy, dx) = the unit advanced dy rows: 8 pixels x row bytes = exactly one swizzle
-      // repeat of either layout, so the canonical K-major descriptors still apply.  8 MMAs per stage: the e4m3 correction
-      // products first (2 x K = 32 per plane pair), then hi * hi (4 x K = 16).
-      constexpr uint32_t idesc8 = (1u << 4) | (static_cast<uint32_t>(COUT >> 3) << 17) |
-                                  (static_cast<uint32_t>((2 * TILE_M) >> 4) << 24);  // D f32, A / B e4m3, M = 256
-      DD_TILE_LOOP {
-        mbar_wait(&tempty_bar[buf], ((acc_phase >> buf) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(buf * C::ACC_COLS);
-        for (int kc = 0; kc < C::KC; ++kc) {
-          for (int dx = 0; dx < 3; ++dx) {
-            mbar_wait(&a_full[sa], pa);
-            const uint32_t a_base = smem_u32(a_ring + sa * C::A_SLOT);
-            for (int dy = 0; dy < 3; ++dy) {
-              mbar_wait(&b_full[sb], pb);
-              tc_fence_after();
-              const uint32_t sa_hi = a_base + dy * HALO_TW * C::ROW_BYTES;
-              const uint32_t sa_a8 = a_base + C::STRIP_PAD + dy * HALO_TW * BK;
-              const uint32_t sa_l8 = sa_a8 + C::STRIP8_PAD;
-              const uint32_t sb_hi = smem_u32(b_ring + sb * C::B_SLOT);
-              const uint32_t sb_w8 = sb_hi + C::B_TILE_PAD;
-              const uint32_t sb_lw8 = sb_w8 + C::B8_TILE_PAD;
-              if (leader) {
-#pragma unroll
-                for (int k = 0; k < BK / 32; ++k) {
-                  umma_f8_pair(d_tmem, umma_smem_desc(sa_l8 + k * 32, BK), umma_smem_desc(sb_w8 + k * 32, BK), idesc8,
-                               (kc | dx | dy | k) != 0 ? 1u : 0u);
-                  umma_f8_pair(d_tmem, umma_smem_desc(sa_a8 + k * 32, BK), umma_smem_desc(sb_lw8 + k * 32, BK), idesc8, 1u);
-                }
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)
-                  umma_f16_pair(d_tmem, umma_smem_desc(sa_hi + k * 32, C::ROW_BYTES),
-                                umma_smem_desc(sb_hi + k * 32, C::ROW_BYTES), idesc, 1u);
-                umma_commit_pair(&b_empty[sb], 3);
-              }
-              __syncwarp();
-              if (++sb == C::B_SLOTS) {
-                sb = 0;
-                pb ^= 1;
-              }
-            }
-            if (leader) {
-              umma_commit_pair(&a_empty[sa], 3);
-              if (kc == C::KC - 1 && dx == 2) umma_commit_pair(&tfull_bar[buf], 3);
-            }
-            __syncwarp();
-            if (++sa == C::A_SLOTS) {
-              sa = 0;
-              pa ^= 1;
-            }
-          }
-        }
-        acc_phase ^= (1u << buf);
-        buf ^= 1;
-      }
-    } else
-    DD_TILE_LOOP {
-      mbar_wait(&tempty_bar[buf], ((acc_phase >> buf) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(buf * C::ACC_COLS);
-      for (int kc = 0; kc < C::KC; ++kc) {
-        mbar_wait(&a_full[sa], pa);
-        const uint32_t a_base = smem_u32(a_ring + sa * C::A_SLOT);
-        for (int tap = 0; tap < 9; ++tap) {
-          const int dy = tap / 3, dx = tap % 3;
-          mbar_wait(&b_full[sb], C::B_RESIDENT ? 0u : pb);  // resident: phase 0 completes once and stays complete
-          tc_fence_after();
-          // strip dx, dy rows down: 8-pixel groups stay dense (8 * ROW_BYTES) and aligned to the swizzle repeat
-          const uint32_t sa_hi = a_base + dx * C::DX_STRIDE + dy * HALO_TW * C::ROW_BYTES;
-          const uint32_t sa_lo = sa_hi + C::STRIP_PAD;
-          const uint32_t sb_hi = smem_u32(b_ring + sb * C::B_SLOT);
-          const uint32_t sb_lo = sb_hi + C::B_TILE_PAD;
-          if (leader) {
-          {
-#ifdef DD_PROBES  // timing probes of DESIGN.md §8 / profiles/README.md (build with -DDD_PROBES); results are garbage
-          if (p.fp8_probe == 3 || p.fp8_probe == 1) {
-            // 3: the intrinsic rate of kind::f8f6f4 — three K = 32 e4m3 MMAs per (chunk, tap) stage and nothing else;
-            // 1: fp16 hi*hi (2 x K16) + the two correction products as ONE e4m3 K = 32 MMA each (4 instructions, not 6).
-            // Operand bytes are reinterpreted (the first 32 bytes of each 64-byte row = 32 e4m3 values).
-            constexpr uint32_t idesc8 = (1u << 4) | (static_cast<uint32_t>(COUT >> 3) << 17) |
-                                        (static_cast<uint32_t>((PAIR ? 2 * TILE_M : TILE_M) >> 4) << 24);
-            const uint64_t d_ah = umma_smem_desc(sa_hi, C::ROW_BYTES), d_al = umma_smem_desc(sa_lo, C::ROW_BYTES);
-            const uint64_t d_bh = umma_smem_desc(sb_hi, C::ROW_BYTES), d_bl = umma_smem_desc(sb_lo, C::ROW_BYTES);
-            const uint32_t first = (kc | tap) != 0 ? 1u : 0u;
-            if (p.fp8_probe == 3) {
-              if constexpr (PAIR) {
-                umma_f8_pair(d_tmem, d_ah, d_bh, idesc8, first);
-                umma_f8_pair(d_tmem, d_al, d_bh, idesc8, 1u);
-                umma_f8_pair(d_tmem, d_ah, d_bl, idesc8, 1u);
-              } else {
-                umma_f8(d_tmem, d_ah, d_bh, idesc8, first);
-                umma_f8(d_tmem, d_al, d_bh, idesc8, 1u);
-                umma_f8(d_tmem, d_ah, d_bl, idesc8, 1u);
-              }
-            } else {
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                if constexpr (PAIR)
-                  umma_f16_pair(d_tmem, umma_smem_desc(sa_hi + k * 32, C::ROW_BYTES), umma_smem_desc(sb_hi + k * 32, C::ROW_BYTES), idesc,
-                                (kc | tap | k) != 0 ? 1u : 0u);
-                else
-                  umma_f16(d_tmem, umma_smem_desc(sa_hi + k * 32, C::ROW_BYTES), umma_smem_desc(sb_hi + k * 32, C::ROW_BYTES), idesc,
-                           (kc | tap | k) != 0 ? 1u : 0u);
-              }
-              if constexpr (PAIR) {
-                umma_f8_pair(d_tmem, d_al, d_bh, idesc8, 1u);
-                umma_f8_pair(d_tmem, d_ah, d_bl, idesc8, 1u);
-              } else {
-                umma_f8(d_tmem, d_al, d_bh, idesc8, 1u);
-                umma_f8(d_tmem, d_ah, d_bl, idesc8, 1u);
-              }
-            }
-          }
-          else
-#endif
-#pragma unroll
-          for (int k = 0; k < C::KSTEPS; ++k) {
-            const uint64_t a_hi = umma_smem_desc(sa_hi + k * 32, C::ROW_BYTES);
-            const uint64_t a_lo = umma_smem_desc(sa_lo + k * 32, C::ROW_BYTES);
-            const uint64_t b_hi = umma_smem_desc(sb_hi + k * 32, C::ROW_BYTES);
-            const uint64_t b_lo = umma_smem_desc(sb_lo + k * 32, C::ROW_BYTES);
-            const uint32_t first = (kc | tap | k) != 0 ? 1u : 0u;
-            // order: neighbours share an operand (B_hi between the first two, A_hi between the last two); measured
-            // neutral against lo*hi, hi*lo, hi*hi (a 5 % difference seen in the ordering probe followed the code path of
-            // the issuing thread, not the order)
-            if constexpr (C::NACC == 3) {
-              umma_f16(d_tmem, a_lo, b_hi, idesc, first);
-              umma_f16(d_tmem + 2 * COUT, a_hi, b_hi, idesc, first);
-              umma_f16(d_tmem + COUT, a_hi, b_lo, idesc, first);
-            } else if constexpr (PAIR) {
-              umma_f16_pair(d_tmem, a_lo, b_hi, idesc, first);
-              umma_f16_pair(d_tmem, a_hi, b_hi, idesc, 1u);
-              umma_f16_pair(d_tmem, a_hi, b_lo, idesc, 1u);
-            } else {
-              umma_f16(d_tmem, a_lo, b_hi, idesc, first);
-              umma_f16(d_tmem, a_hi, b_hi, idesc, 1u);
-              umma_f16(d_tmem, a_hi, b_lo, idesc, 1u);
-            }
-          }
-          }  // !F8
-          if constexpr (PAIR) umma_commit_pair(&b_empty[sb], 3);
-          else if constexpr (!C::B_RESIDENT) umma_commit(&b_empty[sb]);
-          }  // leader
-          __syncwarp();
-          if (++sb == C::B_SLOTS) {
-            sb = 0;
-            pb ^= 1;
-          }
-        }
-        if (leader) {
-          if constexpr (PAIR) {
-            umma_commit_pair(&a_empty[sa], 3);
-            if (kc == C::KC - 1) umma_commit_pair(&tfull_bar[buf], 3);
-          } else {
-            umma_commit(&a_empty[sa]);
-            if (kc == C::KC - 1) umma_commit(&tfull_bar[buf]);
-          }
-        }
-        __syncwarp();
-        if (++sa == C::A_SLOTS) {
-          sa = 0;
-          pa ^= 1;
-        }
-      }
-      acc_phase ^= (1u << buf);
-      buf ^= 1;
     }
   } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue (as conv_umma.cuh, 16x8 tile)
-    const int q = warp & 3;
-    const int es = (warp - 4) >> 2;  // epilogue set (see ConvCfg::EPI_SETS)
-    constexpr int NCH = COUT / C::CH;
-    static_assert(NCH % C::EPI_SETS == 0 && (C::EPI_SETS == 1 || C::STATS_LOCAL || C::GROUP_CH % (C::EPI_SETS * C::CH) == 0),
-                  "chunks split evenly over the sets; a set's chunk never straddles a GroupNorm group");
-    const int m = q * 32 + lane;
+    // ------------------------------------------------------------------ consumers: MMA + epilogue
+    const int wg = (warp >> 2) - 1;  // consumer warpgroup
+    const int t = threadIdx.x & 127;
+    const int q = t >> 5;
+    const bool signal = (t == 0);    // the thread that releases ring slots for its warpgroup
+    float* S = stage + wg * 128 * C::LD;
+    const int m = t;                 // epilogue: this thread's row (pixel) of the tile
     const int r = m >> 3, c = m & 7;
-    uint32_t full_phase = 0;
-    int buf = 0, par = 0;
-    float* T = xpose + (es * 4 + q) * (32 * C::CH);
-    long long clk0 = 0;
-    unsigned long long ns0 = 0;
-    const bool probe = p.clk_probe != nullptr && blockIdx.x == 0 && threadIdx.x == 128;
-    if (probe) {
-      clk0 = clock64();
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns0));
-    }
-    DD_TILE_LOOP {
-      const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
-      const int x = tx * HALO_TW + c, y = ty * HALO_TH + r;
-      const bool valid = (x < p.W) && (y < p.H) && (tile < p.num_tiles);
-      const size_t pix = (static_cast<size_t>(img) * p.H + y) * p.W + x;
-      const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-      const uint32_t row_off = static_cast<uint32_t>(pix * COUT);
+    const uint32_t b_off = static_cast<uint32_t>(wg * NW);  // first weight row of this warpgroup
+    int sa = 0, sb = 0, par = 0;
+    uint32_t pa = 0, pb = 0;
+    float acc[2][NW / 2];
 
-      mbar_wait(&tfull_bar[buf], (full_phase >> buf) & 1u);
-      full_phase ^= (1u << buf);
-      tc_fence_after();
-
-      float tsum[4] = {0.f, 0.f, 0.f, 0.f}, tsq[4] = {0.f, 0.f, 0.f, 0.f};
-      bool overflow = false;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      // ---------------------------------------------------------------- mainloop
+      int prev_b = -1, prev_a = -1;  // slots read by the wgmma group still in flight
+      auto retire_prev = [&]() {
+        if (signal) {
+          if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
+          if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+        }
+        prev_b = prev_a = -1;
+      };
+      {
+        for (int kc = 0; kc < C::KC; ++kc) {
+          mbar_wait(&a_full[sa], pa);
+          const uint32_t a_base = smem_u32(a_ring + sa * C::A_SLOT);
+          for (int tap = 0; tap < 9; ++tap) {
+            const int dy = tap / 3, dx = tap % 3;
+            mbar_wait(&b_full[sb], C::B_RESIDENT ? 0u : pb);  // resident: phase 0 completes once and stays complete
+            // strip dx, dy rows down: 8-pixel groups stay dense (8 * ROW_BYTES) and aligned to the swizzle atom
+            const uint32_t sa_hi = a_base + dx * C::DX_STRIDE + dy * HALO_TW * C::ROW_BYTES;
+            const uint32_t sa_lo = sa_hi + C::STRIP_PAD;
+            const uint32_t sb_hi = smem_u32(b_ring + sb * C::B_SLOT) + b_off * C::ROW_BYTES;
+            const uint32_t sb_lo = sb_hi + C::B_TILE_PAD;
+            wgmma_fence();
 #pragma unroll
-      for (int cj = 0; cj < NCH / C::EPI_SETS; ++cj) {
-        const int ch0 = (cj * C::EPI_SETS + es) * C::CH;
-        float v[C::CH];
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t ho = static_cast<uint32_t>(h * 64 * C::ROW_BYTES);
 #pragma unroll
-        for (int j = 0; j < C::CH; ++j) v[j] = 0.f;
-#pragma unroll
-        for (int acc = 0; acc < C::NACC; ++acc) {  // lo*hi + hi*lo first, hi*hi last
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                                 static_cast<uint32_t>(buf * C::ACC_COLS + acc * COUT + ch0);
-          if constexpr (C::CH == 32) {
-            uint32_t rr[32];
-            tmem_ld_32x32(taddr, rr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += __uint_as_float(rr[j]);
-          } else {
-            uint32_t rr[16];
-            tmem_ld_32x16(taddr, rr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] += __uint_as_float(rr[j]);
+              for (int k = 0; k < C::KSTEPS; ++k) {
+                const uint64_t a_hi = wgmma_desc(sa_hi + ho + k * 32, C::ROW_BYTES);
+                const uint64_t a_lo = wgmma_desc(sa_lo + ho + k * 32, C::ROW_BYTES);
+                const uint64_t b_hi = wgmma_desc(sb_hi + k * 32, C::ROW_BYTES);
+                const uint64_t b_lo = wgmma_desc(sb_lo + k * 32, C::ROW_BYTES);
+                wgmma_f16<NW>(acc[h], a_lo, b_hi, (kc | tap | k) != 0 ? 1u : 0u);  // small terms first
+                wgmma_f16<NW>(acc[h], a_hi, b_lo, 1u);
+                wgmma_f16<NW>(acc[h], a_hi, b_hi, 1u);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            retire_prev();
+            if (!C::B_RESIDENT) prev_b = sb;
+            if (tap == 8) prev_a = sa;
+            if (++sb == C::B_SLOTS) {
+              sb = 0;
+              pb ^= 1;
+            }
+          }
+          if (++sa == C::A_SLOTS) {
+            sa = 0;
+            pa ^= 1;
           }
         }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+      retire_prev();  // the producers refill the rings while this warpgroup drains its accumulators
+
+      // ---------------------------------------------------------------- epilogue
+      const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
+      const int x = tx * HALO_TW + c, y = ty * HALO_TH + r;
+      const bool valid = (x < p.W) && (y < p.H);
+      const size_t pix = (static_cast<size_t>(img) * p.H + y) * p.W + x;
+      const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
+      const uint32_t row_off = static_cast<uint32_t>(pix * COUT);  // < 2^32 elements for every tensor of the path
+      float tsum[C::GPW], tsq[C::GPW];
 #pragma unroll
-        for (int j = 0; j < C::CH; ++j) v[j] = fmaf(v[j], p.acc_scale, __ldg(p.bias + ch0 + j));
+      for (int g = 0; g < C::GPW; ++g) tsum[g] = tsq[g] = 0.f;
+      bool overflow = false;
+#pragma unroll
+      for (int cj = 0; cj < NW / C::CH; ++cj) {
+        const int ch0 = wg * NW + cj * C::CH;
+        named_bar_sync(2 + wg, 128);  // the previous chunk's staging reads are done
+        stage_acc_cols<NW, C::CH, C::LD>(acc[0], S, 0, cj * C::CH / 8);
+        stage_acc_cols<NW, C::CH, C::LD>(acc[1], S, 64, cj * C::CH / 8);
+        named_bar_sync(2 + wg, 128);
+        float v[C::CH];
+#pragma unroll
+        for (int j = 0; j < C::CH; ++j) v[j] = fmaf(S[m * C::LD + j], p.acc_scale, __ldg(p.bias + ch0 + j));
         if constexpr (EPI == EPI_F32_STATS) {
           if (valid) {
 #pragma unroll
             for (int j = 0; j < C::CH; ++j) {
-              // compile-time: chunk cj * SETS + es lies in group cj * SETS * CH / GROUP_CH for either es, except for
-              // Cout = 64 where the set's single chunk holds its own two groups (local index)
-              const int g = C::STATS_LOCAL ? j / C::GROUP_CH : (cj * C::EPI_SETS * C::CH + j) / C::GROUP_CH;
+              const int g = (cj * C::CH + j) / C::GROUP_CH;  // compile-time: group within this warpgroup's columns
               tsum[g] += v[j];
               tsq[g] = fmaf(v[j], v[j], tsq[g]);
             }
           }
         }
-        if constexpr ((EPI == EPI_F32_STATS || EPI == EPI_F32) && C::CH == 16 && C::XPOSE_BYTES > 0) {
-          // [32 px][16 ch] re-distribution tile (XOR-swizzled): each store instruction writes the 64-byte segments of two
-          // pixel rows (lanes 0..15: row 2i, lanes 16..31: row 2i + 1)
+        if constexpr (EPI == EPI_F32_STATS || EPI == EPI_F32) {
+          // thread = row; go back through the staging tile so that lanes = columns and every store instruction writes
+          // whole row segments (row-per-thread stores write 32 partial lines per instruction)
 #pragma unroll
-          for (int j = 0; j < 16; ++j) T[lane * 16 + ((j ^ lane) & 15)] = v[j];
+          for (int j = 0; j < C::CH; ++j) S[m * C::LD + j] = v[j];
           __syncwarp();
-          const int hsel = lane >> 4, cl = lane & 15;
+          if constexpr (C::CH == 32) {
 #pragma unroll 8
-          for (int i = 0; i < 16; ++i) {
-            const int rw = 2 * i + hsel;
-            const uint32_t o = __shfl_sync(0xffffffffu, row_off, rw) + ch0 + cl;
-            if ((vmask >> rw) & 1u) p.y32[o] = T[rw * 16 + ((cl ^ rw) & 15)];
-          }
-          __syncwarp();
-        } else if constexpr ((EPI == EPI_F32_STATS || EPI == EPI_F32) && C::CH == 32 && C::XPOSE_BYTES > 0) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) T[lane * 32 + ((j ^ lane) & 31)] = v[j];
-          __syncwarp();
-#pragma unroll 8
-          for (int rw = 0; rw < 32; ++rw) {
-            const uint32_t o = __shfl_sync(0xffffffffu, row_off, rw) + ch0 + lane;
-            if ((vmask >> rw) & 1u) p.y32[o] = T[rw * 32 + ((lane ^ rw) & 31)];
-          }
-          __syncwarp();
-        } else if (valid) {
-          if constexpr (EPI == EPI_F32_STATS || EPI == EPI_F32) {
-            float4* dst = reinterpret_cast<float4*>(p.y32 + pix * COUT + ch0);
-#pragma unroll
-            for (int j = 0; j < C::CH / 4; ++j)
-              dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          } else if (p.out_a8 != nullptr) {
-            // planes for a consumer with fp8 corrections: hi (fp16) + a8 + l8 (e4m3), 64 + 32 + 32 bytes per 32 channels
-            if constexpr (C::CH == 32) {
-              __align__(16) __half hi[32];
-              __align__(16) uint16_t a8[16];
-              __align__(16) uint16_t l8[16];
-#pragma unroll
-              for (int j = 0; j < 32; j += 2) {
-                const float s0 = v[j] * p.split_scale, s1 = v[j + 1] * p.split_scale;
-                overflow |= (fabsf(s0) > kF8ActMax) | (fabsf(s1) > kF8ActMax);
-                hi[j] = __float2half_rn(s0);
-                hi[j + 1] = __float2half_rn(s1);
-                a8[j >> 1] = e4m3x2(s0 * kF8ActDiv, s1 * kF8ActDiv);
-                l8[j >> 1] = e4m3x2((s0 - __half2float(hi[j])) * kF8LoMul, (s1 - __half2float(hi[j + 1])) * kF8LoMul);
-              }
-              uint4* dh = reinterpret_cast<uint4*>(p.out_hi + pix * COUT + ch0);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) dh[j] = reinterpret_cast<const uint4*>(hi)[j];
-              uint4* da = reinterpret_cast<uint4*>(p.out_a8 + pix * COUT + ch0);
-              uint4* dl = reinterpret_cast<uint4*>(p.out_l8 + pix * COUT + ch0);
-#pragma unroll
-              for (int j = 0; j < 2; ++j) {
-                da[j] = reinterpret_cast<const uint4*>(a8)[j];
-                dl[j] = reinterpret_cast<const uint4*>(l8)[j];
-              }
+            for (int rw = 0; rw < 32; ++rw) {
+              const uint32_t o = __shfl_sync(0xffffffffu, row_off, rw) + ch0 + lane;
+              if ((vmask >> rw) & 1u) p.y32[o] = S[(q * 32 + rw) * C::LD + lane];
             }
           } else {
+            constexpr int RPI = 32 / C::CH;  // rows per store instruction
+            const int hsel = lane / C::CH, cl = lane % C::CH;
+#pragma unroll 8
+            for (int i = 0; i < 32 / RPI; ++i) {
+              const int rw = RPI * i + hsel;
+              const uint32_t o = __shfl_sync(0xffffffffu, row_off, rw) + ch0 + cl;
+              if ((vmask >> rw) & 1u) p.y32[o] = S[(q * 32 + rw) * C::LD + cl];
+            }
+          }
+        } else if (valid) {
+          {
             __align__(16) __half hi[C::CH];
             __align__(16) __half lo[C::CH];
 #pragma unroll
@@ -602,69 +311,45 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[buf]), 0));
-        else mbar_arrive(&tempty_bar[buf]);
-      }
 
       if constexpr (EPI == EPI_F32_STATS) {
+        // warp tree -> shared memory -> 8 threads combine the consumer warps in fixed order (deterministic)
+        const int cw = wg * 4 + q;  // consumer warp index
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
-          float s = tsum[g], s2 = tsq[g];
+          const int gl = g - (C::NWG > 1 ? wg * C::GPW : 0);  // this warpgroup's local group index
+          float s = 0.f, s2 = 0.f;
+#pragma unroll
+          for (int k = 0; k < C::GPW; ++k)
+            if (k == gl) {
+              s = tsum[k];
+              s2 = tsq[k];
+            }
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) {
             s += __shfl_xor_sync(0xffffffffu, s, o);
             s2 += __shfl_xor_sync(0xffffffffu, s2, o);
           }
           if (lane == 0) {
-            if constexpr (!C::STATS_LOCAL) {  // every epilogue warp has a partial sum of every group
-              red[((par * C::EPI_WARPS + es * 4 + q) * 4 + g) * 2 + 0] = s;
-              red[((par * C::EPI_WARPS + es * 4 + q) * 4 + g) * 2 + 1] = s2;
-            } else if (g < 2) {
-              red[((par * 8 + es * 4 + q) * 2 + g) * 2 + 0] = s;
-              red[((par * 8 + es * 4 + q) * 2 + g) * 2 + 1] = s2;
-            }
+            red[((par * 4 * C::NWG + cw) * 4 + g) * 2 + 0] = s;
+            red[((par * 4 * C::NWG + cw) * 4 + g) * 2 + 1] = s2;
           }
         }
-        if constexpr (C::EPI_SETS == 1) asm volatile("bar.sync 1, 128;" ::: "memory");
-        else if constexpr (C::EPI_SETS == 2) asm volatile("bar.sync 1, 256;" ::: "memory");
-        else asm volatile("bar.sync 1, 512;" ::: "memory");
+        named_bar_sync(1, 128 * C::NWG);
         const int e = threadIdx.x - 128;
-        if (e < 8 && tile < p.num_tiles) {
+        if (e < 8) {
           const int g = e >> 1, which = e & 1;
-          float t = 0.f;
-          if constexpr (!C::STATS_LOCAL) {
+          float tt = 0.f;
 #pragma unroll
-            for (int w = 0; w < C::EPI_WARPS; ++w) t += red[((par * C::EPI_WARPS + w) * 4 + g) * 2 + which];
-          } else {
-#pragma unroll
-            for (int w = 0; w < 4; ++w) t += red[((par * 8 + (g >> 1) * 4 + w) * 2 + (g & 1)) * 2 + which];
-          }
-          p.stats_partial[(static_cast<size_t>(tile) * 4 + g) * 2 + which] = t;
+          for (int w = 0; w < 4 * C::NWG; ++w) tt += red[((par * 4 * C::NWG + w) * 4 + g) * 2 + which];
+          p.stats_partial[(static_cast<size_t>(tile) * 4 + g) * 2 + which] = tt;
         }
-        par ^= 1;
+        par ^= 1;  // double-buffered scratch: one barrier per tile is enough
       }
       if constexpr (EPI == EPI_SPLIT) {
         if (overflow) atomicOr(p.status, 1);
       }
-      buf ^= 1;
     }
-    if (probe) {
-      unsigned long long ns1;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns1));
-      atomicAdd(p.clk_probe, static_cast<unsigned long long>(clock64() - clk0));
-      atomicAdd(p.clk_probe + 1, ns1 - ns0);
-    }
-  }
-
-#undef DD_TILE_LOOP
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_pair(tmem_base, C::TMEM_COLS); else tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 

@@ -1,14 +1,15 @@
-// General stride-1 convolution (1x1 or 3x3, zero pad) + per-channel shift (+ReLU, +addend) on tcgen05, used
+// General convolution (1x1 or 3x3, zero pad, stride 1 or 2) + per-channel shift (+activation, +addend) on the warpgroup
+// MMA (wgmma), used
 // for the step-invariant producers: HAHI neck (1x1 / 3x3 ConvModules with eval-BN folded, channel-concatenated
 // inputs) and the FPN (3x3 laterals, 2x2/s2 transposed convs as a 1x1 GEMM with a pixel-shuffle epilogue).
-// Same machinery as conv3x3_umma_kernel (3-pass fp16 hi/lo split, TMA-staged swizzled tiles, TMEM double
-// buffer, warp-specialised persistent CTA) with runtime shapes:
+// Same machinery as conv3x3_halo_kernel (3-pass fp16 hi/lo split, TMA-staged swizzled tiles, register accumulators,
+// warp-specialised persistent CTA) with runtime shapes:
 //   M = 128 pixels (8x16 patch), N tile = NT output channels, K = taps x (cin0 + cin1) in chunks of 32 channels,
 //   the K range may be fed from two source tensors (torch.cat([a, b], dim=1) never materialises).
 // Replaces (reference): mmcv ConvModule calls in src/model/necks/hahi.py:165-276 and the FPN in
 // src/model/head/ddim_depth_estimate_res_swin_addHAHI.py:112-122.
 #pragma once
-#include "conv_umma.cuh"
+#include "conv_common.cuh"
 
 namespace dd {
 
@@ -39,64 +40,53 @@ struct GenConvArgs {
   int* status;
 };
 
-// PAIR = true: two CTAs of one cluster run ONE tcgen05.mma.cta_group::2 with M = 256 (two consecutive M tiles, one per
-// CTA) and each stages only HALF of the weight tile (NT / 2 rows).  Per 32-channel stage a single CTA pulls
-// 2 * (128 + NT) * 64 B from L2 for 3 * NT cycles of MMA work = 64 B/clk at NT = 256, above the ~40 B/clk an SM gets from
-// L2 when all 148 stream at once (profiles/README.md round 2); a pair needs 2 * (128 + NT / 2) * 64 B = 42 B/clk.
-// K chunk of the producer convs / GEMMs: 64 channels = 128-byte operand rows (128-byte swizzle).  With 32-channel chunks
-// (64-byte rows) the tensor pipe sat at 13..40 % in every Swin GEMM (ncu, profiles/README.md round 2) at ~1 us per stage
-// whatever the stage's MMA work: each stage is 2 x (128 + NT) separate 64-byte row requests to TMA; 128-byte rows halve
-// the requests and the barrier round trips per byte.
+// K chunk of the producer convs / GEMMs: 64 channels = 128-byte operand rows (128-byte swizzle): half the TMA row
+// requests and barrier round trips per byte of 32-channel chunks.
 constexpr int GEN_BK = 64;
 
-template <int NT, bool PAIR = false>
+template <int NT>
 struct GenCfg {
   static constexpr int BK = GEN_BK;
   static constexpr int ROW_BYTES = BK * 2;
-  static constexpr int A_BYTES = TILE_M * ROW_BYTES;  // 8 KB per plane
-  static constexpr int B_ROWS = PAIR ? NT / 2 : NT;   // weight rows this CTA stages
-  static constexpr int B_BYTES = B_ROWS * ROW_BYTES;
+  static constexpr int A_BYTES = TILE_M * ROW_BYTES;  // 16 KB per plane
+  static constexpr int B_BYTES = NT * ROW_BYTES;
   static constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);
-  static constexpr int EPI_WARPS = 16;
-  static constexpr int THREADS = 128 + 32 * EPI_WARPS;         // 4 role warps + the epilogue warps
-  static constexpr int XPOSE_BYTES = EPI_WARPS * 32 * 16 * 4;  // per-warp [32][16] fp32 re-distribution tile (XOR-swizzled)
-  static constexpr int STAGES_RAW = (227 * 1024 - 1024 - 512 - XPOSE_BYTES) / STAGE_BYTES;
+  // consumer warpgroups: each owns all 128 rows of the tile and NW = NT / NWG columns (NW registers of accumulators)
+  static constexpr int NWG = NT > 128 ? 2 : 1;
+  static constexpr int NW = NT / NWG;
+  static constexpr int THREADS = 128 * (1 + NWG);
+  static constexpr int LD = 20;  // staging row stride (floats): 16 columns + 4, rows stay 16-byte aligned
+  static constexpr int STAGING_BYTES = NWG * 128 * LD * 4;
+  static constexpr int STAGES_RAW = (227 * 1024 - 1024 - 512 - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
   static_assert(STAGES >= 2, "stage too large");
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512 + XPOSE_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512 + STAGING_BYTES;
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB dynamic shared memory limit");
-  static constexpr int TMEM_COLS = 512;
-  static_assert(NT % 32 == 0 && NT <= 256 && 2 * NT <= 512, "bad N tile");  // instantiated: 64, 128, 192, 256
+  static_assert(NW % 16 == 0 && NT <= 256, "bad N tile");  // instantiated: 64, 128, 192, 256
 };
 
-// PAIR: launched as clusters of 2; work item = (pair of M tiles, N tile); tmB_* then have a box of NT / 2 rows.
-template <int NT, bool PAIR = false>
-__global__ void __launch_bounds__((GenCfg<NT, PAIR>::THREADS), 1)
-convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_constant__ CUtensorMap tmA0_lo,
-                    const __grid_constant__ CUtensorMap tmA1_hi, const __grid_constant__ CUtensorMap tmA1_lo,
-                    const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-                    const GenConvArgs p) {
-  using C = GenCfg<NT, PAIR>;
+// Warp roles: warp 0 = TMA producer of the activation planes, warp 1 = of the weight planes; warpgroups 1 .. NWG =
+// consumers (wgmma mainloop, then the epilogue of their columns, drained 16 columns at a time through a shared-memory
+// staging tile that hands each thread one ROW (pixel / token) of the chunk).
+template <int NT>
+__global__ void __launch_bounds__((GenCfg<NT>::THREADS), 1)
+convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_constant__ CUtensorMap tmA0_lo,
+                     const __grid_constant__ CUtensorMap tmA1_hi, const __grid_constant__ CUtensorMap tmA1_lo,
+                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
+                     const GenConvArgs p) {
+  using C = GenCfg<NT>;
+  constexpr int NW = C::NW;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + C::STAGES;
-  uint64_t* tfull_bar = empty_bar + C::STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  float* xpose = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 512);
+  float* stage_f = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 512);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int kc_total = p.kc0 + p.kc1;
   const int k_iters = p.taps * kc_total;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;  // cluster dims (2,1,1): rank == blockIdx.x & 1
-  // PAIR: both CTAs of a pair walk the same work items (pair of M tiles 2 * mp + rank, N tile); an M tile past the end is
-  // computed on zero-filled (out-of-bounds) patches and never stored
-  const int m_units = PAIR ? (p.m_tiles + 1) / 2 : p.m_tiles;
-  const int num_work = m_units * p.n_tiles;
-  const int work0 = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int work_step = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int num_work = p.m_tiles * p.n_tiles;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA0_hi);
@@ -104,43 +94,27 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
     tma_prefetch_desc(&tmB_hi);
     tma_prefetch_desc(&tmB_lo);
     for (int s = 0; s < C::STAGES; ++s) {
-      // two producers (activation planes / weight planes) arrive per stage; pair mode: those of both CTAs, on the
-      // leader's barrier.  empty / tfull barriers live in each CTA and are hit by multicast commits.
-      mbar_init(&full_bar[s], PAIR ? 4 : 2);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tfull_bar[b], 1);
-      mbar_init(&tempty_bar[b], (PAIR ? 2 : 1) * C::EPI_WARPS);  // the epilogue warps (of both CTAs, on the leader's barrier)
+      mbar_init(&full_bar[s], 2);        // two producers (activation planes / weight planes) arrive per stage
+      mbar_init(&empty_bar[s], C::NWG);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (PAIR) {
-      tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   auto stage_ptr = [&](int s) { return smem + s * C::STAGE_BYTES; };
 
-  if (warp == 0 || warp == 3) {
-    // two TMA producers: warp 0 issues the activation copies, warp 3 the weight copies; the whole warp walks the loop,
-    // one elected lane issues (consecutive UTMALDGs instead of an ELECT / branch loop per copy; see conv_halo.cuh)
+  if constexpr (C::NWG > 1) {
+    if (warp < 4) setmaxnreg_dec<40>();
+    else setmaxnreg_inc<232>();
+  }
+  if (warp == 0 || warp == 1) {
+    // two TMA producers; the whole warp walks the loop, one elected lane issues (consecutive UTMALDGs)
     const bool act = (warp == 0);
     const bool leader = elect_one();
     int stage = 0;
     uint32_t phase = 0;
-    for (int work = work0; work < num_work; work += work_step) {
+    for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
       const int nt = work % p.n_tiles;  // n fastest: neighbours share the A patch in L2
-      const int mt = (PAIR ? 2 * (work / p.n_tiles) + static_cast<int>(rank) : work / p.n_tiles);
-      // an M tile past the end (second CTA of the last pair): image index = B -> every row is out of bounds -> zero fill
+      const int mt = work / p.n_tiles;
       const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
       const int x0 = tx * TILE_W, y0 = ty * TILE_H;
       for (int tap = 0; tap < p.taps; ++tap) {
@@ -152,23 +126,7 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
           // weight K coordinate of this chunk: source 1's channels start right after source 0's REAL channels
           const int kw = kc < p.kc0 ? kc * C::BK : p.c0_ch + (kc - p.kc0) * C::BK;
           if (leader) {
-            if constexpr (PAIR) {
-              const uint32_t lead = mapa_u32(smem_u32(&full_bar[stage]), 0);
-              const int brow = nt * NT + static_cast<int>(rank) * C::B_ROWS;  // this CTA's half of the N tile
-              if (!act) {
-                mbar_arrive_expect_tx_cluster(lead, 2 * C::B_BYTES);
-                tma_load_3d_pair(s + 2 * C::A_BYTES, &tmB_hi, lead, kw, brow, tap);
-                tma_load_3d_pair(s + 2 * C::A_BYTES + C::B_BYTES, &tmB_lo, lead, kw, brow, tap);
-              } else if (kc < p.kc0) {
-                mbar_arrive_expect_tx_cluster(lead, 2 * C::A_BYTES);
-                tma_load_4d_pair(s, &tmA0_hi, lead, kc * C::BK, ax, ay, img);
-                tma_load_4d_pair(s + C::A_BYTES, &tmA0_lo, lead, kc * C::BK, ax, ay, img);
-              } else {
-                mbar_arrive_expect_tx_cluster(lead, 2 * C::A_BYTES);
-                tma_load_4d_pair(s, &tmA1_hi, lead, (kc - p.kc0) * C::BK, ax, ay, img);
-                tma_load_4d_pair(s + C::A_BYTES, &tmA1_lo, lead, (kc - p.kc0) * C::BK, ax, ay, img);
-              }
-            } else if (!act) {
+            if (!act) {
               mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES);
               tma_load_3d(s + 2 * C::A_BYTES, &tmB_hi, &full_bar[stage], kw, nt * NT, tap);
               tma_load_3d(s + 2 * C::A_BYTES + C::B_BYTES, &tmB_lo, &full_bar[stage], kw, nt * NT, tap);
@@ -190,100 +148,81 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
         }
       }
     }
-  } else if (warp == 1 && rank == 0) {
-    // the whole warp walks the loop (waits and operand addresses stay warp-uniform -> uniform registers, MMAs issued
-    // back to back); one elected lane issues the MMAs and commits (see conv_halo.cuh).  Pair mode: the leader CTA only.
-    const bool leader = elect_one();
-    constexpr uint32_t idesc = umma_idesc_f16(PAIR ? 2 * TILE_M : TILE_M, NT);
+  } else if (warp >= 4) {
+    const int wg = (warp >> 2) - 1;
+    const int t = threadIdx.x & 127;
+    const int q = t >> 5;
+    const int m = t;
+    const int r = m >> 4, c = m & 15;
+    float* S = stage_f + wg * 128 * C::LD;
+    float* T = S + q * 32 * C::LD;  // this warp's 32 rows
+    const uint32_t b_off = static_cast<uint32_t>(wg * NW) * C::ROW_BYTES;
     int stage = 0;
-    uint32_t phase = 0, acc_phase = 0;
-    int buf = 0;
-    for (int work = work0; work < num_work; work += work_step) {
-      mbar_wait(&tempty_bar[buf], ((acc_phase >> buf) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(buf * NT);
+    uint32_t phase = 0;
+    bool overflow = false;
+    const int cq = p.cout >> 2;
+    float acc[2][NW / 2];
+    for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+      // ---------------------------------------------------------------- mainloop
+      int prev = -1;
       for (int it = 0; it < k_iters; ++it) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
         const uint32_t sa_hi = smem_u32(stage_ptr(stage));
         const uint32_t sa_lo = sa_hi + C::A_BYTES;
-        const uint32_t sb_hi = sa_hi + 2 * C::A_BYTES;
+        const uint32_t sb_hi = sa_hi + 2 * C::A_BYTES + b_off;
         const uint32_t sb_lo = sb_hi + C::B_BYTES;
-        if (leader) {
+        wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < C::BK / 16; ++k) {
-          const uint64_t a_hi = umma_smem_desc(sa_hi + k * 32, C::ROW_BYTES);
-          const uint64_t a_lo = umma_smem_desc(sa_lo + k * 32, C::ROW_BYTES);
-          const uint64_t b_hi = umma_smem_desc(sb_hi + k * 32, C::ROW_BYTES);
-          const uint64_t b_lo = umma_smem_desc(sb_lo + k * 32, C::ROW_BYTES);
-          // neighbours share an operand (B_hi, then A_hi); see conv_halo.cuh
-          if constexpr (PAIR) {
-            umma_f16_pair(d_tmem, a_lo, b_hi, idesc, (it | k) != 0 ? 1u : 0u);
-            umma_f16_pair(d_tmem, a_hi, b_hi, idesc, 1u);
-            umma_f16_pair(d_tmem, a_hi, b_lo, idesc, 1u);
-          } else {
-            umma_f16(d_tmem, a_lo, b_hi, idesc, (it | k) != 0 ? 1u : 0u);
-            umma_f16(d_tmem, a_hi, b_hi, idesc, 1u);
-            umma_f16(d_tmem, a_hi, b_lo, idesc, 1u);
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t ho = static_cast<uint32_t>(h * 64 * C::ROW_BYTES);
+#pragma unroll
+          for (int k = 0; k < C::BK / 16; ++k) {
+            const uint64_t a_hi = wgmma_desc(sa_hi + ho + k * 32, C::ROW_BYTES);
+            const uint64_t a_lo = wgmma_desc(sa_lo + ho + k * 32, C::ROW_BYTES);
+            const uint64_t b_hi = wgmma_desc(sb_hi + k * 32, C::ROW_BYTES);
+            const uint64_t b_lo = wgmma_desc(sb_lo + k * 32, C::ROW_BYTES);
+            wgmma_f16<NW>(acc[h], a_lo, b_hi, (it | k) != 0 ? 1u : 0u);  // small terms first
+            wgmma_f16<NW>(acc[h], a_hi, b_lo, 1u);
+            wgmma_f16<NW>(acc[h], a_hi, b_hi, 1u);
           }
         }
-        if constexpr (PAIR) {
-          umma_commit_pair(&empty_bar[stage], 3);
-          if (it == k_iters - 1) umma_commit_pair(&tfull_bar[buf], 3);
-        } else {
-          umma_commit(&empty_bar[stage]);
-          if (it == k_iters - 1) umma_commit(&tfull_bar[buf]);
-        }
-        }  // leader
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (t == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
         if (++stage == C::STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      acc_phase ^= (1u << buf);
-      buf ^= 1;
-    }
-  } else if (warp >= 4) {
-    // ---------------------------------------------------------------- epilogue: 16 warps = 4 groups x 128 TMEM lanes;
-    // group g drains the 16-column chunks with index % 4 == g.  (ncu, round 2: with 8 warps on 32-column chunks the
-    // GELU -> planes epilogue of every FFN1 ran at 2 warps per scheduler, 42 % issue-active, and took twice the mainloop:
-    // 16 warps at half the registers each.)  tcgen05.ld hands each thread one ROW (pixel / token) of the chunk.
-    //   fp32-only outputs: a per-warp XOR-swizzled [32][16] shared-memory tile re-distributes the chunk so that a lane
-    //     holds one float4 of a row and 4 lanes cover the row's 64 bytes: every global access is a full 64-byte segment;
-    //   plane outputs (fp16 hi / lo for the next GEMM): row-per-thread, 32 contiguous bytes per row and plane.
-    const int q = warp & 3;
-    const int grp = (warp - 4) >> 2;
-    const int m = q * 32 + lane;
-    const int r = m >> 4, c = m & 15;
-    float* T = xpose + (warp - 4) * (32 * 16);
-    uint32_t full_phase = 0;
-    int buf = 0;
-    bool overflow = false;
-    const int cq = p.cout >> 2;
-    constexpr int NCH = NT / 16;
-    for (int work = work0; work < num_work; work += work_step) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+      if (t == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);
+
+      // ---------------------------------------------------------------- epilogue
+      //   fp32-only outputs: the staging tile re-distributes the chunk so that a lane holds one float4 of a row and 4
+      //     lanes cover the row's 64 bytes: every global access is a full 64-byte segment;
+      //   plane outputs (fp16 hi / lo for the next GEMM): row-per-thread, 32 contiguous bytes per row and plane.
       const int nt = work % p.n_tiles;
-      const int mt = (PAIR ? 2 * (work / p.n_tiles) + static_cast<int>(rank) : work / p.n_tiles);
+      const int mt = work / p.n_tiles;
       const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
       const int x = tx * TILE_W + c, y = ty * TILE_H + r;
-      const bool valid = (mt < p.m_tiles) && (x < p.W) && (y < p.H) && (p.m_valid <= 0 || (y * p.W + x) < p.m_valid);
+      const bool valid = (x < p.W) && (y < p.H) && (p.m_valid <= 0 || (y * p.W + x) < p.m_valid);
       const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
       // element offset of this lane's row at channel 0 (non-shuffle) -- fits 32 bits for every tensor we produce
       const uint32_t row_base = static_cast<uint32_t>(((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.cout);
       const uint32_t row_out = static_cast<uint32_t>(((static_cast<size_t>(img) * p.H + y) * p.W + x) * p.ld_out + p.ch_off);
-      mbar_wait(&tfull_bar[buf], (full_phase >> buf) & 1u);
-      full_phase ^= (1u << buf);
-      tc_fence_after();
-      const bool xpose_path = (p.out_hi == nullptr);  // fp32-only traffic: coalesce through the transpose tile
-      for (int ci = grp; ci < NCH; ci += 4) {
-        const int ch0 = ci * 16;
-        const int n0 = nt * NT + ch0;
+      const bool xpose_path = (p.out_hi == nullptr);
+#pragma unroll
+      for (int ci = 0; ci < NW / 16; ++ci) {
+        const int n0 = nt * NT + wg * NW + ci * 16;
         if (n0 >= p.cout) break;  // columns past the last real output channel (cout not a multiple of NT): zero weights
         const int nvalid = p.cout - n0;  // >= 8, multiple of 8; < 16 only in the last chunk of such a layer
-        uint32_t rr[16];
-        tmem_ld_32x16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(buf * NT + ch0), rr);
-        tmem_ld_wait();
+        named_bar_sync(2 + wg, 128);  // the previous chunk's staging reads are done
+        stage_acc_cols<NW, 16, C::LD>(acc[0], S, 0, ci * 2);
+        stage_acc_cols<NW, 16, C::LD>(acc[1], S, 64, ci * 2);
+        named_bar_sync(2 + wg, 128);
         uint32_t o_lane;
         if (p.shuffle) {
           const int sub = n0 / cq, cc = n0 - sub * cq;
@@ -294,13 +233,6 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
         }
         const uint32_t o_out = p.shuffle ? o_lane : row_out + static_cast<uint32_t>(n0);  // where the outputs go
         if (xpose_path) {
-          // row `lane`, float4 slot s -> T[lane][s ^ ((lane >> 1) & 3)]: conflict-free 16-byte writes and reads
-#pragma unroll
-          for (int sl = 0; sl < 4; ++sl)
-            *reinterpret_cast<float4*>(T + lane * 16 + ((sl ^ ((lane >> 1) & 3)) << 2)) =
-                make_float4(__uint_as_float(rr[4 * sl]), __uint_as_float(rr[4 * sl + 1]), __uint_as_float(rr[4 * sl + 2]),
-                            __uint_as_float(rr[4 * sl + 3]));
-          __syncwarp();
           const int sl = lane & 3;  // this lane's float4 slot: channels n0 + 4 sl .. + 3
           const bool col_ok = 4 * sl < nvalid;
           const float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n0) + sl);  // shift[] is padded to n_tiles * NT
@@ -318,38 +250,38 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
           for (int k = 0; k < 4; ++k) {
             const int row = (lane >> 2) + 8 * k;
             if (!((vmask >> row) & 1u) || !col_ok) continue;
-            const float4 a4 = *reinterpret_cast<const float4*>(T + row * 16 + ((sl ^ ((row >> 1) & 3)) << 2));
-            float t[4] = {fmaf(a4.x, p.acc_scale, sh.x), fmaf(a4.y, p.acc_scale, sh.y), fmaf(a4.z, p.acc_scale, sh.z),
-                          fmaf(a4.w, p.acc_scale, sh.w)};
+            const float4 a4 = *reinterpret_cast<const float4*>(T + row * C::LD + 4 * sl);
+            float tt[4] = {fmaf(a4.x, p.acc_scale, sh.x), fmaf(a4.y, p.acc_scale, sh.y), fmaf(a4.z, p.acc_scale, sh.z),
+                           fmaf(a4.w, p.acc_scale, sh.w)};
             const float av[4] = {ad[k].x, ad[k].y, ad[k].z, ad[k].w};
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-              if (p.add_first) t[j] += av[j];
-              if (p.relu == 1) t[j] = fmaxf(t[j], 0.f);
-              else if (p.relu == 2) t[j] = 0.5f * t[j] * (1.f + erff(t[j] * 0.70710678118654752f));
-              else if (p.relu == 3) t[j] = t[j] * fminf(fmaxf(t[j] + 3.f, 0.f), 6.f) * (1.f / 6.f);
-              if (!p.add_first) t[j] += av[j];
+              if (p.add_first) tt[j] += av[j];
+              if (p.relu == 1) tt[j] = fmaxf(tt[j], 0.f);
+              else if (p.relu == 2) tt[j] = 0.5f * tt[j] * (1.f + erff(tt[j] * 0.70710678118654752f));
+              else if (p.relu == 3) tt[j] = tt[j] * fminf(fmaxf(tt[j] + 3.f, 0.f), 6.f) * (1.f / 6.f);
+              if (!p.add_first) tt[j] += av[j];
             }
-            if (p.y32) *reinterpret_cast<float4*>(p.y32 + oo[k]) = make_float4(t[0], t[1], t[2], t[3]);
+            if (p.y32) *reinterpret_cast<float4*>(p.y32 + oo[k]) = make_float4(tt[0], tt[1], tt[2], tt[3]);
           }
-          __syncwarp();
         } else if (valid) {
           // row-per-thread path (fp16 plane outputs: 32 contiguous bytes per row and plane)
           float v[16];
 #pragma unroll
           for (int j4 = 0; j4 < 4; ++j4) {
             const float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n0) + j4);
-            v[4 * j4] = fmaf(__uint_as_float(rr[4 * j4]), p.acc_scale, sh.x);
-            v[4 * j4 + 1] = fmaf(__uint_as_float(rr[4 * j4 + 1]), p.acc_scale, sh.y);
-            v[4 * j4 + 2] = fmaf(__uint_as_float(rr[4 * j4 + 2]), p.acc_scale, sh.z);
-            v[4 * j4 + 3] = fmaf(__uint_as_float(rr[4 * j4 + 3]), p.acc_scale, sh.w);
+            const float4 a4 = *reinterpret_cast<const float4*>(S + m * C::LD + 4 * j4);
+            v[4 * j4] = fmaf(a4.x, p.acc_scale, sh.x);
+            v[4 * j4 + 1] = fmaf(a4.y, p.acc_scale, sh.y);
+            v[4 * j4 + 2] = fmaf(a4.z, p.acc_scale, sh.z);
+            v[4 * j4 + 3] = fmaf(a4.w, p.acc_scale, sh.w);
           }
           if (p.add32 && p.add_first) {
 #pragma unroll
             for (int j4 = 0; j4 < 4; ++j4) {
               if (4 * j4 < nvalid) {
-                const float4 t = __ldg(reinterpret_cast<const float4*>(p.add32 + o_lane) + j4);
-                v[4 * j4] += t.x; v[4 * j4 + 1] += t.y; v[4 * j4 + 2] += t.z; v[4 * j4 + 3] += t.w;
+                const float4 a = __ldg(reinterpret_cast<const float4*>(p.add32 + o_lane) + j4);
+                v[4 * j4] += a.x; v[4 * j4 + 1] += a.y; v[4 * j4 + 2] += a.z; v[4 * j4 + 3] += a.w;
               }
             }
           }
@@ -367,8 +299,8 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
 #pragma unroll
             for (int j4 = 0; j4 < 4; ++j4) {
               if (4 * j4 < nvalid) {
-                const float4 t = __ldg(reinterpret_cast<const float4*>(p.add32 + o_lane) + j4);
-                v[4 * j4] += t.x; v[4 * j4 + 1] += t.y; v[4 * j4 + 2] += t.z; v[4 * j4 + 3] += t.w;
+                const float4 a = __ldg(reinterpret_cast<const float4*>(p.add32 + o_lane) + j4);
+                v[4 * j4] += a.x; v[4 * j4 + 1] += a.y; v[4 * j4 + 2] += a.z; v[4 * j4 + 3] += a.w;
               }
             }
           }
@@ -403,22 +335,8 @@ convgen_umma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_co
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[buf]), 0));
-        else mbar_arrive(&tempty_bar[buf]);
-      }
-      buf ^= 1;
     }
     if (overflow) atomicOr(p.status, 1);
-  }
-
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_pair(tmem_base, C::TMEM_COLS); else tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 

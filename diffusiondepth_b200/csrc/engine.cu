@@ -1,4 +1,4 @@
-// libddengine.so — C ABI (include/dd_engine.h) over the sm_100a kernels in conv_umma.cuh / kernels.cuh.
+// libddengine.so — C ABI (include/dd_engine.h) over the sm_90a kernels in conv_halo.cuh / convgen.cuh / kernels.cuh.
 // Host side: weight pre-pack, workspace carving, TMA descriptor construction, per-step launch schedule
 // (captured once into a CUDA graph), status polling.  No CPU compute path exists in this library.
 #include <cuda.h>
@@ -17,7 +17,6 @@
 #include "kernels.cuh"
 #include "convgen.cuh"
 #include "conv_halo.cuh"
-#include "conv_swap.cuh"
 #include "swin.cuh"
 #include "mpvit.cuh"
 
@@ -98,54 +97,6 @@ int make_strip_map(CUtensorMap* m, const __half* base, int B, int H, int W, int 
   if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(strip) failed: " + std::to_string((int)r));
   return DD_OK;
 }
-// e4m3 activation strip (fp8-correction planes): [B][H][W][C] bytes, box = {64, 8, 18, 1}: 64-byte rows, 64-byte swizzle
-int make_strip_map8(CUtensorMap* m, const uint8_t* base, int B, int H, int W, int C) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C, (cuuint64_t)W * C, (cuuint64_t)H * W * C};
-  cuuint32_t box[4] = {64, dd::HALO_TW, dd::HALO_TH + 2, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<uint8_t*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(e4m3 strip) failed: " + std::to_string((int)r));
-  return DD_OK;
-}
-// e4m3 weights: [9][COUT][CIN] bytes; box = {64, rows, 1}, 64-byte swizzle
-int make_w_map8(CUtensorMap* m, const uint8_t* base, int cout, int cin, int box_rows) {
-  cuuint64_t gdim[3] = {(cuuint64_t)cin, (cuuint64_t)cout, 9};
-  cuuint64_t gstr[2] = {(cuuint64_t)cin, (cuuint64_t)cout * cin};
-  cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(e4m3 weight) failed: " + std::to_string((int)r));
-  return DD_OK;
-}
-// 16x16 pixel patch for the swapped-operand kernel: box = {bk, 16, 16, 1}
-int make_patch_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bk, dd::SWAP_TW, dd::SWAP_TH, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(patch) failed: " + std::to_string((int)r));
-  return DD_OK;
-}
-// column-shifted strip for the row-halo variant of the swapped-operand kernel: box = {bk, 16, 18, 1}
-int make_swap_strip_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bk, dd::SWAP_TW, dd::SWAP_TH + 2, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(swap strip) failed: " + std::to_string((int)r));
-  return DD_OK;
-}
 // weights: [9][COUT][CIN] fp16; box = {bk, COUT, 1}
 int make_w_map(CUtensorMap* m, const __half* base, int cout, int cin, int bk, int box_rows = 0) {
   cuuint64_t gdim[3] = {(cuuint64_t)cin, (cuuint64_t)cout, 9};
@@ -174,147 +125,23 @@ int make_wgen_map(CUtensorMap* m, const __half* base, int cout, int cin, int tap
 
 // ---- conv shapes served by the engine
 struct ShapeInfo {
-  int cin, cout, bk;
+  int cin, cout;
 };
-constexpr ShapeInfo kShapes[5] = {{16, 64, 16}, {64, 256, 32}, {256, 256, 32}, {256, 64, 64}, {64, 16, 64}};
+constexpr ShapeInfo kShapes[5] = {{16, 64}, {64, 256}, {256, 256}, {256, 64}, {64, 16}};
 int shape_id(int cin, int cout) {
   for (int i = 0; i < 5; ++i)
     if (kShapes[i].cin == cin && kShapes[i].cout == cout) return i;
   return -1;
 }
 
-template <int CIN, int COUT, int BK, int EPI>
-cudaError_t configure_umma() {
-  using C = dd::ConvCfg<CIN, COUT, BK>;
-  return cudaFuncSetAttribute(dd::conv3x3_umma_kernel<CIN, COUT, BK, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              C::SMEM_BYTES);
-}
-template <int CIN, int COUT, int BK>
-cudaError_t configure_umma_all_epi() {
-  cudaError_t e;
-  if ((e = configure_umma<CIN, COUT, BK, dd::EPI_F32_STATS>()) != cudaSuccess) return e;
-  if ((e = configure_umma<CIN, COUT, BK, dd::EPI_SPLIT>()) != cudaSuccess) return e;
-  return configure_umma<CIN, COUT, BK, dd::EPI_F32>();
-}
-cudaError_t configure_all_kernels() {
-  cudaError_t e;
-  if ((e = cudaFuncSetAttribute(dd::window_attention_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::WAU_SMEM)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::DEC_SMEM)) != cudaSuccess)
-    return e;
-  if ((e = configure_umma_all_epi<16, 64, 16>()) != cudaSuccess) return e;
-  if ((e = configure_umma_all_epi<64, 256, 32>()) != cudaSuccess) return e;
-  if ((e = configure_umma_all_epi<256, 256, 32>()) != cudaSuccess) return e;
-  if ((e = configure_umma_all_epi<256, 64, 64>()) != cudaSuccess) return e;
-  if ((e = configure_umma_all_epi<64, 16, 64>()) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<256, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<192, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<192, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<128, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<64, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<256>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<192>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::convgen_umma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::GenCfg<128>::SMEM_BYTES)) != cudaSuccess) return e;
-  return cudaFuncSetAttribute(dd::convgen_umma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              dd::GenCfg<64>::SMEM_BYTES);
-}
-
-template <int CIN, int COUT, int BK, int EPI>
-cudaError_t launch_umma(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
-                        const CUtensorMap& b_lo, const dd::ConvArgs& args, int sm_count, cudaStream_t st) {
-  using C = dd::ConvCfg<CIN, COUT, BK>;
-  auto kern = dd::conv3x3_umma_kernel<CIN, COUT, BK, EPI>;  // smem attribute set in configure_all_kernels()
-  int grid = args.num_tiles < sm_count ? args.num_tiles : sm_count;
-  kern<<<grid, C::THREADS, C::SMEM_BYTES, st>>>(a_hi, a_lo, b_hi, b_lo, args);
-  return cudaGetLastError();
-}
 constexpr int kHaloBK[5] = {16, 32, 32, 32, 32};  // K chunk of the halo kernel per shape id
-constexpr int kSwapBK[5] = {16, 0, 0, 32, 32};    // K chunk of the swapped-operand kernel (narrow-N shapes only)
-// Which kernel serves which shape inside the engine when the flags allow it (measured, profiles/README.md,
-// tiny_probe.py): the swapped-operand kernel wins where MMA issue dominates (256->64: 356 vs 700 us; 64->16: 92 vs 129 us
-// with the quarter-local epilogue); 16->64: halo kernel with the weights resident in shared memory and two epilogue warp
-// sets, 82 us (classic 88, swap 182; its MMAs cost ~210 cycles each on 32-byte operand rows — padding K to 64-byte rows
-// through TMA zero fill was slower still, 110-125 us); row-halo reuse pays for the wide layers.
-constexpr bool kUseSwap[5] = {false, false, false, true, true};
-constexpr bool kUseHalo[5] = {true, true, true, false, false};
-// CTA pairs (cta_group::2, M = 256), measured (profiles/README.md, round 2 `ab_probe.py`, same box, 1 kW power cap):
-// 64->256 with two epilogue warp sets 262 us vs 362 us single-CTA; 256->256 948 us / 1.29 M cycles vs 1119 us / 1.56 M
-// cycles single-CTA (793 cycles per (chunk, tap) stage for 768 cycles of MMA work: the pair halves each SM's weight
-// traffic through shared memory, and since the TMA producers issue from an elected lane of a whole warp the two CTAs'
-// copies no longer trail the MMAs).  Round 1 had measured the 256->256 pair as equal: that was with lone-lane producers.
-constexpr bool kUsePair[5] = {false, true, true, false, false};
-template <int CIN, int COUT, int BK, int EPI, bool HALO = false>
-cudaError_t launch_swap(const CUtensorMap& p_hi, const CUtensorMap& p_lo, const CUtensorMap& w, const dd::ConvArgs& args,
-                        int sm_count, cudaStream_t st) {
-  using C = dd::SwapCfg<CIN, COUT, BK, HALO>;
-  int grid = args.num_tiles < sm_count ? args.num_tiles : sm_count;
-  dd::conv3x3_swap_kernel<CIN, COUT, BK, EPI, HALO><<<grid, 256, C::SMEM_BYTES, st>>>(p_hi, p_lo, w, args);
-  return cudaGetLastError();
-}
-template <int CIN, int COUT, int BK, bool HALO = false>
-cudaError_t configure_swap() {
-  using C = dd::SwapCfg<CIN, COUT, BK, HALO>;
-  cudaError_t e = cudaFuncSetAttribute(dd::conv3x3_swap_kernel<CIN, COUT, BK, dd::EPI_F32_STATS, HALO>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(dd::conv3x3_swap_kernel<CIN, COUT, BK, dd::EPI_F32, HALO>,
-                              cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
-}
-cudaError_t configure_swap_kernels() {
-  cudaError_t e;
-  if ((e = configure_swap<16, 64, 16>()) != cudaSuccess) return e;
-  if ((e = configure_swap<256, 64, 32>()) != cudaSuccess) return e;
-  if ((e = configure_swap<64, 16, 32>()) != cudaSuccess) return e;
-  if ((e = configure_swap<256, 64, 32, true>()) != cudaSuccess) return e;
-  return configure_swap<64, 16, 32, true>();
-}
 template <int CIN, int COUT, int BK, int EPI>
 cudaError_t launch_halo(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
                         const CUtensorMap& b_lo, const dd::ConvArgs& args, int sm_count, cudaStream_t st) {
   using C = dd::HaloCfg<CIN, COUT, BK>;
   int grid = args.num_tiles < sm_count ? args.num_tiles : sm_count;
-  dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(a_hi, a_lo, b_hi, b_lo, a_lo, b_lo, args);
+  dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(a_hi, a_lo, b_hi, b_lo, args);
   return cudaGetLastError();
-}
-// CTA-pair variant (cluster of 2, tcgen05 cta_group::2) of the halo kernel for the 256-wide layers.  F8: fp8 correction
-// products (a_lo / b_lo = the a8 / w8 maps, a_x / b_x = the l8 / lw8 maps).
-template <int CIN, int COUT, int BK, int EPI, bool F8 = false>
-cudaError_t launch_pair(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
-                        const CUtensorMap& b_lo, const dd::ConvArgs& args, int sm_count, cudaStream_t st,
-                        const CUtensorMap* a_x = nullptr, const CUtensorMap* b_x = nullptr) {
-  using C = dd::HaloCfg<CIN, COUT, BK, true, F8>;
-  int grid = ((args.num_tiles + 1) & ~1) < (sm_count & ~1) ? ((args.num_tiles + 1) & ~1) : (sm_count & ~1);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI, true, F8>, a_hi, a_lo, b_hi, b_lo,
-                            a_x ? *a_x : a_lo, b_x ? *b_x : b_lo, args);
-}
-template <int CIN, int COUT, int BK>
-cudaError_t configure_pair_all_epi() {
-  using C = dd::HaloCfg<CIN, COUT, BK, true>;
-  cudaError_t e;
-  if ((e = cudaFuncSetAttribute(dd::conv3x3_halo_kernel<CIN, COUT, BK, dd::EPI_F32_STATS, true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::conv3x3_halo_kernel<CIN, COUT, BK, dd::EPI_SPLIT, true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES)) != cudaSuccess) return e;
-  return cudaFuncSetAttribute(dd::conv3x3_halo_kernel<CIN, COUT, BK, dd::EPI_F32, true>,
-                              cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
 }
 template <int CIN, int COUT, int BK>
 cudaError_t configure_halo_all_epi() {
@@ -327,24 +154,26 @@ cudaError_t configure_halo_all_epi() {
   return cudaFuncSetAttribute(dd::conv3x3_halo_kernel<CIN, COUT, BK, dd::EPI_F32>,
                               cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
 }
-cudaError_t configure_halo_kernels() {
+template <int NT>
+cudaError_t configure_gen() {
+  return cudaFuncSetAttribute(dd::convgen_wgmma_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              dd::GenCfg<NT>::SMEM_BYTES);
+}
+cudaError_t configure_all_kernels() {
   cudaError_t e;
-  if ((e = cudaFuncSetAttribute(dd::conv3x3_halo_kernel<256, 256, 64, dd::EPI_SPLIT, true, true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::HaloCfg<256, 256, 64, true, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::conv3x3_halo_kernel<64, 256, 64, dd::EPI_F32_STATS, true, true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::HaloCfg<64, 256, 64, true, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = cudaFuncSetAttribute(dd::conv3x3_halo_kernel<256, 256, 64, dd::EPI_F32, true, true>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                dd::HaloCfg<256, 256, 64, true, true>::SMEM_BYTES)) != cudaSuccess) return e;
-  if ((e = configure_pair_all_epi<64, 256, 32>()) != cudaSuccess) return e;
-  if ((e = configure_pair_all_epi<256, 256, 32>()) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::window_attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                dd::WAU_SMEM)) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::DEC_SMEM)) != cudaSuccess)
+    return e;
   if ((e = configure_halo_all_epi<16, 64, 16>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<64, 256, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<256, 256, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<256, 64, 32>()) != cudaSuccess) return e;
-  return configure_halo_all_epi<64, 16, 32>();
+  if ((e = configure_halo_all_epi<64, 16, 32>()) != cudaSuccess) return e;
+  if ((e = configure_gen<256>()) != cudaSuccess) return e;
+  if ((e = configure_gen<192>()) != cudaSuccess) return e;
+  if ((e = configure_gen<128>()) != cudaSuccess) return e;
+  return configure_gen<64>();
 }
 
 template <int CIN, int COUT, int EPI>
@@ -362,13 +191,7 @@ struct ConvLayer {
   float* w_simt = nullptr;
   float* bias = nullptr;
   float wscale = 1.f;
-  CUtensorMap mb_hi, mb_lo;
-  CUtensorMap mh_hi, mh_lo;  // same planes, box for the halo kernel's K chunk
-  CUtensorMap mp_hi, mp_lo;  // same, box of COUT/2 rows for the CTA-pair kernel (256-wide layers)
-  __half* w_swap = nullptr;  // [9][128][CIN]: rows co = hi, 64+co = lo (swapped-operand kernel, narrow layers)
-  CUtensorMap mw_swap;
-  uint8_t *w8 = nullptr, *lw8 = nullptr;  // e4m3 correction planes [9][COUT][CIN] (DD_FLAG_FP8_CORR, the Cout = 256 layers)
-  CUtensorMap m8_hi, m8_w, m8_lw;         // 64-channel boxes of COUT / 2 rows (fp16 hi plane, e4m3 planes): CTA-pair fp8 kernel
+  CUtensorMap mh_hi, mh_lo;  // box for the halo kernel's K chunk
 };
 
 struct Raw {
@@ -385,9 +208,8 @@ struct GenLayer {
   float* shift = nullptr;
   float wscale = 1.f;
   CUtensorMap mb_hi, mb_lo;
-  CUtensorMap mp_hi, mp_lo;  // box of nt / 2 rows: each CTA of a pair stages half of the N tile
   bool alt = false;          // cout divisible by 256 and 192: run_gen picks the width whose last wave wastes least
-  CUtensorMap mb_hi_alt, mb_lo_alt, mp_hi_alt, mp_lo_alt;  // boxes of 192 / 96 rows
+  CUtensorMap mb_hi_alt, mb_lo_alt;  // boxes of 192 rows
 };
 struct Planes {
   __half* hi = nullptr;
@@ -402,7 +224,6 @@ struct Gemm {  // Linear layer on the tensor-core GEMM path: W [N][K] as fp16 hi
   CUtensorMap mb_hi, mb_lo;          // box {32, nt}
   bool alt = false;                  // N tiles by both 256 and 192: second pair of maps for the other width
   CUtensorMap mb_hi_alt, mb_lo_alt;  // box {32, 192}
-  CUtensorMap mp_hi, mp_lo, mp_hi_alt, mp_lo_alt;  // the same with boxes of nt / 2 rows (CTA pairs)
 };
 struct SwinBlockW {
   float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr, *table = nullptr;
@@ -495,14 +316,9 @@ struct dd_engine {
   int sm_count = 0;
   int up_qpb = 4;      // quads per block in gn_apply_up_split_kernel; DD_PROBES build: DD_UP_QPB=1 -> one 64-thread block per quad (A/B: equal)
   bool f8_ne3 = true;  // DD_PROBES build: DD_F8_NE3=0 keeps noise_embedding.3 on the 3-pass split (A/B timing)
-  unsigned long long* clk_probe = nullptr;  // DD_CLK_PROBE=1: per-launch SM cycles / nanoseconds (dd_bench_conv)
-  // tuning / timing probes: read from the environment ONCE in dd_create, and only in a -DDD_PROBES build
-  // (profiles/README.md); a product build ignores the variables altogether
-  int probe_fp8 = 0, swap_mask = -1, halo_mask = -1, pair_mask = -1;
-  int genpair_mask = 1;  // DD_GENPAIR=0 (probes build): producer convs / GEMMs on single CTAs
-  int swaphalo_mask = 1; // DD_SWAPHALO=0 (probes build): narrow layers on the plain swapped-operand kernel
+  // tuning switches: read from the environment ONCE in dd_create, and only in a -DDD_PROBES build; a product build
+  // ignores the variables altogether
   int attn_simt = 0;     // DD_ATTN_SIMT=1 (probes build): window attention on the fp32 CUDA-core kernel
-  bool want_clk_probe = false;
   bool weights_ready = false;
   std::map<std::string, Raw> raw;
   // packed parameters (device memory owned by the engine)
@@ -738,11 +554,9 @@ size_t carve(dd_engine* e, void* base) {
 // f8 bit 0: the INPUT planes are hi / a8 / l8 (in_lo = base of the e4m3 pair: a8, then l8 B*P*cin bytes further) and the
 // conv runs with fp8 correction products; bit 1: the OUTPUT planes are written as hi / a8 / l8 (out_lo = their base).
 constexpr int kF8In = 1, kF8Out = 2;
-bool fp8_active(const dd_engine* e) {  // the wide convs of the Swin variant, on the CTA-pair halo kernel only
-  const int need = DD_FLAG_FP8_CORR | DD_FLAG_HALO_CONV | DD_FLAG_PAIR_WIDE;
-  return (e->cfg.flags & need) == need && !(e->cfg.flags & DD_FLAG_SIMT_CONV) && e->cfg.variant == DD_VARIANT_SWIN &&
-         e->pair_mask < 0 && e->halo_mask < 0;
-}
+// DD_FLAG_FP8_CORR is accepted and runs the exact 3-pass split: Hopper's e4m3 wgmma accumulates with reduced precision,
+// so correction products added into the running fp32 sum of the hi * hi product would be lost.
+bool fp8_active(const dd_engine*) { return false; }
 int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, float in_scale, int epi, float* y32,
              float* stats_partial, __half* out_hi, __half* out_lo, cudaStream_t st, int f8 = 0) {
   const Geom g = geom_of(e->cfg);
@@ -768,63 +582,21 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
   }
   a.split_scale = kActScale;
   a.status = e->status;
-  a.fp8_probe = e->probe_fp8;
-  a.clk_probe = e->clk_probe;
   cudaError_t err = cudaSuccess;
   e->launches++;
   int which = -1;
   for (int i = 0; i < 4; ++i)
     if (stats_partial == e->stats[i]) which = i;
   if (which >= 0) e->stats_tiles_img[which] = g.tiles_img;
-  const bool swap_here = e->swap_mask >= 0 ? ((e->swap_mask >> L.sid) & 1) : kUseSwap[L.sid];
-  const bool use_swap = (e->cfg.flags & DD_FLAG_SWAP_NARROW) && !(e->cfg.flags & DD_FLAG_SIMT_CONV) &&
-                        swap_here && kSwapBK[L.sid] > 0 && epi != dd::EPI_SPLIT;
-  const bool halo_here = e->halo_mask >= 0 ? ((e->halo_mask >> L.sid) & 1) : kUseHalo[L.sid];
-  const bool use_halo = (e->cfg.flags & DD_FLAG_HALO_CONV) && !(e->cfg.flags & DD_FLAG_SIMT_CONV) && halo_here;
-  if (!use_swap) {  // tile geometry of the kernel actually launched
-    const int tw = use_halo ? dd::HALO_TW : dd::TILE_W, th = use_halo ? dd::HALO_TH : dd::TILE_H;
-    a.tiles_x = (g.w + tw - 1) / tw;
-    a.tiles_y = (g.h + th - 1) / th;
+  const bool use_tc = !(e->cfg.flags & DD_FLAG_SIMT_CONV);
+  if (use_tc) {  // tile geometry of the tensor-core kernel
+    a.tiles_x = (g.w + dd::HALO_TW - 1) / dd::HALO_TW;
+    a.tiles_y = (g.h + dd::HALO_TH - 1) / dd::HALO_TH;
     a.num_tiles = a.tiles_x * a.tiles_y * g.B;
     if (which >= 0) e->stats_tiles_img[which] = a.tiles_x * a.tiles_y;
   }
-  if (f8 && !use_halo) return fail(DD_ERR_INVALID, "fp8-correction planes need the row-halo CTA-pair kernel");
-  if (use_swap) {
-    a.tiles_x = (g.w + dd::SWAP_TW - 1) / dd::SWAP_TW;
-    a.tiles_y = (g.h + dd::SWAP_TH - 1) / dd::SWAP_TH;
-    a.num_tiles = a.tiles_x * a.tiles_y * g.B;
-    if (which >= 0) e->stats_tiles_img[which] = a.tiles_x * a.tiles_y;
-    CUtensorMap mp_hi, mp_lo;
-    int rc;
-    const int bk = kSwapBK[L.sid];
-    // row-halo variant (three column-shifted strips per chunk instead of nine shifted patches) for the 32-channel-chunk
-    // layers when the engine runs the halo kernels at all
-    const bool swap_halo = (e->cfg.flags & DD_FLAG_HALO_CONV) && bk == 32 && e->swaphalo_mask != 0;
-    if (swap_halo) {
-      if ((rc = make_swap_strip_map(&mp_hi, in_hi, g.B, g.h, g.w, s.cin, bk))) return rc;
-      if ((rc = make_swap_strip_map(&mp_lo, in_lo, g.B, g.h, g.w, s.cin, bk))) return rc;
-    } else {
-      if ((rc = make_patch_map(&mp_hi, in_hi, g.B, g.h, g.w, s.cin, bk))) return rc;
-      if ((rc = make_patch_map(&mp_lo, in_lo, g.B, g.h, g.w, s.cin, bk))) return rc;
-    }
-    const bool st_ = (epi == dd::EPI_F32_STATS);
-    if (swap_halo) {
-      switch (L.sid) {
-        case 3: err = st_ ? launch_swap<256, 64, 32, dd::EPI_F32_STATS, true>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st)
-                          : launch_swap<256, 64, 32, dd::EPI_F32, true>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st); break;
-        case 4: err = st_ ? launch_swap<64, 16, 32, dd::EPI_F32_STATS, true>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st)
-                          : launch_swap<64, 16, 32, dd::EPI_F32, true>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st); break;
-      }
-    } else
-    switch (L.sid) {
-      case 0: err = st_ ? launch_swap<16, 64, 16, dd::EPI_F32_STATS>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st)
-                        : launch_swap<16, 64, 16, dd::EPI_F32>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st); break;
-      case 3: err = st_ ? launch_swap<256, 64, 32, dd::EPI_F32_STATS>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st)
-                        : launch_swap<256, 64, 32, dd::EPI_F32>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st); break;
-      case 4: err = st_ ? launch_swap<64, 16, 32, dd::EPI_F32_STATS>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st)
-                        : launch_swap<64, 16, 32, dd::EPI_F32>(mp_hi, mp_lo, L.mw_swap, a, e->sm_count, st); break;
-    }
-  } else if (e->cfg.flags & DD_FLAG_SIMT_CONV) {
+  if (f8 && !use_tc) return fail(DD_ERR_INVALID, "fp8-correction planes need the tensor-core kernel");
+  if (!use_tc) {
     dd::SimtArgs sa;
     sa.in_hi = in_hi;
     sa.in_lo = in_lo;
@@ -845,44 +617,14 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
       SIMT_CASE(4, 64, 16)
     }
 #undef SIMT_CASE
-  } else if (use_halo) {
+  } else {
     CUtensorMap ma_hi, ma_lo;
     int rc;
     const int hbk = kHaloBK[L.sid];
     if ((rc = make_strip_map(&ma_hi, in_hi, g.B, g.h, g.w, s.cin, hbk))) return rc;
-    if (!(f8 & kF8In))
-      if ((rc = make_strip_map(&ma_lo, in_lo, g.B, g.h, g.w, s.cin, hbk))) return rc;
-    const bool use_pair = (e->cfg.flags & DD_FLAG_PAIR_WIDE) &&
-                          (e->pair_mask >= 0 ? ((e->pair_mask >> L.sid) & 1) && s.cout == 256 : kUsePair[L.sid]);
-    if ((f8 & kF8In) && !(use_pair && L.w8 && ((L.sid == 2 && epi != dd::EPI_F32_STATS) || (L.sid == 1 && epi == dd::EPI_F32_STATS))))
-      return fail(DD_ERR_INVALID, "fp8-correction planes fed to a layer / kernel that does not take them");
-    if ((f8 & kF8Out) && epi != dd::EPI_SPLIT) return fail(DD_ERR_INVALID, "fp8 output planes need the split epilogue");
-    if (f8 & kF8In) {
-      const uint8_t* a8 = reinterpret_cast<const uint8_t*>(in_lo);
-      CUtensorMap m_hi64, m_a8, m_l8;
-      if ((rc = make_strip_map(&m_hi64, in_hi, g.B, g.h, g.w, s.cin, 64))) return rc;
-      if ((rc = make_strip_map8(&m_a8, a8, g.B, g.h, g.w, s.cin))) return rc;
-      if ((rc = make_strip_map8(&m_l8, a8 + static_cast<size_t>(g.B) * g.P * s.cin, g.B, g.h, g.w, s.cin))) return rc;
-      err = (L.sid == 1)
-                ? launch_pair<64, 256, 64, dd::EPI_F32_STATS, true>(m_hi64, m_a8, L.m8_hi, L.m8_w, a, e->sm_count, st, &m_l8, &L.m8_lw)
-            : (epi == dd::EPI_SPLIT)
-                ? launch_pair<256, 256, 64, dd::EPI_SPLIT, true>(m_hi64, m_a8, L.m8_hi, L.m8_w, a, e->sm_count, st, &m_l8, &L.m8_lw)
-                : launch_pair<256, 256, 64, dd::EPI_F32, true>(m_hi64, m_a8, L.m8_hi, L.m8_w, a, e->sm_count, st, &m_l8, &L.m8_lw);
-    } else if (use_pair) {
-#define PAIR_CASE(ID, CI, CO, BK)                                                                                   \
-  case ID:                                                                                                          \
-    err = (epi == dd::EPI_F32_STATS)                                                                                \
-              ? launch_pair<CI, CO, BK, dd::EPI_F32_STATS>(ma_hi, ma_lo, L.mp_hi, L.mp_lo, a, e->sm_count, st)      \
-          : (epi == dd::EPI_SPLIT)                                                                                  \
-              ? launch_pair<CI, CO, BK, dd::EPI_SPLIT>(ma_hi, ma_lo, L.mp_hi, L.mp_lo, a, e->sm_count, st)          \
-              : launch_pair<CI, CO, BK, dd::EPI_F32>(ma_hi, ma_lo, L.mp_hi, L.mp_lo, a, e->sm_count, st);           \
-    break;
-      switch (L.sid) {
-        PAIR_CASE(1, 64, 256, 32)
-        PAIR_CASE(2, 256, 256, 32)
-      }
-#undef PAIR_CASE
-    } else {
+    if ((rc = make_strip_map(&ma_lo, in_lo, g.B, g.h, g.w, s.cin, hbk))) return rc;
+    if (f8) return fail(DD_ERR_INVALID, "fp8-correction planes are not supported by the sm_90a kernels");
+    {
 #define HALO_CASE(ID, CI, CO, BK)                                                                                   \
   case ID:                                                                                                          \
     err = (epi == dd::EPI_F32_STATS)                                                                                \
@@ -891,36 +633,15 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
               ? launch_halo<CI, CO, BK, dd::EPI_SPLIT>(ma_hi, ma_lo, L.mh_hi, L.mh_lo, a, e->sm_count, st)          \
               : launch_halo<CI, CO, BK, dd::EPI_F32>(ma_hi, ma_lo, L.mh_hi, L.mh_lo, a, e->sm_count, st);           \
     break;
-    switch (L.sid) {
-      HALO_CASE(0, 16, 64, 16)
-      HALO_CASE(1, 64, 256, 32)
-      HALO_CASE(2, 256, 256, 32)
-      HALO_CASE(3, 256, 64, 32)
-      HALO_CASE(4, 64, 16, 32)
-    }
+      switch (L.sid) {
+        HALO_CASE(0, 16, 64, 16)
+        HALO_CASE(1, 64, 256, 32)
+        HALO_CASE(2, 256, 256, 32)
+        HALO_CASE(3, 256, 64, 32)
+        HALO_CASE(4, 64, 16, 32)
+      }
 #undef HALO_CASE
     }
-  } else {
-    CUtensorMap ma_hi, ma_lo;
-    int rc;
-    if ((rc = make_act_map(&ma_hi, in_hi, g.B, g.h, g.w, s.cin, s.bk))) return rc;
-    if ((rc = make_act_map(&ma_lo, in_lo, g.B, g.h, g.w, s.cin, s.bk))) return rc;
-#define UMMA_CASE(ID, CI, CO, BK)                                                                                   \
-  case ID:                                                                                                          \
-    err = (epi == dd::EPI_F32_STATS)                                                                                \
-              ? launch_umma<CI, CO, BK, dd::EPI_F32_STATS>(ma_hi, ma_lo, L.mb_hi, L.mb_lo, a, e->sm_count, st)      \
-          : (epi == dd::EPI_SPLIT)                                                                                  \
-              ? launch_umma<CI, CO, BK, dd::EPI_SPLIT>(ma_hi, ma_lo, L.mb_hi, L.mb_lo, a, e->sm_count, st)          \
-              : launch_umma<CI, CO, BK, dd::EPI_F32>(ma_hi, ma_lo, L.mb_hi, L.mb_lo, a, e->sm_count, st);           \
-    break;
-    switch (L.sid) {
-      UMMA_CASE(0, 16, 64, 16)
-      UMMA_CASE(1, 64, 256, 32)
-      UMMA_CASE(2, 256, 256, 32)
-      UMMA_CASE(3, 256, 64, 64)
-      UMMA_CASE(4, 64, 16, 64)
-    }
-#undef UMMA_CASE
   }
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(err));
   return DD_OK;
@@ -1061,7 +782,7 @@ int transpose_out(const float* nhwc, float* nchw, int B, int C, int P, cudaStrea
 int split_planes(dd_engine* e, const float* x, __half* hi, __half* lo, size_t n, float scale, cudaStream_t st) {
   const size_t n4 = n / 4;
   int blocks = static_cast<int>((n4 + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   dd::split_planes_kernel<<<blocks, 256, 0, st>>>(x, hi, lo, n4, scale, e->status);
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("split_planes: ") + cudaGetErrorString(err));
@@ -1136,29 +857,8 @@ int pack_layer(dd_engine* e, ConvLayer& L, const float* w, const float* b, int c
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpyAsync(L.bias, b, cout * 4, cudaMemcpyDeviceToDevice, st));
   const ShapeInfo s = kShapes[L.sid];
-  if ((rc = make_w_map(&L.mb_hi, L.w_hi, cout, cin, s.bk))) return rc;
-  if ((rc = make_w_map(&L.mb_lo, L.w_lo, cout, cin, s.bk))) return rc;
   if ((rc = make_w_map(&L.mh_hi, L.w_hi, cout, cin, kHaloBK[L.sid]))) return rc;
   if ((rc = make_w_map(&L.mh_lo, L.w_lo, cout, cin, kHaloBK[L.sid]))) return rc;
-  if (cout == 256) {
-    if ((rc = make_w_map(&L.mp_hi, L.w_hi, cout, cin, kHaloBK[L.sid], cout / 2))) return rc;
-    if ((rc = make_w_map(&L.mp_lo, L.w_lo, cout, cin, kHaloBK[L.sid], cout / 2))) return rc;
-  }
-  if (cout == 256 && cin % 64 == 0) {  // fp8-correction planes (used when the engine runs with DD_FLAG_FP8_CORR)
-    if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w8), n))) return rc;
-    if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.lw8), n))) return rc;
-    dd::pack_conv_weight8_kernel<<<128, 256, 0, st>>>(w, L.w8, L.lw8, cout, cin, scale);
-    CUDA_TRY(cudaGetLastError());
-    if ((rc = make_w_map(&L.m8_hi, L.w_hi, cout, cin, 64, cout / 2))) return rc;
-    if ((rc = make_w_map8(&L.m8_w, L.w8, cout, cin, cout / 2))) return rc;
-    if ((rc = make_w_map8(&L.m8_lw, L.lw8, cout, cin, cout / 2))) return rc;
-  }
-  if (kSwapBK[L.sid] > 0) {
-    if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_swap), static_cast<size_t>(9) * 128 * cin * 2))) return rc;
-    dd::pack_swap_weight_kernel<<<128, 256, 0, st>>>(w, L.w_swap, cout, cin, scale);
-    CUDA_TRY(cudaGetLastError());
-    if ((rc = make_w_map(&L.mw_swap, L.w_swap, 128, cin, kSwapBK[L.sid]))) return rc;
-  }
   return DD_OK;
 }
 
@@ -1254,14 +954,10 @@ int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::stri
   CUDA_TRY(cudaStreamSynchronize(st));
   if ((rc = make_wgen_map(&L.mb_hi, L.w_hi, L.cout, cp, L.taps, L.nt))) return rc;
   if ((rc = make_wgen_map(&L.mb_lo, L.w_lo, L.cout, cp, L.taps, L.nt))) return rc;
-  if ((rc = make_wgen_map(&L.mp_hi, L.w_hi, L.cout, cp, L.taps, L.nt / 2))) return rc;
-  if ((rc = make_wgen_map(&L.mp_lo, L.w_lo, L.cout, cp, L.taps, L.nt / 2))) return rc;
   L.alt = (L.nt == 256 && L.cout % 256 == 0 && L.cout % 192 == 0 && !L.shuffle);
   if (L.alt) {
     if ((rc = make_wgen_map(&L.mb_hi_alt, L.w_hi, L.cout, cp, L.taps, 192))) return rc;
     if ((rc = make_wgen_map(&L.mb_lo_alt, L.w_lo, L.cout, cp, L.taps, 192))) return rc;
-    if ((rc = make_wgen_map(&L.mp_hi_alt, L.w_hi, L.cout, cp, L.taps, 96))) return rc;
-    if ((rc = make_wgen_map(&L.mp_lo_alt, L.w_lo, L.cout, cp, L.taps, 96))) return rc;
   }
   return DD_OK;
 }
@@ -1290,45 +986,21 @@ int pack_producers(dd_engine* e, cudaStream_t st, float* scratch) {
   return DD_OK;
 }
 
-template <int NT, bool PAIR>
+template <int NT>
 cudaError_t launch_gen(int grid, cudaStream_t st, const CUtensorMap& m0h, const CUtensorMap& m0l, const CUtensorMap& m1h,
                        const CUtensorMap& m1l, const CUtensorMap& bh, const CUtensorMap& bl, const dd::GenConvArgs& a) {
-  if constexpr (!PAIR) {
-    dd::convgen_umma_kernel<NT, false><<<grid, dd::GenCfg<NT, false>::THREADS, dd::GenCfg<NT, false>::SMEM_BYTES, st>>>(m0h, m0l, m1h, m1l, bh, bl, a);
-    return cudaGetLastError();
-  } else {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(dd::GenCfg<NT, true>::THREADS);
-    cfg.dynamicSmemBytes = dd::GenCfg<NT, true>::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2;
-    at[0].val.clusterDim.y = 1;
-    at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, dd::convgen_umma_kernel<NT, true>, m0h, m0l, m1h, m1l, bh, bl, a);
-  }
+  dd::convgen_wgmma_kernel<NT><<<grid, dd::GenCfg<NT>::THREADS, dd::GenCfg<NT>::SMEM_BYTES, st>>>(m0h, m0l, m1h, m1l, bh, bl, a);
+  return cudaGetLastError();
 }
-// m_tiles x n_tiles work items of one producer conv / GEMM -> (use CTA pairs?, grid size).  Pairs (M = 256 per
-// tcgen05.mma, half the weight bytes per SM) whenever there are at least two M tiles and the engine allows it.
-bool gen_use_pair(const dd_engine* e, int m_tiles) {
-  return (e->cfg.flags & DD_FLAG_PAIR_WIDE) && !(e->cfg.flags & DD_FLAG_SIMT_CONV) && m_tiles >= 2 && e->genpair_mask != 0;
-}
-int gen_grid(const dd_engine* e, bool pair, int m_tiles, int n_tiles) {
-  if (!pair) return std::min(m_tiles * n_tiles, e->sm_count);
-  return std::min(2 * ((m_tiles + 1) / 2) * n_tiles, e->sm_count & ~1);
-}
-cudaError_t launch_gen_nt(int nt, bool pair, int grid, cudaStream_t st, const CUtensorMap& m0h, const CUtensorMap& m0l,
+int gen_grid(const dd_engine* e, int m_tiles, int n_tiles) { return std::min(m_tiles * n_tiles, e->sm_count); }
+cudaError_t launch_gen_nt(int nt, int grid, cudaStream_t st, const CUtensorMap& m0h, const CUtensorMap& m0l,
                           const CUtensorMap& m1h, const CUtensorMap& m1l, const CUtensorMap& bh, const CUtensorMap& bl,
                           const dd::GenConvArgs& a) {
   switch (nt) {
-    case 256: return pair ? launch_gen<256, true>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a) : launch_gen<256, false>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-    case 192: return pair ? launch_gen<192, true>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a) : launch_gen<192, false>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-    case 128: return pair ? launch_gen<128, true>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a) : launch_gen<128, false>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-    default: return pair ? launch_gen<64, true>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a) : launch_gen<64, false>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
+    case 256: return launch_gen<256>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
+    case 192: return launch_gen<192>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
+    case 128: return launch_gen<128>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
+    default: return launch_gen<64>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
   }
 }
 
@@ -1346,10 +1018,9 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
   a.m_tiles = a.tiles_x * a.tiles_y * B;
   // wave quantisation (as in run_gemm): with few M tiles pick the N-tile width whose last wave wastes least — the
   // level-2 fusion conv of the HAHI neck (768 channels, 30 tile pairs) runs 2 waves of 192 columns instead of 2 of 256
-  const bool pair = gen_use_pair(e, a.m_tiles);
   int nt = L.nt;
   if (L.alt) {
-    const int units = pair ? (a.m_tiles + 1) / 2 : a.m_tiles, slots = pair ? e->sm_count / 2 : e->sm_count;
+    const int units = a.m_tiles, slots = e->sm_count;
     auto cost = [&](int w) { return ((units * (L.cout / w) + slots - 1) / slots) * w; };
     if (cost(192) < cost(256)) nt = 192;
   }
@@ -1391,11 +1062,10 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
     m1h = m0h;
     m1l = m0l;
   }
-  const int grid = gen_grid(e, pair, a.m_tiles, a.n_tiles);
+  const int grid = gen_grid(e, a.m_tiles, a.n_tiles);
   const bool use_alt = nt != L.nt;
-  const cudaError_t err = launch_gen_nt(nt, pair, grid, st, m0h, m0l, m1h, m1l,
-                                        pair ? (use_alt ? L.mp_hi_alt : L.mp_hi) : (use_alt ? L.mb_hi_alt : L.mb_hi),
-                                        pair ? (use_alt ? L.mp_lo_alt : L.mp_lo) : (use_alt ? L.mb_lo_alt : L.mb_lo), a);
+  const cudaError_t err = launch_gen_nt(nt, grid, st, m0h, m0l, m1h, m1l, use_alt ? L.mb_hi_alt : L.mb_hi,
+                                        use_alt ? L.mb_lo_alt : L.mb_lo, a);
   e->launches++;
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("convgen launch: ") + cudaGetErrorString(err));
   return DD_OK;
@@ -1439,7 +1109,7 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
   {
     const size_t n = static_cast<size_t>(B) * r.H * r.W * dd::GEN_BK;
     int blocks = static_cast<int>((n + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     dd::rgb_to_planes_kernel<<<blocks, 256, 0, st>>>(rgb, r.IN.hi, r.IN.lo, B, r.H * r.W, kProdScale, e->status);
     e->launches++;
     CUDA_TRY(cudaGetLastError());
@@ -1536,14 +1206,10 @@ int pack_gemm(dd_engine* e, Gemm& G, const std::string& wkey, const std::string&
   CUDA_TRY(cudaGetLastError());
   if ((rc = make_wgen_map(&G.mb_hi, G.w_hi, N, K, 1, G.nt))) return rc;
   if ((rc = make_wgen_map(&G.mb_lo, G.w_lo, N, K, 1, G.nt))) return rc;
-  if ((rc = make_wgen_map(&G.mp_hi, G.w_hi, N, K, 1, G.nt / 2))) return rc;
-  if ((rc = make_wgen_map(&G.mp_lo, G.w_lo, N, K, 1, G.nt / 2))) return rc;
   G.alt = (G.nt == 256 && N % 256 == 0 && N % 192 == 0);
   if (G.alt) {
     if ((rc = make_wgen_map(&G.mb_hi_alt, G.w_hi, N, K, 1, 192))) return rc;
     if ((rc = make_wgen_map(&G.mb_lo_alt, G.w_lo, N, K, 1, 192))) return rc;
-    if ((rc = make_wgen_map(&G.mp_hi_alt, G.w_hi, N, K, 1, 96))) return rc;
-    if ((rc = make_wgen_map(&G.mp_lo_alt, G.w_lo, N, K, 1, 96))) return rc;
   }
   return DD_OK;
 }
@@ -1599,15 +1265,14 @@ int run_gemm(dd_engine* e, const Gemm& G, const Planes& A, int M, int act, float
   a.tiles_y = (a.H + dd::TILE_H - 1) / dd::TILE_H;
   a.m_tiles = a.tiles_y;
   // wave quantisation: with few M tiles (deep Swin stages) pick the N-tile width whose last wave wastes least
-  const bool pair = gen_use_pair(e, a.m_tiles);
-  const int units = pair ? (a.m_tiles + 1) / 2 : a.m_tiles, slots = pair ? e->sm_count / 2 : e->sm_count;
+  const int units = a.m_tiles, slots = e->sm_count;
   int nt = G.nt;
   if (G.alt) {
     auto cost = [&](int w) { return ((units * (G.N / w) + slots - 1) / slots) * w; };
     if (cost(192) < cost(256)) nt = 192;
   }
-  const CUtensorMap& mbh = pair ? ((nt == G.nt) ? G.mp_hi : G.mp_hi_alt) : ((nt == G.nt) ? G.mb_hi : G.mb_hi_alt);
-  const CUtensorMap& mbl = pair ? ((nt == G.nt) ? G.mp_lo : G.mp_lo_alt) : ((nt == G.nt) ? G.mb_lo : G.mb_lo_alt);
+  const CUtensorMap& mbh = (nt == G.nt) ? G.mb_hi : G.mb_hi_alt;
+  const CUtensorMap& mbl = (nt == G.nt) ? G.mb_lo : G.mb_lo_alt;
   a.n_tiles = (G.N + nt - 1) / nt;
   a.kc0 = (G.K + dd::GEN_BK - 1) / dd::GEN_BK;
   a.kc1 = 0;
@@ -1633,8 +1298,8 @@ int run_gemm(dd_engine* e, const Gemm& G, const Planes& A, int M, int act, float
   int rc;
   if ((rc = make_act_map(&mh, A.hi, 1, a.H, 16, G.K, dd::GEN_BK))) return rc;
   if ((rc = make_act_map(&ml, A.lo, 1, a.H, 16, G.K, dd::GEN_BK))) return rc;
-  const int grid = gen_grid(e, pair, a.m_tiles, a.n_tiles);
-  const cudaError_t err = launch_gen_nt(nt, pair, grid, st, mh, ml, mh, ml, mbh, mbl, a);
+  const int grid = gen_grid(e, a.m_tiles, a.n_tiles);
+  const cudaError_t err = launch_gen_nt(nt, grid, st, mh, ml, mh, ml, mbh, mbl, a);
   e->launches++;
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("gemm launch: ") + cudaGetErrorString(err));
   return DD_OK;
@@ -1689,10 +1354,10 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
       aa.status = e->status;
       if ((e->cfg.flags & DD_FLAG_SIMT_CONV) || (nH & 1) || e->attn_simt) {  // fp32 CUDA-core check path
         dd::window_attention_kernel<<<B * aa.nWx * aa.nWy * nH, 64, 0, st>>>(aa);
-      } else {  // tcgen05: pairs of heads of one window per M = 128 tile, three persistent CTAs per SM
+      } else {  // wgmma: pairs of heads of one window per M = 128 tile, two persistent CTAs per SM
         const int pairs = B * aa.nWx * aa.nWy * (nH / 2);
-        const int grid = pairs < 3 * e->sm_count ? pairs : 3 * e->sm_count;
-        dd::window_attention_umma_kernel<<<grid, 128, dd::WAU_SMEM, st>>>(aa, pairs);
+        const int grid = pairs < 2 * e->sm_count ? pairs : 2 * e->sm_count;
+        dd::window_attention_wgmma_kernel<<<grid, 128, dd::WAU_SMEM, st>>>(aa, pairs);
       }
       e->launches++;
       CUDA_TRY(cudaGetLastError());
@@ -1745,7 +1410,8 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
   if (cfg->device < 0 || cfg->device >= ndev) return fail(DD_ERR_INVALID, "bad device ordinal");
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return fail(DD_ERR_UNSUPPORTED, "libddengine is built for sm_100a (Blackwell B200) only");
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(DD_ERR_UNSUPPORTED, "libddengine is built for sm_90a (Hopper H100) only");
   CUDA_TRY(cudaSetDevice(cfg->device));
   int rc;
   if ((rc = load_driver())) return rc;
@@ -1753,21 +1419,13 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
 #ifdef DD_PROBES
-  if (const char* v = getenv("DD_FP8_PROBE")) e->probe_fp8 = atoi(v);
-  if (const char* v = getenv("DD_SWAP_MASK")) e->swap_mask = atoi(v);
-  if (const char* v = getenv("DD_HALO_MASK")) e->halo_mask = atoi(v);
-  if (const char* v = getenv("DD_PAIR_MASK")) e->pair_mask = atoi(v);
-  if (const char* v = getenv("DD_GENPAIR")) e->genpair_mask = atoi(v);
-  if (const char* v = getenv("DD_SWAPHALO")) e->swaphalo_mask = atoi(v);
   if (const char* v = getenv("DD_ATTN_SIMT")) e->attn_simt = atoi(v);
-  e->want_clk_probe = getenv("DD_CLK_PROBE") != nullptr;
   if (const char* v = getenv("DD_F8_NE3")) e->f8_ne3 = atoi(v) != 0;
   if (const char* v = getenv("DD_UP_QPB")) e->up_qpb = atoi(v);
 #endif
   if (cudaMallocHost(&e->status_host, 64) != cudaSuccess ||
       cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking) != cudaSuccess ||
-      configure_all_kernels() != cudaSuccess || configure_halo_kernels() != cudaSuccess ||
-      configure_swap_kernels() != cudaSuccess) {
+      configure_all_kernels() != cudaSuccess) {
     std::string msg = std::string("engine setup failed: ") + cudaGetErrorString(cudaGetLastError());
     if (e->status_host) cudaFreeHost(e->status_host);
     if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
@@ -2162,7 +1820,7 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
       if (p.resample) {  // F.adaptive_avg_pool2d(conv_up(pre_x), output_size = lateral size)  (reference head :121)
         const size_t n = static_cast<size_t>(B) * p.H[i - 1] * p.W[i - 1] * 256;
         int blocks = static_cast<int>((n + 255) / 256);
-        if (blocks > 148 * 16) blocks = 148 * 16;
+        if (blocks > 132 * 16) blocks = 132 * 16;
         dd::adaptive_avg_pool_nhwc_kernel<<<blocks, 256, 0, s>>>(up_raw, p.UP[i - 1], B, 2 * p.H[i], 2 * p.W[i], p.H[i - 1],
                                                                  p.W[i - 1], 256);
         h->launches++;
@@ -2313,7 +1971,7 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
 }
 
 // Debug / tuning aid: time the GEMM-mode kernel on synthetic planes.  mode: 0 fp32 out, 1 fp32 out + residual add,
-// 2 GELU -> planes, 3 no output at all (mainloop + TMEM drain only).
+// 2 GELU -> planes, 3 no output at all (mainloop + accumulator drain only).
 int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, int32_t iters, float* ms_out) {
   if (!h || !ms_out || M < 1 || K % dd::GEN_BK || N % 192 && N % 256) return fail(DD_ERR_INVALID, "bad argument");
   CUDA_TRY(cudaSetDevice(h->cfg.device));
@@ -2346,8 +2004,6 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   int rc;
   if ((rc = make_wgen_map(&G.mb_hi, G.w_hi, N, K, 1, G.nt))) return rc;
   if ((rc = make_wgen_map(&G.mb_lo, G.w_lo, N, K, 1, G.nt))) return rc;
-  if ((rc = make_wgen_map(&G.mp_hi, G.w_hi, N, K, 1, G.nt / 2))) return rc;
-  if ((rc = make_wgen_map(&G.mp_lo, G.w_lo, N, K, 1, G.nt / 2))) return rc;
   int* saved = h->status;
   h->status = status;
   auto once = [&]() {
@@ -2423,7 +2079,6 @@ size_t dd_conv3x3_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int3
   add(nw * 2);
   add(nw * 2);
   add(nw * 4);
-  add(static_cast<size_t>(9) * 128 * cin * 2);  // swapped-operand weight tile
   return align_up(off, 1024);
 }
 
@@ -2448,7 +2103,6 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   __half* whi = c.take<__half>(nw);
   __half* wlo = c.take<__half>(nw);
   float* wsimt = c.take<float>(nw);
-  __half* wswap = c.take<__half>(static_cast<size_t>(9) * 128 * cin);
   CUDA_TRY(cudaMemsetAsync(status, 0, 64, st));
   int rc;
   if ((rc = transpose_in(x, xn, batch, cin, height * width, st))) return rc;
@@ -2462,7 +2116,7 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
     return (amax > 0.f && isfinite(amax)) ? exp2f(floorf(log2f(32768.f / amax)) - 1.f) : 1.f;
   };
   const float sx = pow2_scale(am[0]), sw = pow2_scale(am[1]);
-  dd::split_planes_kernel<<<148 * 8, 256, 0, st>>>(xn, hi, lo, BP * cin / 4, sx, status);
+  dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(xn, hi, lo, BP * cin / 4, sx, status);
   dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, whi, wlo, wsimt, cout, cin, sw);
   CUDA_TRY(cudaGetLastError());
   dd::ConvArgs a;
@@ -2481,10 +2135,7 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   a.out_a8 = a.out_l8 = nullptr;
   a.split_scale = 1.f;
   a.status = status;
-  a.fp8_probe = 0;
-  a.clk_probe = nullptr;
   cudaError_t err = cudaSuccess;
-  const ShapeInfo s = kShapes[sid];
   if (h->cfg.flags & DD_FLAG_SIMT_CONV) {
     dd::SimtArgs sa;
     sa.in_hi = hi;
@@ -2499,57 +2150,7 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
       case 3: err = launch_simt<256, 64, dd::EPI_F32>(sa, st); break;
       case 4: err = launch_simt<64, 16, dd::EPI_F32>(sa, st); break;
     }
-  } else if ((h->cfg.flags & DD_FLAG_SWAP_NARROW) && kSwapBK[sid] > 0) {
-    CUtensorMap mp_hi, mp_lo, mw;
-    const int bk = kSwapBK[sid];
-    a.tiles_x = (width + dd::SWAP_TW - 1) / dd::SWAP_TW;
-    a.tiles_y = (height + dd::SWAP_TH - 1) / dd::SWAP_TH;
-    a.num_tiles = a.tiles_x * a.tiles_y * batch;
-    __half* wsw = wswap;
-    dd::pack_swap_weight_kernel<<<128, 256, 0, st>>>(w, wsw, cout, cin, sw);
-    CUDA_TRY(cudaGetLastError());
-    const bool swap_halo = (h->cfg.flags & DD_FLAG_HALO_CONV) && bk == 32 && h->swaphalo_mask != 0;
-    if (swap_halo) {
-      if ((rc = make_swap_strip_map(&mp_hi, hi, batch, height, width, cin, bk))) return rc;
-      if ((rc = make_swap_strip_map(&mp_lo, lo, batch, height, width, cin, bk))) return rc;
-    } else {
-      if ((rc = make_patch_map(&mp_hi, hi, batch, height, width, cin, bk))) return rc;
-      if ((rc = make_patch_map(&mp_lo, lo, batch, height, width, cin, bk))) return rc;
-    }
-    if ((rc = make_w_map(&mw, wsw, 128, cin, bk))) return rc;
-    if (swap_halo) {
-      err = sid == 3 ? launch_swap<256, 64, 32, dd::EPI_F32, true>(mp_hi, mp_lo, mw, a, h->sm_count, st)
-                     : launch_swap<64, 16, 32, dd::EPI_F32, true>(mp_hi, mp_lo, mw, a, h->sm_count, st);
-    } else
-    switch (sid) {
-      case 0: err = launch_swap<16, 64, 16, dd::EPI_F32>(mp_hi, mp_lo, mw, a, h->sm_count, st); break;
-      case 3: err = launch_swap<256, 64, 32, dd::EPI_F32>(mp_hi, mp_lo, mw, a, h->sm_count, st); break;
-      case 4: err = launch_swap<64, 16, 32, dd::EPI_F32>(mp_hi, mp_lo, mw, a, h->sm_count, st); break;
-    }
-  } else if (fp8_active(h) && cin == 256 && cout == 256) {
-    // fp8-correction kernel on a standalone layer (tests): the e4m3 planes reuse the fp16 lo plane's storage, the
-    // weight planes that of the SIMT copy; x is re-split with a scale that keeps |s x| / 4 inside e4m3
-    const float sx8 = (am[0] > 0.f && isfinite(am[0])) ? exp2f(floorf(log2f(1024.f / am[0]))) : 1.f;
-    uint8_t* a8 = reinterpret_cast<uint8_t*>(lo);
-    uint8_t* l8 = a8 + BP * cin;
-    uint8_t* w8 = reinterpret_cast<uint8_t*>(wsimt);
-    uint8_t* lw8 = w8 + nw;
-    dd::split_planes8_kernel<<<148 * 8, 256, 0, st>>>(xn, hi, a8, l8, BP * cin / 8, sx8, status);
-    dd::pack_conv_weight8_kernel<<<128, 256, 0, st>>>(w, w8, lw8, cout, cin, sw);
-    CUDA_TRY(cudaGetLastError());
-    a.acc_scale = 1.f / (sx8 * sw);
-    a.tiles_x = (width + dd::HALO_TW - 1) / dd::HALO_TW;
-    a.tiles_y = (height + dd::HALO_TH - 1) / dd::HALO_TH;
-    a.num_tiles = a.tiles_x * a.tiles_y * batch;
-    CUtensorMap ma_hi, m_a8, m_l8, mb_hi, m_w8, m_lw8;
-    if ((rc = make_strip_map(&ma_hi, hi, batch, height, width, cin, 64))) return rc;
-    if ((rc = make_strip_map8(&m_a8, a8, batch, height, width, cin))) return rc;
-    if ((rc = make_strip_map8(&m_l8, l8, batch, height, width, cin))) return rc;
-    if ((rc = make_w_map(&mb_hi, whi, cout, cin, 64, cout / 2))) return rc;
-    if ((rc = make_w_map8(&m_w8, w8, cout, cin, cout / 2))) return rc;
-    if ((rc = make_w_map8(&m_lw8, lw8, cout, cin, cout / 2))) return rc;
-    err = launch_pair<256, 256, 64, dd::EPI_F32, true>(ma_hi, m_a8, mb_hi, m_w8, a, h->sm_count, st, &m_l8, &m_lw8);
-  } else if (h->cfg.flags & DD_FLAG_HALO_CONV) {
+  } else {
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
     const int hbk = kHaloBK[sid];
     a.tiles_x = (width + dd::HALO_TW - 1) / dd::HALO_TW;
@@ -2557,32 +2158,14 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
     a.num_tiles = a.tiles_x * a.tiles_y * batch;
     if ((rc = make_strip_map(&ma_hi, hi, batch, height, width, cin, hbk))) return rc;
     if ((rc = make_strip_map(&ma_lo, lo, batch, height, width, cin, hbk))) return rc;
-    const bool pair = (h->cfg.flags & DD_FLAG_PAIR_WIDE) && cout == 256;
-    if ((rc = make_w_map(&mb_hi, whi, cout, cin, hbk, pair ? cout / 2 : 0))) return rc;
-    if ((rc = make_w_map(&mb_lo, wlo, cout, cin, hbk, pair ? cout / 2 : 0))) return rc;
-    if (pair) {
-      err = sid == 1 ? launch_pair<64, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st)
-                     : launch_pair<256, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st);
-    } else
+    if ((rc = make_w_map(&mb_hi, whi, cout, cin, hbk))) return rc;
+    if ((rc = make_w_map(&mb_lo, wlo, cout, cin, hbk))) return rc;
     switch (sid) {
       case 0: err = launch_halo<16, 64, 16, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
       case 1: err = launch_halo<64, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
       case 2: err = launch_halo<256, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
       case 3: err = launch_halo<256, 64, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
       case 4: err = launch_halo<64, 16, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-    }
-  } else {
-    CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-    if ((rc = make_act_map(&ma_hi, hi, batch, height, width, cin, s.bk))) return rc;
-    if ((rc = make_act_map(&ma_lo, lo, batch, height, width, cin, s.bk))) return rc;
-    if ((rc = make_w_map(&mb_hi, whi, cout, cin, s.bk))) return rc;
-    if ((rc = make_w_map(&mb_lo, wlo, cout, cin, s.bk))) return rc;
-    switch (sid) {
-      case 0: err = launch_umma<16, 64, 16, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 1: err = launch_umma<64, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 2: err = launch_umma<256, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 3: err = launch_umma<256, 64, 64, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 4: err = launch_umma<64, 16, 64, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
     }
   }
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(err));
@@ -2613,8 +2196,6 @@ int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* 
     if ((rc = run_conv(h, layer, in_hi, in_lo, kActScale, split_out ? dd::EPI_SPLIT : dd::EPI_F32_STATS, h->Y,
                        h->stats[0], h->S_hi[0], h->S_lo[0], st, f8)))
       return rc;
-  if (h->want_clk_probe && !h->clk_probe) CUDA_TRY(cudaMalloc(&h->clk_probe, 16));
-  if (h->clk_probe) CUDA_TRY(cudaMemsetAsync(h->clk_probe, 0, 16, st));
   CUDA_TRY(cudaEventRecord(e0, st));
   for (int i = 0; i < iters; ++i)
     if ((rc = run_conv(h, layer, in_hi, in_lo, kActScale, split_out ? dd::EPI_SPLIT : dd::EPI_F32_STATS, h->Y,
@@ -2626,15 +2207,6 @@ int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* 
   CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
-  if (h->clk_probe) {
-    unsigned long long v[2] = {0, 0};
-    CUDA_TRY(cudaMemcpy(v, h->clk_probe, 16, cudaMemcpyDeviceToHost));
-    if (v[1])
-      fprintf(stderr, "[clk_probe] conv %d->%d: %.0f SM cycles, %.1f us per launch (CTA 0) => %.0f MHz\n", cin, cout,
-              double(v[0]) / iters, double(v[1]) / iters * 1e-3, double(v[0]) / double(v[1]) * 1e3);
-    cudaFree(h->clk_probe);
-    h->clk_probe = nullptr;
-  }
   *ms_out = ms / iters;
   return DD_OK;
 }

@@ -5,7 +5,7 @@
 #pragma once
 #include <type_traits>
 
-#include "conv_umma.cuh"
+#include "conv_common.cuh"
 
 #include "ptx.cuh"
 
@@ -316,11 +316,8 @@ __global__ void __launch_bounds__(256) gn_apply_split_kernel(const ApplyArgs a) 
 }
 
 // Swin-head variant of the above for C = 256 with the bilinear (align_corners=True) condition injection, organised around
-// SOURCE REUSE IN REGISTERS.  ncu on the tiled versions (profiles/r02_loop_convs_ncu_full_summary_session1.csv): DRAM traffic
-// was exactly algorithmic (548 MB read, 381 MB written) at 51 % of the DRAM peak while `l1tex__throughput` sat at 92 %: every
-// output pixel pulled its four 1 KB taps out of shared memory, 4 KB of shared-memory reads per KB of output, and neither
-// staging the conv outputs by cp.async.bulk nor a persistent three-stage ring moved it (267 -> 244 -> 246 us inside the
-// replayed graph, profiles/README.md "Round 2, session 2").  With the condition at half the latent resolution the 2 x 2 output
+// SOURCE REUSE IN REGISTERS.  A tiled version pulls every output pixel's four 1 KB taps out of shared memory (4 KB of
+// shared-memory reads per KB of output) and is bound by L1, not DRAM.  With the condition at half the latent resolution the 2 x 2 output
 // "quad" (rows 2i-1, 2i; columns 2j-1, 2j) interpolates from the SAME 2 x 2 source pixels (i-1, i) x (j-1, j).  64 threads x
 // 4 channels = one quad x 256 channels: they load the four source pixels and the quad's (up to) four conv outputs straight
 // from global memory into registers (8 x LDG.128 per thread in flight, coalesced 1 KB rows, no shared memory), fold the
@@ -390,11 +387,7 @@ __device__ __forceinline__ Lerp1 lerp_coord(float ratio, int o, int n_src) {
   return r;
 }
 
-// V = channels per thread (4: 64 threads per quad, 80 registers, 3 blocks of 256 threads per SM).  Measured variants that
-// changed nothing inside the graph (profiles/README.md, session 2): 8 channels per thread / one warp per quad (128
-// registers, 2 blocks: 214.5 vs 214.5 us, and convA behind it 30 us slower), one quad per 64-thread block so that the
-// quad's scalars are warp-uniform (189-216 vs 201-220 us).  ncu at 1.89 GHz: 185 us, DRAM 61 % of its peak, issue-active
-// 72 %, ALU pipe 57 %: at the power-capped clock of the replayed graph the kernel is issue-bound on its per-quad scalar work.
+// V = channels per thread (4: 64 threads per quad, 80 registers, 3 blocks of 256 threads per SM; 8 = one warp per quad).
 template <int V>
 __device__ __forceinline__ void ldv(const float* p, float (&v)[V]) {
 #pragma unroll
@@ -565,7 +558,7 @@ __global__ void __launch_bounds__(256) gn_relu_ddim_kernel(const FinalArgs a) {
 }
 
 // ------------------------------------------------------------------ fp32 CUDA-core 3x3 conv (validation / DD_FLAG_SIMT_CONV)
-// Same operands and epilogues as the tcgen05 kernel: input fp16 hi/lo planes (x = (hi+lo)/scale), weights fp32
+// Same operands and epilogues as the tensor-core kernel: input fp16 hi/lo planes (x = (hi+lo)/scale), weights fp32
 // [tap][CIN][COUT].  One block = one 8x16 pixel tile x CO_T output channels.
 struct SimtArgs {
   const __half* in_hi;
@@ -701,8 +694,8 @@ struct DecoderArgs {
 };
 constexpr int DEC_TH = 8, DEC_TW = 32;
 constexpr int DEC_SMEM = ((DEC_TH / 2 + 2) * (DEC_TW / 2 + 2) * 16 + (DEC_TH + 2) * (DEC_TW + 2) * 20 + 4096 + 144 + 16) * 4;
-// Round 2 (ncu: the first version spent 618 us per call with the shared-memory pipe 96 % busy — scalar weight reads in
-// the transposed conv, two scalar reads per FMA in the final conv): the transposed conv walks the intermediate pixels
+// Scalar weight reads in the transposed conv and two scalar reads per FMA in the final conv keep the shared-memory pipe
+// saturated, so the transposed conv walks the intermediate pixels
 // PARITY CLASS by parity class, so a warp's (ky, kx) taps and output-channel half are uniform and the folded weights come
 // in as broadcast float4s (2 x LDS.128 + 1 latent read per 8 FMAs); the final conv reads both the intermediate (row stride
 // 20 floats: conflict-free 16-byte reads) and its weights as float4s (8 x LDS.128 per 16 FMAs).

@@ -1,5 +1,5 @@
 // MPViT backbone (reference src/model/backbone/mpvit.py:57-741): the pieces that are not GEMMs.  Every 1x1 conv and Linear
-// of the network runs on convgen_umma_kernel (3-pass fp16 split on tcgen05); what is left is HBM/L2-bound pointwise and
+// of the network runs on convgen_wgmma_kernel (3-pass fp16 split on wgmma); what is left is HBM/L2-bound pointwise and
 // stencil work on fp32 NHWC token maps [B, H, W, C]:
 //   dwconv_nhwc_kernel        depthwise k x k (stride 1 / 2), + bias / folded eval-BN, Hardswish, residual (ConvPosEnc),
 //                             fp32 and / or fp16 hi/lo plane outputs                      (:125-175, :241-259, :482-532)
@@ -144,8 +144,7 @@ __global__ void __launch_bounds__(256) ln_split_generic_kernel(const float* __re
 // ------------------------------------------------------------------------------------------------ factorised attention
 // qkv: fp32 [B][N][3C] (q | k | v, each head-major h * Ch + c).  Token chunks: chunk j of image b covers tokens
 // [j * tpc, min(N, (j + 1) * tpc)).  Launch order per layer: ksoftmax_partial -> ktv_partial -> ktv_combine ->
-// factor_att_apply (first round-2 version: 5 kernels, the apply one with 53 blocks of scalar gathers took 275 us on the
-// deepest stage; ncu launch list profiles/r02_launches_mpvit_B1.csv).
+// factor_att_apply.
 
 // per (image, chunk, channel of k): running max m and sum s = sum exp(k - m) over the chunk's tokens.  256 threads =
 // (256 / C) token slices x C channels; the slices of a channel are merged in slice order.
@@ -205,7 +204,7 @@ __global__ void __launch_bounds__(256) ksoftmax_partial_kernel(const float* __re
 // The block first folds the chunk partials of its k columns into colmax (chunk 0's blocks also store 1 / sum exp for
 // ktv_combine).  256 threads own <= KTV_NP (h, c1, c2) entries each; the host picks HB with HB Ch^2 <= 4096 and
 // HB Ch <= KTV_W, so that the high-resolution stages (Ch = 8, 16) take all 8 heads in one block (one block per head left
-// 64 threads with 32 FMAs between two barriers: 397 us on stage 0).  Tokens are staged 32 at a time.
+// 64 threads with 32 FMAs between two barriers).  Tokens are staged 32 at a time.
 constexpr int KTV_NP = 16;
 constexpr int KTV_T = 32;
 constexpr int KTV_W = 160;
@@ -310,7 +309,7 @@ __global__ void __launch_bounds__(256) ktv_combine_kernel(const float* __restric
 // with float4 loads (the table holds every channel's window centred in a 7 x 7 layout, zeros outside), k^T v and the
 // token's q row come through L1.  One block = a 16 x 8 pixel tile x 64 channels, so that the window overlap of neighbouring
 // pixels in BOTH directions is served by L1 (22 x 14 x 256 B = 79 KB per block: 2.4x the tile instead of the 10x that
-// 16-token row segments pulled from L2 — 252 us per launch on stages 0-2 at B = 4).
+// 16-token row segments pull from L2).
 struct FactorApplyArgs {
   const float* qkv;     // [B][N][3C]
   const float* ktv;     // [B][heads][Ch][Ch]

@@ -1,4 +1,4 @@
-// Swin Transformer pieces that are not GEMMs (the GEMMs run on convgen_umma_kernel in "GEMM mode"):
+// Swin Transformer pieces that are not GEMMs (the GEMMs run on convgen_wgmma_kernel in "GEMM mode"):
 // patch embedding (4x4/s4 conv + LayerNorm), LayerNorm -> fp16 hi/lo planes, 2x2 patch-merge gather + LayerNorm,
 // 7x7 (shifted-)window attention with relative-position bias and the reference's finite -100 shift mask,
 // per-stage output LayerNorm written straight into the neck's input planes.
@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__
 // ------------------------------------------------------------------ patch embed: conv 4x4 s4 (3 -> E) + bias + LayerNorm(E)
 // rgb fp32 NCHW [B,3,H,W] (zero right/bottom pad to a multiple of 4) -> x fp32 [B*Hp*Wp][E].  One block of E threads =
 // PE_TOK consecutive tokens of one token row: their 3 x 4 image rows are 12 contiguous runs of 4 * PE_TOK floats, loaded
-// coalesced into shared memory (ncu, round 2: the per-token gather of the first version kept L1 at 90 % for 366 us);
+// coalesced into shared memory (a per-token gather keeps L1 saturated);
 // thread e then holds the 48 weights of output channel e and walks the tokens 8 at a time.
 constexpr int PE_TOK = 32;
 template <int E>
@@ -315,28 +315,27 @@ __global__ void __launch_bounds__(64) window_attention_kernel(const AttnArgs a) 
 }
 
 
-// ------------------------------------------------------------------ (shifted) 7x7 window attention on tcgen05
-// QK^T and PV as 3-pass fp16-split UMMAs with fp32 accumulators in TMEM; softmax in registers.  One persistent CTA
-// (128 threads = 128 TMEM lanes) walks PAIRS of (window, head) units — the two units of a pair are two consecutive
-// heads of the same window — and thread t owns row t: unit t / 64, query t % 64 (49 real rows, 15 zero rows).
+// ------------------------------------------------------------------ (shifted) 7x7 window attention on wgmma
+// QK^T and PV as 3-pass fp16-split warpgroup MMAs with fp32 register accumulators; softmax in registers.  One
+// persistent CTA (128 threads = one warpgroup) walks PAIRS of (window, head) units — the two units of a pair are two
+// consecutive heads of the same window — and after each product thread t owns row t: unit t / 64, query t % 64 (49
+// real rows, 15 zero rows).
 //   gather   q (pre-scaled by head_dim^-0.5), k, v rows from the fp32 qkv stream (padded tokens carry the qkv bias,
 //            exactly as in window_attention_kernel), split into fp16 hi / lo planes and WRITE them into shared memory in
-//            the swizzled K-major layouts the tensor core reads: Q [128 x 32] and K_u [64 x 32] with 64-byte rows
-//            (16-byte chunk c of row r at chunk c ^ ((r >> 1) & 3)), V_u transposed [32 dims x 64 keys] with 128-byte
-//            rows (chunk c ^ (r & 7));
-//   S        D_S[u] (TMEM columns 64 u ..) = Q K_u^T: 3 passes x 2 K-steps, M = 128, N = 64; only unit u's 64 rows of D_S[u]
-//            are meaningful (the other half is the cross product with the other head and is never read);
-//   softmax  each thread loads its row (tcgen05.ld), adds relative-position bias and the finite -100 shift mask, takes
-//            the softmax over the 49 keys in fp32 and writes P (x 4096) as hi / lo planes [128 x 64], 128-byte rows;
-//   O        D_O[u] (TMEM columns 32 u .., over S) = P V_u: 3 passes x 4 K-steps, M = 128, N = 32;
-//   store    each thread loads its 32 outputs, splits them and writes the proj GEMM's input planes.
-// 36 small MMAs per pair (~105 cycles each: N <= 64 is floor-bound) against ~2 x 3.1 k SM cycles of fp32 FMAs in the
-// SIMT kernel; three CTAs per SM overlap one's softmax with the others' gathers and MMAs.  Replaces reference swin.py:150-189 / 250-325.
-// P re-uses the Q / K tiles (they are dead once the S MMAs have completed) and O re-uses the S columns of TMEM (every row of S is
-// in registers by then): 50 KB of shared memory and 128 TMEM columns per CTA, so three CTAs fit an SM at 168 registers per thread
-// (measured: 2 CTAs 2.59 ms, 3 CTAs 2.08 ms, 4 CTAs at 128 registers 2.28 ms per 4 maps): the phases of a pair are serialised
-// inside a CTA, the overlap comes from its neighbours.
-constexpr int WAU_SMEM = 32768 /*Q + K, then P*/ + 16384 /*Vt*/ + 1024 /*align*/ + 1024 /*ctrl*/;
+//            the swizzled K-major layouts wgmma reads: Q [128 x 32] and K_u [64 x 32] with 64-byte rows (16-byte chunk
+//            c of row r at chunk c ^ ((r >> 1) & 3)), V_u transposed [32 dims x 64 keys] with 128-byte rows (chunk
+//            c ^ (r & 7));
+//   S        S_u = Q_u K_u^T: 3 passes x 2 K-steps of m64n64k16 per unit;
+//   softmax  the accumulators go through a shared-memory staging tile so that each thread holds its row; it adds the
+//            relative-position bias and the finite -100 shift mask, takes the softmax over the 49 keys in fp32 and writes
+//            P (x 4096) as hi / lo planes [128 x 64], 128-byte rows;
+//   O        O_u = P_u V_u: 3 passes x 4 K-steps of m64n32k16 per unit;
+//   store    staged again, each thread splits its 32 outputs and writes the proj GEMM's input planes.
+// P re-uses the Q / K tiles (they are dead once the S products have completed).  Replaces reference swin.py:150-189 /
+// 250-325.
+constexpr int WAU_LD_S = 65, WAU_LD_O = 33;  // staging row strides (floats): conflict-free row reads
+constexpr int WAU_SMEM = 32768 /*Q + K, then P*/ + 16384 /*Vt*/ + 128 * WAU_LD_S * 4 /*staging*/ + 1024 /*align*/ +
+                         1024 /*ctrl*/;
 __device__ __forceinline__ void wau_split8(const float* v, float scale, uint4& hi, uint4& lo, bool& ov) {
   __align__(16) __half2 h[4];
   __align__(16) __half2 l[4];
@@ -353,41 +352,23 @@ __device__ __forceinline__ void wau_split8(const float* v, float scale, uint4& h
   hi = *reinterpret_cast<const uint4*>(h);
   lo = *reinterpret_cast<const uint4*>(l);
 }
-__global__ void __launch_bounds__(128, 3) window_attention_umma_kernel(const AttnArgs a, int num_pairs) {
+__global__ void __launch_bounds__(128, 2) window_attention_wgmma_kernel(const AttnArgs a, int num_pairs) {
   constexpr int WS = 7, N = 49, D = 32;
   constexpr float kP = 4096.f;  // probabilities are split at this scale
   extern __shared__ uint8_t wau_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wau_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                 // [plane][128 rows][64 B]
   uint8_t* sK = smem + 16384;         // [unit][plane][64 rows][64 B]
-  uint8_t* sP = smem;                 // [plane][128 rows][128 B]: over Q and K, written after the S MMAs have completed
+  uint8_t* sP = smem;                 // [plane][128 rows][128 B]: over Q and K, written after the S products have completed
   uint8_t* sV = smem + 32768;         // [unit][plane][32 rows][128 B]
-  uint8_t* ctrl = smem + 49152;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(ctrl);            // [0] S done, [1] O done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ctrl + 16);
-  int* s_tok = reinterpret_cast<int*>(ctrl + 64);               // [49] source token or -1
+  float* stg = reinterpret_cast<float*>(smem + 49152);          // [128][WAU_LD_S] (S), then [128][WAU_LD_O] (O)
+  uint8_t* ctrl = smem + 49152 + 128 * WAU_LD_S * 4;
+  int* s_tok = reinterpret_cast<int*>(ctrl);                    // [49] source token or -1
   int* s_reg = s_tok + 64;                                      // [49] shift-mask region id
-  const int t = threadIdx.x, warp = t >> 5;
+  const int t = threadIdx.x;
   const int u = t >> 6, i = t & 63;                             // unit within the pair, query row
-  if (t == 0) {
-    mbar_init(&bar[0], 1);
-    mbar_init(&bar[1], 1);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const bool leader_warp = (warp == 1);
-  const bool leader = leader_warp && elect_one();
-  constexpr uint32_t idesc_s = umma_idesc_f16(128, 64), idesc_o = umma_idesc_f16(128, 32);
   const float qscale = rsqrtf(static_cast<float>(D));
   const int heads_half = a.nH >> 1;
-  uint32_t phase = 0;
   bool ov = false;
   for (int pair = blockIdx.x; pair < num_pairs; pair += gridDim.x) {
     const int hp = pair % heads_half, win = pair / heads_half;
@@ -455,45 +436,36 @@ __global__ void __launch_bounds__(128, 3) window_attention_umma_kernel(const Att
       }
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    // ---------------------------------------------------------------- S = Q K^T  (lo*hi, hi*hi, hi*lo per K-step)
-    if (leader_warp) {
-      tc_fence_after();
-      if (leader) {
-        const uint32_t q_hi = smem_u32(sQ), q_lo = q_hi + 8192;
-#pragma unroll
-        for (int uu = 0; uu < 2; ++uu) {
-          const uint32_t k_hi = smem_u32(sK) + uu * 8192, k_lo = k_hi + 4096;
-          const uint32_t d_s = tmem_base + uu * 64;
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            umma_f16(d_s, umma_smem_desc(q_lo + k * 32, 64), umma_smem_desc(k_hi + k * 32, 64), idesc_s, k ? 1u : 0u);
-            umma_f16(d_s, umma_smem_desc(q_hi + k * 32, 64), umma_smem_desc(k_hi + k * 32, 64), idesc_s, 1u);
-            umma_f16(d_s, umma_smem_desc(q_hi + k * 32, 64), umma_smem_desc(k_lo + k * 32, 64), idesc_s, 1u);
-          }
-        }
-        umma_commit(&bar[0]);
-      }
-      __syncwarp();
-    }
-    mbar_wait(&bar[0], phase);
-    tc_fence_after();
-    // ---------------------------------------------------------------- softmax of row (u, i)
+    // ---------------------------------------------------------------- S_u = Q_u K_u^T  (lo*hi, hi*lo, hi*hi per K-step)
     float pr[64];
     {
-      uint32_t r0[32], r1[32];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + static_cast<uint32_t>(u * 64);
-      tmem_ld_32x32(taddr, r0);
-      tmem_ld_32x32(taddr + 32, r1);
-      tmem_ld_wait();
+      float sacc[2][32];
+      wgmma_fence();
+      const uint32_t q_hi = smem_u32(sQ), q_lo = q_hi + 8192;
+#pragma unroll
+      for (int uu = 0; uu < 2; ++uu) {
+        const uint32_t k_hi = smem_u32(sK) + uu * 8192, k_lo = k_hi + 4096;
+        const uint32_t qo = uu * 64 * 64;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          wgmma_f16<64>(sacc[uu], wgmma_desc(q_lo + qo + k * 32, 64), wgmma_desc(k_hi + k * 32, 64), k ? 1u : 0u);
+          wgmma_f16<64>(sacc[uu], wgmma_desc(q_hi + qo + k * 32, 64), wgmma_desc(k_lo + k * 32, 64), 1u);
+          wgmma_f16<64>(sacc[uu], wgmma_desc(q_hi + qo + k * 32, 64), wgmma_desc(k_hi + k * 32, 64), 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(sacc[0]);
+      wgmma_fence_regs(sacc[1]);
+      stage_acc_cols<64, 64, WAU_LD_S>(sacc[0], stg, 0, 0);
+      stage_acc_cols<64, 64, WAU_LD_S>(sacc[1], stg, 64, 0);
+      __syncthreads();
       const float inv = 1.f / (a.scale_out * a.scale_out);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        pr[j] = __uint_as_float(r0[j]) * inv;
-        pr[32 + j] = __uint_as_float(r1[j]) * inv;
-      }
+      for (int j = 0; j < 64; ++j) pr[j] = stg[t * WAU_LD_S + j] * inv;
     }
+    // ---------------------------------------------------------------- softmax of row (u, i)
     if (i < N) {
       const int iy = i / WS, ix = i - iy * WS;
       const int my_reg = s_reg[i];
@@ -522,6 +494,7 @@ __global__ void __launch_bounds__(128, 3) window_attention_umma_kernel(const Att
 #pragma unroll
       for (int j = 0; j < 64; ++j) pr[j] = 0.f;
     }
+    __syncthreads();  // every thread has read its S row: the staging tile is free again
     {
       const uint32_t rp = static_cast<uint32_t>(t);
       bool dummy = false;
@@ -535,34 +508,30 @@ __global__ void __launch_bounds__(128, 3) window_attention_umma_kernel(const Att
       }
     }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    // ---------------------------------------------------------------- O = P V
-    if (leader_warp) {
-      tc_fence_after();
-      if (leader) {
-        const uint32_t p_hi = smem_u32(sP), p_lo = p_hi + 16384;
-#pragma unroll
-        for (int uu = 0; uu < 2; ++uu) {
-          const uint32_t v_hi = smem_u32(sV) + uu * 8192, v_lo = v_hi + 4096;
-          const uint32_t d_o = tmem_base + uu * 32;  // over the S columns: all of S is in registers by now
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            umma_f16(d_o, umma_smem_desc(p_lo + k * 32, 128), umma_smem_desc(v_hi + k * 32, 128), idesc_o, k ? 1u : 0u);
-            umma_f16(d_o, umma_smem_desc(p_hi + k * 32, 128), umma_smem_desc(v_hi + k * 32, 128), idesc_o, 1u);
-            umma_f16(d_o, umma_smem_desc(p_hi + k * 32, 128), umma_smem_desc(v_lo + k * 32, 128), idesc_o, 1u);
-          }
-        }
-        umma_commit(&bar[1]);
-      }
-      __syncwarp();
-    }
-    mbar_wait(&bar[1], phase);
-    tc_fence_after();
+    // ---------------------------------------------------------------- O_u = P_u V_u
     {
-      uint32_t ro[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + static_cast<uint32_t>(u * 32), ro);
-      tmem_ld_wait();
+      float oacc[2][16];
+      wgmma_fence();
+      const uint32_t p_hi = smem_u32(sP), p_lo = p_hi + 16384;
+#pragma unroll
+      for (int uu = 0; uu < 2; ++uu) {
+        const uint32_t v_hi = smem_u32(sV) + uu * 8192, v_lo = v_hi + 4096;
+        const uint32_t po = uu * 64 * 128;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_f16<32>(oacc[uu], wgmma_desc(p_lo + po + k * 32, 128), wgmma_desc(v_hi + k * 32, 128), k ? 1u : 0u);
+          wgmma_f16<32>(oacc[uu], wgmma_desc(p_hi + po + k * 32, 128), wgmma_desc(v_lo + k * 32, 128), 1u);
+          wgmma_f16<32>(oacc[uu], wgmma_desc(p_hi + po + k * 32, 128), wgmma_desc(v_hi + k * 32, 128), 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(oacc[0]);
+      wgmma_fence_regs(oacc[1]);
+      stage_acc_cols<32, 32, WAU_LD_O>(oacc[0], stg, 0, 0);
+      stage_acc_cols<32, 32, WAU_LD_O>(oacc[1], stg, 64, 0);
+      __syncthreads();
       if (tok >= 0) {  // padded query rows are cropped by the reference (:319-320); rows >= 49 do not exist
         const float inv = 1.f / (kP * a.scale_out);
         uint4* dh = reinterpret_cast<uint4*>(a.out_hi + static_cast<size_t>(tok) * a.C + head * D);
@@ -571,7 +540,7 @@ __global__ void __launch_bounds__(128, 3) window_attention_umma_kernel(const Att
         for (int c = 0; c < 4; ++c) {
           float o8[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) o8[j] = __uint_as_float(ro[8 * c + j]) * inv;
+          for (int j = 0; j < 8; ++j) o8[j] = stg[t * WAU_LD_O + 8 * c + j] * inv;
           uint4 hi, lo;
           wau_split8(o8, a.scale_out, hi, lo, ov);
           dh[c] = hi;
@@ -579,17 +548,9 @@ __global__ void __launch_bounds__(128, 3) window_attention_umma_kernel(const Att
         }
       }
     }
-    tc_fence_before();
-    __syncthreads();  // TMEM rows and the operand tiles are free for the next pair
-    phase ^= 1;
+    __syncthreads();  // the staging tile and the operand tiles are free for the next pair
   }
   if (ov) atomicOr(a.status, 1);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
-  }
 }
 
 }  // namespace dd

@@ -77,7 +77,7 @@ class DenoiseEngine:
         self.lib = _cabi.load_library()
         device = torch.device(device)
         if device.type != "cuda":
-            raise EngineError("DenoiseEngine runs on CUDA (sm_100a) only; there is no CPU path")
+            raise EngineError("DenoiseEngine runs on CUDA (sm_90a) only; there is no CPU path")
         self.device = device
         self.variant = variant
         self.batch, self.latent_hw, self.cond_hw = int(batch), tuple(latent_hw), tuple(cond_hw)

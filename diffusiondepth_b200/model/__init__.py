@@ -9,7 +9,7 @@ def get(args):
         module = import_module(f"{__name__}.{model_name.lower()}")
     except ModuleNotFoundError as e:
         raise ModuleNotFoundError(
-            f"{model_name}: only the DiffusionDepth model (Diffusion_DCbase_) is served by the B200 engine; "
+            f"{model_name}: only the DiffusionDepth model (Diffusion_DCbase_) is served by the H100 engine; "
             "NLSPN and the DCN extension are out of scope (DESIGN.md)") from e
     return getattr(module, model_name)
 

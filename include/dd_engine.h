@@ -1,5 +1,5 @@
 /*
- * dd_engine.h — C ABI of libddengine.so: the B200-native (sm_100a) DiffusionDepth hot path.
+ * dd_engine.h — C ABI of libddengine.so: the H100-native (sm_90a) DiffusionDepth hot path.
  *
  * The reference (duanyiqun/DiffusionDepth @ e1ca9d5) has no FFI on this path; these entry points
  * are what a binding for it would bind.  Each one names the reference interface it replaces:
@@ -32,7 +32,7 @@
  * call and owns only its pre-packed weights / descriptors / CUDA graph.  Calls are enqueued on the
  * given stream and return without synchronising.  One handle per (process, device); a handle is not
  * re-entrant.  Errors: int status (0 = ok), never an exception across the ABI; text via
- * dd_last_error() (thread-local).  There is NO CPU path: dd_create fails if no sm_100 device is present.
+ * dd_last_error() (thread-local).  There is NO CPU path: dd_create fails if no sm_90 device is present.
  */
 #ifndef DD_ENGINE_H_
 #define DD_ENGINE_H_
@@ -52,7 +52,7 @@ enum dd_status {
   DD_OK = 0,
   DD_ERR_INVALID = 1,     /* bad argument / shape / missing weight */
   DD_ERR_CUDA = 2,        /* a CUDA runtime or driver call failed */
-  DD_ERR_UNSUPPORTED = 3, /* no sm_100 device, unsupported shape */
+  DD_ERR_UNSUPPORTED = 3, /* no sm_90 device, unsupported shape */
   DD_ERR_RANGE = 4        /* an activation left the fp16 split's range (see DESIGN.md "Numerics") */
 };
 
@@ -64,19 +64,15 @@ enum dd_variant {
 
 enum dd_flags {
   DD_FLAG_CUDA_GRAPH = 1 << 0, /* capture the T-step loop once and replay it */
-  DD_FLAG_SIMT_CONV = 1 << 1,  /* debug: fp32 CUDA-core convolutions instead of tcgen05 */
+  DD_FLAG_SIMT_CONV = 1 << 1,  /* debug: fp32 CUDA-core convolutions instead of the tensor cores */
   DD_FLAG_CHECK_RANGE = 1 << 2,/* after the call, sync and report DD_ERR_RANGE if the split overflowed */
-  DD_FLAG_HALO_CONV = 1 << 3,  /* loop convs on the row-halo-reuse kernel (16x8 tiles, 2.7x less activation traffic) */
-  DD_FLAG_SWAP_NARROW = 1 << 4, /* Cout <= 64 convs on the swapped-operand kernel (weights as A, 256 pixels as N) */
-  DD_FLAG_PAIR_WIDE = 1 << 5,   /* Cout = 256 convs on CTA pairs (cluster of 2, tcgen05 cta_group::2, M = 256) */
+  DD_FLAG_HALO_CONV = 1 << 3,  /* kernel selection on Blackwell; the sm_90a build always runs the row-halo kernel */
+  DD_FLAG_SWAP_NARROW = 1 << 4, /* swapped-operand narrow convs (Blackwell only; accepted without effect on sm_90a) */
+  DD_FLAG_PAIR_WIDE = 1 << 5,   /* Cout = 256 convs on CTA pairs (Blackwell only; accepted without effect on sm_90a) */
   DD_FLAG_STEP_DECODE = 1 << 6, /* reserve workspace for dd_denoise_decode_steps (T decoded maps; the *Vis heads) */
-  DD_FLAG_FP8_CORR = 1 << 7     /* Swin variant, with HALO_CONV | PAIR_WIDE: the Cout = 256 convs (convA, convB 256->256 and
-                                   noise_embedding.3 64->256) compute the correction
-                                   products of the split (x_lo * w_hi, x_hi * w_lo) as e4m3 MMAs (kind::f8f6f4, K = 32) and
-                                   only hi * hi in fp16: 2 pass-equivalents instead of 3, ~1.5x on the dominant kernel.
-                                   Error per product ~2^-15 instead of ~2^-22 (DESIGN.md "Numerics": max |dz| 3.4e-4 on
-                                   BASELINE config 3, tolerance 1e-3); activations must stay below 112 in magnitude
-                                   (DD_ERR_RANGE otherwise).  Off = the exact 3-pass fp16 split everywhere. */
+  DD_FLAG_FP8_CORR = 1 << 7     /* correction products of the split as e4m3 MMAs (Blackwell only: Hopper's e4m3 MMA
+                                   accumulates at reduced precision, DESIGN.md "Numerics"); the sm_90a build accepts the
+                                   flag and runs the exact 3-pass fp16 split everywhere */
 };
 
 typedef struct dd_config {

@@ -36,6 +36,18 @@ def is_trained_case(case):
     return case in configs.GOLDEN_TRAINED
 
 
+def ref_fixtures():
+    """Outputs of the real reference stored by oracle/make_ref_fixtures.py (inputs are regenerated from the seeds)."""
+    import numpy as np
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_fixtures.npz"),
+                   allow_pickle=False)
+
+
+def fixture_sample_index(n, k=4096):
+    import numpy as np
+    return np.sort(np.random.default_rng(0).choice(n, min(n, k), replace=False))
+
+
 def weight_checksum(sd):
     keys = sorted(k for k in sd if k.startswith("depth_head.model.") or "conv_inv_transform" in k
                   or k.startswith("depth_head.conv_lateral") or k.endswith("relative_position_bias_table"))

@@ -1,5 +1,5 @@
 """bench.py's measurement contract, as far as it can be exercised without a GPU: the reference arm (CPU oracle port)
-prints ONE JSON line with the agreed keys, and our arm refuses to run without a B200 instead of falling back."""
+prints ONE JSON line with the agreed keys, and our arm refuses to run without an H100 instead of falling back."""
 import json
 import os
 import subprocess

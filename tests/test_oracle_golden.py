@@ -1,10 +1,9 @@
 """Pin the CPU restatement (oracle/restate.py) and the mirror's step-invariant producers against golden
-vectors generated from the REAL reference (oracle/make_golden.py); when /root/reference is present, also
-against the reference itself, live."""
+vectors generated from the REAL reference (oracle/make_golden.py, oracle/make_ref_fixtures.py)."""
 import pytest
 import torch
 
-from oracle import configs, ref_import, restate
+from oracle import configs, restate
 import dd_helpers as helpers
 
 TOL_Z = 5e-5  # fp32-vs-fp32 re-association noise on the logits (SURVEY.md §7.2: 3e-5 vs fp64 over 20 steps)
@@ -78,64 +77,79 @@ def test_denoiser_is_nonnegative_and_batch_independent():
     assert torch.allclose(e2[:1], e0, atol=1e-6)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference sources not present")
-def test_oracle_against_live_reference_swin_head():
-    """Swin *head* path (HAHI neck + FPN + upsample_fuse loop + decoder) live against the reference, fed with
-    synthetic Swin-shaped feature maps so the (slow) Swin-L backbone is not needed on CPU."""
-    from oracle import reference_runner  # noqa: F401
-    mods = ref_import.reference_modules()
-    torch.manual_seed(11)
-    head = mods.head_swin.DDIMDepthEstimate_Swin_ADDHAHI(
-        in_channels=[64, 128, 256, 512], inference_steps=3, num_train_timesteps=1000, depth_feature_dim=16,
-        loss_cfgs=[], init_cfg=None).eval()
-    with torch.no_grad():
-        head.hahineck.level_embed.zero_()
-    sd = {"depth_head." + k: v for k, v in head.state_dict().items()}
+SWIN_HEAD_KW = dict(in_channels=[64, 128, 256, 512], inference_steps=3, num_train_timesteps=1000, depth_feature_dim=16,
+                    loss_cfgs=[], init_cfg=None)
+
+
+def swin_head_inputs():
+    """Synthetic Swin-shaped feature maps (the slow Swin-L backbone is not needed on CPU), gt, initial noise."""
     gen = torch.Generator().manual_seed(2)
     H, W = 40, 56
     fp = [torch.randn(1, c, -(-H // s), -(-W // s), generator=gen) for c, s in ((192, 4), (384, 8), (768, 16), (1536, 32))]
     gt = torch.rand(1, 1, H, W, generator=gen) * 80
     noise = torch.randn(1, 16, H // 2, W // 2, generator=gen)
-    from oracle.reference_runner import _inject_first_randn
-    cap = {}
-    hk = head.depth_transform.conv_inv_transform[3].register_forward_hook(lambda m, a, o: cap.__setitem__("z", o))
-    with torch.no_grad(), _inject_first_randn(noise):
-        out = head(fp, gt, gt > 0, gt_depth_map=gt)
-    hk.remove()
+    return fp, gt, noise
+
+
+def _checksum(sd):
+    return sum(v.double().abs().sum().item() for v in sd.values() if v.is_floating_point())
+
+
+def test_oracle_against_live_reference_swin_head():
+    """Swin *head* path (HAHI neck + FPN + upsample_fuse loop + decoder) against the reference's own head on the same
+    weights (the mirror's seeded initialisation) and inputs (its logits and depth stored by oracle/make_ref_fixtures.py)."""
+    from diffusiondepth_b200.model.registry import HEADS
+    ref = helpers.ref_fixtures()
+    torch.manual_seed(11)
+    head = HEADS.build(dict(type="DDIMDepthEstimate_Swin_ADDHAHI", **SWIN_HEAD_KW)).eval()
+    with torch.no_grad():
+        head.hahineck.level_embed.zero_()
+    assert abs(_checksum(head.state_dict()) - float(ref["head_weight_checksum"])) <= 1e-6 * float(ref["head_weight_checksum"])
+    sd = {"depth_head." + k: v for k, v in head.state_dict().items()}
+    fp, gt, noise = swin_head_inputs()
     with torch.no_grad():
         cond = restate.fpn_condition(sd, restate.hahi_neck(sd, fp))
         lat = restate.ddim_loop(sd, cond, noise, 3, "swin")
         z = restate.decode_logits(sd, lat)
-    assert (z - cap["z"]).abs().max().item() < TOL_Z
-    assert torch.allclose(restate.decode(sd, lat), out["pred"], rtol=1e-4, atol=1e-6)
+    assert (z - torch.from_numpy(ref["head_z"])).abs().max().item() < TOL_Z
+    assert torch.allclose(restate.decode(sd, lat), torch.from_numpy(ref["head_pred"]), rtol=1e-4, atol=1e-6)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference sources not present")
-@pytest.mark.parametrize("hw,shift", [((24, 40), 0), ((24, 40), 3), ((13, 9), 3)])
+WMSA_C, WMSA_HEADS = 96, 3
+WMSA_CASES = [((24, 40), 0), ((24, 40), 3), ((13, 9), 3)]
+
+
+def wmsa_inputs(hw):
+    gen = torch.Generator().manual_seed(6)
+    table = torch.randn(169, WMSA_HEADS, generator=gen) * 0.7
+    x = torch.randn(2, hw[0] * hw[1], WMSA_C, generator=gen)
+    return table, x
+
+
+@pytest.mark.parametrize("hw,shift", WMSA_CASES)
 def test_window_msa_live_reference_trained_regime(hw, shift):
     """The reference's own ShiftWindowMSA / WindowMSA modules (backbone/swin.py:150-189, 250-325) with NON-ZERO
-    relative-position tables, padded (24x40 -> 28x42, 13x9 -> 14x14) and shifted windows, live against (a) the
-    restatement and (b) the mirror's module — the bias / mask / roll path that the `nopretrain` factory leaves at zero."""
-    mods = ref_import.reference_modules()
-    torch.manual_seed(5)
-    C, heads = 96, 3
-    ref = mods.swin.ShiftWindowMSA(embed_dims=C, num_heads=heads, window_size=7, shift_size=shift).eval()
+    relative-position tables, padded (24x40 -> 28x42, 13x9 -> 14x14) and shifted windows (a seeded sample of their output
+    stored by oracle/make_ref_fixtures.py) against (a) the restatement and (b) the mirror's module on the same weights —
+    the bias / mask / roll path that the `nopretrain` factory leaves at zero."""
     from diffusiondepth_b200.model.backbone import swin as mirror_swin
-    mine = mirror_swin.ShiftWindowMSA(C, heads, 7, shift).eval() if hasattr(mirror_swin, "ShiftWindowMSA") else None
-    gen = torch.Generator().manual_seed(6)
+    ref = helpers.ref_fixtures()
+    i = WMSA_CASES.index((hw, shift))
+    torch.manual_seed(5)
+    mine = mirror_swin.ShiftWindowMSA(WMSA_C, WMSA_HEADS, 7, shift).eval()
+    assert abs(_checksum(mine.state_dict()) - float(ref[f"wmsa_{i}_weight_checksum"])) <= 1e-6 * float(ref[f"wmsa_{i}_weight_checksum"])
+    table, x = wmsa_inputs(hw)
     with torch.no_grad():
-        ref.w_msa.relative_position_bias_table.copy_(torch.randn(169, heads, generator=gen) * 0.7)
-    x = torch.randn(2, hw[0] * hw[1], C, generator=gen)
+        mine.w_msa.relative_position_bias_table.copy_(table)
+    idx = torch.from_numpy(helpers.fixture_sample_index(2 * hw[0] * hw[1] * WMSA_C))
+    want = torch.from_numpy(ref[f"wmsa_{i}_sample"])
+    tol = 2e-6 * float(ref[f"wmsa_{i}_absmax"]) + 1e-6
+    sd = {"a." + k: v for k, v in mine.state_dict().items()}
+    got = restate._shift_window_msa(sd, x, hw, "a.", WMSA_HEADS, 7, shift)
+    assert (got.reshape(-1)[idx] - want).abs().max().item() < tol
     with torch.no_grad():
-        want = ref(x, hw)
-    sd = {"a." + k: v for k, v in ref.state_dict().items()}
-    got = restate._shift_window_msa(sd, x, hw, "a.", heads, 7, shift)
-    assert (got - want).abs().max().item() < 2e-6 * want.abs().max().item() + 1e-6
-    if mine is not None:
-        mine.load_state_dict(ref.state_dict(), strict=True)
-        with torch.no_grad():
-            assert (mine(x, hw) - want).abs().max().item() < 2e-6 * want.abs().max().item() + 1e-6
+        assert (mine(x, hw).reshape(-1)[idx] - want).abs().max().item() < tol
     # the bias really matters in this regime
-    with torch.no_grad():
-        ref.w_msa.relative_position_bias_table.zero_()
-        assert (ref(x, hw) - want).abs().max().item() > 1e-3
+    sd["a.w_msa.relative_position_bias_table"] = torch.zeros_like(table)
+    nobias = restate._shift_window_msa(sd, x, hw, "a.", WMSA_HEADS, 7, shift)
+    assert (nobias.reshape(-1)[idx] - want).abs().max().item() > 1e-3

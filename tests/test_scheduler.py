@@ -7,7 +7,8 @@ import torch
 
 from diffusiondepth_b200 import ddim_coefficients
 from diffusiondepth_b200.model.diffusers.schedulers.scheduling_ddim import DDIMScheduler
-from oracle import ref_import, restate
+from oracle import restate
+import dd_helpers
 
 
 def test_tables_and_timesteps():
@@ -65,24 +66,25 @@ def test_add_noise_and_sample_prediction():
         DDIMScheduler().step(n, 10, x0)
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference sources not present")
+REF_STEPS = (5, 20, 50)
+
+
 def test_against_reference_scheduler():
-    ref = ref_import.reference_modules().scheduling_ddim.DDIMScheduler(num_train_timesteps=1000, clip_sample=False)
+    """Bit-for-bit against the reference's own DDIMScheduler (outputs stored by oracle/make_ref_fixtures.py)."""
+    ref = dd_helpers.ref_fixtures()
     mine = DDIMScheduler(num_train_timesteps=1000, clip_sample=False)
-    assert torch.equal(ref.alphas_cumprod, mine.alphas_cumprod)
+    assert torch.equal(torch.from_numpy(ref["sched_alphas_cumprod"]), mine.alphas_cumprod)
     g = torch.Generator().manual_seed(3)
-    for T in (5, 20, 50):
-        ref.set_timesteps(T)
+    for T in REF_STEPS:
         mine.set_timesteps(T)
-        assert torch.equal(ref.timesteps, mine.timesteps)
+        assert torch.equal(torch.from_numpy(ref[f"sched_timesteps_{T}"]), mine.timesteps)
         x = torch.randn(1, 16, 6, 10, generator=g)
-        for t in ref.timesteps:
+        for t in mine.timesteps:
             eps = torch.rand(x.shape, generator=g)
-            a = ref.step(eps, t, x, eta=0.0, use_clipped_model_output=True)
             b = mine.step(eps, t, x, eta=0.0, use_clipped_model_output=True)
-            assert torch.equal(a["prev_sample"], b["prev_sample"])
-            assert torch.equal(a["pred_original_sample"], b["pred_original_sample"])
-            x = a["prev_sample"]
+            x = b["prev_sample"]
+        assert torch.equal(x, torch.from_numpy(ref[f"sched_prev_{T}"]))
+        assert torch.equal(b["pred_original_sample"], torch.from_numpy(ref[f"sched_pred0_{T}"]))
     t = torch.tensor([7, 300])
     x0, n = torch.randn(2, 16, 3, 3, generator=g), torch.randn(2, 16, 3, 3, generator=g)
-    assert torch.equal(ref.add_noise(x0, n, t), mine.add_noise(x0, n, t))
+    assert torch.equal(mine.add_noise(x0, n, t), torch.from_numpy(ref["sched_add_noise"]))
