@@ -50,7 +50,10 @@ struct HaloCfg {
   static constexpr int NWG = COUT > 128 ? 2 : 1;
   static constexpr int NW = COUT / NWG;
   static constexpr int THREADS = 128 * (1 + NWG);
-  static constexpr int CH = NW < 32 ? NW : 32;           // accumulator columns per epilogue chunk
+  // accumulator columns per epilogue chunk.  The two-warpgroup (256-wide) layers drain 16 at a time: the smaller
+  // staging tile (17 KB instead of 33 KB) leaves room for a third weight slot, so the producer runs two taps ahead of
+  // the MMAs instead of one.
+  static constexpr int CH = NWG > 1 ? 16 : (NW < 32 ? NW : 32);
   static constexpr int LD = CH + 1;                                  // staging row stride (floats): conflict-free rows
   static constexpr int STAGE_BYTES = NWG * 128 * LD * 4;
   static constexpr int CTRL_BYTES = 1024;  // barriers, GroupNorm partials [2][4 NWG][4][2]
@@ -61,6 +64,7 @@ struct HaloCfg {
   static constexpr bool B_RESIDENT = (9 * KC * B_SLOT <= 40 * 1024) && (9 * KC <= B_SLOTS_RAW);
   static constexpr int B_SLOTS = B_RESIDENT ? 9 * KC : (B_SLOTS_RAW > 8 ? 8 : B_SLOTS_RAW);
   static_assert(B_SLOTS >= 2, "B ring too small");
+  static_assert(NWG == 1 || B_SLOTS >= 3, "256-wide layers: the producer must be able to run two taps ahead");
   static constexpr int SMEM_BYTES = A_SLOTS * A_SLOT + B_SLOTS * B_SLOT + 1024 + CTRL_BYTES + STAGE_BYTES;
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB dynamic shared memory limit");
   static constexpr int A_TX = 6 * STRIP_BYTES;
@@ -110,62 +114,65 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   }
   __syncthreads();
 
-  if constexpr (C::NWG > 1) {
-    if (warp < 4) setmaxnreg_dec<40>();
-    else setmaxnreg_inc<232>();
-  }
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (A strips).  The WHOLE warp walks
-    // the loop (barrier waits and coordinates stay warp-uniform) and one elected lane issues the copies.
-    const bool leader = elect_one();
-    int sa = 0;
-    uint32_t pa = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
-      const int x0 = tx * HALO_TW, y0 = ty * HALO_TH;
-      for (int kc = 0; kc < C::KC; ++kc) {
-        mbar_wait(&a_empty[sa], pa ^ 1);
-        uint8_t* s = a_ring + sa * C::A_SLOT;
-        if (leader) {
-          mbar_arrive_expect_tx(&a_full[sa], C::A_TX);
-#pragma unroll
-          for (int dx = 0; dx < 3; ++dx) {
-            tma_load_4d(s + (2 * dx) * C::STRIP_PAD, &tmA_hi, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
-            tma_load_4d(s + (2 * dx + 1) * C::STRIP_PAD, &tmA_lo, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
-          }
-        }
-        __syncwarp();
-        if (++sa == C::A_SLOTS) {
-          sa = 0;
-          pa ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ TMA producer (B weight tiles), same structure
-    const bool leader = elect_one();
-    int sb = 0;
-    uint32_t pb = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      if (C::B_RESIDENT && tile != static_cast<int>(blockIdx.x)) break;  // weights stay in their slots after the first tile
-      for (int kc = 0; kc < C::KC; ++kc) {
-        for (int tap = 0; tap < 9; ++tap) {
-          mbar_wait(&b_empty[sb], pb ^ 1);
-          uint8_t* s = b_ring + sb * C::B_SLOT;
+  // setmaxnreg sits at the top of each role's branch and the branches only meet again at the exit.  With a merge point
+  // after it (one if / else, then the role dispatch) ptxas ignored setmaxnreg (C7507) and the consumers' accumulators
+  // spilled at the 168-register launch bound.
+  if (warp < 4) {
+    if constexpr (C::NWG > 1) setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // ---------------------------------------------------------------- TMA producer (A strips).  The WHOLE warp walks
+      // the loop (barrier waits and coordinates stay warp-uniform) and one elected lane issues the copies.
+      const bool leader = elect_one();
+      int sa = 0;
+      uint32_t pa = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
+        const int x0 = tx * HALO_TW, y0 = ty * HALO_TH;
+        for (int kc = 0; kc < C::KC; ++kc) {
+          mbar_wait(&a_empty[sa], pa ^ 1);
+          uint8_t* s = a_ring + sa * C::A_SLOT;
           if (leader) {
-            mbar_arrive_expect_tx(&b_full[sb], C::B_TX);
-            tma_load_3d(s, &tmB_hi, &b_full[sb], kc * BK, 0, tap);
-            tma_load_3d(s + C::B_TILE_PAD, &tmB_lo, &b_full[sb], kc * BK, 0, tap);
+            mbar_arrive_expect_tx(&a_full[sa], C::A_TX);
+#pragma unroll
+            for (int dx = 0; dx < 3; ++dx) {
+              tma_load_4d(s + (2 * dx) * C::STRIP_PAD, &tmA_hi, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
+              tma_load_4d(s + (2 * dx + 1) * C::STRIP_PAD, &tmA_lo, &a_full[sa], kc * BK, x0 + dx - 1, y0 - 1, img);
+            }
           }
           __syncwarp();
-          if (++sb == C::B_SLOTS) {
-            sb = 0;
-            pb ^= 1;
+          if (++sa == C::A_SLOTS) {
+            sa = 0;
+            pa ^= 1;
+          }
+        }
+      }
+    } else if (warp == 1) {
+      // ---------------------------------------------------------------- TMA producer (B weight tiles), same structure
+      const bool leader = elect_one();
+      int sb = 0;
+      uint32_t pb = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        if (C::B_RESIDENT && tile != static_cast<int>(blockIdx.x)) break;  // weights stay in their slots after the first tile
+        for (int kc = 0; kc < C::KC; ++kc) {
+          for (int tap = 0; tap < 9; ++tap) {
+            mbar_wait(&b_empty[sb], pb ^ 1);
+            uint8_t* s = b_ring + sb * C::B_SLOT;
+            if (leader) {
+              mbar_arrive_expect_tx(&b_full[sb], C::B_TX);
+              tma_load_3d(s, &tmB_hi, &b_full[sb], kc * BK, 0, tap);
+              tma_load_3d(s + C::B_TILE_PAD, &tmB_lo, &b_full[sb], kc * BK, 0, tap);
+            }
+            __syncwarp();
+            if (++sb == C::B_SLOTS) {
+              sb = 0;
+              pb ^= 1;
+            }
           }
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    if constexpr (C::NWG > 1) setmaxnreg_inc<232>();
     // ------------------------------------------------------------------ consumers: MMA + epilogue
     const int wg = (warp >> 2) - 1;  // consumer warpgroup
     const int t = threadIdx.x & 127;
@@ -182,11 +189,9 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
       // ---------------------------------------------------------------- mainloop
       int prev_b = -1, prev_a = -1;  // slots read by the wgmma group still in flight
-      auto retire_prev = [&]() {
-        if (signal) {
-          if (prev_b >= 0) mbar_arrive(&b_empty[prev_b]);
-          if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
-        }
+      auto retire_prev = [&]() {  // predicated arrives: no branch between wgmma issue and wait
+        mbar_arrive_if(&b_empty[prev_b < 0 ? 0 : prev_b], signal && prev_b >= 0);
+        mbar_arrive_if(&a_empty[prev_a < 0 ? 0 : prev_a], signal && prev_a >= 0);
         prev_b = prev_a = -1;
       };
       {

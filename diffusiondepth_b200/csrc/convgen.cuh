@@ -102,53 +102,54 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
   __syncthreads();
   auto stage_ptr = [&](int s) { return smem + s * C::STAGE_BYTES; };
 
-  if constexpr (C::NWG > 1) {
-    if (warp < 4) setmaxnreg_dec<40>();
-    else setmaxnreg_inc<232>();
-  }
-  if (warp == 0 || warp == 1) {
-    // two TMA producers; the whole warp walks the loop, one elected lane issues (consecutive UTMALDGs)
-    const bool act = (warp == 0);
-    const bool leader = elect_one();
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
-      const int nt = work % p.n_tiles;  // n fastest: neighbours share the A patch in L2
-      const int mt = work / p.n_tiles;
-      const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
-      const int x0 = tx * TILE_W, y0 = ty * TILE_H;
-      for (int tap = 0; tap < p.taps; ++tap) {
-        const int dy = p.taps == 9 ? tap / 3 - 1 : 0, dx = p.taps == 9 ? tap % 3 - 1 : 0;
-        for (int kc = 0; kc < kc_total; ++kc) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* s = stage_ptr(stage);
-          const int ax = x0 * p.stride + dx, ay = y0 * p.stride + dy;
-          // weight K coordinate of this chunk: source 1's channels start right after source 0's REAL channels
-          const int kw = kc < p.kc0 ? kc * C::BK : p.c0_ch + (kc - p.kc0) * C::BK;
-          if (leader) {
-            if (!act) {
-              mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES);
-              tma_load_3d(s + 2 * C::A_BYTES, &tmB_hi, &full_bar[stage], kw, nt * NT, tap);
-              tma_load_3d(s + 2 * C::A_BYTES + C::B_BYTES, &tmB_lo, &full_bar[stage], kw, nt * NT, tap);
-            } else if (kc < p.kc0) {
-              mbar_arrive_expect_tx(&full_bar[stage], 2 * C::A_BYTES);
-              tma_load_4d(s, &tmA0_hi, &full_bar[stage], kc * C::BK, ax, ay, img);
-              tma_load_4d(s + C::A_BYTES, &tmA0_lo, &full_bar[stage], kc * C::BK, ax, ay, img);
-            } else {
-              mbar_arrive_expect_tx(&full_bar[stage], 2 * C::A_BYTES);
-              tma_load_4d(s, &tmA1_hi, &full_bar[stage], (kc - p.kc0) * C::BK, ax, ay, img);
-              tma_load_4d(s + C::A_BYTES, &tmA1_lo, &full_bar[stage], (kc - p.kc0) * C::BK, ax, ay, img);
+  // setmaxnreg at the top of each role's branch, branches meeting only at the exit (see conv3x3_halo_kernel)
+  if (warp < 4) {
+    if constexpr (C::NWG > 1) setmaxnreg_dec<40>();
+    if (warp == 0 || warp == 1) {
+      // two TMA producers; the whole warp walks the loop, one elected lane issues (consecutive UTMALDGs)
+      const bool act = (warp == 0);
+      const bool leader = elect_one();
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+        const int nt = work % p.n_tiles;  // n fastest: neighbours share the A patch in L2
+        const int mt = work / p.n_tiles;
+        const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
+        const int x0 = tx * TILE_W, y0 = ty * TILE_H;
+        for (int tap = 0; tap < p.taps; ++tap) {
+          const int dy = p.taps == 9 ? tap / 3 - 1 : 0, dx = p.taps == 9 ? tap % 3 - 1 : 0;
+          for (int kc = 0; kc < kc_total; ++kc) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            uint8_t* s = stage_ptr(stage);
+            const int ax = x0 * p.stride + dx, ay = y0 * p.stride + dy;
+            // weight K coordinate of this chunk: source 1's channels start right after source 0's REAL channels
+            const int kw = kc < p.kc0 ? kc * C::BK : p.c0_ch + (kc - p.kc0) * C::BK;
+            if (leader) {
+              if (!act) {
+                mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES);
+                tma_load_3d(s + 2 * C::A_BYTES, &tmB_hi, &full_bar[stage], kw, nt * NT, tap);
+                tma_load_3d(s + 2 * C::A_BYTES + C::B_BYTES, &tmB_lo, &full_bar[stage], kw, nt * NT, tap);
+              } else if (kc < p.kc0) {
+                mbar_arrive_expect_tx(&full_bar[stage], 2 * C::A_BYTES);
+                tma_load_4d(s, &tmA0_hi, &full_bar[stage], kc * C::BK, ax, ay, img);
+                tma_load_4d(s + C::A_BYTES, &tmA0_lo, &full_bar[stage], kc * C::BK, ax, ay, img);
+              } else {
+                mbar_arrive_expect_tx(&full_bar[stage], 2 * C::A_BYTES);
+                tma_load_4d(s, &tmA1_hi, &full_bar[stage], (kc - p.kc0) * C::BK, ax, ay, img);
+                tma_load_4d(s + C::A_BYTES, &tmA1_lo, &full_bar[stage], (kc - p.kc0) * C::BK, ax, ay, img);
+              }
             }
-          }
-          __syncwarp();
-          if (++stage == C::STAGES) {
-            stage = 0;
-            phase ^= 1;
+            __syncwarp();
+            if (++stage == C::STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
           }
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    if constexpr (C::NWG > 1) setmaxnreg_inc<232>();
     const int wg = (warp >> 2) - 1;
     const int t = threadIdx.x & 127;
     const int q = t >> 5;
@@ -188,7 +189,7 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
         }
         wgmma_commit();
         wgmma_wait<1>();
-        if (t == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);
+        mbar_arrive_if(&empty_bar[prev < 0 ? 0 : prev], t == 0 && prev >= 0);  // predicated: no branch before the wait
         prev = stage;
         if (++stage == C::STAGES) {
           stage = 0;
@@ -198,7 +199,7 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
       wgmma_wait<0>();
       wgmma_fence_regs(acc[0]);
       wgmma_fence_regs(acc[1]);
-      if (t == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);
+      mbar_arrive_if(&empty_bar[prev < 0 ? 0 : prev], t == 0 && prev >= 0);
 
       // ---------------------------------------------------------------- epilogue
       //   fp32-only outputs: the staging tile re-distributes the chunk so that a lane holds one float4 of a row and 4

@@ -39,24 +39,34 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Spin with a watchdog: a protocol bug must trap (launch error) instead of hanging the GPU.
+// Spin with a watchdog: a protocol bug must trap (launch error) instead of hanging the GPU.  The loop, the clock check
+// and the trap live in ONE asm block: as C++ control flow they sat between wgmma issue and wgmma.wait_group, and ptxas
+// then serialised every wgmma of the mainloop (C7518, "WG.DP in divergent path").  Labels are scoped to the braces.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) __trap();  // ~4 s at 2 GHz
-  }
+  asm volatile(
+      "{\n\t.reg .pred P;\n\t.reg .s64 t0, t1;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 P, [%0], %1;\n\t"
+      "@P bra DD_WAIT_DONE;\n\t"
+      "mov.u64 t0, %%clock64;\n"
+      "DD_WAIT_LOOP:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 P, [%0], %1;\n\t"
+      "@P bra DD_WAIT_DONE;\n\t"
+      "mov.u64 t1, %%clock64;\n\t"
+      "sub.s64 t1, t1, t0;\n\t"
+      "setp.lt.s64 P, t1, 8000000000;\n\t"  // ~4 s at 2 GHz
+      "@P bra DD_WAIT_LOOP;\n\t"
+      "trap;\n"
+      "DD_WAIT_DONE:\n\t}\n" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
+}
+// mbarrier.arrive by the threads whose `pred` is set, as one predicated instruction (no branch around it).
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}\n" ::"r"(smem_u32(bar)),
+      "r"(static_cast<uint32_t>(pred))
+      : "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -172,7 +182,8 @@ __device__ __forceinline__ void wgmma_e4m3<128>(float (&d)[64], uint64_t a, uint
 }
 
 // Per-warpgroup register budget (all warps of a warpgroup execute the same call): the TMA producer warpgroup gives
-// registers back so that two consumer warpgroups can each hold a 128 x 128 fp32 accumulator without spilling.
+// registers back so that two consumer warpgroups can each hold a 128 x 128 fp32 accumulator without spilling.  Call it
+// first in each role's branch, with no merge point after it before the exit, or ptxas ignores it (C7507).
 template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
