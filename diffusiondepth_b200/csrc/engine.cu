@@ -19,6 +19,7 @@
 #include "conv_halo.cuh"
 #include "swin.cuh"
 #include "mpvit.cuh"
+#include "backward.cuh"
 
 namespace {
 
@@ -110,6 +111,19 @@ int make_w_map(CUtensorMap* m, const __half* base, int cout, int cin, int bk, in
   return DD_OK;
 }
 
+// weight-gradient operand: NHWC fp16 plane [B][H][W][C]; box = {64 channels, 64 pixels of one row}, 128-byte swizzle
+int make_wgm_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C) {
+  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {64, 64, 1, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(wgrad operand) failed: " + std::to_string((int)r));
+  return DD_OK;
+}
+
 // general conv weights: [taps][COUT][CIN] fp16; box = {GEN_BK, NT, 1}
 int make_wgen_map(CUtensorMap* m, const __half* base, int cout, int cin, int taps, int nt) {
   cuuint64_t gdim[3] = {(cuuint64_t)cin, (cuuint64_t)cout, (cuuint64_t)taps};
@@ -154,6 +168,11 @@ cudaError_t configure_halo_all_epi() {
   return cudaFuncSetAttribute(dd::conv3x3_halo_kernel<CIN, COUT, BK, dd::EPI_F32>,
                               cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
 }
+template <int MCO, int NCI>
+cudaError_t configure_wgm() {
+  return cudaFuncSetAttribute(dd::wgrad_wgmma_kernel<MCO, NCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              dd::WgmCfg<MCO, NCI>::SMEM_BYTES);
+}
 template <int NT>
 cudaError_t configure_gen() {
   return cudaFuncSetAttribute(dd::convgen_wgmma_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -170,6 +189,9 @@ cudaError_t configure_all_kernels() {
   if ((e = configure_halo_all_epi<256, 256, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<256, 64, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<64, 16, 32>()) != cudaSuccess) return e;
+  if ((e = configure_wgm<128, 128>()) != cudaSuccess) return e;
+  if ((e = configure_wgm<128, 64>()) != cudaSuccess) return e;
+  if ((e = configure_wgm<64, 128>()) != cudaSuccess) return e;
   if ((e = configure_gen<256>()) != cudaSuccess) return e;
   if ((e = configure_gen<192>()) != cudaSuccess) return e;
   if ((e = configure_gen<128>()) != cudaSuccess) return e;
@@ -322,7 +344,8 @@ struct dd_engine {
   bool weights_ready = false;
   std::map<std::string, Raw> raw;
   // packed parameters (device memory owned by the engine)
-  ConvLayer L[6];  // 0 ne.0, 1 ne.3, 2 convA, 3 convB, 4 pred.0, 5 pred.3
+  ConvLayer L[12];  // 0 ne.0, 1 ne.3, 2 convA, 3 convB, 4 pred.0, 5 pred.3; 6 + i: the data-gradient conv of layer i
+                    // (flipped, transposed weights, zero bias; DD_FLAG_BACKWARD only)
   float* gn_gamma[4] = {nullptr, nullptr, nullptr, nullptr};  // ne.1, ne.4, pred.1, pred.4
   float* gn_beta[4] = {nullptr, nullptr, nullptr, nullptr};
   float* temb = nullptr;    // [1280][256]
@@ -340,6 +363,15 @@ struct dd_engine {
   float *x32 = nullptr, *Y = nullptr, *cond = nullptr, *stats[4] = {}, *mr[4] = {}, *temb_sel = nullptr;
   __half *xs_hi = nullptr, *xs_lo = nullptr, *S_hi[2] = {}, *S_lo[2] = {};
   int* status = nullptr;
+  struct Bwd {  // dd_denoiser_backward's region (DD_FLAG_BACKWARD): the recomputed forward and the gradient buffers
+    float *y1 = nullptr, *y2 = nullptr, *y5 = nullptr, *y6 = nullptr;  // pre-GN conv outputs
+    Planes a1, f0, fa, fp, a5;               // conv input planes (noise_embedding.0 reads xs_hi / xs_lo)
+    float *g[2] = {nullptr, nullptr};        // gradient ping-pong [B][P][256]
+    Planes gp;                               // split planes of the gradient a data-gradient conv reads
+    float *gn_part = nullptr, *ab = nullptr, *col_part = nullptr, *dtemb = nullptr, *dcond = nullptr;
+    float *scales = nullptr, *amax = nullptr;  // [kBwdSlots] on-device gradient scales and their absmax inputs
+    double* wg_part = nullptr;
+  } bw;
   int stats_tiles_img[4] = {0, 0, 0, 0};  // tiles per image of the kernel that last filled stats[i]
   // graph
   Producers prod;
@@ -397,6 +429,35 @@ Geom geom_of(const dd_config& c) {
   g.tiles = g.tiles_img * g.B;
   g.tiles_max = (t816 > t168 ? t816 : t168) * g.B;
   return g;
+}
+
+// ---- backward (DD_FLAG_BACKWARD)
+constexpr int kBwdSlots = 16;  // gradient splits per dd_denoiser_backward call (at most 6 are used)
+// conv layer i: reference key prefix, Cout, Cin
+const char* const kConvKey[6] = {"model.noise_embedding.0", "model.noise_embedding.3", "model.upsample_fuse.convA.conv",
+                                 "model.upsample_fuse.convB.conv", "model.pred.0", "model.pred.3"};
+constexpr int kConvCout[6] = {64, 256, 256, 256, 64, 16};
+constexpr int kConvCin[6] = {16, 64, 256, 256, 256, 64};
+// Split-K plan of wgrad_simt_kernel: about 16 blocks per SM in all, each chunk a multiple of the fp32 flush interval.
+struct WgPlan {
+  int chunks, chunk;
+};
+WgPlan wgrad_plan(int cout, int cin, long long BP) {
+  const int tiles = (cout / std::min(64, cout)) * (cin / std::min(64, cin)) * 9;
+  long long chunks = std::max(1, std::min(128, (2112 + tiles - 1) / tiles));
+  long long chunk = (BP + chunks - 1) / chunks;
+  chunk = std::max<long long>(dd::WG_KS * dd::WG_FLUSH, (chunk + dd::WG_KS - 1) / dd::WG_KS * dd::WG_KS);
+  chunks = (BP + chunk - 1) / chunk;
+  return {static_cast<int>(chunks), static_cast<int>(chunk)};
+}
+int bwd_chunks(int P) { return (P + dd::BWD_CHUNK - 1) / dd::BWD_CHUNK; }
+// Layers whose weight gradient runs on wgrad_wgmma_kernel: the four 256-wide ones.  The two 16-channel layers keep
+// wgrad_simt_kernel (3.6 of 192 ms of a backward call at B = 4, 176 x 608).
+bool wgrad_on_tc(int layer) { return layer >= 1 && layer <= 4; }
+constexpr int kWgmSegs = 128;  // 64-pixel row segments per CTA of wgrad_wgmma_kernel (8192 pixels summed in fp32)
+int wgm_chunks(const Geom& g) {
+  const int nseg = g.B * g.h * ((g.w + 63) / 64);
+  return (nseg + kWgmSegs - 1) / kWgmSegs;
 }
 
 void drop_graphs(dd_engine* e) {
@@ -547,6 +608,42 @@ size_t carve(dd_engine* e, void* base) {
     mv->part_ktv = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * nk);
     mv->ktv = c.take<float>(static_cast<size_t>(g.B) * nk);
   }
+  if (e->cfg.flags & DD_FLAG_BACKWARD) {
+    dd_engine::Bwd* bv = &v->bw;
+    const bool swin = e->cfg.variant == DD_VARIANT_SWIN;
+    const size_t PC = static_cast<size_t>(e->cfg.cond_h) * e->cfg.cond_w;
+    auto planes = [&](Planes& pl, size_t ch) {
+      pl.hi = c.take<__half>(BP * ch);
+      pl.lo = c.take<__half>(BP * ch);
+    };
+    bv->y1 = c.take<float>(BP * 64);
+    bv->y2 = c.take<float>(BP * 256);
+    bv->y5 = c.take<float>(BP * 64);
+    bv->y6 = c.take<float>(BP * 16);
+    planes(bv->a1, 64);
+    if (swin) {
+      planes(bv->f0, 256);
+      planes(bv->fa, 256);
+    }
+    planes(bv->fp, 256);
+    planes(bv->a5, 64);
+    bv->g[0] = c.take<float>(BP * 256);
+    bv->g[1] = c.take<float>(BP * 256);
+    planes(bv->gp, 256);
+    bv->gn_part = c.take<float>(static_cast<size_t>(g.B) * bwd_chunks(g.P) * 256 * 2);
+    bv->ab = c.take<float>(static_cast<size_t>(g.B) * 8);
+    bv->col_part = c.take<float>(static_cast<size_t>(g.B) * bwd_chunks(std::max<int>(g.P, static_cast<int>(PC))) * 256);
+    bv->dtemb = c.take<float>(static_cast<size_t>(g.B) * 256);
+    if (swin) bv->dcond = c.take<float>(static_cast<size_t>(g.B) * PC * 256);
+    bv->scales = c.take<float>(kBwdSlots);
+    bv->amax = c.take<float>(kBwdSlots);
+    size_t wg = 0;
+    for (int i = 0; i < 6; ++i) {
+      const int chunks = wgrad_on_tc(i) ? wgm_chunks(g) : wgrad_plan(kConvCout[i], kConvCin[i], static_cast<long long>(BP)).chunks;
+      wg = std::max(wg, static_cast<size_t>(chunks) * kConvCout[i] * kConvCin[i] * 9);
+    }
+    bv->wg_part = c.take<double>(wg);
+  }
   return align_up(c.off, 1024);
 }
 
@@ -659,10 +756,10 @@ int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st) {
 
 template <int C, int COND>
 int run_apply(dd_engine* e, int which, const float* temb, int temb_bstride, __half* out_hi, __half* out_lo,
-              cudaStream_t st, bool out_f8 = false) {
+              cudaStream_t st, bool out_f8 = false, const float* y = nullptr) {
   const Geom g = geom_of(e->cfg);
   dd::ApplyArgs a;
-  a.y = e->Y;
+  a.y = y != nullptr ? y : e->Y;
   a.mean_rstd = e->mr[which];
   a.gamma = e->gn_gamma[which];
   a.beta = e->gn_beta[which];
@@ -1389,6 +1486,173 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
 
 #include "mpvit_host.inc"
 
+// ------------------------------------------------------------------------------------------------ backward
+int launched(dd_engine* e, const char* what) {
+  e->launches++;
+  const cudaError_t err = cudaGetLastError();
+  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(err));
+  return DD_OK;
+}
+int grid_of(size_t n, int per_block = 256) {
+  const size_t b = (n + per_block - 1) / per_block;
+  return static_cast<int>(std::max<size_t>(1, std::min<size_t>(b, 132 * 16)));
+}
+
+// GroupNorm `which` (0 ne.1, 1 ne.4, 2 pred.1, 3 pred.4) + ReLU backward: dout (times *dscale) -> dy (unscaled)
+template <int C>
+int run_gn_bwd(dd_engine* e, int which, const float* dout, const float* dscale, const float* y, float* dgamma,
+               float* dbeta, float* dy, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  dd::GnBwdArgs a;
+  a.dout = dout;
+  a.dscale = dscale;
+  a.y = y;
+  a.mean_rstd = e->mr[which];
+  a.gamma = e->gn_gamma[which];
+  a.beta = e->gn_beta[which];
+  a.B = g.B;
+  a.P = g.P;
+  a.chunks = bwd_chunks(g.P);
+  a.partial = e->bw.gn_part;
+  a.ab = e->bw.ab;
+  a.dgamma = dgamma;
+  a.dbeta = dbeta;
+  a.dy = dy;
+  int rc;
+  dd::gn_bwd_reduce_kernel<C><<<dim3(a.chunks, g.B), 256, 0, st>>>(a);
+  if ((rc = launched(e, "gn_bwd_reduce"))) return rc;
+  dd::gn_bwd_finalize_kernel<C><<<4, 256, 0, st>>>(a);
+  if ((rc = launched(e, "gn_bwd_finalize"))) return rc;
+  dd::gn_bwd_apply_kernel<C><<<grid_of(static_cast<size_t>(g.B) * g.P * C / 4), 256, 0, st>>>(a);
+  return launched(e, "gn_bwd_apply");
+}
+
+// column sums of x [B][P][C] (times *scale): per image (out_img [B][C]) and / or over the batch in image order (out_sum [C])
+int run_colsum(dd_engine* e, int C, const float* x, const float* scale, int P, float* out_img, float* out_sum,
+               cudaStream_t st) {
+  const int B = e->cfg.batch, chunks = bwd_chunks(P);
+  const dim3 grid(chunks, B);
+  switch (C) {
+    case 16: dd::colsum_partial_kernel<16><<<grid, 256, 0, st>>>(x, scale, P, chunks, e->bw.col_part); break;
+    case 64: dd::colsum_partial_kernel<64><<<grid, 256, 0, st>>>(x, scale, P, chunks, e->bw.col_part); break;
+    case 256: dd::colsum_partial_kernel<256><<<grid, 256, 0, st>>>(x, scale, P, chunks, e->bw.col_part); break;
+    default: return fail(DD_ERR_INVALID, "colsum: unsupported channel count");
+  }
+  int rc;
+  if ((rc = launched(e, "colsum_partial"))) return rc;
+  dd::colsum_finalize_kernel<<<C, 32, 0, st>>>(e->bw.col_part, B, chunks, C, out_img, out_sum);
+  return launched(e, "colsum_finalize");
+}
+
+template <int TM, int TN>
+cudaError_t launch_wgrad(const dd::WgradArgs& a, int chunks, cudaStream_t st) {
+  const dim3 grid(chunks, (a.cout / TM) * (a.cin / TN) * 9);
+  dd::wgrad_simt_kernel<TM, TN><<<grid, TM * TN / 16, 0, st>>>(a);
+  return cudaGetLastError();
+}
+
+// Backward of conv layer `layer` given dy [B][P][Cout] (times *dscale, nullable = 1) and the conv's input planes X (scale
+// x_scale): dw [Cout][Cin][3][3] and db [Cout] (each nullable), and dx (nullable) = conv3x3(dy, W') on the forward's
+// tensor-core kernel, left multiplied by bw.scales[slot].
+int run_conv_bwd(dd_engine* e, int layer, const float* dy, const float* dscale, const __half* x_hi, const __half* x_lo,
+                 float x_scale, float* dw, float* db, float* dx, int slot, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  const int cout = kConvCout[layer], cin = kConvCin[layer];
+  const size_t BP = static_cast<size_t>(g.B) * g.P;
+  int rc;
+  if (db != nullptr && (rc = run_colsum(e, cout, dy, dscale, g.P, nullptr, db, st))) return rc;
+  const bool tc = dw != nullptr && wgrad_on_tc(layer);
+  if (dx != nullptr || tc) {  // split dY: the data-gradient conv and the tensor-core weight gradient read these planes
+    const size_t n = BP * cout;
+    dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(dy, static_cast<int>(n), e->bw.amax + slot);
+    if ((rc = launched(e, "grad absmax"))) return rc;
+    dd::grad_split_kernel<<<grid_of(n / 4), 256, 0, st>>>(dy, e->bw.gp.hi, e->bw.gp.lo, n / 4, e->bw.amax + slot, dscale,
+                                                          e->bw.scales + slot, e->status);
+    if ((rc = launched(e, "grad_split"))) return rc;
+  }
+  if (tc) {
+    CUtensorMap ah, al, bh, bl;
+    if ((rc = make_wgm_map(&ah, e->bw.gp.hi, g.B, g.h, g.w, cout))) return rc;
+    if ((rc = make_wgm_map(&al, e->bw.gp.lo, g.B, g.h, g.w, cout))) return rc;
+    if ((rc = make_wgm_map(&bh, x_hi, g.B, g.h, g.w, cin))) return rc;
+    if ((rc = make_wgm_map(&bl, x_lo, g.B, g.h, g.w, cin))) return rc;
+    dd::WgmArgs a;
+    a.cout = cout;
+    a.cin = cin;
+    a.B = g.B;
+    a.H = g.h;
+    a.W = g.w;
+    a.xsegs = (g.w + 63) / 64;
+    a.nseg = g.B * g.h * a.xsegs;
+    a.segs = kWgmSegs;
+    a.partial = e->bw.wg_part;
+    const int chunks = wgm_chunks(g);
+    if (cout == 256 && cin == 256) {
+      using Cf = dd::WgmCfg<128, 128>;
+      dd::wgrad_wgmma_kernel<128, 128><<<dim3(chunks, 2 * 2 * 9), Cf::THREADS, Cf::SMEM_BYTES, st>>>(ah, al, bh, bl, a);
+    } else if (cin == 64) {
+      using Cf = dd::WgmCfg<128, 64>;
+      dd::wgrad_wgmma_kernel<128, 64><<<dim3(chunks, 2 * 9), Cf::THREADS, Cf::SMEM_BYTES, st>>>(ah, al, bh, bl, a);
+    } else {
+      using Cf = dd::WgmCfg<64, 128>;
+      dd::wgrad_wgmma_kernel<64, 128><<<dim3(chunks, 2 * 9), Cf::THREADS, Cf::SMEM_BYTES, st>>>(ah, al, bh, bl, a);
+    }
+    if ((rc = launched(e, "wgrad_wgmma"))) return rc;
+    const size_t n = static_cast<size_t>(cout) * cin * 9;
+    dd::wgrad_reduce_kernel<<<grid_of(n), 256, 0, st>>>(e->bw.wg_part, chunks, cout, cin, 1, 1.0 / x_scale,
+                                                        e->bw.scales + slot, dw);
+    if ((rc = launched(e, "wgrad_reduce"))) return rc;
+  } else if (dw != nullptr) {
+    const WgPlan pl = wgrad_plan(cout, cin, static_cast<long long>(BP));
+    dd::WgradArgs a;
+    a.dy = dy;
+    a.x_hi = x_hi;
+    a.x_lo = x_lo;
+    a.x_inv_scale = 1.f / x_scale;
+    a.cout = cout;
+    a.cin = cin;
+    a.B = g.B;
+    a.H = g.h;
+    a.W = g.w;
+    a.chunk = pl.chunk;
+    a.partial = e->bw.wg_part;
+    cudaError_t err;
+    err = cout == 16 ? launch_wgrad<16, 64>(a, pl.chunks, st) : launch_wgrad<64, 16>(a, pl.chunks, st);
+    if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("wgrad: ") + cudaGetErrorString(err));
+    e->launches++;
+    const size_t n = static_cast<size_t>(cout) * cin * 9;
+    dd::wgrad_reduce_kernel<<<grid_of(n), 256, 0, st>>>(e->bw.wg_part, pl.chunks, cout, cin, 0, 1.0, dscale, dw);
+    if ((rc = launched(e, "wgrad_reduce"))) return rc;
+  }
+  if (dx != nullptr &&
+      (rc = run_conv(e, 6 + layer, e->bw.gp.hi, e->bw.gp.lo, 1.f, dd::EPI_F32, dx, nullptr, nullptr, nullptr, st)))
+    return rc;
+  return DD_OK;
+}
+
+// The forward again, keeping what the backward reads: pre-GN outputs, mean / rstd and every conv's input planes.
+int run_recompute(dd_engine* e, cudaStream_t st) {
+  dd_engine::Bwd& b = e->bw;
+  int rc;
+  if ((rc = run_conv(e, 0, e->xs_hi, e->xs_lo, kXScale, dd::EPI_F32_STATS, b.y1, e->stats[0], nullptr, nullptr, st))) return rc;
+  if ((rc = run_finalize(e, 0, 64, st))) return rc;
+  if ((rc = run_apply<64, 0>(e, 0, nullptr, 0, b.a1.hi, b.a1.lo, st, false, b.y1))) return rc;
+  if ((rc = run_conv(e, 1, b.a1.hi, b.a1.lo, kActScale, dd::EPI_F32_STATS, b.y2, e->stats[1], nullptr, nullptr, st))) return rc;
+  if ((rc = run_finalize(e, 1, 256, st))) return rc;
+  if (e->cfg.variant == DD_VARIANT_SWIN) {
+    if ((rc = run_apply<256, 2>(e, 1, e->temb_sel, 256, b.f0.hi, b.f0.lo, st, false, b.y2))) return rc;
+    if ((rc = run_conv(e, 2, b.f0.hi, b.f0.lo, kActScale, dd::EPI_SPLIT, nullptr, nullptr, b.fa.hi, b.fa.lo, st))) return rc;
+    if ((rc = run_conv(e, 3, b.fa.hi, b.fa.lo, kActScale, dd::EPI_SPLIT, nullptr, nullptr, b.fp.hi, b.fp.lo, st))) return rc;
+  } else if ((rc = run_apply<256, 1>(e, 1, e->temb_sel, 256, b.fp.hi, b.fp.lo, st, false, b.y2))) {
+    return rc;
+  }
+  if ((rc = run_conv(e, 4, b.fp.hi, b.fp.lo, kActScale, dd::EPI_F32_STATS, b.y5, e->stats[2], nullptr, nullptr, st))) return rc;
+  if ((rc = run_finalize(e, 2, 64, st))) return rc;
+  if ((rc = run_apply<64, 0>(e, 2, nullptr, 0, b.a5.hi, b.a5.lo, st, false, b.y5))) return rc;
+  if ((rc = run_conv(e, 5, b.a5.hi, b.a5.lo, kActScale, dd::EPI_F32_STATS, b.y6, e->stats[3], nullptr, nullptr, st))) return rc;
+  return run_finalize(e, 3, 16, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1511,6 +1775,21 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   }
   if ((rc = pack_layer(h, h->L[4], W("model.pred.0.weight"), W("model.pred.0.bias"), 64, 256, st, scratch))) return rc;
   if ((rc = pack_layer(h, h->L[5], W("model.pred.3.weight"), W("model.pred.3.bias"), 16, 64, st, scratch))) return rc;
+  if (h->cfg.flags & DD_FLAG_BACKWARD) {
+    // data-gradient convs: W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] with zero bias, packed like any forward layer
+    float* zeros = nullptr;
+    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&zeros), 256 * 4))) return rc;
+    CUDA_TRY(cudaMemsetAsync(zeros, 0, 256 * 4, st));
+    for (int i = 0; i < 6; ++i) {
+      if (!swin && (i == 2 || i == 3)) continue;
+      const int co = kConvCout[i], ci = kConvCin[i];
+      float* wt = nullptr;
+      if ((rc = dev_alloc(h, reinterpret_cast<void**>(&wt), static_cast<size_t>(co) * ci * 9 * 4))) return rc;
+      dd::flip_transpose_weight_kernel<<<64, 256, 0, st>>>(W((std::string(kConvKey[i]) + ".weight").c_str()), wt, co, ci);
+      CUDA_TRY(cudaGetLastError());
+      if ((rc = pack_layer(h, h->L[6 + i], wt, zeros, ci, co, st, scratch))) return rc;
+    }
+  }
   const char* gnk[4] = {"model.noise_embedding.1", "model.noise_embedding.4", "model.pred.1", "model.pred.4"};
   const int gnc[4] = {64, 256, 64, 16};
   for (int i = 0; i < 4; ++i) {
@@ -1721,6 +2000,93 @@ int dd_denoiser_forward(dd_handle h, const float* cond, const float* noisy, cons
   float* eps_nhwc = h->Y + static_cast<size_t>(g.B) * g.P * 16;
   if ((rc = run_step(h, h->temb_sel, 256, 0.f, 0.f, eps_nhwc, st))) return rc;
   if ((rc = transpose_out(eps_nhwc, eps_out, g.B, 16, g.P, st))) return rc;
+  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
+  return DD_OK;
+}
+
+int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host, const float* d_eps,
+                         float* d_cond_out, float* d_noisy_out, float* const* d_params, void* workspace,
+                         size_t workspace_bytes, void* cuda_stream) {
+  if (!h || !cond || !noisy || !t_host || !d_eps) return fail(DD_ERR_INVALID, "null argument");
+  if (!(h->cfg.flags & DD_FLAG_BACKWARD))
+    return fail(DD_ERR_INVALID, "dd_denoiser_backward needs an engine created with DD_FLAG_BACKWARD");
+  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  const Geom g = geom_of(h->cfg);
+  for (int b = 0; b < g.B; ++b)
+    if (t_host[b] < 0 || t_host[b] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
+  if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
+    return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  int rc;
+  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
+  const int npar = swin ? 21 : 17;
+  float* P[21] = {};
+  if (d_params)
+    for (int i = 0; i < npar; ++i) P[i] = d_params[i];
+  dd_engine::Bwd& bw = h->bw;
+  const size_t BP = static_cast<size_t>(g.B) * g.P;
+  const int PC = h->cfg.cond_h * h->cfg.cond_w;
+  h->launches = 0;
+  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+  CUDA_TRY(cudaMemsetAsync(bw.amax, 0, kBwdSlots * 4, st));
+  for (int b = 0; b < g.B; ++b)
+    CUDA_TRY(cudaMemcpyAsync(h->temb_sel + b * 256, h->temb + t_host[b] * 256, 1024, cudaMemcpyDeviceToDevice, st));
+  if ((rc = transpose_in(cond, h->cond, g.B, 256, PC, st))) return rc;
+  if ((rc = transpose_in(noisy, h->x32, g.B, 16, g.P, st))) return rc;
+  if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, BP * 16, kXScale, st))) return rc;
+  if ((rc = run_recompute(h, st))) return rc;
+  float *g0 = bw.g[0], *g1 = bw.g[1];
+  const float* sc = bw.scales;
+  // eps = relu(GN(y6)) -> pred.3
+  if ((rc = transpose_in(d_eps, g0, g.B, 16, g.P, st))) return rc;
+  if ((rc = run_gn_bwd<16>(h, 3, g0, nullptr, bw.y6, P[15], P[16], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 5, g1, nullptr, bw.a5.hi, bw.a5.lo, kActScale, P[13], P[14], g0, 0, st))) return rc;
+  // pred.1 -> pred.0
+  if ((rc = run_gn_bwd<64>(h, 2, g0, sc + 0, bw.y5, P[11], P[12], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 4, g1, nullptr, bw.fp.hi, bw.fp.lo, kActScale, P[9], P[10], g0, 1, st))) return rc;
+  // g0 = dF (times scales[1]).  Swin: F = convB(convA(up(cond + temb) + ne)); Res: F = cond + temb + ne
+  const float* dne_scale = sc + 1;
+  if (swin) {
+    if ((rc = run_conv_bwd(h, 3, g0, sc + 1, bw.fa.hi, bw.fa.lo, kActScale, P[19], P[20], g1, 2, st))) return rc;
+    if ((rc = run_conv_bwd(h, 2, g1, sc + 2, bw.f0.hi, bw.f0.lo, kActScale, P[17], P[18], g0, 3, st))) return rc;
+    dne_scale = sc + 3;
+    if (d_cond_out || P[8]) {
+      const float ry = g.h > 1 ? static_cast<float>(h->cfg.cond_h - 1) / static_cast<float>(g.h - 1) : 0.f;
+      const float rx = g.w > 1 ? static_cast<float>(h->cfg.cond_w - 1) / static_cast<float>(g.w - 1) : 0.f;
+      dd::up_adjoint_kernel<<<dim3(h->cfg.cond_w, h->cfg.cond_h, g.B), 256, 0, st>>>(g0, dne_scale, g.h, g.w, h->cfg.cond_h,
+                                                                                      h->cfg.cond_w, ry, rx, bw.dcond);
+      if ((rc = launched(h, "up_adjoint"))) return rc;
+      if (P[8] && (rc = run_colsum(h, 256, bw.dcond, nullptr, PC, bw.dtemb, nullptr, st))) return rc;
+      if (d_cond_out && (rc = transpose_out(bw.dcond, d_cond_out, g.B, 256, PC, st))) return rc;
+    }
+  } else {
+    if (P[8] && (rc = run_colsum(h, 256, g0, dne_scale, g.P, bw.dtemb, nullptr, st))) return rc;
+    if (d_cond_out) {
+      if ((rc = transpose_out(g0, d_cond_out, g.B, 256, g.P, st))) return rc;
+      dd::unscale_kernel<<<grid_of(BP * 256), 256, 0, st>>>(d_cond_out, BP * 256, dne_scale);
+      if ((rc = launched(h, "unscale"))) return rc;
+    }
+  }
+  if (P[8]) {  // dense [1280][256]: row t_b collects image b's d_temb, rows shared by several images sum in image order
+    CUDA_TRY(cudaMemsetAsync(P[8], 0, static_cast<size_t>(DD_TIME_ROWS) * 256 * 4, st));
+    for (int b = 0; b < g.B; ++b) {
+      dd::temb_row_add_kernel<<<1, 256, 0, st>>>(P[8] + t_host[b] * 256, bw.dtemb + b * 256);
+      if ((rc = launched(h, "temb_row_add"))) return rc;
+    }
+  }
+  // ne = relu(GN(y2)) -> noise_embedding.3 -> relu(GN(y1)) -> noise_embedding.0
+  if ((rc = run_gn_bwd<256>(h, 1, g0, dne_scale, bw.y2, P[6], P[7], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 1, g1, nullptr, bw.a1.hi, bw.a1.lo, kActScale, P[4], P[5], g0, 4, st))) return rc;
+  if ((rc = run_gn_bwd<64>(h, 0, g0, sc + 4, bw.y1, P[2], P[3], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 0, g1, nullptr, h->xs_hi, h->xs_lo, kXScale, P[0], P[1], d_noisy_out ? g0 : nullptr, 5, st)))
+    return rc;
+  if (d_noisy_out) {
+    if ((rc = transpose_out(g0, d_noisy_out, g.B, 16, g.P, st))) return rc;
+    dd::unscale_kernel<<<grid_of(BP * 16), 256, 0, st>>>(d_noisy_out, BP * 16, sc + 5);
+    if ((rc = launched(h, "unscale"))) return rc;
+  }
   if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
   return DD_OK;
 }

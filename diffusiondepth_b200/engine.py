@@ -24,6 +24,18 @@ ENCODER_KEYS = (
     "depth_transform.conv_transform.0.1.running_var", "depth_transform.conv_transform.1.0.weight",
     "depth_transform.conv_transform.1.1.weight", "depth_transform.conv_transform.1.1.bias",
     "depth_transform.conv_transform.1.1.running_mean", "depth_transform.conv_transform.1.1.running_var")
+# shapes of the denoiser's parameters (reference ScheduledCNNRefine, head :336-359) in DENOISER_KEYS + FUSE_KEYS order
+_PARAM_SHAPES = {
+    "model.noise_embedding.0.weight": (64, 16, 3, 3), "model.noise_embedding.0.bias": (64,),
+    "model.noise_embedding.1.weight": (64,), "model.noise_embedding.1.bias": (64,),
+    "model.noise_embedding.3.weight": (256, 64, 3, 3), "model.noise_embedding.3.bias": (256,),
+    "model.noise_embedding.4.weight": (256,), "model.noise_embedding.4.bias": (256,),
+    "model.time_embedding.weight": (1280, 256),
+    "model.pred.0.weight": (64, 256, 3, 3), "model.pred.0.bias": (64,), "model.pred.1.weight": (64,),
+    "model.pred.1.bias": (64,), "model.pred.3.weight": (16, 64, 3, 3), "model.pred.3.bias": (16,),
+    "model.pred.4.weight": (16,), "model.pred.4.bias": (16,),
+    "model.upsample_fuse.convA.conv.weight": (256, 256, 3, 3), "model.upsample_fuse.convA.conv.bias": (256,),
+    "model.upsample_fuse.convB.conv.weight": (256, 256, 3, 3), "model.upsample_fuse.convB.conv.bias": (256,)}
 DECODER_KEYS = (
     "depth_transform.conv_inv_transform.0.weight", "depth_transform.conv_inv_transform.0.bias",
     "depth_transform.conv_inv_transform.1.weight", "depth_transform.conv_inv_transform.1.bias",
@@ -73,7 +85,7 @@ class DenoiseEngine:
                  num_inference_steps: int, device: torch.device, cuda_graph: bool = True,
                  simt_conv: bool = False, check_range: bool = False, halo_conv: bool = True,
                  swap_narrow: bool = True, pair_wide: bool = True, step_decode: bool = False, workspace_pool=None,
-                 fp8_corr: bool = True):
+                 fp8_corr: bool = True, backward: bool = False):
         self.lib = _cabi.load_library()
         device = torch.device(device)
         if device.type != "cuda":
@@ -85,8 +97,10 @@ class DenoiseEngine:
         flags = (_cabi.FLAG_CUDA_GRAPH if cuda_graph else 0) | (_cabi.FLAG_SIMT_CONV if simt_conv else 0) | \
                 (_cabi.FLAG_CHECK_RANGE if check_range else 0) | (_cabi.FLAG_HALO_CONV if halo_conv else 0) | \
                 (_cabi.FLAG_SWAP_NARROW if swap_narrow else 0) | (_cabi.FLAG_PAIR_WIDE if pair_wide else 0) | \
-                (_cabi.FLAG_STEP_DECODE if step_decode else 0) | (_cabi.FLAG_FP8_CORR if fp8_corr else 0)
+                (_cabi.FLAG_STEP_DECODE if step_decode else 0) | (_cabi.FLAG_FP8_CORR if fp8_corr else 0) | \
+                (_cabi.FLAG_BACKWARD if backward else 0)
         self.fp8_corr = bool(fp8_corr)
+        self.backward = bool(backward)
         self.step_decode = bool(step_decode)
         cfg = _cabi.DDConfig(_cabi.ABI_VERSION, {"res": _cabi.VARIANT_RES, "swin": _cabi.VARIANT_SWIN}[variant],
                              self.batch, self.latent_hw[0], self.latent_hw[1], self.cond_hw[0], self.cond_hw[1],
@@ -251,15 +265,46 @@ class DenoiseEngine:
         B, (h, w) = self.batch, self.latent_hw
         self._check_in(cond, (B, 256, *self.cond_hw))
         self._check_in(noisy, (B, 16, h, w))
-        ts = [int(t)] * B if not hasattr(t, "__len__") else [int(v) for v in t]
-        if len(ts) == 1:
-            ts = ts * B
+        ts = self._timesteps(t)
         eps = torch.empty_like(noisy)
         ws = self._workspace()
         _cabi.check(self.lib.dd_denoiser_forward(
             self._h, C.c_void_p(cond.data_ptr()), C.c_void_p(noisy.data_ptr()), (C.c_int64 * B)(*ts),
             C.c_void_p(eps.data_ptr()), C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
         return eps
+
+    def _timesteps(self, t):
+        B = self.batch
+        ts = [int(t)] * B if not hasattr(t, "__len__") else [int(v) for v in t]
+        return ts * B if len(ts) == 1 else ts
+
+    def denoiser_backward(self, cond: torch.Tensor, noisy: torch.Tensor, t, d_eps: torch.Tensor, want_cond=True,
+                          want_noisy=True, want_params=True):
+        """Gradients of eps = ScheduledCNNRefine(noisy, t, cond) given d_eps = dL/d eps (engine created with
+        backward=True): (d_cond or None, d_noisy or None, {reference key relative to `depth_head.`: gradient}).
+        time_embedding.weight's gradient is dense [1280, 256]; rows used by several images are summed in image order."""
+        if not self.backward:
+            raise EngineError("engine was created without backward=True")
+        B, (h, w) = self.batch, self.latent_hw
+        self._check_in(cond, (B, 256, *self.cond_hw))
+        self._check_in(noisy, (B, 16, h, w))
+        self._check_in(d_eps, (B, 16, h, w))
+        ts = self._timesteps(t)
+        d_cond = torch.empty_like(cond) if want_cond else None
+        d_noisy = torch.empty_like(noisy) if want_noisy else None
+        keys = DENOISER_KEYS + (FUSE_KEYS if self.variant == "swin" else ())
+        grads = {}
+        if want_params:
+            for k in keys:
+                grads[k] = torch.empty(_PARAM_SHAPES[k], device=self.device, dtype=torch.float32)
+        ptrs = (C.c_void_p * len(keys))(*[grads[k].data_ptr() if k in grads else 0 for k in keys])
+        ws = self._workspace()
+        _cabi.check(self.lib.dd_denoiser_backward(
+            self._h, C.c_void_p(cond.data_ptr()), C.c_void_p(noisy.data_ptr()), (C.c_int64 * B)(*ts),
+            C.c_void_p(d_eps.data_ptr()), C.c_void_p(d_cond.data_ptr() if want_cond else 0),
+            C.c_void_p(d_noisy.data_ptr() if want_noisy else 0), ptrs, C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
+            C.c_void_p(self._stream())))
+        return d_cond, d_noisy, grads
 
     def encode(self, depth: torch.Tensor) -> torch.Tensor:
         """latent = depth_transform.t(depth): [B,1,H,W] -> [B,16,ceil(H/2),ceil(W/2)]."""

@@ -99,6 +99,31 @@ def _fpn_up():
     return nn.Sequential(nn.ConvTranspose2d(FPN_DIM, FPN_DIM, 2, 2, bias=False), nn.BatchNorm2d(FPN_DIM), nn.ReLU(True))
 
 
+class _DenoiserFunction(torch.autograd.Function):
+    """eps = ScheduledCNNRefine(noisy, t, cond) as an autograd node over (noisy, cond, *denoiser parameters).  The forward
+    is the head's plain `dd_denoiser_forward` call (eps bit-identical to the no-grad path) and keeps only the inputs; the
+    backward runs `dd_denoiser_backward` on an engine of the same geometry created with backward=True, which recomputes
+    the activations from those inputs."""
+
+    @staticmethod
+    def forward(ctx, head, t, keys, noisy, cond, *params):
+        eng = head._any_engine(noisy.shape[0], noisy.shape[-2:], cond.shape[-2:], noisy.device)
+        eps = eng.denoiser_forward(cond.contiguous().float(), noisy.contiguous().float(), t)
+        ctx.save_for_backward(noisy, cond, *params)
+        ctx.head, ctx.t, ctx.keys = head, t, keys
+        return eps
+
+    @staticmethod
+    def backward(ctx, d_eps):
+        noisy, cond = ctx.saved_tensors[:2]
+        need = ctx.needs_input_grad
+        eng = ctx.head._engine(noisy.shape[0], noisy.shape[-2:], cond.shape[-2:], noisy.device, backward=True)
+        d_cond, d_noisy, grads = eng.denoiser_backward(
+            cond.contiguous().float(), noisy.contiguous().float(), ctx.t, d_eps.contiguous().float(),
+            want_cond=need[4], want_noisy=need[3], want_params=any(need[5:]))
+        return (None, None, None, d_noisy, d_cond) + tuple(grads[k] if need[5 + i] else None for i, k in enumerate(ctx.keys))
+
+
 class DDIMHeadBase(nn.Module):
     """Common ctor surface: HEADS.build(dict(type=..., in_channels, inference_steps, num_train_timesteps,
     depth_feature_dim=16, loss_cfgs, init_cfg=args)) as in reference diffusion_dcbase_model.py:77-91."""
@@ -289,27 +314,29 @@ class DDIMHeadBase(nn.Module):
                     tensors[k] = v
         return tensors
 
-    def _engine(self, batch, latent_hw, cond_hw, device, feats=None, image_hw=None, backbone=None) -> DenoiseEngine:
+    def _engine(self, batch, latent_hw, cond_hw, device, feats=None, image_hw=None, backbone=None,
+                backward=False) -> DenoiseEngine:
         """feats: backbone feature maps, or a (channels, sizes) pyramid spec -> native neck/FPN;
-        image_hw: additionally run the backbone natively (`backbone`: the module holding its parameters)."""
+        image_hw: additionally run the backbone natively (`backbone`: the module holding its parameters);
+        backward: an engine that also serves `denoiser_backward`."""
         with self._lock:
-            return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone)
+            return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward)
 
-    def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone) -> DenoiseEngine:
+    def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward) -> DenoiseEngine:
         native = feats is not None
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
         key = (batch, tuple(latent_hw), tuple(cond_hw), str(device), self.diffusion_inference_steps,
                self.use_cuda_graph, native, tuple(image_hw) if image_hw is not None else None,
-               bool(self.return_intermediates), bool(self.fp8_corrections))
+               bool(self.return_intermediates), bool(self.fp8_corrections), bool(backward))
         eng = self._engines.get(key)
         if eng is None:
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
             eng = DenoiseEngine(self.variant, batch, latent_hw, cond_hw, self.diffusion_inference_steps, device,
                                 cuda_graph=self.use_cuda_graph, check_range=False,
                                 step_decode=bool(self.return_intermediates), workspace_pool=pool,
-                                fp8_corr=bool(self.fp8_corrections))
+                                fp8_corr=bool(self.fp8_corrections), backward=bool(backward))
             if native:
                 eng.enable_producers(feats[0], feats[1], has_neck=self.has_neck)
             if image_hw is not None:
@@ -362,11 +389,22 @@ class DDIMHeadBase(nn.Module):
                 break
         return self._engine(batch, latent_hw, cond_hw, device)
 
+    def _denoiser_params(self):
+        """The denoiser's parameters in DENOISER_KEYS (+ FUSE_KEYS) order: the order of dd_denoiser_backward's gradients."""
+        keys = DENOISER_KEYS + (FUSE_KEYS if self.variant == "swin" else ())
+        return keys, [self.get_submodule(k.rpartition(".")[0]).get_parameter(k.rpartition(".")[2]) for k in keys]
+
     def denoiser(self, noisy, t, cond):
-        """`self.model(noisy, t, cond, None, None, None)` of the reference, on the engine."""
+        """`self.model(noisy, t, cond, None, None, None)` of the reference, on the engine.  Differentiable (through
+        `_DenoiserFunction`, native backward) when grad is enabled and `noisy`, `cond` or a denoiser parameter requires
+        grad; otherwise the plain forward call."""
+        tl = t.reshape(-1).tolist() if torch.is_tensor(t) else t
+        if torch.is_grad_enabled():
+            keys, params = self._denoiser_params()
+            if noisy.requires_grad or cond.requires_grad or any(p.requires_grad for p in params):
+                return _DenoiserFunction.apply(self, tl, keys, noisy, cond, *params)
         B = noisy.shape[0]
         eng = self._any_engine(B, noisy.shape[-2:], cond.shape[-2:], noisy.device)
-        tl = t.reshape(-1).tolist() if torch.is_tensor(t) else t
         return eng.denoiser_forward(cond.contiguous().float(), noisy.contiguous().float(), tl)
 
     # ------------------------------------------------------------------------------------------ condition path
@@ -395,7 +433,11 @@ class DDIMHeadBase(nn.Module):
     def forward(self, fp, depth_map, depth_mask, gt_depth_map=None, return_loss=False, noise=None, image=None,
                 backbone=None, **kwargs):
         """fp: backbone feature maps — or None, meaning "run the backbone natively from `image`" (the model
-        wrapper does that when `can_run_backbone` holds, and passes `backbone` = the module holding its weights)."""
+        wrapper does that when `can_run_backbone` holds, and passes `backbone` = the module holding its weights).
+
+        Gradients: the condition map comes from the native producers (or the torch producers under no_grad) and carries
+        no gradient, so `ddim_loss` trains the denoiser's parameters only.  A caller who trains the producers passes a
+        differentiable `cond` to the operator itself, `self.model(noisy, t, cond)`, whose backward also returns d_cond."""
         with_backbone = fp is None
         if with_backbone:
             B, dev, dtype = image.shape[0], image.device, torch.float32

@@ -23,6 +23,9 @@
  *                                    (src/model/ops/depth_transform.py:33-35)
  *   dd_denoiser_forward           <- one bare `ScheduledCNNRefine.forward(noisy, t, cond, ...)` call
  *                                    (the operator `ddim_loss` invokes, head :207-223)
+ *   dd_denoiser_backward          <- reverse-mode differentiation of that call: the gradients of
+ *                                    `ScheduledCNNRefine` (head :336-382 / res.py:301-344) that `ddim_loss`
+ *                                    (head :207-223) needs for training
  *   dd_decode                     <- `depth_transform.inv_t(latent)` alone (the *Vis heads call it
  *                                    per step, ..._swin_addHAHI_vis.py)
  *
@@ -70,9 +73,12 @@ enum dd_flags {
   DD_FLAG_SWAP_NARROW = 1 << 4, /* swapped-operand narrow convs (Blackwell only; accepted without effect on sm_90a) */
   DD_FLAG_PAIR_WIDE = 1 << 5,   /* Cout = 256 convs on CTA pairs (Blackwell only; accepted without effect on sm_90a) */
   DD_FLAG_STEP_DECODE = 1 << 6, /* reserve workspace for dd_denoise_decode_steps (T decoded maps; the *Vis heads) */
-  DD_FLAG_FP8_CORR = 1 << 7     /* correction products of the split as e4m3 MMAs (Blackwell only: Hopper's e4m3 MMA
+  DD_FLAG_FP8_CORR = 1 << 7,    /* correction products of the split as e4m3 MMAs (Blackwell only: Hopper's e4m3 MMA
                                    accumulates at reduced precision, DESIGN.md "Numerics"); the sm_90a build accepts the
                                    flag and runs the exact 3-pass fp16 split everywhere */
+  DD_FLAG_BACKWARD = 1 << 8     /* enable dd_denoiser_backward: dd_finalize_weights also packs the flipped, transposed
+                                   conv weights of the data gradients, and dd_workspace_bytes includes the backward's
+                                   region (recomputed activations, gradient buffers; DESIGN.md "Backward") */
 };
 
 typedef struct dd_config {
@@ -192,6 +198,28 @@ int dd_denoise_decode_steps(dd_handle h, const float* cond, const float* noise, 
  * eps_out [B,16,h,w]. */
 int dd_denoiser_forward(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host, float* eps_out,
                         void* workspace, size_t workspace_bytes, void* cuda_stream);
+
+/* Backward of dd_denoiser_forward (reference ScheduledCNNRefine.forward, head :361-382 / res.py:324-344, differentiated
+ * in reverse mode): given d_eps [B,16,h,w] = dL/d eps for eps = ScheduledCNNRefine(noisy, t, cond), write
+ *   d_cond_out  [B,256,cond_h,cond_w]  dL/d cond   (nullable)
+ *   d_noisy_out [B,16,h,w]             dL/d noisy  (nullable)
+ *   d_params[i]                        dL/d parameter i in the reference layout (the array and each entry nullable), in
+ *                                      the order of the reference state_dict keys under `depth_head.model.`:
+ *      0 noise_embedding.0.weight [64,16,3,3]   1 noise_embedding.0.bias   2 noise_embedding.1.weight [64]
+ *      3 noise_embedding.1.bias               4 noise_embedding.3.weight [256,64,3,3]   5 noise_embedding.3.bias
+ *      6 noise_embedding.4.weight [256]       7 noise_embedding.4.bias   8 time_embedding.weight [1280,256]
+ *      9 pred.0.weight [64,256,3,3]          10 pred.0.bias   11 pred.1.weight [64]   12 pred.1.bias
+ *     13 pred.3.weight [16,64,3,3]           14 pred.3.bias   15 pred.4.weight [16]   16 pred.4.bias
+ *   and for DD_VARIANT_SWIN also
+ *     17 upsample_fuse.convA.conv.weight [256,256,3,3]   18 convA.conv.bias   19 convB.conv.weight   20 convB.conv.bias.
+ * time_embedding.weight's gradient is dense: zero except at the rows t_host[b]; a row shared by several images is the sum
+ * of their contributions in image order.  The call recomputes the forward from (cond, noisy, t) into the backward's own
+ * workspace region, then runs the backward; it does not synchronise.  Results are bit-identical run to run.
+ * Needs DD_FLAG_BACKWARD at dd_create (else DD_ERR_INVALID), as does a null cond / noisy / t_host / d_eps or a timestep
+ * outside [0, 1280).  DD_FLAG_CHECK_RANGE and dd_poll_status also report an overflow of the gradient split. */
+int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host, const float* d_eps,
+                         float* d_cond_out, float* d_noisy_out, float* const* d_params, void* workspace,
+                         size_t workspace_bytes, void* cuda_stream);
 
 /* depth = inv_t(latent): latent [B,16,h,w] -> logit_out (nullable), depth_out [B,1,2h,2w]. */
 int dd_decode(dd_handle h, const float* latent, float* logit_out, float* depth_out, void* workspace,
