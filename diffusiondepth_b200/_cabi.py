@@ -32,7 +32,7 @@ class DDBackboneConfig(C.Structure):
 ABI_VERSION = 1
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
-FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD = 64, 128, 256
+FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD, FLAG_LOOP_BACKWARD = 64, 128, 256, 512
 STATUS = {0: "DD_OK", 1: "DD_ERR_INVALID", 2: "DD_ERR_CUDA", 3: "DD_ERR_UNSUPPORTED", 4: "DD_ERR_RANGE"}
 
 # name -> (restype, argtypes); every symbol include/dd_engine.h declares
@@ -60,7 +60,12 @@ SIGNATURES = {
     "dd_denoiser_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t,
                                        C.c_void_p]),
+    "dd_denoise_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p,
+                                      C.c_void_p, C.c_size_t, C.c_void_p]),
     "dd_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "dd_decode_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
+                                     C.c_void_p, C.c_size_t, C.c_void_p]),
     "dd_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "dd_last_launch_count": (C.c_int64, [C.c_void_p]),
     "dd_poll_status": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -494,4 +494,333 @@ __global__ void __launch_bounds__(256) up_adjoint_kernel(const float* __restrict
   out[((static_cast<size_t>(b) * ch + cy) * cw + cx) * 256 + c] = acc * inv;
 }
 
+// ------------------------------------------------------------------ walk back through the DDIM loop (dd_denoise_backward)
+// x_{s+1} = c_x x_s + c_eps eps(x_s):  d_eps = c_eps g,  g <- c_x g + d_noisy.
+__global__ void scale_copy_kernel(const float* __restrict__ x, float s, float* __restrict__ out, size_t n) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    out[i] = s * x[i];
+}
+// g = cx * g + d / *dscale (dscale nullable = 1)
+__global__ void latent_grad_step_kernel(float* __restrict__ g, const float* __restrict__ d, const float* __restrict__ dscale,
+                                        float cx, size_t n) {
+  const float inv = dscale != nullptr ? 1.f / dscale[0] : 1.f;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    g[i] = fmaf(cx, g[i], d[i] * inv);
+}
+// acc += x / *scale in fp64 (scale nullable = 1; every scale here is a power of two, so the division is exact)
+__global__ void acc_add_kernel(double* __restrict__ acc, const float* __restrict__ x, const float* __restrict__ scale,
+                               size_t n) {
+  const double inv = scale != nullptr ? 1.0 / static_cast<double>(scale[0]) : 1.0;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    acc[i] += static_cast<double>(x[i]) * inv;
+}
+// time_embedding row of one step: acc_row += sum over images of d_temb[b], in image order (every image uses the row)
+__global__ void temb_acc_kernel(double* __restrict__ acc_row, const float* __restrict__ dtemb, int B) {
+  double s = 0.0;
+  for (int b = 0; b < B; ++b) s += static_cast<double>(dtemb[b * 256 + threadIdx.x]);
+  acc_row[threadIdx.x] += s;
+}
+__global__ void acc_store_kernel(const double* __restrict__ acc, float* __restrict__ out, size_t n) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    out[i] = static_cast<float>(acc[i]);
+}
+
+// ------------------------------------------------------------------ decoder backward (reverse of decoder_kernel)
+// Forward (kernels.cuh decoder_kernel): u = ConvT4x4/s2/p1(x) + b_t,  v = s (u - mean) + beta  (eval BatchNorm, s = gamma
+// rstd; the forward evaluates v with the folded weights),  r = relu(v),  z = conv3x3(r, w_c) + b_c,
+// depth = 1 / max(sigmoid(z), eps) - 1.  Reverse:
+//   dz = -d_depth e^{-z} where sigmoid(z) >= eps, else 0 (torch.clamp's gradient);
+//   dr(q) = sum_tap w_c[tap] dz(q - tap),  dw_c[ci][tap] = sum_q r[ci](q) dz(q - tap),  db_c = sum dz;
+//   dv = dr [v > 0];  dbeta = sum dv,  dgamma = sum dv (u - mean) rstd,  du = s dv,  db_t = sum du = s dbeta;
+//   dx(i) = sum over the 4 x 4 outputs o = 2 i - 1 + k of W_t[ci][co][k] du[co](o),  dW_t[ci][co][k] = sum_i x[ci](i) du[co](o).
+// 16 channels: fp32 CUDA-core kernels.  Every reduction writes fixed per-block fp64 partials that dec_bwd_finish_kernel
+// sums in block order.
+constexpr int DEC_ACT_PIX = 1024;  // output pixels per block of dec_bwd_act_kernel (4 per thread)
+constexpr int DEC_WC_PIX = 4096;   // output pixels per block of dec_bwd_wc_kernel
+constexpr int DEC_WT_PIX = 1024;   // latent pixels per block of dec_bwd_wt_kernel
+constexpr int DEC_ACT_N = 33;      // partials of dec_bwd_act_kernel: sum dv [16], sum dv * vhat [16], sum dz
+constexpr int DEC_GRAD_N = 4096 + 16 + 16 + 16 + 144 + 1;  // the six decoder gradients, reference layouts back to back
+
+struct DecBwdArgs {
+  const float* x;   // latent NHWC [B][h][w][16]
+  const float* wt;  // folded ConvT weights [ky][kx][ci][co] (the forward's)
+  const float* bt;  // folded bias [16]
+  const float* wu;  // unfolded ConvT weights [ky][kx][ci][co]
+  const float* bu;  // unfolded bias [16]
+  const float* bn;  // [3][16]: s = gamma * rstd, running mean, rstd
+  const float* wc;  // final conv [tap][ci]
+  const float* dz;  // [B][2h][2w]
+  float* r;         // [B][2h][2w][16] relu output
+  float* du;        // [B][2h][2w][16]
+  double* part_act; // [blocks][DEC_ACT_N]
+  double* part_wc;  // [blocks][144], column tap * 16 + ci
+  double* part_wt;  // [blocks][4096], column ((ky * 4 + kx) * 16 + co) * 16 + ci
+  float* dx;        // [B][h][w][16]
+  int B, h, w;
+};
+
+// dz from the forward's logit z (in place) and d_depth [B][2h][2w]; sigmoid and the clamp test as decoder_kernel does them
+__global__ void dec_dz_kernel(float* __restrict__ z, const float* __restrict__ d_depth, size_t n, float eps) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const float zv = z[i];
+    const float s = 1.0f / (1.0f + expf(-zv));
+    z[i] = s >= eps ? -d_depth[i] * expf(-zv) : 0.f;
+  }
+}
+
+// One thread per output pixel: u and v again (v in the forward's own FMA order, so the ReLU mask and r are the forward's),
+// dr from the 3 x 3 dz neighbourhood, then r, du and the per-block sums of dv, dv * vhat and dz.
+__global__ void __launch_bounds__(256) dec_bwd_act_kernel(const DecBwdArgs a) {
+  __shared__ __align__(16) float s_wt[4096];
+  __shared__ __align__(16) float s_wu[4096];
+  __shared__ double s_red[8][DEC_ACT_N];
+  for (int i = threadIdx.x; i < 1024; i += 256) {
+    reinterpret_cast<float4*>(s_wt)[i] = reinterpret_cast<const float4*>(a.wt)[i];
+    reinterpret_cast<float4*>(s_wu)[i] = reinterpret_cast<const float4*>(a.wu)[i];
+  }
+  __syncthreads();
+  const int H = 2 * a.h, W = 2 * a.w;
+  const long long N = static_cast<long long>(a.B) * H * W;
+  float acc[DEC_ACT_N];
+#pragma unroll
+  for (int j = 0; j < DEC_ACT_N; ++j) acc[j] = 0.f;
+  const long long base = static_cast<long long>(blockIdx.x) * DEC_ACT_PIX;
+  for (int k = 0; k < DEC_ACT_PIX / 256; ++k) {
+    const long long q = base + k * 256 + threadIdx.x;
+    if (q >= N) break;
+    const int b = static_cast<int>(q / (static_cast<long long>(H) * W));
+    const int Y = static_cast<int>((q / W) % H), X = static_cast<int>(q % W);
+    float of[16], ou[16];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      of[c] = a.bt[c];
+      ou[c] = a.bu[c];
+    }
+    const int ky0 = (Y + 1) & 1, kx0 = (X + 1) & 1;
+#pragma unroll
+    for (int a2 = 0; a2 < 2; ++a2) {
+      const int ky = ky0 + 2 * a2;
+      const int iy = (Y + 1 - ky) / 2;
+      if (Y + 1 - ky < 0 || iy >= a.h) continue;
+#pragma unroll
+      for (int b2 = 0; b2 < 2; ++b2) {
+        const int kx = kx0 + 2 * b2;
+        const int ix = (X + 1 - kx) / 2;
+        if (X + 1 - kx < 0 || ix >= a.w) continue;
+        const float* lp = a.x + ((static_cast<size_t>(b) * a.h + iy) * a.w + ix) * 16;
+        const float* wf = s_wt + (ky * 4 + kx) * 256;
+        const float* wn = s_wu + (ky * 4 + kx) * 256;
+#pragma unroll
+        for (int ci = 0; ci < 16; ++ci) {
+          const float v = lp[ci];
+#pragma unroll
+          for (int c = 0; c < 16; ++c) {
+            of[c] = fmaf(v, wf[ci * 16 + c], of[c]);
+            ou[c] = fmaf(v, wn[ci * 16 + c], ou[c]);
+          }
+        }
+      }
+    }
+    float dzn[9];
+#pragma unroll
+    for (int tap = 0; tap < 9; ++tap) {
+      const int yy = Y - (tap / 3 - 1), xx = X - (tap % 3 - 1);
+      dzn[tap] = (yy >= 0 && yy < H && xx >= 0 && xx < W) ? a.dz[(static_cast<size_t>(b) * H + yy) * W + xx] : 0.f;
+    }
+    acc[32] += dzn[4];
+    float rv[16], duv[16];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+      float dr = 0.f;
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) dr = fmaf(a.wc[tap * 16 + c], dzn[tap], dr);
+      const bool on = of[c] > 0.f;
+      const float dv = on ? dr : 0.f;
+      rv[c] = on ? of[c] : 0.f;
+      duv[c] = a.bn[c] * dv;
+      acc[c] += dv;
+      acc[16 + c] = fmaf(dv, (ou[c] - a.bn[16 + c]) * a.bn[32 + c], acc[16 + c]);
+    }
+    float4* rp = reinterpret_cast<float4*>(a.r + q * 16);
+    float4* dp = reinterpret_cast<float4*>(a.du + q * 16);
+#pragma unroll
+    for (int c4 = 0; c4 < 4; ++c4) {
+      rp[c4] = make_float4(rv[4 * c4], rv[4 * c4 + 1], rv[4 * c4 + 2], rv[4 * c4 + 3]);
+      dp[c4] = make_float4(duv[4 * c4], duv[4 * c4 + 1], duv[4 * c4 + 2], duv[4 * c4 + 3]);
+    }
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < DEC_ACT_N; ++j) {
+    double s = static_cast<double>(acc[j]);
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) s_red[warp][j] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < DEC_ACT_N) {
+    double s = 0.0;
+    for (int w8 = 0; w8 < 8; ++w8) s += s_red[w8][threadIdx.x];
+    a.part_act[static_cast<size_t>(blockIdx.x) * DEC_ACT_N + threadIdx.x] = s;
+  }
+}
+
+// dw_c: thread (tap, ci) = (t / 16, t % 16) walks the block's DEC_WC_PIX output pixels, fp32 for 256 pixels at a time.
+__global__ void __launch_bounds__(160) dec_bwd_wc_kernel(const DecBwdArgs a) {
+  const int t = threadIdx.x;
+  if (t >= 144) return;
+  const int tap = t / 16, ci = t % 16, dy = tap / 3 - 1, dx = tap % 3 - 1;
+  const int H = 2 * a.h, W = 2 * a.w;
+  const long long N = static_cast<long long>(a.B) * H * W;
+  const long long q0 = static_cast<long long>(blockIdx.x) * DEC_WC_PIX, q1 = min(N, q0 + DEC_WC_PIX);
+  double total = 0.0;
+  for (long long s0 = q0; s0 < q1; s0 += 256) {
+    float acc = 0.f;
+    const long long s1 = min(q1, s0 + 256);
+    for (long long q = s0; q < s1; ++q) {
+      const int Y = static_cast<int>((q / W) % H), X = static_cast<int>(q % W);
+      const int yy = Y - dy, xx = X - dx;
+      if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
+      acc = fmaf(a.r[q * 16 + ci], a.dz[q + static_cast<long long>(-dy) * W - dx], acc);
+    }
+    total += static_cast<double>(acc);
+  }
+  a.part_wc[static_cast<size_t>(blockIdx.x) * 144 + t] = total;
+}
+
+// d_latent: one thread per latent pixel gathers its 4 x 4 output pixels (unfolded weights, transposed to [k][co][ci]).
+__global__ void __launch_bounds__(256) dec_bwd_dx_kernel(const DecBwdArgs a) {
+  __shared__ __align__(16) float s_w[4096];
+  for (int i = threadIdx.x; i < 4096; i += 256) {
+    const int k = i / 256, co = (i / 16) % 16, ci = i % 16;
+    s_w[i] = a.wu[k * 256 + ci * 16 + co];
+  }
+  __syncthreads();
+  const int H = 2 * a.h, W = 2 * a.w;
+  const long long p = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (p >= static_cast<long long>(a.B) * a.h * a.w) return;
+  const int b = static_cast<int>(p / (static_cast<long long>(a.h) * a.w));
+  const int iy = static_cast<int>((p / a.w) % a.h), ix = static_cast<int>(p % a.w);
+  float acc[16];
+#pragma unroll
+  for (int c = 0; c < 16; ++c) acc[c] = 0.f;
+  for (int ky = 0; ky < 4; ++ky) {
+    const int Y = 2 * iy - 1 + ky;
+    if (Y < 0 || Y >= H) continue;
+    for (int kx = 0; kx < 4; ++kx) {
+      const int X = 2 * ix - 1 + kx;
+      if (X < 0 || X >= W) continue;
+      const float4* dp = reinterpret_cast<const float4*>(a.du + ((static_cast<size_t>(b) * H + Y) * W + X) * 16);
+      const float* wk = s_w + (ky * 4 + kx) * 256;
+#pragma unroll
+      for (int c4 = 0; c4 < 4; ++c4) {
+        const float4 d4 = dp[c4];
+        const float dv[4] = {d4.x, d4.y, d4.z, d4.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float* wr = wk + (4 * c4 + j) * 16;
+#pragma unroll
+          for (int ci = 0; ci < 16; ++ci) acc[ci] = fmaf(dv[j], wr[ci], acc[ci]);
+        }
+      }
+    }
+  }
+  float4* op = reinterpret_cast<float4*>(a.dx + p * 16);
+#pragma unroll
+  for (int c4 = 0; c4 < 4; ++c4) op[c4] = make_float4(acc[4 * c4], acc[4 * c4 + 1], acc[4 * c4 + 2], acc[4 * c4 + 3]);
+}
+
+// dW_t: thread (k, co) = (t / 16, t % 16) holds the 16 input channels; the block's latent pixels pass through shared
+// memory 64 at a time and are flushed to fp64 after each stage.
+__global__ void __launch_bounds__(256) dec_bwd_wt_kernel(const DecBwdArgs a) {
+  __shared__ __align__(16) float s_x[64][16];
+  const int t = threadIdx.x, k = t / 16, co = t % 16, ky = k / 4, kx = k % 4;
+  const int H = 2 * a.h, W = 2 * a.w;
+  const long long NP = static_cast<long long>(a.B) * a.h * a.w;
+  const long long p0 = static_cast<long long>(blockIdx.x) * DEC_WT_PIX, p1 = min(NP, p0 + DEC_WT_PIX);
+  double total[16];
+#pragma unroll
+  for (int c = 0; c < 16; ++c) total[c] = 0.0;
+  for (long long s0 = p0; s0 < p1; s0 += 64) {
+    const int n = static_cast<int>(min(64LL, p1 - s0));
+    __syncthreads();
+    {
+      const int lp = t / 4, c4 = t % 4;
+      if (lp < n) reinterpret_cast<float4*>(s_x[lp])[c4] = reinterpret_cast<const float4*>(a.x + (s0 + lp) * 16)[c4];
+    }
+    __syncthreads();
+    float acc[16];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) acc[c] = 0.f;
+    for (int j = 0; j < n; ++j) {
+      const long long p = s0 + j;
+      const int b = static_cast<int>(p / (static_cast<long long>(a.h) * a.w));
+      const int iy = static_cast<int>((p / a.w) % a.h), ix = static_cast<int>(p % a.w);
+      const int Y = 2 * iy - 1 + ky, X = 2 * ix - 1 + kx;
+      if (Y < 0 || Y >= H || X < 0 || X >= W) continue;
+      const float d = a.du[((static_cast<size_t>(b) * H + Y) * W + X) * 16 + co];
+#pragma unroll
+      for (int c4 = 0; c4 < 4; ++c4) {
+        const float4 xv = reinterpret_cast<const float4*>(s_x[j])[c4];
+        acc[4 * c4] = fmaf(xv.x, d, acc[4 * c4]);
+        acc[4 * c4 + 1] = fmaf(xv.y, d, acc[4 * c4 + 1]);
+        acc[4 * c4 + 2] = fmaf(xv.z, d, acc[4 * c4 + 2]);
+        acc[4 * c4 + 3] = fmaf(xv.w, d, acc[4 * c4 + 3]);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 16; ++c) total[c] += static_cast<double>(acc[c]);
+  }
+  double* out = a.part_wt + static_cast<size_t>(blockIdx.x) * 4096 + t * 16;
+#pragma unroll
+  for (int c = 0; c < 16; ++c) out[c] = total[c];
+}
+
+// The six gradients in the reference layouts, each partial column summed over the blocks in block order:
+// out[0] ConvT weight [16 ci][16 co][4][4], out[1] its bias, out[2] BN weight, out[3] BN bias, out[4] conv [1][16][3][3],
+// out[5] conv bias (each nullable).
+struct DecFinishArgs {
+  const double* part_act;
+  const double* part_wc;
+  const double* part_wt;
+  int nb_act, nb_wc, nb_wt;
+  const float* bn;
+  float* out[6];
+};
+__global__ void dec_bwd_finish_kernel(const DecFinishArgs f) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= DEC_GRAD_N) return;
+  double s = 0.0;
+  float* dst;
+  int o;
+  if (i < 4096) {  // [ci][co][ky][kx] <- column ((ky * 4 + kx) * 16 + co) * 16 + ci
+    const int ci = i / 256, co = (i / 16) % 16, k = i % 16;
+    const int col = (k * 16 + co) * 16 + ci;
+    for (int b = 0; b < f.nb_wt; ++b) s += f.part_wt[static_cast<size_t>(b) * 4096 + col];
+    dst = f.out[0];
+    o = i;
+  } else if (i < 4096 + 48) {  // ConvT bias = s * sum dv, BN weight = sum dv * vhat, BN bias = sum dv
+    const int j = i - 4096, c = j % 16, which = j / 16;
+    const int col = which == 1 ? 16 + c : c;
+    for (int b = 0; b < f.nb_act; ++b) s += f.part_act[static_cast<size_t>(b) * DEC_ACT_N + col];
+    if (which == 0) s *= static_cast<double>(f.bn[c]);
+    dst = which == 0 ? f.out[1] : (which == 1 ? f.out[2] : f.out[3]);  // constant indices: no local-memory copy of f
+    o = c;
+  } else if (i < 4096 + 48 + 144) {  // [ci][tap] <- column tap * 16 + ci
+    const int j = i - 4096 - 48, ci = j / 9, tap = j % 9;
+    for (int b = 0; b < f.nb_wc; ++b) s += f.part_wc[static_cast<size_t>(b) * 144 + tap * 16 + ci];
+    dst = f.out[4];
+    o = j;
+  } else {
+    for (int b = 0; b < f.nb_act; ++b) s += f.part_act[static_cast<size_t>(b) * DEC_ACT_N + 32];
+    dst = f.out[5];
+    o = 0;
+  }
+  if (dst != nullptr) dst[o] = static_cast<float>(s);
+}
+
 }  // namespace dd

@@ -353,6 +353,9 @@ struct dd_engine {
   float* dec_bt = nullptr;  // [16]
   float* dec_wc = nullptr;  // [9][16]
   float dec_bc = 0.f;
+  float* dec_wu = nullptr;  // [4][4][16][16] unfolded ConvT weights, [ky][kx][ci][co] (DD_FLAG_LOOP_BACKWARD only)
+  float* dec_bu = nullptr;  // [16] unfolded ConvT bias
+  float* dec_bn = nullptr;  // [3][16] BatchNorm scale gamma * rstd, running mean, rstd
   float *enc_w1 = nullptr, *enc_b1 = nullptr, *enc_w2 = nullptr, *enc_b2 = nullptr;  // folded encoder (optional)
   std::vector<void*> owned;
   // schedule
@@ -372,6 +375,15 @@ struct dd_engine {
     float *scales = nullptr, *amax = nullptr;  // [kBwdSlots] on-device gradient scales and their absmax inputs
     double* wg_part = nullptr;
   } bw;
+  struct LoopBwd {  // dd_denoise_backward's region (DD_FLAG_LOOP_BACKWARD)
+    float* stash = nullptr;     // [T + 1][B][P][16] the loop's latents x_T .. x_0
+    float* gl = nullptr;        // [B][P][16] running latent gradient
+    float* stage = nullptr;     // one step's parameter gradients, laid out as `acc`
+    double* acc = nullptr;      // parameter gradients summed over the steps (time_embedding dense)
+    double* acc_cond = nullptr; // [B][cond_h][cond_w][256]
+    float *z = nullptr, *r = nullptr, *du = nullptr;  // decoder backward: logit / dz [B][2h][2w], r and du [..][16]
+    double *part_act = nullptr, *part_wc = nullptr, *part_wt = nullptr;
+  } lp;
   int stats_tiles_img[4] = {0, 0, 0, 0};  // tiles per image of the kernel that last filled stats[i]
   // graph
   Producers prod;
@@ -459,6 +471,22 @@ int wgm_chunks(const Geom& g) {
   const int nseg = g.B * g.h * ((g.w + 63) / 64);
   return (nseg + kWgmSegs - 1) / kWgmSegs;
 }
+// DD_FLAG_LOOP_BACKWARD implies DD_FLAG_BACKWARD
+bool has_backward(const dd_config& c) { return (c.flags & (DD_FLAG_BACKWARD | DD_FLAG_LOOP_BACKWARD)) != 0; }
+// Elements of the denoiser's parameters in dd_denoiser_backward's order (time_embedding dense); offsets into lp.acc.
+constexpr size_t kParamNumel[21] = {64 * 16 * 9, 64, 64, 64, 256 * 64 * 9, 256, 256, 256, DD_TIME_ROWS * 256,
+                                    64 * 256 * 9, 64, 64, 64, 16 * 64 * 9, 16, 16, 16,
+                                    256 * 256 * 9, 256, 256 * 256 * 9, 256};
+int param_count(const dd_config& c) { return c.variant == DD_VARIANT_SWIN ? 21 : 17; }
+size_t param_offset(int i) {
+  size_t o = 0;
+  for (int k = 0; k < i; ++k) o += kParamNumel[k];
+  return o;
+}
+// block counts of the decoder backward's reductions
+int dec_act_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P * 4 + dd::DEC_ACT_PIX - 1) / dd::DEC_ACT_PIX); }
+int dec_wc_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P * 4 + dd::DEC_WC_PIX - 1) / dd::DEC_WC_PIX); }
+int dec_wt_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P + dd::DEC_WT_PIX - 1) / dd::DEC_WT_PIX); }
 
 void drop_graphs(dd_engine* e) {
   for (int i = 0; i < dd_engine::G_COUNT; ++i)
@@ -608,7 +636,7 @@ size_t carve(dd_engine* e, void* base) {
     mv->part_ktv = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * nk);
     mv->ktv = c.take<float>(static_cast<size_t>(g.B) * nk);
   }
-  if (e->cfg.flags & DD_FLAG_BACKWARD) {
+  if (has_backward(e->cfg)) {
     dd_engine::Bwd* bv = &v->bw;
     const bool swin = e->cfg.variant == DD_VARIANT_SWIN;
     const size_t PC = static_cast<size_t>(e->cfg.cond_h) * e->cfg.cond_w;
@@ -643,6 +671,21 @@ size_t carve(dd_engine* e, void* base) {
       wg = std::max(wg, static_cast<size_t>(chunks) * kConvCout[i] * kConvCin[i] * 9);
     }
     bv->wg_part = c.take<double>(wg);
+  }
+  if (e->cfg.flags & DD_FLAG_LOOP_BACKWARD) {
+    dd_engine::LoopBwd* lv = &v->lp;
+    const size_t np = param_offset(param_count(e->cfg)), nout = BP * 4;
+    lv->stash = c.take<float>(static_cast<size_t>(e->cfg.num_inference_steps + 1) * BP * 16);
+    lv->gl = c.take<float>(BP * 16);
+    lv->stage = c.take<float>(np);
+    lv->acc = c.take<double>(np);
+    lv->acc_cond = c.take<double>(static_cast<size_t>(g.B) * e->cfg.cond_h * e->cfg.cond_w * 256);
+    lv->z = c.take<float>(nout);
+    lv->r = c.take<float>(nout * 16);
+    lv->du = c.take<float>(nout * 16);
+    lv->part_act = c.take<double>(static_cast<size_t>(dec_act_blocks(g)) * dd::DEC_ACT_N);
+    lv->part_wc = c.take<double>(static_cast<size_t>(dec_wc_blocks(g)) * 144);
+    lv->part_wt = c.take<double>(static_cast<size_t>(dec_wt_blocks(g)) * 4096);
   }
   return align_up(c.off, 1024);
 }
@@ -1631,7 +1674,8 @@ int run_conv_bwd(dd_engine* e, int layer, const float* dy, const float* dscale, 
 }
 
 // The forward again, keeping what the backward reads: pre-GN outputs, mean / rstd and every conv's input planes.
-int run_recompute(dd_engine* e, cudaStream_t st) {
+// Image b's time-embedding row is temb + b * temb_bstride.
+int run_recompute(dd_engine* e, const float* temb, int temb_bstride, cudaStream_t st) {
   dd_engine::Bwd& b = e->bw;
   int rc;
   if ((rc = run_conv(e, 0, e->xs_hi, e->xs_lo, kXScale, dd::EPI_F32_STATS, b.y1, e->stats[0], nullptr, nullptr, st))) return rc;
@@ -1640,10 +1684,10 @@ int run_recompute(dd_engine* e, cudaStream_t st) {
   if ((rc = run_conv(e, 1, b.a1.hi, b.a1.lo, kActScale, dd::EPI_F32_STATS, b.y2, e->stats[1], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 1, 256, st))) return rc;
   if (e->cfg.variant == DD_VARIANT_SWIN) {
-    if ((rc = run_apply<256, 2>(e, 1, e->temb_sel, 256, b.f0.hi, b.f0.lo, st, false, b.y2))) return rc;
+    if ((rc = run_apply<256, 2>(e, 1, temb, temb_bstride, b.f0.hi, b.f0.lo, st, false, b.y2))) return rc;
     if ((rc = run_conv(e, 2, b.f0.hi, b.f0.lo, kActScale, dd::EPI_SPLIT, nullptr, nullptr, b.fa.hi, b.fa.lo, st))) return rc;
     if ((rc = run_conv(e, 3, b.fa.hi, b.fa.lo, kActScale, dd::EPI_SPLIT, nullptr, nullptr, b.fp.hi, b.fp.lo, st))) return rc;
-  } else if ((rc = run_apply<256, 1>(e, 1, e->temb_sel, 256, b.fp.hi, b.fp.lo, st, false, b.y2))) {
+  } else if ((rc = run_apply<256, 1>(e, 1, temb, temb_bstride, b.fp.hi, b.fp.lo, st, false, b.y2))) {
     return rc;
   }
   if ((rc = run_conv(e, 4, b.fp.hi, b.fp.lo, kActScale, dd::EPI_F32_STATS, b.y5, e->stats[2], nullptr, nullptr, st))) return rc;
@@ -1652,6 +1696,113 @@ int run_recompute(dd_engine* e, cudaStream_t st) {
   if ((rc = run_conv(e, 5, b.a5.hi, b.a5.lo, kActScale, dd::EPI_F32_STATS, b.y6, e->stats[3], nullptr, nullptr, st))) return rc;
   return run_finalize(e, 3, 16, st);
 }
+
+// Reverse mode of one ScheduledCNNRefine call on the latent in x32 / xs planes and the condition map in the workspace,
+// given d_eps (unscaled, NHWC) in bw.g[0].  Serves dd_denoiser_backward and every step of dd_denoise_backward.
+//   P[i]        (each nullable; P[8] is never written) parameter gradients in dd_denoiser_backward's order
+//   want_dtemb  per-image time-embedding gradients into bw.dtemb [B][256]; the dense table is the caller's
+//   dcond_sink  called with (d_cond NHWC [B][cond_h][cond_w][256], its scale or nullptr) at the point where d_cond is
+//               complete (for Res that buffer is reused right after); nullptr: d_cond is not needed
+//   want_dnoisy leave d_noisy times bw.scales[5] in bw.g[0]
+template <typename Sink>
+int run_denoiser_bwd(dd_engine* h, const float* temb, int temb_bstride, float* const* P, bool want_dtemb,
+                     const Sink* dcond_sink, bool want_dnoisy, cudaStream_t st) {
+  const Geom g = geom_of(h->cfg);
+  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
+  dd_engine::Bwd& bw = h->bw;
+  const int PC = h->cfg.cond_h * h->cfg.cond_w;
+  int rc;
+  CUDA_TRY(cudaMemsetAsync(bw.amax, 0, kBwdSlots * 4, st));
+  if ((rc = run_recompute(h, temb, temb_bstride, st))) return rc;
+  float *g0 = bw.g[0], *g1 = bw.g[1];
+  const float* sc = bw.scales;
+  // eps = relu(GN(y6)) -> pred.3
+  if ((rc = run_gn_bwd<16>(h, 3, g0, nullptr, bw.y6, P[15], P[16], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 5, g1, nullptr, bw.a5.hi, bw.a5.lo, kActScale, P[13], P[14], g0, 0, st))) return rc;
+  // pred.1 -> pred.0
+  if ((rc = run_gn_bwd<64>(h, 2, g0, sc + 0, bw.y5, P[11], P[12], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 4, g1, nullptr, bw.fp.hi, bw.fp.lo, kActScale, P[9], P[10], g0, 1, st))) return rc;
+  // g0 = dF (times scales[1]).  Swin: F = convB(convA(up(cond + temb) + ne)); Res: F = cond + temb + ne
+  const float* dne_scale = sc + 1;
+  if (swin) {
+    if ((rc = run_conv_bwd(h, 3, g0, sc + 1, bw.fa.hi, bw.fa.lo, kActScale, P[19], P[20], g1, 2, st))) return rc;
+    if ((rc = run_conv_bwd(h, 2, g1, sc + 2, bw.f0.hi, bw.f0.lo, kActScale, P[17], P[18], g0, 3, st))) return rc;
+    dne_scale = sc + 3;
+    if (dcond_sink || want_dtemb) {
+      const float ry = g.h > 1 ? static_cast<float>(h->cfg.cond_h - 1) / static_cast<float>(g.h - 1) : 0.f;
+      const float rx = g.w > 1 ? static_cast<float>(h->cfg.cond_w - 1) / static_cast<float>(g.w - 1) : 0.f;
+      dd::up_adjoint_kernel<<<dim3(h->cfg.cond_w, h->cfg.cond_h, g.B), 256, 0, st>>>(g0, dne_scale, g.h, g.w, h->cfg.cond_h,
+                                                                                      h->cfg.cond_w, ry, rx, bw.dcond);
+      if ((rc = launched(h, "up_adjoint"))) return rc;
+      if (want_dtemb && (rc = run_colsum(h, 256, bw.dcond, nullptr, PC, bw.dtemb, nullptr, st))) return rc;
+      if (dcond_sink && (rc = (*dcond_sink)(bw.dcond, nullptr))) return rc;
+    }
+  } else {
+    if (want_dtemb && (rc = run_colsum(h, 256, g0, dne_scale, g.P, bw.dtemb, nullptr, st))) return rc;
+    if (dcond_sink && (rc = (*dcond_sink)(g0, dne_scale))) return rc;
+  }
+  // ne = relu(GN(y2)) -> noise_embedding.3 -> relu(GN(y1)) -> noise_embedding.0
+  if ((rc = run_gn_bwd<256>(h, 1, g0, dne_scale, bw.y2, P[6], P[7], g1, st))) return rc;
+  if ((rc = run_conv_bwd(h, 1, g1, nullptr, bw.a1.hi, bw.a1.lo, kActScale, P[4], P[5], g0, 4, st))) return rc;
+  if ((rc = run_gn_bwd<64>(h, 0, g0, sc + 4, bw.y1, P[2], P[3], g1, st))) return rc;
+  return run_conv_bwd(h, 0, g1, nullptr, h->xs_hi, h->xs_lo, kXScale, P[0], P[1], want_dnoisy ? g0 : nullptr, 5, st);
+}
+
+// Reverse mode of run_decoder for the latent in x32: d_depth [B][2h][2w] -> dx (NHWC [B][P][16], nullable) and the six
+// decoder gradients dp[0..5] (array and entries nullable), in DECODER_KEYS order without the running statistics.
+int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* dp, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  dd_engine::LoopBwd& l = e->lp;
+  const size_t nout = static_cast<size_t>(g.B) * g.P * 4;
+  int rc;
+  if ((rc = run_decoder(e, l.z, l.r, st))) return rc;  // the forward's logit z; its depth lands in r (scratch until below)
+  dd::dec_dz_kernel<<<grid_of(nout), 256, 0, st>>>(l.z, d_depth, nout, 1e-6f);
+  if ((rc = launched(e, "dec_dz"))) return rc;
+  dd::DecBwdArgs a;
+  a.x = e->x32;
+  a.wt = e->dec_wt;
+  a.bt = e->dec_bt;
+  a.wu = e->dec_wu;
+  a.bu = e->dec_bu;
+  a.bn = e->dec_bn;
+  a.wc = e->dec_wc;
+  a.dz = l.z;
+  a.r = l.r;
+  a.du = l.du;
+  a.part_act = l.part_act;
+  a.part_wc = l.part_wc;
+  a.part_wt = l.part_wt;
+  a.dx = dx;
+  a.B = g.B;
+  a.h = g.h;
+  a.w = g.w;
+  dd::dec_bwd_act_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a);
+  if ((rc = launched(e, "dec_bwd_act"))) return rc;
+  if (dx != nullptr) {
+    dd::dec_bwd_dx_kernel<<<static_cast<int>((static_cast<size_t>(g.B) * g.P + 255) / 256), 256, 0, st>>>(a);
+    if ((rc = launched(e, "dec_bwd_dx"))) return rc;
+  }
+  bool any = false;
+  for (int i = 0; i < 6 && dp != nullptr; ++i) any |= dp[i] != nullptr;
+  if (!any) return DD_OK;
+  dd::dec_bwd_wc_kernel<<<dec_wc_blocks(g), 160, 0, st>>>(a);
+  if ((rc = launched(e, "dec_bwd_wc"))) return rc;
+  dd::dec_bwd_wt_kernel<<<dec_wt_blocks(g), 256, 0, st>>>(a);
+  if ((rc = launched(e, "dec_bwd_wt"))) return rc;
+  dd::DecFinishArgs f;
+  f.part_act = l.part_act;
+  f.part_wc = l.part_wc;
+  f.part_wt = l.part_wt;
+  f.nb_act = dec_act_blocks(g);
+  f.nb_wc = dec_wc_blocks(g);
+  f.nb_wt = dec_wt_blocks(g);
+  f.bn = e->dec_bn;
+  for (int i = 0; i < 6; ++i) f.out[i] = dp[i];
+  dd::dec_bwd_finish_kernel<<<(dd::DEC_GRAD_N + 255) / 256, 256, 0, st>>>(f);
+  return launched(e, "dec_bwd_finish");
+}
+
+constexpr size_t kDecGradNumel[6] = {16 * 16 * 4 * 4, 16, 16, 16, 16 * 9, 1};
 
 }  // namespace
 
@@ -1775,7 +1926,7 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   }
   if ((rc = pack_layer(h, h->L[4], W("model.pred.0.weight"), W("model.pred.0.bias"), 64, 256, st, scratch))) return rc;
   if ((rc = pack_layer(h, h->L[5], W("model.pred.3.weight"), W("model.pred.3.bias"), 16, 64, st, scratch))) return rc;
-  if (h->cfg.flags & DD_FLAG_BACKWARD) {
+  if (has_backward(h->cfg)) {
     // data-gradient convs: W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] with zero bias, packed like any forward layer
     float* zeros = nullptr;
     if ((rc = dev_alloc(h, reinterpret_cast<void**>(&zeros), 256 * 4))) return rc;
@@ -1830,6 +1981,23 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   CUDA_TRY(cudaMemcpyAsync(h->dec_bt, bt_f.data(), 64, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(h->dec_wc, wc_f.data(), wc_f.size() * 4, cudaMemcpyHostToDevice, st));
   h->dec_bc = bc[0];
+  if (h->cfg.flags & DD_FLAG_LOOP_BACKWARD) {  // the decoder backward needs the BatchNorm unfolded
+    std::vector<float> wu(4 * 4 * 16 * 16), bn(3 * 16);
+    for (int co = 0; co < 16; ++co) {
+      const double rstd = 1.0 / sqrt(static_cast<double>(var[co]) + 1e-5);
+      bn[co] = static_cast<float>(static_cast<double>(g[co]) * rstd);
+      bn[16 + co] = mu[co];
+      bn[32 + co] = static_cast<float>(rstd);
+      for (int ci = 0; ci < 16; ++ci)
+        for (int k = 0; k < 16; ++k) wu[(k * 16 + ci) * 16 + co] = wt[(ci * 16 + co) * 16 + k];
+    }
+    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_wu), wu.size() * 4))) return rc;
+    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_bu), 64))) return rc;
+    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_bn), bn.size() * 4))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(h->dec_wu, wu.data(), wu.size() * 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->dec_bu, bt.data(), 64, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->dec_bn, bn.data(), bn.size() * 4, cudaMemcpyHostToDevice, st));
+  }
   CUDA_TRY(cudaStreamSynchronize(st));
   h->enc_w1 = nullptr;
   if (find(h, "depth_transform.conv_transform.0.0.weight")) {
@@ -2008,8 +2176,8 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
                          float* d_cond_out, float* d_noisy_out, float* const* d_params, void* workspace,
                          size_t workspace_bytes, void* cuda_stream) {
   if (!h || !cond || !noisy || !t_host || !d_eps) return fail(DD_ERR_INVALID, "null argument");
-  if (!(h->cfg.flags & DD_FLAG_BACKWARD))
-    return fail(DD_ERR_INVALID, "dd_denoiser_backward needs an engine created with DD_FLAG_BACKWARD");
+  if (!has_backward(h->cfg))
+    return fail(DD_ERR_INVALID, "dd_denoiser_backward needs an engine created with DD_FLAG_BACKWARD (or DD_FLAG_LOOP_BACKWARD)");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   const Geom g = geom_of(h->cfg);
   for (int b = 0; b < g.B; ++b)
@@ -2030,45 +2198,23 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
   const int PC = h->cfg.cond_h * h->cfg.cond_w;
   h->launches = 0;
   CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
-  CUDA_TRY(cudaMemsetAsync(bw.amax, 0, kBwdSlots * 4, st));
   for (int b = 0; b < g.B; ++b)
     CUDA_TRY(cudaMemcpyAsync(h->temb_sel + b * 256, h->temb + t_host[b] * 256, 1024, cudaMemcpyDeviceToDevice, st));
   if ((rc = transpose_in(cond, h->cond, g.B, 256, PC, st))) return rc;
   if ((rc = transpose_in(noisy, h->x32, g.B, 16, g.P, st))) return rc;
   if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, BP * 16, kXScale, st))) return rc;
-  if ((rc = run_recompute(h, st))) return rc;
-  float *g0 = bw.g[0], *g1 = bw.g[1];
-  const float* sc = bw.scales;
-  // eps = relu(GN(y6)) -> pred.3
-  if ((rc = transpose_in(d_eps, g0, g.B, 16, g.P, st))) return rc;
-  if ((rc = run_gn_bwd<16>(h, 3, g0, nullptr, bw.y6, P[15], P[16], g1, st))) return rc;
-  if ((rc = run_conv_bwd(h, 5, g1, nullptr, bw.a5.hi, bw.a5.lo, kActScale, P[13], P[14], g0, 0, st))) return rc;
-  // pred.1 -> pred.0
-  if ((rc = run_gn_bwd<64>(h, 2, g0, sc + 0, bw.y5, P[11], P[12], g1, st))) return rc;
-  if ((rc = run_conv_bwd(h, 4, g1, nullptr, bw.fp.hi, bw.fp.lo, kActScale, P[9], P[10], g0, 1, st))) return rc;
-  // g0 = dF (times scales[1]).  Swin: F = convB(convA(up(cond + temb) + ne)); Res: F = cond + temb + ne
-  const float* dne_scale = sc + 1;
-  if (swin) {
-    if ((rc = run_conv_bwd(h, 3, g0, sc + 1, bw.fa.hi, bw.fa.lo, kActScale, P[19], P[20], g1, 2, st))) return rc;
-    if ((rc = run_conv_bwd(h, 2, g1, sc + 2, bw.f0.hi, bw.f0.lo, kActScale, P[17], P[18], g0, 3, st))) return rc;
-    dne_scale = sc + 3;
-    if (d_cond_out || P[8]) {
-      const float ry = g.h > 1 ? static_cast<float>(h->cfg.cond_h - 1) / static_cast<float>(g.h - 1) : 0.f;
-      const float rx = g.w > 1 ? static_cast<float>(h->cfg.cond_w - 1) / static_cast<float>(g.w - 1) : 0.f;
-      dd::up_adjoint_kernel<<<dim3(h->cfg.cond_w, h->cfg.cond_h, g.B), 256, 0, st>>>(g0, dne_scale, g.h, g.w, h->cfg.cond_h,
-                                                                                      h->cfg.cond_w, ry, rx, bw.dcond);
-      if ((rc = launched(h, "up_adjoint"))) return rc;
-      if (P[8] && (rc = run_colsum(h, 256, bw.dcond, nullptr, PC, bw.dtemb, nullptr, st))) return rc;
-      if (d_cond_out && (rc = transpose_out(bw.dcond, d_cond_out, g.B, 256, PC, st))) return rc;
-    }
-  } else {
-    if (P[8] && (rc = run_colsum(h, 256, g0, dne_scale, g.P, bw.dtemb, nullptr, st))) return rc;
-    if (d_cond_out) {
-      if ((rc = transpose_out(g0, d_cond_out, g.B, 256, g.P, st))) return rc;
-      dd::unscale_kernel<<<grid_of(BP * 256), 256, 0, st>>>(d_cond_out, BP * 256, dne_scale);
-      if ((rc = launched(h, "unscale"))) return rc;
-    }
-  }
+  if ((rc = transpose_in(d_eps, bw.g[0], g.B, 16, g.P, st))) return rc;
+  auto sink = [&](const float* dc, const float* scale) -> int {
+    int r;
+    if ((r = transpose_out(dc, d_cond_out, g.B, 256, PC, st))) return r;
+    if (scale == nullptr) return DD_OK;
+    dd::unscale_kernel<<<grid_of(static_cast<size_t>(g.B) * PC * 256), 256, 0, st>>>(d_cond_out,
+                                                                                     static_cast<size_t>(g.B) * PC * 256, scale);
+    return launched(h, "unscale");
+  };
+  if ((rc = run_denoiser_bwd(h, h->temb_sel, 256, P, P[8] != nullptr, d_cond_out ? &sink : nullptr, d_noisy_out != nullptr,
+                             st)))
+    return rc;
   if (P[8]) {  // dense [1280][256]: row t_b collects image b's d_temb, rows shared by several images sum in image order
     CUDA_TRY(cudaMemsetAsync(P[8], 0, static_cast<size_t>(DD_TIME_ROWS) * 256 * 4, st));
     for (int b = 0; b < g.B; ++b) {
@@ -2076,18 +2222,135 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
       if ((rc = launched(h, "temb_row_add"))) return rc;
     }
   }
-  // ne = relu(GN(y2)) -> noise_embedding.3 -> relu(GN(y1)) -> noise_embedding.0
-  if ((rc = run_gn_bwd<256>(h, 1, g0, dne_scale, bw.y2, P[6], P[7], g1, st))) return rc;
-  if ((rc = run_conv_bwd(h, 1, g1, nullptr, bw.a1.hi, bw.a1.lo, kActScale, P[4], P[5], g0, 4, st))) return rc;
-  if ((rc = run_gn_bwd<64>(h, 0, g0, sc + 4, bw.y1, P[2], P[3], g1, st))) return rc;
-  if ((rc = run_conv_bwd(h, 0, g1, nullptr, h->xs_hi, h->xs_lo, kXScale, P[0], P[1], d_noisy_out ? g0 : nullptr, 5, st)))
-    return rc;
   if (d_noisy_out) {
-    if ((rc = transpose_out(g0, d_noisy_out, g.B, 16, g.P, st))) return rc;
-    dd::unscale_kernel<<<grid_of(BP * 16), 256, 0, st>>>(d_noisy_out, BP * 16, sc + 5);
+    if ((rc = transpose_out(bw.g[0], d_noisy_out, g.B, 16, g.P, st))) return rc;
+    dd::unscale_kernel<<<grid_of(BP * 16), 256, 0, st>>>(d_noisy_out, BP * 16, bw.scales + 5);
     if ((rc = launched(h, "unscale"))) return rc;
   }
   if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
+  return DD_OK;
+}
+
+int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, const float* d_depth, const float* d_latent,
+                        float* d_cond_out, float* d_noise_out, float* const* d_params, float* const* d_dec_params,
+                        float* latents_out, void* workspace, size_t workspace_bytes, void* cuda_stream) {
+  if (!h || !noise) return fail(DD_ERR_INVALID, "null argument");
+  if (!(h->cfg.flags & DD_FLAG_LOOP_BACKWARD))
+    return fail(DD_ERR_INVALID, "dd_denoise_backward needs an engine created with DD_FLAG_LOOP_BACKWARD");
+  if (!d_depth && !d_latent) return fail(DD_ERR_INVALID, "d_depth and d_latent are both NULL");
+  if (!cond && !h->cond_ready) return fail(DD_ERR_INVALID, "cond is NULL but dd_build_condition has not run");
+  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  const int T = h->cfg.num_inference_steps;
+  if (static_cast<int>(h->ts.size()) != T) return fail(DD_ERR_INVALID, "dd_set_schedule has not been called");
+  const Geom g = geom_of(h->cfg);
+  if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
+    return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  int rc;
+  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  dd_engine::LoopBwd& l = h->lp;
+  const size_t BP = static_cast<size_t>(g.B) * g.P, nx = BP * 16;
+  const size_t ncond = static_cast<size_t>(g.B) * h->cfg.cond_h * h->cfg.cond_w * 256;
+  const int npar = param_count(h->cfg);
+  if (cond) {
+    h->launches = 0;
+    CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+    if ((rc = transpose_in(cond, h->cond, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
+  }  // else: dd_build_condition left the NHWC condition map in place
+  h->cond_ready = false;
+  // 1. the forward again, un-graphed, with the forward's kernels: stash[s] = x before step s, stash[T] = x_0
+  if ((rc = transpose_in(noise, h->x32, g.B, 16, g.P, st))) return rc;
+  if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, nx, kXScale, st))) return rc;
+  for (int s = 0; s < T; ++s) {
+    CUDA_TRY(cudaMemcpyAsync(l.stash + s * nx, h->x32, nx * 4, cudaMemcpyDeviceToDevice, st));
+    if ((rc = run_step(h, h->temb + h->ts[s] * 256, 0, h->cx[s], h->ce[s], nullptr, st))) return rc;
+  }
+  CUDA_TRY(cudaMemcpyAsync(l.stash + T * nx, h->x32, nx * 4, cudaMemcpyDeviceToDevice, st));
+  if (latents_out)
+    for (int s = 0; s <= T; ++s)
+      if ((rc = transpose_out(l.stash + s * nx, latents_out + s * nx, g.B, 16, g.P, st))) return rc;
+  // 2. seed: g = d_latent + the decoder's backward at x_0 (still in x32)
+  if (d_latent) {
+    if ((rc = transpose_in(d_latent, l.gl, g.B, 16, g.P, st))) return rc;
+  } else {
+    CUDA_TRY(cudaMemsetAsync(l.gl, 0, nx * 4, st));
+  }
+  if (d_depth) {
+    if ((rc = run_decode_bwd(h, d_depth, h->bw.g[1], d_dec_params, st))) return rc;
+    dd::latent_grad_step_kernel<<<grid_of(nx), 256, 0, st>>>(l.gl, h->bw.g[1], nullptr, 1.f, nx);
+    if ((rc = launched(h, "latent_grad_step"))) return rc;
+  } else if (d_dec_params) {  // the depth does not enter the loss: zero decoder gradients
+    for (int i = 0; i < 6; ++i)
+      if (d_dec_params[i]) CUDA_TRY(cudaMemsetAsync(d_dec_params[i], 0, kDecGradNumel[i] * 4, st));
+  }
+  // 3. walk back: step s maps x_s -> x_{s+1} = c_x x_s + c_eps eps(x_s)
+  float* P[21] = {};
+  bool want_dtemb = false;
+  if (d_params) {
+    for (int i = 0; i < npar; ++i)
+      if (d_params[i] && i != 8) P[i] = l.stage + param_offset(i);
+    want_dtemb = d_params[8] != nullptr;
+  }
+  CUDA_TRY(cudaMemsetAsync(l.acc, 0, param_offset(npar) * 8, st));
+  if (d_cond_out) CUDA_TRY(cudaMemsetAsync(l.acc_cond, 0, ncond * 8, st));
+  auto sink = [&](const float* dc, const float* scale) -> int {
+    dd::acc_add_kernel<<<grid_of(ncond), 256, 0, st>>>(l.acc_cond, dc, scale, ncond);
+    return launched(h, "acc_add");
+  };
+  for (int s = T - 1; s >= 0; --s) {
+    CUDA_TRY(cudaMemcpyAsync(h->x32, l.stash + s * nx, nx * 4, cudaMemcpyDeviceToDevice, st));
+    if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, nx, kXScale, st))) return rc;
+    dd::scale_copy_kernel<<<grid_of(nx), 256, 0, st>>>(l.gl, h->ce[s], h->bw.g[0], nx);
+    if ((rc = launched(h, "scale_copy"))) return rc;
+    const bool want_dnoisy = s > 0 || d_noise_out != nullptr;
+    if ((rc = run_denoiser_bwd(h, h->temb + h->ts[s] * 256, 0, P, want_dtemb, d_cond_out ? &sink : nullptr, want_dnoisy, st)))
+      return rc;
+    for (int i = 0; i < npar; ++i) {
+      if (!P[i]) continue;
+      dd::acc_add_kernel<<<grid_of(kParamNumel[i]), 256, 0, st>>>(l.acc + param_offset(i), P[i], nullptr, kParamNumel[i]);
+      if ((rc = launched(h, "acc_add"))) return rc;
+    }
+    if (want_dtemb) {
+      dd::temb_acc_kernel<<<1, 256, 0, st>>>(l.acc + param_offset(8) + h->ts[s] * 256, h->bw.dtemb, g.B);
+      if ((rc = launched(h, "temb_acc"))) return rc;
+    }
+    if (want_dnoisy) {
+      dd::latent_grad_step_kernel<<<grid_of(nx), 256, 0, st>>>(l.gl, h->bw.g[0], h->bw.scales + 5, h->cx[s], nx);
+      if ((rc = launched(h, "latent_grad_step"))) return rc;
+    }
+  }
+  // 4. outputs
+  if (d_noise_out && (rc = transpose_out(l.gl, d_noise_out, g.B, 16, g.P, st))) return rc;
+  for (int i = 0; i < npar && d_params; ++i) {
+    if (!d_params[i]) continue;
+    dd::acc_store_kernel<<<grid_of(kParamNumel[i]), 256, 0, st>>>(l.acc + param_offset(i), d_params[i], kParamNumel[i]);
+    if ((rc = launched(h, "acc_store"))) return rc;
+  }
+  if (d_cond_out) {  // fp32 NHWC in a backward buffer of at least that size, then NCHW
+    float* dc32 = h->cfg.variant == DD_VARIANT_SWIN ? h->bw.dcond : h->bw.g[1];
+    dd::acc_store_kernel<<<grid_of(ncond), 256, 0, st>>>(l.acc_cond, dc32, ncond);
+    if ((rc = launched(h, "acc_store"))) return rc;
+    if ((rc = transpose_out(dc32, d_cond_out, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
+  }
+  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
+  return DD_OK;
+}
+
+int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, float* d_latent_out,
+                       float* const* d_dec_params, void* workspace, size_t workspace_bytes, void* cuda_stream) {
+  if (!h || !latent || !d_depth) return fail(DD_ERR_INVALID, "null argument");
+  if (!(h->cfg.flags & DD_FLAG_LOOP_BACKWARD))
+    return fail(DD_ERR_INVALID, "dd_decode_backward needs an engine created with DD_FLAG_LOOP_BACKWARD");
+  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  int rc;
+  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  const Geom g = geom_of(h->cfg);
+  if ((rc = transpose_in(latent, h->x32, g.B, 16, g.P, st))) return rc;
+  if ((rc = run_decode_bwd(h, d_depth, d_latent_out ? h->bw.g[1] : nullptr, d_dec_params, st))) return rc;
+  if (d_latent_out) return transpose_out(h->bw.g[1], d_latent_out, g.B, 16, g.P, st);
   return DD_OK;
 }
 

@@ -41,6 +41,11 @@ DECODER_KEYS = (
     "depth_transform.conv_inv_transform.1.weight", "depth_transform.conv_inv_transform.1.bias",
     "depth_transform.conv_inv_transform.1.running_mean", "depth_transform.conv_inv_transform.1.running_var",
     "depth_transform.conv_inv_transform.3.0.weight", "depth_transform.conv_inv_transform.3.0.bias")
+# the decoder's parameters (DECODER_KEYS without the running statistics): the order of dd_denoise_backward's d_dec_params
+DECODER_PARAM_KEYS = tuple(k for k in DECODER_KEYS if "running" not in k)
+_DECODER_SHAPES = {"depth_transform.conv_inv_transform.0.weight": (16, 16, 4, 4),
+                   "depth_transform.conv_inv_transform.3.0.weight": (1, 16, 3, 3),
+                   "depth_transform.conv_inv_transform.3.0.bias": (1,)}
 
 
 def ddim_coefficients(alphas_cumprod: torch.Tensor, num_inference_steps: int, num_train_timesteps: int,
@@ -85,7 +90,7 @@ class DenoiseEngine:
                  num_inference_steps: int, device: torch.device, cuda_graph: bool = True,
                  simt_conv: bool = False, check_range: bool = False, halo_conv: bool = True,
                  swap_narrow: bool = True, pair_wide: bool = True, step_decode: bool = False, workspace_pool=None,
-                 fp8_corr: bool = True, backward: bool = False):
+                 fp8_corr: bool = True, backward: bool = False, loop_backward: bool = False):
         self.lib = _cabi.load_library()
         device = torch.device(device)
         if device.type != "cuda":
@@ -98,9 +103,10 @@ class DenoiseEngine:
                 (_cabi.FLAG_CHECK_RANGE if check_range else 0) | (_cabi.FLAG_HALO_CONV if halo_conv else 0) | \
                 (_cabi.FLAG_SWAP_NARROW if swap_narrow else 0) | (_cabi.FLAG_PAIR_WIDE if pair_wide else 0) | \
                 (_cabi.FLAG_STEP_DECODE if step_decode else 0) | (_cabi.FLAG_FP8_CORR if fp8_corr else 0) | \
-                (_cabi.FLAG_BACKWARD if backward else 0)
+                (_cabi.FLAG_BACKWARD if backward else 0) | (_cabi.FLAG_LOOP_BACKWARD if loop_backward else 0)
         self.fp8_corr = bool(fp8_corr)
-        self.backward = bool(backward)
+        self.backward = bool(backward or loop_backward)  # the loop backward includes the operator's
+        self.loop_backward = bool(loop_backward)
         self.step_decode = bool(step_decode)
         cfg = _cabi.DDConfig(_cabi.ABI_VERSION, {"res": _cabi.VARIANT_RES, "swin": _cabi.VARIANT_SWIN}[variant],
                              self.batch, self.latent_hw[0], self.latent_hw[1], self.cond_hw[0], self.cond_hw[1],
@@ -305,6 +311,65 @@ class DenoiseEngine:
             C.c_void_p(d_noisy.data_ptr() if want_noisy else 0), ptrs, C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
             C.c_void_p(self._stream())))
         return d_cond, d_noisy, grads
+
+    def _grad_buffers(self, keys, shapes, default=None):
+        grads = {k: torch.empty(shapes.get(k, default), device=self.device, dtype=torch.float32) for k in keys}
+        return grads, (C.c_void_p * len(keys))(*[grads[k].data_ptr() for k in keys])
+
+    def denoise_backward(self, cond: Optional[torch.Tensor], noise: torch.Tensor, d_depth: Optional[torch.Tensor],
+                         d_latent: Optional[torch.Tensor], want_latents=False, want_cond=True, want_noise=True,
+                         want_params=True):
+        """Gradients of (depth, latent) = denoise_decode(cond, noise) through all T steps and the decoder (engine
+        created with loop_backward=True), given d_depth [B,1,2h,2w] and / or d_latent [B,16,h,w]:
+        (d_cond or None, d_noise or None, {reference key relative to `depth_head.`: gradient} for the denoiser and the
+        decoder parameters, latents [T+1,B,16,h,w] (x_T .. x_0 as recomputed) or None).  time_embedding.weight's
+        gradient is dense [1280, 256].  `cond` may be None right after build_condition."""
+        if not self.loop_backward:
+            raise EngineError("engine was created without loop_backward=True")
+        if d_depth is None and d_latent is None:
+            raise EngineError("denoise_backward needs d_depth or d_latent")
+        B, (h, w) = self.batch, self.latent_hw
+        if cond is not None:
+            self._check_in(cond, (B, 256, *self.cond_hw))
+        self._check_in(noise, (B, 16, h, w))
+        if d_depth is not None:
+            self._check_in(d_depth, (B, 1, 2 * h, 2 * w))
+        if d_latent is not None:
+            self._check_in(d_latent, (B, 16, h, w))
+        d_cond = torch.empty(B, 256, *self.cond_hw, device=self.device) if want_cond else None
+        d_noise = torch.empty_like(noise) if want_noise else None
+        latents = torch.empty(self.steps + 1, B, 16, h, w, device=self.device) if want_latents else None
+        keys = DENOISER_KEYS + (FUSE_KEYS if self.variant == "swin" else ())
+        grads, ptrs = self._grad_buffers(keys if want_params else (), _PARAM_SHAPES)
+        dgrads, dptrs = self._grad_buffers(DECODER_PARAM_KEYS if want_params else (), _DECODER_SHAPES, (16,))
+        ws = self._workspace()
+
+        def ptr(t):
+            return C.c_void_p(t.data_ptr() if t is not None else 0)
+
+        _cabi.check(self.lib.dd_denoise_backward(
+            self._h, ptr(cond), ptr(noise), ptr(d_depth), ptr(d_latent), ptr(d_cond), ptr(d_noise),
+            ptrs if want_params else None, dptrs if want_params else None, ptr(latents), C.c_void_p(self._aligned(ws)),
+            ws.numel() - 1024, C.c_void_p(self._stream())))
+        grads.update(dgrads)
+        return d_cond, d_noise, grads, latents
+
+    def decode_backward(self, latent: torch.Tensor, d_depth: torch.Tensor, want_latent=True, want_params=True):
+        """Gradients of depth = decode(latent) given d_depth [B,1,2h,2w] (engine created with loop_backward=True):
+        (d_latent or None, {decoder key relative to `depth_head.`: gradient})."""
+        if not self.loop_backward:
+            raise EngineError("engine was created without loop_backward=True")
+        B, (h, w) = self.batch, self.latent_hw
+        self._check_in(latent, (B, 16, h, w))
+        self._check_in(d_depth, (B, 1, 2 * h, 2 * w))
+        d_latent = torch.empty_like(latent) if want_latent else None
+        grads, ptrs = self._grad_buffers(DECODER_PARAM_KEYS if want_params else (), _DECODER_SHAPES, (16,))
+        ws = self._workspace()
+        _cabi.check(self.lib.dd_decode_backward(
+            self._h, C.c_void_p(latent.data_ptr()), C.c_void_p(d_depth.data_ptr()),
+            C.c_void_p(d_latent.data_ptr() if want_latent else 0), ptrs if want_params else None,
+            C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
+        return d_latent, grads
 
     def encode(self, depth: torch.Tensor) -> torch.Tensor:
         """latent = depth_transform.t(depth): [B,1,H,W] -> [B,16,ceil(H/2),ceil(W/2)]."""

@@ -22,8 +22,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from diffusiondepth_b200._cabi import EngineError
-from diffusiondepth_b200.engine import (DECODER_KEYS, DENOISER_KEYS, ENCODER_KEYS, FUSE_KEYS, DenoiseEngine,
-                                        WorkspacePool)
+from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS, FUSE_KEYS,
+                                        DenoiseEngine, WorkspacePool)
 from .._blocks import ConvModule, exact_fp32
 from ..diffusers.schedulers.scheduling_ddim import DDIMScheduler
 from ..ops import depth_transform as _codec  # noqa: F401  (registers the codec classes)
@@ -117,11 +117,42 @@ class _DenoiserFunction(torch.autograd.Function):
     def backward(ctx, d_eps):
         noisy, cond = ctx.saved_tensors[:2]
         need = ctx.needs_input_grad
-        eng = ctx.head._engine(noisy.shape[0], noisy.shape[-2:], cond.shape[-2:], noisy.device, backward=True)
+        eng = ctx.head._grad_engine(noisy.shape[0], noisy.shape[-2:], cond.shape[-2:], noisy.device)
         d_cond, d_noisy, grads = eng.denoiser_backward(
             cond.contiguous().float(), noisy.contiguous().float(), ctx.t, d_eps.contiguous().float(),
             want_cond=need[4], want_noisy=need[3], want_params=any(need[5:]))
         return (None, None, None, d_noisy, d_cond) + tuple(grads[k] if need[5 + i] else None for i, k in enumerate(ctx.keys))
+
+
+class _LoopFunction(torch.autograd.Function):
+    """(depth, latent) = inv_t(CNNDDIMPipiline(cond, noise)) as an autograd node over (cond, noise, *denoiser parameters,
+    *decoder parameters).  The forward is the head's own `denoise_decode` call on `eng` (with native producers
+    cond = None: the condition map is already in the workspace), so both outputs are bit-identical to the no-grad path;
+    it keeps cond and noise.  The backward runs `dd_denoise_backward` on an engine of the same geometry created with
+    loop_backward=True, which re-runs the loop and walks back through every step and the decoder."""
+
+    @staticmethod
+    def forward(ctx, head, eng, box, cond_in_workspace, keys, cond, noise, *params):
+        depth, latent, logits = eng.denoise_decode(None if cond_in_workspace else cond, noise, want_latent=True,
+                                                   want_logits=head.capture_logits)
+        box["logits"] = logits
+        ctx.save_for_backward(cond, noise)
+        ctx.head, ctx.keys = head, keys
+        ctx.set_materialize_grads(False)
+        return depth, latent
+
+    @staticmethod
+    def backward(ctx, d_depth, d_latent):
+        cond, noise = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        if d_depth is None and d_latent is None:
+            return (None,) * len(need)
+        eng = ctx.head._engine(noise.shape[0], noise.shape[-2:], cond.shape[-2:], noise.device, loop_backward=True)
+        d_cond, d_noise, grads, _ = eng.denoise_backward(
+            cond.contiguous().float(), noise, None if d_depth is None else d_depth.contiguous().float(),
+            None if d_latent is None else d_latent.contiguous().float(),
+            want_cond=need[5], want_noise=need[6], want_params=any(need[7:]))
+        return (None,) * 5 + (d_cond, d_noise) + tuple(grads[k] if need[7 + i] else None for i, k in enumerate(ctx.keys))
 
 
 class DDIMHeadBase(nn.Module):
@@ -132,6 +163,11 @@ class DDIMHeadBase(nn.Module):
     fpn_in_channels = (64, 128, 256, 512)
     has_neck = False         # HAHI neck in front of the FPN (the *HAHI heads)
     return_intermediates = False  # *Vis heads: also decode every intermediate latent -> 'pred_inter'
+    # Training through the sampling loop: when True, grad is enabled and a denoiser / decoder parameter (or cond) requires
+    # grad, `pred` and the final latent carry the reference's training-graph gradients through all T steps and the
+    # decoder (native dd_denoise_backward), so the L1 / L2 depth losses train the head and `ddim_loss` also reaches the
+    # loop through its re-noised latent.  Off by default: it changes what `ddim_loss.backward()` costs and computes.
+    grad_through_loop = False
 
     def __init__(self, in_channels=None, up_scale_factor=1, inference_steps=20, num_train_timesteps=1000,
                  return_indices=None, depth_transform_cfg=None, detach_fp=False, depth_embed_dim=16,
@@ -315,28 +351,41 @@ class DDIMHeadBase(nn.Module):
         return tensors
 
     def _engine(self, batch, latent_hw, cond_hw, device, feats=None, image_hw=None, backbone=None,
-                backward=False) -> DenoiseEngine:
+                backward=False, loop_backward=False) -> DenoiseEngine:
         """feats: backbone feature maps, or a (channels, sizes) pyramid spec -> native neck/FPN;
         image_hw: additionally run the backbone natively (`backbone`: the module holding its parameters);
-        backward: an engine that also serves `denoiser_backward`."""
+        backward: an engine that also serves `denoiser_backward`; loop_backward: one that also serves
+        `denoise_backward` / `decode_backward` (and `denoiser_backward`)."""
         with self._lock:
-            return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward)
+            return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
+                                       loop_backward)
 
-    def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward) -> DenoiseEngine:
+    def _grad_engine(self, batch, latent_hw, cond_hw, device) -> DenoiseEngine:
+        """The engine `denoiser_backward` runs on: the loop-backward engine of this geometry when the head trains through
+        the loop or that engine exists (its flag is a superset), else a backward-only one."""
+        loop_key = (batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)), self.diffusion_inference_steps,
+                    self.use_cuda_graph, False, None, bool(self.return_intermediates), bool(self.fp8_corrections),
+                    False, True)
+        loop = self.grad_through_loop or loop_key in self._engines
+        return self._engine(batch, latent_hw, cond_hw, device, backward=not loop, loop_backward=loop)
+
+    def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
+                       loop_backward) -> DenoiseEngine:
         native = feats is not None
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
         key = (batch, tuple(latent_hw), tuple(cond_hw), str(device), self.diffusion_inference_steps,
                self.use_cuda_graph, native, tuple(image_hw) if image_hw is not None else None,
-               bool(self.return_intermediates), bool(self.fp8_corrections), bool(backward))
+               bool(self.return_intermediates), bool(self.fp8_corrections), bool(backward), bool(loop_backward))
         eng = self._engines.get(key)
         if eng is None:
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
             eng = DenoiseEngine(self.variant, batch, latent_hw, cond_hw, self.diffusion_inference_steps, device,
                                 cuda_graph=self.use_cuda_graph, check_range=False,
                                 step_decode=bool(self.return_intermediates), workspace_pool=pool,
-                                fp8_corr=bool(self.fp8_corrections), backward=bool(backward))
+                                fp8_corr=bool(self.fp8_corrections), backward=bool(backward),
+                                loop_backward=bool(loop_backward))
             if native:
                 eng.enable_producers(feats[0], feats[1], has_neck=self.has_neck)
             if image_hw is not None:
@@ -394,6 +443,14 @@ class DDIMHeadBase(nn.Module):
         keys = DENOISER_KEYS + (FUSE_KEYS if self.variant == "swin" else ())
         return keys, [self.get_submodule(k.rpartition(".")[0]).get_parameter(k.rpartition(".")[2]) for k in keys]
 
+    def _loop_params(self):
+        """The denoiser's then the decoder's parameters: the order of dd_denoise_backward's d_params, d_dec_params."""
+        keys, params = self._denoiser_params()
+        keys = keys + DECODER_PARAM_KEYS
+        params = params + [self.get_submodule(k.rpartition(".")[0]).get_parameter(k.rpartition(".")[2])
+                           for k in DECODER_PARAM_KEYS]
+        return keys, params
+
     def denoiser(self, noisy, t, cond):
         """`self.model(noisy, t, cond, None, None, None)` of the reference, on the engine.  Differentiable (through
         `_DenoiserFunction`, native backward) when grad is enabled and `noisy`, `cond` or a denoiser parameter requires
@@ -437,7 +494,9 @@ class DDIMHeadBase(nn.Module):
 
         Gradients: the condition map comes from the native producers (or the torch producers under no_grad) and carries
         no gradient, so `ddim_loss` trains the denoiser's parameters only.  A caller who trains the producers passes a
-        differentiable `cond` to the operator itself, `self.model(noisy, t, cond)`, whose backward also returns d_cond."""
+        differentiable `cond` to the operator itself, `self.model(noisy, t, cond)`, whose backward also returns d_cond.
+        With `grad_through_loop = True`, `pred` and the final latent are differentiable too (denoiser and decoder
+        parameters, through every step: `_LoopFunction`)."""
         with_backbone = fp is None
         if with_backbone:
             B, dev, dtype = image.shape[0], image.device, torch.float32
@@ -460,8 +519,10 @@ class DDIMHeadBase(nn.Module):
         else:
             cond = None
         x_T = self._draw_noise((B, 16, *latent_hw), dev, dtype, noise)
+        if self.grad_through_loop and self.return_intermediates:
+            raise EngineError("grad_through_loop is not supported by the *Vis heads (pred_inter has no backward)")
         if native:  # (backbone +) neck + FPN + loop + decoder inside the engine; the condition map never leaves NHWC
-            want_cond = self.capture_cond or self.training or self.eval_ddim_loss
+            want_cond = self.capture_cond or self.training or self.eval_ddim_loss or self.grad_through_loop
             if with_backbone:
                 eng = self._engine(B, latent_hw, sizes[0], dev, feats=(list(self.fpn_in_channels), sizes),
                                    image_hw=tuple(image.shape[-2:]), backbone=backbone)
@@ -476,7 +537,17 @@ class DDIMHeadBase(nn.Module):
             eng = self._engine(B, latent_hw, tuple(cond.shape[-2:]), dev)
             loop_cond = cond
         inter = None
-        if self.return_intermediates:  # *Vis heads: inv_t of every intermediate latent, decoded inside the graph
+        loop_keys, loop_params = None, None
+        if self.grad_through_loop and torch.is_grad_enabled():
+            loop_keys, loop_params = self._loop_params()
+            if not (cond.requires_grad or any(p.requires_grad for p in loop_params)):
+                loop_keys = None
+        if loop_keys is not None:  # the same denoise_decode call, as an autograd node (native backward through the loop)
+            box = {}
+            refined_depth, refined_depth_t = _LoopFunction.apply(self, eng, box, loop_cond is None, loop_keys, cond,
+                                                                 x_T, *loop_params)
+            logits = box["logits"]
+        elif self.return_intermediates:  # *Vis heads: inv_t of every intermediate latent, decoded inside the graph
             steps, refined_depth_t, logits = eng.denoise_decode_steps(loop_cond, x_T, want_latent=True,
                                                                       want_logits=self.capture_logits)
             inter = list(steps.unbind(0))

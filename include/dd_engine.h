@@ -26,8 +26,12 @@
  *   dd_denoiser_backward          <- reverse-mode differentiation of that call: the gradients of
  *                                    `ScheduledCNNRefine` (head :336-382 / res.py:301-344) that `ddim_loss`
  *                                    (head :207-223) needs for training
+ *   dd_denoise_backward           <- reverse-mode differentiation of dd_denoise_decode: the training graph of
+ *                                    `pred` and the final latent under the reference's L1 + L2 + DDIM loss
+ *                                    (head :130-146, :165-175, :207-223) through every step and the decoder
  *   dd_decode                     <- `depth_transform.inv_t(latent)` alone (the *Vis heads call it
  *                                    per step, ..._swin_addHAHI_vis.py)
+ *   dd_decode_backward            <- reverse-mode differentiation of `inv_t` (eval BatchNorm)
  *
  * Conventions (inherited from the reference, SURVEY.md §8b): every tensor is fp32, NCHW, contiguous,
  * resident on the engine's CUDA device; no autograd.  Ownership: the caller (PyTorch's allocator)
@@ -76,9 +80,14 @@ enum dd_flags {
   DD_FLAG_FP8_CORR = 1 << 7,    /* correction products of the split as e4m3 MMAs (Blackwell only: Hopper's e4m3 MMA
                                    accumulates at reduced precision, DESIGN.md "Numerics"); the sm_90a build accepts the
                                    flag and runs the exact 3-pass fp16 split everywhere */
-  DD_FLAG_BACKWARD = 1 << 8     /* enable dd_denoiser_backward: dd_finalize_weights also packs the flipped, transposed
+  DD_FLAG_BACKWARD = 1 << 8,    /* enable dd_denoiser_backward: dd_finalize_weights also packs the flipped, transposed
                                    conv weights of the data gradients, and dd_workspace_bytes includes the backward's
                                    region (recomputed activations, gradient buffers; DESIGN.md "Backward") */
+  DD_FLAG_LOOP_BACKWARD = 1 << 9 /* everything DD_FLAG_BACKWARD does, and enable dd_denoise_backward / dd_decode_backward:
+                                   dd_finalize_weights also keeps the decoder's unfolded ConvTranspose weights and
+                                   BatchNorm scale, and the workspace adds the loop backward's region (the T + 1 latents
+                                   [T+1][B,P,16] fp32, fp64 gradient accumulators, the running latent gradient, the
+                                   decoder backward's scratch) */
 };
 
 typedef struct dd_config {
@@ -221,9 +230,35 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
                          float* d_cond_out, float* d_noisy_out, float* const* d_params, void* workspace,
                          size_t workspace_bytes, void* cuda_stream);
 
+/* Backward of dd_denoise_decode (reference CNNDDIMPipiline.__call__ + DeepDepthTransformWithUpsampling.inv_t, head
+ * :254-303 / depth_transform.py:33-35, differentiated in reverse mode through all T denoiser calls, the T DDIM updates
+ * and the decoder; the decoder's BatchNorm uses its running statistics, as the forward does).  Given
+ *   d_depth  [B,1,2h,2w]  dL/d depth         (nullable)
+ *   d_latent [B,16,h,w]   dL/d final latent  (nullable; not both NULL)
+ * for depth, latent = dd_denoise_decode(cond, noise), write (every output nullable)
+ *   d_cond_out [B,256,cond_h,cond_w], d_noise_out [B,16,h,w] (dL/d x_T),
+ *   d_params[i]      the denoiser's 17 / 21 gradients in dd_denoiser_backward's order; time_embedding.weight is dense,
+ *                    non-zero at the rows of the schedule's timesteps,
+ *   d_dec_params[i]  6 decoder gradients: conv_inv_transform.0.weight [16,16,4,4], .0.bias, .1.weight, .1.bias,
+ *                    .3.0.weight [1,16,3,3], .3.0.bias (zero when d_depth is NULL),
+ *   latents_out      [T+1][B,16,h,w]: x_T = noise, then the latent after every step, as the call recomputed them.
+ * The call re-runs the loop un-graphed with the forward's kernels (bit-identical to dd_denoise_decode's), keeping every
+ * latent, then walks back: at each step the recompute + backward chain of dd_denoiser_backward, with per-step gradients
+ * summed in fp64 in step order.  Results are bit-identical run to run; the call does not synchronise.  cond may be NULL
+ * right after dd_build_condition.  Needs DD_FLAG_LOOP_BACKWARD and dd_set_schedule (else DD_ERR_INVALID).
+ * DD_FLAG_CHECK_RANGE and dd_poll_status also report an overflow of the gradient split. */
+int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, const float* d_depth, const float* d_latent,
+                        float* d_cond_out, float* d_noise_out, float* const* d_params, float* const* d_dec_params,
+                        float* latents_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
+
 /* depth = inv_t(latent): latent [B,16,h,w] -> logit_out (nullable), depth_out [B,1,2h,2w]. */
 int dd_decode(dd_handle h, const float* latent, float* logit_out, float* depth_out, void* workspace,
               size_t workspace_bytes, void* cuda_stream);
+
+/* Backward of dd_decode: d_depth [B,1,2h,2w] -> d_latent_out [B,16,h,w] and d_dec_params[0..5] (as in
+ * dd_denoise_backward; the array and every output nullable).  Needs DD_FLAG_LOOP_BACKWARD. */
+int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, float* d_latent_out,
+                       float* const* d_dec_params, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* latent = depth_transform.t(depth) (reference src/model/ops/depth_transform.py:29-31): depth [B,1,height,width] ->
  * latent_out [B,16,ceil(height/2),ceil(width/2)].  Needs the optional keys `depth_transform.conv_transform.*`. */
