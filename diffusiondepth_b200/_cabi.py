@@ -33,6 +33,7 @@ ABI_VERSION = 1
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
 FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD, FLAG_LOOP_BACKWARD = 64, 128, 256, 512
+FLAG_CHAIN_PRED = 1024
 STATUS = {0: "DD_OK", 1: "DD_ERR_INVALID", 2: "DD_ERR_CUDA", 3: "DD_ERR_UNSUPPORTED", 4: "DD_ERR_RANGE"}
 
 # name -> (restype, argtypes); every symbol include/dd_engine.h declares
@@ -75,6 +76,8 @@ SIGNATURES = {
     "dd_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     "dd_bench_conv": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_void_p,
                                 C.c_size_t, C.c_void_p]),
+    "dd_bench_pred_fold": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float), C.c_void_p, C.c_size_t,
+                                     C.c_void_p]),
 }
 
 

@@ -17,6 +17,7 @@
 #include "kernels.cuh"
 #include "convgen.cuh"
 #include "conv_halo.cuh"
+#include "pred_fold.cuh"
 #include "swin.cuh"
 #include "mpvit.cuh"
 #include "backward.cuh"
@@ -96,6 +97,20 @@ int make_strip_map(CUtensorMap* m, const __half* base, int B, int H, int W, int 
                         CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(strip) failed: " + std::to_string((int)r));
+  return DD_OK;
+}
+// halo patch of conv5x5_fold_kernel: the NHWC [B][H][W][256] fp16 plane seen as {8 ch, y, x, channel group, image};
+// box = {8, 20, 36, 2, 1} lands in shared memory as [channel group][x][y][8 ch], no swizzle
+int make_patch_map(CUtensorMap* m, const __half* base, int B, int H, int W) {
+  const cuuint64_t px = 256 * 2;  // bytes per pixel
+  cuuint64_t gdim[5] = {8, (cuuint64_t)H, (cuuint64_t)W, 32, (cuuint64_t)B};
+  cuuint64_t gstr[4] = {(cuuint64_t)W * px, px, 16, (cuuint64_t)H * W * px};
+  cuuint32_t box[5] = {8, dd::F5::PH, dd::F5::PW, 2, 1};
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<__half*>(base), gdim, gstr, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(patch) failed: " + std::to_string((int)r));
   return DD_OK;
 }
 // weights: [9][COUT][CIN] fp16; box = {bk, COUT, 1}
@@ -189,6 +204,10 @@ cudaError_t configure_all_kernels() {
   if ((e = configure_halo_all_epi<256, 256, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<256, 64, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<64, 16, 32>()) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::conv5x5_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                dd::F5::SMEM_BYTES)) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::ring_fix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::RING_SMEM)) !=
+      cudaSuccess) return e;
   if ((e = configure_wgm<128, 128>()) != cudaSuccess) return e;
   if ((e = configure_wgm<128, 64>()) != cudaSuccess) return e;
   if ((e = configure_wgm<64, 128>()) != cudaSuccess) return e;
@@ -346,6 +365,11 @@ struct dd_engine {
   // packed parameters (device memory owned by the engine)
   ConvLayer L[12];  // 0 ne.0, 1 ne.3, 2 convA, 3 convB, 4 pred.0, 5 pred.3; 6 + i: the data-gradient conv of layer i
                     // (flipped, transposed weights, zero bias; DD_FLAG_BACKWARD only)
+  struct Fold {  // convB -> pred.0 composed into one 5x5 conv (Swin, unless DD_FLAG_CHAIN_PRED / DD_FLAG_SIMT_CONV)
+    __half* w = nullptr;     // packed K5 hi / lo (pred_fold.cuh)
+    float* bias = nullptr;   // b5 [64]
+    float wscale = 1.f;
+  } fold;
   float* gn_gamma[4] = {nullptr, nullptr, nullptr, nullptr};  // ne.1, ne.4, pred.1, pred.4
   float* gn_beta[4] = {nullptr, nullptr, nullptr, nullptr};
   float* temb = nullptr;    // [1280][256]
@@ -787,10 +811,11 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
   return DD_OK;
 }
 
-int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st) {
+int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st, const float* ring = nullptr, int ring_per_img = 0) {
   const Geom g = geom_of(e->cfg);
   const double inv = 1.0 / (static_cast<double>(g.P) * (channels / 4));
-  dd::gn_finalize_kernel<<<g.B * 4, 256, 0, st>>>(e->stats[which], e->stats_tiles_img[which], inv, 1e-5f, e->mr[which]);
+  dd::gn_finalize_kernel<<<g.B * 4, 256, 0, st>>>(e->stats[which], e->stats_tiles_img[which], ring, ring_per_img, inv,
+                                                   1e-5f, e->mr[which]);
   e->launches++;
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("gn_finalize: ") + cudaGetErrorString(err));
@@ -844,6 +869,63 @@ int run_apply(dd_engine* e, int which, const float* temb, int temb_bstride, __ha
   return DD_OK;
 }
 
+bool fold_active(const dd_engine* e) {
+  return e->cfg.variant == DD_VARIANT_SWIN && !(e->cfg.flags & (DD_FLAG_SIMT_CONV | DD_FLAG_CHAIN_PRED));
+}
+// Ring partials of the composed pred.0 conv: segments spread over at most as many blocks per image as stats[3] has
+// tile slots (stats[3] is free until pred.3 runs).
+int ring_blocks_per_img(const Geom& g) {
+  return std::min(dd::ring_segments(g.h, g.w), g.tiles_max / g.B);
+}
+
+// convB -> pred.0 as the composed 5x5 conv on convA's split output (S_hi[0] / S_lo[0]) + the ring correction: Y and the
+// pred.0 GroupNorm partials (tiles in stats[2], ring in stats[3]) as the two-conv chain would leave them.
+int run_fold(dd_engine* e, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  int rc;
+  CUtensorMap m_hi, m_lo;
+  if ((rc = make_patch_map(&m_hi, e->S_hi[0], g.B, g.h, g.w))) return rc;
+  if ((rc = make_patch_map(&m_lo, e->S_lo[0], g.B, g.h, g.w))) return rc;
+  dd::FoldArgs a;
+  a.B = g.B;
+  a.H = g.h;
+  a.W = g.w;
+  a.tiles_x = (g.w + dd::F5_TW - 1) / dd::F5_TW;
+  a.tiles_y = (g.h + dd::F5_TH - 1) / dd::F5_TH;
+  a.num_tiles = a.tiles_x * a.tiles_y * g.B;
+  a.w = e->fold.w;
+  a.bias = e->fold.bias;
+  a.acc_scale = 1.f / (kActScale * e->fold.wscale);
+  a.y32 = e->Y;
+  a.stats_partial = e->stats[2];
+  e->stats_tiles_img[2] = a.tiles_x * a.tiles_y;
+  const int grid = std::min(a.num_tiles, e->sm_count);
+  dd::conv5x5_fold_kernel<<<grid, dd::F5::THREADS, dd::F5::SMEM_BYTES, st>>>(m_hi, m_lo, a);
+  e->launches++;
+  cudaError_t err = cudaGetLastError();
+  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv5x5_fold: ") + cudaGetErrorString(err));
+  dd::RingArgs r;
+  r.H = g.h;
+  r.W = g.w;
+  r.nseg = dd::ring_segments(g.h, g.w);
+  r.blocks_per_img = ring_blocks_per_img(g);
+  r.a_hi = e->S_hi[0];
+  r.a_lo = e->S_lo[0];
+  r.a_inv_scale = 1.f / kActScale;
+  r.wb = e->L[3].w_simt;
+  r.bb = e->L[3].bias;
+  r.wp = e->L[4].w_simt;
+  r.y32 = e->Y;
+  r.ring_partial = e->stats[3];
+  dd::ring_fix_kernel<<<dim3(r.blocks_per_img, g.B), 256, dd::RING_SMEM, st>>>(r);
+  e->launches++;
+  err = cudaGetLastError();
+  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("ring_fix: ") + cudaGetErrorString(err));
+  return DD_OK;
+}
+
+int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st);
+
 // One ScheduledCNNRefine.forward + (optionally) the DDIM update.
 int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float ce, float* eps_out, cudaStream_t st) {
   const Geom g = geom_of(e->cfg);
@@ -867,6 +949,11 @@ int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float 
     if ((rc = run_apply<256, 2>(e, 1, temb, temb_bstride, e->S_hi[1], e->S_lo[1], st, f8))) return rc;
     if ((rc = run_conv(e, 2, e->S_hi[1], e->S_lo[1], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[0], e->S_lo[0], st,
                        f8 ? (kF8In | kF8Out) : 0))) return rc;
+    if (fold_active(e)) {  // convB + pred.0 as one composed conv + its ring correction
+      if ((rc = run_fold(e, st))) return rc;
+      if ((rc = run_finalize(e, 2, 64, st, e->stats[3], ring_blocks_per_img(g)))) return rc;
+      return run_tail(e, cx, ce, eps_out, st);
+    }
     if ((rc = run_conv(e, 3, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[1], e->S_lo[1], st,
                        f8 ? kF8In : 0))) return rc;
     p_hi = e->S_hi[1];
@@ -879,6 +966,13 @@ int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float 
   // pred.0 : 256 -> 64, GN stats
   if ((rc = run_conv(e, 4, p_hi, p_lo, kActScale, dd::EPI_F32_STATS, e->Y, e->stats[2], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 2, 64, st))) return rc;
+  return run_tail(e, cx, ce, eps_out, st);
+}
+
+// pred.0's GroupNorm + ReLU, pred.3 and its GroupNorm + ReLU, and the DDIM update (Y holds pred.0's output).
+int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  int rc;
   if ((rc = run_apply<64, 0>(e, 2, nullptr, 0, e->S_hi[0], e->S_lo[0], st))) return rc;
   // pred.3 : 64 -> 16, GN stats
   if ((rc = run_conv(e, 5, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_F32_STATS, e->Y, e->stats[3], nullptr, nullptr, st))) return rc;
@@ -1925,6 +2019,32 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
     if ((rc = pack_layer(h, h->L[3], W("model.upsample_fuse.convB.conv.weight"), W("model.upsample_fuse.convB.conv.bias"), 256, 256, st, scratch))) return rc;
   }
   if ((rc = pack_layer(h, h->L[4], W("model.pred.0.weight"), W("model.pred.0.bias"), 64, 256, st, scratch))) return rc;
+  if (fold_active(h)) {
+    // K5 / b5 in fp64, then one fp16 hi / lo split with a power-of-two scale as in pack_layer
+    const size_t n5 = 64 * 256 * 25;
+    double* k5 = nullptr;
+    float* k5_abs = nullptr;
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&k5), n5 * 8));
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&k5_abs), n5 * 4));
+    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->fold.w), dd::F5::W_ELEMS * 2))) return rc;
+    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->fold.bias), 64 * 4))) return rc;
+    dd::compose_fold_kernel<<<256, 256, 0, st>>>(W("model.pred.0.weight"), W("model.pred.0.bias"),
+                                                 W("model.upsample_fuse.convB.conv.weight"),
+                                                 W("model.upsample_fuse.convB.conv.bias"), k5, k5_abs, h->fold.bias);
+    CUDA_TRY(cudaMemsetAsync(scratch, 0, 4, st));
+    dd::absmax_kernel<<<absmax_grid(n5), 256, 0, st>>>(k5_abs, static_cast<int>(n5), scratch);
+    float amax = 0.f;
+    CUDA_TRY(cudaMemcpyAsync(&amax, scratch, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    float scale = 1.f;
+    if (amax > 0.f && isfinite(amax)) scale = exp2f(floorf(log2f(32768.f / amax)) - 1.f);
+    h->fold.wscale = scale;
+    dd::pack_fold_kernel<<<256, 256, 0, st>>>(k5, h->fold.w, static_cast<double>(scale));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
+    cudaFree(k5);
+    cudaFree(k5_abs);
+  }
   if ((rc = pack_layer(h, h->L[5], W("model.pred.3.weight"), W("model.pred.3.bias"), 16, 64, st, scratch))) return rc;
   if (has_backward(h->cfg)) {
     // data-gradient convs: W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] with zero bias, packed like any forward layer
@@ -2799,6 +2919,34 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   }
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(err));
   return transpose_out(yn, y, batch, cout, height * width, st);
+}
+
+int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,
+                       void* cuda_stream) {
+  if (!h || !ms_out || iters < 1) return fail(DD_ERR_INVALID, "bad argument");
+  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  if (!fold_active(h)) return fail(DD_ERR_UNSUPPORTED, "this engine runs convB and pred.0 as two convs");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  int rc;
+  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  cudaEvent_t e0, e1;
+  CUDA_TRY(cudaEventCreate(&e0));
+  CUDA_TRY(cudaEventCreate(&e1));
+  // whatever the planes currently hold is fine for timing: MMA time is data independent
+  for (int w = 0; w < 2; ++w)
+    if ((rc = run_fold(h, st))) return rc;
+  CUDA_TRY(cudaEventRecord(e0, st));
+  for (int i = 0; i < iters; ++i)
+    if ((rc = run_fold(h, st))) return rc;
+  CUDA_TRY(cudaEventRecord(e1, st));
+  CUDA_TRY(cudaEventSynchronize(e1));
+  float ms = 0.f;
+  CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  *ms_out = ms / iters;
+  return DD_OK;
 }
 
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,

@@ -152,14 +152,17 @@ __global__ void absmax_kernel(const float* __restrict__ w, int n, float* __restr
 }
 
 // ------------------------------------------------------------------ GroupNorm(4, C) finalize
-// partial [tiles_total][4][2] (fp32 sums over one 128-pixel tile) -> mean/rstd per (image, group).
+// partial [tiles_total][4][2] (fp32 sums over one conv tile) and, optionally, ring [B][ring_per_img][4][2] (the
+// border pixels the composed pred.0 conv leaves to ring_fix_kernel) -> mean/rstd per (image, group).
 // Combined in fp64 in a fixed order (deterministic; SURVEY.md §7.2-4).
-__global__ void gn_finalize_kernel(const float* __restrict__ partial, int tiles_per_img, double inv_count, float eps,
+__global__ void gn_finalize_kernel(const float* __restrict__ partial, int tiles_per_img, const float* __restrict__ ring,
+                                   int ring_per_img, double inv_count, float eps,
                                    float* __restrict__ mean_rstd /* [B][4][2] */) {
   const int b = blockIdx.x >> 2, g = blockIdx.x & 3;
   double s = 0.0, s2 = 0.0;
-  for (int t = threadIdx.x; t < tiles_per_img; t += blockDim.x) {
-    const float* q = partial + (static_cast<size_t>(b) * tiles_per_img + t) * 8 + g * 2;
+  for (int t = threadIdx.x; t < tiles_per_img + ring_per_img; t += blockDim.x) {
+    const float* q = (t < tiles_per_img ? partial + (static_cast<size_t>(b) * tiles_per_img + t) * 8
+                                        : ring + (static_cast<size_t>(b) * ring_per_img + t - tiles_per_img) * 8) + g * 2;
     s += static_cast<double>(q[0]);
     s2 += static_cast<double>(q[1]);
   }

@@ -90,7 +90,8 @@ class DenoiseEngine:
                  num_inference_steps: int, device: torch.device, cuda_graph: bool = True,
                  simt_conv: bool = False, check_range: bool = False, halo_conv: bool = True,
                  swap_narrow: bool = True, pair_wide: bool = True, step_decode: bool = False, workspace_pool=None,
-                 fp8_corr: bool = True, backward: bool = False, loop_backward: bool = False):
+                 fp8_corr: bool = True, backward: bool = False, loop_backward: bool = False,
+                 chain_pred: bool = False):
         self.lib = _cabi.load_library()
         device = torch.device(device)
         if device.type != "cuda":
@@ -103,7 +104,8 @@ class DenoiseEngine:
                 (_cabi.FLAG_CHECK_RANGE if check_range else 0) | (_cabi.FLAG_HALO_CONV if halo_conv else 0) | \
                 (_cabi.FLAG_SWAP_NARROW if swap_narrow else 0) | (_cabi.FLAG_PAIR_WIDE if pair_wide else 0) | \
                 (_cabi.FLAG_STEP_DECODE if step_decode else 0) | (_cabi.FLAG_FP8_CORR if fp8_corr else 0) | \
-                (_cabi.FLAG_BACKWARD if backward else 0) | (_cabi.FLAG_LOOP_BACKWARD if loop_backward else 0)
+                (_cabi.FLAG_BACKWARD if backward else 0) | (_cabi.FLAG_LOOP_BACKWARD if loop_backward else 0) | \
+                (_cabi.FLAG_CHAIN_PRED if chain_pred else 0)
         self.fp8_corr = bool(fp8_corr)
         self.backward = bool(backward or loop_backward)  # the loop backward includes the operator's
         self.loop_backward = bool(loop_backward)
@@ -411,6 +413,14 @@ class DenoiseEngine:
         ws = self._workspace()
         _cabi.check(self.lib.dd_bench_conv(self._h, cin, cout, iters, C.byref(ms), C.c_void_p(self._aligned(ws)),
                                            ws.numel() - 1024, C.c_void_p(self._stream())))
+        return float(ms.value)
+
+    def bench_pred_fold(self, iters: int = 20) -> float:
+        """Average milliseconds of the Swin step's composed convB -> pred.0 (5x5 conv + ring correction)."""
+        ms = C.c_float()
+        ws = self._workspace()
+        _cabi.check(self.lib.dd_bench_pred_fold(self._h, iters, C.byref(ms), C.c_void_p(self._aligned(ws)),
+                                                ws.numel() - 1024, C.c_void_p(self._stream())))
         return float(ms.value)
 
     def bench_gemm(self, M: int, K: int, N: int, mode: int = 0, iters: int = 20) -> float:

@@ -83,11 +83,13 @@ enum dd_flags {
   DD_FLAG_BACKWARD = 1 << 8,    /* enable dd_denoiser_backward: dd_finalize_weights also packs the flipped, transposed
                                    conv weights of the data gradients, and dd_workspace_bytes includes the backward's
                                    region (recomputed activations, gradient buffers; DESIGN.md "Backward") */
-  DD_FLAG_LOOP_BACKWARD = 1 << 9 /* everything DD_FLAG_BACKWARD does, and enable dd_denoise_backward / dd_decode_backward:
+  DD_FLAG_LOOP_BACKWARD = 1 << 9, /* everything DD_FLAG_BACKWARD does, and enable dd_denoise_backward / dd_decode_backward:
                                    dd_finalize_weights also keeps the decoder's unfolded ConvTranspose weights and
                                    BatchNorm scale, and the workspace adds the loop backward's region (the T + 1 latents
                                    [T+1][B,P,16] fp32, fp64 gradient accumulators, the running latent gradient, the
                                    decoder backward's scratch) */
+  DD_FLAG_CHAIN_PRED = 1 << 10  /* Swin: run convB and pred.0 as two 3x3 convs instead of one composed 5x5 conv + its
+                                   border correction (A/B runs and tests; DD_FLAG_SIMT_CONV always runs the chain) */
 };
 
 typedef struct dd_config {
@@ -285,6 +287,11 @@ size_t dd_conv3x3_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int3
  * CUDA events on `cuda_stream`; returns average milliseconds per launch in *ms_out. */
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,
                   size_t workspace_bytes, void* cuda_stream);
+
+/* Time the Swin step's composed convB -> pred.0 (the 5x5 conv + its ring correction, two launches) `iters` times with
+ * CUDA events; average milliseconds per pair in *ms_out.  DD_ERR_UNSUPPORTED when the engine runs the chain. */
+int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,
+                       void* cuda_stream);
 
 /* Tuning aid: average milliseconds per launch of the GEMM-mode kernel (tokens [M,K] x weights [N,K]^T) on
  * synthetic operands.  mode 0: fp32 out, 1: fp32 out + residual add, 2: GELU -> fp16 planes, 3: no output. */

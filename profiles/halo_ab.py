@@ -8,6 +8,8 @@ Every loop conv shape is timed with DenoiseEngine.bench_conv (CUDA events around
 the C3 latent grid: B = 4, 176 x 608.  Each library runs in its own process (the library is chosen when the package
 loads it, through DD_ENGINE_LIB), and the libraries alternate for `--rounds` rounds so that clock and load drift hit
 both alike.  Rates are algorithmic: 2 * pixels * COUT * 9 * CIN FLOPs per launch (the 3-pass split issues 3x that).
+The Swin step runs convB + pred.0 as one composed 5x5 conv + its ring correction (DenoiseEngine.bench_pred_fold,
+row "fold", rate counted as 2 * pixels * 64 * 25 * 256 FLOPs); 256->256 is convA, 256->64 the chain's pred.0.
 
 The profile mode runs the full C3 forward (Swin-L, T = 20) once with the profiler on, without CUDA graphs so that
 every kernel is recorded, and groups device time by kernel name.  It is a breakdown, not a timing: take times from
@@ -22,7 +24,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SHAPES = [(16, 64), (64, 256), (256, 256), (256, 64), (64, 16)]  # the loop's conv shapes (CIN, COUT)
 B, LH, LW = 4, 176, 608  # C3 latent grid: 352 x 1216 at half resolution
-PER_STEP = {(16, 64): 1, (64, 256): 1, (256, 256): 2, (256, 64): 1, (64, 16): 1}  # launches per DDIM step
+PER_STEP = {(16, 64): 1, (64, 256): 1, (256, 256): 1, (256, 64): 0, (64, 16): 1}  # launches per DDIM step (+ fold)
 
 
 def worker(iters, warmup):
@@ -43,6 +45,8 @@ def worker(iters, warmup):
     for cin, cout in SHAPES:
         eng.bench_conv(cin, cout, warmup)
         res["ms"][f"{cin}->{cout}"] = eng.bench_conv(cin, cout, iters)
+    eng.bench_pred_fold(warmup)
+    res["ms"]["fold"] = eng.bench_pred_fold(iters)
     print(json.dumps(res), flush=True)
 
 
@@ -70,7 +74,14 @@ def ab(libs, rounds, iters, warmup):
             summary.setdefault(key, {})[name] = {"ms": ms, "tflops_best": tflops(cin, cout, best)}
             cells.append(f"{' '.join(f'{m:.3f}' for m in ms):>28} {tflops(cin, cout, best):9.1f}")
         print(f"{key:>9} " + " ".join(cells))
-    per_step = {name: sum(PER_STEP[(ci, co)] * min(summary[f"{ci}->{co}"][name]["ms"]) for ci, co in SHAPES)
+    cells = []
+    for name, _ in libs:
+        ms = [r["ms"]["fold"] for r in runs[name]]
+        summary.setdefault("fold", {})[name] = {"ms": ms, "tflops_best": tflops(256, 64, min(ms)) * 25 / 9}
+        cells.append(f"{' '.join(f'{m:.3f}' for m in ms):>28} {tflops(256, 64, min(ms)) * 25 / 9:9.1f}")
+    print(f"{'fold':>9} " + " ".join(cells))
+    per_step = {name: min(summary["fold"][name]["ms"]) +
+                sum(PER_STEP[(ci, co)] * min(summary[f"{ci}->{co}"][name]["ms"]) for ci, co in SHAPES)
                 for name, _ in libs}
     print("loop conv ms per DDIM step (best runs): " + ", ".join(f"{n} {v:.2f}" for n, v in per_step.items()))
     print(json.dumps({"gpu": runs[libs[0][0]][0]["gpu"], "grid": [B, LH, LW], "iters": iters, "summary": summary,
