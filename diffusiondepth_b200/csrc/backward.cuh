@@ -329,7 +329,11 @@ __global__ void __launch_bounds__(TM * TN / 16) wgrad_simt_kernel(const WgradArg
 // + dY_hi X_lo.  Warp 0 of warpgroup 0 produces into a STAGES-deep ring; MCO / 64 consumer warpgroups each own 64 output
 // channels x NCI input channels.  A CTA sums `segs` segments (split K) and writes its fp32 tile as an fp64 partial
 // [chunk][tap][cout][cin]; wgrad_reduce_kernel adds the chunks in order.
+// A tensor-core accumulator loses a little at every wgmma that adds into it: one accumulator over a CTA's 128 segments
+// (1,536 wgmmas) was 3.0-3.4e-5 of max |dW| from fp64 on an H100.  So the wgmma accumulator only ever holds WGM_FLUSH
+// segments; it is then added into a second, ordinary fp32 register accumulator and cleared.
 constexpr int WGM_STAGES = 3;
+constexpr int WGM_FLUSH = 4;
 template <int MCO, int NCI>
 struct WgmCfg {
   static constexpr int NCWG = MCO / 64;
@@ -372,7 +376,10 @@ __global__ void __launch_bounds__(WgmCfg<MCO, NCI>::THREADS, 1)
     fence_barrier_init();
   }
   __syncthreads();
+  // setmaxnreg at the top of each role's branch, branches meeting only at the exit (see conv3x3_halo_kernel): the two
+  // consumer warpgroups' 2 x NCI / 2 accumulators do not fit the 168-register launch bound of a 384-thread CTA
   if (wg == 0) {
+    if constexpr (Cfg::NCWG > 1) setmaxnreg_dec<40>();
     if (threadIdx.x < 32) {
       const bool leader = elect_one();
       for (int s = s_begin, it = 0; s < s_end; ++s, ++it) {
@@ -399,9 +406,10 @@ __global__ void __launch_bounds__(WgmCfg<MCO, NCI>::THREADS, 1)
       }
     }
   } else {
-    float d[NCI / 2];
+    if constexpr (Cfg::NCWG > 1) setmaxnreg_inc<232>();
+    float d[NCI / 2], acc[NCI / 2];  // d: the wgmma accumulator of the current WGM_FLUSH segments; acc: their fp32 sum
 #pragma unroll
-    for (int i = 0; i < NCI / 2; ++i) d[i] = 0.f;
+    for (int i = 0; i < NCI / 2; ++i) d[i] = acc[i] = 0.f;
     const int cw = wg - 1;  // this warpgroup's 64 output channels
     for (int s = s_begin, it = 0; s < s_end; ++s, ++it) {
       const int st = it % WGM_STAGES;
@@ -422,8 +430,15 @@ __global__ void __launch_bounds__(WgmCfg<MCO, NCI>::THREADS, 1)
       wgmma_wait<0>();
       wgmma_fence_regs(d);
       mbar_arrive(&empty[st]);
+      if ((it + 1) % WGM_FLUSH == 0 || s + 1 == s_end) {
+#pragma unroll
+        for (int i = 0; i < NCI / 2; ++i) {
+          acc[i] += d[i];
+          d[i] = 0.f;
+        }
+      }
     }
-    // d[4 i + e] = D[16 (t / 32) + (t % 32) / 4 + 8 (e / 2)][8 i + 2 (t % 4) + (e % 2)]
+    // acc[4 i + e] (d's layout) = D[16 (t / 32) + (t % 32) / 4 + 8 (e / 2)][8 i + 2 (t % 4) + (e % 2)]
     const int t = threadIdx.x & 127;
     double* out = a.partial + (static_cast<size_t>(blockIdx.x) * 9 + tap) * a.cout * a.cin;
 #pragma unroll
@@ -432,7 +447,7 @@ __global__ void __launch_bounds__(WgmCfg<MCO, NCI>::THREADS, 1)
       for (int e = 0; e < 4; ++e) {
         const int co = co0 + 64 * cw + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * (e >> 1);
         const int ci = ci0 + 8 * i + 2 * (t & 3) + (e & 1);
-        out[static_cast<size_t>(co) * a.cin + ci] = static_cast<double>(d[4 * i + e]);
+        out[static_cast<size_t>(co) * a.cin + ci] = static_cast<double>(acc[4 * i + e]);
       }
   }
 }

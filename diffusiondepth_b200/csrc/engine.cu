@@ -487,13 +487,19 @@ WgPlan wgrad_plan(int cout, int cin, long long BP) {
   return {static_cast<int>(chunks), static_cast<int>(chunk)};
 }
 int bwd_chunks(int P) { return (P + dd::BWD_CHUNK - 1) / dd::BWD_CHUNK; }
-// Layers whose weight gradient runs on wgrad_wgmma_kernel: the four 256-wide ones.  The two 16-channel layers keep
+// Shapes whose weight gradient runs on wgrad_wgmma_kernel: the 256-wide ones.  The two 16-channel shapes keep
 // wgrad_simt_kernel (3.6 of 192 ms of a backward call at B = 4, 176 x 608).
-bool wgrad_on_tc(int layer) { return layer >= 1 && layer <= 4; }
+bool wgrad_on_tc(int cout, int cin) { return cout == 256 || cin == 256; }
 constexpr int kWgmSegs = 128;  // 64-pixel row segments per CTA of wgrad_wgmma_kernel (8192 pixels summed in fp32)
-int wgm_chunks(const Geom& g) {
-  const int nseg = g.B * g.h * ((g.w + 63) / 64);
+int wgm_chunks(int B, int H, int W) {
+  const int nseg = B * H * ((W + 63) / 64);
   return (nseg + kWgmSegs - 1) / kWgmSegs;
+}
+// fp64 partials run_wgrad writes for one (cout, cin) conv at B x H x W
+size_t wgrad_partial_elems(int cout, int cin, int B, int H, int W) {
+  const int chunks = wgrad_on_tc(cout, cin) ? wgm_chunks(B, H, W)
+                                            : wgrad_plan(cout, cin, static_cast<long long>(B) * H * W).chunks;
+  return static_cast<size_t>(chunks) * cout * cin * 9;
 }
 // DD_FLAG_LOOP_BACKWARD implies DD_FLAG_BACKWARD
 bool has_backward(const dd_config& c) { return (c.flags & (DD_FLAG_BACKWARD | DD_FLAG_LOOP_BACKWARD)) != 0; }
@@ -690,10 +696,7 @@ size_t carve(dd_engine* e, void* base) {
     bv->scales = c.take<float>(kBwdSlots);
     bv->amax = c.take<float>(kBwdSlots);
     size_t wg = 0;
-    for (int i = 0; i < 6; ++i) {
-      const int chunks = wgrad_on_tc(i) ? wgm_chunks(g) : wgrad_plan(kConvCout[i], kConvCin[i], static_cast<long long>(BP)).chunks;
-      wg = std::max(wg, static_cast<size_t>(chunks) * kConvCout[i] * kConvCin[i] * 9);
-    }
+    for (int i = 0; i < 6; ++i) wg = std::max(wg, wgrad_partial_elems(kConvCout[i], kConvCin[i], g.B, g.h, g.w));
     bv->wg_part = c.take<double>(wg);
   }
   if (e->cfg.flags & DD_FLAG_LOOP_BACKWARD) {
@@ -1664,20 +1667,21 @@ int run_gn_bwd(dd_engine* e, int which, const float* dout, const float* dscale, 
   return launched(e, "gn_bwd_apply");
 }
 
-// column sums of x [B][P][C] (times *scale): per image (out_img [B][C]) and / or over the batch in image order (out_sum [C])
-int run_colsum(dd_engine* e, int C, const float* x, const float* scale, int P, float* out_img, float* out_sum,
-               cudaStream_t st) {
-  const int B = e->cfg.batch, chunks = bwd_chunks(P);
+// column sums of x [B][P][C] (times *scale): per image (out_img [B][C]) and / or over the batch in image order (out_sum
+// [C]); partial holds B * bwd_chunks(P) * C floats
+int run_colsum(dd_engine* e, int C, const float* x, const float* scale, int B, int P, float* partial, float* out_img,
+               float* out_sum, cudaStream_t st) {
+  const int chunks = bwd_chunks(P);
   const dim3 grid(chunks, B);
   switch (C) {
-    case 16: dd::colsum_partial_kernel<16><<<grid, 256, 0, st>>>(x, scale, P, chunks, e->bw.col_part); break;
-    case 64: dd::colsum_partial_kernel<64><<<grid, 256, 0, st>>>(x, scale, P, chunks, e->bw.col_part); break;
-    case 256: dd::colsum_partial_kernel<256><<<grid, 256, 0, st>>>(x, scale, P, chunks, e->bw.col_part); break;
+    case 16: dd::colsum_partial_kernel<16><<<grid, 256, 0, st>>>(x, scale, P, chunks, partial); break;
+    case 64: dd::colsum_partial_kernel<64><<<grid, 256, 0, st>>>(x, scale, P, chunks, partial); break;
+    case 256: dd::colsum_partial_kernel<256><<<grid, 256, 0, st>>>(x, scale, P, chunks, partial); break;
     default: return fail(DD_ERR_INVALID, "colsum: unsupported channel count");
   }
   int rc;
   if ((rc = launched(e, "colsum_partial"))) return rc;
-  dd::colsum_finalize_kernel<<<C, 32, 0, st>>>(e->bw.col_part, B, chunks, C, out_img, out_sum);
+  dd::colsum_finalize_kernel<<<C, 32, 0, st>>>(partial, B, chunks, C, out_img, out_sum);
   return launched(e, "colsum_finalize");
 }
 
@@ -1688,42 +1692,52 @@ cudaError_t launch_wgrad(const dd::WgradArgs& a, int chunks, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-// Backward of conv layer `layer` given dy [B][P][Cout] (times *dscale, nullable = 1) and the conv's input planes X (scale
-// x_scale): dw [Cout][Cin][3][3] and db [Cout] (each nullable), and dx (nullable) = conv3x3(dy, W') on the forward's
-// tensor-core kernel, left multiplied by bw.scales[slot].
-int run_conv_bwd(dd_engine* e, int layer, const float* dy, const float* dscale, const __half* x_hi, const __half* x_lo,
-                 float x_scale, float* dw, float* db, float* dx, int slot, cudaStream_t st) {
-  const Geom g = geom_of(e->cfg);
-  const int cout = kConvCout[layer], cin = kConvCin[layer];
-  const size_t BP = static_cast<size_t>(g.B) * g.P;
+// Buffers of run_wgrad: the dY split planes [B*H*W][cout] fp16, the split's absmax (zeroed before the call) and scale
+// (written), the status word a non-finite dY sets, and wgrad_partial_elems fp64 partials.
+struct WgradBufs {
+  Planes gp;
+  float* amax;
+  float* scale;
+  int* status;
+  double* partial;
+};
+
+// Weight gradient of one 3x3 conv at B x H x W: dw [cout][cin][3][3] (nullable) = sum over pixels of dY (x) X, dY
+// [B*H*W][cout] times *dscale (nullable = 1), X the conv's fp16 hi/lo input planes at scale x_scale.  dY is split into
+// bufs.gp with an on-device power-of-two scale when the tensor cores read it (the 256-wide shapes) or when `split` asks
+// for the planes anyway (the data-gradient conv reads them); *bufs.scale = *dscale times that scale.
+int run_wgrad(dd_engine* e, int B, int H, int W, int cout, int cin, const float* dy, const float* dscale,
+              const __half* x_hi, const __half* x_lo, float x_scale, float* dw, bool split, const WgradBufs& bufs,
+              cudaStream_t st) {
+  const size_t BP = static_cast<size_t>(B) * H * W;
+  const size_t nw = static_cast<size_t>(cout) * cin * 9;
+  const bool tc = dw != nullptr && wgrad_on_tc(cout, cin);
   int rc;
-  if (db != nullptr && (rc = run_colsum(e, cout, dy, dscale, g.P, nullptr, db, st))) return rc;
-  const bool tc = dw != nullptr && wgrad_on_tc(layer);
-  if (dx != nullptr || tc) {  // split dY: the data-gradient conv and the tensor-core weight gradient read these planes
+  if (split || tc) {
     const size_t n = BP * cout;
-    dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(dy, static_cast<int>(n), e->bw.amax + slot);
+    dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(dy, static_cast<int>(n), bufs.amax);
     if ((rc = launched(e, "grad absmax"))) return rc;
-    dd::grad_split_kernel<<<grid_of(n / 4), 256, 0, st>>>(dy, e->bw.gp.hi, e->bw.gp.lo, n / 4, e->bw.amax + slot, dscale,
-                                                          e->bw.scales + slot, e->status);
+    dd::grad_split_kernel<<<grid_of(n / 4), 256, 0, st>>>(dy, bufs.gp.hi, bufs.gp.lo, n / 4, bufs.amax, dscale,
+                                                          bufs.scale, bufs.status);
     if ((rc = launched(e, "grad_split"))) return rc;
   }
   if (tc) {
     CUtensorMap ah, al, bh, bl;
-    if ((rc = make_wgm_map(&ah, e->bw.gp.hi, g.B, g.h, g.w, cout))) return rc;
-    if ((rc = make_wgm_map(&al, e->bw.gp.lo, g.B, g.h, g.w, cout))) return rc;
-    if ((rc = make_wgm_map(&bh, x_hi, g.B, g.h, g.w, cin))) return rc;
-    if ((rc = make_wgm_map(&bl, x_lo, g.B, g.h, g.w, cin))) return rc;
+    if ((rc = make_wgm_map(&ah, bufs.gp.hi, B, H, W, cout))) return rc;
+    if ((rc = make_wgm_map(&al, bufs.gp.lo, B, H, W, cout))) return rc;
+    if ((rc = make_wgm_map(&bh, x_hi, B, H, W, cin))) return rc;
+    if ((rc = make_wgm_map(&bl, x_lo, B, H, W, cin))) return rc;
     dd::WgmArgs a;
     a.cout = cout;
     a.cin = cin;
-    a.B = g.B;
-    a.H = g.h;
-    a.W = g.w;
-    a.xsegs = (g.w + 63) / 64;
-    a.nseg = g.B * g.h * a.xsegs;
+    a.B = B;
+    a.H = H;
+    a.W = W;
+    a.xsegs = (W + 63) / 64;
+    a.nseg = B * H * a.xsegs;
     a.segs = kWgmSegs;
-    a.partial = e->bw.wg_part;
-    const int chunks = wgm_chunks(g);
+    a.partial = bufs.partial;
+    const int chunks = wgm_chunks(B, H, W);
     if (cout == 256 && cin == 256) {
       using Cf = dd::WgmCfg<128, 128>;
       dd::wgrad_wgmma_kernel<128, 128><<<dim3(chunks, 2 * 2 * 9), Cf::THREADS, Cf::SMEM_BYTES, st>>>(ah, al, bh, bl, a);
@@ -1735,32 +1749,43 @@ int run_conv_bwd(dd_engine* e, int layer, const float* dy, const float* dscale, 
       dd::wgrad_wgmma_kernel<64, 128><<<dim3(chunks, 2 * 9), Cf::THREADS, Cf::SMEM_BYTES, st>>>(ah, al, bh, bl, a);
     }
     if ((rc = launched(e, "wgrad_wgmma"))) return rc;
-    const size_t n = static_cast<size_t>(cout) * cin * 9;
-    dd::wgrad_reduce_kernel<<<grid_of(n), 256, 0, st>>>(e->bw.wg_part, chunks, cout, cin, 1, 1.0 / x_scale,
-                                                        e->bw.scales + slot, dw);
-    if ((rc = launched(e, "wgrad_reduce"))) return rc;
-  } else if (dw != nullptr) {
-    const WgPlan pl = wgrad_plan(cout, cin, static_cast<long long>(BP));
-    dd::WgradArgs a;
-    a.dy = dy;
-    a.x_hi = x_hi;
-    a.x_lo = x_lo;
-    a.x_inv_scale = 1.f / x_scale;
-    a.cout = cout;
-    a.cin = cin;
-    a.B = g.B;
-    a.H = g.h;
-    a.W = g.w;
-    a.chunk = pl.chunk;
-    a.partial = e->bw.wg_part;
-    cudaError_t err;
-    err = cout == 16 ? launch_wgrad<16, 64>(a, pl.chunks, st) : launch_wgrad<64, 16>(a, pl.chunks, st);
-    if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("wgrad: ") + cudaGetErrorString(err));
-    e->launches++;
-    const size_t n = static_cast<size_t>(cout) * cin * 9;
-    dd::wgrad_reduce_kernel<<<grid_of(n), 256, 0, st>>>(e->bw.wg_part, pl.chunks, cout, cin, 0, 1.0, dscale, dw);
-    if ((rc = launched(e, "wgrad_reduce"))) return rc;
+    dd::wgrad_reduce_kernel<<<grid_of(nw), 256, 0, st>>>(bufs.partial, chunks, cout, cin, 1, 1.0 / x_scale, bufs.scale,
+                                                         dw);
+    return launched(e, "wgrad_reduce");
   }
+  if (dw == nullptr) return DD_OK;
+  const WgPlan pl = wgrad_plan(cout, cin, static_cast<long long>(BP));
+  dd::WgradArgs a;
+  a.dy = dy;
+  a.x_hi = x_hi;
+  a.x_lo = x_lo;
+  a.x_inv_scale = 1.f / x_scale;
+  a.cout = cout;
+  a.cin = cin;
+  a.B = B;
+  a.H = H;
+  a.W = W;
+  a.chunk = pl.chunk;
+  a.partial = bufs.partial;
+  const cudaError_t err = cout == 16 ? launch_wgrad<16, 64>(a, pl.chunks, st) : launch_wgrad<64, 16>(a, pl.chunks, st);
+  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("wgrad: ") + cudaGetErrorString(err));
+  e->launches++;
+  dd::wgrad_reduce_kernel<<<grid_of(nw), 256, 0, st>>>(bufs.partial, pl.chunks, cout, cin, 0, 1.0, dscale, dw);
+  return launched(e, "wgrad_reduce");
+}
+
+// Backward of conv layer `layer` given dy [B][P][Cout] (times *dscale, nullable = 1) and the conv's input planes X (scale
+// x_scale): dw [Cout][Cin][3][3] and db [Cout] (each nullable), and dx (nullable) = conv3x3(dy, W') on the forward's
+// tensor-core kernel, left multiplied by bw.scales[slot].
+int run_conv_bwd(dd_engine* e, int layer, const float* dy, const float* dscale, const __half* x_hi, const __half* x_lo,
+                 float x_scale, float* dw, float* db, float* dx, int slot, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  const int cout = kConvCout[layer], cin = kConvCin[layer];
+  int rc;
+  if (db != nullptr && (rc = run_colsum(e, cout, dy, dscale, g.B, g.P, e->bw.col_part, nullptr, db, st))) return rc;
+  const WgradBufs bufs{e->bw.gp, e->bw.amax + slot, e->bw.scales + slot, e->status, e->bw.wg_part};
+  if ((rc = run_wgrad(e, g.B, g.h, g.w, cout, cin, dy, dscale, x_hi, x_lo, x_scale, dw, dx != nullptr, bufs, st)))
+    return rc;
   if (dx != nullptr &&
       (rc = run_conv(e, 6 + layer, e->bw.gp.hi, e->bw.gp.lo, 1.f, dd::EPI_F32, dx, nullptr, nullptr, nullptr, st)))
     return rc;
@@ -1828,11 +1853,12 @@ int run_denoiser_bwd(dd_engine* h, const float* temb, int temb_bstride, float* c
       dd::up_adjoint_kernel<<<dim3(h->cfg.cond_w, h->cfg.cond_h, g.B), 256, 0, st>>>(g0, dne_scale, g.h, g.w, h->cfg.cond_h,
                                                                                       h->cfg.cond_w, ry, rx, bw.dcond);
       if ((rc = launched(h, "up_adjoint"))) return rc;
-      if (want_dtemb && (rc = run_colsum(h, 256, bw.dcond, nullptr, PC, bw.dtemb, nullptr, st))) return rc;
+      if (want_dtemb && (rc = run_colsum(h, 256, bw.dcond, nullptr, g.B, PC, bw.col_part, bw.dtemb, nullptr, st)))
+        return rc;
       if (dcond_sink && (rc = (*dcond_sink)(bw.dcond, nullptr))) return rc;
     }
   } else {
-    if (want_dtemb && (rc = run_colsum(h, 256, g0, dne_scale, g.P, bw.dtemb, nullptr, st))) return rc;
+    if (want_dtemb && (rc = run_colsum(h, 256, g0, dne_scale, g.B, g.P, bw.col_part, bw.dtemb, nullptr, st))) return rc;
     if (dcond_sink && (rc = (*dcond_sink)(g0, dne_scale))) return rc;
   }
   // ne = relu(GN(y2)) -> noise_embedding.3 -> relu(GN(y1)) -> noise_embedding.0
@@ -2919,6 +2945,71 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   }
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(err));
   return transpose_out(yn, y, batch, cout, height * width, st);
+}
+
+// ---------------------------------------------------------------- standalone weight gradient (tests / roofline)
+size_t dd_conv3x3_wgrad_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int32_t height, int32_t width) {
+  const size_t BP = static_cast<size_t>(batch) * height * width;
+  size_t off = 0;
+  auto add = [&](size_t bytes) { off = align_up(off, 1024) + bytes; };
+  add(64);             // status + scratch
+  add(BP * cin * 4);   // x nhwc
+  add(BP * cin * 2);   // x hi
+  add(BP * cin * 2);   // x lo
+  add(BP * cout * 4);  // dy nhwc
+  add(BP * cout * 2);  // dy hi
+  add(BP * cout * 2);  // dy lo
+  add(wgrad_partial_elems(cout, cin, batch, height, width) * 8);
+  add(static_cast<size_t>(batch) * bwd_chunks(height * width) * cout * 4);  // bias-gradient partials
+  return align_up(off, 1024);
+}
+
+int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, float* db, int32_t batch, int32_t cin,
+                     int32_t cout, int32_t height, int32_t width, void* workspace, size_t workspace_bytes,
+                     void* cuda_stream) {
+  if (!h || !x || !dy || !dw || !db) return fail(DD_ERR_INVALID, "null argument");
+  if (shape_id(cin, cout) < 0) return fail(DD_ERR_UNSUPPORTED, "conv shape not on the DiffusionDepth hot path");
+  if (batch < 1 || height < 1 || width < 1) return fail(DD_ERR_INVALID, "empty geometry");
+  if (workspace_bytes < dd_conv3x3_wgrad_workspace_bytes(batch, cin, cout, height, width) ||
+      (reinterpret_cast<uintptr_t>(workspace) & 1023))
+    return fail(DD_ERR_INVALID, "wgrad workspace too small or misaligned");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const int P = height * width;
+  const size_t BP = static_cast<size_t>(batch) * P;
+  Carver c{reinterpret_cast<uint8_t*>(workspace)};
+  int* status = c.take<int>(16);
+  float* xn = c.take<float>(BP * cin);
+  __half* xhi = c.take<__half>(BP * cin);
+  __half* xlo = c.take<__half>(BP * cin);
+  float* dyn = c.take<float>(BP * cout);
+  Planes gp;
+  gp.hi = c.take<__half>(BP * cout);
+  gp.lo = c.take<__half>(BP * cout);
+  double* partial = c.take<double>(wgrad_partial_elems(cout, cin, batch, height, width));
+  float* col_part = c.take<float>(static_cast<size_t>(batch) * bwd_chunks(P) * cout);
+  float* scratch = reinterpret_cast<float*>(status) + 8;  // [0] x absmax, [1] dy absmax, [2] dy split scale
+  CUDA_TRY(cudaMemsetAsync(status, 0, 64, st));
+  int rc;
+  if ((rc = transpose_in(x, xn, batch, cin, P, st))) return rc;
+  if ((rc = transpose_in(dy, dyn, batch, cout, P, st))) return rc;
+  // X: host-side power-of-two scale, as dd_conv3x3 splits its input
+  dd::absmax_kernel<<<absmax_grid(BP * cin), 256, 0, st>>>(xn, static_cast<int>(BP * cin), scratch);
+  float ax = 0.f;
+  CUDA_TRY(cudaMemcpyAsync(&ax, scratch, 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  const float sx = (ax > 0.f && isfinite(ax)) ? exp2f(floorf(log2f(32768.f / ax)) - 1.f) : 1.f;
+  dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(xn, xhi, xlo, BP * cin / 4, sx, status);
+  if ((rc = launched(h, "split_planes"))) return rc;
+  // dY: the backward's own on-device split (also for the SIMT shapes, so a non-finite dY is reported for every shape)
+  if ((rc = run_colsum(h, cout, dyn, nullptr, batch, P, col_part, nullptr, db, st))) return rc;
+  const WgradBufs bufs{gp, scratch + 1, scratch + 2, status, partial};
+  if ((rc = run_wgrad(h, batch, height, width, cout, cin, dyn, nullptr, xhi, xlo, sx, dw, true, bufs, st))) return rc;
+  int flag = 0;
+  CUDA_TRY(cudaMemcpyAsync(&flag, status, 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (flag) return fail(DD_ERR_RANGE, "non-finite or out-of-range value in x or dy");
+  return DD_OK;
 }
 
 int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,

@@ -407,6 +407,23 @@ class DenoiseEngine:
                                         C.c_void_p(self._aligned(ws)), need, C.c_void_p(self._stream())))
         return y
 
+    def conv3x3_wgrad(self, x: torch.Tensor, dy: torch.Tensor):
+        """Weight and bias gradient of that conv on the backward's kernels: x [B,Cin,H,W], dy [B,Cout,H,W] ->
+        (dw [Cout,Cin,3,3], db [Cout]).  Raises EngineError (DD_ERR_RANGE) for a non-finite x or dy."""
+        B, cin, H, W = x.shape
+        cout = dy.shape[1]
+        if tuple(dy.shape) != (B, cout, H, W):
+            raise EngineError(f"dy {tuple(dy.shape)} does not match x {tuple(x.shape)}")
+        x, dy = (t.detach().to(self.device, torch.float32).contiguous() for t in (x, dy))
+        dw = torch.empty(cout, cin, 3, 3, device=self.device, dtype=torch.float32)
+        db = torch.empty(cout, device=self.device, dtype=torch.float32)
+        need = int(self.lib.dd_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W))
+        ws = torch.empty(need + 1024, dtype=torch.uint8, device=self.device)
+        _cabi.check(self.lib.dd_conv3x3_wgrad(self._h, C.c_void_p(x.data_ptr()), C.c_void_p(dy.data_ptr()),
+                                              C.c_void_p(dw.data_ptr()), C.c_void_p(db.data_ptr()), B, cin, cout, H, W,
+                                              C.c_void_p(self._aligned(ws)), need, C.c_void_p(self._stream())))
+        return dw, db
+
     def bench_conv(self, cin: int, cout: int, iters: int = 20) -> float:
         """Average milliseconds per launch of the (cin -> cout) conv on this engine's latent grid."""
         ms = C.c_float()

@@ -283,6 +283,17 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
                void* cuda_stream);
 size_t dd_conv3x3_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int32_t height, int32_t width);
 
+/* Standalone weight gradient of that convolution on the backward's own kernels (the tensor-core kernel for the
+ * 256-wide shapes, the fp32 CUDA-core kernel for 16->64 and 64->16), chosen by shape as dd_denoiser_backward chooses
+ * them.  x [B,Cin,H,W] and dy [B,Cout,H,W] (device fp32 NCHW) -> dw [Cout,Cin,3,3] = sum over images and pixels of
+ * dy (x) x, db [Cout] = sum of dy.  dy is split to fp16 hi/lo with the backward's on-device power-of-two scale.
+ * DD_ERR_UNSUPPORTED for a shape off the hot path; synchronises `cuda_stream` and returns DD_ERR_RANGE when x or dy held
+ * a non-finite value or left the split's range.  Does not touch the engine's workspace. */
+int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, float* db, int32_t batch, int32_t cin,
+                     int32_t cout, int32_t height, int32_t width, void* workspace, size_t workspace_bytes,
+                     void* cuda_stream);
+size_t dd_conv3x3_wgrad_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int32_t height, int32_t width);
+
 /* Time the dominant kernel (convA-shaped 256->256 3x3 on the engine's latent grid) `iters` times with
  * CUDA events on `cuda_stream`; returns average milliseconds per launch in *ms_out. */
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,

@@ -50,7 +50,8 @@ def _check(tag, got, ref, env):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("variant", ["swin", "res"])
-@pytest.mark.parametrize("hw", [(19, 27), (18, 26), (35, 53), (8, 16)])
+# (176, 352), B = 3: the wide layers' weight gradients sum 25 split-K chunks of 6-segment rows (a 352 x 704 crop)
+@pytest.mark.parametrize("hw", [(19, 27), (18, 26), (35, 53), (8, 16), (176, 352)])
 def test_gradients_vs_fp64_restatement(variant, hw):
     sd = denoiser_state(variant)
     head = make_head(variant, sd, DEV)

@@ -91,7 +91,10 @@ def test_composition_of_operator_backwards(variant, hw, T, B):
         assert m[k] <= CHAIN_TOL, (k, m[k])
 
 
+# the last two run the wide layers' weight gradients over 6 and 5 split-K chunks, rows of 4 and 3 segments (the second
+# with a 2-pixel tail segment)
 CASES = [(v, hw, 3) for v in ("swin", "res") for hw in ((19, 27), (18, 26), (35, 53), (8, 16))] + [("swin", (19, 27), 20)]
+CASES += [("swin", (64, 200), 3), ("res", (67, 130), 3)]
 
 
 @pytest.mark.gpu
