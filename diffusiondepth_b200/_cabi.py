@@ -61,6 +61,8 @@ SIGNATURES = {
     "dd_denoiser_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t,
                                        C.c_void_p]),
+    "dd_denoiser_relu_inputs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
+                                          C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_void_p]),
     "dd_denoise_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p,
                                       C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -74,15 +74,37 @@ struct GnBwdArgs {
   float* dy;               // [B][P][C]
 };
 
+// z, the ReLU's input, of channel c of image b.  The backward's mask is z > 0; gn_pre_relu_kernel exports the same z
+// (dd_denoiser_relu_inputs), so both go through this one expression.
+template <int C>
+__device__ __forceinline__ float gn_pre_relu(const GnBwdArgs& a, int b, int c, float yv) {
+  const int g = c / (C / 4);
+  const float mean = a.mean_rstd[(b * 4 + g) * 2], rstd = a.mean_rstd[(b * 4 + g) * 2 + 1];
+  const float sa = rstd * a.gamma[c];
+  return fmaf(yv, sa, a.beta[c] - sa * mean);  // the forward's expression (gn_apply_split_kernel)
+}
+
 template <int C>
 __device__ __forceinline__ void gn_bwd_point(const GnBwdArgs& a, int b, int c, float yv, float dov, float inv, float& dz,
                                              float& xh) {
   const int g = c / (C / 4);
   const float mean = a.mean_rstd[(b * 4 + g) * 2], rstd = a.mean_rstd[(b * 4 + g) * 2 + 1];
-  const float sa = rstd * a.gamma[c];
-  const float z = fmaf(yv, sa, a.beta[c] - sa * mean);  // the forward's expression (gn_apply_split_kernel)
-  dz = z > 0.f ? dov * inv : 0.f;
+  dz = gn_pre_relu<C>(a, b, c, yv) > 0.f ? dov * inv : 0.f;
   xh = (yv - mean) * rstd;
+}
+
+// z = gn_pre_relu of every element of a.y [B][P][C], written as fp32 NCHW [B][C][P] (uses a.y, mean_rstd, gamma, beta,
+// B, P only)
+template <int C>
+__global__ void __launch_bounds__(256) gn_pre_relu_kernel(const GnBwdArgs a, float* __restrict__ z) {
+  const size_t n = static_cast<size_t>(a.B) * C * a.P;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int p = static_cast<int>(i % a.P);
+    const int c = static_cast<int>(i / a.P % C);
+    const int b = static_cast<int>(i / a.P / C);
+    z[i] = gn_pre_relu<C>(a, b, c, a.y[(static_cast<size_t>(b) * a.P + p) * C + c]);
+  }
 }
 
 template <int C>

@@ -1638,20 +1638,27 @@ int grid_of(size_t n, int per_block = 256) {
   return static_cast<int>(std::max<size_t>(1, std::min<size_t>(b, 132 * 16)));
 }
 
-// GroupNorm `which` (0 ne.1, 1 ne.4, 2 pred.1, 3 pred.4) + ReLU backward: dout (times *dscale) -> dy (unscaled)
-template <int C>
-int run_gn_bwd(dd_engine* e, int which, const float* dout, const float* dscale, const float* y, float* dgamma,
-               float* dbeta, float* dy, cudaStream_t st) {
+// GroupNorm `which` (0 ne.1, 1 ne.4, 2 pred.1, 3 pred.4) of the pre-GN output y: its mean / rstd, gamma, beta
+dd::GnBwdArgs gn_args(dd_engine* e, int which, const float* y) {
   const Geom g = geom_of(e->cfg);
-  dd::GnBwdArgs a;
-  a.dout = dout;
-  a.dscale = dscale;
+  dd::GnBwdArgs a{};
   a.y = y;
   a.mean_rstd = e->mr[which];
   a.gamma = e->gn_gamma[which];
   a.beta = e->gn_beta[which];
   a.B = g.B;
   a.P = g.P;
+  return a;
+}
+
+// GroupNorm `which` + ReLU backward: dout (times *dscale) -> dy (unscaled)
+template <int C>
+int run_gn_bwd(dd_engine* e, int which, const float* dout, const float* dscale, const float* y, float* dgamma,
+               float* dbeta, float* dy, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  dd::GnBwdArgs a = gn_args(e, which, y);
+  a.dout = dout;
+  a.dscale = dscale;
   a.chunks = bwd_chunks(g.P);
   a.partial = e->bw.gn_part;
   a.ab = e->bw.ab;
@@ -1665,6 +1672,14 @@ int run_gn_bwd(dd_engine* e, int which, const float* dout, const float* dscale, 
   if ((rc = launched(e, "gn_bwd_finalize"))) return rc;
   dd::gn_bwd_apply_kernel<C><<<grid_of(static_cast<size_t>(g.B) * g.P * C / 4), 256, 0, st>>>(a);
   return launched(e, "gn_bwd_apply");
+}
+
+// GroupNorm `which`'s output before its ReLU, fp32 NCHW [B][C][h][w]: z > 0 is run_gn_bwd's mask, bit for bit
+template <int C>
+int run_gn_pre_relu(dd_engine* e, int which, const float* y, float* z, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  dd::gn_pre_relu_kernel<C><<<grid_of(static_cast<size_t>(g.B) * g.P * C), 256, 0, st>>>(gn_args(e, which, y), z);
+  return launched(e, "gn_pre_relu");
 }
 
 // column sums of x [B][P][C] (times *scale): per image (out_img [B][C]) and / or over the batch in image order (out_sum
@@ -1923,6 +1938,32 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
 }
 
 constexpr size_t kDecGradNumel[6] = {16 * 16 * 4 * 4, 16, 16, 16, 16 * 9, 1};
+
+// Checks of an entry that recomputes one denoiser call on the backward's region (dd_denoiser_backward,
+// dd_denoiser_relu_inputs), after its own null-pointer checks.
+int check_operator_bwd_call(const dd_engine* h, const char* entry, const int64_t* t_host) {
+  if (!has_backward(h->cfg))
+    return fail(DD_ERR_INVALID, std::string(entry) + " needs an engine created with DD_FLAG_BACKWARD (or DD_FLAG_LOOP_BACKWARD)");
+  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  const Geom g = geom_of(h->cfg);
+  for (int b = 0; b < g.B; ++b)
+    if (t_host[b] < 0 || t_host[b] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
+  if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
+    return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");
+  return DD_OK;
+}
+
+// One denoiser call's inputs as run_recompute reads them: image b's time-embedding row t_host[b] (checked) in
+// temb_sel, cond and noisy as NHWC, the latent's fp16 split planes.
+int stage_operator_inputs(dd_engine* h, const float* cond, const float* noisy, const int64_t* t_host, cudaStream_t st) {
+  const Geom g = geom_of(h->cfg);
+  int rc;
+  for (int b = 0; b < g.B; ++b)
+    CUDA_TRY(cudaMemcpyAsync(h->temb_sel + b * 256, h->temb + t_host[b] * 256, 1024, cudaMemcpyDeviceToDevice, st));
+  if ((rc = transpose_in(cond, h->cond, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
+  if ((rc = transpose_in(noisy, h->x32, g.B, 16, g.P, st))) return rc;
+  return split_planes(h, h->x32, h->xs_hi, h->xs_lo, static_cast<size_t>(g.B) * g.P * 16, kXScale, st);
+}
 
 }  // namespace
 
@@ -2322,17 +2363,11 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
                          float* d_cond_out, float* d_noisy_out, float* const* d_params, void* workspace,
                          size_t workspace_bytes, void* cuda_stream) {
   if (!h || !cond || !noisy || !t_host || !d_eps) return fail(DD_ERR_INVALID, "null argument");
-  if (!has_backward(h->cfg))
-    return fail(DD_ERR_INVALID, "dd_denoiser_backward needs an engine created with DD_FLAG_BACKWARD (or DD_FLAG_LOOP_BACKWARD)");
-  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  int rc;
+  if ((rc = check_operator_bwd_call(h, "dd_denoiser_backward", t_host))) return rc;
   const Geom g = geom_of(h->cfg);
-  for (int b = 0; b < g.B; ++b)
-    if (t_host[b] < 0 || t_host[b] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
-  if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
-    return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CUDA_TRY(cudaSetDevice(h->cfg.device));
-  int rc;
   if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
   const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
   const int npar = swin ? 21 : 17;
@@ -2344,11 +2379,7 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
   const int PC = h->cfg.cond_h * h->cfg.cond_w;
   h->launches = 0;
   CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
-  for (int b = 0; b < g.B; ++b)
-    CUDA_TRY(cudaMemcpyAsync(h->temb_sel + b * 256, h->temb + t_host[b] * 256, 1024, cudaMemcpyDeviceToDevice, st));
-  if ((rc = transpose_in(cond, h->cond, g.B, 256, PC, st))) return rc;
-  if ((rc = transpose_in(noisy, h->x32, g.B, 16, g.P, st))) return rc;
-  if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, BP * 16, kXScale, st))) return rc;
+  if ((rc = stage_operator_inputs(h, cond, noisy, t_host, st))) return rc;
   if ((rc = transpose_in(d_eps, bw.g[0], g.B, 16, g.P, st))) return rc;
   auto sink = [&](const float* dc, const float* scale) -> int {
     int r;
@@ -2373,6 +2404,27 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
     dd::unscale_kernel<<<grid_of(BP * 16), 256, 0, st>>>(d_noisy_out, BP * 16, bw.scales + 5);
     if ((rc = launched(h, "unscale"))) return rc;
   }
+  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
+  return DD_OK;
+}
+
+int dd_denoiser_relu_inputs(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host,
+                            float* const* z_out, void* workspace, size_t workspace_bytes, void* cuda_stream) {
+  if (!h || !cond || !noisy || !t_host || !z_out) return fail(DD_ERR_INVALID, "null argument");
+  int rc;
+  if ((rc = check_operator_bwd_call(h, "dd_denoiser_relu_inputs", t_host))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  const dd_engine::Bwd& bw = h->bw;
+  h->launches = 0;
+  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+  if ((rc = stage_operator_inputs(h, cond, noisy, t_host, st))) return rc;
+  if ((rc = run_recompute(h, h->temb_sel, 256, st))) return rc;
+  if (z_out[0] && (rc = run_gn_pre_relu<64>(h, 0, bw.y1, z_out[0], st))) return rc;
+  if (z_out[1] && (rc = run_gn_pre_relu<256>(h, 1, bw.y2, z_out[1], st))) return rc;
+  if (z_out[2] && (rc = run_gn_pre_relu<64>(h, 2, bw.y5, z_out[2], st))) return rc;
+  if (z_out[3] && (rc = run_gn_pre_relu<16>(h, 3, bw.y6, z_out[3], st))) return rc;
   if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
   return DD_OK;
 }

@@ -36,6 +36,8 @@ _PARAM_SHAPES = {
     "model.pred.4.weight": (16,), "model.pred.4.bias": (16,),
     "model.upsample_fuse.convA.conv.weight": (256, 256, 3, 3), "model.upsample_fuse.convA.conv.bias": (256,),
     "model.upsample_fuse.convB.conv.weight": (256, 256, 3, 3), "model.upsample_fuse.convB.conv.bias": (256,)}
+# the denoiser's GroupNorm(4, C) + ReLU layers in forward order (dd_denoiser_relu_inputs' z_out order): channels
+GN_LAYERS = {"noise_embedding.1": 64, "noise_embedding.4": 256, "pred.1": 64, "pred.4": 16}
 DECODER_KEYS = (
     "depth_transform.conv_inv_transform.0.weight", "depth_transform.conv_inv_transform.0.bias",
     "depth_transform.conv_inv_transform.1.weight", "depth_transform.conv_inv_transform.1.bias",
@@ -313,6 +315,24 @@ class DenoiseEngine:
             C.c_void_p(d_noisy.data_ptr() if want_noisy else 0), ptrs, C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
             C.c_void_p(self._stream())))
         return d_cond, d_noisy, grads
+
+    def denoiser_relu_inputs(self, cond: torch.Tensor, noisy: torch.Tensor, t) -> Dict[str, torch.Tensor]:
+        """The inputs of the denoiser's four ReLUs, z = GroupNorm(y) [B,C,h,w], as `denoiser_backward` recomputes them
+        (engine created with backward=True): {GroupNorm layer name: z}, in GN_LAYERS order.  z > 0 is exactly the mask
+        that backward applies."""
+        if not self.backward:
+            raise EngineError("engine was created without backward=True")
+        B, (h, w) = self.batch, self.latent_hw
+        self._check_in(cond, (B, 256, *self.cond_hw))
+        self._check_in(noisy, (B, 16, h, w))
+        ts = self._timesteps(t)
+        z = {k: torch.empty(B, c, h, w, device=self.device, dtype=torch.float32) for k, c in GN_LAYERS.items()}
+        ws = self._workspace()
+        _cabi.check(self.lib.dd_denoiser_relu_inputs(
+            self._h, C.c_void_p(cond.data_ptr()), C.c_void_p(noisy.data_ptr()), (C.c_int64 * B)(*ts),
+            (C.c_void_p * 4)(*[v.data_ptr() for v in z.values()]), C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
+            C.c_void_p(self._stream())))
+        return z
 
     def _grad_buffers(self, keys, shapes, default=None):
         grads = {k: torch.empty(shapes.get(k, default), device=self.device, dtype=torch.float32) for k in keys}

@@ -26,7 +26,9 @@
  *   dd_denoiser_backward          <- reverse-mode differentiation of that call: the gradients of
  *                                    `ScheduledCNNRefine` (head :336-382 / res.py:301-344) that `ddim_loss`
  *                                    (head :207-223) needs for training
- *   dd_denoise_backward           <- reverse-mode differentiation of dd_denoise_decode: the training graph of
+ *   dd_denoiser_relu_inputs       <- the inputs of that call's four `nn.ReLU` after `nn.GroupNorm(4, C)`
+ *                                    (head :341-358 / res.py:305-321), as the backward recomputes them
+ *   dd_denoise_backward          <- reverse-mode differentiation of dd_denoise_decode: the training graph of
  *                                    `pred` and the final latent under the reference's L1 + L2 + DDIM loss
  *                                    (head :130-146, :165-175, :207-223) through every step and the decoder
  *   dd_decode                     <- `depth_transform.inv_t(latent)` alone (the *Vis heads call it
@@ -231,6 +233,19 @@ int dd_denoiser_forward(dd_handle h, const float* cond, const float* noisy, cons
 int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host, const float* d_eps,
                          float* d_cond_out, float* d_noisy_out, float* const* d_params, void* workspace,
                          size_t workspace_bytes, void* cuda_stream);
+
+/* The inputs of the four ReLUs of ScheduledCNNRefine (reference head :341-358 / res.py:305-321, `nn.ReLU` after each
+ * `nn.GroupNorm(4, C)`) as dd_denoiser_backward's recompute produces them: z = gamma * xhat + beta of
+ *   z_out[0] noise_embedding.1 [B,64,h,w]    z_out[1] noise_embedding.4 [B,256,h,w]
+ *   z_out[2] pred.1            [B,64,h,w]    z_out[3] pred.4            [B,16,h,w]
+ * (fp32 NCHW, each entry nullable) for eps = ScheduledCNNRefine(noisy, t, cond).  The inputs are staged and the
+ * forward recomputed exactly as dd_denoiser_backward does, and z comes from the expression its GroupNorm + ReLU
+ * backward evaluates, so z > 0 is, bit for bit, the mask that backward applies.  For checking the backward against a
+ * higher-precision computation at the same masks.  Argument checks as dd_denoiser_backward (DD_FLAG_BACKWARD or
+ * DD_FLAG_LOOP_BACKWARD, null arguments, timesteps, workspace); DD_FLAG_CHECK_RANGE is honoured; does not synchronise
+ * otherwise.  Results are bit-identical run to run. */
+int dd_denoiser_relu_inputs(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host,
+                            float* const* z_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* Backward of dd_denoise_decode (reference CNNDDIMPipiline.__call__ + DeepDepthTransformWithUpsampling.inv_t, head
  * :254-303 / depth_transform.py:33-35, differentiated in reverse mode through all T denoiser calls, the T DDIM updates

@@ -26,24 +26,67 @@ class _FlipReluTorch:
         return getattr(torch, name)
 
 
-def restatement_grads(variant, sd, noisy, cond, t, d_eps, dtype=torch.float64, band=0.0):
-    """Gradients of sum(eps * d_eps) for eps = restate.denoiser, by torch autograd in `dtype` on CPU; `band` > 0 flips
-    the ReLU masks within `band` of the kink (see kink_envelope)."""
+class _MaskedReluTorch:
+    """Stands in for the `torch` module inside oracle.restate during one denoiser call: everything is torch's, except
+    that its k-th relu(z) returns z * masks[k] (masks: the four ReLUs' 0 / 1 masks in forward order, e.g. the engine's
+    own; None: z > 0, the restatement's own) and records z in fp64.  A call that runs more or fewer than len(masks) relus
+    is an error."""
+
+    def __init__(self, masks):
+        self._masks = list(masks)
+        self.z = []
+
+    def relu(self, z):
+        if len(self.z) == len(self._masks):
+            raise RuntimeError(f"more than {len(self._masks)} relu calls")
+        m = self._masks[len(self.z)]
+        if m is None:
+            m = z.detach() > 0
+        if tuple(m.shape) != tuple(z.shape):
+            raise RuntimeError(f"mask {len(self.z)} has shape {tuple(m.shape)}, relu input {tuple(z.shape)}")
+        self.z.append(z.detach().to(torch.float64))
+        return z * m.to(z.dtype)
+
+    def check_complete(self):
+        if len(self.z) != len(self._masks):
+            raise RuntimeError(f"{len(self.z)} relu calls, {len(self._masks)} masks")
+
+    def __getattr__(self, name):
+        return getattr(torch, name)
+
+
+def _grads_with(stand_in, variant, sd, noisy, cond, t, d_eps, dtype):
+    """Gradients of sum(eps * d_eps), eps = restate.denoiser with `stand_in` (None: torch itself) as restate's torch."""
     p = {k: v.detach().cpu().to(dtype).requires_grad_(True) for k, v in sd.items()}
     x = noisy.detach().cpu().to(dtype).requires_grad_(True)
     c = cond.detach().cpu().to(dtype).requires_grad_(True)
-    if band == 0:
+    if stand_in is not None:
+        restate.torch = stand_in
+    try:
         eps = restate.denoiser(p, x, torch.as_tensor(t).cpu(), c, variant, prefix="model.")
-    else:
-        restate.torch = _FlipReluTorch(band)
-        try:
-            eps = restate.denoiser(p, x, torch.as_tensor(t).cpu(), c, variant, prefix="model.")
-        finally:
-            restate.torch = torch
+    finally:
+        restate.torch = torch
     (eps * d_eps.detach().cpu().to(dtype)).sum().backward()
     out = {"d_noisy": x.grad, "d_cond": c.grad}
     out.update({k: v.grad for k, v in p.items()})
     return out
+
+
+def restatement_grads(variant, sd, noisy, cond, t, d_eps, dtype=torch.float64, band=0.0):
+    """Gradients of sum(eps * d_eps) for eps = restate.denoiser, by torch autograd in `dtype` on CPU; `band` > 0 flips
+    the ReLU masks within `band` of the kink (see kink_envelope)."""
+    return _grads_with(_FlipReluTorch(band) if band != 0 else None, variant, sd, noisy, cond, t, d_eps, dtype)
+
+
+def masked_restatement_grads(variant, sd, noisy, cond, t, d_eps, masks):
+    """As restatement_grads in fp64, but with the four ReLU masks given (forward order, [B,C,h,w] each, e.g. the
+    engine's `z > 0`; None: the fp64 forward's own) instead of taken from the fp64 forward: (gradients, the four ReLU
+    inputs z in fp64).  At the
+    engine's own masks the gradients differ from the engine's by rounding alone, with no kink to allow for."""
+    relu = _MaskedReluTorch(masks)
+    grads = _grads_with(relu, variant, sd, noisy, cond, t, d_eps, torch.float64)
+    relu.check_complete()
+    return grads, relu.z
 
 
 def golden_margins(golden, case, grads):

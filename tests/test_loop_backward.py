@@ -11,7 +11,7 @@ import torch.nn.functional as F
 
 from diffusiondepth_b200 import _cabi
 from diffusiondepth_b200.engine import DECODER_PARAM_KEYS, DenoiseEngine
-from grad_helpers import tensor_margins
+from grad_helpers import masked_restatement_grads, tensor_margins
 from loop_grad_helpers import decode_restatement_grads, loop_restatement_grads, make_loop_head
 from oracle import restate
 from oracle.make_loop_grads import loop_state
@@ -41,7 +41,9 @@ def _loop_engine(head, B, hw, chw):
 
 
 def _native(eng, cond, noise, d_depth, d_latent, want_latents=False):
-    d_cond, d_noise, grads, lat = eng.denoise_backward(cond.to(DEV), noise.to(DEV), d_depth.to(DEV), d_latent.to(DEV),
+    d_cond, d_noise, grads, lat = eng.denoise_backward(cond.to(DEV), noise.to(DEV),
+                                                       d_depth.to(DEV) if d_depth is not None else None,
+                                                       d_latent.to(DEV) if d_latent is not None else None,
                                                        want_latents=want_latents)
     eng.poll_status()
     out = {"d_cond": d_cond, "d_noise": d_noise}
@@ -134,6 +136,48 @@ def test_loop_gradients_vs_fp64_restatement(variant, hw, T):
         assert m[k] <= TOL + 2 * env[k], (k, m[k], env[k])
     rows = got["model.time_embedding.weight"].abs().sum(1).nonzero().flatten().tolist()
     assert rows == sorted(head.scheduler.fused_coefficients(T)[0])
+
+
+# the last two run the wide layers' weight gradients over 6 and 5 split-K chunks (the second with a 2-pixel tail segment)
+MASK_CASES = [("swin", (19, 27), 3), ("swin", (19, 27), 20), ("res", (35, 53), 3), ("swin", (64, 200), 3),
+              ("res", (67, 130), 3)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant,hw,T", MASK_CASES)
+def test_loop_gradients_vs_fp64_at_engine_masks(variant, hw, T):
+    """d_latent only: the loop backward against an fp64 chain of operator VJPs at the engine's own latents, each step
+    evaluated at the ReLU masks the engine's backward applied there (denoiser_relu_inputs on the same engine), so that
+    rounding is the only difference left: no kink envelope."""
+    sd = loop_state(variant)
+    cond, noise, _, d_latent = _inputs(variant, hw)
+    B = cond.shape[0]
+    head = make_loop_head(variant, sd, T, DEV)
+    eng = _loop_engine(head, B, hw, tuple(cond.shape[-2:]))
+    got, lat = _native(eng, cond, noise, None, d_latent, want_latents=True)
+    for k in DECODER_PARAM_KEYS:  # the depth does not enter the loss
+        assert float(got[k].abs().max()) == 0.0, k
+    ts, cx, ce = head.scheduler.fused_coefficients(T)
+    msd = {k: v for k, v in sd.items() if k.startswith("model.")}
+    c = cond.to(DEV)
+    g = d_latent.double()
+    ref = {"d_cond": torch.zeros(cond.shape, dtype=torch.float64)}
+    flips = 0
+    for s in reversed(range(T)):
+        x = lat[s].contiguous()
+        z = eng.denoiser_relu_inputs(c, x, ts[s])
+        masks = [v.cpu() > 0 for v in z.values()]
+        gr, z64 = masked_restatement_grads(variant, msd, x.cpu(), cond, [ts[s]] * B, float(np.float32(ce[s])) * g, masks)
+        flips += sum(int((m != (zr > 0)).sum()) for m, zr in zip(masks, z64))
+        ref["d_cond"] += gr["d_cond"]
+        for k in msd:
+            ref[k] = ref.get(k, 0) + gr[k]
+        g = float(np.float32(cx[s])) * g + gr["d_noisy"]
+    ref["d_noise"] = g
+    m = tensor_margins(got, ref)
+    _report(f"fp64 at engine masks {variant} {hw} T={T}; {flips} masks differ from fp64's", m)
+    for k in m:
+        assert m[k] <= 1e-4, (k, m[k])
 
 
 @pytest.mark.gpu
