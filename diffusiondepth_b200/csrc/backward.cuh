@@ -13,7 +13,7 @@ constexpr int WG_KS = 32;       // pixels per shared-memory stage of the weight-
 constexpr int WG_FLUSH = 8;     // stages summed in fp32 before the per-thread fp64 accumulators take them
 
 // Largest power of two k with amax * k < 2^14 (the rule of the weight split); 1 when amax is 0, inf or NaN.
-__device__ __forceinline__ float grad_scale_of(float amax) {
+__host__ __device__ __forceinline__ float grad_scale_of(float amax) {
   if (!(amax > 0.f) || !isfinite(amax)) return 1.f;
   return exp2f(floorf(log2f(32768.f / amax)) - 1.f);
 }

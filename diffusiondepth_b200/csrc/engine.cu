@@ -37,6 +37,19 @@ int fail(int code, const std::string& msg) {
       return fail(DD_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));             \
   } while (0)
 
+// The check after every kernel launch.  check_launch leaves the engine's launch count alone (weight packing, the
+// standalone layer entries, and the transposes / splits whose callers count them); launched() counts one launch.
+int check_launch(const char* what) {
+  const cudaError_t err = cudaGetLastError();
+  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(err));
+  return DD_OK;
+}
+// Blocks of per_block elements each for a grid-stride kernel over n elements, capped at 16 per SM of an H100 (132 SMs).
+int grid_of(size_t n, int per_block = 256) {
+  const size_t b = (n + per_block - 1) / per_block;
+  return static_cast<int>(std::max<size_t>(1, std::min<size_t>(b, 132 * 16)));
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -58,98 +71,81 @@ int absmax_grid(size_t n) {  // blocks of 256 threads, ~4 elements per thread, a
   return static_cast<int>(b < 1 ? 1 : (b > 296 ? 296 : b));
 }
 
+// Power-of-two split scale (dd::grad_scale_of) of the absmax that `launch_absmax` leaves in the device word *amax_dev:
+// the largest power of two with amax * scale < 2^15, so hi stays finite and lo = O(2^4) stays normal.  The word is
+// zeroed first; st is synchronised to read it back.
+template <typename Absmax>
+int split_scale(float* amax_dev, cudaStream_t st, float* scale, Absmax&& launch_absmax) {
+  CUDA_TRY(cudaMemsetAsync(amax_dev, 0, 4, st));
+  launch_absmax();
+  int rc;
+  if ((rc = check_launch("absmax"))) return rc;
+  float amax = 0.f;
+  CUDA_TRY(cudaMemcpyAsync(&amax, amax_dev, 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  *scale = dd::grad_scale_of(amax);
+  return DD_OK;
+}
+// ... of the n device floats at x
+int split_scale_of(const float* x, size_t n, float* amax_dev, cudaStream_t st, float* scale) {
+  return split_scale(amax_dev, st, scale, [&] {
+    dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(x, static_cast<int>(n), amax_dev);
+  });
+}
+
 CUtensorMapSwizzle swizzle_for(int bk) {
   return bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-// activations: NHWC fp16 plane [B][H][W][C]; box = {bk, 16, 8, 1}
-int make_act_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bk, dd::TILE_W, dd::TILE_H, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(activation) failed: " + std::to_string((int)r));
+// The one cuTensorMapEncodeTiled call: an fp16 tensor of `rank` dims (innermost first; strides in bytes of dims 1..),
+// no interleave, out-of-bounds elements read as zero.  `what` names the map in the error message.
+int encode_map(CUtensorMap* m, const char* what, cuuint32_t rank, const __half* base, const cuuint64_t* dims,
+               const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swizzle,
+               CUtensorMapL2promotion l2) {
+  const CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<__half*>(base), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(DD_ERR_CUDA, std::string("cuTensorMapEncodeTiled(") + what + ") failed: " + std::to_string((int)r));
   return DD_OK;
 }
-// activations sampled with a spatial stride (stride-2 convs): elementStrides = {1, s, s, 1}; the box spans 16*s x 8*s
-// input positions and still delivers 16 x 8 pixels
-int make_act_map_strided(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk, int stride) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bk, (cuuint32_t)(dd::TILE_W * stride), (cuuint32_t)(dd::TILE_H * stride), 1};
-  cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(strided activation) failed: " + std::to_string((int)r));
-  return DD_OK;
+
+// NHWC fp16 plane [B][H][W][C] read in boxes of {box_c, box_w, box_h, 1}.  With stride s > 1 (stride-2 convs) the
+// element strides are {1, s, s, 1}: a box spanning box_w x box_h input positions delivers box_w / s x box_h / s pixels.
+//   convgen activations  box {bk, 16 s, 8 s}, swizzle_for(bk)
+//   halo-kernel strip    box {bk, 8, 18},     swizzle_for(bk)
+//   wgrad operand        box {64, 64, 1},     128-byte swizzle (64 channels x 64 pixels of one row)
+int make_nhwc_map(CUtensorMap* m, const char* what, const __half* base, int B, int H, int W, int C, int box_c, int box_w,
+                  int box_h, CUtensorMapSwizzle swizzle, int stride = 1) {
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+  return encode_map(m, what, 4, base, dims, strides, box, estr, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
-// activation strip for the halo kernel: box = {bk, 8, 18, 1}
-int make_strip_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)bk, dd::HALO_TW, dd::HALO_TH + 2, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(strip) failed: " + std::to_string((int)r));
-  return DD_OK;
+// activations of the convgen kernel: 16 x 8 output pixels (sampled with `stride`) by bk channels
+int make_act_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk, int stride = 1) {
+  return make_nhwc_map(m, "activation", base, B, H, W, C, bk, dd::TILE_W * stride, dd::TILE_H * stride, swizzle_for(bk),
+                       stride);
 }
 // halo patch of conv5x5_fold_kernel: the NHWC [B][H][W][256] fp16 plane seen as {8 ch, y, x, channel group, image};
 // box = {8, 20, 36, 2, 1} lands in shared memory as [channel group][x][y][8 ch], no swizzle
 int make_patch_map(CUtensorMap* m, const __half* base, int B, int H, int W) {
   const cuuint64_t px = 256 * 2;  // bytes per pixel
-  cuuint64_t gdim[5] = {8, (cuuint64_t)H, (cuuint64_t)W, 32, (cuuint64_t)B};
-  cuuint64_t gstr[4] = {(cuuint64_t)W * px, px, 16, (cuuint64_t)H * W * px};
-  cuuint32_t box[5] = {8, dd::F5::PH, dd::F5::PW, 2, 1};
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(patch) failed: " + std::to_string((int)r));
-  return DD_OK;
+  const cuuint64_t dims[5] = {8, (cuuint64_t)H, (cuuint64_t)W, 32, (cuuint64_t)B};
+  const cuuint64_t strides[4] = {(cuuint64_t)W * px, px, 16, (cuuint64_t)H * W * px};
+  const cuuint32_t box[5] = {8, dd::F5::PH, dd::F5::PW, 2, 1};
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  return encode_map(m, "patch", 5, base, dims, strides, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
-// weights: [9][COUT][CIN] fp16; box = {bk, COUT, 1}
-int make_w_map(CUtensorMap* m, const __half* base, int cout, int cin, int bk, int box_rows = 0) {
-  cuuint64_t gdim[3] = {(cuuint64_t)cin, (cuuint64_t)cout, 9};
-  cuuint64_t gstr[2] = {(cuuint64_t)cin * 2, (cuuint64_t)cout * cin * 2};
-  cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)(box_rows ? box_rows : cout), 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(bk), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(weight) failed: " + std::to_string((int)r));
-  return DD_OK;
-}
-
-// weight-gradient operand: NHWC fp16 plane [B][H][W][C]; box = {64 channels, 64 pixels of one row}, 128-byte swizzle
-int make_wgm_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C) {
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t gstr[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {64, 64, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(wgrad operand) failed: " + std::to_string((int)r));
-  return DD_OK;
-}
-
-// general conv weights: [taps][COUT][CIN] fp16; box = {GEN_BK, NT, 1}
-int make_wgen_map(CUtensorMap* m, const __half* base, int cout, int cin, int taps, int nt) {
-  cuuint64_t gdim[3] = {(cuuint64_t)cin, (cuuint64_t)cout, (cuuint64_t)taps};
-  cuuint64_t gstr[2] = {(cuuint64_t)cin * 2, (cuuint64_t)cout * cin * 2};
-  cuuint32_t box[3] = {dd::GEN_BK, (cuuint32_t)nt, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(base), gdim, gstr, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(dd::GEN_BK), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(DD_ERR_CUDA, "cuTensorMapEncodeTiled(gen weight) failed: " + std::to_string((int)r));
-  return DD_OK;
+// conv weights [taps][cout][cin] fp16 read in boxes of {box_k, rows, 1}: the halo kernel's (9 taps, all cout rows, its
+// K chunk) and the convgen kernel's (GEN_BK, one N tile of rows)
+int make_weight_map(CUtensorMap* m, const __half* base, int cout, int cin, int taps, int box_k, int rows) {
+  const cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)cout, (cuuint64_t)taps};
+  const cuuint64_t strides[2] = {(cuuint64_t)cin * 2, (cuuint64_t)cout * cin * 2};
+  const cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)rows, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  return encode_map(m, "weight", 3, base, dims, strides, box, estr, swizzle_for(box_k), CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // ---- conv shapes served by the engine
@@ -164,14 +160,66 @@ int shape_id(int cin, int cout) {
 }
 
 constexpr int kHaloBK[5] = {16, 32, 32, 32, 32};  // K chunk of the halo kernel per shape id
+
+// One 3x3 conv kernel: conv3x3_simt_kernel (fp32 CUDA cores, reads sa) or the persistent conv3x3_halo_kernel (reads
+// the strip maps m[0..1] of the input planes and the weight maps m[2..3]).
 template <int CIN, int COUT, int BK, int EPI>
-cudaError_t launch_halo(const CUtensorMap& a_hi, const CUtensorMap& a_lo, const CUtensorMap& b_hi,
-                        const CUtensorMap& b_lo, const dd::ConvArgs& args, int sm_count, cudaStream_t st) {
-  using C = dd::HaloCfg<CIN, COUT, BK>;
-  int grid = args.num_tiles < sm_count ? args.num_tiles : sm_count;
-  dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(a_hi, a_lo, b_hi, b_lo, args);
-  return cudaGetLastError();
+void conv3x3_kernel(bool simt, const dd::SimtArgs& sa, const CUtensorMap* m, const dd::ConvArgs& a, int sm_count,
+                    cudaStream_t st) {
+  if (simt) {
+    constexpr int CO_T = COUT < 64 ? COUT : 64;
+    dd::conv3x3_simt_kernel<CIN, COUT, EPI><<<dim3(a.num_tiles, COUT / CO_T), 256, 0, st>>>(sa);
+  } else {
+    using C = dd::HaloCfg<CIN, COUT, BK>;
+    const int grid = a.num_tiles < sm_count ? a.num_tiles : sm_count;
+    dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(m[0], m[1], m[2], m[3], a);
+  }
 }
+template <int CIN, int COUT, int BK>
+void conv3x3_epi(int epi, bool simt, const dd::SimtArgs& sa, const CUtensorMap* m, const dd::ConvArgs& a, int sm_count,
+                 cudaStream_t st) {
+  if (epi == dd::EPI_F32_STATS) conv3x3_kernel<CIN, COUT, BK, dd::EPI_F32_STATS>(simt, sa, m, a, sm_count, st);
+  else if (epi == dd::EPI_SPLIT) conv3x3_kernel<CIN, COUT, BK, dd::EPI_SPLIT>(simt, sa, m, a, sm_count, st);
+  else conv3x3_kernel<CIN, COUT, BK, dd::EPI_F32>(simt, sa, m, a, sm_count, st);
+}
+
+// Launch the 3x3 conv of shape `sid` with epilogue `epi` on a's B x H x W grid, from fp16 hi / lo input planes at
+// scale in_scale: conv3x3_simt_kernel on 16 x 8 tiles (simt; weights w_simt) or conv3x3_halo_kernel on 8 x 16 tiles
+// (weight maps w_hi / w_lo).  Sets a's tile fields to the chosen kernel's tiling; the caller checks the launch.
+int launch_conv3x3(int sid, int epi, bool simt, dd::ConvArgs& a, const __half* in_hi, const __half* in_lo,
+                   float in_scale, const float* w_simt, const CUtensorMap& w_hi, const CUtensorMap& w_lo, int sm_count,
+                   cudaStream_t st) {
+  const int tw = simt ? dd::TILE_W : dd::HALO_TW, th = simt ? dd::TILE_H : dd::HALO_TH;
+  a.tiles_x = (a.W + tw - 1) / tw;
+  a.tiles_y = (a.H + th - 1) / th;
+  a.num_tiles = a.tiles_x * a.tiles_y * a.B;
+  CUtensorMap m[4] = {{}, {}, w_hi, w_lo};
+  dd::SimtArgs sa{};
+  if (simt) {
+    sa.in_hi = in_hi;
+    sa.in_lo = in_lo;
+    sa.in_inv_scale = 1.f / in_scale;
+    sa.w = w_simt;
+    sa.c = a;
+  } else {
+    const int cin = kShapes[sid].cin, bk = kHaloBK[sid];
+    int rc;
+    if ((rc = make_nhwc_map(&m[0], "strip", in_hi, a.B, a.H, a.W, cin, bk, dd::HALO_TW, dd::HALO_TH + 2, swizzle_for(bk))))
+      return rc;
+    if ((rc = make_nhwc_map(&m[1], "strip", in_lo, a.B, a.H, a.W, cin, bk, dd::HALO_TW, dd::HALO_TH + 2, swizzle_for(bk))))
+      return rc;
+  }
+  switch (sid) {
+    case 0: conv3x3_epi<16, 64, kHaloBK[0]>(epi, simt, sa, m, a, sm_count, st); break;
+    case 1: conv3x3_epi<64, 256, kHaloBK[1]>(epi, simt, sa, m, a, sm_count, st); break;
+    case 2: conv3x3_epi<256, 256, kHaloBK[2]>(epi, simt, sa, m, a, sm_count, st); break;
+    case 3: conv3x3_epi<256, 64, kHaloBK[3]>(epi, simt, sa, m, a, sm_count, st); break;
+    case 4: conv3x3_epi<64, 16, kHaloBK[4]>(epi, simt, sa, m, a, sm_count, st); break;
+    default: return fail(DD_ERR_UNSUPPORTED, "unsupported conv shape");
+  }
+  return DD_OK;
+}
+
 template <int CIN, int COUT, int BK>
 cudaError_t configure_halo_all_epi() {
   using C = dd::HaloCfg<CIN, COUT, BK>;
@@ -217,14 +265,6 @@ cudaError_t configure_all_kernels() {
   return configure_gen<64>();
 }
 
-template <int CIN, int COUT, int EPI>
-cudaError_t launch_simt(const dd::SimtArgs& a, cudaStream_t st) {
-  constexpr int CO_T = COUT < 64 ? COUT : 64;
-  dim3 grid(a.c.num_tiles, COUT / CO_T);
-  dd::conv3x3_simt_kernel<CIN, COUT, EPI><<<grid, 256, 0, st>>>(a);
-  return cudaGetLastError();
-}
-
 struct ConvLayer {
   int sid = -1;
   __half* w_hi = nullptr;
@@ -240,7 +280,8 @@ struct Raw {
   std::vector<int64_t> shape;
 };
 
-// One producer convolution (neck / FPN): eval-BN folded into the weights (scale) and `shift`.
+// One layer on the convgen_wgmma_kernel path: a producer convolution (neck / FPN / backbone; eval-BN folded into the
+// weights and `shift`) or a Linear (taps = 1, `shift` = its bias, zeros if it has none).
 struct GenLayer {
   int cin = 0, cout = 0, taps = 1, nt = 256, relu = 1, shuffle = 0;
   int stride = 1, add_first = 0;
@@ -249,31 +290,21 @@ struct GenLayer {
   float* shift = nullptr;
   float wscale = 1.f;
   CUtensorMap mb_hi, mb_lo;
-  bool alt = false;          // cout divisible by 256 and 192: run_gen picks the width whose last wave wastes least
+  bool alt = false;          // cout divisible by 256 and 192: launch_gen picks the width whose last wave wastes least
   CUtensorMap mb_hi_alt, mb_lo_alt;  // boxes of 192 rows
 };
 struct Planes {
   __half* hi = nullptr;
   __half* lo = nullptr;
 };
-struct Gemm {  // Linear layer on the tensor-core GEMM path: W [N][K] as fp16 hi/lo planes
-  int K = 0, N = 0, nt = 256;
-  __half* w_hi = nullptr;
-  __half* w_lo = nullptr;
-  float* bias = nullptr;  // [N] (zeros if the layer has none)
-  float wscale = 1.f;
-  CUtensorMap mb_hi, mb_lo;          // box {32, nt}
-  bool alt = false;                  // N tiles by both 256 and 192: second pair of maps for the other width
-  CUtensorMap mb_hi_alt, mb_lo_alt;  // box {32, 192}
-};
 struct SwinBlockW {
   float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr, *table = nullptr;
-  Gemm qkv, proj, ffn1, ffn2;
+  GenLayer qkv, proj, ffn1, ffn2;
 };
 struct SwinStageW {
   std::vector<SwinBlockW> blocks;
   float *out_g = nullptr, *out_b = nullptr, *dn_g = nullptr, *dn_b = nullptr;
-  Gemm reduction;
+  GenLayer reduction;
 };
 struct Backbone {
   bool enabled = false, ready = false;
@@ -319,7 +350,7 @@ struct DwLayer {
 };
 struct MpBlockW {
   float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
-  Gemm qkv, proj, fc1, fc2;
+  GenLayer qkv, proj, fc1, fc2;
 };
 struct MpEncoderW {
   DwLayer cpe;              // ConvPosEnc, shared by the encoder's layers
@@ -429,6 +460,11 @@ struct dd_engine {
 };
 
 namespace {
+
+int launched(dd_engine* e, const char* what) {
+  e->launches++;
+  return check_launch(what);
+}
 
 constexpr float kActScale = 16.f;  // power-of-two pre-scale of conv inputs before the fp16 split
 constexpr float kXScale = 1.f;     // the raw latent keeps scale 1 (random-init trajectories reach |x| ~ 5e2)
@@ -728,14 +764,10 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
              float* stats_partial, __half* out_hi, __half* out_lo, cudaStream_t st, int f8 = 0) {
   const Geom g = geom_of(e->cfg);
   ConvLayer& L = e->L[layer];
-  const ShapeInfo s = kShapes[L.sid];
   dd::ConvArgs a;
   a.B = g.B;
   a.H = g.h;
   a.W = g.w;
-  a.tiles_x = g.tiles_x;
-  a.tiles_y = g.tiles_y;
-  a.num_tiles = g.tiles;
   a.bias = L.bias;
   a.acc_scale = 1.f / (in_scale * L.wscale);
   a.y32 = y32;
@@ -745,73 +777,20 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
   a.out_a8 = a.out_l8 = nullptr;
   if (f8 & kF8Out) {
     a.out_a8 = reinterpret_cast<uint8_t*>(out_lo);
-    a.out_l8 = a.out_a8 + static_cast<size_t>(g.B) * g.P * kShapes[e->L[layer].sid].cout;
+    a.out_l8 = a.out_a8 + static_cast<size_t>(g.B) * g.P * kShapes[L.sid].cout;
   }
   a.split_scale = kActScale;
   a.status = e->status;
-  cudaError_t err = cudaSuccess;
-  e->launches++;
-  int which = -1;
-  for (int i = 0; i < 4; ++i)
-    if (stats_partial == e->stats[i]) which = i;
-  if (which >= 0) e->stats_tiles_img[which] = g.tiles_img;
-  const bool use_tc = !(e->cfg.flags & DD_FLAG_SIMT_CONV);
-  if (use_tc) {  // tile geometry of the tensor-core kernel
-    a.tiles_x = (g.w + dd::HALO_TW - 1) / dd::HALO_TW;
-    a.tiles_y = (g.h + dd::HALO_TH - 1) / dd::HALO_TH;
-    a.num_tiles = a.tiles_x * a.tiles_y * g.B;
-    if (which >= 0) e->stats_tiles_img[which] = a.tiles_x * a.tiles_y;
-  }
-  if (f8 && !use_tc) return fail(DD_ERR_INVALID, "fp8-correction planes need the tensor-core kernel");
-  if (!use_tc) {
-    dd::SimtArgs sa;
-    sa.in_hi = in_hi;
-    sa.in_lo = in_lo;
-    sa.in_inv_scale = 1.f / in_scale;
-    sa.w = L.w_simt;
-    sa.c = a;
-#define SIMT_CASE(ID, CI, CO)                                                           \
-  case ID:                                                                              \
-    err = (epi == dd::EPI_F32_STATS) ? launch_simt<CI, CO, dd::EPI_F32_STATS>(sa, st)   \
-          : (epi == dd::EPI_SPLIT)   ? launch_simt<CI, CO, dd::EPI_SPLIT>(sa, st)       \
-                                     : launch_simt<CI, CO, dd::EPI_F32>(sa, st);        \
-    break;
-    switch (L.sid) {
-      SIMT_CASE(0, 16, 64)
-      SIMT_CASE(1, 64, 256)
-      SIMT_CASE(2, 256, 256)
-      SIMT_CASE(3, 256, 64)
-      SIMT_CASE(4, 64, 16)
-    }
-#undef SIMT_CASE
-  } else {
-    CUtensorMap ma_hi, ma_lo;
-    int rc;
-    const int hbk = kHaloBK[L.sid];
-    if ((rc = make_strip_map(&ma_hi, in_hi, g.B, g.h, g.w, s.cin, hbk))) return rc;
-    if ((rc = make_strip_map(&ma_lo, in_lo, g.B, g.h, g.w, s.cin, hbk))) return rc;
-    if (f8) return fail(DD_ERR_INVALID, "fp8-correction planes are not supported by the sm_90a kernels");
-    {
-#define HALO_CASE(ID, CI, CO, BK)                                                                                   \
-  case ID:                                                                                                          \
-    err = (epi == dd::EPI_F32_STATS)                                                                                \
-              ? launch_halo<CI, CO, BK, dd::EPI_F32_STATS>(ma_hi, ma_lo, L.mh_hi, L.mh_lo, a, e->sm_count, st)      \
-          : (epi == dd::EPI_SPLIT)                                                                                  \
-              ? launch_halo<CI, CO, BK, dd::EPI_SPLIT>(ma_hi, ma_lo, L.mh_hi, L.mh_lo, a, e->sm_count, st)          \
-              : launch_halo<CI, CO, BK, dd::EPI_F32>(ma_hi, ma_lo, L.mh_hi, L.mh_lo, a, e->sm_count, st);           \
-    break;
-      switch (L.sid) {
-        HALO_CASE(0, 16, 64, 16)
-        HALO_CASE(1, 64, 256, 32)
-        HALO_CASE(2, 256, 256, 32)
-        HALO_CASE(3, 256, 64, 32)
-        HALO_CASE(4, 64, 16, 32)
-      }
-#undef HALO_CASE
-    }
-  }
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(err));
-  return DD_OK;
+  const bool simt = (e->cfg.flags & DD_FLAG_SIMT_CONV) != 0;
+  if (f8)
+    return fail(DD_ERR_INVALID, simt ? "fp8-correction planes need the tensor-core kernel"
+                                     : "fp8-correction planes are not supported by the sm_90a kernels");
+  int rc;
+  if ((rc = launch_conv3x3(L.sid, epi, simt, a, in_hi, in_lo, in_scale, L.w_simt, L.mh_hi, L.mh_lo, e->sm_count, st)))
+    return rc;
+  for (int i = 0; i < 4; ++i)  // the GroupNorm finalize sums this kernel's tiles
+    if (stats_partial == e->stats[i]) e->stats_tiles_img[i] = a.tiles_x * a.tiles_y;
+  return launched(e, "conv3x3");
 }
 
 int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st, const float* ring = nullptr, int ring_per_img = 0) {
@@ -819,10 +798,7 @@ int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st, const f
   const double inv = 1.0 / (static_cast<double>(g.P) * (channels / 4));
   dd::gn_finalize_kernel<<<g.B * 4, 256, 0, st>>>(e->stats[which], e->stats_tiles_img[which], ring, ring_per_img, inv,
                                                    1e-5f, e->mr[which]);
-  e->launches++;
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("gn_finalize: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launched(e, "gn_finalize");
 }
 
 template <int C, int COND>
@@ -866,10 +842,7 @@ int run_apply(dd_engine* e, int which, const float* temb, int temb_bstride, __ha
     dim3 grid((g.P + PPB - 1) / PPB, g.B);
     dd::gn_apply_split_kernel<C, COND><<<grid, 256, 0, st>>>(a);
   }
-  e->launches++;
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("gn_apply: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launched(e, "gn_apply");
 }
 
 bool fold_active(const dd_engine* e) {
@@ -904,9 +877,7 @@ int run_fold(dd_engine* e, cudaStream_t st) {
   e->stats_tiles_img[2] = a.tiles_x * a.tiles_y;
   const int grid = std::min(a.num_tiles, e->sm_count);
   dd::conv5x5_fold_kernel<<<grid, dd::F5::THREADS, dd::F5::SMEM_BYTES, st>>>(m_hi, m_lo, a);
-  e->launches++;
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv5x5_fold: ") + cudaGetErrorString(err));
+  if ((rc = launched(e, "conv5x5_fold"))) return rc;
   dd::RingArgs r;
   r.H = g.h;
   r.W = g.w;
@@ -921,10 +892,7 @@ int run_fold(dd_engine* e, cudaStream_t st) {
   r.y32 = e->Y;
   r.ring_partial = e->stats[3];
   dd::ring_fix_kernel<<<dim3(r.blocks_per_img, g.B), 256, dd::RING_SMEM, st>>>(r);
-  e->launches++;
-  err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("ring_fix: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launched(e, "ring_fix");
 }
 
 int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st);
@@ -996,34 +964,23 @@ int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st) 
   f.status = e->status;
   dim3 grid((g.P * 4 + 255) / 256, g.B);
   dd::gn_relu_ddim_kernel<<<grid, 256, 0, st>>>(f);
-  e->launches++;
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("gn_relu_ddim: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launched(e, "gn_relu_ddim");
 }
 
+// The layout changes and the latent split leave counting their launch to their callers.
 int transpose_in(const float* nchw, float* nhwc, int B, int C, int P, cudaStream_t st) {
   dim3 grid((P + 31) / 32, (C + 31) / 32, B), block(32, 8);
   dd::nchw_to_nhwc_kernel<<<grid, block, 0, st>>>(nchw, nhwc, C, P);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("nchw_to_nhwc: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return check_launch("nchw_to_nhwc");
 }
 int transpose_out(const float* nhwc, float* nchw, int B, int C, int P, cudaStream_t st) {
   dim3 grid((P + 31) / 32, (C + 31) / 32, B), block(32, 8);
   dd::nhwc_to_nchw_kernel<<<grid, block, 0, st>>>(nhwc, nchw, C, P);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("nhwc_to_nchw: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return check_launch("nhwc_to_nchw");
 }
 int split_planes(dd_engine* e, const float* x, __half* hi, __half* lo, size_t n, float scale, cudaStream_t st) {
-  const size_t n4 = n / 4;
-  int blocks = static_cast<int>((n4 + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  dd::split_planes_kernel<<<blocks, 256, 0, st>>>(x, hi, lo, n4, scale, e->status);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("split_planes: ") + cudaGetErrorString(err));
-  return DD_OK;
+  dd::split_planes_kernel<<<grid_of(n / 4), 256, 0, st>>>(x, hi, lo, n / 4, scale, e->status);
+  return check_launch("split_planes");
 }
 
 int run_decoder(dd_engine* e, float* logit, float* depth, cudaStream_t st) {
@@ -1041,10 +998,7 @@ int run_decoder(dd_engine* e, float* logit, float* depth, cudaStream_t st) {
   a.eps = 1e-6f;
   dim3 grid((2 * g.w + dd::DEC_TW - 1) / dd::DEC_TW, (2 * g.h + dd::DEC_TH - 1) / dd::DEC_TH, g.B);
   dd::decoder_kernel<<<grid, 256, dd::DEC_SMEM, st>>>(a);
-  e->launches++;
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("decoder: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launched(e, "decoder");
 }
 
 int bind_workspace(dd_engine* e, void* ws, size_t bytes) {
@@ -1081,22 +1035,12 @@ int pack_layer(dd_engine* e, ConvLayer& L, const float* w, const float* b, int c
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_lo), n * 2))) return rc;
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_simt), n * 4))) return rc;
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.bias), cout * 4))) return rc;
-  CUDA_TRY(cudaMemsetAsync(scratch_dev, 0, 4, st));
-  dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(w, static_cast<int>(n), scratch_dev);
-  float amax = 0.f;
-  CUDA_TRY(cudaMemcpyAsync(&amax, scratch_dev, 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  // largest power of two with amax * scale < 2^15: hi stays finite, lo = O(2^4) stays normal
-  float scale = 1.f;
-  if (amax > 0.f && isfinite(amax)) scale = exp2f(floorf(log2f(32768.f / amax)) - 1.f);
-  L.wscale = scale;
-  dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, L.w_hi, L.w_lo, L.w_simt, cout, cin, scale);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = split_scale_of(w, n, scratch_dev, st, &L.wscale))) return rc;
+  dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, L.w_hi, L.w_lo, L.w_simt, cout, cin, L.wscale);
+  if ((rc = check_launch("pack_conv_weight"))) return rc;
   CUDA_TRY(cudaMemcpyAsync(L.bias, b, cout * 4, cudaMemcpyDeviceToDevice, st));
-  const ShapeInfo s = kShapes[L.sid];
-  if ((rc = make_w_map(&L.mh_hi, L.w_hi, cout, cin, kHaloBK[L.sid]))) return rc;
-  if ((rc = make_w_map(&L.mh_lo, L.w_lo, cout, cin, kHaloBK[L.sid]))) return rc;
-  return DD_OK;
+  if ((rc = make_weight_map(&L.mh_hi, L.w_hi, cout, cin, 9, kHaloBK[L.sid], cout))) return rc;
+  return make_weight_map(&L.mh_lo, L.w_lo, cout, cin, 9, kHaloBK[L.sid], cout);
 }
 
 
@@ -1125,17 +1069,12 @@ int bn_fold(dd_engine* e, const std::string& bn, int ch, std::vector<float>& sca
   return DD_OK;
 }
 
-// conv weight key `wkey` ([cout][cin][k][k], or ConvT [cin][co][2][2] when transposed) followed by eval-BN `bnkey`
-// (folded), or — bnkey empty — by the plain bias `biaskey`.  cin_pad >= cin zero-pads the input-channel axis (RGB -> 32).
-int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::string& bnkey, int cin, int cout_conv,
-             int taps, bool transposed, cudaStream_t st, float* scratch, int cin_pad = 0,
-             const std::string& biaskey = std::string()) {
-  const Raw* w = find(e, wkey);
-  if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
-  const int k = taps == 9 ? 3 : (transposed ? 2 : 1);
-  std::vector<int64_t> want = transposed ? std::vector<int64_t>{cin, cout_conv, 2, 2}
-                                         : std::vector<int64_t>{cout_conv, cin, k, k};
-  if (w->shape != want) return fail(DD_ERR_INVALID, "weight shape mismatch: " + wkey);
+// Pack one layer of the convgen_wgmma_kernel path, a producer conv or a Linear, from its raw weight w ([cout][cin]
+// [taps], or ConvT [cin][co][2][2] when transposed) followed by eval-BN `bnkey` (folded), or — bnkey empty — by the
+// plain bias `biaskey` (empty: none).  cin_pad >= cin zero-pads the input-channel axis (RGB -> 64).  `name` labels errors.
+int pack_gen_weights(dd_engine* e, GenLayer& L, const float* w, const std::string& name, const std::string& bnkey,
+                     const std::string& biaskey, int cin, int cout_conv, int taps, bool transposed, int cin_pad,
+                     cudaStream_t st, float* scratch) {
   std::vector<float> scale(cout_conv, 1.f), shift(cout_conv, 0.f);
   int rc;
   if (!bnkey.empty()) {
@@ -1153,7 +1092,8 @@ int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::stri
   L.shuffle = transposed ? 1 : 0;
   L.relu = 1;
   // N tile: the width in {256, 192, 128} that wastes the fewest padded columns (ties -> wider); 64 for cout <= 64.
-  // A last tile wider than the remaining channels reads zero weight rows (TMA out-of-bounds fill), the epilogue drops them.
+  // A last tile wider than the remaining channels reads zero weight rows (TMA out-of-bounds fill), the epilogue drops
+  // them; partial K chunks are completed with zeros the same way (MPViT widths: 216, 288, 648, 864 ...).
   L.nt = 64;
   if (L.cout > 64) {
     int best = 1 << 30;
@@ -1162,41 +1102,64 @@ int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::stri
       if (padded < best) { best = padded; L.nt = nt; }
     }
   }
-  if (L.cout % 8 != 0 || cp % 8 != 0) return fail(DD_ERR_UNSUPPORTED, "producer conv channels must be multiples of 8: " + wkey);
+  if (L.cout % 8 != 0 || cp % 8 != 0) return fail(DD_ERR_UNSUPPORTED, "channels must be multiples of 8: " + name);
   const int cout_pad = (L.cout + L.nt - 1) / L.nt * L.nt;
   const size_t n = static_cast<size_t>(L.cout) * cp * L.taps;
-  float *d_scale = nullptr;
+  float* d_scale = nullptr;  // per output channel; nullptr: 1
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_hi), n * 2))) return rc;
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_lo), n * 2))) return rc;
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.shift), cout_pad * 4))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&d_scale), cout_conv * 4))) return rc;
+  if (!bnkey.empty()) {
+    if ((rc = dev_alloc(e, reinterpret_cast<void**>(&d_scale), cout_conv * 4))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(d_scale, scale.data(), cout_conv * 4, cudaMemcpyHostToDevice, st));
+  }
   if (cp != cin) {
     CUDA_TRY(cudaMemsetAsync(L.w_hi, 0, n * 2, st));
     CUDA_TRY(cudaMemsetAsync(L.w_lo, 0, n * 2, st));
   }
-  CUDA_TRY(cudaMemcpyAsync(d_scale, scale.data(), cout_conv * 4, cudaMemcpyHostToDevice, st));
   std::vector<float> shift_full(cout_pad, 0.f);
   for (int i = 0; i < L.cout; ++i) shift_full[i] = shift[i % cout_conv];
   CUDA_TRY(cudaMemcpyAsync(L.shift, shift_full.data(), cout_pad * 4, cudaMemcpyHostToDevice, st));
   const int nraw = static_cast<int>(static_cast<size_t>(cout_conv) * cin * (transposed ? 4 : taps));
-  CUDA_TRY(cudaMemsetAsync(scratch, 0, 4, st));
-  dd::absmax_scaled_kernel<<<absmax_grid(nraw), 256, 0, st>>>(w->ptr, d_scale, nraw, cin * taps, cout_conv, transposed ? 1 : 0, scratch);
-  float amax = 0.f;
-  CUDA_TRY(cudaMemcpyAsync(&amax, scratch, 4, cudaMemcpyDeviceToHost, st));
+  if ((rc = split_scale(scratch, st, &L.wscale, [&] {
+         dd::absmax_scaled_kernel<<<absmax_grid(nraw), 256, 0, st>>>(w, d_scale, nraw, cin * L.taps, cout_conv,
+                                                                     L.shuffle, scratch);
+       })))
+    return rc;
+  dd::pack_gen_weight_kernel<<<256, 256, 0, st>>>(w, d_scale, L.w_hi, L.w_lo, L.cout, cin, L.taps, L.shuffle, L.wscale, cp);
+  if ((rc = check_launch("pack_gen_weight"))) return rc;
   CUDA_TRY(cudaStreamSynchronize(st));
-  L.wscale = (amax > 0.f && isfinite(amax)) ? exp2f(floorf(log2f(32768.f / amax)) - 1.f) : 1.f;
-  dd::pack_gen_weight_kernel<<<256, 256, 0, st>>>(w->ptr, d_scale, L.w_hi, L.w_lo, L.cout, cin, L.taps,
-                                                  transposed ? 1 : 0, L.wscale, cp);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaStreamSynchronize(st));
-  if ((rc = make_wgen_map(&L.mb_hi, L.w_hi, L.cout, cp, L.taps, L.nt))) return rc;
-  if ((rc = make_wgen_map(&L.mb_lo, L.w_lo, L.cout, cp, L.taps, L.nt))) return rc;
+  if ((rc = make_weight_map(&L.mb_hi, L.w_hi, L.cout, cp, L.taps, dd::GEN_BK, L.nt))) return rc;
+  if ((rc = make_weight_map(&L.mb_lo, L.w_lo, L.cout, cp, L.taps, dd::GEN_BK, L.nt))) return rc;
+  // cout divisible by 256 and 192: launch_gen may pick the width whose last wave wastes least
   L.alt = (L.nt == 256 && L.cout % 256 == 0 && L.cout % 192 == 0 && !L.shuffle);
   if (L.alt) {
-    if ((rc = make_wgen_map(&L.mb_hi_alt, L.w_hi, L.cout, cp, L.taps, 192))) return rc;
-    if ((rc = make_wgen_map(&L.mb_lo_alt, L.w_lo, L.cout, cp, L.taps, 192))) return rc;
+    if ((rc = make_weight_map(&L.mb_hi_alt, L.w_hi, L.cout, cp, L.taps, dd::GEN_BK, 192))) return rc;
+    if ((rc = make_weight_map(&L.mb_lo_alt, L.w_lo, L.cout, cp, L.taps, dd::GEN_BK, 192))) return rc;
   }
   return DD_OK;
+}
+
+// conv weight key `wkey` ([cout][cin][k][k], or ConvT [cin][co][2][2] when transposed); see pack_gen_weights
+int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::string& bnkey, int cin, int cout_conv,
+             int taps, bool transposed, cudaStream_t st, float* scratch, int cin_pad = 0,
+             const std::string& biaskey = std::string()) {
+  const Raw* w = find(e, wkey);
+  if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
+  const int k = taps == 9 ? 3 : (transposed ? 2 : 1);
+  std::vector<int64_t> want = transposed ? std::vector<int64_t>{cin, cout_conv, 2, 2}
+                                         : std::vector<int64_t>{cout_conv, cin, k, k};
+  if (w->shape != want) return fail(DD_ERR_INVALID, "weight shape mismatch: " + wkey);
+  return pack_gen_weights(e, L, w->ptr, wkey, bnkey, biaskey, cin, cout_conv, taps, transposed, cin_pad, st, scratch);
+}
+
+// nn.Linear: weight key `wkey` [N][K], bias key `bkey` (empty: none).  run_gemm supplies the activation.
+int pack_linear(dd_engine* e, GenLayer& L, const std::string& wkey, const std::string& bkey, int N, int K,
+                cudaStream_t st, float* scratch) {
+  const Raw* w = find(e, wkey);
+  if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
+  if (w->shape != std::vector<int64_t>{N, K}) return fail(DD_ERR_INVALID, "weight shape mismatch: " + wkey);
+  return pack_gen_weights(e, L, w->ptr, wkey, "", bkey, K, N, 1, false, 0, st, scratch);
 }
 
 int pack_producers(dd_engine* e, cudaStream_t st, float* scratch) {
@@ -1224,36 +1187,31 @@ int pack_producers(dd_engine* e, cudaStream_t st, float* scratch) {
 }
 
 template <int NT>
-cudaError_t launch_gen(int grid, cudaStream_t st, const CUtensorMap& m0h, const CUtensorMap& m0l, const CUtensorMap& m1h,
-                       const CUtensorMap& m1l, const CUtensorMap& bh, const CUtensorMap& bl, const dd::GenConvArgs& a) {
-  dd::convgen_wgmma_kernel<NT><<<grid, dd::GenCfg<NT>::THREADS, dd::GenCfg<NT>::SMEM_BYTES, st>>>(m0h, m0l, m1h, m1l, bh, bl, a);
-  return cudaGetLastError();
-}
-int gen_grid(const dd_engine* e, int m_tiles, int n_tiles) { return std::min(m_tiles * n_tiles, e->sm_count); }
-cudaError_t launch_gen_nt(int nt, int grid, cudaStream_t st, const CUtensorMap& m0h, const CUtensorMap& m0l,
-                          const CUtensorMap& m1h, const CUtensorMap& m1l, const CUtensorMap& bh, const CUtensorMap& bl,
-                          const dd::GenConvArgs& a) {
-  switch (nt) {
-    case 256: return launch_gen<256>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-    case 192: return launch_gen<192>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-    case 128: return launch_gen<128>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-    default: return launch_gen<64>(grid, st, m0h, m0l, m1h, m1l, bh, bl, a);
-  }
+void convgen_kernel(int grid, cudaStream_t st, const CUtensorMap* m, const dd::GenConvArgs& a) {
+  dd::convgen_wgmma_kernel<NT><<<grid, dd::GenCfg<NT>::THREADS, dd::GenCfg<NT>::SMEM_BYTES, st>>>(m[0], m[1], m[2], m[3],
+                                                                                                 m[4], m[5], a);
 }
 
-// H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.
-int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
-            float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
-            int ld_out = 0, int ch_off = 0) {
-  const int B = e->cfg.batch;
+// Output grid of one convgen_wgmma_kernel launch: B images of H x W pixels, the first m_valid of them real (0: all).
+// A stride-2 layer reads its sources on the src_h x src_w grid.
+struct GenGrid {
+  int B, H, W, m_valid, src_h, src_w;
+};
+
+// Every launch of layer L on convgen_wgmma_kernel (producer convs and Linears): activation act, sources a0 (c0
+// channels) and a1 (c1, concatenated after a0; c1 = 0: none), outputs y32 (fp32, + add32) and / or the split planes
+// *out with row width ld_out (0: L.cout) from channel ch_off on.
+int launch_gen(dd_engine* e, const GenLayer& L, int act, const GenGrid& g, const Planes& a0, int c0, const Planes& a1,
+               int c1, float* y32, const float* add32, const Planes* out, int ld_out, int ch_off, cudaStream_t st) {
+  if (c0 + c1 != L.cin) return fail(DD_ERR_INVALID, "producer conv: source channels do not match the layer");
   dd::GenConvArgs a;
-  a.B = B;
-  a.H = H;
-  a.W = W;
-  a.tiles_x = (W + dd::TILE_W - 1) / dd::TILE_W;
-  a.tiles_y = (H + dd::TILE_H - 1) / dd::TILE_H;
-  a.m_tiles = a.tiles_x * a.tiles_y * B;
-  // wave quantisation (as in run_gemm): with few M tiles pick the N-tile width whose last wave wastes least — the
+  a.B = g.B;
+  a.H = g.H;
+  a.W = g.W;
+  a.tiles_x = (g.W + dd::TILE_W - 1) / dd::TILE_W;
+  a.tiles_y = (g.H + dd::TILE_H - 1) / dd::TILE_H;
+  a.m_tiles = a.tiles_x * a.tiles_y * g.B;
+  // wave quantisation: with few M tiles pick the N-tile width whose last wave wastes least — deep Swin stages, and the
   // level-2 fusion conv of the HAHI neck (768 channels, 30 tile pairs) runs 2 waves of 192 columns instead of 2 of 256
   int nt = L.nt;
   if (L.alt) {
@@ -1271,8 +1229,8 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
   a.ch_off = ch_off;
   a.shift = L.shift;
   a.acc_scale = 1.f / (kProdScale * L.wscale);
-  a.relu = L.relu;
-  a.m_valid = 0;
+  a.relu = act;
+  a.m_valid = g.m_valid;
   a.stride = L.stride;
   a.add_first = L.add_first;
   a.shuffle = L.shuffle;
@@ -1282,30 +1240,37 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
   a.out_lo = out ? out->lo : nullptr;
   a.split_scale = kProdScale;
   a.status = e->status;
-  if (c0 + c1 != L.cin) return fail(DD_ERR_INVALID, "producer conv: source channels do not match the layer");
-  CUtensorMap m0h, m0l, m1h, m1l;
-  int rc;
-  if (L.stride == 1) {
-    if ((rc = make_act_map(&m0h, a0.hi, B, H, W, c0, dd::GEN_BK))) return rc;
-    if ((rc = make_act_map(&m0l, a0.lo, B, H, W, c0, dd::GEN_BK))) return rc;
-  } else {
-    if ((rc = make_act_map_strided(&m0h, a0.hi, B, src_h, src_w, c0, dd::GEN_BK, L.stride))) return rc;
-    if ((rc = make_act_map_strided(&m0l, a0.lo, B, src_h, src_w, c0, dd::GEN_BK, L.stride))) return rc;
-  }
-  if (c1 > 0) {
-    if ((rc = make_act_map(&m1h, a1.hi, B, H, W, c1, dd::GEN_BK))) return rc;
-    if ((rc = make_act_map(&m1l, a1.lo, B, H, W, c1, dd::GEN_BK))) return rc;
-  } else {
-    m1h = m0h;
-    m1l = m0l;
-  }
-  const int grid = gen_grid(e, a.m_tiles, a.n_tiles);
   const bool use_alt = nt != L.nt;
-  const cudaError_t err = launch_gen_nt(nt, grid, st, m0h, m0l, m1h, m1l, use_alt ? L.mb_hi_alt : L.mb_hi,
-                                        use_alt ? L.mb_lo_alt : L.mb_lo, a);
-  e->launches++;
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("convgen launch: ") + cudaGetErrorString(err));
-  return DD_OK;
+  CUtensorMap m[6];  // sources 0 and 1 (hi, lo), weights (hi, lo)
+  const int sh = L.stride == 1 ? g.H : g.src_h, sw = L.stride == 1 ? g.W : g.src_w;
+  int rc;
+  if ((rc = make_act_map(&m[0], a0.hi, g.B, sh, sw, c0, dd::GEN_BK, L.stride))) return rc;
+  if ((rc = make_act_map(&m[1], a0.lo, g.B, sh, sw, c0, dd::GEN_BK, L.stride))) return rc;
+  if (c1 > 0) {
+    if ((rc = make_act_map(&m[2], a1.hi, g.B, g.H, g.W, c1, dd::GEN_BK))) return rc;
+    if ((rc = make_act_map(&m[3], a1.lo, g.B, g.H, g.W, c1, dd::GEN_BK))) return rc;
+  } else {
+    m[2] = m[0];
+    m[3] = m[1];
+  }
+  m[4] = use_alt ? L.mb_hi_alt : L.mb_hi;
+  m[5] = use_alt ? L.mb_lo_alt : L.mb_lo;
+  const int grid = std::min(a.m_tiles * a.n_tiles, e->sm_count);
+  switch (nt) {
+    case 256: convgen_kernel<256>(grid, st, m, a); break;
+    case 192: convgen_kernel<192>(grid, st, m, a); break;
+    case 128: convgen_kernel<128>(grid, st, m, a); break;
+    default: convgen_kernel<64>(grid, st, m, a); break;
+  }
+  return launched(e, "convgen");
+}
+
+// H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.
+int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
+            float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
+            int ld_out = 0, int ch_off = 0) {
+  return launch_gen(e, L, L.relu, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, y32, add32, out, ld_out, ch_off,
+                    st);
 }
 
 // ------------------------------------------------------------------------------------------------ ResNet backbone
@@ -1345,14 +1310,11 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
   const int B = e->cfg.batch;
   {
     const size_t n = static_cast<size_t>(B) * r.H * r.W * dd::GEN_BK;
-    int blocks = static_cast<int>((n + 255) / 256);
-    if (blocks > 132 * 16) blocks = 132 * 16;
-    dd::rgb_to_planes_kernel<<<blocks, 256, 0, st>>>(rgb, r.IN.hi, r.IN.lo, B, r.H * r.W, kProdScale, e->status);
-    e->launches++;
-    CUDA_TRY(cudaGetLastError());
+    dd::rgb_to_planes_kernel<<<grid_of(n), 256, 0, st>>>(rgb, r.IN.hi, r.IN.lo, B, r.H * r.W, kProdScale, e->status);
   }
-  const Planes none;
   int rc;
+  if ((rc = launched(e, "rgb_to_planes"))) return rc;
+  const Planes none;
   Planes src = r.IN;
   int src_c = dd::GEN_BK, src_h = r.H, src_w = r.W;
   for (int s = 0; s < 4; ++s) {
@@ -1390,6 +1352,7 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
 
 // ------------------------------------------------------------------------------------------------ Swin backbone
 constexpr float kTokScale = 16.f;  // fp16-split pre-scale of token activations (LayerNorm / GELU / attention outputs)
+static_assert(kTokScale == kProdScale, "run_gemm reads token planes at the producers' split scale");
 
 int copy_param(dd_engine* e, const std::string& key, size_t n, float** out, cudaStream_t st) {
   const Raw* r = find(e, key);
@@ -1400,54 +1363,6 @@ int copy_param(dd_engine* e, const std::string& key, size_t n, float** out, cuda
   int rc;
   if ((rc = dev_alloc(e, reinterpret_cast<void**>(out), n * 4))) return rc;
   CUDA_TRY(cudaMemcpyAsync(*out, r->ptr, n * 4, cudaMemcpyDeviceToDevice, st));
-  return DD_OK;
-}
-
-int pack_gemm(dd_engine* e, Gemm& G, const std::string& wkey, const std::string& bkey, int N, int K, cudaStream_t st,
-              float* scratch) {
-  const Raw* w = find(e, wkey);
-  if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
-  if (w->shape != std::vector<int64_t>{N, K}) return fail(DD_ERR_INVALID, "weight shape mismatch: " + wkey);
-  G.K = K;
-  G.N = N;
-  // N tile as in pack_gen: fewest padded columns among {256, 192, 128}, 64 for N <= 64; partial K chunks / N tiles are
-  // completed with zeros by TMA (Swin-L: every N is a multiple of 256 or 192, every K of 64; MPViT: 216, 288, 648, 864 ...)
-  G.nt = 64;
-  if (N > 64) {
-    int best = 1 << 30;
-    for (int nt : {256, 192, 128}) {
-      const int padded = (N + nt - 1) / nt * nt;
-      if (padded < best) { best = padded; G.nt = nt; }
-    }
-  }
-  if (N % 8 != 0 || K % 8 != 0) return fail(DD_ERR_UNSUPPORTED, "linear layer widths must be multiples of 8: " + wkey);
-  const int n_pad = (N + G.nt - 1) / G.nt * G.nt;
-  const size_t n = static_cast<size_t>(N) * K;
-  int rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&G.w_hi), n * 2))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&G.w_lo), n * 2))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&G.bias), n_pad * 4))) return rc;
-  CUDA_TRY(cudaMemsetAsync(G.bias, 0, n_pad * 4, st));
-  if (!bkey.empty()) {
-    const Raw* b = find(e, bkey);
-    if (!b) return fail(DD_ERR_INVALID, "missing weights: " + bkey);
-    CUDA_TRY(cudaMemcpyAsync(G.bias, b->ptr, N * 4, cudaMemcpyDeviceToDevice, st));
-  }
-  CUDA_TRY(cudaMemsetAsync(scratch, 0, 4, st));
-  dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(w->ptr, static_cast<int>(n), scratch);
-  float amax = 0.f;
-  CUDA_TRY(cudaMemcpyAsync(&amax, scratch, 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  G.wscale = (amax > 0.f && isfinite(amax)) ? exp2f(floorf(log2f(32768.f / amax)) - 1.f) : 1.f;
-  dd::pack_gen_weight_kernel<<<256, 256, 0, st>>>(w->ptr, nullptr, G.w_hi, G.w_lo, N, K, 1, 0, G.wscale);
-  CUDA_TRY(cudaGetLastError());
-  if ((rc = make_wgen_map(&G.mb_hi, G.w_hi, N, K, 1, G.nt))) return rc;
-  if ((rc = make_wgen_map(&G.mb_lo, G.w_lo, N, K, 1, G.nt))) return rc;
-  G.alt = (G.nt == 256 && N % 256 == 0 && N % 192 == 0);
-  if (G.alt) {
-    if ((rc = make_wgen_map(&G.mb_hi_alt, G.w_hi, N, K, 1, 192))) return rc;
-    if ((rc = make_wgen_map(&G.mb_lo_alt, G.w_lo, N, K, 1, 192))) return rc;
-  }
   return DD_OK;
 }
 
@@ -1471,10 +1386,10 @@ int pack_backbone(dd_engine* e, cudaStream_t st, float* scratch) {
       if ((rc = copy_param(e, bp + "norm2.weight", C, &W.ln2_g, st))) return rc;
       if ((rc = copy_param(e, bp + "norm2.bias", C, &W.ln2_b, st))) return rc;
       if ((rc = copy_param(e, bp + "attn.w_msa.relative_position_bias_table", static_cast<size_t>(169) * b.heads[s], &W.table, st))) return rc;
-      if ((rc = pack_gemm(e, W.qkv, bp + "attn.w_msa.qkv.weight", bp + "attn.w_msa.qkv.bias", 3 * C, C, st, scratch))) return rc;
-      if ((rc = pack_gemm(e, W.proj, bp + "attn.w_msa.proj.weight", bp + "attn.w_msa.proj.bias", C, C, st, scratch))) return rc;
-      if ((rc = pack_gemm(e, W.ffn1, bp + "ffn.layers.0.0.weight", bp + "ffn.layers.0.0.bias", 4 * C, C, st, scratch))) return rc;
-      if ((rc = pack_gemm(e, W.ffn2, bp + "ffn.layers.1.weight", bp + "ffn.layers.1.bias", C, 4 * C, st, scratch))) return rc;
+      if ((rc = pack_linear(e, W.qkv, bp + "attn.w_msa.qkv.weight", bp + "attn.w_msa.qkv.bias", 3 * C, C, st, scratch))) return rc;
+      if ((rc = pack_linear(e, W.proj, bp + "attn.w_msa.proj.weight", bp + "attn.w_msa.proj.bias", C, C, st, scratch))) return rc;
+      if ((rc = pack_linear(e, W.ffn1, bp + "ffn.layers.0.0.weight", bp + "ffn.layers.0.0.bias", 4 * C, C, st, scratch))) return rc;
+      if ((rc = pack_linear(e, W.ffn2, bp + "ffn.layers.1.weight", bp + "ffn.layers.1.bias", C, 4 * C, st, scratch))) return rc;
     }
     const std::string np = P + "norm" + std::to_string(s) + ".";
     if ((rc = copy_param(e, np + "weight", C, &S.out_g, st))) return rc;
@@ -1483,7 +1398,7 @@ int pack_backbone(dd_engine* e, cudaStream_t st, float* scratch) {
       const std::string dp = P + "stages." + std::to_string(s) + ".downsample.";
       if ((rc = copy_param(e, dp + "norm.weight", 4 * C, &S.dn_g, st))) return rc;
       if ((rc = copy_param(e, dp + "norm.bias", 4 * C, &S.dn_b, st))) return rc;
-      if ((rc = pack_gemm(e, S.reduction, dp + "reduction.weight", "", 2 * C, 4 * C, st, scratch))) return rc;
+      if ((rc = pack_linear(e, S.reduction, dp + "reduction.weight", "", 2 * C, 4 * C, st, scratch))) return rc;
     }
   }
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -1492,54 +1407,10 @@ int pack_backbone(dd_engine* e, cudaStream_t st, float* scratch) {
 }
 
 // y = act(A[M][K] @ W^T + bias) (+ add32): tokens are laid out as a [ceil(M/16)][16] "image" for the conv kernel
-int run_gemm(dd_engine* e, const Gemm& G, const Planes& A, int M, int act, float* y32, const float* add32,
+int run_gemm(dd_engine* e, const GenLayer& L, const Planes& A, int M, int act, float* y32, const float* add32,
              const Planes* out, cudaStream_t st, int ld_out = 0, int ch_off = 0) {
-  dd::GenConvArgs a;
-  a.B = 1;
-  a.W = 16;
-  a.H = (M + 15) / 16;
-  a.tiles_x = 1;
-  a.tiles_y = (a.H + dd::TILE_H - 1) / dd::TILE_H;
-  a.m_tiles = a.tiles_y;
-  // wave quantisation: with few M tiles (deep Swin stages) pick the N-tile width whose last wave wastes least
-  const int units = a.m_tiles, slots = e->sm_count;
-  int nt = G.nt;
-  if (G.alt) {
-    auto cost = [&](int w) { return ((units * (G.N / w) + slots - 1) / slots) * w; };
-    if (cost(192) < cost(256)) nt = 192;
-  }
-  const CUtensorMap& mbh = (nt == G.nt) ? G.mb_hi : G.mb_hi_alt;
-  const CUtensorMap& mbl = (nt == G.nt) ? G.mb_lo : G.mb_lo_alt;
-  a.n_tiles = (G.N + nt - 1) / nt;
-  a.kc0 = (G.K + dd::GEN_BK - 1) / dd::GEN_BK;
-  a.kc1 = 0;
-  a.c0_ch = G.K;
-  a.taps = 1;
-  a.cout = G.N;
-  a.ld_out = ld_out > 0 ? ld_out : G.N;
-  a.ch_off = ch_off;
-  a.shift = G.bias;
-  a.acc_scale = 1.f / (kTokScale * G.wscale);
-  a.relu = act;
-  a.m_valid = M;
-  a.stride = 1;
-  a.add_first = 0;
-  a.shuffle = 0;
-  a.y32 = y32;
-  a.add32 = add32;
-  a.out_hi = out ? out->hi : nullptr;
-  a.out_lo = out ? out->lo : nullptr;
-  a.split_scale = kTokScale;
-  a.status = e->status;
-  CUtensorMap mh, ml;
-  int rc;
-  if ((rc = make_act_map(&mh, A.hi, 1, a.H, 16, G.K, dd::GEN_BK))) return rc;
-  if ((rc = make_act_map(&ml, A.lo, 1, a.H, 16, G.K, dd::GEN_BK))) return rc;
-  const int grid = gen_grid(e, a.m_tiles, a.n_tiles);
-  const cudaError_t err = launch_gen_nt(nt, grid, st, mh, ml, mh, ml, mbh, mbl, a);
-  e->launches++;
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("gemm launch: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launch_gen(e, L, act, {1, (M + 15) / 16, 16, M, 0, 0}, A, L.cin, Planes(), 0, y32, add32, out, ld_out, ch_off,
+                    st);
 }
 
 int run_ln(dd_engine* e, int C, const float* x, const float* g, const float* b, const Planes& out, int M, float* nchw,
@@ -1552,10 +1423,7 @@ int run_ln(dd_engine* e, int C, const float* x, const float* g, const float* b, 
     case 1536: dd::ln_split_kernel<1536><<<grid, 256, 0, st>>>(x, g, b, out.hi, out.lo, kTokScale, M, nchw, HW, e->status); break;
     default: return fail(DD_ERR_UNSUPPORTED, "LayerNorm width not instantiated");
   }
-  e->launches++;
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("ln_split: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return launched(e, "ln_split");
 }
 
 int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream_t st) {
@@ -1565,10 +1433,9 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
     const int segs = (b.Ws[0] + dd::PE_TOK - 1) / dd::PE_TOK;
     dd::patch_embed_kernel<192><<<segs * b.Hs[0] * B, 192, 0, st>>>(rgb, b.pe_w, b.pe_b, b.pe_g, b.pe_beta, b.X[0], B, b.H,
                                                                      b.W, b.Hs[0], b.Ws[0]);
-    e->launches++;
-    CUDA_TRY(cudaGetLastError());
   }
   int rc;
+  if ((rc = launched(e, "patch_embed"))) return rc;
   for (int s = 0; s < 4; ++s) {
     const int C = b.E << s, H = b.Hs[s], W = b.Ws[s], M = B * H * W, nH = b.heads[s];
     float* x = b.X[s & 1];
@@ -1580,7 +1447,7 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
       if ((rc = run_gemm(e, Wt.qkv, b.AP, M, 0, b.QKV, nullptr, nullptr, st))) return rc;
       dd::AttnArgs aa;
       aa.qkv = b.QKV;
-      aa.qkv_bias = Wt.qkv.bias;
+      aa.qkv_bias = Wt.qkv.shift;
       aa.bias_table = Wt.table;
       aa.out_hi = b.AP.hi;
       aa.out_lo = b.AP.lo;
@@ -1596,8 +1463,7 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
         const int grid = pairs < 2 * e->sm_count ? pairs : 2 * e->sm_count;
         dd::window_attention_wgmma_kernel<<<grid, 128, dd::WAU_SMEM, st>>>(aa, pairs);
       }
-      e->launches++;
-      CUDA_TRY(cudaGetLastError());
+      if ((rc = launched(e, "window_attention"))) return rc;
       if ((rc = run_gemm(e, Wt.proj, b.AP, M, 0, x, x, nullptr, st))) return rc;      // x += proj(attn)
       if ((rc = run_ln(e, C, x, Wt.ln2_g, Wt.ln2_b, b.AP, M, nullptr, 0, st))) return rc;
       if ((rc = run_gemm(e, Wt.ffn1, b.AP, M, 2, nullptr, nullptr, &b.HP, st))) return rc;  // GELU(fc1) -> planes
@@ -1616,8 +1482,7 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
         case 768: dd::merge_ln_split_kernel<768><<<grid, 256, 0, st>>>(x, S.dn_g, S.dn_b, b.AP.hi, b.AP.lo, kTokScale, B, H, W, e->status); break;
         default: return fail(DD_ERR_UNSUPPORTED, "patch merging width not instantiated");
       }
-      e->launches++;
-      CUDA_TRY(cudaGetLastError());
+      if ((rc = launched(e, "merge_ln_split"))) return rc;
       if ((rc = run_gemm(e, S.reduction, b.AP, M2, 0, b.X[(s + 1) & 1], nullptr, nullptr, st))) return rc;
     }
   }
@@ -1627,16 +1492,6 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
 #include "mpvit_host.inc"
 
 // ------------------------------------------------------------------------------------------------ backward
-int launched(dd_engine* e, const char* what) {
-  e->launches++;
-  const cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(err));
-  return DD_OK;
-}
-int grid_of(size_t n, int per_block = 256) {
-  const size_t b = (n + per_block - 1) / per_block;
-  return static_cast<int>(std::max<size_t>(1, std::min<size_t>(b, 132 * 16)));
-}
 
 // GroupNorm `which` (0 ne.1, 1 ne.4, 2 pred.1, 3 pred.4) of the pre-GN output y: its mean / rstd, gamma, beta
 dd::GnBwdArgs gn_args(dd_engine* e, int which, const float* y) {
@@ -1701,10 +1556,9 @@ int run_colsum(dd_engine* e, int C, const float* x, const float* scale, int B, i
 }
 
 template <int TM, int TN>
-cudaError_t launch_wgrad(const dd::WgradArgs& a, int chunks, cudaStream_t st) {
+void launch_wgrad(const dd::WgradArgs& a, int chunks, cudaStream_t st) {
   const dim3 grid(chunks, (a.cout / TM) * (a.cin / TN) * 9);
   dd::wgrad_simt_kernel<TM, TN><<<grid, TM * TN / 16, 0, st>>>(a);
-  return cudaGetLastError();
 }
 
 // Buffers of run_wgrad: the dY split planes [B*H*W][cout] fp16, the split's absmax (zeroed before the call) and scale
@@ -1738,10 +1592,11 @@ int run_wgrad(dd_engine* e, int B, int H, int W, int cout, int cin, const float*
   }
   if (tc) {
     CUtensorMap ah, al, bh, bl;
-    if ((rc = make_wgm_map(&ah, bufs.gp.hi, B, H, W, cout))) return rc;
-    if ((rc = make_wgm_map(&al, bufs.gp.lo, B, H, W, cout))) return rc;
-    if ((rc = make_wgm_map(&bh, x_hi, B, H, W, cin))) return rc;
-    if ((rc = make_wgm_map(&bl, x_lo, B, H, W, cin))) return rc;
+    const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
+    if ((rc = make_nhwc_map(&ah, "wgrad operand", bufs.gp.hi, B, H, W, cout, 64, 64, 1, sw))) return rc;
+    if ((rc = make_nhwc_map(&al, "wgrad operand", bufs.gp.lo, B, H, W, cout, 64, 64, 1, sw))) return rc;
+    if ((rc = make_nhwc_map(&bh, "wgrad operand", x_hi, B, H, W, cin, 64, 64, 1, sw))) return rc;
+    if ((rc = make_nhwc_map(&bl, "wgrad operand", x_lo, B, H, W, cin, 64, 64, 1, sw))) return rc;
     dd::WgmArgs a;
     a.cout = cout;
     a.cin = cin;
@@ -1782,9 +1637,9 @@ int run_wgrad(dd_engine* e, int B, int H, int W, int cout, int cin, const float*
   a.W = W;
   a.chunk = pl.chunk;
   a.partial = bufs.partial;
-  const cudaError_t err = cout == 16 ? launch_wgrad<16, 64>(a, pl.chunks, st) : launch_wgrad<64, 16>(a, pl.chunks, st);
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("wgrad: ") + cudaGetErrorString(err));
-  e->launches++;
+  if (cout == 16) launch_wgrad<16, 64>(a, pl.chunks, st);
+  else launch_wgrad<64, 16>(a, pl.chunks, st);
+  if ((rc = launched(e, "wgrad"))) return rc;
   dd::wgrad_reduce_kernel<<<grid_of(nw), 256, 0, st>>>(bufs.partial, pl.chunks, cout, cin, 0, 1.0, dscale, dw);
   return launched(e, "wgrad_reduce");
 }
@@ -1965,6 +1820,28 @@ int stage_operator_inputs(dd_engine* h, const float* cond, const float* noisy, c
   return split_planes(h, h->x32, h->xs_hi, h->xs_lo, static_cast<size_t>(g.B) * g.P * 16, kXScale, st);
 }
 
+// Milliseconds per call of `body` (which returns a DD_* code) over `iters` calls on st, after `warmup` untimed calls.
+template <typename F>
+int time_per_call(cudaStream_t st, int warmup, int iters, float* ms_out, F&& body) {
+  int rc;
+  for (int i = 0; i < warmup; ++i)
+    if ((rc = body())) return rc;
+  cudaEvent_t e0, e1;
+  CUDA_TRY(cudaEventCreate(&e0));
+  CUDA_TRY(cudaEventCreate(&e1));
+  CUDA_TRY(cudaEventRecord(e0, st));
+  for (int i = 0; i < iters; ++i)
+    if ((rc = body())) return rc;
+  CUDA_TRY(cudaEventRecord(e1, st));
+  CUDA_TRY(cudaEventSynchronize(e1));
+  float ms = 0.f;
+  CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  *ms_out = ms / iters;
+  return DD_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2098,16 +1975,10 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
     dd::compose_fold_kernel<<<256, 256, 0, st>>>(W("model.pred.0.weight"), W("model.pred.0.bias"),
                                                  W("model.upsample_fuse.convB.conv.weight"),
                                                  W("model.upsample_fuse.convB.conv.bias"), k5, k5_abs, h->fold.bias);
-    CUDA_TRY(cudaMemsetAsync(scratch, 0, 4, st));
-    dd::absmax_kernel<<<absmax_grid(n5), 256, 0, st>>>(k5_abs, static_cast<int>(n5), scratch);
-    float amax = 0.f;
-    CUDA_TRY(cudaMemcpyAsync(&amax, scratch, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    float scale = 1.f;
-    if (amax > 0.f && isfinite(amax)) scale = exp2f(floorf(log2f(32768.f / amax)) - 1.f);
-    h->fold.wscale = scale;
-    dd::pack_fold_kernel<<<256, 256, 0, st>>>(k5, h->fold.w, static_cast<double>(scale));
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = check_launch("compose_fold"))) return rc;
+    if ((rc = split_scale_of(k5_abs, n5, scratch, st, &h->fold.wscale))) return rc;
+    dd::pack_fold_kernel<<<256, 256, 0, st>>>(k5, h->fold.w, static_cast<double>(h->fold.wscale));
+    if ((rc = check_launch("pack_fold"))) return rc;
     CUDA_TRY(cudaStreamSynchronize(st));
     cudaFree(k5);
     cudaFree(k5_abs);
@@ -2124,7 +1995,7 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
       float* wt = nullptr;
       if ((rc = dev_alloc(h, reinterpret_cast<void**>(&wt), static_cast<size_t>(co) * ci * 9 * 4))) return rc;
       dd::flip_transpose_weight_kernel<<<64, 256, 0, st>>>(W((std::string(kConvKey[i]) + ".weight").c_str()), wt, co, ci);
-      CUDA_TRY(cudaGetLastError());
+      if ((rc = check_launch("flip_transpose_weight"))) return rc;
       if ((rc = pack_layer(h, h->L[6 + i], wt, zeros, ci, co, st, scratch))) return rc;
     }
   }
@@ -2617,9 +2488,8 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
     const int P = p.H[i] * p.W[i];
     dim3 grid((P + 31) / 32, (p.C[i] + 31) / 32, B), block(32, 8);
     dd::nchw_to_nhwc_split_kernel<<<grid, block, 0, st>>>(feats[i], p.F[i].hi, p.F[i].lo, p.C[i], P, kProdScale, h->status);
-    h->launches++;
+    if ((rc = launched(h, "nchw_to_nhwc_split"))) return rc;
   }
-  CUDA_TRY(cudaGetLastError());
   auto build = [&](cudaStream_t s) -> int {
   const Planes none;
   for (int i = 0; i < p.nlev; ++i) {
@@ -2646,12 +2516,9 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
       if ((rc = run_gen(h, p.fu[i - 1], p.XP[i], 256, none, 0, p.H[i], p.W[i], up_raw, nullptr, nullptr, s))) return rc;
       if (p.resample) {  // F.adaptive_avg_pool2d(conv_up(pre_x), output_size = lateral size)  (reference head :121)
         const size_t n = static_cast<size_t>(B) * p.H[i - 1] * p.W[i - 1] * 256;
-        int blocks = static_cast<int>((n + 255) / 256);
-        if (blocks > 132 * 16) blocks = 132 * 16;
-        dd::adaptive_avg_pool_nhwc_kernel<<<blocks, 256, 0, s>>>(up_raw, p.UP[i - 1], B, 2 * p.H[i], 2 * p.W[i], p.H[i - 1],
-                                                                 p.W[i - 1], 256);
-        h->launches++;
-        CUDA_TRY(cudaGetLastError());
+        dd::adaptive_avg_pool_nhwc_kernel<<<grid_of(n), 256, 0, s>>>(up_raw, p.UP[i - 1], B, 2 * p.H[i], 2 * p.W[i],
+                                                                     p.H[i - 1], p.W[i - 1], 256);
+        if ((rc = launched(h, "adaptive_avg_pool"))) return rc;
       }
     }
   }
@@ -2805,7 +2672,7 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   cudaStream_t st = h->cap_stream;
   const size_t Mp = (static_cast<size_t>(M) + 127) / 128 * 128 + 128;
   Planes A, O;
-  Gemm G;
+  GenLayer L;
   float *y = nullptr, *bias = nullptr;
   int* status = nullptr;
   CUDA_TRY(cudaMalloc(&A.hi, Mp * K * 2));
@@ -2813,47 +2680,32 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   CUDA_TRY(cudaMalloc(&O.hi, Mp * N * 2));
   CUDA_TRY(cudaMalloc(&O.lo, Mp * N * 2));
   CUDA_TRY(cudaMalloc(&y, Mp * N * 4));
-  CUDA_TRY(cudaMalloc(&G.w_hi, static_cast<size_t>(N) * K * 2));
-  CUDA_TRY(cudaMalloc(&G.w_lo, static_cast<size_t>(N) * K * 2));
+  CUDA_TRY(cudaMalloc(&L.w_hi, static_cast<size_t>(N) * K * 2));
+  CUDA_TRY(cudaMalloc(&L.w_lo, static_cast<size_t>(N) * K * 2));
   CUDA_TRY(cudaMalloc(&bias, N * 4));
   CUDA_TRY(cudaMalloc(&status, 64));
   CUDA_TRY(cudaMemsetAsync(A.hi, 0x11, Mp * K * 2, st));
   CUDA_TRY(cudaMemsetAsync(A.lo, 0x01, Mp * K * 2, st));
-  CUDA_TRY(cudaMemsetAsync(G.w_hi, 0x11, static_cast<size_t>(N) * K * 2, st));
-  CUDA_TRY(cudaMemsetAsync(G.w_lo, 0x01, static_cast<size_t>(N) * K * 2, st));
+  CUDA_TRY(cudaMemsetAsync(L.w_hi, 0x11, static_cast<size_t>(N) * K * 2, st));
+  CUDA_TRY(cudaMemsetAsync(L.w_lo, 0x01, static_cast<size_t>(N) * K * 2, st));
   CUDA_TRY(cudaMemsetAsync(bias, 0, N * 4, st));
   CUDA_TRY(cudaMemsetAsync(y, 0, Mp * N * 4, st));
-  G.K = K;
-  G.N = N;
-  G.nt = (N % 256 == 0) ? 256 : 192;
-  G.bias = bias;
-  G.wscale = 1.f;
+  L.cin = K;
+  L.cout = N;
+  L.nt = (N % 256 == 0) ? 256 : 192;
+  L.shift = bias;
   int rc;
-  if ((rc = make_wgen_map(&G.mb_hi, G.w_hi, N, K, 1, G.nt))) return rc;
-  if ((rc = make_wgen_map(&G.mb_lo, G.w_lo, N, K, 1, G.nt))) return rc;
+  if ((rc = make_weight_map(&L.mb_hi, L.w_hi, N, K, 1, dd::GEN_BK, L.nt))) return rc;
+  if ((rc = make_weight_map(&L.mb_lo, L.w_lo, N, K, 1, dd::GEN_BK, L.nt))) return rc;
   int* saved = h->status;
   h->status = status;
-  auto once = [&]() {
-    return run_gemm(h, G, A, M, mode == 2 ? 2 : 0, (mode == 0 || mode == 1) ? y : nullptr, mode == 1 ? y : nullptr,
-                    mode == 2 ? &O : nullptr, st);
-  };
-  for (int i = 0; i < 3; ++i)
-    if ((rc = once())) return rc;
-  cudaEvent_t e0, e1;
-  CUDA_TRY(cudaEventCreate(&e0));
-  CUDA_TRY(cudaEventCreate(&e1));
-  CUDA_TRY(cudaEventRecord(e0, st));
-  for (int i = 0; i < iters; ++i)
-    if ((rc = once())) return rc;
-  CUDA_TRY(cudaEventRecord(e1, st));
-  CUDA_TRY(cudaEventSynchronize(e1));
-  float ms = 0.f;
-  CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
-  *ms_out = ms / iters;
+  if ((rc = time_per_call(st, 3, iters, ms_out, [&]() {
+         return run_gemm(h, L, A, M, mode == 2 ? 2 : 0, (mode == 0 || mode == 1) ? y : nullptr, mode == 1 ? y : nullptr,
+                         mode == 2 ? &O : nullptr, st);
+       })))
+    return rc;
   h->status = saved;
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  for (void* p : {(void*)A.hi, (void*)A.lo, (void*)O.hi, (void*)O.lo, (void*)y, (void*)G.w_hi, (void*)G.w_lo, (void*)bias, (void*)status})
+  for (void* p : {(void*)A.hi, (void*)A.lo, (void*)O.hi, (void*)O.lo, (void*)y, (void*)L.w_hi, (void*)L.w_lo, (void*)bias, (void*)status})
     cudaFree(p);
   return DD_OK;
 }
@@ -2878,9 +2730,7 @@ int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, fl
   a.w = h->cfg.latent_w;
   dim3 grid((a.w + 15) / 16, (a.h + 15) / 16, h->cfg.batch);
   dd::encoder_kernel<<<grid, 256, 0, st>>>(a);
-  cudaError_t err = cudaGetLastError();
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("encoder: ") + cudaGetErrorString(err));
-  return DD_OK;
+  return check_launch("encoder");
 }
 
 int64_t dd_last_launch_count(dd_handle h) { return h ? h->launches : 0; }
@@ -2934,25 +2784,17 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   int rc;
   if ((rc = transpose_in(x, xn, batch, cin, height * width, st))) return rc;
   float* amax_dev = reinterpret_cast<float*>(status) + 8;
-  dd::absmax_kernel<<<absmax_grid(BP * cin), 256, 0, st>>>(xn, static_cast<int>(std::min<size_t>(BP * cin, 1u << 30)), amax_dev);  // zeroed with status
-  dd::absmax_kernel<<<absmax_grid(nw), 256, 0, st>>>(w, static_cast<int>(nw), amax_dev + 1);
-  float am[2] = {0.f, 0.f};
-  CUDA_TRY(cudaMemcpyAsync(am, amax_dev, 8, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  auto pow2_scale = [](float amax) {
-    return (amax > 0.f && isfinite(amax)) ? exp2f(floorf(log2f(32768.f / amax)) - 1.f) : 1.f;
-  };
-  const float sx = pow2_scale(am[0]), sw = pow2_scale(am[1]);
+  float sx, sw;
+  if ((rc = split_scale_of(xn, std::min<size_t>(BP * cin, 1u << 30), amax_dev, st, &sx))) return rc;
+  if ((rc = split_scale_of(w, nw, amax_dev, st, &sw))) return rc;
   dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(xn, hi, lo, BP * cin / 4, sx, status);
+  if ((rc = check_launch("split_planes"))) return rc;
   dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, whi, wlo, wsimt, cout, cin, sw);
-  CUDA_TRY(cudaGetLastError());
+  if ((rc = check_launch("pack_conv_weight"))) return rc;
   dd::ConvArgs a;
   a.B = batch;
   a.H = height;
   a.W = width;
-  a.tiles_x = (width + dd::TILE_W - 1) / dd::TILE_W;
-  a.tiles_y = (height + dd::TILE_H - 1) / dd::TILE_H;
-  a.num_tiles = a.tiles_x * a.tiles_y * batch;
   a.bias = b;
   a.acc_scale = 1.f / (sx * sw);
   a.y32 = yn;
@@ -2962,40 +2804,14 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   a.out_a8 = a.out_l8 = nullptr;
   a.split_scale = 1.f;
   a.status = status;
-  cudaError_t err = cudaSuccess;
-  if (h->cfg.flags & DD_FLAG_SIMT_CONV) {
-    dd::SimtArgs sa;
-    sa.in_hi = hi;
-    sa.in_lo = lo;
-    sa.in_inv_scale = 1.f / sx;
-    sa.w = wsimt;
-    sa.c = a;
-    switch (sid) {
-      case 0: err = launch_simt<16, 64, dd::EPI_F32>(sa, st); break;
-      case 1: err = launch_simt<64, 256, dd::EPI_F32>(sa, st); break;
-      case 2: err = launch_simt<256, 256, dd::EPI_F32>(sa, st); break;
-      case 3: err = launch_simt<256, 64, dd::EPI_F32>(sa, st); break;
-      case 4: err = launch_simt<64, 16, dd::EPI_F32>(sa, st); break;
-    }
-  } else {
-    CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-    const int hbk = kHaloBK[sid];
-    a.tiles_x = (width + dd::HALO_TW - 1) / dd::HALO_TW;
-    a.tiles_y = (height + dd::HALO_TH - 1) / dd::HALO_TH;
-    a.num_tiles = a.tiles_x * a.tiles_y * batch;
-    if ((rc = make_strip_map(&ma_hi, hi, batch, height, width, cin, hbk))) return rc;
-    if ((rc = make_strip_map(&ma_lo, lo, batch, height, width, cin, hbk))) return rc;
-    if ((rc = make_w_map(&mb_hi, whi, cout, cin, hbk))) return rc;
-    if ((rc = make_w_map(&mb_lo, wlo, cout, cin, hbk))) return rc;
-    switch (sid) {
-      case 0: err = launch_halo<16, 64, 16, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 1: err = launch_halo<64, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 2: err = launch_halo<256, 256, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 3: err = launch_halo<256, 64, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-      case 4: err = launch_halo<64, 16, 32, dd::EPI_F32>(ma_hi, ma_lo, mb_hi, mb_lo, a, h->sm_count, st); break;
-    }
+  const bool simt = (h->cfg.flags & DD_FLAG_SIMT_CONV) != 0;
+  CUtensorMap mb_hi{}, mb_lo{};
+  if (!simt) {
+    if ((rc = make_weight_map(&mb_hi, whi, cout, cin, 9, kHaloBK[sid], cout))) return rc;
+    if ((rc = make_weight_map(&mb_lo, wlo, cout, cin, 9, kHaloBK[sid], cout))) return rc;
   }
-  if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(err));
+  if ((rc = launch_conv3x3(sid, dd::EPI_F32, simt, a, hi, lo, sx, wsimt, mb_hi, mb_lo, h->sm_count, st))) return rc;
+  if ((rc = check_launch("conv3x3"))) return rc;
   return transpose_out(yn, y, batch, cout, height * width, st);
 }
 
@@ -3046,11 +2862,8 @@ int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, fl
   if ((rc = transpose_in(x, xn, batch, cin, P, st))) return rc;
   if ((rc = transpose_in(dy, dyn, batch, cout, P, st))) return rc;
   // X: host-side power-of-two scale, as dd_conv3x3 splits its input
-  dd::absmax_kernel<<<absmax_grid(BP * cin), 256, 0, st>>>(xn, static_cast<int>(BP * cin), scratch);
-  float ax = 0.f;
-  CUDA_TRY(cudaMemcpyAsync(&ax, scratch, 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  const float sx = (ax > 0.f && isfinite(ax)) ? exp2f(floorf(log2f(32768.f / ax)) - 1.f) : 1.f;
+  float sx;
+  if ((rc = split_scale_of(xn, BP * cin, scratch, st, &sx))) return rc;
   dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(xn, xhi, xlo, BP * cin / 4, sx, status);
   if ((rc = launched(h, "split_planes"))) return rc;
   // dY: the backward's own on-device split (also for the SIMT shapes, so a non-finite dY is reported for every shape)
@@ -3073,23 +2886,8 @@ int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspac
   CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
   if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
-  cudaEvent_t e0, e1;
-  CUDA_TRY(cudaEventCreate(&e0));
-  CUDA_TRY(cudaEventCreate(&e1));
   // whatever the planes currently hold is fine for timing: MMA time is data independent
-  for (int w = 0; w < 2; ++w)
-    if ((rc = run_fold(h, st))) return rc;
-  CUDA_TRY(cudaEventRecord(e0, st));
-  for (int i = 0; i < iters; ++i)
-    if ((rc = run_fold(h, st))) return rc;
-  CUDA_TRY(cudaEventRecord(e1, st));
-  CUDA_TRY(cudaEventSynchronize(e1));
-  float ms = 0.f;
-  CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  *ms_out = ms / iters;
-  return DD_OK;
+  return time_per_call(st, 2, iters, ms_out, [&]() { return run_fold(h, st); });
 }
 
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,
@@ -3106,29 +2904,13 @@ int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* 
   if (layer < 0) return fail(DD_ERR_UNSUPPORTED, "no packed layer with that shape in this engine variant");
   const bool split_out = (cin == 256 && cout == 256);
   const int f8 = ((split_out || (cin == 64 && cout == 256 && h->f8_ne3)) && fp8_active(h)) ? kF8In : 0;  // time the kernel the loop actually runs
-  cudaEvent_t e0, e1;
-  CUDA_TRY(cudaEventCreate(&e0));
-  CUDA_TRY(cudaEventCreate(&e1));
   // whatever the planes currently hold is fine for timing: MMA time is data independent
   const __half* in_hi = cin == 16 ? h->xs_hi : h->S_hi[1];
   const __half* in_lo = cin == 16 ? h->xs_lo : h->S_lo[1];
-  for (int w = 0; w < 2; ++w)
-    if ((rc = run_conv(h, layer, in_hi, in_lo, kActScale, split_out ? dd::EPI_SPLIT : dd::EPI_F32_STATS, h->Y,
-                       h->stats[0], h->S_hi[0], h->S_lo[0], st, f8)))
-      return rc;
-  CUDA_TRY(cudaEventRecord(e0, st));
-  for (int i = 0; i < iters; ++i)
-    if ((rc = run_conv(h, layer, in_hi, in_lo, kActScale, split_out ? dd::EPI_SPLIT : dd::EPI_F32_STATS, h->Y,
-                       h->stats[0], h->S_hi[0], h->S_lo[0], st, f8)))
-      return rc;
-  CUDA_TRY(cudaEventRecord(e1, st));
-  CUDA_TRY(cudaEventSynchronize(e1));
-  float ms = 0.f;
-  CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  *ms_out = ms / iters;
-  return DD_OK;
+  return time_per_call(st, 2, iters, ms_out, [&]() {
+    return run_conv(h, layer, in_hi, in_lo, kActScale, split_out ? dd::EPI_SPLIT : dd::EPI_F32_STATS, h->Y, h->stats[0],
+                    h->S_hi[0], h->S_lo[0], st, f8);
+  });
 }
 
 }  // extern "C"
