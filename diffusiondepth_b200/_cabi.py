@@ -29,6 +29,12 @@ class DDBackboneConfig(C.Structure):
                 ("mp_dims", C.c_int32 * 4), ("mp_paths", C.c_int32 * 4), ("mlp_ratio", C.c_int32)]
 
 
+class DDGenLayerDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("taps", "stride", "transposed", "act", "add_first", "tokens", "batch",
+                                         "height", "width", "src_h", "src_w", "c0", "c1", "cin", "cout", "ld_out",
+                                         "ch_off", "n_tile", "alt_tile")]
+
+
 ABI_VERSION = 1
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
@@ -78,6 +84,12 @@ SIGNATURES = {
     "dd_conv3x3_wgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
     "dd_conv3x3_wgrad_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "dd_gen_layer": (C.c_int, [C.c_void_p, C.POINTER(DDGenLayerDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.POINTER(C.c_int32), C.c_void_p]),
+    "dd_window_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32),
+                                      C.c_void_p]),
     "dd_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     "dd_bench_conv": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_void_p,
                                 C.c_size_t, C.c_void_p]),

@@ -114,18 +114,20 @@ int encode_map(CUtensorMap* m, const char* what, cuuint32_t rank, const __half* 
 //   convgen activations  box {bk, 16 s, 8 s}, swizzle_for(bk)
 //   halo-kernel strip    box {bk, 8, 18},     swizzle_for(bk)
 //   wgrad operand        box {64, 64, 1},     128-byte swizzle (64 channels x 64 pixels of one row)
+// ld > C: the C channels from base on of rows that are ld channels wide.
 int make_nhwc_map(CUtensorMap* m, const char* what, const __half* base, int B, int H, int W, int C, int box_c, int box_w,
-                  int box_h, CUtensorMapSwizzle swizzle, int stride = 1) {
+                  int box_h, CUtensorMapSwizzle swizzle, int stride = 1, int ld = 0) {
+  const cuuint64_t L = ld > 0 ? ld : C;
   const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint64_t strides[3] = {L * 2, (cuuint64_t)W * L * 2, (cuuint64_t)H * W * L * 2};
   const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
   const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
   return encode_map(m, what, 4, base, dims, strides, box, estr, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // activations of the convgen kernel: 16 x 8 output pixels (sampled with `stride`) by bk channels
-int make_act_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk, int stride = 1) {
+int make_act_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk, int stride = 1, int ld = 0) {
   return make_nhwc_map(m, "activation", base, B, H, W, C, bk, dd::TILE_W * stride, dd::TILE_H * stride, swizzle_for(bk),
-                       stride);
+                       stride, ld);
 }
 // halo patch of conv5x5_fold_kernel: the NHWC [B][H][W][256] fp16 plane seen as {8 ch, y, x, channel group, image};
 // box = {8, 20, 36, 2, 1} lands in shared memory as [channel group][x][y][8 ch], no swizzle
@@ -139,10 +141,11 @@ int make_patch_map(CUtensorMap* m, const __half* base, int B, int H, int W) {
                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // conv weights [taps][cout][cin] fp16 read in boxes of {box_k, rows, 1}: the halo kernel's (9 taps, all cout rows, its
-// K chunk) and the convgen kernel's (GEN_BK, one N tile of rows)
-int make_weight_map(CUtensorMap* m, const __half* base, int cout, int cin, int taps, int box_k, int rows) {
+// K chunk) and the convgen kernel's (GEN_BK, one N tile of rows); ld > cin: cin columns from base on of ld-wide rows
+int make_weight_map(CUtensorMap* m, const __half* base, int cout, int cin, int taps, int box_k, int rows, int ld = 0) {
+  const cuuint64_t L = ld > 0 ? ld : cin;
   const cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)cout, (cuuint64_t)taps};
-  const cuuint64_t strides[2] = {(cuuint64_t)cin * 2, (cuuint64_t)cout * cin * 2};
+  const cuuint64_t strides[2] = {L * 2, (cuuint64_t)cout * L * 2};
   const cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)rows, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   return encode_map(m, "weight", 3, base, dims, strides, box, estr, swizzle_for(box_k), CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
@@ -292,7 +295,17 @@ struct GenLayer {
   CUtensorMap mb_hi, mb_lo;
   bool alt = false;          // cout divisible by 256 and 192: launch_gen picks the width whose last wave wastes least
   CUtensorMap mb_hi_alt, mb_lo_alt;  // boxes of 192 rows
+  float* zero_shift = nullptr;       // layers deep enough to be split along K (gen_parts): the partial launches' shift
 };
+
+// K iterations (64-channel chunk x tap, 12 wgmma each) that one fp32 wgmma accumulator of convgen_wgmma_kernel takes.
+// The accumulator loses a little at every wgmma: measured against fp64, 1,152 wgmma stay at 0.8 of the 3e-5 bound and
+// 2,160 / 2,592 / 3,456 wgmma reach 3.7e-5 / 5.8e-5 / 7.9e-5.  Deeper layers (the level 1..3 fusion convs of the HAHI
+// neck and the widest FPN laterals of Swin) run as gen_parts launches over contiguous channel ranges, summed in fp32 in
+// a fixed order through an fp32 partial buffer (launch_gen).
+constexpr int kGenSplitIters = 110;
+int gen_parts(int taps, int kc_total) { return (taps * kc_total + kGenSplitIters - 1) / kGenSplitIters; }
+int gen_chunks(int c) { return (c + dd::GEN_BK - 1) / dd::GEN_BK; }
 struct Planes {
   __half* hi = nullptr;
   __half* lo = nullptr;
@@ -327,6 +340,7 @@ struct Producers {
   float* UP[3] = {nullptr, nullptr, nullptr};           // fp32 NHWC upsampled maps at level i
   bool resample = false;                                // pyramid is not exactly 2x: adaptive_avg_pool2d is a real resample
   float* UPR[3] = {nullptr, nullptr, nullptr};          // raw ConvT output [B, 2H[i+1], 2W[i+1], 256] before pooling to level i
+  float* KS = nullptr;                                  // fp32 partial sums of the convs split along K (gen_parts)
 };
 struct ResBlockW {
   GenLayer c1, c2, ds;
@@ -618,6 +632,13 @@ size_t carve(dd_engine* e, void* base) {
   if (e->prod.enabled) {
     const Producers& pc = e->prod;
     Producers* pv = &v->prod;
+    size_t ks = 0;  // the largest output of a conv split along K: neck fusion (C + 512 -> C), FPN lateral (C -> 256)
+    for (int i = 0; i < pc.nlev; ++i) {
+      const size_t px = static_cast<size_t>(g.B) * pc.H[i] * pc.W[i];
+      if (pc.neck && gen_parts(9, gen_chunks(pc.C[i]) + gen_chunks(512)) > 1) ks = std::max(ks, px * pc.C[i]);
+      if (gen_parts(9, gen_chunks(pc.C[i])) > 1) ks = std::max(ks, px * 256);
+    }
+    if (ks) pv->KS = c.take<float>(ks);
     for (int i = 0; i < pc.nlev; ++i) {
       const size_t px = static_cast<size_t>(g.B) * pc.H[i] * pc.W[i];
       auto planes = [&](Planes& pl, size_t ch) {
@@ -1018,12 +1039,14 @@ const Raw* find(dd_engine* e, const std::string& k) {
   return it == e->raw.end() ? nullptr : &it->second;
 }
 
-int dev_alloc(dd_engine* e, void** p, size_t bytes) {
+// cudaMalloc recorded in `owned`, which the owner frees (the engine's list: at dd_destroy)
+int dev_alloc(std::vector<void*>& owned, void** p, size_t bytes) {
   cudaError_t err = cudaMalloc(p, bytes);
   if (err != cudaSuccess) return fail(DD_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(err));
-  e->owned.push_back(*p);
+  owned.push_back(*p);
   return DD_OK;
 }
+int dev_alloc(dd_engine* e, void** p, size_t bytes) { return dev_alloc(e->owned, p, bytes); }
 
 int pack_layer(dd_engine* e, ConvLayer& L, const float* w, const float* b, int cout, int cin, cudaStream_t st,
                float* scratch_dev) {
@@ -1047,16 +1070,13 @@ int pack_layer(dd_engine* e, ConvLayer& L, const float* w, const float* b, int c
 // ------------------------------------------------------------------------------------------------ producers
 constexpr float kProdScale = 16.f;  // fp16-split pre-scale of every producer activation
 
-// Fold eval-BN (prefix.{weight,bias,running_mean,running_var}) into per-channel (scale, shift) on the host.
-int bn_fold(dd_engine* e, const std::string& bn, int ch, std::vector<float>& scale, std::vector<float>& shift,
-            cudaStream_t st) {
-  const char* parts[4] = {".weight", ".bias", ".running_mean", ".running_var"};
+// Fold eval-BN, given as the device vectors bn[0..3] = (weight, bias, running_mean, running_var), into per-channel
+// (scale, shift) on the host.
+int bn_fold(const float* const* bn, int ch, std::vector<float>& scale, std::vector<float>& shift, cudaStream_t st) {
   std::vector<float> v[4];
   for (int i = 0; i < 4; ++i) {
-    const Raw* r = find(e, bn + parts[i]);
-    if (!r) return fail(DD_ERR_INVALID, "missing weights: " + bn + parts[i]);
     v[i].resize(ch);
-    CUDA_TRY(cudaMemcpyAsync(v[i].data(), r->ptr, ch * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(v[i].data(), bn[i], ch * 4, cudaMemcpyDeviceToHost, st));
   }
   CUDA_TRY(cudaStreamSynchronize(st));
   scale.resize(ch);
@@ -1068,21 +1088,38 @@ int bn_fold(dd_engine* e, const std::string& bn, int ch, std::vector<float>& sca
   }
   return DD_OK;
 }
+// the registered eval-BN vectors prefix.{weight,bias,running_mean,running_var} -> bn[0..3]
+int find_bn(dd_engine* e, const std::string& prefix, const float** bn) {
+  const char* parts[4] = {".weight", ".bias", ".running_mean", ".running_var"};
+  for (int i = 0; i < 4; ++i) {
+    const Raw* r = find(e, prefix + parts[i]);
+    if (!r) return fail(DD_ERR_INVALID, "missing weights: " + prefix + parts[i]);
+    bn[i] = r->ptr;
+  }
+  return DD_OK;
+}
+int bn_fold(dd_engine* e, const std::string& prefix, int ch, std::vector<float>& scale, std::vector<float>& shift,
+            cudaStream_t st) {
+  const float* bn[4];
+  int rc;
+  if ((rc = find_bn(e, prefix, bn))) return rc;
+  return bn_fold(bn, ch, scale, shift, st);
+}
 
 // Pack one layer of the convgen_wgmma_kernel path, a producer conv or a Linear, from its raw weight w ([cout][cin]
-// [taps], or ConvT [cin][co][2][2] when transposed) followed by eval-BN `bnkey` (folded), or — bnkey empty — by the
-// plain bias `biaskey` (empty: none).  cin_pad >= cin zero-pads the input-channel axis (RGB -> 64).  `name` labels errors.
-int pack_gen_weights(dd_engine* e, GenLayer& L, const float* w, const std::string& name, const std::string& bnkey,
-                     const std::string& biaskey, int cin, int cout_conv, int taps, bool transposed, int cin_pad,
-                     cudaStream_t st, float* scratch) {
+// [taps], or ConvT [cin][co][2][2] when transposed) followed by eval-BN bn[0..3] (device vectors of cout_conv, see
+// bn_fold; folded), or — bn null — by the plain device bias `bias` (null: none).  cin_pad >= cin zero-pads the
+// input-channel axis (RGB -> 64).  nt > 0 forces the N-tile width (64, 128, 192 or 256; 0: the width chosen below).
+// Every device buffer is recorded in `owned`.  `name` labels errors.
+int pack_gen_weights(dd_engine* e, std::vector<void*>& owned, GenLayer& L, const float* w, const std::string& name,
+                     const float* const* bn, const float* bias, int cin, int cout_conv, int taps, bool transposed,
+                     int cin_pad, int nt, cudaStream_t st, float* scratch) {
   std::vector<float> scale(cout_conv, 1.f), shift(cout_conv, 0.f);
   int rc;
-  if (!bnkey.empty()) {
-    if ((rc = bn_fold(e, bnkey, cout_conv, scale, shift, st))) return rc;
-  } else if (!biaskey.empty()) {
-    const Raw* b = find(e, biaskey);
-    if (!b) return fail(DD_ERR_INVALID, "missing weights: " + biaskey);
-    CUDA_TRY(cudaMemcpyAsync(shift.data(), b->ptr, cout_conv * 4, cudaMemcpyDeviceToHost, st));
+  if (bn) {
+    if ((rc = bn_fold(bn, cout_conv, scale, shift, st))) return rc;
+  } else if (bias) {
+    CUDA_TRY(cudaMemcpyAsync(shift.data(), bias, cout_conv * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
   }
   const int cp = cin_pad > 0 ? cin_pad : cin;
@@ -1095,22 +1132,25 @@ int pack_gen_weights(dd_engine* e, GenLayer& L, const float* w, const std::strin
   // A last tile wider than the remaining channels reads zero weight rows (TMA out-of-bounds fill), the epilogue drops
   // them; partial K chunks are completed with zeros the same way (MPViT widths: 216, 288, 648, 864 ...).
   L.nt = 64;
-  if (L.cout > 64) {
+  if (nt > 0) {
+    if (nt != 64 && nt != 128 && nt != 192 && nt != 256) return fail(DD_ERR_INVALID, "N tile must be 64, 128, 192 or 256");
+    L.nt = nt;
+  } else if (L.cout > 64) {
     int best = 1 << 30;
-    for (int nt : {256, 192, 128}) {
-      const int padded = (L.cout + nt - 1) / nt * nt;
-      if (padded < best) { best = padded; L.nt = nt; }
+    for (int width : {256, 192, 128}) {
+      const int padded = (L.cout + width - 1) / width * width;
+      if (padded < best) { best = padded; L.nt = width; }
     }
   }
   if (L.cout % 8 != 0 || cp % 8 != 0) return fail(DD_ERR_UNSUPPORTED, "channels must be multiples of 8: " + name);
   const int cout_pad = (L.cout + L.nt - 1) / L.nt * L.nt;
   const size_t n = static_cast<size_t>(L.cout) * cp * L.taps;
   float* d_scale = nullptr;  // per output channel; nullptr: 1
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_hi), n * 2))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_lo), n * 2))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.shift), cout_pad * 4))) return rc;
-  if (!bnkey.empty()) {
-    if ((rc = dev_alloc(e, reinterpret_cast<void**>(&d_scale), cout_conv * 4))) return rc;
+  if ((rc = dev_alloc(owned, reinterpret_cast<void**>(&L.w_hi), n * 2))) return rc;
+  if ((rc = dev_alloc(owned, reinterpret_cast<void**>(&L.w_lo), n * 2))) return rc;
+  if ((rc = dev_alloc(owned, reinterpret_cast<void**>(&L.shift), cout_pad * 4))) return rc;
+  if (bn) {
+    if ((rc = dev_alloc(owned, reinterpret_cast<void**>(&d_scale), cout_conv * 4))) return rc;
     CUDA_TRY(cudaMemcpyAsync(d_scale, scale.data(), cout_conv * 4, cudaMemcpyHostToDevice, st));
   }
   if (cp != cin) {
@@ -1120,6 +1160,10 @@ int pack_gen_weights(dd_engine* e, GenLayer& L, const float* w, const std::strin
   std::vector<float> shift_full(cout_pad, 0.f);
   for (int i = 0; i < L.cout; ++i) shift_full[i] = shift[i % cout_conv];
   CUDA_TRY(cudaMemcpyAsync(L.shift, shift_full.data(), cout_pad * 4, cudaMemcpyHostToDevice, st));
+  if (gen_parts(L.taps, gen_chunks(cp) + 1) > 1) {  // two sources may add a partial chunk
+    if ((rc = dev_alloc(owned, reinterpret_cast<void**>(&L.zero_shift), cout_pad * 4))) return rc;
+    CUDA_TRY(cudaMemsetAsync(L.zero_shift, 0, cout_pad * 4, st));
+  }
   const int nraw = static_cast<int>(static_cast<size_t>(cout_conv) * cin * (transposed ? 4 : taps));
   if ((rc = split_scale(scratch, st, &L.wscale, [&] {
          dd::absmax_scaled_kernel<<<absmax_grid(nraw), 256, 0, st>>>(w, d_scale, nraw, cin * L.taps, cout_conv,
@@ -1150,7 +1194,18 @@ int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::stri
   std::vector<int64_t> want = transposed ? std::vector<int64_t>{cin, cout_conv, 2, 2}
                                          : std::vector<int64_t>{cout_conv, cin, k, k};
   if (w->shape != want) return fail(DD_ERR_INVALID, "weight shape mismatch: " + wkey);
-  return pack_gen_weights(e, L, w->ptr, wkey, bnkey, biaskey, cin, cout_conv, taps, transposed, cin_pad, st, scratch);
+  const float* bn[4] = {nullptr, nullptr, nullptr, nullptr};
+  const float* bias = nullptr;
+  int rc;
+  if (!bnkey.empty()) {
+    if ((rc = find_bn(e, bnkey, bn))) return rc;
+  } else if (!biaskey.empty()) {
+    const Raw* b = find(e, biaskey);
+    if (!b) return fail(DD_ERR_INVALID, "missing weights: " + biaskey);
+    bias = b->ptr;
+  }
+  return pack_gen_weights(e, e->owned, L, w->ptr, wkey, bnkey.empty() ? nullptr : bn, bias, cin, cout_conv, taps,
+                          transposed, cin_pad, 0, st, scratch);
 }
 
 // nn.Linear: weight key `wkey` [N][K], bias key `bkey` (empty: none).  run_gemm supplies the activation.
@@ -1159,7 +1214,10 @@ int pack_linear(dd_engine* e, GenLayer& L, const std::string& wkey, const std::s
   const Raw* w = find(e, wkey);
   if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
   if (w->shape != std::vector<int64_t>{N, K}) return fail(DD_ERR_INVALID, "weight shape mismatch: " + wkey);
-  return pack_gen_weights(e, L, w->ptr, wkey, "", bkey, K, N, 1, false, 0, st, scratch);
+  const Raw* b = nullptr;
+  if (!bkey.empty() && !(b = find(e, bkey))) return fail(DD_ERR_INVALID, "missing weights: " + bkey);
+  return pack_gen_weights(e, e->owned, L, w->ptr, wkey, nullptr, b ? b->ptr : nullptr, K, N, 1, false, 0, 0, st,
+                          scratch);
 }
 
 int pack_producers(dd_engine* e, cudaStream_t st, float* scratch) {
@@ -1198,11 +1256,19 @@ struct GenGrid {
   int B, H, W, m_valid, src_h, src_w;
 };
 
+// What one launch_gen launched: the N-tile width, the work items (M tiles x N tiles) and the persistent grid.
+struct GenLaunch {
+  int nt, work, grid, parts;
+};
+
 // Every launch of layer L on convgen_wgmma_kernel (producer convs and Linears): activation act, sources a0 (c0
 // channels) and a1 (c1, concatenated after a0; c1 = 0: none), outputs y32 (fp32, + add32) and / or the split planes
-// *out with row width ld_out (0: L.cout) from channel ch_off on.
+// *out with row width ld_out (0: L.cout) from channel ch_off on.  alt: a layer with 192-wide alternative maps uses them
+// when its last wave wastes less (0), always (1) or never (-1).  info (nullable) receives what was launched (per launch
+// of a layer split along K).  partial: fp32 [pixels][L.cout] for the partial sums of a layer split along K.
 int launch_gen(dd_engine* e, const GenLayer& L, int act, const GenGrid& g, const Planes& a0, int c0, const Planes& a1,
-               int c1, float* y32, const float* add32, const Planes* out, int ld_out, int ch_off, cudaStream_t st) {
+               int c1, float* y32, const float* add32, const Planes* out, int ld_out, int ch_off, cudaStream_t st,
+               int alt = 0, GenLaunch* info = nullptr, float* partial = nullptr) {
   if (c0 + c1 != L.cin) return fail(DD_ERR_INVALID, "producer conv: source channels do not match the layer");
   dd::GenConvArgs a;
   a.B = g.B;
@@ -1214,10 +1280,10 @@ int launch_gen(dd_engine* e, const GenLayer& L, int act, const GenGrid& g, const
   // wave quantisation: with few M tiles pick the N-tile width whose last wave wastes least — deep Swin stages, and the
   // level-2 fusion conv of the HAHI neck (768 channels, 30 tile pairs) runs 2 waves of 192 columns instead of 2 of 256
   int nt = L.nt;
-  if (L.alt) {
+  if (L.alt && alt >= 0) {
     const int units = a.m_tiles, slots = e->sm_count;
     auto cost = [&](int w) { return ((units * (L.cout / w) + slots - 1) / slots) * w; };
-    if (cost(192) < cost(256)) nt = 192;
+    if (alt > 0 || cost(192) < cost(256)) nt = 192;
   }
   a.n_tiles = (L.cout + nt - 1) / nt;
   a.kc0 = (c0 + dd::GEN_BK - 1) / dd::GEN_BK;  // a partial last chunk is zero-filled by TMA on both operands
@@ -1243,26 +1309,91 @@ int launch_gen(dd_engine* e, const GenLayer& L, int act, const GenGrid& g, const
   const bool use_alt = nt != L.nt;
   CUtensorMap m[6];  // sources 0 and 1 (hi, lo), weights (hi, lo)
   const int sh = L.stride == 1 ? g.H : g.src_h, sw = L.stride == 1 ? g.W : g.src_w;
-  int rc;
-  if ((rc = make_act_map(&m[0], a0.hi, g.B, sh, sw, c0, dd::GEN_BK, L.stride))) return rc;
-  if ((rc = make_act_map(&m[1], a0.lo, g.B, sh, sw, c0, dd::GEN_BK, L.stride))) return rc;
-  if (c1 > 0) {
-    if ((rc = make_act_map(&m[2], a1.hi, g.B, g.H, g.W, c1, dd::GEN_BK))) return rc;
-    if ((rc = make_act_map(&m[3], a1.lo, g.B, g.H, g.W, c1, dd::GEN_BK))) return rc;
-  } else {
-    m[2] = m[0];
-    m[3] = m[1];
-  }
-  m[4] = use_alt ? L.mb_hi_alt : L.mb_hi;
-  m[5] = use_alt ? L.mb_lo_alt : L.mb_lo;
   const int grid = std::min(a.m_tiles * a.n_tiles, e->sm_count);
-  switch (nt) {
-    case 256: convgen_kernel<256>(grid, st, m, a); break;
-    case 192: convgen_kernel<192>(grid, st, m, a); break;
-    case 128: convgen_kernel<128>(grid, st, m, a); break;
-    default: convgen_kernel<64>(grid, st, m, a); break;
+  const int parts = gen_parts(L.taps, a.kc0 + a.kc1);
+  if (info) *info = {nt, a.m_tiles * a.n_tiles, grid, parts};
+  auto launch = [&](const dd::GenConvArgs& args) {
+    switch (nt) {
+      case 256: convgen_kernel<256>(grid, st, m, args); break;
+      case 192: convgen_kernel<192>(grid, st, m, args); break;
+      case 128: convgen_kernel<128>(grid, st, m, args); break;
+      default: convgen_kernel<64>(grid, st, m, args); break;
+    }
+    return launched(e, "convgen");
+  };
+  int rc;
+  if (parts == 1) {
+    if ((rc = make_act_map(&m[0], a0.hi, g.B, sh, sw, c0, dd::GEN_BK, L.stride))) return rc;
+    if ((rc = make_act_map(&m[1], a0.lo, g.B, sh, sw, c0, dd::GEN_BK, L.stride))) return rc;
+    if (c1 > 0) {
+      if ((rc = make_act_map(&m[2], a1.hi, g.B, g.H, g.W, c1, dd::GEN_BK))) return rc;
+      if ((rc = make_act_map(&m[3], a1.lo, g.B, g.H, g.W, c1, dd::GEN_BK))) return rc;
+    } else {
+      m[2] = m[0];
+      m[3] = m[1];
+    }
+    m[4] = use_alt ? L.mb_hi_alt : L.mb_hi;
+    m[5] = use_alt ? L.mb_lo_alt : L.mb_lo;
+    return launch(a);
   }
-  return launched(e, "convgen");
+  // Split along K (kGenSplitIters): `parts` launches over contiguous ranges of the concatenated 64-channel chunks, every
+  // tap each.  Launch p < parts - 1 writes partial = acc_p (+ partial), the last one adds the partial sum before its shift
+  // and activation and writes the real outputs: a fixed-order fp32 sum, bit-reproducible.
+  if (add32 || L.shuffle || !partial || !L.zero_shift)
+    return fail(DD_ERR_UNSUPPORTED, "producer conv deeper than one accumulator takes, with an addend or no partial buffer");
+  const int kc_total = a.kc0 + a.kc1, per = (kc_total + parts - 1) / parts;
+  for (int p = 0; p * per < kc_total; ++p) {
+    const int ka = p * per, kb = std::min(kc_total, ka + per);
+    // chunks [ka, kb): source-0 chunks [s0a, s0b) (channels from s0a * GEN_BK, w0 of them), then source-1 chunks
+    const int s0a = std::min(ka, a.kc0), s0b = std::min(kb, a.kc0);
+    const int s1a = std::max(ka, a.kc0) - a.kc0, s1b = std::max(kb, a.kc0) - a.kc0;
+    const int w0 = std::min(s0b * dd::GEN_BK, c0) - s0a * dd::GEN_BK;
+    const int w1 = std::min(s1b * dd::GEN_BK, c1) - s1a * dd::GEN_BK;
+    // The part's weight columns are contiguous (a part that reaches into source 1 holds source 0's last chunk).  Every
+    // map starts on a 64-channel (128-byte) boundary: a source-1-only part behind a source 0 of c0 % 64 != 0 channels
+    // runs as a source 0 of no chunks whose source-1 weights start c0 % 64 columns into its map.
+    dd::GenConvArgs ap = a;
+    int wcol, wlen;
+    if (w0 > 0) {
+      if ((rc = make_act_map(&m[0], a0.hi + s0a * dd::GEN_BK, g.B, sh, sw, w0, dd::GEN_BK, L.stride, c0))) return rc;
+      if ((rc = make_act_map(&m[1], a0.lo + s0a * dd::GEN_BK, g.B, sh, sw, w0, dd::GEN_BK, L.stride, c0))) return rc;
+      ap.kc0 = s0b - s0a;
+      ap.c0_ch = w0;
+      wcol = s0a * dd::GEN_BK;
+      wlen = w0 + w1;
+    } else {
+      ap.kc0 = 0;
+      ap.c0_ch = (c0 + s1a * dd::GEN_BK) % dd::GEN_BK;
+      wcol = c0 + s1a * dd::GEN_BK - ap.c0_ch;
+      wlen = ap.c0_ch + w1;
+    }
+    ap.kc1 = s1b - s1a;
+    if (w1 > 0) {
+      if ((rc = make_act_map(&m[2], a1.hi + s1a * dd::GEN_BK, g.B, g.H, g.W, w1, dd::GEN_BK, 1, c1))) return rc;
+      if ((rc = make_act_map(&m[3], a1.lo + s1a * dd::GEN_BK, g.B, g.H, g.W, w1, dd::GEN_BK, 1, c1))) return rc;
+    }
+    if (w0 == 0) {
+      m[0] = m[2];
+      m[1] = m[3];
+    } else if (w1 == 0) {
+      m[2] = m[0];
+      m[3] = m[1];
+    }
+    if ((rc = make_weight_map(&m[4], L.w_hi + wcol, L.cout, wlen, L.taps, dd::GEN_BK, nt, L.cin))) return rc;
+    if ((rc = make_weight_map(&m[5], L.w_lo + wcol, L.cout, wlen, L.taps, dd::GEN_BK, nt, L.cin))) return rc;
+    const bool last = kb == kc_total;
+    ap.relu = last ? act : 0;
+    ap.shift = last ? L.shift : L.zero_shift;
+    ap.add_first = 1;
+    ap.add32 = p > 0 ? partial : nullptr;
+    ap.y32 = last ? y32 : partial;
+    ap.out_hi = last ? a.out_hi : nullptr;
+    ap.out_lo = last ? a.out_lo : nullptr;
+    ap.ld_out = last ? a.ld_out : L.cout;
+    ap.ch_off = last ? ch_off : 0;
+    if ((rc = launch(ap))) return rc;
+  }
+  return DD_OK;
 }
 
 // H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.
@@ -1270,7 +1401,7 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
             float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
             int ld_out = 0, int ch_off = 0) {
   return launch_gen(e, L, L.relu, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, y32, add32, out, ld_out, ch_off,
-                    st);
+                    st, 0, nullptr, e->prod.KS);
 }
 
 // ------------------------------------------------------------------------------------------------ ResNet backbone
@@ -1426,6 +1557,47 @@ int run_ln(dd_engine* e, int C, const float* x, const float* g, const float* b, 
   return launched(e, "ln_split");
 }
 
+// Window attention on the fp32 CUDA-core kernel: the check path (DD_FLAG_SIMT_CONV, probes switch) and any odd head
+// count (the wgmma kernel takes heads in pairs).
+bool attn_simt(const dd_engine* e, int nH) {
+  return (e->cfg.flags & DD_FLAG_SIMT_CONV) || (nH & 1) || e->attn_simt;
+}
+
+// One (shifted-)window attention launch (7 x 7 windows, head_dim 32): qkv fp32 [B*H*W][3C] (padded tokens carry
+// qkv_bias), relative-position table [169][nH] -> out planes [B*H*W][C] at kTokScale.  simt: window_attention_kernel,
+// one block per (window, head); else window_attention_wgmma_kernel on pairs of heads of one window (nH even).
+// work / grid (nullable) receive the units of work and the grid launched.
+int launch_attention(dd_engine* e, const float* qkv, const float* qkv_bias, const float* table, const Planes& out,
+                     int B, int H, int W, int C, int nH, int shift, bool simt, cudaStream_t st, int* work = nullptr,
+                     int* grid_out = nullptr) {
+  constexpr int ws = 7;
+  const int Hp = (H + ws - 1) / ws * ws, Wp = (W + ws - 1) / ws * ws;
+  dd::AttnArgs aa;
+  aa.qkv = qkv;
+  aa.qkv_bias = qkv_bias;
+  aa.bias_table = table;
+  aa.out_hi = out.hi;
+  aa.out_lo = out.lo;
+  aa.scale_out = kTokScale;
+  aa.B = B; aa.H = H; aa.W = W; aa.C = C; aa.nH = nH;
+  aa.shift = shift;
+  aa.Hp = Hp; aa.Wp = Wp; aa.nWx = Wp / ws; aa.nWy = Hp / ws;
+  aa.status = e->status;
+  int units, grid;
+  if (simt) {  // fp32 CUDA-core check path
+    units = grid = B * aa.nWx * aa.nWy * nH;
+    dd::window_attention_kernel<<<grid, 64, 0, st>>>(aa);
+  } else {  // wgmma: pairs of heads of one window per M = 128 tile, two persistent CTAs per SM
+    if (nH & 1) return fail(DD_ERR_UNSUPPORTED, "the wgmma window attention takes heads in pairs");
+    units = B * aa.nWx * aa.nWy * (nH / 2);
+    grid = units < 2 * e->sm_count ? units : 2 * e->sm_count;
+    dd::window_attention_wgmma_kernel<<<grid, 128, dd::WAU_SMEM, st>>>(aa, units);
+  }
+  if (work) *work = units;
+  if (grid_out) *grid_out = grid;
+  return launched(e, "window_attention");
+}
+
 int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream_t st) {
   Backbone& b = e->bb;
   const int B = e->cfg.batch;
@@ -1440,30 +1612,12 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
     const int C = b.E << s, H = b.Hs[s], W = b.Ws[s], M = B * H * W, nH = b.heads[s];
     float* x = b.X[s & 1];
     const int ws = b.window;
-    const int Hp = (H + ws - 1) / ws * ws, Wp = (W + ws - 1) / ws * ws;
     for (int k = 0; k < b.depths[s]; ++k) {
       const SwinBlockW& Wt = b.stage[s].blocks[k];
       if ((rc = run_ln(e, C, x, Wt.ln1_g, Wt.ln1_b, b.AP, M, nullptr, 0, st))) return rc;
       if ((rc = run_gemm(e, Wt.qkv, b.AP, M, 0, b.QKV, nullptr, nullptr, st))) return rc;
-      dd::AttnArgs aa;
-      aa.qkv = b.QKV;
-      aa.qkv_bias = Wt.qkv.shift;
-      aa.bias_table = Wt.table;
-      aa.out_hi = b.AP.hi;
-      aa.out_lo = b.AP.lo;
-      aa.scale_out = kTokScale;
-      aa.B = B; aa.H = H; aa.W = W; aa.C = C; aa.nH = nH;
-      aa.shift = (k & 1) ? ws / 2 : 0;
-      aa.Hp = Hp; aa.Wp = Wp; aa.nWx = Wp / ws; aa.nWy = Hp / ws;
-      aa.status = e->status;
-      if ((e->cfg.flags & DD_FLAG_SIMT_CONV) || (nH & 1) || e->attn_simt) {  // fp32 CUDA-core check path
-        dd::window_attention_kernel<<<B * aa.nWx * aa.nWy * nH, 64, 0, st>>>(aa);
-      } else {  // wgmma: pairs of heads of one window per M = 128 tile, two persistent CTAs per SM
-        const int pairs = B * aa.nWx * aa.nWy * (nH / 2);
-        const int grid = pairs < 2 * e->sm_count ? pairs : 2 * e->sm_count;
-        dd::window_attention_wgmma_kernel<<<grid, 128, dd::WAU_SMEM, st>>>(aa, pairs);
-      }
-      if ((rc = launched(e, "window_attention"))) return rc;
+      if ((rc = launch_attention(e, b.QKV, Wt.qkv.shift, Wt.table, b.AP, B, H, W, C, nH, (k & 1) ? ws / 2 : 0,
+                                 attn_simt(e, nH), st))) return rc;
       if ((rc = run_gemm(e, Wt.proj, b.AP, M, 0, x, x, nullptr, st))) return rc;      // x += proj(attn)
       if ((rc = run_ln(e, C, x, Wt.ln2_g, Wt.ln2_b, b.AP, M, nullptr, 0, st))) return rc;
       if ((rc = run_gemm(e, Wt.ffn1, b.AP, M, 2, nullptr, nullptr, &b.HP, st))) return rc;  // GELU(fc1) -> planes
@@ -1841,6 +1995,37 @@ int time_per_call(cudaStream_t st, int warmup, int iters, float* ms_out, F&& bod
   *ms_out = ms / iters;
   return DD_OK;
 }
+
+// The buffers of one standalone layer call (dd_gen_layer, dd_window_attention), freed when it returns, and the engine's
+// status word pointed at the call's own word meanwhile (the launch helpers report to e->status, a workspace word).
+struct StandaloneCall {
+  dd_engine* e;
+  int* saved;
+  std::vector<void*> owned;
+  int* status = nullptr;
+  explicit StandaloneCall(dd_engine* eng) : e(eng), saved(eng->status) {}
+  ~StandaloneCall() {
+    e->status = saved;
+    for (void* p : owned) cudaFree(p);
+  }
+  int begin(cudaStream_t st) {
+    int rc;
+    if ((rc = dev_alloc(owned, reinterpret_cast<void**>(&status), 64))) return rc;
+    CUDA_TRY(cudaMemsetAsync(status, 0, 64, st));
+    e->status = status;
+    return DD_OK;
+  }
+  template <typename T>
+  int alloc(T** p, size_t n) { return dev_alloc(owned, reinterpret_cast<void**>(p), n * sizeof(T)); }
+  // synchronise st and report the status word
+  int finish(cudaStream_t st, const char* what) {
+    int flag = 0;
+    CUDA_TRY(cudaMemcpyAsync(&flag, status, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (flag) return fail(DD_ERR_RANGE, std::string("non-finite or out-of-range value in ") + what);
+    return DD_OK;
+  }
+};
 
 }  // namespace
 
@@ -2874,6 +3059,114 @@ int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, fl
   CUDA_TRY(cudaMemcpyAsync(&flag, status, 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   if (flag) return fail(DD_ERR_RANGE, "non-finite or out-of-range value in x or dy");
+  return DD_OK;
+}
+
+// ---------------------------------------------------------------- standalone producer layers (tests)
+int dd_gen_layer(dd_handle h, const dd_gen_layer_desc* d, const float* x0, const float* x1, const float* w,
+                 const float* bias, const float* const* bn, const float* add32, float* y32, void* out_hi, void* out_lo,
+                 int32_t* launch_out, void* cuda_stream) {
+  if (!h || !d || !x0 || !w || (d->c1 > 0 && !x1)) return fail(DD_ERR_INVALID, "null argument");
+  if (!y32 && !(out_hi && out_lo)) return fail(DD_ERR_INVALID, "no output");
+  const bool gemm = d->tokens > 0, xp = d->transposed != 0;
+  const int c0 = d->c0, c1 = d->c1, cout = d->cout;
+  const int cin = d->cin > 0 ? d->cin : c0 + c1;
+  if ((d->taps != 1 && d->taps != 9) || (d->stride != 1 && d->stride != 2) || d->act < 0 || d->act > 3 || c0 < 8 ||
+      c1 < 0 || c0 % 8 || c1 % 8 || cout < 8 || cin > c0 + c1 || (cin < c0 + c1 && c1 > 0))
+    return fail(DD_ERR_INVALID, "bad layer descriptor");
+  if (d->stride == 2 && (gemm || c1 > 0 || xp)) return fail(DD_ERR_INVALID, "stride 2: conv mode, one source");
+  if (xp && (d->taps != 1 || c1 > 0 || d->ld_out > 0 || d->ch_off > 0))
+    return fail(DD_ERR_INVALID, "transposed: one 1x1 source, dense output");
+  const int ld_out = d->ld_out > 0 ? d->ld_out : (xp ? 4 * cout : cout);
+  if (d->ch_off < 0 || d->ch_off + cout > ld_out || ld_out % 8 || d->ch_off % 8)  // 16-byte plane stores
+    return fail(DD_ERR_INVALID, "bad output row width / channel offset");
+  GenGrid g;
+  if (gemm) {
+    g = {1, (d->tokens + dd::TILE_W - 1) / dd::TILE_W, dd::TILE_W, d->tokens, 0, 0};
+  } else {
+    if (d->batch < 1 || d->height < 1 || d->width < 1) return fail(DD_ERR_INVALID, "empty geometry");
+    g = {d->batch, d->height, d->width, 0, d->stride == 2 ? d->src_h : d->height, d->stride == 2 ? d->src_w : d->width};
+    if (d->stride == 2 && ((g.src_h + 1) / 2 != g.H || (g.src_w + 1) / 2 != g.W))
+      return fail(DD_ERR_INVALID, "stride 2: the output grid must be ceil(source / 2)");
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  float* scratch = reinterpret_cast<float*>(call.status) + 8;
+  GenLayer L;
+  if ((rc = pack_gen_weights(h, call.owned, L, w, "standalone layer", bn, bias, cin, cout, d->taps, xp,
+                             cin < c0 ? c0 : 0, d->n_tile, st, scratch)))
+    return rc;
+  L.stride = d->stride;
+  L.add_first = d->add_first;
+  // sources: fp32 -> split planes; a GEMM's token rows are padded to whole 16-row "image" rows with zeros
+  const size_t rows0 = gemm ? static_cast<size_t>(g.H) * g.W : static_cast<size_t>(g.B) * g.src_h * g.src_w;
+  const size_t rows1 = gemm ? rows0 : static_cast<size_t>(g.B) * g.H * g.W;
+  const size_t real0 = gemm ? static_cast<size_t>(d->tokens) : rows0, real1 = gemm ? real0 : rows1;
+  Planes a0, a1;
+  if ((rc = call.alloc(&a0.hi, rows0 * c0)) || (rc = call.alloc(&a0.lo, rows0 * c0))) return rc;
+  if (gemm) {
+    CUDA_TRY(cudaMemsetAsync(a0.hi, 0, rows0 * c0 * 2, st));
+    CUDA_TRY(cudaMemsetAsync(a0.lo, 0, rows0 * c0 * 2, st));
+  }
+  if ((rc = split_planes(h, x0, a0.hi, a0.lo, real0 * c0, kProdScale, st))) return rc;
+  if (c1 > 0) {
+    if ((rc = call.alloc(&a1.hi, rows1 * c1)) || (rc = call.alloc(&a1.lo, rows1 * c1))) return rc;
+    if (gemm) {
+      CUDA_TRY(cudaMemsetAsync(a1.hi, 0, rows1 * c1 * 2, st));
+      CUDA_TRY(cudaMemsetAsync(a1.lo, 0, rows1 * c1 * 2, st));
+    }
+    if ((rc = split_planes(h, x1, a1.hi, a1.lo, real1 * c1, kProdScale, st))) return rc;
+  }
+  float* partial = nullptr;  // a layer split along K (gen_parts)
+  if (gen_parts(L.taps, gen_chunks(c0) + gen_chunks(c1)) > 1 &&
+      (rc = call.alloc(&partial, static_cast<size_t>(g.B) * g.H * g.W * L.cout)))
+    return rc;
+  const Planes out{static_cast<__half*>(out_hi), static_cast<__half*>(out_lo)};
+  GenLaunch info;
+  if ((rc = launch_gen(h, L, d->act, g, a0, c0, a1, c1, y32, add32, (out_hi && out_lo) ? &out : nullptr,
+                       d->ld_out > 0 ? d->ld_out : 0, d->ch_off, st, d->alt_tile, &info, partial)))
+    return rc;
+  if ((rc = call.finish(st, "an input or an output plane"))) return rc;
+  if (launch_out) {
+    launch_out[0] = info.nt;
+    launch_out[1] = info.work;
+    launch_out[2] = info.grid;
+    launch_out[3] = info.parts;
+  }
+  return DD_OK;
+}
+
+int dd_window_attention(dd_handle h, const float* qkv, const float* qkv_bias, const float* table, float* out,
+                        int32_t batch, int32_t height, int32_t width, int32_t num_heads, int32_t shift, int32_t kernel,
+                        int32_t* launch_out, void* cuda_stream) {
+  if (!h || !qkv || !qkv_bias || !table || !out) return fail(DD_ERR_INVALID, "null argument");
+  if (batch < 1 || height < 1 || width < 1 || num_heads < 1 || shift < 0 || shift >= 7 || kernel < 0 || kernel > 2)
+    return fail(DD_ERR_INVALID, "bad attention geometry");
+  if (kernel == 2 && (num_heads & 1)) return fail(DD_ERR_UNSUPPORTED, "the wgmma window attention takes heads in pairs");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const int C = 32 * num_heads;
+  const size_t n = static_cast<size_t>(batch) * height * width * C;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  Planes o;
+  if ((rc = call.alloc(&o.hi, n)) || (rc = call.alloc(&o.lo, n))) return rc;
+  const bool simt = kernel == 0 ? attn_simt(h, num_heads) : kernel == 1;
+  int work = 0, grid = 0;
+  if ((rc = launch_attention(h, qkv, qkv_bias, table, o, batch, height, width, C, num_heads, shift, simt, st, &work,
+                             &grid)))
+    return rc;
+  dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
+  if ((rc = check_launch("join_planes"))) return rc;
+  if ((rc = call.finish(st, "qkv or the attention output"))) return rc;
+  if (launch_out) {
+    launch_out[0] = work;
+    launch_out[1] = grid;
+  }
   return DD_OK;
 }
 

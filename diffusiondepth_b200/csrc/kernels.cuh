@@ -13,7 +13,7 @@ namespace dd {
 
 __device__ __forceinline__ void split_f16(float v, float scale, __half& hi, __half& lo, bool& overflow) {
   const float s = v * scale;
-  overflow |= (fabsf(s) > 60000.f);
+  overflow |= !(fabsf(s) <= 60000.f);  // also catches NaN
   hi = __float2half_rn(s);
   lo = __float2half_rn(s - __half2float(hi));
 }
@@ -70,6 +70,14 @@ __global__ void split_planes_kernel(const float* __restrict__ x, __half* __restr
     reinterpret_cast<uint2*>(lo)[i] = *reinterpret_cast<const uint2*>(l);
   }
   if (ov) atomicOr(status, 1);
+}
+
+// scaled fp16 hi/lo planes -> fp32 (hi + lo) * inv_scale (n elements): reads a split tensor back (standalone layer entries)
+__global__ void join_planes_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, float* __restrict__ x,
+                                   size_t n, float inv_scale) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    x[i] = (__half2float(hi[i]) + __half2float(lo[i])) * inv_scale;
 }
 
 // fp32 NHWC -> fp16 hi plane + e4m3 a8 / l8 planes (standalone-layer path of the fp8-correction kernel)

@@ -444,6 +444,70 @@ class DenoiseEngine:
                                               C.c_void_p(self._aligned(ws)), need, C.c_void_p(self._stream())))
         return dw, db
 
+    def gen_layer(self, x0: torch.Tensor, w: torch.Tensor, x1: Optional[torch.Tensor] = None,
+                  bias: Optional[torch.Tensor] = None, bn=None, add: Optional[torch.Tensor] = None,
+                  stride: int = 1, transposed: bool = False, act: int = 0, add_first: bool = False, cin: int = 0,
+                  ld_out: int = 0, ch_off: int = 0, n_tile: int = 0, alt_tile: int = 0, y32=True, planes=None):
+        """One producer layer on the engine's tensor-core conv / GEMM kernel (dd_gen_layer), NHWC in and out.
+        x0 [M, c0] (GEMM mode) or [B, Hs, Ws, c0] (conv mode), x1 (second source, concatenated after x0) on the output
+        grid; w in the reference layout (Linear [cout, cin], conv [cout, cin, k, k], ConvT [c0, cout, 2, 2]); bn =
+        (weight, bias, running_mean, running_var) folded after the conv, else `bias`; `add` the fp32 addend.
+        y32 / planes: True allocates the output (planes: fp16 hi / lo at the producers' scale), a tensor (pair) is
+        written in place (rows ld_out wide, columns [ch_off, ch_off + cout)), None / False skips it.
+        Returns (y32, (hi, lo), {"nt", "work", "grid", "parts"}) with None for a skipped output; "parts" > 1: the
+        layer ran split along K."""
+        dev = self.device
+
+        def f32(t):
+            return None if t is None else t.detach().to(dev, torch.float32).contiguous()
+
+        x0, x1, w, bias, add = f32(x0), f32(x1), f32(w), f32(bias), f32(add)
+        bn = None if bn is None else [f32(t) for t in bn]
+        d = _cabi.DDGenLayerDesc()
+        d.taps = 1 if (transposed or w.dim() == 2) else w.shape[2] * w.shape[3]
+        d.stride, d.transposed, d.act, d.add_first = int(stride), int(transposed), int(act), int(add_first)
+        d.c0, d.c1 = x0.shape[-1], (0 if x1 is None else x1.shape[-1])
+        d.cin, d.cout = int(cin), (w.shape[1] if transposed else w.shape[0])
+        d.ld_out, d.ch_off, d.n_tile, d.alt_tile = int(ld_out), int(ch_off), int(n_tile), int(alt_tile)
+        width = int(ld_out) or d.cout
+        if x0.dim() == 2:
+            d.tokens = x0.shape[0]
+            shape = (x0.shape[0], width)
+        else:
+            d.batch, d.src_h, d.src_w = x0.shape[0], x0.shape[1], x0.shape[2]
+            d.height, d.width = (d.src_h, d.src_w) if stride == 1 else ((d.src_h + 1) // 2, (d.src_w + 1) // 2)
+            shape = (d.batch, 2 * d.height, 2 * d.width, d.cout) if transposed else (d.batch, d.height, d.width, width)
+        if y32 is True:
+            y32 = torch.full(shape, float("nan"), device=dev)
+        if planes is True:
+            planes = tuple(torch.zeros(shape, dtype=torch.float16, device=dev) for _ in range(2))
+        y32 = None if y32 is False else y32
+        planes = None if planes is False else planes
+        info = (C.c_int32 * 4)()
+        bn_ptrs = None if bn is None else (C.c_void_p * 4)(*[t.data_ptr() for t in bn])
+
+        def ptr(t):
+            return C.c_void_p(0 if t is None else t.data_ptr())
+
+        _cabi.check(self.lib.dd_gen_layer(self._h, C.byref(d), ptr(x0), ptr(x1), ptr(w), ptr(bias), bn_ptrs, ptr(add),
+                                          ptr(y32), ptr(planes[0] if planes else None),
+                                          ptr(planes[1] if planes else None), info, C.c_void_p(self._stream())))
+        return y32, planes, {"nt": info[0], "work": info[1], "grid": info[2], "parts": info[3]}
+
+    def window_attention(self, qkv: torch.Tensor, qkv_bias: torch.Tensor, table: torch.Tensor, batch: int,
+                         hw: Sequence[int], num_heads: int, shift: int, kernel: int = 0):
+        """Swin (shifted-)window attention on the engine's kernels (dd_window_attention): qkv [B*H*W, 3C] fp32 (padded
+        tokens carry qkv_bias [3C]), table [169, nH].  kernel: 0 the engine's choice, 1 fp32 CUDA cores, 2 wgmma.
+        Returns (out [B*H*W, C] fp32, {"work", "grid"})."""
+        qkv, qkv_bias, table = (t.detach().to(self.device, torch.float32).contiguous() for t in (qkv, qkv_bias, table))
+        out = torch.empty(qkv.shape[0], qkv.shape[1] // 3, device=self.device, dtype=torch.float32)
+        info = (C.c_int32 * 2)()
+        _cabi.check(self.lib.dd_window_attention(self._h, C.c_void_p(qkv.data_ptr()), C.c_void_p(qkv_bias.data_ptr()),
+                                                 C.c_void_p(table.data_ptr()), C.c_void_p(out.data_ptr()), int(batch),
+                                                 int(hw[0]), int(hw[1]), int(num_heads), int(shift), int(kernel), info,
+                                                 C.c_void_p(self._stream())))
+        return out, {"work": info[0], "grid": info[1]}
+
     def bench_conv(self, cin: int, cout: int, iters: int = 20) -> float:
         """Average milliseconds per launch of the (cin -> cout) conv on this engine's latent grid."""
         ms = C.c_float()

@@ -309,6 +309,50 @@ int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, fl
                      void* cuda_stream);
 size_t dd_conv3x3_wgrad_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int32_t height, int32_t width);
 
+/* One layer of the producers (backbone, HAHI neck, FPN) on their tensor-core conv / GEMM kernel, described by: */
+typedef struct dd_gen_layer_desc {
+  int32_t taps;                 /* 1 (1x1 conv, Linear) or 9 (3x3, pad 1) */
+  int32_t stride;               /* 1, or 2 (conv mode, one source, not transposed) */
+  int32_t transposed;           /* 1: ConvTranspose2d(k=2, s=2), taps 1, one source; pixel-shuffled output */
+  int32_t act;                  /* 0 none, 1 ReLU, 2 exact (erf) GELU, 3 Hardswish */
+  int32_t add_first;            /* 1: the addend goes in before the activation, 0: after it */
+  int32_t tokens;               /* > 0: GEMM mode on that many token rows (batch .. src_w ignored) */
+  int32_t batch, height, width; /* conv mode: the output grid */
+  int32_t src_h, src_w;         /* stride 2: the source grid */
+  int32_t c0, c1;               /* channels of source 0 and of source 1 (concatenated after it; 0: none) */
+  int32_t cin;                  /* the weight's input channels: 0 = c0 + c1; below c0 (one source) zero-pads it to c0 */
+  int32_t cout;                 /* output channels (transposed: per output pixel) */
+  int32_t ld_out, ch_off;       /* output rows are ld_out channels wide (0: cout), written from channel ch_off */
+  int32_t n_tile;               /* N-tile width 64 / 128 / 192 / 256, 0: the engine's choice */
+  int32_t alt_tile;             /* layers with 192-wide alternative maps: 0 by wave cost, 1 always, -1 never */
+} dd_gen_layer_desc;
+
+/* Standalone run of that kernel for layer tests, packing and launching the layer exactly as the engine does:
+ *   x0 [tokens][c0] or [B][src grid][c0], x1 [.. output grid ..][c1] (nullable when c1 = 0): device fp32 NHWC, split at
+ *      the producers' scale;
+ *   w  the reference layout: conv [cout][cin][k][k], Linear [cout][cin], ConvT [c0][cout][2][2];
+ *   bn (nullable) four device vectors [cout] (weight, bias, running_mean, running_var) of an eval-BN folded after the
+ *      conv, otherwise bias [cout] (nullable);
+ *   add32 (nullable) fp32 addend, dense [rows][cout] (transposed: [B][2H][2W][cout]);
+ *   y32 fp32 and / or out_hi, out_lo fp16 planes (at the producers' scale) of [rows][ld_out]: only the layer's rows
+ *      (not the GEMM tail) and channels [ch_off, ch_off + cout) are written (transposed: [B][2H][2W][cout]).
+ * launch_out (nullable) receives {N-tile width, work items, grid, launches}: a layer deeper than one fp32 accumulator
+ * should take runs as that many launches over channel ranges, summed in fp32 in a fixed order.  Allocates and frees its own buffers, touches neither
+ * the workspace nor the packed weights; synchronises `cuda_stream` and returns DD_ERR_RANGE when an input or an output
+ * plane held a non-finite value or left the split's range. */
+int dd_gen_layer(dd_handle h, const dd_gen_layer_desc* d, const float* x0, const float* x1, const float* w,
+                 const float* bias, const float* const* bn, const float* add32, float* y32, void* out_hi, void* out_lo,
+                 int32_t* launch_out, void* cuda_stream);
+
+/* Standalone (shifted-)window attention of a Swin block (7 x 7 windows, head_dim 32, C = 32 nH): qkv [B*H*W][3C] (device
+ * fp32, the qkv Linear's output; padded tokens carry qkv_bias [3C]), table [169][nH] -> out [B*H*W][C] fp32, rebuilt from
+ * the kernel's hi/lo output planes.  kernel: 0 the engine's choice, 1 the fp32 CUDA-core kernel, 2 the wgmma kernel (nH
+ * even).  launch_out (nullable) receives {units of work, grid}.  Allocates and frees its own buffers; synchronises and
+ * returns DD_ERR_RANGE as dd_gen_layer does. */
+int dd_window_attention(dd_handle h, const float* qkv, const float* qkv_bias, const float* table, float* out,
+                        int32_t batch, int32_t height, int32_t width, int32_t num_heads, int32_t shift, int32_t kernel,
+                        int32_t* launch_out, void* cuda_stream);
+
 /* Time the dominant kernel (convA-shaped 256->256 3x3 on the engine's latent grid) `iters` times with
  * CUDA events on `cuda_stream`; returns average milliseconds per launch in *ms_out. */
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,
