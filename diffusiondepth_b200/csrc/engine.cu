@@ -912,7 +912,7 @@ int run_fold(dd_engine* e, cudaStream_t st) {
   r.wp = e->L[4].w_simt;
   r.y32 = e->Y;
   r.ring_partial = e->stats[3];
-  dd::ring_fix_kernel<<<dim3(r.blocks_per_img, g.B), 256, dd::RING_SMEM, st>>>(r);
+  dd::ring_fix_kernel<<<dim3(r.blocks_per_img, g.B), dd::RING_THREADS, dd::RING_SMEM, st>>>(r);
   return launched(e, "ring_fix");
 }
 

@@ -276,7 +276,14 @@ conv5x5_fold_kernel(const __grid_constant__ CUtensorMap tmP_hi, const __grid_con
 constexpr int RING_S = 16;
 constexpr int RING_BOX = RING_S + 2;   // outside positions q of a segment: 3 x (n + 2) box around it
 constexpr int RING_ABOX = RING_S + 4;  // a(q + d'): 5 x (n + 4) box
-constexpr int RING_SMEM = (5 * RING_ABOX + 3 * RING_BOX + 2) * 256 * 4;
+// Each convB output channel cm of b_ext is worked by RING_JG threads, one per slice of RING_JB box columns: the 156 KB
+// of boxes allow one block per SM, and with one thread per cm its 8 warps, each waiting on L2 for its weights every 4
+// input channels, ran the kernel at ~3 TFLOP/s.  Every sum keeps its operand order, so the result does not depend on
+// RING_JG.
+constexpr int RING_JG = 4;
+constexpr int RING_JB = (RING_BOX + RING_JG - 1) / RING_JG;
+constexpr int RING_THREADS = 256 * RING_JG;
+constexpr int RING_SMEM = (5 * RING_ABOX + 3 * RING_BOX + 2) * 256 * 4 + RING_S * 64 * 4;
 
 struct RingSide {
   int y0, x0, vert, len;
@@ -318,12 +325,13 @@ struct RingArgs {
 
 __device__ __forceinline__ bool inside_img(int y, int x, int H, int W) { return y >= 0 && y < H && x >= 0 && x < W; }
 
-// grid (blocks_per_img, B), 256 threads
-__global__ void __launch_bounds__(256) ring_fix_kernel(const RingArgs p) {
+// grid (blocks_per_img, B), RING_THREADS threads
+__global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p) {
   extern __shared__ float4 ring_smem4[];
   float* abox = reinterpret_cast<float*>(ring_smem4);  // [5][RING_ABOX][256]
   float* bbox = abox + 5 * RING_ABOX * 256;           // [3][RING_BOX][256]
   float* red = bbox + 3 * RING_BOX * 256;             // [2][256]
+  float* ycor = red + 2 * 256;                        // [RING_S][64] corrected outputs of the segment
   const int img = blockIdx.y, t = threadIdx.x;
   const int H = p.H, W = p.W;
   RingSide sd[4];
@@ -343,7 +351,7 @@ __global__ void __launch_bounds__(256) ring_fix_kernel(const RingArgs p) {
     const int oy = sd[si].y0 + k * RING_S * ly, ox = sd[si].x0 + k * RING_S * lx;
     __syncthreads();  // the previous segment's shared-memory reads are done
     // a on the 5 x (n + 4) box, zero outside the image, reconstructed from the split planes as the convs read it
-    for (int i = t; i < 5 * RING_ABOX * 32; i += 256) {
+    for (int i = t; i < 5 * RING_ABOX * 32; i += RING_THREADS) {
       const int c8 = i & 31, pos = i >> 5;
       const int r = pos / RING_ABOX - 2, c = pos % RING_ABOX - 2;
       const int y = oy + r * ay + c * ly, x = ox + r * ax + c * lx;
@@ -362,31 +370,35 @@ __global__ void __launch_bounds__(256) ring_fix_kernel(const RingArgs p) {
       d[1] = make_float4(v[4], v[5], v[6], v[7]);
     }
     __syncthreads();
-    // b_ext at the box's outside positions, one box row at a time; thread = convB output channel cm
-    const int cm = t;
+    // b_ext at the box's outside positions, one box row at a time; thread = (convB output channel cm, box columns
+    // [j0, j0 + RING_JB))
+    const int cm = t & 255, j0 = (t >> 8) * RING_JB;
     for (int r = -1; r <= 1; ++r) {
       uint32_t omask = 0;
-      for (int j = 0; j < n + 2; ++j)
-        if (!inside_img(oy + r * ay + (j - 1) * ly, ox + r * ax + (j - 1) * lx, H, W)) omask |= 1u << j;
+      for (int j = j0; j < min(n + 2, j0 + RING_JB); ++j)
+        if (!inside_img(oy + r * ay + (j - 1) * ly, ox + r * ax + (j - 1) * lx, H, W)) omask |= 1u << (j - j0);
       if (omask == 0) continue;
-      float acc[RING_BOX];
+      float acc[RING_JB];
 #pragma unroll
-      for (int j = 0; j < RING_BOX; ++j) acc[j] = 0.f;
+      for (int j = 0; j < RING_JB; ++j) acc[j] = 0.f;
       for (int tp = 0; tp < 9; ++tp) {
         const int rr = tp / 3 - 1, cc = tp % 3 - 1;  // box offset (across, along)
         uint32_t vmask = 0;
-        for (int j = 0; j < n + 2; ++j)
-          if (((omask >> j) & 1u) && inside_img(oy + (r + rr) * ay + (j - 1 + cc) * ly, ox + (r + rr) * ax + (j - 1 + cc) * lx, H, W))
+        for (int j = 0; j < RING_JB; ++j) {
+          const int jb = j0 + j;
+          if (((omask >> j) & 1u) && inside_img(oy + (r + rr) * ay + (jb - 1 + cc) * ly, ox + (r + rr) * ax + (jb - 1 + cc) * lx, H, W))
             vmask |= 1u << j;
+        }
         if (vmask == 0) continue;
         const int dy = rr * ay + cc * ly, dx = rr * ax + cc * lx;
         const float* wt = p.wb + static_cast<size_t>((dy + 1) * 3 + (dx + 1)) * 65536 + cm;
-        const float* arow = abox + ((r + rr + 2) * RING_ABOX + cc + 1) * 256;  // box column of j = 0
+        const float* arow = abox + ((r + rr + 2) * RING_ABOX + j0 + cc + 1) * 256;  // box column of j = j0
+#pragma unroll 4
         for (int ci = 0; ci < 256; ci += 4) {
           const float w0 = __ldg(wt + (ci + 0) * 256), w1 = __ldg(wt + (ci + 1) * 256);
           const float w2 = __ldg(wt + (ci + 2) * 256), w3 = __ldg(wt + (ci + 3) * 256);
 #pragma unroll
-          for (int j = 0; j < RING_BOX; ++j)
+          for (int j = 0; j < RING_JB; ++j)
             if ((vmask >> j) & 1u) {
               const float4 av = *reinterpret_cast<const float4*>(arow + j * 256 + ci);
               acc[j] = fmaf(w3, av.w, fmaf(w2, av.z, fmaf(w1, av.y, fmaf(w0, av.x, acc[j]))));
@@ -395,13 +407,13 @@ __global__ void __launch_bounds__(256) ring_fix_kernel(const RingArgs p) {
       }
       const float bias = __ldg(p.bb + cm);
 #pragma unroll
-      for (int j = 0; j < RING_BOX; ++j)
-        if ((omask >> j) & 1u) bbox[((r + 1) * RING_BOX + j) * 256 + cm] = acc[j] + bias;
+      for (int j = 0; j < RING_JB; ++j)
+        if ((omask >> j) & 1u) bbox[((r + 1) * RING_BOX + j0 + j) * 256 + cm] = acc[j] + bias;
     }
     __syncthreads();
-    // y(p) -= sum over pred.0 taps that land outside; thread = (output channel, every 4th pixel of the segment)
+    // y(p) -= sum over pred.0 taps that land outside; thread = (output channel, every RING_THREADS / 64-th pixel)
     const int co = t & 63;
-    for (int j = t >> 6; j < n; j += 4) {
+    for (int j = t >> 6; j < n; j += RING_THREADS / 64) {
       const int y = oy + j * ly, x = ox + j * lx;
       float corr = 0.f;
       for (int tp = 0; tp < 9; ++tp) {
@@ -421,13 +433,22 @@ __global__ void __launch_bounds__(256) ring_fix_kernel(const RingArgs p) {
       float* yp = p.y32 + ((static_cast<size_t>(img) * H + y) * W + x) * 64 + co;
       const float v = *yp - corr;
       *yp = v;
-      ts += v;
-      tq = fmaf(v, v, tq);
+      ycor[j * 64 + co] = v;
     }
+    __syncthreads();
+    // GroupNorm sums: thread t < 256 takes every 4th pixel, in the same order whatever RING_THREADS is
+    if (t < 256)
+      for (int j = t >> 6; j < n; j += 4) {
+        const float v = ycor[j * 64 + co];
+        ts += v;
+        tq = fmaf(v, v, tq);
+      }
   }
   // GroupNorm partials of this block's ring pixels, summed in a fixed order
-  red[t] = ts;
-  red[256 + t] = tq;
+  if (t < 256) {
+    red[t] = ts;
+    red[256 + t] = tq;
+  }
   __syncthreads();
   if (t < 8) {
     const int g = t >> 1, which = t & 1;
