@@ -377,12 +377,17 @@ struct MpStageW {
   GenLayer pe_pw[4], inv1, inv2, agg;
   MpEncoderW enc[4];
 };
+constexpr int kMpHeads = 8;        // MPViT's attention heads in every stage
+constexpr int kMpChunksMax = 256;  // token chunks of the factorised attention's reductions
+// the factorised attention's token-chunk partials, sized for kMpChunksMax chunks
+struct FactorAttBufs {
+  float *part_m = nullptr, *part_s = nullptr, *colinv = nullptr, *part_ktv = nullptr, *ktv = nullptr;
+};
 struct MPViTW {
   bool enabled = false, ready = false;
-  int H = 0, W = 0, heads = 8, mlp_ratio = 4;
+  int H = 0, W = 0, heads = kMpHeads, mlp_ratio = 4;
   int dims[4] = {0, 0, 0, 0}, out_dims[4] = {0, 0, 0, 0}, layers[4] = {0, 0, 0, 0}, paths[4] = {0, 0, 0, 0};
   int Hs[4] = {0, 0, 0, 0}, Ws[4] = {0, 0, 0, 0};
-  int radius[16] = {0};     // crpe window / 2 per head ({3: 2, 5: 3, 7: 3} heads)
   GenLayer stem0, stem1;
   MpStageW stage[4];
   // workspace views
@@ -391,9 +396,8 @@ struct MPViTW {
   float* E[4] = {nullptr, nullptr, nullptr, nullptr};  // the paths' token maps + one swap buffer
   float* R1 = nullptr;
   float* QKV = nullptr;
-  float *part_m = nullptr, *part_s = nullptr, *colinv = nullptr, *part_ktv = nullptr, *ktv = nullptr;
+  FactorAttBufs fab;
 };
-constexpr int kMpChunksMax = 256;  // token chunks of the factorised attention's reductions
 
 }  // namespace
 
@@ -717,11 +721,11 @@ size_t carve(dd_engine* e, void* base) {
     planes(mv->HP, tok * mc.mlp_ratio);
     planes(mv->CAT, cat);
     const size_t chm = static_cast<size_t>(cmax / mc.heads), nk = static_cast<size_t>(mc.heads) * chm * chm;
-    mv->part_m = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * cmax);
-    mv->part_s = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * cmax);
-    mv->colinv = c.take<float>(static_cast<size_t>(g.B) * cmax);
-    mv->part_ktv = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * nk);
-    mv->ktv = c.take<float>(static_cast<size_t>(g.B) * nk);
+    mv->fab.part_m = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * cmax);
+    mv->fab.part_s = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * cmax);
+    mv->fab.colinv = c.take<float>(static_cast<size_t>(g.B) * cmax);
+    mv->fab.part_ktv = c.take<float>(static_cast<size_t>(g.B) * kMpChunksMax * nk);
+    mv->fab.ktv = c.take<float>(static_cast<size_t>(g.B) * nk);
   }
   if (has_backward(e->cfg)) {
     dd_engine::Bwd* bv = &v->bw;
@@ -3168,6 +3172,91 @@ int dd_window_attention(dd_handle h, const float* qkv, const float* qkv_bias, co
     launch_out[1] = grid;
   }
   return DD_OK;
+}
+
+int dd_factor_attention(dd_handle h, const float* qkv, const float* const* crpe_w, const float* const* crpe_b, float* out,
+                        int32_t batch, int32_t height, int32_t width, int32_t channels, int32_t* launch_out,
+                        void* cuda_stream) {
+  if (!h || !qkv || !crpe_w || !crpe_b || !out) return fail(DD_ERR_INVALID, "null argument");
+  for (int g = 0; g < 3; ++g)
+    if (!crpe_w[g] || !crpe_b[g]) return fail(DD_ERR_INVALID, "null argument");
+  if (batch < 1 || height < 1 || width < 1 || channels < 1) return fail(DD_ERR_INVALID, "bad attention geometry");
+  if (channels % kMpHeads != 0 || channels / kMpHeads > dd::KTV_CH_MAX)
+    return fail(DD_ERR_UNSUPPORTED, "factorised attention: channels must be a multiple of 8 (8 heads), at most 512");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const int C = channels, Ch = C / kMpHeads;
+  const size_t n = static_cast<size_t>(batch) * height * width * C;
+  const size_t nk = static_cast<size_t>(batch) * kMpHeads * Ch * Ch;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  float *cw = nullptr, *cb = nullptr;
+  if ((rc = pack_crpe(call.owned, crpe_w, crpe_b, C, cw, cb, st))) return rc;
+  FactorAttBufs bf;
+  if ((rc = call.alloc(&bf.part_m, static_cast<size_t>(batch) * kMpChunksMax * C)) ||
+      (rc = call.alloc(&bf.part_s, static_cast<size_t>(batch) * kMpChunksMax * C)) ||
+      (rc = call.alloc(&bf.colinv, static_cast<size_t>(batch) * C)) ||
+      (rc = call.alloc(&bf.part_ktv, nk * kMpChunksMax)) || (rc = call.alloc(&bf.ktv, nk)))
+    return rc;
+  Planes o;
+  if ((rc = call.alloc(&o.hi, n)) || (rc = call.alloc(&o.lo, n))) return rc;
+  int info[4];
+  if ((rc = run_factor_att(h, qkv, cw, cb, bf, o, batch, height, width, C, st, info))) return rc;
+  dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
+  if ((rc = check_launch("join_planes"))) return rc;
+  if ((rc = call.finish(st, "qkv or the attention output"))) return rc;
+  if (launch_out)
+    for (int i = 0; i < 4; ++i) launch_out[i] = info[i];
+  return DD_OK;
+}
+
+int dd_depthwise_conv(dd_handle h, const float* x, const float* w, const float* bias, const float* const* bn, float* y32,
+                      void* out_hi, void* out_lo, int32_t batch, int32_t height, int32_t width, int32_t channels,
+                      int32_t stride, int32_t act, int32_t residual, int32_t* launch_out, void* cuda_stream) {
+  if (!h || !x || !w) return fail(DD_ERR_INVALID, "null argument");
+  if (!y32 && !(out_hi && out_lo)) return fail(DD_ERR_INVALID, "no output");
+  if (bn && bias) return fail(DD_ERR_INVALID, "a bias or an eval-BN, not both");
+  if (bn && !(bn[0] && bn[1] && bn[2] && bn[3])) return fail(DD_ERR_INVALID, "null argument");
+  if (batch < 1 || height < 1 || width < 1 || channels < 1 || (stride != 1 && stride != 2) || (act != 0 && act != 3) ||
+      (residual != 0 && residual != 1) || (residual && stride != 1))
+    return fail(DD_ERR_INVALID, "bad depthwise conv descriptor");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  DwLayer L;
+  if ((rc = pack_dw(call.owned, L, w, bn, bias, channels, 3, "standalone depthwise conv", st))) return rc;
+  const Planes o{static_cast<__half*>(out_hi), static_cast<__half*>(out_lo)};
+  int info[2];
+  if ((rc = run_dw(h, L, x, batch, height, width, stride, act, residual, y32, (out_hi && out_lo) ? &o : nullptr, st,
+                   info)))
+    return rc;
+  if ((rc = call.finish(st, "the depthwise conv output"))) return rc;
+  if (launch_out) {
+    launch_out[0] = info[0];
+    launch_out[1] = info[1];
+  }
+  return DD_OK;
+}
+
+int dd_layer_norm(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, int32_t tokens,
+                  int32_t channels, float eps, void* cuda_stream) {
+  if (!h || !x || !gamma || !beta || !out) return fail(DD_ERR_INVALID, "null argument");
+  if (tokens < 1 || channels < 1 || !(eps > 0.f)) return fail(DD_ERR_INVALID, "bad LayerNorm geometry");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const size_t n = static_cast<size_t>(tokens) * channels;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  Planes o;
+  if ((rc = call.alloc(&o.hi, n)) || (rc = call.alloc(&o.lo, n))) return rc;
+  if ((rc = run_ln_generic(h, channels, x, gamma, beta, o, tokens, eps, st))) return rc;
+  dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
+  if ((rc = check_launch("join_planes"))) return rc;
+  return call.finish(st, "x or the LayerNorm output");
 }
 
 int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,

@@ -118,12 +118,22 @@ __global__ void __launch_bounds__(256) ln_split_generic_kernel(const float* __re
     s += v[i];
   }
   const float inv_c = 1.f / static_cast<float>(C);
-  const float mean = warp_sum(s) * inv_c;
+  // The mean in two parts: the fp32 mean m0, then the mean mc of v - m0.  A row with a large mean and a small spread
+  // (1e3 +- 1e-2) would otherwise lose the spread to m0's rounding (~1e-4 there), and a constant row would come out as
+  // rounding noise times rsqrt(eps) instead of beta; v - m0 is exact for v within a factor 2 of m0.
+  const float m0 = warp_sum(s) * inv_c;
+  float s1 = 0.f;
+#pragma unroll
+  for (int i = 0; i < VMAX; ++i) {
+    v[i] = (lane + 32 * i < C) ? v[i] - m0 : 0.f;
+    s1 += v[i];
+  }
+  const float mc = warp_sum(s1) * inv_c;
   float s2 = 0.f;
 #pragma unroll
   for (int i = 0; i < VMAX; ++i) {
-    const float d = (lane + 32 * i < C) ? v[i] - mean : 0.f;
-    s2 = fmaf(d, d, s2);
+    v[i] = (lane + 32 * i < C) ? v[i] - mc : 0.f;
+    s2 = fmaf(v[i], v[i], s2);
   }
   const float rstd = rsqrtf(warp_sum(s2) * inv_c + eps);
   bool ov = false;
@@ -131,7 +141,7 @@ __global__ void __launch_bounds__(256) ln_split_generic_kernel(const float* __re
   for (int i = 0; i < VMAX; ++i) {
     const int c = lane + 32 * i;
     if (c < C) {
-      const float y = (v[i] - mean) * rstd * gamma[c] + beta[c];
+      const float y = v[i] * rstd * gamma[c] + beta[c];
       __half h, l;
       split_f16(y, scale, h, l, ov);
       hi[static_cast<size_t>(token) * C + c] = h;

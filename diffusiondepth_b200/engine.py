@@ -508,6 +508,61 @@ class DenoiseEngine:
                                                  C.c_void_p(self._stream())))
         return out, {"work": info[0], "grid": info[1]}
 
+    def factor_attention(self, qkv: torch.Tensor, crpe_w: Sequence[torch.Tensor], crpe_b: Sequence[torch.Tensor],
+                         batch: int, hw: Sequence[int]):
+        """MPViT's factorised attention with convolutional relative position encoding on the engine's kernels
+        (dd_factor_attention; 8 heads, crpe windows {3: 2, 5: 3, 7: 3}): qkv [B*H*W, 3C] fp32, crpe_w / crpe_b the three
+        crpe.conv_list weights [nh*Ch, 1, k, k] / biases.  Returns (out [B*H*W, C] fp32, {"tpc", "chunks", "hb",
+        "grid"})."""
+        def f32(t):
+            return t.detach().to(self.device, torch.float32).contiguous()
+
+        qkv, crpe_w, crpe_b = f32(qkv), [f32(t) for t in crpe_w], [f32(t) for t in crpe_b]
+        out = torch.empty(qkv.shape[0], qkv.shape[1] // 3, device=self.device, dtype=torch.float32)
+        info = (C.c_int32 * 4)()
+        _cabi.check(self.lib.dd_factor_attention(self._h, C.c_void_p(qkv.data_ptr()),
+                                                 (C.c_void_p * 3)(*[t.data_ptr() for t in crpe_w]),
+                                                 (C.c_void_p * 3)(*[t.data_ptr() for t in crpe_b]),
+                                                 C.c_void_p(out.data_ptr()), int(batch), int(hw[0]), int(hw[1]),
+                                                 out.shape[1], info, C.c_void_p(self._stream())))
+        return out, {"tpc": info[0], "chunks": info[1], "hb": info[2], "grid": info[3]}
+
+    def depthwise_conv(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, bn=None,
+                       stride: int = 1, act: int = 0, residual: bool = False, y32=True, planes=False):
+        """MPViT's depthwise 3x3 conv on the engine's kernel (dd_depthwise_conv): x [B, H, W, C] fp32 NHWC, w [C, 1, 3,
+        3], then bn = (weight, bias, running_mean, running_var) folded or `bias`; act 0 / 3 (Hardswish); residual adds x
+        (stride 1).  y32 / planes: True allocates the output (planes: fp16 hi / lo at the producers' scale), False skips
+        it.  Returns (y32, (hi, lo), {"grid", "work"}) with None for a skipped output."""
+        def f32(t):
+            return None if t is None else t.detach().to(self.device, torch.float32).contiguous()
+
+        def ptr(t):
+            return C.c_void_p(0 if t is None else t.data_ptr())
+
+        x, w, bias = f32(x), f32(w), f32(bias)
+        bn = None if bn is None else [f32(t) for t in bn]
+        B, H, W, Cc = x.shape
+        shape = (B, (H - 1) // stride + 1, (W - 1) // stride + 1, Cc)
+        y32 = torch.full(shape, float("nan"), device=self.device) if y32 else None
+        planes = tuple(torch.zeros(shape, dtype=torch.float16, device=self.device) for _ in range(2)) if planes else None
+        info = (C.c_int32 * 2)()
+        bn_ptrs = None if bn is None else (C.c_void_p * 4)(*[t.data_ptr() for t in bn])
+        _cabi.check(self.lib.dd_depthwise_conv(self._h, ptr(x), ptr(w), ptr(bias), bn_ptrs, ptr(y32),
+                                               ptr(planes[0] if planes else None), ptr(planes[1] if planes else None),
+                                               B, H, W, Cc, int(stride), int(act), int(residual), info,
+                                               C.c_void_p(self._stream())))
+        return y32, planes, {"grid": info[0], "work": info[1]}
+
+    def layer_norm(self, x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
+        """LayerNorm over the last axis on the MPViT encoders' kernel (dd_layer_norm, C <= 512): x [M, C] fp32 ->
+        fp32 [M, C], rebuilt from the kernel's hi / lo planes."""
+        x, gamma, beta = (t.detach().to(self.device, torch.float32).contiguous() for t in (x, gamma, beta))
+        out = torch.empty_like(x)
+        _cabi.check(self.lib.dd_layer_norm(self._h, C.c_void_p(x.data_ptr()), C.c_void_p(gamma.data_ptr()),
+                                           C.c_void_p(beta.data_ptr()), C.c_void_p(out.data_ptr()), x.shape[0],
+                                           x.shape[1], float(eps), C.c_void_p(self._stream())))
+        return out
+
     def bench_conv(self, cin: int, cout: int, iters: int = 20) -> float:
         """Average milliseconds per launch of the (cin -> cout) conv on this engine's latent grid."""
         ms = C.c_float()

@@ -353,6 +353,35 @@ int dd_window_attention(dd_handle h, const float* qkv, const float* qkv_bias, co
                         int32_t batch, int32_t height, int32_t width, int32_t num_heads, int32_t shift, int32_t kernel,
                         int32_t* launch_out, void* cuda_stream);
 
+/* Standalone factorised attention of an MPViT encoder layer (8 heads, crpe windows {3: 2 heads, 5: 3, 7: 3}, C = 8 Ch,
+ * Ch <= 64), through the backbone's own launch sequence: qkv [B*H*W][3C] (device fp32, the qkv Linear's output, q | k |
+ * v head-major), crpe_w[g] / crpe_b[g] the reference's crpe.conv_list.{0,1,2}.weight [nh Ch][1][k][k] / .bias [nh Ch]
+ * -> out [B*H*W][C] = Ch^-0.5 q (softmax over the tokens of k)^T v + q * crpe(v) in fp32, rebuilt from the kernel's hi/lo
+ * output planes.  launch_out (nullable) receives {tokens per chunk, chunks, heads per k^T v block, apply grid}.
+ * DD_ERR_UNSUPPORTED for C not a multiple of 8 or above 512.  Allocates and frees its own buffers; synchronises and
+ * returns DD_ERR_RANGE as dd_gen_layer does. */
+int dd_factor_attention(dd_handle h, const float* qkv, const float* const* crpe_w, const float* const* crpe_b, float* out,
+                        int32_t batch, int32_t height, int32_t width, int32_t channels, int32_t* launch_out,
+                        void* cuda_stream);
+
+/* Standalone depthwise 3x3 conv of the MPViT backbone (pad 1), packed and launched as the backbone does: x [B][H][W][C]
+ * (device fp32 NHWC, the source grid), w [C][1][3][3] followed by eval-BN bn (nullable: four device vectors [C] weight,
+ * bias, running_mean, running_var, folded) or by bias [C] (nullable; not both); stride 1 or 2; act 0 none, 3 Hardswish;
+ * residual 1 adds x before the activation (ConvPosEnc; stride 1 only) -> y32 fp32 and / or out_hi, out_lo fp16 planes
+ * (at the producers' scale) of [B][ceil(H / stride)][ceil(W / stride)][C].  launch_out (nullable) receives {grid, work
+ * items of 4 channels}.  DD_ERR_UNSUPPORTED for C not a multiple of 4.  Allocates and frees its own buffers;
+ * synchronises and returns DD_ERR_RANGE when an output plane held a non-finite value or left the split's range (an fp32
+ * output alone is not range-checked). */
+int dd_depthwise_conv(dd_handle h, const float* x, const float* w, const float* bias, const float* const* bn, float* y32,
+                      void* out_hi, void* out_lo, int32_t batch, int32_t height, int32_t width, int32_t channels,
+                      int32_t stride, int32_t act, int32_t residual, int32_t* launch_out, void* cuda_stream);
+
+/* Standalone LayerNorm of the MPViT encoders (any C <= 512): x [tokens][C] (device fp32), gamma / beta [C] -> out
+ * [tokens][C] fp32, rebuilt from the kernel's hi/lo output planes.  DD_ERR_UNSUPPORTED for C above 512.  Allocates and
+ * frees its own buffers; synchronises and returns DD_ERR_RANGE as dd_gen_layer does. */
+int dd_layer_norm(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, int32_t tokens,
+                  int32_t channels, float eps, void* cuda_stream);
+
 /* Time the dominant kernel (convA-shaped 256->256 3x3 on the engine's latent grid) `iters` times with
  * CUDA events on `cuda_stream`; returns average milliseconds per launch in *ms_out. */
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,

@@ -293,12 +293,14 @@ def test_native_resnet_backbone_and_resampling_fpn_vs_oracle(family, hw):
                     mod.running_var.fill_(1.0)
 
 
-@pytest.mark.parametrize("hw", [(64, 96), (70, 106)])
+@pytest.mark.parametrize("hw", [(64, 96), (70, 106), (228, 304)])
 def test_native_mpvit_backbone_vs_oracle(hw):
     """dd_run_backbone(kind = MPViT): full-resolution stem, chained depthwise-separable patch embeddings, conv path,
     factorised-attention encoders (token-axis softmax of k, k^T v, convolutional relative position encoding with 3 / 5 / 7
     windows), 1x1 aggregate — vs the fp64 restatement of reference backbone/mpvit.py:601-730, stage by stage; then neck +
-    FPN on the resulting planes.  70x106 -> 35x53 / 18x27 / 9x14 / 5x7: odd sizes on every level."""
+    FPN on the resulting planes.  70x106 -> 35x53 / 18x27 / 9x14 / 5x7: odd sizes on every level.  228x304 (an NYU
+    image): stage 0 at 114x152 = 17,328 tokens, past the 16,384 where the attention's token chunks grow beyond 64
+    tokens.  The restatement runs in fp64 on the GPU."""
     m = helpers.build_mirror("mpvit_s", 2).to(DEV)
     bb, head = m.depth_backbone, m.depth_head
     g = torch.Generator().manual_seed(41)
@@ -308,9 +310,9 @@ def test_native_mpvit_backbone_vs_oracle(hw):
             mod.running_mean.copy_(torch.randn(mod.running_mean.shape, generator=g) * 0.1)
             mod.running_var.copy_(torch.rand(mod.running_var.shape, generator=g) * 0.6 + 0.7)
     try:
-        sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
+        sd = {k: v.detach().clone() for k, v in m.state_dict().items()}
         rgb = torch.randn(2, 3, *hw, generator=g)
-        ref = restate.mpvit_backbone(sd, rgb.double(), "mpvit_small")
+        ref = restate.mpvit_backbone(sd, rgb.double().to(DEV), "mpvit_small")
         sizes = head.backbone_pyramid(hw, bb)
         assert [tuple(r.shape[-2:]) for r in ref] == sizes and head.can_run_backbone(bb, rgb.to(DEV))
         eng = head._engine(2, sizes[0], sizes[0], DEV, feats=([128, 216, 288, 288], sizes), image_hw=hw, backbone=bb)
@@ -319,12 +321,12 @@ def test_native_mpvit_backbone_vs_oracle(hw):
         errs = []
         for s, (f, r) in enumerate(zip(feats, ref)):
             assert f.shape == r.shape
-            errs.append((f.double().cpu() - r).abs().max().item() / r.abs().max().item())
+            errs.append((f.double() - r).abs().max().item() / r.abs().max().item())
         print("[mpvit stages] rel err", ["%.2e" % e for e in errs])
         assert max(errs) < 1e-4, errs
         c1 = eng.build_condition(None, want_cond=True)
         cref = restate.fpn_condition(sd, restate.hahi_neck(sd, ref))
-        err = (c1.double().cpu() - cref).abs().max().item() / cref.abs().max().item()
+        err = (c1.double() - cref).abs().max().item() / cref.abs().max().item()
         assert err < 1e-4, err
         feats2 = eng.run_backbone(rgb.to(DEV), want_feats=True)
         assert all(torch.equal(a, b) for a, b in zip(feats, feats2)), "run-to-run determinism"

@@ -221,6 +221,12 @@ CONVS = [
     Case("mpvit.pw.choff", 216, 216, B=1, H=6, W=10, bn=True, act=3, ld_out=864, ch_off=432, out="planes"),
     Case("mpvit.pw.choff.y32", 288, 288, B=2, H=3, W=5, bn=True, act=3, ld_out=1152, ch_off=288, out="both"),
     Case("mpvit.fc1.gelu", 216, 864, M=60, bias=True, act=2, out="planes"),
+    # MPViT encoder Linears at stage 0 of two KITTI 352x1216 images (2 x 176 x 608 tokens): qkv, proj + residual,
+    # fc1 + GELU to planes, fc2 + residual into the stage's concatenated planes (3 x 64 wide, path 1 at offset 128)
+    Case("mpvit.qkv.s0.M214016", 64, 192, M=214016, bias=True, out="y32"),
+    Case("mpvit.proj.s0.M214016", 64, 64, M=214016, bias=True, add="after", out="y32"),
+    Case("mpvit.fc1.s0.M214016", 64, 256, M=214016, bias=True, act=2, out="planes"),
+    Case("mpvit.fc2.s0.M214016", 256, 64, M=214016, bias=True, add="after", ld_out=192, ch_off=128, out="planes"),
 ]
 # one layer (ffn1 of stage 0: 768 = 3 x 256 = 4 x 192 columns) at every N-tile width; (n_tile, alt_tile, width hit)
 WIDTHS = [(64, -1, 64), (128, -1, 128), (192, -1, 192), (256, -1, 256), (0, -1, 256), (0, 1, 192)]
