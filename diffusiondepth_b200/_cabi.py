@@ -50,6 +50,8 @@ SIGNATURES = {
     "dd_destroy": (C.c_int, [C.c_void_p]),
     "dd_set_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32]),
     "dd_finalize_weights": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "dd_update_weights": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "dd_graph_capture_count": (C.c_int64, [C.c_void_p]),
     "dd_set_schedule": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_double),
                                   C.POINTER(C.c_double), C.c_int32]),
     "dd_workspace_bytes": (C.c_size_t, [C.c_void_p]),

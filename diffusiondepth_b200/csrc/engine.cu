@@ -278,6 +278,19 @@ struct ConvLayer {
   CUtensorMap mh_hi, mh_lo;  // box for the halo kernel's K chunk
 };
 
+// Pinned host side of the denoiser / codec pack, so that its copies are asynchronous and one synchronisation serves a
+// whole pack: the abs-max words of the conv weights, the decoder's and encoder's raw tensors as last registered (an
+// update re-reads only the registered ones; the BatchNorm folds need all of them), and what the host folds produce.
+struct PackStage {
+  float amax[16];  // slot i: conv layer i (0..5), 6 + i: its data-gradient layer, 12: the composed 5x5 conv
+  // device -> host
+  float dec_wt[16 * 16 * 16], dec_bt[16], dec_g[16], dec_be[16], dec_mu[16], dec_var[16], dec_wc[16 * 9], dec_bc[1];
+  float enc_w1[144], enc_bn1[4][16], enc_w2[2304], enc_bn2[4][16];
+  // host -> device
+  float wt_f[4 * 4 * 16 * 16], bt_f[16], wc_f[9 * 16], wu[4 * 4 * 16 * 16], bn[3 * 16];
+  float f1[144], t1[16], f2[2304], t2[16];
+};
+
 struct Raw {
   const float* ptr;
   std::vector<int64_t> shape;
@@ -410,6 +423,7 @@ struct dd_engine {
   // ignores the variables altogether
   int attn_simt = 0;     // DD_ATTN_SIMT=1 (probes build): window attention on the fp32 CUDA-core kernel
   bool weights_ready = false;
+  bool packed = false;  // a dd_finalize_weights has completed and its buffers are intact (dd_update_weights needs that)
   std::map<std::string, Raw> raw;
   // packed parameters (device memory owned by the engine)
   ConvLayer L[12];  // 0 ne.0, 1 ne.3, 2 convA, 3 convB, 4 pred.0, 5 pred.3; 6 + i: the data-gradient conv of layer i
@@ -418,7 +432,14 @@ struct dd_engine {
     __half* w = nullptr;     // packed K5 hi / lo (pred_fold.cuh)
     float* bias = nullptr;   // b5 [64]
     float wscale = 1.f;
+    float* src[2] = {nullptr, nullptr};  // convB's and pred.0's weights as registered: an update of one composes with the other
+    double* k5 = nullptr;                // [64][256][25] the composition in fp64, and its magnitudes for the scale
+    float* k5_abs = nullptr;
   } fold;
+  float* w_flip[6] = {};       // data-gradient layer 6 + i: layer i's weights flipped and transposed, before the split
+  float* amax = nullptr;       // [16] abs-max words of the pack (PackStage::amax)
+  PackStage* stage = nullptr;  // pinned
+  cudaEvent_t pack_done = nullptr;  // after the last pack's copies out of `stage`: the next pack's stream waits for it
   float* gn_gamma[4] = {nullptr, nullptr, nullptr, nullptr};  // ne.1, ne.4, pred.1, pred.4
   float* gn_beta[4] = {nullptr, nullptr, nullptr, nullptr};
   float* temb = nullptr;    // [1280][256]
@@ -470,6 +491,7 @@ struct dd_engine {
   enum { G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_COUNT = 4 };
   cudaGraphExec_t graphs[G_COUNT] = {nullptr, nullptr, nullptr, nullptr};
   int64_t graph_launches[G_COUNT] = {0, 0, 0, 0};  // kernel nodes per graph (added to `launches` per replay)
+  int64_t graph_captures = 0;                      // graph instantiations since dd_create (dd_graph_capture_count)
   cudaStream_t cap_stream = nullptr;  // capture happens here (the caller's stream may be the legacy default stream)
   float* rgb_stage = nullptr;         // workspace copy of the image batch the backbone graph reads
   float* inter = nullptr;             // [T][B][2h][2w] per-step decoded depth (DD_FLAG_STEP_DECODE)
@@ -572,12 +594,14 @@ int dec_act_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>
 int dec_wc_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P * 4 + dd::DEC_WC_PIX - 1) / dd::DEC_WC_PIX); }
 int dec_wt_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P + dd::DEC_WT_PIX - 1) / dd::DEC_WT_PIX); }
 
+void drop_graph(dd_engine* e, int which) {
+  if (e->graphs[which]) {
+    cudaGraphExecDestroy(e->graphs[which]);
+    e->graphs[which] = nullptr;
+  }
+}
 void drop_graphs(dd_engine* e) {
-  for (int i = 0; i < dd_engine::G_COUNT; ++i)
-    if (e->graphs[i]) {
-      cudaGraphExecDestroy(e->graphs[i]);
-      e->graphs[i] = nullptr;
-    }
+  for (int i = 0; i < dd_engine::G_COUNT; ++i) drop_graph(e, i);
 }
 
 // Capture `body(stream)` into graph slot `which` on first use, then replay it on `st`.  Every pointer the body's kernels
@@ -600,6 +624,7 @@ int graph_run(dd_engine* e, int which, cudaStream_t st, F&& body) {
     const cudaError_t ci = cudaGraphInstantiate(&e->graphs[which], graph, 0);
     cudaGraphDestroy(graph);
     if (ci != cudaSuccess) return fail(DD_ERR_CUDA, std::string("graph instantiate: ") + cudaGetErrorString(ci));
+    e->graph_captures++;
   }
   CUDA_TRY(cudaGraphLaunch(e->graphs[which], st));
   e->launches += e->graph_launches[which];
@@ -1052,28 +1077,36 @@ int dev_alloc(std::vector<void*>& owned, void** p, size_t bytes) {
 }
 int dev_alloc(dd_engine* e, void** p, size_t bytes) { return dev_alloc(e->owned, p, bytes); }
 
-int pack_layer(dd_engine* e, ConvLayer& L, const float* w, const float* b, int cout, int cin, cudaStream_t st,
-               float* scratch_dev) {
+template <typename T>
+int dev_array(dd_engine* e, T** p, size_t elems) {
+  return dev_alloc(e->owned, reinterpret_cast<void**>(p), elems * sizeof(T));
+}
+
+// The buffers and TMA descriptors of one conv layer; fill_pack writes the contents.
+int alloc_layer(dd_engine* e, ConvLayer& L, int cout, int cin) {
   L.sid = shape_id(cin, cout);
   if (L.sid < 0) return fail(DD_ERR_UNSUPPORTED, "unsupported conv shape");
   const size_t n = static_cast<size_t>(cout) * cin * 9;
   int rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_hi), n * 2))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_lo), n * 2))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.w_simt), n * 4))) return rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(&L.bias), cout * 4))) return rc;
-  if ((rc = split_scale_of(w, n, scratch_dev, st, &L.wscale))) return rc;
-  dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, L.w_hi, L.w_lo, L.w_simt, cout, cin, L.wscale);
-  if ((rc = check_launch("pack_conv_weight"))) return rc;
-  CUDA_TRY(cudaMemcpyAsync(L.bias, b, cout * 4, cudaMemcpyDeviceToDevice, st));
+  if ((rc = dev_array(e, &L.w_hi, n))) return rc;
+  if ((rc = dev_array(e, &L.w_lo, n))) return rc;
+  if ((rc = dev_array(e, &L.w_simt, n))) return rc;
+  if ((rc = dev_array(e, &L.bias, cout))) return rc;
   if ((rc = make_weight_map(&L.mh_hi, L.w_hi, cout, cin, 9, kHaloBK[L.sid], cout))) return rc;
   return make_weight_map(&L.mh_lo, L.w_lo, cout, cin, 9, kHaloBK[L.sid], cout);
 }
 
-
 // ------------------------------------------------------------------------------------------------ producers
 constexpr float kProdScale = 16.f;  // fp16-split pre-scale of every producer activation
 
+// Eval-BN (weight, bias, running_mean, running_var) = bn[0..3], host vectors of ch, as per-channel (scale, shift).
+void bn_fold_host(const float* const* bn, int ch, float* scale, float* shift) {
+  for (int c = 0; c < ch; ++c) {
+    const double sc = static_cast<double>(bn[0][c]) / sqrt(static_cast<double>(bn[3][c]) + 1e-5);
+    scale[c] = static_cast<float>(sc);
+    shift[c] = static_cast<float>(static_cast<double>(bn[1][c]) - static_cast<double>(bn[2][c]) * sc);
+  }
+}
 // Fold eval-BN, given as the device vectors bn[0..3] = (weight, bias, running_mean, running_var), into per-channel
 // (scale, shift) on the host.
 int bn_fold(const float* const* bn, int ch, std::vector<float>& scale, std::vector<float>& shift, cudaStream_t st) {
@@ -1085,11 +1118,8 @@ int bn_fold(const float* const* bn, int ch, std::vector<float>& scale, std::vect
   CUDA_TRY(cudaStreamSynchronize(st));
   scale.resize(ch);
   shift.resize(ch);
-  for (int c = 0; c < ch; ++c) {
-    const double sc = static_cast<double>(v[0][c]) / sqrt(static_cast<double>(v[3][c]) + 1e-5);
-    scale[c] = static_cast<float>(sc);
-    shift[c] = static_cast<float>(static_cast<double>(v[1][c]) - static_cast<double>(v[2][c]) * sc);
-  }
+  const float* host[4] = {v[0].data(), v[1].data(), v[2].data(), v[3].data()};
+  bn_fold_host(host, ch, scale.data(), shift.data());
   return DD_OK;
 }
 // the registered eval-BN vectors prefix.{weight,bias,running_mean,running_var} -> bn[0..3]
@@ -1102,12 +1132,261 @@ int find_bn(dd_engine* e, const std::string& prefix, const float** bn) {
   }
   return DD_OK;
 }
-int bn_fold(dd_engine* e, const std::string& prefix, int ch, std::vector<float>& scale, std::vector<float>& shift,
-            cudaStream_t st) {
-  const float* bn[4];
+
+// ------------------------------------------------------------------------------------------------ denoiser + codec pack
+// dd_finalize_weights allocates (alloc_pack) and fills (fill_pack) everything; dd_update_weights validates
+// (check_update) and fills what depends on the registered keys, at the same addresses.
+const char* const kGnKey[4] = {"model.noise_embedding.1", "model.noise_embedding.4", "model.pred.1", "model.pred.4"};
+constexpr int kGnCh[4] = {64, 256, 64, 16};
+const std::string kDecPrefix = "depth_transform.conv_inv_transform.";
+const std::string kEncPrefix = "depth_transform.conv_transform.";
+struct CodecKey {
+  const char* leaf;
+  size_t host_off;  // floats from the start of PackStage
+  std::vector<int64_t> shape;
+};
+#define DD_STAGE_OFF(m) (offsetof(PackStage, m) / sizeof(float))
+const CodecKey kDecKeys[8] = {{"0.weight", DD_STAGE_OFF(dec_wt), {16, 16, 4, 4}}, {"0.bias", DD_STAGE_OFF(dec_bt), {16}},
+                              {"1.weight", DD_STAGE_OFF(dec_g), {16}},            {"1.bias", DD_STAGE_OFF(dec_be), {16}},
+                              {"1.running_mean", DD_STAGE_OFF(dec_mu), {16}},     {"1.running_var", DD_STAGE_OFF(dec_var), {16}},
+                              {"3.0.weight", DD_STAGE_OFF(dec_wc), {1, 16, 3, 3}}, {"3.0.bias", DD_STAGE_OFF(dec_bc), {1}}};
+const CodecKey kEncKeys[10] = {
+    {"0.0.weight", DD_STAGE_OFF(enc_w1), {16, 1, 3, 3}},        {"0.1.weight", DD_STAGE_OFF(enc_bn1[0]), {16}},
+    {"0.1.bias", DD_STAGE_OFF(enc_bn1[1]), {16}},               {"0.1.running_mean", DD_STAGE_OFF(enc_bn1[2]), {16}},
+    {"0.1.running_var", DD_STAGE_OFF(enc_bn1[3]), {16}},        {"1.0.weight", DD_STAGE_OFF(enc_w2), {16, 16, 3, 3}},
+    {"1.1.weight", DD_STAGE_OFF(enc_bn2[0]), {16}},             {"1.1.bias", DD_STAGE_OFF(enc_bn2[1]), {16}},
+    {"1.1.running_mean", DD_STAGE_OFF(enc_bn2[2]), {16}},       {"1.1.running_var", DD_STAGE_OFF(enc_bn2[3]), {16}}};
+#undef DD_STAGE_OFF
+size_t numel(const std::vector<int64_t>& s) {
+  size_t n = 1;
+  for (int64_t d : s) n *= static_cast<size_t>(d);
+  return n;
+}
+
+int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
+  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
   int rc;
-  if ((rc = find_bn(e, prefix, bn))) return rc;
-  return bn_fold(bn, ch, scale, shift, st);
+  if ((rc = dev_array(h, &h->amax, 16))) return rc;
+  for (int i = 0; i < 6; ++i) {
+    if (!swin && (i == 2 || i == 3)) continue;
+    const int co = kConvCout[i], ci = kConvCin[i];
+    if ((rc = alloc_layer(h, h->L[i], co, ci))) return rc;
+    if (has_backward(h->cfg)) {
+      // data-gradient convs: W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] with zero bias, packed like any forward layer
+      if ((rc = dev_array(h, &h->w_flip[i], static_cast<size_t>(co) * ci * 9))) return rc;
+      if ((rc = alloc_layer(h, h->L[6 + i], ci, co))) return rc;
+      CUDA_TRY(cudaMemsetAsync(h->L[6 + i].bias, 0, ci * 4, st));
+    }
+  }
+  if (fold_active(h)) {
+    const size_t n5 = 64 * 256 * 25;
+    if ((rc = dev_array(h, &h->fold.w, dd::F5::W_ELEMS))) return rc;
+    if ((rc = dev_array(h, &h->fold.bias, 64))) return rc;
+    if ((rc = dev_array(h, &h->fold.src[0], 256 * 256 * 9))) return rc;
+    if ((rc = dev_array(h, &h->fold.src[1], 64 * 256 * 9))) return rc;
+    if ((rc = dev_array(h, &h->fold.k5, n5))) return rc;
+    if ((rc = dev_array(h, &h->fold.k5_abs, n5))) return rc;
+  }
+  for (int i = 0; i < 4; ++i) {
+    if ((rc = dev_array(h, &h->gn_gamma[i], kGnCh[i]))) return rc;
+    if ((rc = dev_array(h, &h->gn_beta[i], kGnCh[i]))) return rc;
+  }
+  if ((rc = dev_array(h, &h->temb, DD_TIME_ROWS * 256))) return rc;
+  if ((rc = dev_array(h, &h->dec_wt, 4 * 4 * 16 * 16))) return rc;
+  if ((rc = dev_array(h, &h->dec_bt, 16))) return rc;
+  if ((rc = dev_array(h, &h->dec_wc, 9 * 16))) return rc;
+  if (h->cfg.flags & DD_FLAG_LOOP_BACKWARD) {  // the decoder backward needs the BatchNorm unfolded
+    if ((rc = dev_array(h, &h->dec_wu, 4 * 4 * 16 * 16))) return rc;
+    if ((rc = dev_array(h, &h->dec_bu, 16))) return rc;
+    if ((rc = dev_array(h, &h->dec_bn, 3 * 16))) return rc;
+  }
+  h->enc_w1 = nullptr;
+  if (encoder) {
+    if ((rc = dev_array(h, &h->enc_w1, 144))) return rc;
+    if ((rc = dev_array(h, &h->enc_b1, 16))) return rc;
+    if ((rc = dev_array(h, &h->enc_w2, 2304))) return rc;
+    if ((rc = dev_array(h, &h->enc_b2, 16))) return rc;
+  }
+  return DD_OK;
+}
+
+// Every key registered for dd_update_weights belongs to the denoiser / codec pack and has the packed shape.
+int check_update(dd_engine* h) {
+  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
+  std::map<std::string, std::vector<int64_t>> want;
+  for (int i = 0; i < 6; ++i) {
+    if (!swin && (i == 2 || i == 3)) continue;
+    want[std::string(kConvKey[i]) + ".weight"] = {kConvCout[i], kConvCin[i], 3, 3};
+    want[std::string(kConvKey[i]) + ".bias"] = {kConvCout[i]};
+  }
+  for (int i = 0; i < 4; ++i) want[std::string(kGnKey[i]) + ".weight"] = want[std::string(kGnKey[i]) + ".bias"] = {kGnCh[i]};
+  want["model.time_embedding.weight"] = {DD_TIME_ROWS, 256};
+  for (const CodecKey& k : kDecKeys) want[kDecPrefix + k.leaf] = k.shape;
+  if (h->enc_w1)
+    for (const CodecKey& k : kEncKeys) want[kEncPrefix + k.leaf] = k.shape;
+  for (const auto& kv : h->raw) {
+    const std::string& name = kv.first;
+    for (const char* p : {"hahineck.", "conv_lateral.", "conv_up.", "backbone."})
+      if (name.compare(0, strlen(p), p) == 0)
+        return fail(DD_ERR_UNSUPPORTED, name + ": the neck, FPN and backbone are re-packed by dd_finalize_weights only");
+    auto it = want.find(name);
+    if (it == want.end()) return fail(DD_ERR_INVALID, name + " is not part of this engine's pack");
+    if (kv.second.shape != it->second) return fail(DD_ERR_INVALID, name + ": shape differs from the packed tensor");
+  }
+  return DD_OK;
+}
+
+// The loop graphs hold acc_scale = 1 / (in_scale * wscale) of the convs run_step launches, by value.
+bool loop_reads_wscale(const dd_engine* e, int layer) { return !(fold_active(e) && (layer == 3 || layer == 4)); }
+
+// Write every packed object that depends on a key in h->raw (dd_finalize_weights: all of them).  Enqueued on st with one
+// synchronisation in the middle, where the abs-max words and the registered codec tensors reach the host; the conv
+// weights are read again after it, so the registered tensors must stay valid until the work enqueued here has run.
+int fill_pack(dd_engine* h, cudaStream_t st) {
+  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
+  PackStage* sg = h->stage;
+  float* sg_f = reinterpret_cast<float*>(sg);
+  auto W = [&](const std::string& k) -> const float* {
+    const Raw* r = find(h, k);
+    return r ? r->ptr : nullptr;
+  };
+  int rc;
+  CUDA_TRY(cudaStreamWaitEvent(st, h->pack_done, 0));
+  CUDA_TRY(cudaMemsetAsync(h->amax, 0, 16 * 4, st));
+  const float* w[6] = {};
+  bool fold = false;
+  for (int i = 0; i < 6; ++i) {
+    if (!swin && (i == 2 || i == 3)) continue;
+    const int co = kConvCout[i], ci = kConvCin[i];
+    const int n = co * ci * 9;
+    w[i] = W(std::string(kConvKey[i]) + ".weight");
+    const float* b = W(std::string(kConvKey[i]) + ".bias");
+    if (b) CUDA_TRY(cudaMemcpyAsync(h->L[i].bias, b, co * 4, cudaMemcpyDeviceToDevice, st));
+    if (w[i]) {
+      dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(w[i], n, h->amax + i);
+      if ((rc = check_launch("absmax"))) return rc;
+      if (has_backward(h->cfg)) {
+        dd::flip_transpose_weight_kernel<<<64, 256, 0, st>>>(w[i], h->w_flip[i], co, ci);
+        if ((rc = check_launch("flip_transpose_weight"))) return rc;
+        dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(h->w_flip[i], n, h->amax + 6 + i);
+        if ((rc = check_launch("absmax"))) return rc;
+      }
+    }
+    if (fold_active(h) && (i == 3 || i == 4)) {
+      if (w[i]) CUDA_TRY(cudaMemcpyAsync(h->fold.src[i - 3], w[i], static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice, st));
+      fold |= w[i] || b;
+    }
+  }
+  if (fold) {  // K5 / b5 in fp64, then one fp16 hi / lo split with a power-of-two scale as for the 3x3 layers
+    dd::compose_fold_kernel<<<256, 256, 0, st>>>(h->fold.src[1], h->L[4].bias, h->fold.src[0], h->L[3].bias, h->fold.k5,
+                                                 h->fold.k5_abs, h->fold.bias);
+    if ((rc = check_launch("compose_fold"))) return rc;
+    dd::absmax_kernel<<<absmax_grid(64 * 256 * 25), 256, 0, st>>>(h->fold.k5_abs, 64 * 256 * 25, h->amax + 12);
+    if ((rc = check_launch("absmax"))) return rc;
+  }
+  for (int i = 0; i < 4; ++i) {
+    if (const float* g = W(std::string(kGnKey[i]) + ".weight"))
+      CUDA_TRY(cudaMemcpyAsync(h->gn_gamma[i], g, kGnCh[i] * 4, cudaMemcpyDeviceToDevice, st));
+    if (const float* b = W(std::string(kGnKey[i]) + ".bias"))
+      CUDA_TRY(cudaMemcpyAsync(h->gn_beta[i], b, kGnCh[i] * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  if (const float* t = W("model.time_embedding.weight"))
+    CUDA_TRY(cudaMemcpyAsync(h->temb, t, DD_TIME_ROWS * 256 * 4, cudaMemcpyDeviceToDevice, st));
+  bool dec = false, enc = false;
+  for (const CodecKey& k : kDecKeys)
+    if (const float* p = W(kDecPrefix + k.leaf)) {
+      CUDA_TRY(cudaMemcpyAsync(sg_f + k.host_off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
+      dec = true;
+    }
+  if (h->enc_w1)
+    for (const CodecKey& k : kEncKeys)
+      if (const float* p = W(kEncPrefix + k.leaf)) {
+        CUDA_TRY(cudaMemcpyAsync(sg_f + k.host_off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
+        enc = true;
+      }
+  CUDA_TRY(cudaMemcpyAsync(sg->amax, h->amax, 16 * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+
+  // A graph stays valid across a re-pack (the buffers keep their addresses) unless a kernel argument it holds by value
+  // changed: a conv's or the fold's scale in both loop graphs, the decoder's final bias in the step-decode one.
+  bool loop_stale = false, steps_stale = false;
+  for (int i = 0; i < 6; ++i) {
+    if (!w[i]) continue;
+    const int co = kConvCout[i], ci = kConvCin[i];
+    ConvLayer& L = h->L[i];
+    const float s = dd::grad_scale_of(sg->amax[i]);
+    loop_stale |= s != L.wscale && loop_reads_wscale(h, i);
+    L.wscale = s;
+    dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w[i], L.w_hi, L.w_lo, L.w_simt, co, ci, L.wscale);
+    if ((rc = check_launch("pack_conv_weight"))) return rc;
+    if (has_backward(h->cfg)) {
+      ConvLayer& D = h->L[6 + i];
+      D.wscale = dd::grad_scale_of(sg->amax[6 + i]);
+      dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(h->w_flip[i], D.w_hi, D.w_lo, D.w_simt, ci, co, D.wscale);
+      if ((rc = check_launch("pack_conv_weight"))) return rc;
+    }
+  }
+  if (fold) {
+    const float s = dd::grad_scale_of(sg->amax[12]);
+    loop_stale |= s != h->fold.wscale;
+    h->fold.wscale = s;
+    dd::pack_fold_kernel<<<256, 256, 0, st>>>(h->fold.k5, h->fold.w, static_cast<double>(h->fold.wscale));
+    if ((rc = check_launch("pack_fold"))) return rc;
+  }
+  if (dec) {  // fold eval-BN into the transposed conv (tiny: on the host in fp64)
+    for (int co = 0; co < 16; ++co) {
+      const double sc = static_cast<double>(sg->dec_g[co]) / sqrt(static_cast<double>(sg->dec_var[co]) + 1e-5);
+      sg->bt_f[co] = static_cast<float>((static_cast<double>(sg->dec_bt[co]) - sg->dec_mu[co]) * sc + sg->dec_be[co]);
+      for (int ci = 0; ci < 16; ++ci)
+        for (int ky = 0; ky < 4; ++ky)
+          for (int kx = 0; kx < 4; ++kx)  // ConvTranspose2d weight layout: [Cin][Cout][kh][kw]
+            sg->wt_f[((ky * 4 + kx) * 16 + ci) * 16 + co] =
+                static_cast<float>(static_cast<double>(sg->dec_wt[((ci * 16 + co) * 4 + ky) * 4 + kx]) * sc);
+    }
+    for (int ci = 0; ci < 16; ++ci)
+      for (int tap = 0; tap < 9; ++tap) sg->wc_f[tap * 16 + ci] = sg->dec_wc[ci * 9 + tap];
+    CUDA_TRY(cudaMemcpyAsync(h->dec_wt, sg->wt_f, sizeof(sg->wt_f), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->dec_bt, sg->bt_f, sizeof(sg->bt_f), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->dec_wc, sg->wc_f, sizeof(sg->wc_f), cudaMemcpyHostToDevice, st));
+    steps_stale |= sg->dec_bc[0] != h->dec_bc;
+    h->dec_bc = sg->dec_bc[0];
+    if (h->cfg.flags & DD_FLAG_LOOP_BACKWARD) {
+      for (int co = 0; co < 16; ++co) {
+        const double rstd = 1.0 / sqrt(static_cast<double>(sg->dec_var[co]) + 1e-5);
+        sg->bn[co] = static_cast<float>(static_cast<double>(sg->dec_g[co]) * rstd);
+        sg->bn[16 + co] = sg->dec_mu[co];
+        sg->bn[32 + co] = static_cast<float>(rstd);
+        for (int ci = 0; ci < 16; ++ci)
+          for (int k = 0; k < 16; ++k) sg->wu[(k * 16 + ci) * 16 + co] = sg->dec_wt[(ci * 16 + co) * 16 + k];
+      }
+      CUDA_TRY(cudaMemcpyAsync(h->dec_wu, sg->wu, sizeof(sg->wu), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(h->dec_bu, sg->dec_bt, sizeof(sg->dec_bt), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(h->dec_bn, sg->bn, sizeof(sg->bn), cudaMemcpyHostToDevice, st));
+    }
+  }
+  if (enc) {
+    float s1[16], s2[16];
+    const float* bn1[4] = {sg->enc_bn1[0], sg->enc_bn1[1], sg->enc_bn1[2], sg->enc_bn1[3]};
+    const float* bn2[4] = {sg->enc_bn2[0], sg->enc_bn2[1], sg->enc_bn2[2], sg->enc_bn2[3]};
+    bn_fold_host(bn1, 16, s1, sg->t1);
+    bn_fold_host(bn2, 16, s2, sg->t2);
+    for (int co = 0; co < 16; ++co)
+      for (int tap = 0; tap < 9; ++tap)
+        sg->f1[tap * 16 + co] = static_cast<float>(static_cast<double>(sg->enc_w1[co * 9 + tap]) * s1[co]);
+    for (int co = 0; co < 16; ++co)
+      for (int ci = 0; ci < 16; ++ci)
+        for (int tap = 0; tap < 9; ++tap)
+          sg->f2[(tap * 16 + ci) * 16 + co] =
+              static_cast<float>(static_cast<double>(sg->enc_w2[(co * 16 + ci) * 9 + tap]) * s2[co]);
+    CUDA_TRY(cudaMemcpyAsync(h->enc_w1, sg->f1, sizeof(sg->f1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->enc_b1, sg->t1, sizeof(sg->t1), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->enc_w2, sg->f2, sizeof(sg->f2), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->enc_b2, sg->t2, sizeof(sg->t2), cudaMemcpyHostToDevice, st));
+  }
+  CUDA_TRY(cudaEventRecord(h->pack_done, st));
+  if (loop_stale) drop_graph(h, dd_engine::G_LOOP);
+  if (loop_stale || steps_stale) drop_graph(h, dd_engine::G_LOOP_STEPS);
+  return DD_OK;
 }
 
 // Pack one layer of the convgen_wgmma_kernel path, a producer conv or a Linear, from its raw weight w ([cout][cin]
@@ -2066,10 +2345,14 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
   if (const char* v = getenv("DD_UP_QPB")) e->up_qpb = atoi(v);
 #endif
   if (cudaMallocHost(&e->status_host, 64) != cudaSuccess ||
+      cudaMallocHost(&e->stage, sizeof(PackStage)) != cudaSuccess ||
+      cudaEventCreateWithFlags(&e->pack_done, cudaEventDisableTiming) != cudaSuccess ||
       cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking) != cudaSuccess ||
       configure_all_kernels() != cudaSuccess) {
     std::string msg = std::string("engine setup failed: ") + cudaGetErrorString(cudaGetLastError());
     if (e->status_host) cudaFreeHost(e->status_host);
+    if (e->stage) cudaFreeHost(e->stage);
+    if (e->pack_done) cudaEventDestroy(e->pack_done);
     if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
     delete e;
     return fail(DD_ERR_CUDA, msg);
@@ -2084,6 +2367,8 @@ int dd_destroy(dd_handle h) {
   drop_graphs(h);
   for (void* p : h->owned) cudaFree(p);
   if (h->status_host) cudaFreeHost(h->status_host);
+  if (h->stage) cudaFreeHost(h->stage);
+  if (h->pack_done) cudaEventDestroy(h->pack_done);
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
   delete h;
   return DD_OK;
@@ -2137,144 +2422,23 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
       (swin && (!expect("model.upsample_fuse.convA.conv.weight", {256, 256, 3, 3}) ||
                 !expect("model.upsample_fuse.convB.conv.weight", {256, 256, 3, 3}))))
     return fail(DD_ERR_INVALID, "weight shape mismatch with the reference architecture");
-  // drop any previous pack
-  drop_graphs(h);
-  for (void* p : h->owned) cudaFree(p);
-  h->owned.clear();
-  float* scratch = nullptr;
-  int rc;
-  if ((rc = dev_alloc(h, reinterpret_cast<void**>(&scratch), 64))) return rc;
-  auto W = [&](const char* k) { return find(h, k)->ptr; };
-  if ((rc = pack_layer(h, h->L[0], W("model.noise_embedding.0.weight"), W("model.noise_embedding.0.bias"), 64, 16, st, scratch))) return rc;
-  if ((rc = pack_layer(h, h->L[1], W("model.noise_embedding.3.weight"), W("model.noise_embedding.3.bias"), 256, 64, st, scratch))) return rc;
-  if (swin) {
-    if ((rc = pack_layer(h, h->L[2], W("model.upsample_fuse.convA.conv.weight"), W("model.upsample_fuse.convA.conv.bias"), 256, 256, st, scratch))) return rc;
-    if ((rc = pack_layer(h, h->L[3], W("model.upsample_fuse.convB.conv.weight"), W("model.upsample_fuse.convB.conv.bias"), 256, 256, st, scratch))) return rc;
-  }
-  if ((rc = pack_layer(h, h->L[4], W("model.pred.0.weight"), W("model.pred.0.bias"), 64, 256, st, scratch))) return rc;
-  if (fold_active(h)) {
-    // K5 / b5 in fp64, then one fp16 hi / lo split with a power-of-two scale as in pack_layer
-    const size_t n5 = 64 * 256 * 25;
-    double* k5 = nullptr;
-    float* k5_abs = nullptr;
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&k5), n5 * 8));
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&k5_abs), n5 * 4));
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->fold.w), dd::F5::W_ELEMS * 2))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->fold.bias), 64 * 4))) return rc;
-    dd::compose_fold_kernel<<<256, 256, 0, st>>>(W("model.pred.0.weight"), W("model.pred.0.bias"),
-                                                 W("model.upsample_fuse.convB.conv.weight"),
-                                                 W("model.upsample_fuse.convB.conv.bias"), k5, k5_abs, h->fold.bias);
-    if ((rc = check_launch("compose_fold"))) return rc;
-    if ((rc = split_scale_of(k5_abs, n5, scratch, st, &h->fold.wscale))) return rc;
-    dd::pack_fold_kernel<<<256, 256, 0, st>>>(k5, h->fold.w, static_cast<double>(h->fold.wscale));
-    if ((rc = check_launch("pack_fold"))) return rc;
-    CUDA_TRY(cudaStreamSynchronize(st));
-    cudaFree(k5);
-    cudaFree(k5_abs);
-  }
-  if ((rc = pack_layer(h, h->L[5], W("model.pred.3.weight"), W("model.pred.3.bias"), 16, 64, st, scratch))) return rc;
-  if (has_backward(h->cfg)) {
-    // data-gradient convs: W'[ci][co][ky][kx] = W[co][ci][2-ky][2-kx] with zero bias, packed like any forward layer
-    float* zeros = nullptr;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&zeros), 256 * 4))) return rc;
-    CUDA_TRY(cudaMemsetAsync(zeros, 0, 256 * 4, st));
-    for (int i = 0; i < 6; ++i) {
-      if (!swin && (i == 2 || i == 3)) continue;
-      const int co = kConvCout[i], ci = kConvCin[i];
-      float* wt = nullptr;
-      if ((rc = dev_alloc(h, reinterpret_cast<void**>(&wt), static_cast<size_t>(co) * ci * 9 * 4))) return rc;
-      dd::flip_transpose_weight_kernel<<<64, 256, 0, st>>>(W((std::string(kConvKey[i]) + ".weight").c_str()), wt, co, ci);
-      if ((rc = check_launch("flip_transpose_weight"))) return rc;
-      if ((rc = pack_layer(h, h->L[6 + i], wt, zeros, ci, co, st, scratch))) return rc;
-    }
-  }
-  const char* gnk[4] = {"model.noise_embedding.1", "model.noise_embedding.4", "model.pred.1", "model.pred.4"};
-  const int gnc[4] = {64, 256, 64, 16};
-  for (int i = 0; i < 4; ++i) {
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->gn_gamma[i]), gnc[i] * 4))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->gn_beta[i]), gnc[i] * 4))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(h->gn_gamma[i], W((std::string(gnk[i]) + ".weight").c_str()), gnc[i] * 4, cudaMemcpyDeviceToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->gn_beta[i], W((std::string(gnk[i]) + ".bias").c_str()), gnc[i] * 4, cudaMemcpyDeviceToDevice, st));
-  }
-  if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->temb), DD_TIME_ROWS * 256 * 4))) return rc;
-  CUDA_TRY(cudaMemcpyAsync(h->temb, W("model.time_embedding.weight"), DD_TIME_ROWS * 256 * 4, cudaMemcpyDeviceToDevice, st));
-  // decoder: fold eval-BN into the transposed conv (tiny: do it on the host in fp64)
-  std::vector<float> wt(16 * 16 * 16), bt(16), g(16), be(16), mu(16), var(16), wc(16 * 9), bc(1);
-  CUDA_TRY(cudaMemcpyAsync(wt.data(), W("depth_transform.conv_inv_transform.0.weight"), wt.size() * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(bt.data(), W("depth_transform.conv_inv_transform.0.bias"), 64, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(g.data(), W("depth_transform.conv_inv_transform.1.weight"), 64, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(be.data(), W("depth_transform.conv_inv_transform.1.bias"), 64, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(mu.data(), W("depth_transform.conv_inv_transform.1.running_mean"), 64, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(var.data(), W("depth_transform.conv_inv_transform.1.running_var"), 64, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(wc.data(), W("depth_transform.conv_inv_transform.3.0.weight"), wc.size() * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(bc.data(), W("depth_transform.conv_inv_transform.3.0.bias"), 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  std::vector<float> wt_f(4 * 4 * 16 * 16), bt_f(16), wc_f(9 * 16);
-  for (int co = 0; co < 16; ++co) {
-    const double sc = static_cast<double>(g[co]) / sqrt(static_cast<double>(var[co]) + 1e-5);
-    bt_f[co] = static_cast<float>((static_cast<double>(bt[co]) - mu[co]) * sc + be[co]);
-    for (int ci = 0; ci < 16; ++ci)
-      for (int ky = 0; ky < 4; ++ky)
-        for (int kx = 0; kx < 4; ++kx)  // ConvTranspose2d weight layout: [Cin][Cout][kh][kw]
-          wt_f[((ky * 4 + kx) * 16 + ci) * 16 + co] =
-              static_cast<float>(static_cast<double>(wt[((ci * 16 + co) * 4 + ky) * 4 + kx]) * sc);
-  }
-  for (int ci = 0; ci < 16; ++ci)
-    for (int tap = 0; tap < 9; ++tap) wc_f[tap * 16 + ci] = wc[ci * 9 + tap];
-  if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_wt), wt_f.size() * 4))) return rc;
-  if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_bt), 64))) return rc;
-  if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_wc), wc_f.size() * 4))) return rc;
-  CUDA_TRY(cudaMemcpyAsync(h->dec_wt, wt_f.data(), wt_f.size() * 4, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(h->dec_bt, bt_f.data(), 64, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(h->dec_wc, wc_f.data(), wc_f.size() * 4, cudaMemcpyHostToDevice, st));
-  h->dec_bc = bc[0];
-  if (h->cfg.flags & DD_FLAG_LOOP_BACKWARD) {  // the decoder backward needs the BatchNorm unfolded
-    std::vector<float> wu(4 * 4 * 16 * 16), bn(3 * 16);
-    for (int co = 0; co < 16; ++co) {
-      const double rstd = 1.0 / sqrt(static_cast<double>(var[co]) + 1e-5);
-      bn[co] = static_cast<float>(static_cast<double>(g[co]) * rstd);
-      bn[16 + co] = mu[co];
-      bn[32 + co] = static_cast<float>(rstd);
-      for (int ci = 0; ci < 16; ++ci)
-        for (int k = 0; k < 16; ++k) wu[(k * 16 + ci) * 16 + co] = wt[(ci * 16 + co) * 16 + k];
-    }
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_wu), wu.size() * 4))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_bu), 64))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->dec_bn), bn.size() * 4))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(h->dec_wu, wu.data(), wu.size() * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->dec_bu, bt.data(), 64, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->dec_bn, bn.data(), bn.size() * 4, cudaMemcpyHostToDevice, st));
-  }
-  CUDA_TRY(cudaStreamSynchronize(st));
-  h->enc_w1 = nullptr;
-  if (find(h, "depth_transform.conv_transform.0.0.weight")) {
-    const std::string P = "depth_transform.conv_transform.";
-    const Raw *w1 = find(h, P + "0.0.weight"), *w2 = find(h, P + "1.0.weight");
+  const bool encoder = find(h, kEncPrefix + "0.0.weight") != nullptr;
+  if (encoder) {
+    const Raw *w1 = find(h, kEncPrefix + "0.0.weight"), *w2 = find(h, kEncPrefix + "1.0.weight");
     if (!w2 || w1->shape != std::vector<int64_t>{16, 1, 3, 3} || w2->shape != std::vector<int64_t>{16, 16, 3, 3})
       return fail(DD_ERR_INVALID, "encoder weights missing / wrong shape");
-    std::vector<float> s1, t1, s2, t2, hw1(144), hw2(2304);
-    if ((rc = bn_fold(h, P + "0.1", 16, s1, t1, st))) return rc;
-    if ((rc = bn_fold(h, P + "1.1", 16, s2, t2, st))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(hw1.data(), w1->ptr, 144 * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(hw2.data(), w2->ptr, 2304 * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    std::vector<float> f1(144), f2(2304);
-    for (int co = 0; co < 16; ++co)
-      for (int tap = 0; tap < 9; ++tap) f1[tap * 16 + co] = static_cast<float>(static_cast<double>(hw1[co * 9 + tap]) * s1[co]);
-    for (int co = 0; co < 16; ++co)
-      for (int ci = 0; ci < 16; ++ci)
-        for (int tap = 0; tap < 9; ++tap)
-          f2[(tap * 16 + ci) * 16 + co] = static_cast<float>(static_cast<double>(hw2[(co * 16 + ci) * 9 + tap]) * s2[co]);
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->enc_w1), 144 * 4))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->enc_b1), 64))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->enc_w2), 2304 * 4))) return rc;
-    if ((rc = dev_alloc(h, reinterpret_cast<void**>(&h->enc_b2), 64))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(h->enc_w1, f1.data(), 144 * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_b1, t1.data(), 64, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_w2, f2.data(), 2304 * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_b2, t2.data(), 64, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    for (const CodecKey& k : kEncKeys)
+      if (!find(h, kEncPrefix + k.leaf)) return fail(DD_ERR_INVALID, "missing weights: " + kEncPrefix + k.leaf);
   }
+  // drop any previous pack
+  drop_graphs(h);
+  h->packed = false;
+  for (void* p : h->owned) cudaFree(p);
+  h->owned.clear();
+  int rc;
+  if ((rc = alloc_pack(h, encoder, st))) return rc;
+  if ((rc = fill_pack(h, st))) return rc;
+  float* scratch = h->amax;
   h->prod.ready = false;
   if (h->prod.enabled)
     if ((rc = pack_producers(h, st, scratch))) return rc;
@@ -2287,12 +2451,30 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   h->mp.ready = false;
   if (h->mp.enabled)
     if ((rc = pack_mpvit(h, st, scratch))) return rc;
-  // the registered pointers were borrowed for this call only (include/dd_engine.h): forget them, so a later finalize
-  // cannot read memory the caller has freed in the meantime — every key has to be registered again
+  // the registered pointers were borrowed for this call only (include/dd_engine.h): wait for the kernels that read them
+  // and forget them, so a later finalize cannot read memory the caller has freed in the meantime
+  CUDA_TRY(cudaStreamSynchronize(st));
   h->raw.clear();
-  h->weights_ready = true;
+  h->weights_ready = h->packed = true;
   return DD_OK;
 }
+
+int dd_update_weights(dd_handle h, void* cuda_stream) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  int rc = DD_OK;
+  if (!h->packed) {
+    rc = fail(DD_ERR_INVALID, "dd_update_weights needs a completed dd_finalize_weights");
+  } else if (!h->raw.empty() && (rc = check_update(h)) == DD_OK) {
+    if (cudaSetDevice(h->cfg.device) != cudaSuccess) rc = fail(DD_ERR_CUDA, "cudaSetDevice failed");
+    else rc = fill_pack(h, static_cast<cudaStream_t>(cuda_stream));
+    if (rc != DD_OK) h->packed = false;  // the pack is partly written: only dd_finalize_weights restores it
+  }
+  h->raw.clear();
+  h->weights_ready = h->packed;
+  return rc;
+}
+
+int64_t dd_graph_capture_count(dd_handle h) { return h ? h->graph_captures : 0; }
 
 int dd_set_schedule(dd_handle h, const int64_t* timesteps, const double* c_x, const double* c_eps, int32_t n) {
   if (!h || !timesteps || !c_x || !c_eps) return fail(DD_ERR_INVALID, "null argument");
@@ -2650,6 +2832,7 @@ int dd_enable_producers(dd_handle h, const dd_producer_config* pc) {
     return fail(DD_ERR_INVALID, "level-0 feature size must equal the condition map size");
   h->prod = p;
   h->weights_ready = false;  // producer weights are packed by dd_finalize_weights
+  h->packed = false;
   h->ws = nullptr;           // workspace layout changed
   drop_graphs(h);
   return DD_OK;
@@ -2751,6 +2934,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
     h->bb.enabled = false;
     h->mp.enabled = false;
     h->weights_ready = false;
+    h->packed = false;
     h->ws = nullptr;
     drop_graphs(h);
     return DD_OK;
@@ -2788,6 +2972,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
     h->bb.enabled = false;
     h->rn.enabled = false;
     h->weights_ready = false;
+    h->packed = false;
     h->ws = nullptr;
     drop_graphs(h);
     return DD_OK;
@@ -2819,6 +3004,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
   h->rn.enabled = false;
   h->mp.enabled = false;
   h->weights_ready = false;
+  h->packed = false;
   h->ws = nullptr;
   drop_graphs(h);
   return DD_OK;

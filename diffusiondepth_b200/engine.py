@@ -48,6 +48,13 @@ DECODER_PARAM_KEYS = tuple(k for k in DECODER_KEYS if "running" not in k)
 _DECODER_SHAPES = {"depth_transform.conv_inv_transform.0.weight": (16, 16, 4, 4),
                    "depth_transform.conv_inv_transform.3.0.weight": (1, 16, 3, 3),
                    "depth_transform.conv_inv_transform.3.0.bias": (1,)}
+# keys `DenoiseEngine.update_weights` re-packs in place (the denoiser and the depth codec); the neck, FPN and backbone
+# packs are rebuilt by `load_weights` only
+UPDATABLE_PREFIXES = ("model.", "depth_transform.conv_inv_transform.", "depth_transform.conv_transform.")
+
+
+def is_updatable(key: str) -> bool:
+    return key.startswith(UPDATABLE_PREFIXES)
 
 
 def ddim_coefficients(alphas_cumprod: torch.Tensor, num_inference_steps: int, num_train_timesteps: int,
@@ -147,6 +154,29 @@ class DenoiseEngine:
             _cabi.check(self.lib.dd_set_weight(self._h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
         _cabi.check(self.lib.dd_finalize_weights(self._h, C.c_void_p(self._stream())))
         self._keep = []
+
+    def update_weights(self, tensors: Dict[str, torch.Tensor]):
+        """After `load_weights`: re-pack, in place, what depends on `tensors` — only the parameters / buffers that
+        changed, all of them `is_updatable`.  Buffers, TMA descriptors and CUDA graphs are kept (a loop graph is
+        captured again only when a conv's power-of-two weight scale changed); the result is bit-identical to a
+        `load_weights` of the whole model.  On EngineError the previous pack is intact."""
+        known = DENOISER_KEYS + FUSE_KEYS + DECODER_KEYS + ENCODER_KEYS
+        for k, v in tensors.items():  # what dd_set_weight would reject, before anything is registered
+            if not (k in known or k.startswith(("hahineck.", "conv_lateral.", "conv_up.", "backbone."))) or v.dim() > 4:
+                raise EngineError(f"unknown weight key: {k}")
+        self._keep = []
+        for k, v in tensors.items():
+            t = v.detach().to(self.device, torch.float32).contiguous()
+            self._keep.append(t)
+            shape = (C.c_int64 * t.dim())(*t.shape)
+            _cabi.check(self.lib.dd_set_weight(self._h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+        status = self.lib.dd_update_weights(self._h, C.c_void_p(self._stream()))
+        self._keep = []  # still read on the stream: the caching allocator reuses the memory in stream order
+        _cabi.check(status)
+
+    def graph_capture_count(self) -> int:
+        """CUDA graph instantiations of this engine so far."""
+        return int(self.lib.dd_graph_capture_count(self._h))
 
     def enable_producers(self, channels, sizes, has_neck: bool):
         """Run the HAHI neck (if any) + FPN natively too; call before load_weights.  `sizes`: [(h, w)] per level."""

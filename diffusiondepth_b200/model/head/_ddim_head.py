@@ -23,7 +23,7 @@ import torch.nn.functional as F
 
 from diffusiondepth_b200._cabi import EngineError
 from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS, FUSE_KEYS,
-                                        DenoiseEngine, WorkspacePool)
+                                        DenoiseEngine, WorkspacePool, is_updatable)
 from .._blocks import ConvModule, exact_fp32
 from ..diffusers.schedulers.scheduling_ddim import DDIMScheduler
 from ..ops import depth_transform as _codec  # noqa: F401  (registers the codec classes)
@@ -54,6 +54,21 @@ def collect_tensors(module: nn.Module, prefix: str = "") -> Dict[str, torch.Tens
 
     walk(module, prefix)
     return out
+
+
+def _signature(tensors):
+    return tuple((t.data_ptr(), t._version) for t in tensors.values())
+
+
+def repack_plan(old_keys, old_sig, new_keys, new_sig, incremental=True):
+    """What an engine packed from tensors `old_keys` with signature `old_sig` (None: never packed) needs to serve the
+    tensors `new_keys` / `new_sig`: the list of changed keys for `DenoiseEngine.update_weights` (empty: nothing), or
+    None for a full `load_weights` — a different key set, a changed tensor the update does not re-pack (neck, FPN,
+    backbone), or `incremental` off."""
+    if not incremental or old_sig is None or tuple(old_keys) != tuple(new_keys):
+        return None
+    changed = [k for k, a, b in zip(new_keys, old_sig, new_sig) if a != b]
+    return changed if all(is_updatable(k) for k in changed) else None
 
 
 def _gn_conv_stack(cin, mid, cout):
@@ -190,6 +205,8 @@ class DDIMHeadBase(nn.Module):
         self.check_range = True
         self.capture_logits = False      # tests: also keep the decoder's pre-sigmoid z of the last forward
         self.native_producers = True     # neck + FPN on the engine's tensor-core conv path when the pyramid allows
+        self.incremental_repack = True   # after an optimizer step re-pack only the changed denoiser / codec tensors, in
+        #                                  place (DenoiseEngine.update_weights; bit-identical); False: always the full pack
         self.native_backbone = True      # Swin-L backbone on the engine's GEMM/attention path (needs native_producers)
         self.fp8_corrections = True      # Swin heads: correction products of convA / convB as e4m3 MMAs (DD_FLAG_FP8_CORR;
         #                                  ~1.5x on the dominant kernel, max |dz| 3.4e-4 of the 1e-3 budget on config 3).
@@ -208,7 +225,8 @@ class DDIMHeadBase(nn.Module):
 
     def invalidate_engines(self):
         """Close every engine (call after replacing Parameter OBJECTS; in-place updates, load_state_dict and .to() are
-        picked up automatically through data_ptr / _version)."""
+        picked up automatically through data_ptr / _version: a change confined to denoiser / codec tensors is re-packed
+        in place by `DenoiseEngine.update_weights`, anything else by a full `load_weights`)."""
         for e in self._engines.values():
             e.close()
         self._reset_engine_state()
@@ -416,13 +434,18 @@ class DDIMHeadBase(nn.Module):
             sig = None
         else:
             tensors = packed[0]
-            sig = tuple((t.data_ptr(), t._version) for t in tensors.values())
+            sig = _signature(tensors)
         if packed is None or sig != packed[1]:
+            changed = None
             if packed is not None:  # something changed: the owning modules may hold new tensors
                 tensors = self._gather(native, image_hw, backbone)
-            eng.load_weights(tensors)
-            self._packed[key] = (tensors, tuple((t.data_ptr(), t._version) for t in tensors.values()),
-                                 backbone if image_hw is not None else None)
+                changed = repack_plan(packed[0].keys(), packed[1], tensors.keys(), _signature(tensors),
+                                      self.incremental_repack)
+            if changed is None:
+                eng.load_weights(tensors)
+            elif changed:
+                eng.update_weights({k: tensors[k] for k in changed})
+            self._packed[key] = (tensors, _signature(tensors), backbone if image_hw is not None else None)
         return eng
 
     def _any_engine(self, batch, latent_hw, cond_hw, device):
@@ -432,7 +455,7 @@ class DDIMHeadBase(nn.Module):
         for key in reversed(self._engines):
             if key[:4] == want and key[4] == self.diffusion_inference_steps and self._packed.get(key) is not None:
                 tensors, sig, _ = self._packed[key]
-                if tuple((t.data_ptr(), t._version) for t in tensors.values()) == sig:
+                if _signature(tensors) == sig:
                     self._engines.move_to_end(key)
                     return self._engines[key]
                 break

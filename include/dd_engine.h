@@ -8,7 +8,7 @@
  *                                    `DeepDepthTransformWithUpsampling` inside the head ctor
  *                                    (src/model/head/ddim_depth_estimate_res_swin_addHAHI.py:45-49,
  *                                     src/model/head/ddim_depth_estimate_res.py:36-40)
- *   dd_set_weight / dd_finalize_weights
+ *   dd_set_weight / dd_finalize_weights / dd_update_weights
  *                                 <- `load_state_dict(ckpt['net'])` for the keys under
  *                                    `depth_head.model.*` and `depth_head.depth_transform.*`
  *                                    (src/main.py:418-432; key layout SURVEY.md Appendix A)
@@ -119,14 +119,41 @@ int dd_destroy(dd_handle h);
 
 /* Register one parameter/buffer by its reference state_dict key relative to `depth_head.`
  * (e.g. "model.noise_embedding.0.weight", "depth_transform.conv_inv_transform.1.running_var").
- * `dev_ptr` is a device fp32 pointer in the reference's own layout/shape; it is read during the next
- * dd_finalize_weights only, which then forgets every registered pointer (a re-pack registers all keys again).
- * Unknown keys are rejected (DD_ERR_INVALID). */
+ * `dev_ptr` is a device fp32 pointer in the reference's own layout/shape; it is read by the next
+ * dd_finalize_weights or dd_update_weights only, which then forgets every registered pointer (a re-pack registers
+ * all keys again, an update the changed ones).  Unknown keys are rejected (DD_ERR_INVALID). */
 int dd_set_weight(dd_handle h, const char* name, const float* dev_ptr, const int64_t* shape, int32_t ndim);
 
 /* Pre-pack: fold eval-BatchNorm into the decoder, repack conv weights tap-major, split them into
  * scaled fp16 hi/lo planes for the 3-pass tensor-core product.  Fails listing any missing key. */
 int dd_finalize_weights(dd_handle h, void* cuda_stream);
+
+/* After an optimizer step: re-pack, in place, what depends on the tensors registered with dd_set_weight since the
+ * last successful dd_finalize_weights / dd_update_weights: ONLY the tensors that changed, under the same keys and
+ * shapes.  Every refreshed buffer ends up with exactly the bytes a dd_finalize_weights from the same tensors would
+ * write, at the address that finalize allocated: nothing is allocated or freed, no TMA descriptor is re-encoded.
+ *   a denoiser conv's `.weight` / `.bias`     that layer's split planes, bias and scale (and, with DD_FLAG_BACKWARD /
+ *                                             DD_FLAG_LOOP_BACKWARD, its data-gradient layer)
+ *   `upsample_fuse.convB.conv.*`, `pred.0.*`  also the composed 5x5 conv, where the engine runs it
+ *   a GroupNorm `.weight` / `.bias`, `model.time_embedding.weight`
+ *                                             the engine's copy
+ *   `depth_transform.conv_inv_transform.*`    the folded decoder (and the unfolded one of DD_FLAG_LOOP_BACKWARD)
+ *   `depth_transform.conv_transform.*`        the folded encoder
+ *   `hahineck.*`, `conv_lateral.*`, `conv_up.*`, `backbone.*`
+ *                                             DD_ERR_UNSUPPORTED: those packs are rebuilt by dd_finalize_weights only
+ * CUDA graphs are kept.  The one exception: the loop graphs hold each conv's power-of-two weight scale (and the
+ * step-decode graph the decoder's final bias) as kernel arguments, so when such a value changes (max |w| of a layer
+ * crosses a power of two) the graphs holding it are captured again on their next use.
+ * The work is enqueued on `cuda_stream` and the call synchronises that stream once; the registered tensors are read on
+ * the stream after the call returns as well, so free them in stream order.  Successive calls that touch the weights
+ * belong on one stream, or on streams the caller orders.
+ * Every key and shape is validated before anything is written: on DD_ERR_INVALID (a key this engine did not pack, a
+ * different shape, no finalize yet) or DD_ERR_UNSUPPORTED the registrations are forgotten and the engine is as it was
+ * before the dd_set_weight calls.  With nothing registered the call does nothing. */
+int dd_update_weights(dd_handle h, void* cuda_stream);
+
+/* CUDA graph instantiations since dd_create: lets a test or a timing script see which calls captured a graph. */
+int64_t dd_graph_capture_count(dd_handle h);
 
 /* Per-step timesteps (descending, as DDIMScheduler.set_timesteps produces) and the collapsed DDIM
  * coefficients; n must equal num_inference_steps. */
