@@ -44,30 +44,38 @@ struct GenConvArgs {
 // requests and barrier round trips per byte of 32-channel chunks.
 constexpr int GEN_BK = 64;
 
+// Columns of one consumer unit of an NT-wide work item: 128 x NT items split into two units of NT / 2 columns when
+// 128 x NT fp32 accumulators would not fit one warpgroup's registers.  Also the row count of the weight maps' boxes.
+constexpr int gen_unit_cols(int nt) { return nt > 128 ? nt / 2 : nt; }
+
 template <int NT>
 struct GenCfg {
   static constexpr int BK = GEN_BK;
   static constexpr int ROW_BYTES = BK * 2;
+  // one unit: all 128 rows of the tile and NW columns (NW registers of accumulators per consumer thread)
+  static constexpr int NW = gen_unit_cols(NT);
+  static constexpr int UNITS = NT / NW;  // units per work item
   static constexpr int A_BYTES = TILE_M * ROW_BYTES;  // 16 KB per plane
-  static constexpr int B_BYTES = NT * ROW_BYTES;
-  static constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);
-  // consumer warpgroups: each owns all 128 rows of the tile and NW = NT / NWG columns (NW registers of accumulators)
-  static constexpr int NWG = NT > 128 ? 2 : 1;
-  static constexpr int NW = NT / NWG;
-  static constexpr int THREADS = 128 * (1 + NWG);
+  static constexpr int B_BYTES = NW * ROW_BYTES;
+  static constexpr int STAGE_BYTES = 2 * (A_BYTES + B_BYTES);  // one unit's K chunk
+  static constexpr int THREADS = 384;  // producer warpgroup + two consumer warpgroups taking units in turn
   static constexpr int LD = 20;  // staging row stride (floats): 16 columns + 4, rows stay 16-byte aligned
-  static constexpr int STAGING_BYTES = NWG * 128 * LD * 4;
+  static constexpr int STAGING_BYTES = 2 * 128 * LD * 4;
   static constexpr int STAGES_RAW = (227 * 1024 - 1024 - 512 - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-  static_assert(STAGES >= 2, "stage too large");
+  static_assert(STAGES >= 3, "stage too large");
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 512 + STAGING_BYTES;
   static_assert(SMEM_BYTES <= 232448, "exceeds the 227 KB dynamic shared memory limit");
   static_assert(NW % 16 == 0 && NT <= 256, "bad N tile");  // instantiated: 64, 128, 192, 256
 };
 
-// Warp roles: warp 0 = TMA producer of the activation planes, warp 1 = of the weight planes; warpgroups 1 .. NWG =
-// consumers (wgmma mainloop, then the epilogue of their columns, drained 16 columns at a time through a shared-memory
-// staging tile that hands each thread one ROW (pixel / token) of the chunk).
+// Warp roles: warp 0 = TMA producer of the activation planes, warp 1 = of the weight planes; warpgroups 1 and 2 =
+// consumers.  The CTA's work items are cut into units (128 rows x NW columns, UNITS per item) and numbered in order;
+// consumer warpgroup w takes the units j with j % 2 == w: wgmma mainloop, then the epilogue of the unit, drained 16
+// columns at a time through a shared-memory staging tile that hands each thread one ROW (pixel / token) of the chunk.
+// The producers fill the stage ring unit after unit, and a pair of named barriers hands the tensor cores from unit j's
+// mainloop to unit j + 1's: one warpgroup's epilogue runs under the other's MMAs, and every consumer finds the ring
+// position of its unit (j * k_iters) filled in order.
 template <int NT>
 __global__ void __launch_bounds__((GenCfg<NT>::THREADS), 1)
 convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_constant__ CUtensorMap tmA0_lo,
@@ -95,7 +103,7 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
     tma_prefetch_desc(&tmB_lo);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full_bar[s], 2);        // two producers (activation planes / weight planes) arrive per stage
-      mbar_init(&empty_bar[s], C::NWG);  // one arrive per consumer warpgroup
+      mbar_init(&empty_bar[s], 1);       // the one consumer warpgroup of the stage's unit
     }
     fence_barrier_init();
   }
@@ -104,7 +112,7 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
 
   // setmaxnreg at the top of each role's branch, branches meeting only at the exit (see conv3x3_halo_kernel)
   if (warp < 4) {
-    if constexpr (C::NWG > 1) setmaxnreg_dec<40>();
+    setmaxnreg_dec<40>();
     if (warp == 0 || warp == 1) {
       // two TMA producers; the whole warp walks the loop, one elected lane issues (consecutive UTMALDGs)
       const bool act = (warp == 0);
@@ -116,6 +124,8 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
         const int mt = work / p.n_tiles;
         const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
         const int x0 = tx * TILE_W, y0 = ty * TILE_H;
+        // the item's units one after the other; each loads its own copy of the A tile (an L2 hit after the first)
+        for (int u = 0; u < C::UNITS; ++u) {
         for (int tap = 0; tap < p.taps; ++tap) {
           const int dy = p.taps == 9 ? tap / 3 - 1 : 0, dx = p.taps == 9 ? tap % 3 - 1 : 0;
           for (int kc = 0; kc < kc_total; ++kc) {
@@ -127,8 +137,8 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
             if (leader) {
               if (!act) {
                 mbar_arrive_expect_tx(&full_bar[stage], 2 * C::B_BYTES);
-                tma_load_3d(s + 2 * C::A_BYTES, &tmB_hi, &full_bar[stage], kw, nt * NT, tap);
-                tma_load_3d(s + 2 * C::A_BYTES + C::B_BYTES, &tmB_lo, &full_bar[stage], kw, nt * NT, tap);
+                tma_load_3d(s + 2 * C::A_BYTES, &tmB_hi, &full_bar[stage], kw, nt * NT + u * C::NW, tap);
+                tma_load_3d(s + 2 * C::A_BYTES + C::B_BYTES, &tmB_lo, &full_bar[stage], kw, nt * NT + u * C::NW, tap);
               } else if (kc < p.kc0) {
                 mbar_arrive_expect_tx(&full_bar[stage], 2 * C::A_BYTES);
                 tma_load_4d(s, &tmA0_hi, &full_bar[stage], kc * C::BK, ax, ay, img);
@@ -146,10 +156,11 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
             }
           }
         }
+        }
       }
     }
   } else {
-    if constexpr (C::NWG > 1) setmaxnreg_inc<232>();
+    setmaxnreg_inc<232>();
     const int wg = (warp >> 2) - 1;
     const int t = threadIdx.x & 127;
     const int q = t >> 5;
@@ -157,20 +168,23 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
     const int r = m >> 4, c = m & 15;
     float* S = stage_f + wg * 128 * C::LD;
     float* T = S + q * 32 * C::LD;  // this warp's 32 rows
-    const uint32_t b_off = static_cast<uint32_t>(wg * NW) * C::ROW_BYTES;
-    int stage = 0;
-    uint32_t phase = 0;
     bool overflow = false;
     const int cq = p.cout >> 2;
     float acc[2][NW / 2];
+    int unit = -1;  // index of the CTA's current unit
     for (int work = blockIdx.x; work < num_work; work += gridDim.x) {
+    for (int u = 0; u < C::UNITS; ++u) {
+      if (((++unit) & 1) != wg) continue;
       // ---------------------------------------------------------------- mainloop
+      if (unit > 0) named_bar_sync(4 + wg, 256);  // the previous unit has issued its MMAs
+      int stage = (unit * k_iters) % C::STAGES;
+      uint32_t phase = ((unit * k_iters) / C::STAGES) & 1;
       int prev = -1;
       for (int it = 0; it < k_iters; ++it) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa_hi = smem_u32(stage_ptr(stage));
         const uint32_t sa_lo = sa_hi + C::A_BYTES;
-        const uint32_t sb_hi = sa_hi + 2 * C::A_BYTES + b_off;
+        const uint32_t sb_hi = sa_hi + 2 * C::A_BYTES;
         const uint32_t sb_lo = sb_hi + C::B_BYTES;
         wgmma_fence();
 #pragma unroll
@@ -196,6 +210,8 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
           phase ^= 1;
         }
       }
+      if (u + 1 < C::UNITS || work + static_cast<int>(gridDim.x) < num_work)
+        named_bar_arrive(4 + (wg ^ 1), 256);  // the next unit (the other warpgroup's) may issue its MMAs
       wgmma_wait<0>();
       wgmma_fence_regs(acc[0]);
       wgmma_fence_regs(acc[1]);
@@ -217,7 +233,7 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
       const bool xpose_path = (p.out_hi == nullptr);
 #pragma unroll
       for (int ci = 0; ci < NW / 16; ++ci) {
-        const int n0 = nt * NT + wg * NW + ci * 16;
+        const int n0 = nt * NT + u * NW + ci * 16;
         if (n0 >= p.cout) break;  // columns past the last real output channel (cout not a multiple of NT): zero weights
         const int nvalid = p.cout - n0;  // >= 8, multiple of 8; < 16 only in the last chunk of such a layer
         named_bar_sync(2 + wg, 128);  // the previous chunk's staging reads are done
@@ -336,6 +352,7 @@ convgen_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0_hi, const __grid_c
           }
         }
       }
+    }
     }
     if (overflow) atomicOr(p.status, 1);
   }

@@ -141,7 +141,7 @@ int make_patch_map(CUtensorMap* m, const __half* base, int B, int H, int W) {
                     CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // conv weights [taps][cout][cin] fp16 read in boxes of {box_k, rows, 1}: the halo kernel's (9 taps, all cout rows, its
-// K chunk) and the convgen kernel's (GEN_BK, one N tile of rows); ld > cin: cin columns from base on of ld-wide rows
+// K chunk) and the convgen kernel's (GEN_BK, one unit's gen_unit_cols rows); ld > cin: cin columns from base on of ld-wide rows
 int make_weight_map(CUtensorMap* m, const __half* base, int cout, int cin, int taps, int box_k, int rows, int ld = 0) {
   const cuuint64_t L = ld > 0 ? ld : cin;
   const cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)cout, (cuuint64_t)taps};
@@ -307,7 +307,7 @@ struct GenLayer {
   float wscale = 1.f;
   CUtensorMap mb_hi, mb_lo;
   bool alt = false;          // cout divisible by 256 and 192: launch_gen picks the width whose last wave wastes least
-  CUtensorMap mb_hi_alt, mb_lo_alt;  // boxes of 192 rows
+  CUtensorMap mb_hi_alt, mb_lo_alt;  // for N tiles of 192 columns
   float* zero_shift = nullptr;       // layers deep enough to be split along K (gen_parts): the partial launches' shift
 };
 
@@ -1456,13 +1456,13 @@ int pack_gen_weights(dd_engine* e, std::vector<void*>& owned, GenLayer& L, const
   dd::pack_gen_weight_kernel<<<256, 256, 0, st>>>(w, d_scale, L.w_hi, L.w_lo, L.cout, cin, L.taps, L.shuffle, L.wscale, cp);
   if ((rc = check_launch("pack_gen_weight"))) return rc;
   CUDA_TRY(cudaStreamSynchronize(st));
-  if ((rc = make_weight_map(&L.mb_hi, L.w_hi, L.cout, cp, L.taps, dd::GEN_BK, L.nt))) return rc;
-  if ((rc = make_weight_map(&L.mb_lo, L.w_lo, L.cout, cp, L.taps, dd::GEN_BK, L.nt))) return rc;
+  if ((rc = make_weight_map(&L.mb_hi, L.w_hi, L.cout, cp, L.taps, dd::GEN_BK, dd::gen_unit_cols(L.nt)))) return rc;
+  if ((rc = make_weight_map(&L.mb_lo, L.w_lo, L.cout, cp, L.taps, dd::GEN_BK, dd::gen_unit_cols(L.nt)))) return rc;
   // cout divisible by 256 and 192: launch_gen may pick the width whose last wave wastes least
   L.alt = (L.nt == 256 && L.cout % 256 == 0 && L.cout % 192 == 0 && !L.shuffle);
   if (L.alt) {
-    if ((rc = make_weight_map(&L.mb_hi_alt, L.w_hi, L.cout, cp, L.taps, dd::GEN_BK, 192))) return rc;
-    if ((rc = make_weight_map(&L.mb_lo_alt, L.w_lo, L.cout, cp, L.taps, dd::GEN_BK, 192))) return rc;
+    if ((rc = make_weight_map(&L.mb_hi_alt, L.w_hi, L.cout, cp, L.taps, dd::GEN_BK, dd::gen_unit_cols(192)))) return rc;
+    if ((rc = make_weight_map(&L.mb_lo_alt, L.w_lo, L.cout, cp, L.taps, dd::GEN_BK, dd::gen_unit_cols(192)))) return rc;
   }
   return DD_OK;
 }
@@ -1662,8 +1662,8 @@ int launch_gen(dd_engine* e, const GenLayer& L, int act, const GenGrid& g, const
       m[2] = m[0];
       m[3] = m[1];
     }
-    if ((rc = make_weight_map(&m[4], L.w_hi + wcol, L.cout, wlen, L.taps, dd::GEN_BK, nt, L.cin))) return rc;
-    if ((rc = make_weight_map(&m[5], L.w_lo + wcol, L.cout, wlen, L.taps, dd::GEN_BK, nt, L.cin))) return rc;
+    if ((rc = make_weight_map(&m[4], L.w_hi + wcol, L.cout, wlen, L.taps, dd::GEN_BK, dd::gen_unit_cols(nt), L.cin))) return rc;
+    if ((rc = make_weight_map(&m[5], L.w_lo + wcol, L.cout, wlen, L.taps, dd::GEN_BK, dd::gen_unit_cols(nt), L.cin))) return rc;
     const bool last = kb == kc_total;
     ap.relu = last ? act : 0;
     ap.shift = last ? L.shift : L.zero_shift;
@@ -3070,8 +3070,8 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   L.nt = (N % 256 == 0) ? 256 : 192;
   L.shift = bias;
   int rc;
-  if ((rc = make_weight_map(&L.mb_hi, L.w_hi, N, K, 1, dd::GEN_BK, L.nt))) return rc;
-  if ((rc = make_weight_map(&L.mb_lo, L.w_lo, N, K, 1, dd::GEN_BK, L.nt))) return rc;
+  if ((rc = make_weight_map(&L.mb_hi, L.w_hi, N, K, 1, dd::GEN_BK, dd::gen_unit_cols(L.nt)))) return rc;
+  if ((rc = make_weight_map(&L.mb_lo, L.w_lo, N, K, 1, dd::GEN_BK, dd::gen_unit_cols(L.nt)))) return rc;
   int* saved = h->status;
   h->status = status;
   if ((rc = time_per_call(st, 3, iters, ms_out, [&]() {

@@ -263,6 +263,10 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// Signals named barrier `id` without waiting on it (the waiting side calls named_bar_sync with the same count).
+__device__ __forceinline__ void named_bar_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // Writes columns [c0, c0 + CH) of a 64 x N wgmma accumulator (rows row0 .. row0 + 63 of the tile) into a row-major
 // fp32 staging tile with row stride LD floats, so that one thread can then read a whole row.
