@@ -826,6 +826,7 @@ struct DecFinishArgs {
   const double* part_wt;
   int nb_act, nb_wc, nb_wt;
   const float* bn;
+  const double* part_db;  // null, or [nb_act][16] sums of du (training-mode BatchNorm: the ConvT bias gradient)
   float* out[6];
 };
 __global__ void dec_bwd_finish_kernel(const DecFinishArgs f) {
@@ -843,8 +844,12 @@ __global__ void dec_bwd_finish_kernel(const DecFinishArgs f) {
   } else if (i < 4096 + 48) {  // ConvT bias = s * sum dv, BN weight = sum dv * vhat, BN bias = sum dv
     const int j = i - 4096, c = j % 16, which = j / 16;
     const int col = which == 1 ? 16 + c : c;
-    for (int b = 0; b < f.nb_act; ++b) s += f.part_act[static_cast<size_t>(b) * DEC_ACT_N + col];
-    if (which == 0) s *= static_cast<double>(f.bn[c]);
+    if (which == 0 && f.part_db) {
+      for (int b = 0; b < f.nb_act; ++b) s += f.part_db[static_cast<size_t>(b) * 16 + c];
+    } else {
+      for (int b = 0; b < f.nb_act; ++b) s += f.part_act[static_cast<size_t>(b) * DEC_ACT_N + col];
+      if (which == 0) s *= static_cast<double>(f.bn[c]);
+    }
     dst = which == 0 ? f.out[1] : (which == 1 ? f.out[2] : f.out[3]);  // constant indices: no local-memory copy of f
     o = c;
   } else if (i < 4096 + 48 + 144) {  // [ci][tap] <- column tap * 16 + ci

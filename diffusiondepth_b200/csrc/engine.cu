@@ -21,6 +21,7 @@
 #include "swin.cuh"
 #include "mpvit.cuh"
 #include "backward.cuh"
+#include "codec_train.cuh"
 
 namespace {
 
@@ -289,6 +290,7 @@ struct PackStage {
   // host -> device
   float wt_f[4 * 4 * 16 * 16], bt_f[16], wc_f[9 * 16], wu[4 * 4 * 16 * 16], bn[3 * 16];
   float f1[144], t1[16], f2[2304], t2[16];
+  float e1u[144], e2u[2304], enc_gb[4][16];  // unfolded encoder for DD_CODEC_TRAIN: [tap][co], [tap][ci][co]; gamma / beta
 };
 
 struct Raw {
@@ -447,10 +449,25 @@ struct dd_engine {
   float* dec_bt = nullptr;  // [16]
   float* dec_wc = nullptr;  // [9][16]
   float dec_bc = 0.f;
-  float* dec_wu = nullptr;  // [4][4][16][16] unfolded ConvT weights, [ky][kx][ci][co] (DD_FLAG_LOOP_BACKWARD only)
+  float* dec_wu = nullptr;  // [4][4][16][16] unfolded ConvT weights, [ky][kx][ci][co]
   float* dec_bu = nullptr;  // [16] unfolded ConvT bias
   float* dec_bn = nullptr;  // [3][16] BatchNorm scale gamma * rstd, running mean, rstd
   float *enc_w1 = nullptr, *enc_b1 = nullptr, *enc_w2 = nullptr, *enc_b2 = nullptr;  // folded encoder (optional)
+  // DD_CODEC_TRAIN (dd_set_codec_mode): the codec's BatchNorms on batch statistics.  The unfolded parameters (filled
+  // with the pack), the batch-folded copies decoder_kernel / encoder_kernel run on, and the statistics' scratch; all
+  // engine-owned, so the workspace size does not depend on the mode.
+  int codec_mode = DD_CODEC_EVAL;
+  struct CodecTrain {
+    float *dec_gb = nullptr;                                  // [2][16] decoder BatchNorm weight, bias
+    float *dec_wt = nullptr, *dec_bt = nullptr, *dec_bn = nullptr;  // batch-folded decoder; [3][16] s, mean, rstd
+    float* zero16 = nullptr;  // [16] zeros: the ConvT bias of the decoder backward's xhat (bn's mean is bias-free)
+    float *enc_w1 = nullptr, *enc_w2 = nullptr, *enc_gb = nullptr;  // unfolded encoder; [4][16] gamma1, beta1, gamma2, beta2
+    float *enc_w1f = nullptr, *enc_b1f = nullptr, *enc_w2f = nullptr, *enc_b2f = nullptr;  // batch-folded encoder
+    double *part = nullptr, *sum1 = nullptr;     // bn_stats_kernel partials [blocks][32]; pass-1 sums [16]
+    double *sums = nullptr, *part_db = nullptr;  // decoder backward: [32] sum dv, sum dv xhat; [act blocks][16]
+    float* rec = nullptr;                        // [max(T, 2)][2][16] batch mean, unbiased variance
+    int nrec = 0;                                // records the last forward entry wrote
+  } ct;
   std::vector<void*> owned;
   // schedule
   std::vector<int64_t> ts;
@@ -488,9 +505,10 @@ struct dd_engine {
   bool cond_ready = false;  // dd_build_condition has filled `cond` for the next dd_denoise_decode(cond = NULL)
   // CUDA graphs (DD_FLAG_CUDA_GRAPH), captured on first use and replayed: the T-step loop, the same loop with a decode
   // after every step (dd_denoise_decode_steps), the native backbone, the neck + FPN
-  enum { G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_COUNT = 4 };
-  cudaGraphExec_t graphs[G_COUNT] = {nullptr, nullptr, nullptr, nullptr};
-  int64_t graph_launches[G_COUNT] = {0, 0, 0, 0};  // kernel nodes per graph (added to `launches` per replay)
+  // (G_LOOP_STEPS_TRAIN: the step-decode loop in DD_CODEC_TRAIN, batch statistics before every decode)
+  enum { G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_LOOP_STEPS_TRAIN = 4, G_COUNT = 5 };
+  cudaGraphExec_t graphs[G_COUNT] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+  int64_t graph_launches[G_COUNT] = {0, 0, 0, 0, 0};  // kernel nodes per graph (added to `launches` per replay)
   int64_t graph_captures = 0;                      // graph instantiations since dd_create (dd_graph_capture_count)
   cudaStream_t cap_stream = nullptr;  // capture happens here (the caller's stream may be the legacy default stream)
   float* rgb_stage = nullptr;         // workspace copy of the image batch the backbone graph reads
@@ -593,6 +611,8 @@ size_t param_offset(int i) {
 int dec_act_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P * 4 + dd::DEC_ACT_PIX - 1) / dd::DEC_ACT_PIX); }
 int dec_wc_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P * 4 + dd::DEC_WC_PIX - 1) / dd::DEC_WC_PIX); }
 int dec_wt_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P + dd::DEC_WT_PIX - 1) / dd::DEC_WT_PIX); }
+// blocks of bn_stats_kernel over n items (the decoder's B x 2h x 2w is the largest codec BatchNorm)
+int codec_stats_blocks(long long n) { return static_cast<int>((n + dd::BNS_PIX - 1) / dd::BNS_PIX); }
 
 void drop_graph(dd_engine* e, int which) {
   if (e->graphs[which]) {
@@ -1033,12 +1053,56 @@ int split_planes(dd_engine* e, const float* x, __half* hi, __half* lo, size_t n,
   return check_launch("split_planes");
 }
 
+// Training-mode BatchNorm over n items of op's pre-BN value: two statistics passes, then the fold of (gamma, beta) =
+// gb[0..15], gb[16..31] into w_out / b_out (see dd::BnFoldArgs for the other pointers).
+template <class Op>
+int run_bn_batch(dd_engine* e, const Op& op, long long n, const float* gb, const float* bias, const float* w, int nw,
+                 float* w_out, float* b_out, float* bn_out, float* rec, cudaStream_t st) {
+  dd_engine::CodecTrain& ct = e->ct;
+  const int nblk = codec_stats_blocks(n);
+  int rc;
+  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, nullptr, ct.part);
+  if ((rc = launched(e, "bn_stats"))) return rc;
+  dd::part_colsum_kernel<<<1, 32, 0, st>>>(ct.part, nblk, dd::BNS_COLS, 16, ct.sum1);
+  if ((rc = launched(e, "part_colsum"))) return rc;
+  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, ct.sum1, ct.part);
+  if ((rc = launched(e, "bn_stats"))) return rc;
+  dd::BnFoldArgs f;
+  f.sum1 = ct.sum1;
+  f.part = ct.part;
+  f.nblk = nblk;
+  f.n = n;
+  f.gamma = gb;
+  f.beta = gb + 16;
+  f.bias = bias;
+  f.w = w;
+  f.nw = nw;
+  f.w_out = w_out;
+  f.b_out = b_out;
+  f.bn_out = bn_out;
+  f.rec = rec;
+  dd::bn_fold_kernel<<<1, 256, 0, st>>>(f);
+  return launched(e, "bn_fold");
+}
+
+// DD_CODEC_TRAIN: the decoder BatchNorm's statistics over the latent in x32, folded into ct.dec_wt / dec_bt / dec_bn
+// (which run_decoder then reads); rec: where the record goes (null: none).
+int run_dec_batch_stats(dd_engine* e, float* rec, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  const dd::DecPreBn op{e->x32, e->dec_wu, g.h, g.w};
+  dd_engine::CodecTrain& ct = e->ct;
+  return run_bn_batch(e, op, static_cast<long long>(g.B) * g.P * 4, ct.dec_gb, e->dec_bu, e->dec_wu, 4096, ct.dec_wt,
+                      ct.dec_bt, ct.dec_bn, rec, st);
+}
+
+// decoder_kernel on the running-statistics fold, or in DD_CODEC_TRAIN on the batch fold of the last run_dec_batch_stats
 int run_decoder(dd_engine* e, float* logit, float* depth, cudaStream_t st) {
   const Geom g = geom_of(e->cfg);
+  const bool train = e->codec_mode == DD_CODEC_TRAIN;
   dd::DecoderArgs a;
   a.x = e->x32;
-  a.wt = e->dec_wt;
-  a.bt = e->dec_bt;
+  a.wt = train ? e->ct.dec_wt : e->dec_wt;
+  a.bt = train ? e->ct.dec_bt : e->dec_bt;
   a.wc = e->dec_wc;
   a.bc = e->dec_bc;
   a.logit = logit;
@@ -1195,17 +1259,39 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
   if ((rc = dev_array(h, &h->dec_wt, 4 * 4 * 16 * 16))) return rc;
   if ((rc = dev_array(h, &h->dec_bt, 16))) return rc;
   if ((rc = dev_array(h, &h->dec_wc, 9 * 16))) return rc;
-  if (h->cfg.flags & DD_FLAG_LOOP_BACKWARD) {  // the decoder backward needs the BatchNorm unfolded
-    if ((rc = dev_array(h, &h->dec_wu, 4 * 4 * 16 * 16))) return rc;
-    if ((rc = dev_array(h, &h->dec_bu, 16))) return rc;
-    if ((rc = dev_array(h, &h->dec_bn, 3 * 16))) return rc;
-  }
+  // the decoder backward and DD_CODEC_TRAIN need the BatchNorm unfolded
+  if ((rc = dev_array(h, &h->dec_wu, 4 * 4 * 16 * 16))) return rc;
+  if ((rc = dev_array(h, &h->dec_bu, 16))) return rc;
+  if ((rc = dev_array(h, &h->dec_bn, 3 * 16))) return rc;
+  dd_engine::CodecTrain& ct = h->ct;
+  if ((rc = dev_array(h, &ct.dec_gb, 2 * 16))) return rc;
+  if ((rc = dev_array(h, &ct.dec_wt, 4 * 4 * 16 * 16))) return rc;
+  if ((rc = dev_array(h, &ct.dec_bt, 16))) return rc;
+  if ((rc = dev_array(h, &ct.dec_bn, 3 * 16))) return rc;
+  if ((rc = dev_array(h, &ct.zero16, 16))) return rc;
+  CUDA_TRY(cudaMemsetAsync(ct.zero16, 0, 16 * 4, st));
+  const Geom g = geom_of(h->cfg);
+  if ((rc = dev_array(h, &ct.part, static_cast<size_t>(codec_stats_blocks(static_cast<long long>(g.B) * g.P * 4)) *
+                                         dd::BNS_COLS)))
+    return rc;
+  if ((rc = dev_array(h, &ct.sum1, 16))) return rc;
+  if ((rc = dev_array(h, &ct.sums, 32))) return rc;
+  if ((rc = dev_array(h, &ct.part_db, static_cast<size_t>(dec_act_blocks(g)) * 16))) return rc;
+  if ((rc = dev_array(h, &ct.rec, static_cast<size_t>(std::max(h->cfg.num_inference_steps, 2)) * 32))) return rc;
+  ct.nrec = 0;
   h->enc_w1 = nullptr;
   if (encoder) {
     if ((rc = dev_array(h, &h->enc_w1, 144))) return rc;
     if ((rc = dev_array(h, &h->enc_b1, 16))) return rc;
     if ((rc = dev_array(h, &h->enc_w2, 2304))) return rc;
     if ((rc = dev_array(h, &h->enc_b2, 16))) return rc;
+    if ((rc = dev_array(h, &ct.enc_w1, 144))) return rc;
+    if ((rc = dev_array(h, &ct.enc_w2, 2304))) return rc;
+    if ((rc = dev_array(h, &ct.enc_gb, 4 * 16))) return rc;
+    if ((rc = dev_array(h, &ct.enc_w1f, 144))) return rc;
+    if ((rc = dev_array(h, &ct.enc_b1f, 16))) return rc;
+    if ((rc = dev_array(h, &ct.enc_w2f, 2304))) return rc;
+    if ((rc = dev_array(h, &ct.enc_b2f, 16))) return rc;
   }
   return DD_OK;
 }
@@ -1350,19 +1436,19 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     CUDA_TRY(cudaMemcpyAsync(h->dec_wc, sg->wc_f, sizeof(sg->wc_f), cudaMemcpyHostToDevice, st));
     steps_stale |= sg->dec_bc[0] != h->dec_bc;
     h->dec_bc = sg->dec_bc[0];
-    if (h->cfg.flags & DD_FLAG_LOOP_BACKWARD) {
-      for (int co = 0; co < 16; ++co) {
-        const double rstd = 1.0 / sqrt(static_cast<double>(sg->dec_var[co]) + 1e-5);
-        sg->bn[co] = static_cast<float>(static_cast<double>(sg->dec_g[co]) * rstd);
-        sg->bn[16 + co] = sg->dec_mu[co];
-        sg->bn[32 + co] = static_cast<float>(rstd);
-        for (int ci = 0; ci < 16; ++ci)
-          for (int k = 0; k < 16; ++k) sg->wu[(k * 16 + ci) * 16 + co] = sg->dec_wt[(ci * 16 + co) * 16 + k];
-      }
-      CUDA_TRY(cudaMemcpyAsync(h->dec_wu, sg->wu, sizeof(sg->wu), cudaMemcpyHostToDevice, st));
-      CUDA_TRY(cudaMemcpyAsync(h->dec_bu, sg->dec_bt, sizeof(sg->dec_bt), cudaMemcpyHostToDevice, st));
-      CUDA_TRY(cudaMemcpyAsync(h->dec_bn, sg->bn, sizeof(sg->bn), cudaMemcpyHostToDevice, st));
+    for (int co = 0; co < 16; ++co) {  // unfolded: the decoder backward and DD_CODEC_TRAIN
+      const double rstd = 1.0 / sqrt(static_cast<double>(sg->dec_var[co]) + 1e-5);
+      sg->bn[co] = static_cast<float>(static_cast<double>(sg->dec_g[co]) * rstd);
+      sg->bn[16 + co] = sg->dec_mu[co];
+      sg->bn[32 + co] = static_cast<float>(rstd);
+      for (int ci = 0; ci < 16; ++ci)
+        for (int k = 0; k < 16; ++k) sg->wu[(k * 16 + ci) * 16 + co] = sg->dec_wt[(ci * 16 + co) * 16 + k];
     }
+    CUDA_TRY(cudaMemcpyAsync(h->dec_wu, sg->wu, sizeof(sg->wu), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->dec_bu, sg->dec_bt, sizeof(sg->dec_bt), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->dec_bn, sg->bn, sizeof(sg->bn), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->ct.dec_gb, sg->dec_g, 16 * 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->ct.dec_gb + 16, sg->dec_be, 16 * 4, cudaMemcpyHostToDevice, st));
   }
   if (enc) {
     float s1[16], s2[16];
@@ -1382,10 +1468,26 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     CUDA_TRY(cudaMemcpyAsync(h->enc_b1, sg->t1, sizeof(sg->t1), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(h->enc_w2, sg->f2, sizeof(sg->f2), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(h->enc_b2, sg->t2, sizeof(sg->t2), cudaMemcpyHostToDevice, st));
+    for (int co = 0; co < 16; ++co) {  // unfolded, for DD_CODEC_TRAIN
+      for (int tap = 0; tap < 9; ++tap) {
+        sg->e1u[tap * 16 + co] = sg->enc_w1[co * 9 + tap];
+        for (int ci = 0; ci < 16; ++ci) sg->e2u[(tap * 16 + ci) * 16 + co] = sg->enc_w2[(co * 16 + ci) * 9 + tap];
+      }
+      sg->enc_gb[0][co] = sg->enc_bn1[0][co];
+      sg->enc_gb[1][co] = sg->enc_bn1[1][co];
+      sg->enc_gb[2][co] = sg->enc_bn2[0][co];
+      sg->enc_gb[3][co] = sg->enc_bn2[1][co];
+    }
+    CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w1, sg->e1u, sizeof(sg->e1u), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w2, sg->e2u, sizeof(sg->e2u), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->ct.enc_gb, sg->enc_gb, sizeof(sg->enc_gb), cudaMemcpyHostToDevice, st));
   }
   CUDA_TRY(cudaEventRecord(h->pack_done, st));
   if (loop_stale) drop_graph(h, dd_engine::G_LOOP);
-  if (loop_stale || steps_stale) drop_graph(h, dd_engine::G_LOOP_STEPS);
+  if (loop_stale || steps_stale) {
+    drop_graph(h, dd_engine::G_LOOP_STEPS);
+    drop_graph(h, dd_engine::G_LOOP_STEPS_TRAIN);
+  }
   return DD_OK;
 }
 
@@ -2181,17 +2283,20 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
   const Geom g = geom_of(e->cfg);
   dd_engine::LoopBwd& l = e->lp;
   const size_t nout = static_cast<size_t>(g.B) * g.P * 4;
+  const bool train = e->codec_mode == DD_CODEC_TRAIN;
   int rc;
+  // DD_CODEC_TRAIN: the same statistics in the same order as the forward's, so the fold and the ReLU mask are its own
+  if (train && (rc = run_dec_batch_stats(e, nullptr, st))) return rc;
   if ((rc = run_decoder(e, l.z, l.r, st))) return rc;  // the forward's logit z; its depth lands in r (scratch until below)
   dd::dec_dz_kernel<<<grid_of(nout), 256, 0, st>>>(l.z, d_depth, nout, 1e-6f);
   if ((rc = launched(e, "dec_dz"))) return rc;
   dd::DecBwdArgs a;
   a.x = e->x32;
-  a.wt = e->dec_wt;
-  a.bt = e->dec_bt;
+  a.wt = train ? e->ct.dec_wt : e->dec_wt;
+  a.bt = train ? e->ct.dec_bt : e->dec_bt;
   a.wu = e->dec_wu;
-  a.bu = e->dec_bu;
-  a.bn = e->dec_bn;
+  a.bu = train ? e->ct.zero16 : e->dec_bu;  // DD_CODEC_TRAIN: xhat from the bias-free conv, as its statistics
+  a.bn = train ? e->ct.dec_bn : e->dec_bn;
   a.wc = e->dec_wc;
   a.dz = l.z;
   a.r = l.r;
@@ -2205,6 +2310,12 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
   a.w = g.w;
   dd::dec_bwd_act_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a);
   if ((rc = launched(e, "dec_bwd_act"))) return rc;
+  if (train) {  // du through the batch mean and variance
+    dd::part_colsum_kernel<<<1, 32, 0, st>>>(l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, e->ct.sums);
+    if ((rc = launched(e, "part_colsum"))) return rc;
+    dd::dec_bwd_bn_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a, e->ct.sums, e->ct.part_db);
+    if ((rc = launched(e, "dec_bwd_bn"))) return rc;
+  }
   if (dx != nullptr) {
     dd::dec_bwd_dx_kernel<<<static_cast<int>((static_cast<size_t>(g.B) * g.P + 255) / 256), 256, 0, st>>>(a);
     if ((rc = launched(e, "dec_bwd_dx"))) return rc;
@@ -2223,7 +2334,8 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
   f.nb_act = dec_act_blocks(g);
   f.nb_wc = dec_wc_blocks(g);
   f.nb_wt = dec_wt_blocks(g);
-  f.bn = e->dec_bn;
+  f.bn = a.bn;
+  f.part_db = train ? e->ct.part_db : nullptr;
   for (int i = 0; i < 6; ++i) f.out[i] = dp[i];
   dd::dec_bwd_finish_kernel<<<(dd::DEC_GRAD_N + 255) / 256, 256, 0, st>>>(f);
   return launched(e, "dec_bwd_finish");
@@ -2532,16 +2644,20 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
   const int T = h->cfg.num_inference_steps;
   const size_t map_elems = static_cast<size_t>(g.B) * g.P * 4;  // one decoded batch [B][2h][2w]
   const bool steps = depth_steps_out != nullptr;
+  const bool train = h->codec_mode == DD_CODEC_TRAIN;  // batch statistics before every decode, one record each
+  h->ct.nrec = 0;
   auto loop = [&](cudaStream_t s) -> int {
     for (int i = 0; i < T; ++i) {
       int r = run_step(h, h->temb + h->ts[i] * 256, 0, h->cx[i], h->ce[i], nullptr, s);
+      if (r == DD_OK && steps && train) r = run_dec_batch_stats(h, h->ct.rec + i * 32, s);
       if (r == DD_OK && steps) r = run_decoder(h, nullptr, h->inter + i * map_elems, s);
       if (r != DD_OK) return r;
     }
     return DD_OK;
   };
   if (h->cfg.flags & DD_FLAG_CUDA_GRAPH) {
-    if ((rc = graph_run(h, steps ? dd_engine::G_LOOP_STEPS : dd_engine::G_LOOP, st, loop))) return rc;
+    const int which = steps ? (train ? dd_engine::G_LOOP_STEPS_TRAIN : dd_engine::G_LOOP_STEPS) : dd_engine::G_LOOP;
+    if ((rc = graph_run(h, which, st, loop))) return rc;
   } else if ((rc = loop(st))) {
     return rc;
   }
@@ -2550,10 +2666,15 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
     if (depth_out)
       CUDA_TRY(cudaMemcpyAsync(depth_out, h->inter + static_cast<size_t>(T - 1) * map_elems, map_elems * 4,
                                cudaMemcpyDeviceToDevice, st));
-    if (logit_out)  // the logits of the final map only: one more (cheap) decode, its depth lands in the scratch slot
+    // the logits of the final map only: one more (cheap) decode, its depth lands in the scratch slot; in
+    // DD_CODEC_TRAIN it reuses the last step's batch fold and records nothing
+    if (logit_out)
       if ((rc = run_decoder(h, logit_out, h->inter + static_cast<size_t>(T - 1) * map_elems, st))) return rc;
-  } else if ((rc = run_decoder(h, logit_out, depth_out, st))) {
-    return rc;
+    h->ct.nrec = train ? T : 0;
+  } else {
+    if (train && (rc = run_dec_batch_stats(h, h->ct.rec, st))) return rc;
+    if ((rc = run_decoder(h, logit_out, depth_out, st))) return rc;
+    h->ct.nrec = train ? 1 : 0;
   }
   if (latent_out) {
     if ((rc = transpose_out(h->x32, latent_out, g.B, 16, g.P, st))) return rc;
@@ -2804,7 +2925,31 @@ int dd_decode(dd_handle h, const float* latent, float* logit_out, float* depth_o
   if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
   const Geom g = geom_of(h->cfg);
   if ((rc = transpose_in(latent, h->x32, g.B, 16, g.P, st))) return rc;
+  const bool train = h->codec_mode == DD_CODEC_TRAIN;
+  h->ct.nrec = 0;
+  if (train && (rc = run_dec_batch_stats(h, h->ct.rec, st))) return rc;
+  h->ct.nrec = train ? 1 : 0;
   return run_decoder(h, logit_out, depth_out, st);
+}
+
+int dd_set_codec_mode(dd_handle h, int32_t mode) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  if (mode != DD_CODEC_EVAL && mode != DD_CODEC_TRAIN) return fail(DD_ERR_INVALID, "codec mode must be DD_CODEC_EVAL or DD_CODEC_TRAIN");
+  h->codec_mode = mode;
+  return DD_OK;
+}
+
+int dd_codec_batch_stats(dd_handle h, float* dev_out, int32_t capacity, int32_t* n_out, void* cuda_stream) {
+  if (!h || !n_out) return fail(DD_ERR_INVALID, "null argument");
+  const int n = h->ct.nrec;
+  if (n > 0) {
+    if (!dev_out || capacity < n) return fail(DD_ERR_INVALID, "dev_out holds fewer records than the last forward wrote");
+    CUDA_TRY(cudaSetDevice(h->cfg.device));
+    CUDA_TRY(cudaMemcpyAsync(dev_out, h->ct.rec, static_cast<size_t>(n) * 32 * 4, cudaMemcpyDeviceToDevice,
+                             static_cast<cudaStream_t>(cuda_stream)));
+  }
+  *n_out = n;
+  return DD_OK;
 }
 
 int dd_enable_producers(dd_handle h, const dd_producer_config* pc) {
@@ -3090,14 +3235,31 @@ int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, fl
   if (!h->weights_ready || !h->enc_w1) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
   if ((height + 1) / 2 != h->cfg.latent_h || (width + 1) / 2 != h->cfg.latent_w)
     return fail(DD_ERR_INVALID, "depth map size does not match the engine's latent grid");
+  const bool train = h->codec_mode == DD_CODEC_TRAIN;
+  if (train && static_cast<long long>(h->cfg.batch) * h->cfg.latent_h * h->cfg.latent_w < 2)
+    return fail(DD_ERR_INVALID, "training-mode BatchNorm needs more than 1 value per channel (batch x latent = 1)");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CUDA_TRY(cudaSetDevice(h->cfg.device));
+  dd_engine::CodecTrain& ct = h->ct;
+  ct.nrec = 0;
+  if (train) {  // BN1 over conv1, then BN2 over conv2 of the batch-normalised, activated conv1; records 0 and 1
+    const long long n = static_cast<long long>(h->cfg.batch) * h->cfg.latent_h * h->cfg.latent_w;
+    const dd::EncPreBn1 op1{depth, ct.enc_w1, height, width, h->cfg.latent_h, h->cfg.latent_w};
+    int rc;
+    if ((rc = run_bn_batch(h, op1, n, ct.enc_gb, nullptr, ct.enc_w1, 144, ct.enc_w1f, ct.enc_b1f, nullptr, ct.rec, st)))
+      return rc;
+    const dd::EncPreBn2 op2{depth, ct.enc_w1f, ct.enc_b1f, ct.enc_w2, height, width, h->cfg.latent_h, h->cfg.latent_w};
+    if ((rc = run_bn_batch(h, op2, n, ct.enc_gb + 32, nullptr, ct.enc_w2, 2304, ct.enc_w2f, ct.enc_b2f, nullptr,
+                           ct.rec + 32, st)))
+      return rc;
+    ct.nrec = 2;
+  }
   dd::EncoderArgs a;
   a.depth = depth;
-  a.w1 = h->enc_w1;
-  a.b1 = h->enc_b1;
-  a.w2 = h->enc_w2;
-  a.b2 = h->enc_b2;
+  a.w1 = train ? ct.enc_w1f : h->enc_w1;
+  a.b1 = train ? ct.enc_b1f : h->enc_b1;
+  a.w2 = train ? ct.enc_w2f : h->enc_w2;
+  a.b2 = train ? ct.enc_b2f : h->enc_b2;
   a.out = latent_out;
   a.H = height;
   a.W = width;

@@ -433,6 +433,22 @@ class DenoiseEngine:
                                        C.c_void_p(self._stream())))
         return out
 
+    def set_codec_mode(self, training: bool):
+        """The depth codec's BatchNorms on batch statistics (`training`, as torch's BatchNorm2d in training mode) or on
+        their running statistics (the default) for every later encode / decode / denoise_decode(_steps) and their
+        backward.  The engine never updates running statistics; `codec_batch_stats` returns what a caller needs to."""
+        _cabi.check(self.lib.dd_set_codec_mode(self._h, _cabi.CODEC_TRAIN if training else _cabi.CODEC_EVAL))
+
+    def codec_batch_stats(self) -> torch.Tensor:
+        """[n, 2, 16]: (batch mean, unbiased batch variance) of every codec BatchNorm the last forward call evaluated in
+        training mode, in evaluation order (decode: 1, denoise_decode_steps: T, encode: 2; n = 0 after an eval-mode
+        call).  Ordered on the current stream; no synchronisation."""
+        out = torch.empty(max(self.steps, 2), 2, 16, device=self.device, dtype=torch.float32)
+        n = C.c_int32()
+        _cabi.check(self.lib.dd_codec_batch_stats(self._h, C.c_void_p(out.data_ptr()), out.shape[0], C.byref(n),
+                                                  C.c_void_p(self._stream())))
+        return out[:n.value]
+
     def decode(self, latent: torch.Tensor, want_logits=False):
         B, (h, w) = self.batch, self.latent_hw
         self._check_in(latent, (B, 16, h, w))

@@ -147,12 +147,13 @@ class _LoopFunction(torch.autograd.Function):
     loop_backward=True, which re-runs the loop and walks back through every step and the decoder."""
 
     @staticmethod
-    def forward(ctx, head, eng, box, cond_in_workspace, keys, cond, noise, *params):
+    def forward(ctx, head, eng, box, cond_in_workspace, keys, codec_train, cond, noise, *params):
+        eng.set_codec_mode(codec_train)
         depth, latent, logits = eng.denoise_decode(None if cond_in_workspace else cond, noise, want_latent=True,
                                                    want_logits=head.capture_logits)
         box["logits"] = logits
         ctx.save_for_backward(cond, noise)
-        ctx.head, ctx.keys = head, keys
+        ctx.head, ctx.keys, ctx.codec_train = head, keys, codec_train
         ctx.set_materialize_grads(False)
         return depth, latent
 
@@ -163,11 +164,25 @@ class _LoopFunction(torch.autograd.Function):
         if d_depth is None and d_latent is None:
             return (None,) * len(need)
         eng = ctx.head._engine(noise.shape[0], noise.shape[-2:], cond.shape[-2:], noise.device, loop_backward=True)
+        eng.set_codec_mode(ctx.codec_train)  # differentiate the decoder the forward ran
         d_cond, d_noise, grads, _ = eng.denoise_backward(
             cond.contiguous().float(), noise, None if d_depth is None else d_depth.contiguous().float(),
             None if d_latent is None else d_latent.contiguous().float(),
-            want_cond=need[5], want_noise=need[6], want_params=any(need[7:]))
-        return (None,) * 5 + (d_cond, d_noise) + tuple(grads[k] if need[7 + i] else None for i, k in enumerate(ctx.keys))
+            want_cond=need[6], want_noise=need[7], want_params=any(need[8:]))
+        return (None,) * 6 + (d_cond, d_noise) + tuple(grads[k] if need[8 + i] else None for i, k in enumerate(ctx.keys))
+
+
+def bn_running_update(bn: nn.BatchNorm2d, mean: torch.Tensor, var: torch.Tensor):
+    """The running-statistic update torch's training-mode BatchNorm (F.batch_norm) makes after one batch with mean `mean`
+    and UNBIASED variance `var`: num_batches_tracked += 1, then running = (1 - f) running + f batch with f = momentum,
+    or 1 / num_batches_tracked when momentum is None.  Stays on the buffers' device (no synchronisation)."""
+    if not bn.track_running_stats:
+        return
+    with torch.no_grad():
+        bn.num_batches_tracked.add_(1)
+        f = bn.momentum if bn.momentum is not None else 1.0 / bn.num_batches_tracked.to(bn.running_mean.dtype)
+        bn.running_mean.mul_(1 - f).add_(mean.to(bn.running_mean) * f)
+        bn.running_var.mul_(1 - f).add_(var.to(bn.running_var) * f)
 
 
 class DDIMHeadBase(nn.Module):
@@ -183,6 +198,12 @@ class DDIMHeadBase(nn.Module):
     # decoder (native dd_denoise_backward), so the L1 / L2 depth losses train the head and `ddim_loss` also reaches the
     # loop through its re-noised latent.  Off by default: it changes what `ddim_loss.backward()` costs and computes.
     grad_through_loop = False
+    # Training-mode BatchNorm in the depth codec (reference `net.train()`): when True and `depth_transform.training`, the
+    # engine's encoder and decoder normalise with the statistics of the batch they see, the decoder's gradients flow
+    # through those statistics, and every forward applies torch's running-statistic update to the codec's BatchNorm
+    # buffers (re-packed by `update_weights` before the next call).  Off by default: the codec then runs on its running
+    # statistics in every mode.
+    codec_train_bn = False
 
     def __init__(self, in_channels=None, up_scale_factor=1, inference_steps=20, num_train_timesteps=1000,
                  return_indices=None, depth_transform_cfg=None, detach_fp=False, depth_embed_dim=16,
@@ -487,6 +508,30 @@ class DDIMHeadBase(nn.Module):
         eng = self._any_engine(B, noisy.shape[-2:], cond.shape[-2:], noisy.device)
         return eng.denoiser_forward(cond.contiguous().float(), noisy.contiguous().float(), tl)
 
+    # ------------------------------------------------------------------------------------------ codec BatchNorms
+    def _codec_bns(self):
+        """The codec's BatchNorms: encoder (conv_transform.0.1, .1.1), decoder (conv_inv_transform.1)."""
+        dt = self.depth_transform
+        return dt.conv_transform[0][1], dt.conv_transform[1][1], dt.conv_inv_transform[1]
+
+    def _codec_training(self) -> bool:
+        """Whether this forward runs the codec's BatchNorms on batch statistics (`codec_train_bn` and the codec in
+        training mode); the engine's BatchNorms use eps = 1e-5 only."""
+        if not (self.codec_train_bn and getattr(self.depth_transform, "training", False)):
+            return False
+        for bn in self._codec_bns():
+            if bn.eps != 1e-5:
+                raise EngineError(f"codec_train_bn: the engine's codec BatchNorms use eps = 1e-5, got {bn.eps}")
+        return True
+
+    @staticmethod
+    def _codec_records(eng, bns, order=None):
+        """[(BatchNorm, batch mean, unbiased batch variance)] from `eng`'s records of its last forward call: record
+        `order[i]` (default: i) for the i-th entry of `bns`."""
+        rec = eng.codec_batch_stats()
+        return [(bn, rec[i if order is None else order[i], 0], rec[i if order is None else order[i], 1])
+                for i, bn in enumerate(bns)]
+
     # ------------------------------------------------------------------------------------------ condition path
     def _condition(self, fp):
         """Top-down FPN that builds the 256-channel condition map x (head :112-122 / res.py:108-118)."""
@@ -544,6 +589,9 @@ class DDIMHeadBase(nn.Module):
         x_T = self._draw_noise((B, 16, *latent_hw), dev, dtype, noise)
         if self.grad_through_loop and self.return_intermediates:
             raise EngineError("grad_through_loop is not supported by the *Vis heads (pred_inter has no backward)")
+        codec_train = self._codec_training()
+        enc_bn1, enc_bn2, dec_bn = self._codec_bns() if codec_train else (None,) * 3
+        codec_updates = []  # applied at the end: the buffers keep the signature the engines were packed with until then
         if native:  # (backbone +) neck + FPN + loop + decoder inside the engine; the condition map never leaves NHWC
             want_cond = self.capture_cond or self.training or self.eval_ddim_loss or self.grad_through_loop
             if with_backbone:
@@ -554,7 +602,10 @@ class DDIMHeadBase(nn.Module):
             else:
                 eng = self._engine(B, latent_hw, tuple(fp[0].shape[-2:]), dev, feats=fp)
                 cond = eng.build_condition(fp, want_cond=want_cond)
+            eng.set_codec_mode(codec_train)
             gt_map_t = eng.encode(gt_depth_map.contiguous().float())  # returned as pred_init / gt_map_t only
+            if codec_train:
+                codec_updates += self._codec_records(eng, (enc_bn1, enc_bn2))
             loop_cond = None
         else:
             eng = self._engine(B, latent_hw, tuple(cond.shape[-2:]), dev)
@@ -567,22 +618,32 @@ class DDIMHeadBase(nn.Module):
                 loop_keys = None
         if loop_keys is not None:  # the same denoise_decode call, as an autograd node (native backward through the loop)
             box = {}
-            refined_depth, refined_depth_t = _LoopFunction.apply(self, eng, box, loop_cond is None, loop_keys, cond,
-                                                                 x_T, *loop_params)
+            refined_depth, refined_depth_t = _LoopFunction.apply(self, eng, box, loop_cond is None, loop_keys,
+                                                                 codec_train, cond, x_T, *loop_params)
             logits = box["logits"]
         elif self.return_intermediates:  # *Vis heads: inv_t of every intermediate latent, decoded inside the graph
+            eng.set_codec_mode(codec_train)
             steps, refined_depth_t, logits = eng.denoise_decode_steps(loop_cond, x_T, want_latent=True,
                                                                       want_logits=self.capture_logits)
             inter = list(steps.unbind(0))
             refined_depth = inter[-1]
         else:
+            eng.set_codec_mode(codec_train)
             refined_depth, refined_depth_t, logits = eng.denoise_decode(loop_cond, x_T, want_latent=True,
                                                                         want_logits=self.capture_logits)
+        if codec_train:
+            if self.return_intermediates:  # the reference's order: inv_t of the final map, then of steps 1 .. T
+                T = self.diffusion_inference_steps
+                codec_updates += self._codec_records(eng, (dec_bn,) * (T + 1), order=[T - 1] + list(range(T)))
+            else:
+                codec_updates += self._codec_records(eng, (dec_bn,))
         self.last_latent, self.last_logits, self.last_cond = refined_depth_t, logits, cond
         if self.check_range:
             eng.poll_status()  # syncs; raises if an activation left the fp16 split range (DESIGN.md "Numerics")
         ddim_loss = self._ddim_loss(cond, refined_depth_t) if (self.eval_ddim_loss or self.training) \
             else refined_depth.new_zeros(())
+        for bn, mean, var in codec_updates:
+            bn_running_update(bn, mean, var)
         return {'pred': refined_depth, 'pred_init': gt_map_t, 'blur_depth_t': gt_map_t, 'ddim_loss': ddim_loss,
                 'gt_map_t': gt_map_t, 'pred_uncertainty': None, 'pred_inter': inter, 'weight_map': None,
                 'guidance': None, 'offset': None, 'aff': None, 'gamma': None, 'confidence': None}

@@ -308,6 +308,26 @@ int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, f
  * latent_out [B,16,ceil(height/2),ceil(width/2)].  Needs the optional keys `depth_transform.conv_transform.*`. */
 int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, void* cuda_stream);
 
+/* How the depth codec's BatchNorms normalise.  DD_CODEC_EVAL (the default): running statistics, folded into the
+ * weights at dd_finalize_weights.  DD_CODEC_TRAIN: as BatchNorm2d in training mode, the statistics of the batch
+ * each call sees (biased variance, eps 1e-5), computed and folded on the device without synchronising:
+ *   dd_decode, dd_denoise_decode           one batch-statistics decode                      (1 record)
+ *   dd_denoise_decode_steps                one per step, inside a CUDA graph of its own      (T records)
+ *   dd_encode                              both BatchNorms, the second after the first       (2 records)
+ *   dd_decode_backward, dd_denoise_backward  differentiate through the batch mean and variance
+ * The backward's recompute and the steps variant's extra logit decode record nothing.  The engine never writes running
+ * statistics: the caller applies the running update from the records and registers the new buffers with
+ * dd_update_weights.  In DD_CODEC_TRAIN dd_encode returns DD_ERR_INVALID when batch x latent is 1 (one value per
+ * channel).  The mode is engine state; DD_ERR_INVALID for a value other than the two below. */
+enum dd_codec_mode { DD_CODEC_EVAL = 0, DD_CODEC_TRAIN = 1 };
+int dd_set_codec_mode(dd_handle h, int32_t mode);
+
+/* Batch statistics of every codec BatchNorm the last forward entry (dd_decode, dd_denoise_decode(_steps), dd_encode)
+ * evaluated in DD_CODEC_TRAIN, in evaluation order: dev_out [n][2][16] fp32 (batch mean, unbiased variance),
+ * *n_out = n (0 after a forward in DD_CODEC_EVAL).  Enqueued on cuda_stream, no synchronisation; DD_ERR_INVALID when
+ * capacity < n. */
+int dd_codec_batch_stats(dd_handle h, float* dev_out, int32_t capacity, int32_t* n_out, void* cuda_stream);
+
 /* Synchronise `cuda_stream` and report DD_ERR_RANGE if any activation left the fp16 split's range since the
  * last hot-path call started (DD_OK otherwise).  The hot-path calls themselves never synchronise unless
  * DD_FLAG_CHECK_RANGE is set. */
