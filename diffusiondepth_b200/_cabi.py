@@ -39,8 +39,9 @@ ABI_VERSION = 1
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
 FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD, FLAG_LOOP_BACKWARD = 64, 128, 256, 512
-FLAG_CHAIN_PRED = 1024
+FLAG_CHAIN_PRED, FLAG_PRODUCER_TRAIN = 1024, 2048
 CODEC_EVAL, CODEC_TRAIN = 0, 1
+PRODUCER_EVAL, PRODUCER_TRAIN = 0, 1
 STATUS = {0: "DD_OK", 1: "DD_ERR_INVALID", 2: "DD_ERR_CUDA", 3: "DD_ERR_UNSUPPORTED", 4: "DD_ERR_RANGE"}
 
 # name -> (restype, argtypes); every symbol include/dd_engine.h declares
@@ -81,6 +82,10 @@ SIGNATURES = {
     "dd_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "dd_set_codec_mode": (C.c_int, [C.c_void_p, C.c_int32]),
     "dd_codec_batch_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
+    "dd_set_producer_mode": (C.c_int, [C.c_void_p, C.c_int32]),
+    "dd_producer_batch_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.c_void_p]),
+    "dd_producer_bn_info": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int32),
+                                      C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
     "dd_last_launch_count": (C.c_int64, [C.c_void_p]),
     "dd_poll_status": (C.c_int, [C.c_void_p, C.c_void_p]),
     "dd_conv3x3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

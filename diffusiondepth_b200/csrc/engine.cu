@@ -22,6 +22,7 @@
 #include "mpvit.cuh"
 #include "backward.cuh"
 #include "codec_train.cuh"
+#include "producer_train.cuh"
 
 namespace {
 
@@ -468,6 +469,30 @@ struct dd_engine {
     float* rec = nullptr;                        // [max(T, 2)][2][16] batch mean, unbiased variance
     int nrec = 0;                                // records the last forward entry wrote
   } ct;
+  // DD_PRODUCER_TRAIN (dd_set_producer_mode; DD_FLAG_PRODUCER_TRAIN): the producers' BatchNorms on batch statistics.
+  // Every BatchNorm'ed producer layer, in evaluation order (ResNet bn1 / bn2 block by block, then per level the neck's
+  // lateral / proj / fusion, then the FPN top-down: lateral, conv_up), keeps an unfolded pack of its conv and device
+  // copies of gamma / beta; the scratch below is engine-owned and sized for the largest layer.
+  int producer_mode = DD_PRODUCER_EVAL;
+  struct ProdBn {
+    const GenLayer* eval = nullptr;  // the layer's eval (folded) pack, which names it at run time
+    GenLayer raw;                    // conv (or ConvT) weights alone: no BatchNorm, zero shift
+    float *gamma = nullptr, *beta = nullptr;
+    int C = 0;                       // BatchNorm channels
+    int stage = 0;                   // 0: dd_run_backbone, 1: dd_build_condition
+    long long n = 0;                 // pixels of the pre-BN output (a ConvT's: B x 2H x 2W)
+    bool fresh = false;              // evaluated in DD_PRODUCER_TRAIN since the forward started
+    size_t rec_off = 0;              // floats into `rec`: [2][C] batch mean, unbiased batch variance
+    std::string key;                 // registered key prefix of the BatchNorm
+  };
+  struct ProdTrain {
+    std::vector<ProdBn> layers;
+    std::map<const GenLayer*, int> index;
+    float* U = nullptr;                              // pre-BN conv output, fp32 NHWC
+    double *part = nullptr, *sum1 = nullptr;         // pbn_stats_kernel partials [blocks][2][C]; pass-1 sums [C]
+    float *s = nullptr, *t = nullptr, *rec = nullptr;  // batch scale / shift [C]; records
+    size_t rec_floats = 0;
+  } pt;
   std::vector<void*> owned;
   // schedule
   std::vector<int64_t> ts;
@@ -506,9 +531,13 @@ struct dd_engine {
   // CUDA graphs (DD_FLAG_CUDA_GRAPH), captured on first use and replayed: the T-step loop, the same loop with a decode
   // after every step (dd_denoise_decode_steps), the native backbone, the neck + FPN
   // (G_LOOP_STEPS_TRAIN: the step-decode loop in DD_CODEC_TRAIN, batch statistics before every decode)
-  enum { G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_LOOP_STEPS_TRAIN = 4, G_COUNT = 5 };
-  cudaGraphExec_t graphs[G_COUNT] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  int64_t graph_launches[G_COUNT] = {0, 0, 0, 0, 0};  // kernel nodes per graph (added to `launches` per replay)
+  // (G_BACKBONE_TRAIN, G_COND_TRAIN: the ResNet backbone and the neck + FPN in DD_PRODUCER_TRAIN)
+  enum {
+    G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_LOOP_STEPS_TRAIN = 4, G_BACKBONE_TRAIN = 5,
+    G_COND_TRAIN = 6, G_COUNT = 7
+  };
+  cudaGraphExec_t graphs[G_COUNT] = {};
+  int64_t graph_launches[G_COUNT] = {};  // kernel nodes per graph (added to `launches` per replay)
   int64_t graph_captures = 0;                      // graph instantiations since dd_create (dd_graph_capture_count)
   cudaStream_t cap_stream = nullptr;  // capture happens here (the caller's stream may be the legacy default stream)
   float* rgb_stage = nullptr;         // workspace copy of the image batch the backbone graph reads
@@ -1789,6 +1818,162 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
                     st, 0, nullptr, e->prod.KS);
 }
 
+// ------------------------------------------------------------------------------------------------ producer BatchNorms
+// DD_PRODUCER_TRAIN (producer_train.cuh).  One BatchNorm'ed layer: the unfolded pack of its conv weight `wkey` (as
+// pack_gen reads it, without the BatchNorm), device copies of gamma / beta of `bnkey`, and its pre-BN output size.
+int add_bn_layer(dd_engine* e, const GenLayer& ev, const std::string& wkey, const std::string& bnkey, int cin,
+                 int cout_conv, int taps, bool transposed, int cin_pad, int stage, long long n, cudaStream_t st,
+                 float* scratch) {
+  dd_engine::ProdBn b;
+  b.eval = &ev;
+  b.C = cout_conv;
+  b.stage = stage;
+  b.n = n;
+  b.key = bnkey;
+  const Raw* w = find(e, wkey);
+  if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
+  const float* bn[4] = {nullptr, nullptr, nullptr, nullptr};
+  int rc;
+  if ((rc = find_bn(e, bnkey, bn))) return rc;
+  if ((rc = pack_gen_weights(e, e->owned, b.raw, w->ptr, wkey, nullptr, nullptr, cin, cout_conv, taps, transposed,
+                             cin_pad, 0, st, scratch)))
+    return rc;
+  b.raw.stride = ev.stride;
+  if ((rc = dev_array(e, &b.gamma, cout_conv))) return rc;
+  if ((rc = dev_array(e, &b.beta, cout_conv))) return rc;
+  CUDA_TRY(cudaMemcpyAsync(b.gamma, bn[0], cout_conv * 4, cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(b.beta, bn[1], cout_conv * 4, cudaMemcpyDeviceToDevice, st));
+  e->pt.layers.push_back(b);
+  return DD_OK;
+}
+
+int pbn_blocks(long long n) { return static_cast<int>((n + dd::PBN_ROWS - 1) / dd::PBN_ROWS); }
+
+// Every BatchNorm'ed producer layer in evaluation order (after pack_producers / pack_resnet), and the scratch for the
+// largest of them.  DD_FLAG_PRODUCER_TRAIN only.
+int pack_prod_train(dd_engine* e, cudaStream_t st, float* scratch) {
+  dd_engine::ProdTrain& pt = e->pt;  // reset by dd_finalize_weights: the previous pack's buffers went with `owned`
+  const long long B = e->cfg.batch;
+  int rc;
+  if (e->rn.enabled) {
+    ResNetW& r = e->rn;
+    for (int s = 0; s < 4; ++s) {
+      const int cprev = s == 0 ? 3 : r.C[s - 1];
+      const long long n = B * r.Hs[s] * r.Ws[s];
+      for (int b = 0; b < r.depths[s]; ++b) {
+        const std::string bp = "backbone.layers." + std::to_string(s) + "." + std::to_string(b) + ".";
+        const int cin = b == 0 ? cprev : r.C[s];
+        const int pad = (cin % dd::GEN_BK) ? dd::GEN_BK : 0;
+        if ((rc = add_bn_layer(e, r.blocks[s][b].c1, bp + "conv1.weight", bp + "bn1", cin, r.C[s], 9, false, pad, 0, n,
+                               st, scratch))) return rc;
+        if ((rc = add_bn_layer(e, r.blocks[s][b].c2, bp + "conv2.weight", bp + "bn2", r.C[s], r.C[s], 9, false, 0, 0, n,
+                               st, scratch))) return rc;
+      }
+    }
+  }
+  if (e->prod.enabled) {
+    Producers& p = e->prod;
+    for (int i = 0; p.neck && i < p.nlev; ++i) {
+      const std::string si = std::to_string(i), h = "hahineck.";
+      const long long n = B * p.H[i] * p.W[i];
+      const std::string pj = i == 0 ? h + "conv_proj.0" : h + "trans_proj." + std::to_string(i - 1);
+      const std::string fs = i == 0 ? h + "conv_fusion.0" : h + "trans_fusion." + std::to_string(i - 1);
+      if ((rc = add_bn_layer(e, p.lat[i], h + "lateral_convs." + si + ".conv.weight", h + "lateral_convs." + si + ".bn",
+                             p.C[i], p.C[i], 1, false, 0, 1, n, st, scratch))) return rc;
+      if ((rc = add_bn_layer(e, p.proj[i], pj + ".conv.weight", pj + ".bn", p.C[i], 512, 1, false, 0, 1, n, st, scratch)))
+        return rc;
+      if ((rc = add_bn_layer(e, p.fus[i], fs + ".conv.weight", fs + ".bn", p.C[i] + 512, p.C[i], 9, false, 0, 1, n, st,
+                             scratch))) return rc;
+    }
+    for (int i = p.nlev - 1; i >= 0; --i) {
+      const std::string si = std::to_string(i);
+      if ((rc = add_bn_layer(e, p.fl[i], "conv_lateral." + si + ".0.weight", "conv_lateral." + si + ".1", p.C[i], 256, 9,
+                             false, 0, 1, B * p.H[i] * p.W[i], st, scratch))) return rc;
+      if (i > 0) {
+        const std::string su = std::to_string(i - 1);
+        if ((rc = add_bn_layer(e, p.fu[i - 1], "conv_up." + su + ".0.weight", "conv_up." + su + ".1", 256, 256, 1, true, 0,
+                               1, 4 * B * p.H[i] * p.W[i], st, scratch))) return rc;
+      }
+    }
+  }
+  size_t u_max = 0, part_max = 0;
+  int c_max = 0;
+  for (size_t k = 0; k < pt.layers.size(); ++k) {
+    dd_engine::ProdBn& b = pt.layers[k];
+    pt.index[b.eval] = static_cast<int>(k);
+    b.rec_off = pt.rec_floats;
+    pt.rec_floats += 2 * static_cast<size_t>(b.C);
+    u_max = std::max(u_max, static_cast<size_t>(b.n) * b.C);
+    part_max = std::max(part_max, static_cast<size_t>(pbn_blocks(b.n)) * 2 * b.C);
+    c_max = std::max(c_max, b.C);
+  }
+  if (pt.layers.empty()) return DD_OK;
+  if ((rc = dev_array(e, &pt.U, u_max))) return rc;
+  if ((rc = dev_array(e, &pt.part, part_max))) return rc;
+  if ((rc = dev_array(e, &pt.sum1, c_max))) return rc;
+  if ((rc = dev_array(e, &pt.s, c_max))) return rc;
+  if ((rc = dev_array(e, &pt.t, c_max))) return rc;
+  if ((rc = dev_array(e, &pt.rec, pt.rec_floats))) return rc;
+  CUDA_TRY(cudaMemsetAsync(pt.rec, 0, pt.rec_floats * 4, st));
+  return DD_OK;
+}
+
+// run_gen for a layer followed by a BatchNorm: in DD_PRODUCER_TRAIN the conv on the unfolded pack into pt.U, the
+// batch statistics and fold (record written), then act(s u + t) with the eval layer's addend and outputs; otherwise
+// the eval layer itself.
+int run_bn_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
+               float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0) {
+  dd_engine::ProdTrain& pt = e->pt;
+  const auto it = e->producer_mode == DD_PRODUCER_TRAIN ? pt.index.find(&L) : pt.index.end();
+  if (it == pt.index.end()) return run_gen(e, L, a0, c0, a1, c1, H, W, y32, add32, out, st, src_h, src_w);
+  const dd_engine::ProdBn& b = pt.layers[it->second];
+  const long long n = static_cast<long long>(e->cfg.batch) * H * W * (L.shuffle ? 4 : 1);
+  if (n != b.n) return fail(DD_ERR_INVALID, b.key + ": output grid differs from the packed geometry");
+  int rc;
+  if ((rc = launch_gen(e, b.raw, 0, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, pt.U, nullptr, nullptr, 0, 0,
+                       st, 0, nullptr, e->prod.KS)))
+    return rc;
+  const int C = b.C, nblk = pbn_blocks(n);
+  const dim3 grid(nblk, (C + dd::PBN_CH - 1) / dd::PBN_CH), block(dd::PBN_CH, 8);
+  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, nullptr, pt.part);
+  if ((rc = launched(e, "pbn_stats"))) return rc;
+  dd::pbn_colsum_kernel<<<(C + 255) / 256, 256, 0, st>>>(pt.part, nblk, C, pt.sum1);
+  if ((rc = launched(e, "pbn_colsum"))) return rc;
+  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, pt.sum1, pt.part);
+  if ((rc = launched(e, "pbn_stats"))) return rc;
+  dd::pbn_fold_kernel<<<(C + 255) / 256, 256, 0, st>>>(pt.sum1, pt.part, nblk, n, C, b.gamma, b.beta, pt.s, pt.t,
+                                                        pt.rec + b.rec_off);
+  if ((rc = launched(e, "pbn_fold"))) return rc;
+  dd::PbnApplyArgs a;
+  a.u = pt.U;
+  a.n = n;
+  a.C = C;
+  a.relu = L.relu;
+  a.add_first = L.add_first;
+  a.s = pt.s;
+  a.t = pt.t;
+  a.add32 = add32;
+  a.y32 = y32;
+  a.out_hi = out ? out->hi : nullptr;
+  a.out_lo = out ? out->lo : nullptr;
+  a.ld_out = C;
+  a.ch_off = 0;
+  a.split_scale = kProdScale;
+  a.status = e->status;
+  dd::pbn_apply_kernel<<<grid_of(static_cast<size_t>(n) * C / 8), 256, 0, st>>>(a);
+  return launched(e, "pbn_apply");
+}
+
+// A forward starts (dd_run_backbone, dd_build_condition with feature maps): no record is current.
+void producer_forward_start(dd_engine* e) {
+  for (auto& b : e->pt.layers) b.fresh = false;
+}
+// After a call of `stage` (0 backbone, 1 neck + FPN) in DD_PRODUCER_TRAIN: its layers' records are current.
+void producer_mark_fresh(dd_engine* e, int stage) {
+  for (auto& b : e->pt.layers)
+    if (b.stage == stage) b.fresh = true;
+}
+
 // ------------------------------------------------------------------------------------------------ ResNet backbone
 // ResNetForMMBEV with BasicBlocks and no stem (reference src/model/backbone/mmbev_resnet.py:124-160; block = mmdet
 // BasicBlock): per stage, block 0 = conv3x3(s2)+BN+ReLU -> conv3x3+BN, skip = biased conv3x3(s2) without BN; other
@@ -1842,7 +2027,7 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
       const int k = b & 1;
       const Planes& in = (b == 0) ? src : r.Yp[cur];
       const int in_c = (b == 0) ? src_c : C;
-      if ((rc = run_gen(e, Wt.c1, in, in_c, none, 0, H, W, nullptr, nullptr, &r.T, st, src_h, src_w))) return rc;
+      if ((rc = run_bn_gen(e, Wt.c1, in, in_c, none, 0, H, W, nullptr, nullptr, &r.T, st, src_h, src_w))) return rc;
       const float* skip;
       if (Wt.has_ds) {
         if ((rc = run_gen(e, Wt.ds, in, in_c, none, 0, H, W, r.D32, nullptr, nullptr, st, src_h, src_w))) return rc;
@@ -1851,7 +2036,7 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
         skip = r.Y32[cur];
       }
       const Planes& outp = last ? e->prod.F[s] : r.Yp[k];
-      if ((rc = run_gen(e, Wt.c2, r.T, C, none, 0, H, W, r.Y32[k], skip, &outp, st))) return rc;
+      if ((rc = run_bn_gen(e, Wt.c2, r.T, C, none, 0, H, W, r.Y32[k], skip, &outp, st))) return rc;
       cur = k;
     }
     if (feats_out && feats_out[s]) {
@@ -2563,6 +2748,9 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   h->mp.ready = false;
   if (h->mp.enabled)
     if ((rc = pack_mpvit(h, st, scratch))) return rc;
+  h->pt = dd_engine::ProdTrain();
+  if (h->cfg.flags & DD_FLAG_PRODUCER_TRAIN)
+    if ((rc = pack_prod_train(h, st, scratch))) return rc;
   // the registered pointers were borrowed for this call only (include/dd_engine.h): wait for the kernels that read them
   // and forget them, so a later finalize cannot read memory the caller has freed in the meantime
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -2952,6 +3140,46 @@ int dd_codec_batch_stats(dd_handle h, float* dev_out, int32_t capacity, int32_t*
   return DD_OK;
 }
 
+int dd_set_producer_mode(dd_handle h, int32_t mode) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  if (mode != DD_PRODUCER_EVAL && mode != DD_PRODUCER_TRAIN)
+    return fail(DD_ERR_INVALID, "producer mode must be DD_PRODUCER_EVAL or DD_PRODUCER_TRAIN");
+  if (mode == DD_PRODUCER_TRAIN && !(h->cfg.flags & DD_FLAG_PRODUCER_TRAIN))
+    return fail(DD_ERR_INVALID, "DD_PRODUCER_TRAIN needs an engine created with DD_FLAG_PRODUCER_TRAIN");
+  h->producer_mode = mode;
+  return DD_OK;
+}
+
+int dd_producer_batch_stats(dd_handle h, float* dev_out, int64_t capacity, int32_t* n_out, void* cuda_stream) {
+  if (!h || !n_out) return fail(DD_ERR_INVALID, "null argument");
+  const dd_engine::ProdTrain& pt = h->pt;
+  if (dev_out && !pt.layers.empty()) {
+    if (capacity < static_cast<int64_t>(pt.rec_floats))
+      return fail(DD_ERR_INVALID, "dev_out holds fewer floats than the records");
+    CUDA_TRY(cudaSetDevice(h->cfg.device));
+    CUDA_TRY(cudaMemcpyAsync(dev_out, pt.rec, pt.rec_floats * 4, cudaMemcpyDeviceToDevice,
+                             static_cast<cudaStream_t>(cuda_stream)));
+  }
+  *n_out = static_cast<int32_t>(pt.layers.size());
+  return DD_OK;
+}
+
+int dd_producer_bn_info(dd_handle h, int32_t i, char* key, int32_t key_capacity, int32_t* channels, int64_t* offset,
+                        int32_t* fresh) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  if (i < 0 || i >= static_cast<int32_t>(h->pt.layers.size())) return fail(DD_ERR_INVALID, "record index out of range");
+  const dd_engine::ProdBn& b = h->pt.layers[i];
+  if (key && key_capacity > 0) {
+    const size_t n = std::min(b.key.size(), static_cast<size_t>(key_capacity - 1));
+    memcpy(key, b.key.data(), n);
+    key[n] = 0;
+  }
+  if (channels) *channels = b.C;
+  if (offset) *offset = static_cast<int64_t>(b.rec_off);
+  if (fresh) *fresh = b.fresh ? 1 : 0;
+  return DD_OK;
+}
+
 int dd_enable_producers(dd_handle h, const dd_producer_config* pc) {
   if (!h || !pc) return fail(DD_ERR_INVALID, "null argument");
   if (pc->num_levels < 2 || pc->num_levels > 4) return fail(DD_ERR_INVALID, "producers need 2..4 pyramid levels");
@@ -2998,6 +3226,7 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
   if (feats) {
     CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
     h->launches = 0;
+    producer_forward_start(h);
   }  // else: dd_run_backbone already wrote the input planes F[i] (and owns the status / launch counters)
   h->feats_ready = false;
   for (int i = 0; feats && i < p.nlev; ++i) {
@@ -3015,22 +3244,22 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
       continue;
     }
     // HAHI neck, attention gates off (reference necks/hahi.py:173-176, 226-250, 253-272)
-    if ((rc = run_gen(h, p.lat[i], p.F[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.L[i], s))) return rc;
-    if ((rc = run_gen(h, p.proj[i], p.L[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.P[i], s))) return rc;
+    if ((rc = run_bn_gen(h, p.lat[i], p.F[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.L[i], s))) return rc;
+    if ((rc = run_bn_gen(h, p.proj[i], p.L[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.P[i], s))) return rc;
     if (i == 0) {  // cat([conv_proj(lat), lat])
-      if ((rc = run_gen(h, p.fus[i], p.P[i], 512, p.L[i], p.C[i], p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
+      if ((rc = run_bn_gen(h, p.fus[i], p.P[i], 512, p.L[i], p.C[i], p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
     } else {       // cat([lat, trans_proj(lat)])
-      if ((rc = run_gen(h, p.fus[i], p.L[i], p.C[i], p.P[i], 512, p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
+      if ((rc = run_bn_gen(h, p.fus[i], p.L[i], p.C[i], p.P[i], 512, p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
     }
   }
   // FPN top-down (reference head :112-122): x_i = relu(bn(conv3x3(O_i))) + relu(bn(convT2x2(x_{i+1})))
   for (int i = p.nlev - 1; i >= 0; --i) {
     const float* add = (i < p.nlev - 1) ? p.UP[i] : nullptr;
-    if ((rc = run_gen(h, p.fl[i], p.O[i], p.C[i], none, 0, p.H[i], p.W[i], p.X[i], add, i > 0 ? &p.XP[i] : nullptr, s)))
+    if ((rc = run_bn_gen(h, p.fl[i], p.O[i], p.C[i], none, 0, p.H[i], p.W[i], p.X[i], add, i > 0 ? &p.XP[i] : nullptr, s)))
       return rc;
     if (i > 0) {
       float* up_raw = p.resample ? p.UPR[i - 1] : p.UP[i - 1];
-      if ((rc = run_gen(h, p.fu[i - 1], p.XP[i], 256, none, 0, p.H[i], p.W[i], up_raw, nullptr, nullptr, s))) return rc;
+      if ((rc = run_bn_gen(h, p.fu[i - 1], p.XP[i], 256, none, 0, p.H[i], p.W[i], up_raw, nullptr, nullptr, s))) return rc;
       if (p.resample) {  // F.adaptive_avg_pool2d(conv_up(pre_x), output_size = lateral size)  (reference head :121)
         const size_t n = static_cast<size_t>(B) * p.H[i - 1] * p.W[i - 1] * 256;
         dd::adaptive_avg_pool_nhwc_kernel<<<grid_of(n), 256, 0, s>>>(up_raw, p.UP[i - 1], B, 2 * p.H[i], 2 * p.W[i],
@@ -3042,11 +3271,13 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
   return DD_OK;
   };
   // every pointer of the neck / FPN kernels lives in the workspace -> replayable as a graph
+  const bool train = h->producer_mode == DD_PRODUCER_TRAIN;
   if (h->cfg.flags & DD_FLAG_CUDA_GRAPH) {
-    if ((rc = graph_run(h, dd_engine::G_COND, st, build))) return rc;
+    if ((rc = graph_run(h, train ? dd_engine::G_COND_TRAIN : dd_engine::G_COND, st, build))) return rc;
   } else if ((rc = build(st))) {
     return rc;
   }
+  if (train) producer_mark_fresh(h, 1);
   h->cond_ready = true;
   if (cond_out) {
     if ((rc = transpose_out(h->cond, cond_out, B, 256, p.H[0] * p.W[0], st))) return rc;
@@ -3169,6 +3400,9 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
   if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
   CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
   h->launches = 0;
+  producer_forward_start(h);
+  // the ResNet's BatchNorms follow the producer mode; Swin has none, MPViT's are not covered (always eval)
+  const bool train = resnet && h->producer_mode == DD_PRODUCER_TRAIN;
   bool want_out = false;
   for (int i = 0; feats_out && i < 4; ++i) want_out |= (feats_out[i] != nullptr);
   if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !want_out) {
@@ -3176,10 +3410,13 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
     const size_t n = static_cast<size_t>(h->cfg.batch) * 3 *
                      (swin ? h->bb.H * h->bb.W : (resnet ? h->rn.H * h->rn.W : h->mp.H * h->mp.W));
     CUDA_TRY(cudaMemcpyAsync(h->rgb_stage, rgb, n * 4, cudaMemcpyDeviceToDevice, st));
-    if ((rc = graph_run(h, dd_engine::G_BACKBONE, st, [&](cudaStream_t s) { return run(h->rgb_stage, nullptr, s); }))) return rc;
+    if ((rc = graph_run(h, train ? dd_engine::G_BACKBONE_TRAIN : dd_engine::G_BACKBONE, st,
+                        [&](cudaStream_t s) { return run(h->rgb_stage, nullptr, s); })))
+      return rc;
   } else if ((rc = run(rgb, feats_out, st))) {
     return rc;
   }
+  if (train) producer_mark_fresh(h, 0);
   h->feats_ready = true;
   return DD_OK;
 }

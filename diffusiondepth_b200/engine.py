@@ -100,7 +100,7 @@ class DenoiseEngine:
                  simt_conv: bool = False, check_range: bool = False, halo_conv: bool = True,
                  swap_narrow: bool = True, pair_wide: bool = True, step_decode: bool = False, workspace_pool=None,
                  fp8_corr: bool = True, backward: bool = False, loop_backward: bool = False,
-                 chain_pred: bool = False):
+                 chain_pred: bool = False, producer_train: bool = False):
         self.lib = _cabi.load_library()
         device = torch.device(device)
         if device.type != "cuda":
@@ -114,7 +114,8 @@ class DenoiseEngine:
                 (_cabi.FLAG_SWAP_NARROW if swap_narrow else 0) | (_cabi.FLAG_PAIR_WIDE if pair_wide else 0) | \
                 (_cabi.FLAG_STEP_DECODE if step_decode else 0) | (_cabi.FLAG_FP8_CORR if fp8_corr else 0) | \
                 (_cabi.FLAG_BACKWARD if backward else 0) | (_cabi.FLAG_LOOP_BACKWARD if loop_backward else 0) | \
-                (_cabi.FLAG_CHAIN_PRED if chain_pred else 0)
+                (_cabi.FLAG_CHAIN_PRED if chain_pred else 0) | (_cabi.FLAG_PRODUCER_TRAIN if producer_train else 0)
+        self.producer_train = bool(producer_train)
         self.fp8_corr = bool(fp8_corr)
         self.backward = bool(backward or loop_backward)  # the loop backward includes the operator's
         self.loop_backward = bool(loop_backward)
@@ -448,6 +449,42 @@ class DenoiseEngine:
         _cabi.check(self.lib.dd_codec_batch_stats(self._h, C.c_void_p(out.data_ptr()), out.shape[0], C.byref(n),
                                                   C.c_void_p(self._stream())))
         return out[:n.value]
+
+    def set_producer_mode(self, training: bool):
+        """The condition producers' BatchNorms (ResNet backbone, HAHI neck, FPN) on batch statistics (`training`, as
+        torch's BatchNorm2d in training mode; engine created with producer_train=True) or on their running statistics
+        (the default) for every later run_backbone / build_condition.  The engine never updates running statistics;
+        `producer_batch_stats` returns what a caller needs to."""
+        _cabi.check(self.lib.dd_set_producer_mode(self._h, _cabi.PRODUCER_TRAIN if training else _cabi.PRODUCER_EVAL))
+
+    def _producer_records(self):
+        n = C.c_int32()
+        _cabi.check(self.lib.dd_producer_batch_stats(self._h, None, 0, C.byref(n), None))
+        buf, ch, off, fresh = C.create_string_buffer(256), C.c_int32(), C.c_int64(), C.c_int32()
+        info = []
+        for i in range(n.value):
+            _cabi.check(self.lib.dd_producer_bn_info(self._h, i, buf, 256, C.byref(ch), C.byref(off), C.byref(fresh)))
+            info.append((buf.value.decode(), ch.value, off.value, bool(fresh.value)))
+        return info
+
+    def producer_bn_keys(self):
+        """[(BatchNorm key prefix, channels, offset into the records)] of every BatchNorm'ed producer layer, in
+        evaluation order (empty without producer_train=True)."""
+        return [(k, c, o) for k, c, o, _ in self._producer_records()]
+
+    def producer_batch_stats(self) -> Dict[str, Tuple[torch.Tensor, torch.Tensor]]:
+        """{BatchNorm key prefix: (batch mean [C], unbiased batch variance [C])} of every producer BatchNorm the forward
+        that last started (run_backbone, or build_condition with feature maps) evaluated in training mode, in
+        evaluation order.  Ordered on the current stream; no synchronisation."""
+        info = self._producer_records()
+        total = max((o + 2 * c for _, c, o, _ in info), default=0)
+        if total == 0:
+            return {}
+        rec = torch.empty(total, device=self.device, dtype=torch.float32)
+        n = C.c_int32()
+        _cabi.check(self.lib.dd_producer_batch_stats(self._h, C.c_void_p(rec.data_ptr()), total, C.byref(n),
+                                                     C.c_void_p(self._stream())))
+        return {k: (rec[o:o + c], rec[o + c:o + 2 * c]) for k, c, o, f in info if f}
 
     def decode(self, latent: torch.Tensor, want_logits=False):
         B, (h, w) = self.batch, self.latent_hw

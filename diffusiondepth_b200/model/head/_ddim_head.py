@@ -60,15 +60,25 @@ def _signature(tensors):
     return tuple((t.data_ptr(), t._version) for t in tensors.values())
 
 
-def repack_plan(old_keys, old_sig, new_keys, new_sig, incremental=True):
+def repack_plan(old_keys, old_sig, new_keys, new_sig, incremental=True, deferred=None):
     """What an engine packed from tensors `old_keys` with signature `old_sig` (None: never packed) needs to serve the
     tensors `new_keys` / `new_sig`: the list of changed keys for `DenoiseEngine.update_weights` (empty: nothing), or
     None for a full `load_weights` — a different key set, a changed tensor the update does not re-pack (neck, FPN,
-    backbone), or `incremental` off."""
+    backbone), or `incremental` off.  `deferred` (a predicate on keys, optional): changes of those keys are left out
+    of the plan; the caller re-packs them later."""
     if not incremental or old_sig is None or tuple(old_keys) != tuple(new_keys):
         return None
-    changed = [k for k, a, b in zip(new_keys, old_sig, new_sig) if a != b]
+    changed = [k for k, a, b in zip(new_keys, old_sig, new_sig) if a != b and not (deferred and deferred(k))]
     return changed if all(is_updatable(k) for k in changed) else None
+
+
+_PRODUCER_PREFIXES = ("hahineck.", "conv_lateral.", "conv_up.", "backbone.")
+
+
+def is_producer_running_stat(key: str) -> bool:
+    """A running-statistic buffer of a producer BatchNorm: what the running update of a training-mode forward changes,
+    and what the training-mode producers do not read."""
+    return key.startswith(_PRODUCER_PREFIXES) and key.endswith((".running_mean", ".running_var", ".num_batches_tracked"))
 
 
 def _gn_conv_stack(cin, mid, cout):
@@ -204,6 +214,14 @@ class DDIMHeadBase(nn.Module):
     # buffers (re-packed by `update_weights` before the next call).  Off by default: the codec then runs on its running
     # statistics in every mode.
     codec_train_bn = False
+    # Training-mode BatchNorm in the condition producers (reference `net.train()`): when True, the HAHI neck and the FPN
+    # (when `hahineck` / `conv_lateral` are in training mode) and the native ResNet backbone (when it is in training
+    # mode) normalise with the statistics of the batch, and every forward applies torch's running-statistic update to
+    # their BatchNorm buffers.  Engines are created with DenoiseEngine(producer_train=True).  While they run in training
+    # mode those buffer updates do not re-pack; the first eval-mode forward on the engine re-packs once.  An MPViT
+    # backbone in training mode runs in torch (its BatchNorms are not covered).  Off by default: the producers then run
+    # on their running statistics in every mode.
+    producer_train_bn = False
 
     def __init__(self, in_channels=None, up_scale_factor=1, inference_steps=20, num_train_timesteps=1000,
                  return_indices=None, depth_transform_cfg=None, detach_fp=False, depth_embed_dim=16,
@@ -243,6 +261,7 @@ class DDIMHeadBase(nn.Module):
         self.__dict__['_packed'] = {}                          # key -> (tensor list, signature) of the packed weights
         self.__dict__['_pools'] = {}                           # device -> WorkspacePool
         self.__dict__['_lock'] = threading.RLock()             # nn.DataParallel replicas (threads) share the three dicts
+        self.__dict__['_stale'] = set()  # keys of engines whose eval producer pack predates a running-statistic update
 
     def invalidate_engines(self):
         """Close every engine (call after replacing Parameter OBJECTS; in-place updates, load_state_dict and .to() are
@@ -258,7 +277,7 @@ class DDIMHeadBase(nn.Module):
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
         for k, v in self.__dict__.items():
-            if k in ("_engines", "_packed", "_pools", "_backbone_ref", "_lock"):
+            if k in ("_engines", "_packed", "_pools", "_backbone_ref", "_lock", "_stale"):
                 continue
             new.__dict__[k] = copy.deepcopy(v, memo)
         new.__dict__['_backbone_ref'] = None
@@ -364,6 +383,8 @@ class DDIMHeadBase(nn.Module):
             return False
         name = type(backbone).__name__
         if name == "MPViT":
+            if self.producer_train_bn and backbone.training:
+                return False  # its BatchNorms in training mode: torch runs it, the neck and FPN stay native
             spec = self.mpvit_spec(backbone)
             if spec is None or self.variant != "swin" or list(self.fpn_in_channels) != list(backbone.out_channels):
                 return False
@@ -390,33 +411,36 @@ class DDIMHeadBase(nn.Module):
         return tensors
 
     def _engine(self, batch, latent_hw, cond_hw, device, feats=None, image_hw=None, backbone=None,
-                backward=False, loop_backward=False) -> DenoiseEngine:
+                backward=False, loop_backward=False, producer_train=False) -> DenoiseEngine:
         """feats: backbone feature maps, or a (channels, sizes) pyramid spec -> native neck/FPN;
         image_hw: additionally run the backbone natively (`backbone`: the module holding its parameters);
         backward: an engine that also serves `denoiser_backward`; loop_backward: one that also serves
-        `denoise_backward` / `decode_backward` (and `denoiser_backward`)."""
+        `denoise_backward` / `decode_backward` (and `denoiser_backward`); producer_train: this forward runs a producer
+        BatchNorm in training mode (the eval producer pack may then lag behind their running statistics)."""
         with self._lock:
             return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
-                                       loop_backward)
+                                       loop_backward, producer_train)
 
     def _grad_engine(self, batch, latent_hw, cond_hw, device) -> DenoiseEngine:
         """The engine `denoiser_backward` runs on: the loop-backward engine of this geometry when the head trains through
         the loop or that engine exists (its flag is a superset), else a backward-only one."""
         loop_key = (batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)), self.diffusion_inference_steps,
                     self.use_cuda_graph, False, None, bool(self.return_intermediates), bool(self.fp8_corrections),
-                    False, True)
+                    False, False, True)
         loop = self.grad_through_loop or loop_key in self._engines
         return self._engine(batch, latent_hw, cond_hw, device, backward=not loop, loop_backward=loop)
 
     def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
-                       loop_backward) -> DenoiseEngine:
+                       loop_backward, producer_train=False) -> DenoiseEngine:
         native = feats is not None
+        ptrain_flag = native and bool(self.producer_train_bn)
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
         key = (batch, tuple(latent_hw), tuple(cond_hw), str(device), self.diffusion_inference_steps,
                self.use_cuda_graph, native, tuple(image_hw) if image_hw is not None else None,
-               bool(self.return_intermediates), bool(self.fp8_corrections), bool(backward), bool(loop_backward))
+               bool(self.return_intermediates), bool(self.fp8_corrections), ptrain_flag, bool(backward),
+               bool(loop_backward))
         eng = self._engines.get(key)
         if eng is None:
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
@@ -424,7 +448,7 @@ class DDIMHeadBase(nn.Module):
                                 cuda_graph=self.use_cuda_graph, check_range=False,
                                 step_decode=bool(self.return_intermediates), workspace_pool=pool,
                                 fp8_corr=bool(self.fp8_corrections), backward=bool(backward),
-                                loop_backward=bool(loop_backward))
+                                loop_backward=bool(loop_backward), producer_train=ptrain_flag)
             if native:
                 eng.enable_producers(feats[0], feats[1], has_neck=self.has_neck)
             if image_hw is not None:
@@ -439,10 +463,12 @@ class DDIMHeadBase(nn.Module):
             eng.set_schedule(ts, cx, ce)
             self._engines[key] = eng
             self._packed.pop(key, None)
+            self._stale.discard(key)
             while len(self._engines) > MAX_ENGINES:  # a ragged last batch / a new image size must not pile up engines
                 old_key, old = self._engines.popitem(last=False)
                 old.close()
                 self._packed.pop(old_key, None)
+                self._stale.discard(old_key)
         else:
             self._engines.move_to_end(key)
         # Re-pack when a parameter changed.  The ~500 tensors are walked once per pack; per forward only their
@@ -456,14 +482,24 @@ class DDIMHeadBase(nn.Module):
         else:
             tensors = packed[0]
             sig = _signature(tensors)
-        if packed is None or sig != packed[1]:
+        # In a training-mode producer forward, changes confined to producer running statistics (the previous forward's
+        # running update) are deferred: the batch-statistics path does not read them.  The eval pack is then stale and
+        # the next eval-mode forward re-packs it in full.
+        stale = key in self._stale and not producer_train
+        if packed is None or sig != packed[1] or stale:
             changed = None
             if packed is not None:  # something changed: the owning modules may hold new tensors
                 tensors = self._gather(native, image_hw, backbone)
-                changed = repack_plan(packed[0].keys(), packed[1], tensors.keys(), _signature(tensors),
-                                      self.incremental_repack)
+                new_sig = _signature(tensors)
+                defer = is_producer_running_stat if producer_train else None
+                changed = None if stale else repack_plan(packed[0].keys(), packed[1], tensors.keys(), new_sig,
+                                                         self.incremental_repack, defer)
+                if changed is not None and defer is not None and any(
+                        a != b and defer(k) for k, a, b in zip(tensors.keys(), packed[1], new_sig)):
+                    self._stale.add(key)
             if changed is None:
                 eng.load_weights(tensors)
+                self._stale.discard(key)
             elif changed:
                 eng.update_weights({k: tensors[k] for k in changed})
             self._packed[key] = (tensors, _signature(tensors), backbone if image_hw is not None else None)
@@ -532,6 +568,36 @@ class DDIMHeadBase(nn.Module):
         return [(bn, rec[i if order is None else order[i], 0], rec[i if order is None else order[i], 1])
                 for i, bn in enumerate(bns)]
 
+    # ------------------------------------------------------------------------------------------ producer BatchNorms
+    def _producer_training(self, backbone=None):
+        """(neck + FPN, native backbone) run their BatchNorms on batch statistics in this forward: `producer_train_bn`
+        and the modules in training mode.  `backbone`: the natively run backbone module (None: torch runs it); only the
+        ResNet's BatchNorms are on the engine.  The engine's BatchNorms use eps = 1e-5 and track running statistics."""
+        if not self.producer_train_bn:
+            return False, False
+        cond_mods = [self._modules[n] for n in ("hahineck", "conv_lateral") if n in self._modules]
+        cond = any(m.training for m in cond_mods)
+        bb = backbone is not None and type(backbone).__name__ == "ResNetForMMBEV" and backbone.training
+        mods = ([self._modules[n] for n in ("hahineck", "conv_lateral", "conv_up") if n in self._modules] if cond else []) \
+            + ([backbone] if bb else [])
+        for m in mods:
+            for bn in m.modules():
+                if isinstance(bn, nn.modules.batchnorm._BatchNorm):
+                    if bn.eps != 1e-5 or not bn.track_running_stats:
+                        raise EngineError("producer_train_bn: the engine's producer BatchNorms use eps = 1e-5 and "
+                                          f"running statistics, got eps = {bn.eps}, track_running_stats = "
+                                          f"{bn.track_running_stats}")
+        return cond, bb
+
+    def _producer_records(self, eng, backbone=None):
+        """[(BatchNorm, batch mean, unbiased batch variance)] of the producer BatchNorms `eng`'s last forward ran in
+        training mode (keys `backbone.*` name modules of `backbone`)."""
+        out = []
+        for key, (mean, var) in eng.producer_batch_stats().items():
+            bn = backbone.get_submodule(key[len("backbone."):]) if key.startswith("backbone.") else self.get_submodule(key)
+            out.append((bn, mean, var))
+        return out
+
     # ------------------------------------------------------------------------------------------ condition path
     def _condition(self, fp):
         """Top-down FPN that builds the 256-channel condition map x (head :112-122 / res.py:108-118)."""
@@ -591,21 +657,32 @@ class DDIMHeadBase(nn.Module):
             raise EngineError("grad_through_loop is not supported by the *Vis heads (pred_inter has no backward)")
         codec_train = self._codec_training()
         enc_bn1, enc_bn2, dec_bn = self._codec_bns() if codec_train else (None,) * 3
-        codec_updates = []  # applied at the end: the buffers keep the signature the engines were packed with until then
+        bn_updates = []  # applied at the end: the buffers keep the signature the engines were packed with until then
         if native:  # (backbone +) neck + FPN + loop + decoder inside the engine; the condition map never leaves NHWC
             want_cond = self.capture_cond or self.training or self.eval_ddim_loss or self.grad_through_loop
+            bb_mod = self._backbone(backbone) if with_backbone else None
+            ptrain_cond, ptrain_bb = self._producer_training(bb_mod)
+            ptrain = ptrain_cond or ptrain_bb
             if with_backbone:
                 eng = self._engine(B, latent_hw, sizes[0], dev, feats=(list(self.fpn_in_channels), sizes),
-                                   image_hw=tuple(image.shape[-2:]), backbone=backbone)
+                                   image_hw=tuple(image.shape[-2:]), backbone=backbone, producer_train=ptrain)
+                if eng.producer_train:
+                    eng.set_producer_mode(ptrain_bb)
                 eng.run_backbone(image.contiguous().float())
+                if eng.producer_train:
+                    eng.set_producer_mode(ptrain_cond)
                 cond = eng.build_condition(None, want_cond=want_cond)
             else:
-                eng = self._engine(B, latent_hw, tuple(fp[0].shape[-2:]), dev, feats=fp)
+                eng = self._engine(B, latent_hw, tuple(fp[0].shape[-2:]), dev, feats=fp, producer_train=ptrain)
+                if eng.producer_train:
+                    eng.set_producer_mode(ptrain_cond)
                 cond = eng.build_condition(fp, want_cond=want_cond)
+            if ptrain:
+                bn_updates += self._producer_records(eng, bb_mod)
             eng.set_codec_mode(codec_train)
             gt_map_t = eng.encode(gt_depth_map.contiguous().float())  # returned as pred_init / gt_map_t only
             if codec_train:
-                codec_updates += self._codec_records(eng, (enc_bn1, enc_bn2))
+                bn_updates += self._codec_records(eng, (enc_bn1, enc_bn2))
             loop_cond = None
         else:
             eng = self._engine(B, latent_hw, tuple(cond.shape[-2:]), dev)
@@ -634,15 +711,15 @@ class DDIMHeadBase(nn.Module):
         if codec_train:
             if self.return_intermediates:  # the reference's order: inv_t of the final map, then of steps 1 .. T
                 T = self.diffusion_inference_steps
-                codec_updates += self._codec_records(eng, (dec_bn,) * (T + 1), order=[T - 1] + list(range(T)))
+                bn_updates += self._codec_records(eng, (dec_bn,) * (T + 1), order=[T - 1] + list(range(T)))
             else:
-                codec_updates += self._codec_records(eng, (dec_bn,))
+                bn_updates += self._codec_records(eng, (dec_bn,))
         self.last_latent, self.last_logits, self.last_cond = refined_depth_t, logits, cond
         if self.check_range:
             eng.poll_status()  # syncs; raises if an activation left the fp16 split range (DESIGN.md "Numerics")
         ddim_loss = self._ddim_loss(cond, refined_depth_t) if (self.eval_ddim_loss or self.training) \
             else refined_depth.new_zeros(())
-        for bn, mean, var in codec_updates:
+        for bn, mean, var in bn_updates:
             bn_running_update(bn, mean, var)
         return {'pred': refined_depth, 'pred_init': gt_map_t, 'blur_depth_t': gt_map_t, 'ddim_loss': ddim_loss,
                 'gt_map_t': gt_map_t, 'pred_uncertainty': None, 'pred_inter': inter, 'weight_map': None,

@@ -90,8 +90,13 @@ enum dd_flags {
                                    BatchNorm scale, and the workspace adds the loop backward's region (the T + 1 latents
                                    [T+1][B,P,16] fp32, fp64 gradient accumulators, the running latent gradient, the
                                    decoder backward's scratch) */
-  DD_FLAG_CHAIN_PRED = 1 << 10  /* Swin: run convB and pred.0 as two 3x3 convs instead of one composed 5x5 conv + its
+  DD_FLAG_CHAIN_PRED = 1 << 10, /* Swin: run convB and pred.0 as two 3x3 convs instead of one composed 5x5 conv + its
                                    border correction (A/B runs and tests; DD_FLAG_SIMT_CONV always runs the chain) */
+  DD_FLAG_PRODUCER_TRAIN = 1 << 11 /* enable dd_set_producer_mode(DD_PRODUCER_TRAIN): dd_finalize_weights also packs every
+                                   BatchNorm'ed producer layer (ResNet bn1 / bn2, HAHI neck, FPN) unfolded — its conv
+                                   alone, with gamma / beta kept on the device — and allocates engine-owned scratch for
+                                   the largest pre-BN output.  The eval pack, graphs and dd_workspace_bytes are those of
+                                   an engine without the flag. */
 };
 
 typedef struct dd_config {
@@ -327,6 +332,34 @@ int dd_set_codec_mode(dd_handle h, int32_t mode);
  * *n_out = n (0 after a forward in DD_CODEC_EVAL).  Enqueued on cuda_stream, no synchronisation; DD_ERR_INVALID when
  * capacity < n. */
 int dd_codec_batch_stats(dd_handle h, float* dev_out, int32_t capacity, int32_t* n_out, void* cuda_stream);
+
+/* How the condition producers' BatchNorms normalise: the ResNet backbone's BasicBlock bn1 / bn2 (reference
+ * mmbev_resnet.py:150-160), the HAHI neck's ConvModules (necks/hahi.py:54-97) and the FPN's conv_lateral.i.1 /
+ * conv_up.i.1 (head :112-122).  DD_PRODUCER_EVAL (the default): running statistics, folded into the weights at
+ * dd_finalize_weights.  DD_PRODUCER_TRAIN (needs DD_FLAG_PRODUCER_TRAIN, else DD_ERR_INVALID): as BatchNorm2d in
+ * training mode, the statistics of the batch each call sees (biased variance, eps 1e-5).  dd_run_backbone (ResNet) and
+ * dd_build_condition then run each such layer as the conv on its unfolded pack into engine-owned fp32 scratch (a ConvT
+ * pixel-shuffled: its statistics cover all B x 2H x 2W pixels before the FPN's adaptive_avg_pool2d), two statistics
+ * passes, a fold s = gamma / sqrt(var + 1e-5), t = beta - s mean, and act(s u + t) with the eval layer's addend and
+ * outputs; no host synchronisation, CUDA graphs of their own (the eval graphs are kept).  The Swin and MPViT backbones
+ * are not affected.  The engine never writes running statistics: the caller applies the running update from the
+ * records (dd_producer_batch_stats) and re-packs the eval weights with dd_finalize_weights when it next runs in
+ * DD_PRODUCER_EVAL.  The mode is engine state, read by each call. */
+enum dd_producer_mode { DD_PRODUCER_EVAL = 0, DD_PRODUCER_TRAIN = 1 };
+int dd_set_producer_mode(dd_handle h, int32_t mode);
+
+/* Records of the producers' BatchNorms: one per BatchNorm'ed layer, in evaluation order, [2][C] fp32 (batch mean,
+ * unbiased batch variance) at a fixed offset (dd_producer_bn_info).  Copies all of them back to back into dev_out
+ * (capacity in floats; dev_out may be NULL to query *n_out, the number of records); enqueued on cuda_stream, no
+ * synchronisation.  A record is current when the forward that last started (dd_run_backbone, or dd_build_condition
+ * with feature maps) evaluated its layer in DD_PRODUCER_TRAIN (dd_producer_bn_info's *fresh). */
+int dd_producer_batch_stats(dd_handle h, float* dev_out, int64_t capacity, int32_t* n_out, void* cuda_stream);
+
+/* Record i: the registered key prefix of its BatchNorm (e.g. `hahineck.trans_fusion.1.bn`, `conv_up.0.1`,
+ * `backbone.layers.2.0.bn1`; NUL-terminated, truncated to key_capacity), its channels, its offset in floats into
+ * dd_producer_batch_stats' output, and whether it is current.  DD_ERR_INVALID for i out of range. */
+int dd_producer_bn_info(dd_handle h, int32_t i, char* key, int32_t key_capacity, int32_t* channels, int64_t* offset,
+                        int32_t* fresh);
 
 /* Synchronise `cuda_stream` and report DD_ERR_RANGE if any activation left the fp16 split's range since the
  * last hot-path call started (DD_OK otherwise).  The hot-path calls themselves never synchronise unless
