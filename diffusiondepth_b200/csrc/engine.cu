@@ -1156,6 +1156,52 @@ int bind_workspace(dd_engine* e, void* ws, size_t bytes) {
   return DD_OK;
 }
 
+// The first step of every entry that runs on the engine's workspace: its device, then the workspace bound.
+int enter_workspace(dd_engine* h, void* ws, size_t bytes) {
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  return bind_workspace(h, ws, bytes);
+}
+
+// A forward starts: the status word its kernels flag range faults in and the launch count start from zero.
+int start_forward(dd_engine* h, cudaStream_t st) {
+  h->launches = 0;
+  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+  return DD_OK;
+}
+
+// Synchronise st and report a flagged range fault in the engine's status word.
+int poll_status(dd_engine* h, cudaStream_t st) {
+  CUDA_TRY(cudaMemcpyAsync(h->status_host, h->status, 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (*h->status_host & 1)
+    return fail(DD_ERR_RANGE, "an activation exceeded the operand split's range (16 |v| > 6e4; with fp8 corrections, "
+                              "DD_FLAG_FP8_CORR, 16 |v| > 1792: create the engine without that flag / set "
+                              "head.fp8_corrections = False)");
+  return DD_OK;
+}
+
+// A forward ends: with DD_FLAG_CHECK_RANGE it waits for st and reports a range fault.
+int finish_forward(dd_engine* h, cudaStream_t st) {
+  return (h->cfg.flags & DD_FLAG_CHECK_RANGE) ? poll_status(h, st) : DD_OK;
+}
+
+// After dd_enable_producers / dd_enable_backbone: the pack and the workspace layout no longer fit the engine, so the
+// weights must be finalized again, the next entry re-carves its workspace, and every graph is captured again.
+void invalidate_pack(dd_engine* h) {
+  h->weights_ready = h->packed = false;
+  h->ws = nullptr;
+  drop_graphs(h);
+}
+
+// Copy a standalone call's status word back, synchronise st and report a flag as DD_ERR_RANGE in `what`.
+int check_status_word(const int* status, cudaStream_t st, const char* what) {
+  int flag = 0;
+  CUDA_TRY(cudaMemcpyAsync(&flag, status, 4, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (flag) return fail(DD_ERR_RANGE, std::string("non-finite or out-of-range value in ") + what);
+  return DD_OK;
+}
+
 const Raw* find(dd_engine* e, const std::string& k) {
   auto it = e->raw.find(k);
   return it == e->raw.end() ? nullptr : &it->second;
@@ -2530,23 +2576,23 @@ constexpr size_t kDecGradNumel[6] = {16 * 16 * 4 * 4, 16, 16, 16, 16 * 9, 1};
 
 // Checks of an entry that recomputes one denoiser call on the backward's region (dd_denoiser_backward,
 // dd_denoiser_relu_inputs), after its own null-pointer checks.
-int check_operator_bwd_call(const dd_engine* h, const char* entry, const int64_t* t_host) {
+int check_operator_bwd_call(const dd_engine* h, const char* entry) {
   if (!has_backward(h->cfg))
     return fail(DD_ERR_INVALID, std::string(entry) + " needs an engine created with DD_FLAG_BACKWARD (or DD_FLAG_LOOP_BACKWARD)");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   const Geom g = geom_of(h->cfg);
-  for (int b = 0; b < g.B; ++b)
-    if (t_host[b] < 0 || t_host[b] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
   if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
     return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");
   return DD_OK;
 }
 
-// One denoiser call's inputs as run_recompute reads them: image b's time-embedding row t_host[b] (checked) in
-// temb_sel, cond and noisy as NHWC, the latent's fp16 split planes.
+// One denoiser call's inputs as run_step / run_recompute read them: image b's time-embedding row t_host[b] in
+// temb_sel (every row checked first), cond and noisy as NHWC, the latent's fp16 split planes.
 int stage_operator_inputs(dd_engine* h, const float* cond, const float* noisy, const int64_t* t_host, cudaStream_t st) {
   const Geom g = geom_of(h->cfg);
   int rc;
+  for (int b = 0; b < g.B; ++b)
+    if (t_host[b] < 0 || t_host[b] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
   for (int b = 0; b < g.B; ++b)
     CUDA_TRY(cudaMemcpyAsync(h->temb_sel + b * 256, h->temb + t_host[b] * 256, 1024, cudaMemcpyDeviceToDevice, st));
   if ((rc = transpose_in(cond, h->cond, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
@@ -2560,23 +2606,27 @@ int time_per_call(cudaStream_t st, int warmup, int iters, float* ms_out, F&& bod
   int rc;
   for (int i = 0; i < warmup; ++i)
     if ((rc = body())) return rc;
-  cudaEvent_t e0, e1;
-  CUDA_TRY(cudaEventCreate(&e0));
-  CUDA_TRY(cudaEventCreate(&e1));
-  CUDA_TRY(cudaEventRecord(e0, st));
+  struct Events {  // destroyed on every return
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~Events() {
+      if (e0) cudaEventDestroy(e0);
+      if (e1) cudaEventDestroy(e1);
+    }
+  } ev;
+  CUDA_TRY(cudaEventCreate(&ev.e0));
+  CUDA_TRY(cudaEventCreate(&ev.e1));
+  CUDA_TRY(cudaEventRecord(ev.e0, st));
   for (int i = 0; i < iters; ++i)
     if ((rc = body())) return rc;
-  CUDA_TRY(cudaEventRecord(e1, st));
-  CUDA_TRY(cudaEventSynchronize(e1));
+  CUDA_TRY(cudaEventRecord(ev.e1, st));
+  CUDA_TRY(cudaEventSynchronize(ev.e1));
   float ms = 0.f;
-  CUDA_TRY(cudaEventElapsedTime(&ms, e0, e1));
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
+  CUDA_TRY(cudaEventElapsedTime(&ms, ev.e0, ev.e1));
   *ms_out = ms / iters;
   return DD_OK;
 }
 
-// The buffers of one standalone layer call (dd_gen_layer, dd_window_attention), freed when it returns, and the engine's
+// The buffers of one standalone call (the layer entries, dd_bench_gemm), freed when it returns, and the engine's
 // status word pointed at the call's own word meanwhile (the launch helpers report to e->status, a workspace word).
 struct StandaloneCall {
   dd_engine* e;
@@ -2597,15 +2647,65 @@ struct StandaloneCall {
   }
   template <typename T>
   int alloc(T** p, size_t n) { return dev_alloc(owned, reinterpret_cast<void**>(p), n * sizeof(T)); }
-  // synchronise st and report the status word
-  int finish(cudaStream_t st, const char* what) {
-    int flag = 0;
-    CUDA_TRY(cudaMemcpyAsync(&flag, status, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (flag) return fail(DD_ERR_RANGE, std::string("non-finite or out-of-range value in ") + what);
-    return DD_OK;
-  }
+  int finish(cudaStream_t st, const char* what) { return check_status_word(status, st, what); }
 };
+
+// Frees what dd_create and dd_finalize_weights allocated; also takes an engine whose dd_create failed part-way.
+void release(dd_engine* e) {
+  cudaSetDevice(e->cfg.device);
+  drop_graphs(e);
+  for (void* p : e->owned) cudaFree(p);
+  if (e->status_host) cudaFreeHost(e->status_host);
+  if (e->stage) cudaFreeHost(e->stage);
+  if (e->pack_done) cudaEventDestroy(e->pack_done);
+  if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
+  delete e;
+}
+
+// The standalone conv's workspace: the status word (+ scratch), x as NHWC fp32 and its split planes, y as NHWC fp32,
+// the packed weights.  With base == nullptr only the size is computed, as carve() does.
+struct Conv3x3Ws {
+  int* status;
+  float *xn, *yn, *wsimt;
+  Planes x, w;
+};
+size_t conv3x3_layout(void* base, int batch, int cin, int cout, int height, int width, Conv3x3Ws& v) {
+  const size_t BP = static_cast<size_t>(batch) * height * width;
+  const size_t nw = static_cast<size_t>(cin) * cout * 9;
+  Carver c{reinterpret_cast<uint8_t*>(base)};
+  v.status = c.take<int>(16);
+  v.xn = c.take<float>(BP * cin);
+  v.x.hi = c.take<__half>(BP * cin);
+  v.x.lo = c.take<__half>(BP * cin);
+  v.yn = c.take<float>(BP * cout);
+  v.w.hi = c.take<__half>(nw);
+  v.w.lo = c.take<__half>(nw);
+  v.wsimt = c.take<float>(nw);
+  return align_up(c.off, 1024);
+}
+
+// The standalone weight gradient's workspace: the status word (+ scratch), x and dy as NHWC fp32 and their split
+// planes, the fp64 weight-gradient partials, the bias-gradient partials.  base == nullptr: the size only.
+struct WgradWs {
+  int* status;
+  float *xn, *dyn, *col_part;
+  Planes x, dy;
+  double* partial;
+};
+size_t wgrad_layout(void* base, int batch, int cin, int cout, int height, int width, WgradWs& v) {
+  const size_t BP = static_cast<size_t>(batch) * height * width;
+  Carver c{reinterpret_cast<uint8_t*>(base)};
+  v.status = c.take<int>(16);
+  v.xn = c.take<float>(BP * cin);
+  v.x.hi = c.take<__half>(BP * cin);
+  v.x.lo = c.take<__half>(BP * cin);
+  v.dyn = c.take<float>(BP * cout);
+  v.dy.hi = c.take<__half>(BP * cout);
+  v.dy.lo = c.take<__half>(BP * cout);
+  v.partial = c.take<double>(wgrad_partial_elems(cout, cin, batch, height, width));
+  v.col_part = c.take<float>(static_cast<size_t>(batch) * bwd_chunks(height * width) * cout);
+  return align_up(c.off, 1024);
+}
 
 }  // namespace
 
@@ -2647,11 +2747,7 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
       cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking) != cudaSuccess ||
       configure_all_kernels() != cudaSuccess) {
     std::string msg = std::string("engine setup failed: ") + cudaGetErrorString(cudaGetLastError());
-    if (e->status_host) cudaFreeHost(e->status_host);
-    if (e->stage) cudaFreeHost(e->stage);
-    if (e->pack_done) cudaEventDestroy(e->pack_done);
-    if (e->cap_stream) cudaStreamDestroy(e->cap_stream);
-    delete e;
+    release(e);
     return fail(DD_ERR_CUDA, msg);
   }
   *out = e;
@@ -2659,15 +2755,7 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
 }
 
 int dd_destroy(dd_handle h) {
-  if (!h) return DD_OK;
-  cudaSetDevice(h->cfg.device);
-  drop_graphs(h);
-  for (void* p : h->owned) cudaFree(p);
-  if (h->status_host) cudaFreeHost(h->status_host);
-  if (h->stage) cudaFreeHost(h->stage);
-  if (h->pack_done) cudaEventDestroy(h->pack_done);
-  if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
-  delete h;
+  if (h) release(h);
   return DD_OK;
 }
 
@@ -2793,16 +2881,6 @@ int dd_set_schedule(dd_handle h, const int64_t* timesteps, const double* c_x, co
 
 size_t dd_workspace_bytes(dd_handle h) { return h ? carve(h, nullptr) : 0; }
 
-static int poll_status(dd_handle h, cudaStream_t st) {
-  CUDA_TRY(cudaMemcpyAsync(h->status_host, h->status, 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  if (*h->status_host & 1)
-    return fail(DD_ERR_RANGE, "an activation exceeded the operand split's range (16 |v| > 6e4; with fp8 corrections, "
-                              "DD_FLAG_FP8_CORR, 16 |v| > 1792: create the engine without that flag / set "
-                              "head.fp8_corrections = False)");
-  return DD_OK;
-}
-
 // dd_denoise_decode and dd_denoise_decode_steps: the T-step loop (+ a decode after every step when depth_steps_out
 // is given: the *Vis heads' `pred_inter`, reference ..._swin_addHAHI_vis.py:130-149,289-304), then the final decode.
 static int denoise_impl(dd_handle h, const float* cond, const float* noise, float* latent_out, float* logit_out,
@@ -2815,13 +2893,11 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
   if (depth_steps_out && !(h->cfg.flags & DD_FLAG_STEP_DECODE))
     return fail(DD_ERR_INVALID, "dd_denoise_decode_steps needs an engine created with DD_FLAG_STEP_DECODE");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   const Geom g = geom_of(h->cfg);
   if (cond) {
-    h->launches = 0;
-    CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+    if ((rc = start_forward(h, st))) return rc;
     if ((rc = transpose_in(cond, h->cond, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
     h->launches += 1;
   }  // else: dd_build_condition left the NHWC condition map (and the launch / status counters) in place
@@ -2868,8 +2944,7 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
     if ((rc = transpose_out(h->x32, latent_out, g.B, 16, g.P, st))) return rc;
     h->launches++;
   }
-  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
-  return DD_OK;
+  return finish_forward(h, st);
 }
 
 int dd_denoise_decode(dd_handle h, const float* cond, const float* noise, float* latent_out, float* logit_out,
@@ -2889,25 +2964,16 @@ int dd_denoiser_forward(dd_handle h, const float* cond, const float* noisy, cons
   if (!h || !cond || !noisy || !t_host || !eps_out) return fail(DD_ERR_INVALID, "null argument");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = start_forward(h, st))) return rc;
+  if ((rc = stage_operator_inputs(h, cond, noisy, t_host, st))) return rc;
   const Geom g = geom_of(h->cfg);
-  h->launches = 0;
-  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
-  for (int b = 0; b < g.B; ++b) {
-    if (t_host[b] < 0 || t_host[b] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
-    CUDA_TRY(cudaMemcpyAsync(h->temb_sel + b * 256, h->temb + t_host[b] * 256, 1024, cudaMemcpyDeviceToDevice, st));
-  }
-  if ((rc = transpose_in(cond, h->cond, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
-  if ((rc = transpose_in(noisy, h->x32, g.B, 16, g.P, st))) return rc;
-  if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, static_cast<size_t>(g.B) * g.P * 16, kXScale, st))) return rc;
   // eps (NHWC) lands in the tail of Y's storage: Y holds y6 in its first B*P*16 floats at that point
   float* eps_nhwc = h->Y + static_cast<size_t>(g.B) * g.P * 16;
   if ((rc = run_step(h, h->temb_sel, 256, 0.f, 0.f, eps_nhwc, st))) return rc;
   if ((rc = transpose_out(eps_nhwc, eps_out, g.B, 16, g.P, st))) return rc;
-  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
-  return DD_OK;
+  return finish_forward(h, st);
 }
 
 int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host, const float* d_eps,
@@ -2915,11 +2981,10 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
                          size_t workspace_bytes, void* cuda_stream) {
   if (!h || !cond || !noisy || !t_host || !d_eps) return fail(DD_ERR_INVALID, "null argument");
   int rc;
-  if ((rc = check_operator_bwd_call(h, "dd_denoiser_backward", t_host))) return rc;
+  if ((rc = check_operator_bwd_call(h, "dd_denoiser_backward"))) return rc;
   const Geom g = geom_of(h->cfg);
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
   const int npar = swin ? 21 : 17;
   float* P[21] = {};
@@ -2928,8 +2993,7 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
   dd_engine::Bwd& bw = h->bw;
   const size_t BP = static_cast<size_t>(g.B) * g.P;
   const int PC = h->cfg.cond_h * h->cfg.cond_w;
-  h->launches = 0;
-  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+  if ((rc = start_forward(h, st))) return rc;
   if ((rc = stage_operator_inputs(h, cond, noisy, t_host, st))) return rc;
   if ((rc = transpose_in(d_eps, bw.g[0], g.B, 16, g.P, st))) return rc;
   auto sink = [&](const float* dc, const float* scale) -> int {
@@ -2955,29 +3019,25 @@ int dd_denoiser_backward(dd_handle h, const float* cond, const float* noisy, con
     dd::unscale_kernel<<<grid_of(BP * 16), 256, 0, st>>>(d_noisy_out, BP * 16, bw.scales + 5);
     if ((rc = launched(h, "unscale"))) return rc;
   }
-  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
-  return DD_OK;
+  return finish_forward(h, st);
 }
 
 int dd_denoiser_relu_inputs(dd_handle h, const float* cond, const float* noisy, const int64_t* t_host,
                             float* const* z_out, void* workspace, size_t workspace_bytes, void* cuda_stream) {
   if (!h || !cond || !noisy || !t_host || !z_out) return fail(DD_ERR_INVALID, "null argument");
   int rc;
-  if ((rc = check_operator_bwd_call(h, "dd_denoiser_relu_inputs", t_host))) return rc;
+  if ((rc = check_operator_bwd_call(h, "dd_denoiser_relu_inputs"))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   const dd_engine::Bwd& bw = h->bw;
-  h->launches = 0;
-  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+  if ((rc = start_forward(h, st))) return rc;
   if ((rc = stage_operator_inputs(h, cond, noisy, t_host, st))) return rc;
   if ((rc = run_recompute(h, h->temb_sel, 256, st))) return rc;
   if (z_out[0] && (rc = run_gn_pre_relu<64>(h, 0, bw.y1, z_out[0], st))) return rc;
   if (z_out[1] && (rc = run_gn_pre_relu<256>(h, 1, bw.y2, z_out[1], st))) return rc;
   if (z_out[2] && (rc = run_gn_pre_relu<64>(h, 2, bw.y5, z_out[2], st))) return rc;
   if (z_out[3] && (rc = run_gn_pre_relu<16>(h, 3, bw.y6, z_out[3], st))) return rc;
-  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
-  return DD_OK;
+  return finish_forward(h, st);
 }
 
 int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, const float* d_depth, const float* d_latent,
@@ -2995,16 +3055,14 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
   if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
     return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   dd_engine::LoopBwd& l = h->lp;
   const size_t BP = static_cast<size_t>(g.B) * g.P, nx = BP * 16;
   const size_t ncond = static_cast<size_t>(g.B) * h->cfg.cond_h * h->cfg.cond_w * 256;
   const int npar = param_count(h->cfg);
   if (cond) {
-    h->launches = 0;
-    CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
+    if ((rc = start_forward(h, st))) return rc;
     if ((rc = transpose_in(cond, h->cond, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
   }  // else: dd_build_condition left the NHWC condition map in place
   h->cond_ready = false;
@@ -3082,8 +3140,7 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
     if ((rc = launched(h, "acc_store"))) return rc;
     if ((rc = transpose_out(dc32, d_cond_out, g.B, 256, h->cfg.cond_h * h->cfg.cond_w, st))) return rc;
   }
-  if (h->cfg.flags & DD_FLAG_CHECK_RANGE) return poll_status(h, st);
-  return DD_OK;
+  return finish_forward(h, st);
 }
 
 int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, float* d_latent_out,
@@ -3093,9 +3150,8 @@ int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, f
     return fail(DD_ERR_INVALID, "dd_decode_backward needs an engine created with DD_FLAG_LOOP_BACKWARD");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   const Geom g = geom_of(h->cfg);
   if ((rc = transpose_in(latent, h->x32, g.B, 16, g.P, st))) return rc;
   if ((rc = run_decode_bwd(h, d_depth, d_latent_out ? h->bw.g[1] : nullptr, d_dec_params, st))) return rc;
@@ -3108,9 +3164,8 @@ int dd_decode(dd_handle h, const float* latent, float* logit_out, float* depth_o
   if (!h || !latent || !depth_out) return fail(DD_ERR_INVALID, "null argument");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   const Geom g = geom_of(h->cfg);
   if ((rc = transpose_in(latent, h->x32, g.B, 16, g.P, st))) return rc;
   const bool train = h->codec_mode == DD_CODEC_TRAIN;
@@ -3204,10 +3259,7 @@ int dd_enable_producers(dd_handle h, const dd_producer_config* pc) {
   if (p.H[0] != h->cfg.cond_h || p.W[0] != h->cfg.cond_w)
     return fail(DD_ERR_INVALID, "level-0 feature size must equal the condition map size");
   h->prod = p;
-  h->weights_ready = false;  // producer weights are packed by dd_finalize_weights
-  h->packed = false;
-  h->ws = nullptr;           // workspace layout changed
-  drop_graphs(h);
+  invalidate_pack(h);
   return DD_OK;
 }
 
@@ -3218,14 +3270,12 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
   if (!h->prod.enabled || !h->weights_ready || !h->prod.ready)
     return fail(DD_ERR_INVALID, "producers not enabled / weights not finalized");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   Producers& p = h->prod;
   const int B = h->cfg.batch;
   if (feats) {
-    CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
-    h->launches = 0;
+    if ((rc = start_forward(h, st))) return rc;
     producer_forward_start(h);
   }  // else: dd_run_backbone already wrote the input planes F[i] (and owns the status / launch counters)
   h->feats_ready = false;
@@ -3309,10 +3359,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
     h->rn = r;
     h->bb.enabled = false;
     h->mp.enabled = false;
-    h->weights_ready = false;
-    h->packed = false;
-    h->ws = nullptr;
-    drop_graphs(h);
+    invalidate_pack(h);
     return DD_OK;
   }
   if (bc->kind == DD_BACKBONE_MPVIT) {
@@ -3347,10 +3394,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
     h->mp = m;
     h->bb.enabled = false;
     h->rn.enabled = false;
-    h->weights_ready = false;
-    h->packed = false;
-    h->ws = nullptr;
-    drop_graphs(h);
+    invalidate_pack(h);
     return DD_OK;
   }
   if (bc->kind != DD_BACKBONE_SWIN) return fail(DD_ERR_UNSUPPORTED, "unknown backbone kind");
@@ -3379,10 +3423,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
   h->bb = b;
   h->rn.enabled = false;
   h->mp.enabled = false;
-  h->weights_ready = false;
-  h->packed = false;
-  h->ws = nullptr;
-  drop_graphs(h);
+  invalidate_pack(h);
   return DD_OK;
 }
 
@@ -3395,11 +3436,9 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
     return swin ? run_swin(h, img, outs, s) : (resnet ? run_resnet(h, img, outs, s) : run_mpvit(h, img, outs, s));
   };
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
-  CUDA_TRY(cudaMemsetAsync(h->status, 0, 64, st));
-  h->launches = 0;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = start_forward(h, st))) return rc;
   producer_forward_start(h);
   // the ResNet's BatchNorms follow the producer mode; Swin has none, MPViT's are not covered (always eval)
   const bool train = resnet && h->producer_mode == DD_PRODUCER_TRAIN;
@@ -3428,19 +3467,17 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   CUDA_TRY(cudaSetDevice(h->cfg.device));
   cudaStream_t st = h->cap_stream;
   const size_t Mp = (static_cast<size_t>(M) + 127) / 128 * 128 + 128;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
   Planes A, O;
   GenLayer L;
   float *y = nullptr, *bias = nullptr;
-  int* status = nullptr;
-  CUDA_TRY(cudaMalloc(&A.hi, Mp * K * 2));
-  CUDA_TRY(cudaMalloc(&A.lo, Mp * K * 2));
-  CUDA_TRY(cudaMalloc(&O.hi, Mp * N * 2));
-  CUDA_TRY(cudaMalloc(&O.lo, Mp * N * 2));
-  CUDA_TRY(cudaMalloc(&y, Mp * N * 4));
-  CUDA_TRY(cudaMalloc(&L.w_hi, static_cast<size_t>(N) * K * 2));
-  CUDA_TRY(cudaMalloc(&L.w_lo, static_cast<size_t>(N) * K * 2));
-  CUDA_TRY(cudaMalloc(&bias, N * 4));
-  CUDA_TRY(cudaMalloc(&status, 64));
+  if ((rc = call.alloc(&A.hi, Mp * K)) || (rc = call.alloc(&A.lo, Mp * K)) || (rc = call.alloc(&O.hi, Mp * N)) ||
+      (rc = call.alloc(&O.lo, Mp * N)) || (rc = call.alloc(&y, Mp * N)) ||
+      (rc = call.alloc(&L.w_hi, static_cast<size_t>(N) * K)) || (rc = call.alloc(&L.w_lo, static_cast<size_t>(N) * K)) ||
+      (rc = call.alloc(&bias, N)))
+    return rc;
   CUDA_TRY(cudaMemsetAsync(A.hi, 0x11, Mp * K * 2, st));
   CUDA_TRY(cudaMemsetAsync(A.lo, 0x01, Mp * K * 2, st));
   CUDA_TRY(cudaMemsetAsync(L.w_hi, 0x11, static_cast<size_t>(N) * K * 2, st));
@@ -3451,20 +3488,12 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   L.cout = N;
   L.nt = (N % 256 == 0) ? 256 : 192;
   L.shift = bias;
-  int rc;
   if ((rc = make_weight_map(&L.mb_hi, L.w_hi, N, K, 1, dd::GEN_BK, dd::gen_unit_cols(L.nt)))) return rc;
   if ((rc = make_weight_map(&L.mb_lo, L.w_lo, N, K, 1, dd::GEN_BK, dd::gen_unit_cols(L.nt)))) return rc;
-  int* saved = h->status;
-  h->status = status;
-  if ((rc = time_per_call(st, 3, iters, ms_out, [&]() {
-         return run_gemm(h, L, A, M, mode == 2 ? 2 : 0, (mode == 0 || mode == 1) ? y : nullptr, mode == 1 ? y : nullptr,
-                         mode == 2 ? &O : nullptr, st);
-       })))
-    return rc;
-  h->status = saved;
-  for (void* p : {(void*)A.hi, (void*)A.lo, (void*)O.hi, (void*)O.lo, (void*)y, (void*)L.w_hi, (void*)L.w_lo, (void*)bias, (void*)status})
-    cudaFree(p);
-  return DD_OK;
+  return time_per_call(st, 3, iters, ms_out, [&]() {
+    return run_gemm(h, L, A, M, mode == 2 ? 2 : 0, (mode == 0 || mode == 1) ? y : nullptr, mode == 1 ? y : nullptr,
+                    mode == 2 ? &O : nullptr, st);
+  });
 }
 
 int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, void* cuda_stream) {
@@ -3518,19 +3547,8 @@ int dd_poll_status(dd_handle h, void* cuda_stream) {
 
 // ---------------------------------------------------------------- standalone conv (tests / roofline)
 size_t dd_conv3x3_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int32_t height, int32_t width) {
-  const size_t BP = static_cast<size_t>(batch) * height * width;
-  const size_t nw = static_cast<size_t>(cin) * cout * 9;
-  size_t off = 0;
-  auto add = [&](size_t bytes) { off = align_up(off, 1024) + bytes; };
-  add(64);            // status + scratch
-  add(BP * cin * 4);  // x nhwc
-  add(BP * cin * 2);  // hi
-  add(BP * cin * 2);  // lo
-  add(BP * cout * 4); // y nhwc
-  add(nw * 2);
-  add(nw * 2);
-  add(nw * 4);
-  return align_up(off, 1024);
+  Conv3x3Ws v;
+  return conv3x3_layout(nullptr, batch, cin, cout, height, width, v);
 }
 
 int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, float* y, int32_t batch, int32_t cin,
@@ -3545,25 +3563,18 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   CUDA_TRY(cudaSetDevice(h->cfg.device));
   const size_t BP = static_cast<size_t>(batch) * height * width;
   const size_t nw = static_cast<size_t>(cin) * cout * 9;
-  Carver c{reinterpret_cast<uint8_t*>(workspace)};
-  int* status = c.take<int>(16);
-  float* xn = c.take<float>(BP * cin);
-  __half* hi = c.take<__half>(BP * cin);
-  __half* lo = c.take<__half>(BP * cin);
-  float* yn = c.take<float>(BP * cout);
-  __half* whi = c.take<__half>(nw);
-  __half* wlo = c.take<__half>(nw);
-  float* wsimt = c.take<float>(nw);
-  CUDA_TRY(cudaMemsetAsync(status, 0, 64, st));
+  Conv3x3Ws v;
+  conv3x3_layout(workspace, batch, cin, cout, height, width, v);
+  CUDA_TRY(cudaMemsetAsync(v.status, 0, 64, st));
   int rc;
-  if ((rc = transpose_in(x, xn, batch, cin, height * width, st))) return rc;
-  float* amax_dev = reinterpret_cast<float*>(status) + 8;
+  if ((rc = transpose_in(x, v.xn, batch, cin, height * width, st))) return rc;
+  float* amax_dev = reinterpret_cast<float*>(v.status) + 8;
   float sx, sw;
-  if ((rc = split_scale_of(xn, std::min<size_t>(BP * cin, 1u << 30), amax_dev, st, &sx))) return rc;
+  if ((rc = split_scale_of(v.xn, std::min<size_t>(BP * cin, 1u << 30), amax_dev, st, &sx))) return rc;
   if ((rc = split_scale_of(w, nw, amax_dev, st, &sw))) return rc;
-  dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(xn, hi, lo, BP * cin / 4, sx, status);
+  dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(v.xn, v.x.hi, v.x.lo, BP * cin / 4, sx, v.status);
   if ((rc = check_launch("split_planes"))) return rc;
-  dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, whi, wlo, wsimt, cout, cin, sw);
+  dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, v.w.hi, v.w.lo, v.wsimt, cout, cin, sw);
   if ((rc = check_launch("pack_conv_weight"))) return rc;
   dd::ConvArgs a;
   a.B = batch;
@@ -3571,39 +3582,29 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   a.W = width;
   a.bias = b;
   a.acc_scale = 1.f / (sx * sw);
-  a.y32 = yn;
+  a.y32 = v.yn;
   a.stats_partial = nullptr;
   a.out_hi = nullptr;
   a.out_lo = nullptr;
   a.out_a8 = a.out_l8 = nullptr;
   a.split_scale = 1.f;
-  a.status = status;
+  a.status = v.status;
   const bool simt = (h->cfg.flags & DD_FLAG_SIMT_CONV) != 0;
   CUtensorMap mb_hi{}, mb_lo{};
   if (!simt) {
-    if ((rc = make_weight_map(&mb_hi, whi, cout, cin, 9, kHaloBK[sid], cout))) return rc;
-    if ((rc = make_weight_map(&mb_lo, wlo, cout, cin, 9, kHaloBK[sid], cout))) return rc;
+    if ((rc = make_weight_map(&mb_hi, v.w.hi, cout, cin, 9, kHaloBK[sid], cout))) return rc;
+    if ((rc = make_weight_map(&mb_lo, v.w.lo, cout, cin, 9, kHaloBK[sid], cout))) return rc;
   }
-  if ((rc = launch_conv3x3(sid, dd::EPI_F32, simt, a, hi, lo, sx, wsimt, mb_hi, mb_lo, h->sm_count, st))) return rc;
+  if ((rc = launch_conv3x3(sid, dd::EPI_F32, simt, a, v.x.hi, v.x.lo, sx, v.wsimt, mb_hi, mb_lo, h->sm_count, st)))
+    return rc;
   if ((rc = check_launch("conv3x3"))) return rc;
-  return transpose_out(yn, y, batch, cout, height * width, st);
+  return transpose_out(v.yn, y, batch, cout, height * width, st);
 }
 
 // ---------------------------------------------------------------- standalone weight gradient (tests / roofline)
 size_t dd_conv3x3_wgrad_workspace_bytes(int32_t batch, int32_t cin, int32_t cout, int32_t height, int32_t width) {
-  const size_t BP = static_cast<size_t>(batch) * height * width;
-  size_t off = 0;
-  auto add = [&](size_t bytes) { off = align_up(off, 1024) + bytes; };
-  add(64);             // status + scratch
-  add(BP * cin * 4);   // x nhwc
-  add(BP * cin * 2);   // x hi
-  add(BP * cin * 2);   // x lo
-  add(BP * cout * 4);  // dy nhwc
-  add(BP * cout * 2);  // dy hi
-  add(BP * cout * 2);  // dy lo
-  add(wgrad_partial_elems(cout, cin, batch, height, width) * 8);
-  add(static_cast<size_t>(batch) * bwd_chunks(height * width) * cout * 4);  // bias-gradient partials
-  return align_up(off, 1024);
+  WgradWs v;
+  return wgrad_layout(nullptr, batch, cin, cout, height, width, v);
 }
 
 int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, float* db, int32_t batch, int32_t cin,
@@ -3619,36 +3620,24 @@ int dd_conv3x3_wgrad(dd_handle h, const float* x, const float* dy, float* dw, fl
   CUDA_TRY(cudaSetDevice(h->cfg.device));
   const int P = height * width;
   const size_t BP = static_cast<size_t>(batch) * P;
-  Carver c{reinterpret_cast<uint8_t*>(workspace)};
-  int* status = c.take<int>(16);
-  float* xn = c.take<float>(BP * cin);
-  __half* xhi = c.take<__half>(BP * cin);
-  __half* xlo = c.take<__half>(BP * cin);
-  float* dyn = c.take<float>(BP * cout);
-  Planes gp;
-  gp.hi = c.take<__half>(BP * cout);
-  gp.lo = c.take<__half>(BP * cout);
-  double* partial = c.take<double>(wgrad_partial_elems(cout, cin, batch, height, width));
-  float* col_part = c.take<float>(static_cast<size_t>(batch) * bwd_chunks(P) * cout);
-  float* scratch = reinterpret_cast<float*>(status) + 8;  // [0] x absmax, [1] dy absmax, [2] dy split scale
-  CUDA_TRY(cudaMemsetAsync(status, 0, 64, st));
+  WgradWs v;
+  wgrad_layout(workspace, batch, cin, cout, height, width, v);
+  float* scratch = reinterpret_cast<float*>(v.status) + 8;  // [0] x absmax, [1] dy absmax, [2] dy split scale
+  CUDA_TRY(cudaMemsetAsync(v.status, 0, 64, st));
   int rc;
-  if ((rc = transpose_in(x, xn, batch, cin, P, st))) return rc;
-  if ((rc = transpose_in(dy, dyn, batch, cout, P, st))) return rc;
+  if ((rc = transpose_in(x, v.xn, batch, cin, P, st))) return rc;
+  if ((rc = transpose_in(dy, v.dyn, batch, cout, P, st))) return rc;
   // X: host-side power-of-two scale, as dd_conv3x3 splits its input
   float sx;
-  if ((rc = split_scale_of(xn, BP * cin, scratch, st, &sx))) return rc;
-  dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(xn, xhi, xlo, BP * cin / 4, sx, status);
+  if ((rc = split_scale_of(v.xn, BP * cin, scratch, st, &sx))) return rc;
+  dd::split_planes_kernel<<<132 * 8, 256, 0, st>>>(v.xn, v.x.hi, v.x.lo, BP * cin / 4, sx, v.status);
   if ((rc = launched(h, "split_planes"))) return rc;
   // dY: the backward's own on-device split (also for the SIMT shapes, so a non-finite dY is reported for every shape)
-  if ((rc = run_colsum(h, cout, dyn, nullptr, batch, P, col_part, nullptr, db, st))) return rc;
-  const WgradBufs bufs{gp, scratch + 1, scratch + 2, status, partial};
-  if ((rc = run_wgrad(h, batch, height, width, cout, cin, dyn, nullptr, xhi, xlo, sx, dw, true, bufs, st))) return rc;
-  int flag = 0;
-  CUDA_TRY(cudaMemcpyAsync(&flag, status, 4, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  if (flag) return fail(DD_ERR_RANGE, "non-finite or out-of-range value in x or dy");
-  return DD_OK;
+  if ((rc = run_colsum(h, cout, v.dyn, nullptr, batch, P, v.col_part, nullptr, db, st))) return rc;
+  const WgradBufs bufs{v.dy, scratch + 1, scratch + 2, v.status, v.partial};
+  if ((rc = run_wgrad(h, batch, height, width, cout, cin, v.dyn, nullptr, v.x.hi, v.x.lo, sx, dw, true, bufs, st)))
+    return rc;
+  return check_status_word(v.status, st, "x or dy");
 }
 
 // ---------------------------------------------------------------- standalone producer layers (tests)
@@ -3850,9 +3839,8 @@ int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspac
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   if (!fold_active(h)) return fail(DD_ERR_UNSUPPORTED, "this engine runs convB and pred.0 as two convs");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   // whatever the planes currently hold is fine for timing: MMA time is data independent
   return time_per_call(st, 2, iters, ms_out, [&]() { return run_fold(h, st); });
 }
@@ -3862,9 +3850,8 @@ int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* 
   if (!h || !ms_out || iters < 1) return fail(DD_ERR_INVALID, "bad argument");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  CUDA_TRY(cudaSetDevice(h->cfg.device));
   int rc;
-  if ((rc = bind_workspace(h, workspace, workspace_bytes))) return rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   int layer = -1;
   for (int i = 0; i < 6; ++i)
     if (h->L[i].sid >= 0 && kShapes[h->L[i].sid].cin == cin && kShapes[h->L[i].sid].cout == cout) layer = i;

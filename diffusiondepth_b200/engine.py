@@ -57,6 +57,16 @@ def is_updatable(key: str) -> bool:
     return key.startswith(UPDATABLE_PREFIXES)
 
 
+def _ptr(t: Optional[torch.Tensor]) -> C.c_void_p:
+    """The device pointer the C ABI takes for a tensor; NULL for None."""
+    return C.c_void_p(0 if t is None else t.data_ptr())
+
+
+def _f32(t: Optional[torch.Tensor], device) -> Optional[torch.Tensor]:
+    """t as a contiguous fp32 tensor on device, copied only when it is not one already; None stays None."""
+    return None if t is None else t.detach().to(device, torch.float32).contiguous()
+
+
 def ddim_coefficients(alphas_cumprod: torch.Tensor, num_inference_steps: int, num_train_timesteps: int,
                       final_alpha_cumprod: float = 1.0) -> Tuple[list, list, list]:
     """Timesteps of `DDIMScheduler.set_timesteps` (reference scheduling_ddim.py:215-229) and the two scalars
@@ -145,14 +155,10 @@ class DenoiseEngine:
                                 and not k.endswith("num_batches_tracked") and tensors[k].dim() <= 4
                                 and not k.startswith(("hahineck.multi_att", "hahineck.self_attn",
                                                       "hahineck.reference_points", "hahineck.level_embed")))
-        self._keep = []
         for k in keys:
             if k not in tensors:
                 raise EngineError(f"missing parameter {k}")
-            t = tensors[k].detach().to(self.device, torch.float32).contiguous()
-            self._keep.append(t)
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _cabi.check(self.lib.dd_set_weight(self._h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+        self._register((k, tensors[k]) for k in keys)
         _cabi.check(self.lib.dd_finalize_weights(self._h, C.c_void_p(self._stream())))
         self._keep = []
 
@@ -165,15 +171,18 @@ class DenoiseEngine:
         for k, v in tensors.items():  # what dd_set_weight would reject, before anything is registered
             if not (k in known or k.startswith(("hahineck.", "conv_lateral.", "conv_up.", "backbone."))) or v.dim() > 4:
                 raise EngineError(f"unknown weight key: {k}")
-        self._keep = []
-        for k, v in tensors.items():
-            t = v.detach().to(self.device, torch.float32).contiguous()
-            self._keep.append(t)
-            shape = (C.c_int64 * t.dim())(*t.shape)
-            _cabi.check(self.lib.dd_set_weight(self._h, k.encode(), C.c_void_p(t.data_ptr()), shape, t.dim()))
+        self._register(tensors.items())
         status = self.lib.dd_update_weights(self._h, C.c_void_p(self._stream()))
         self._keep = []  # still read on the stream: the caching allocator reuses the memory in stream order
         _cabi.check(status)
+
+    def _register(self, items):
+        """dd_set_weight for every (key, tensor) of items, from fp32 copies kept in `_keep` for the pack to read."""
+        self._keep = []
+        for k, v in items:
+            t = _f32(v, self.device)
+            self._keep.append(t)
+            _cabi.check(self.lib.dd_set_weight(self._h, k.encode(), _ptr(t), (C.c_int64 * t.dim())(*t.shape), t.dim()))
 
     def graph_capture_count(self) -> int:
         """CUDA graph instantiations of this engine so far."""
@@ -227,6 +236,12 @@ class DenoiseEngine:
     def _aligned(ws: torch.Tensor) -> int:
         return (ws.data_ptr() + 1023) // 1024 * 1024
 
+    def _ws_args(self):
+        """The last three arguments of every entry that runs on the engine's workspace: its 1024-byte aligned start,
+        the bytes usable from there, the current stream."""
+        ws = self._workspace()
+        return C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())
+
     def _check_in(self, t: torch.Tensor, shape):
         if t.device != self.device or t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
             raise EngineError(f"expected contiguous fp32 {tuple(shape)} on {self.device}, got {tuple(t.shape)} "
@@ -241,9 +256,7 @@ class DenoiseEngine:
         chans, sizes, _ = self.producers
         feats = [torch.empty(self.batch, c, *hw, device=self.device) for c, hw in zip(chans, sizes)] if want_feats else None
         ptrs = (C.c_void_p * 4)(*[f.data_ptr() for f in feats]) if want_feats else None
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_run_backbone(self._h, C.c_void_p(rgb.data_ptr()), ptrs, C.c_void_p(self._aligned(ws)),
-                                             ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_run_backbone(self._h, _ptr(rgb), ptrs, *self._ws_args()))
         return feats
 
     def build_condition(self, feats, want_cond=False):
@@ -258,10 +271,7 @@ class DenoiseEngine:
                 self._check_in(f, (self.batch, c, *hw))
             ptrs = (C.c_void_p * 4)(*([f.data_ptr() for f in feats] + [0] * (4 - len(feats))))
         cond = torch.empty(self.batch, 256, *self.cond_hw, device=self.device) if want_cond else None
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_build_condition(self._h, ptrs, C.c_void_p(cond.data_ptr() if want_cond else 0),
-                                                C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
-                                                C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_build_condition(self._h, ptrs, _ptr(cond), *self._ws_args()))
         return cond
 
     def denoise_decode(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False, want_logits=False):
@@ -274,11 +284,8 @@ class DenoiseEngine:
         depth = torch.empty(B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32)
         latent = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32) if want_latent else None
         logits = torch.empty_like(depth) if want_logits else None
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_denoise_decode(
-            self._h, C.c_void_p(cond.data_ptr() if cond is not None else 0), C.c_void_p(noise.data_ptr()),
-            C.c_void_p(latent.data_ptr() if want_latent else 0), C.c_void_p(logits.data_ptr() if want_logits else 0),
-            C.c_void_p(depth.data_ptr()), C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_denoise_decode(self._h, _ptr(cond), _ptr(noise), _ptr(latent), _ptr(logits), _ptr(depth),
+                                               *self._ws_args()))
         return depth, latent, logits
 
     def denoise_decode_steps(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False,
@@ -294,11 +301,8 @@ class DenoiseEngine:
         steps = torch.empty(self.steps, B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32)
         latent = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32) if want_latent else None
         logits = torch.empty(B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32) if want_logits else None
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_denoise_decode_steps(
-            self._h, C.c_void_p(cond.data_ptr() if cond is not None else 0), C.c_void_p(noise.data_ptr()),
-            C.c_void_p(latent.data_ptr() if want_latent else 0), C.c_void_p(logits.data_ptr() if want_logits else 0),
-            C.c_void_p(steps.data_ptr()), C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_denoise_decode_steps(self._h, _ptr(cond), _ptr(noise), _ptr(latent), _ptr(logits),
+                                                     _ptr(steps), *self._ws_args()))
         return steps, latent, logits
 
     def denoiser_forward(self, cond: torch.Tensor, noisy: torch.Tensor, t) -> torch.Tensor:
@@ -308,10 +312,8 @@ class DenoiseEngine:
         self._check_in(noisy, (B, 16, h, w))
         ts = self._timesteps(t)
         eps = torch.empty_like(noisy)
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_denoiser_forward(
-            self._h, C.c_void_p(cond.data_ptr()), C.c_void_p(noisy.data_ptr()), (C.c_int64 * B)(*ts),
-            C.c_void_p(eps.data_ptr()), C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_denoiser_forward(self._h, _ptr(cond), _ptr(noisy), (C.c_int64 * B)(*ts), _ptr(eps),
+                                                 *self._ws_args()))
         return eps
 
     def _timesteps(self, t):
@@ -339,12 +341,8 @@ class DenoiseEngine:
             for k in keys:
                 grads[k] = torch.empty(_PARAM_SHAPES[k], device=self.device, dtype=torch.float32)
         ptrs = (C.c_void_p * len(keys))(*[grads[k].data_ptr() if k in grads else 0 for k in keys])
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_denoiser_backward(
-            self._h, C.c_void_p(cond.data_ptr()), C.c_void_p(noisy.data_ptr()), (C.c_int64 * B)(*ts),
-            C.c_void_p(d_eps.data_ptr()), C.c_void_p(d_cond.data_ptr() if want_cond else 0),
-            C.c_void_p(d_noisy.data_ptr() if want_noisy else 0), ptrs, C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
-            C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_denoiser_backward(self._h, _ptr(cond), _ptr(noisy), (C.c_int64 * B)(*ts), _ptr(d_eps),
+                                                  _ptr(d_cond), _ptr(d_noisy), ptrs, *self._ws_args()))
         return d_cond, d_noisy, grads
 
     def denoiser_relu_inputs(self, cond: torch.Tensor, noisy: torch.Tensor, t) -> Dict[str, torch.Tensor]:
@@ -358,11 +356,9 @@ class DenoiseEngine:
         self._check_in(noisy, (B, 16, h, w))
         ts = self._timesteps(t)
         z = {k: torch.empty(B, c, h, w, device=self.device, dtype=torch.float32) for k, c in GN_LAYERS.items()}
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_denoiser_relu_inputs(
-            self._h, C.c_void_p(cond.data_ptr()), C.c_void_p(noisy.data_ptr()), (C.c_int64 * B)(*ts),
-            (C.c_void_p * 4)(*[v.data_ptr() for v in z.values()]), C.c_void_p(self._aligned(ws)), ws.numel() - 1024,
-            C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_denoiser_relu_inputs(self._h, _ptr(cond), _ptr(noisy), (C.c_int64 * B)(*ts),
+                                                     (C.c_void_p * 4)(*[v.data_ptr() for v in z.values()]),
+                                                     *self._ws_args()))
         return z
 
     def _grad_buffers(self, keys, shapes, default=None):
@@ -395,15 +391,9 @@ class DenoiseEngine:
         keys = DENOISER_KEYS + (FUSE_KEYS if self.variant == "swin" else ())
         grads, ptrs = self._grad_buffers(keys if want_params else (), _PARAM_SHAPES)
         dgrads, dptrs = self._grad_buffers(DECODER_PARAM_KEYS if want_params else (), _DECODER_SHAPES, (16,))
-        ws = self._workspace()
-
-        def ptr(t):
-            return C.c_void_p(t.data_ptr() if t is not None else 0)
-
         _cabi.check(self.lib.dd_denoise_backward(
-            self._h, ptr(cond), ptr(noise), ptr(d_depth), ptr(d_latent), ptr(d_cond), ptr(d_noise),
-            ptrs if want_params else None, dptrs if want_params else None, ptr(latents), C.c_void_p(self._aligned(ws)),
-            ws.numel() - 1024, C.c_void_p(self._stream())))
+            self._h, _ptr(cond), _ptr(noise), _ptr(d_depth), _ptr(d_latent), _ptr(d_cond), _ptr(d_noise),
+            ptrs if want_params else None, dptrs if want_params else None, _ptr(latents), *self._ws_args()))
         grads.update(dgrads)
         return d_cond, d_noise, grads, latents
 
@@ -417,11 +407,8 @@ class DenoiseEngine:
         self._check_in(d_depth, (B, 1, 2 * h, 2 * w))
         d_latent = torch.empty_like(latent) if want_latent else None
         grads, ptrs = self._grad_buffers(DECODER_PARAM_KEYS if want_params else (), _DECODER_SHAPES, (16,))
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_decode_backward(
-            self._h, C.c_void_p(latent.data_ptr()), C.c_void_p(d_depth.data_ptr()),
-            C.c_void_p(d_latent.data_ptr() if want_latent else 0), ptrs if want_params else None,
-            C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_decode_backward(self._h, _ptr(latent), _ptr(d_depth), _ptr(d_latent),
+                                                ptrs if want_params else None, *self._ws_args()))
         return d_latent, grads
 
     def encode(self, depth: torch.Tensor) -> torch.Tensor:
@@ -430,8 +417,7 @@ class DenoiseEngine:
         H, W = depth.shape[-2:]
         self._check_in(depth, (B, 1, H, W))
         out = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32)
-        _cabi.check(self.lib.dd_encode(self._h, C.c_void_p(depth.data_ptr()), H, W, C.c_void_p(out.data_ptr()),
-                                       C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_encode(self._h, _ptr(depth), H, W, _ptr(out), C.c_void_p(self._stream())))
         return out
 
     def set_codec_mode(self, training: bool):
@@ -446,8 +432,7 @@ class DenoiseEngine:
         call).  Ordered on the current stream; no synchronisation."""
         out = torch.empty(max(self.steps, 2), 2, 16, device=self.device, dtype=torch.float32)
         n = C.c_int32()
-        _cabi.check(self.lib.dd_codec_batch_stats(self._h, C.c_void_p(out.data_ptr()), out.shape[0], C.byref(n),
-                                                  C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_codec_batch_stats(self._h, _ptr(out), out.shape[0], C.byref(n), C.c_void_p(self._stream())))
         return out[:n.value]
 
     def set_producer_mode(self, training: bool):
@@ -482,8 +467,7 @@ class DenoiseEngine:
             return {}
         rec = torch.empty(total, device=self.device, dtype=torch.float32)
         n = C.c_int32()
-        _cabi.check(self.lib.dd_producer_batch_stats(self._h, C.c_void_p(rec.data_ptr()), total, C.byref(n),
-                                                     C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_producer_batch_stats(self._h, _ptr(rec), total, C.byref(n), C.c_void_p(self._stream())))
         return {k: (rec[o:o + c], rec[o + c:o + 2 * c]) for k, c, o, f in info if f}
 
     def decode(self, latent: torch.Tensor, want_logits=False):
@@ -491,22 +475,18 @@ class DenoiseEngine:
         self._check_in(latent, (B, 16, h, w))
         depth = torch.empty(B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32)
         logits = torch.empty_like(depth) if want_logits else None
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_decode(self._h, C.c_void_p(latent.data_ptr()),
-                                       C.c_void_p(logits.data_ptr() if want_logits else 0), C.c_void_p(depth.data_ptr()),
-                                       C.c_void_p(self._aligned(ws)), ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_decode(self._h, _ptr(latent), _ptr(logits), _ptr(depth), *self._ws_args()))
         return depth, logits
 
     def conv3x3(self, x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
         """Single 3x3/s1/p1 conv + bias on the engine's convolution path (parity tests, roofline)."""
         B, cin, H, W = x.shape
         cout = w.shape[0]
-        x, w, b = (t.detach().to(self.device, torch.float32).contiguous() for t in (x, w, b))
+        x, w, b = (_f32(t, self.device) for t in (x, w, b))
         y = torch.empty(B, cout, H, W, device=self.device, dtype=torch.float32)
         need = int(self.lib.dd_conv3x3_workspace_bytes(B, cin, cout, H, W))
         ws = torch.empty(need + 1024, dtype=torch.uint8, device=self.device)
-        _cabi.check(self.lib.dd_conv3x3(self._h, C.c_void_p(x.data_ptr()), C.c_void_p(w.data_ptr()),
-                                        C.c_void_p(b.data_ptr()), C.c_void_p(y.data_ptr()), B, cin, cout, H, W,
+        _cabi.check(self.lib.dd_conv3x3(self._h, _ptr(x), _ptr(w), _ptr(b), _ptr(y), B, cin, cout, H, W,
                                         C.c_void_p(self._aligned(ws)), need, C.c_void_p(self._stream())))
         return y
 
@@ -517,13 +497,12 @@ class DenoiseEngine:
         cout = dy.shape[1]
         if tuple(dy.shape) != (B, cout, H, W):
             raise EngineError(f"dy {tuple(dy.shape)} does not match x {tuple(x.shape)}")
-        x, dy = (t.detach().to(self.device, torch.float32).contiguous() for t in (x, dy))
+        x, dy = _f32(x, self.device), _f32(dy, self.device)
         dw = torch.empty(cout, cin, 3, 3, device=self.device, dtype=torch.float32)
         db = torch.empty(cout, device=self.device, dtype=torch.float32)
         need = int(self.lib.dd_conv3x3_wgrad_workspace_bytes(B, cin, cout, H, W))
         ws = torch.empty(need + 1024, dtype=torch.uint8, device=self.device)
-        _cabi.check(self.lib.dd_conv3x3_wgrad(self._h, C.c_void_p(x.data_ptr()), C.c_void_p(dy.data_ptr()),
-                                              C.c_void_p(dw.data_ptr()), C.c_void_p(db.data_ptr()), B, cin, cout, H, W,
+        _cabi.check(self.lib.dd_conv3x3_wgrad(self._h, _ptr(x), _ptr(dy), _ptr(dw), _ptr(db), B, cin, cout, H, W,
                                               C.c_void_p(self._aligned(ws)), need, C.c_void_p(self._stream())))
         return dw, db
 
@@ -540,12 +519,8 @@ class DenoiseEngine:
         Returns (y32, (hi, lo), {"nt", "work", "grid", "parts"}) with None for a skipped output; "parts" > 1: the
         layer ran split along K."""
         dev = self.device
-
-        def f32(t):
-            return None if t is None else t.detach().to(dev, torch.float32).contiguous()
-
-        x0, x1, w, bias, add = f32(x0), f32(x1), f32(w), f32(bias), f32(add)
-        bn = None if bn is None else [f32(t) for t in bn]
+        x0, x1, w, bias, add = (_f32(t, dev) for t in (x0, x1, w, bias, add))
+        bn = None if bn is None else [_f32(t, dev) for t in bn]
         d = _cabi.DDGenLayerDesc()
         d.taps = 1 if (transposed or w.dim() == 2) else w.shape[2] * w.shape[3]
         d.stride, d.transposed, d.act, d.add_first = int(stride), int(transposed), int(act), int(add_first)
@@ -568,13 +543,9 @@ class DenoiseEngine:
         planes = None if planes is False else planes
         info = (C.c_int32 * 4)()
         bn_ptrs = None if bn is None else (C.c_void_p * 4)(*[t.data_ptr() for t in bn])
-
-        def ptr(t):
-            return C.c_void_p(0 if t is None else t.data_ptr())
-
-        _cabi.check(self.lib.dd_gen_layer(self._h, C.byref(d), ptr(x0), ptr(x1), ptr(w), ptr(bias), bn_ptrs, ptr(add),
-                                          ptr(y32), ptr(planes[0] if planes else None),
-                                          ptr(planes[1] if planes else None), info, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_gen_layer(self._h, C.byref(d), _ptr(x0), _ptr(x1), _ptr(w), _ptr(bias), bn_ptrs,
+                                          _ptr(add), _ptr(y32), _ptr(planes[0] if planes else None),
+                                          _ptr(planes[1] if planes else None), info, C.c_void_p(self._stream())))
         return y32, planes, {"nt": info[0], "work": info[1], "grid": info[2], "parts": info[3]}
 
     def window_attention(self, qkv: torch.Tensor, qkv_bias: torch.Tensor, table: torch.Tensor, batch: int,
@@ -582,11 +553,10 @@ class DenoiseEngine:
         """Swin (shifted-)window attention on the engine's kernels (dd_window_attention): qkv [B*H*W, 3C] fp32 (padded
         tokens carry qkv_bias [3C]), table [169, nH].  kernel: 0 the engine's choice, 1 fp32 CUDA cores, 2 wgmma.
         Returns (out [B*H*W, C] fp32, {"work", "grid"})."""
-        qkv, qkv_bias, table = (t.detach().to(self.device, torch.float32).contiguous() for t in (qkv, qkv_bias, table))
+        qkv, qkv_bias, table = (_f32(t, self.device) for t in (qkv, qkv_bias, table))
         out = torch.empty(qkv.shape[0], qkv.shape[1] // 3, device=self.device, dtype=torch.float32)
         info = (C.c_int32 * 2)()
-        _cabi.check(self.lib.dd_window_attention(self._h, C.c_void_p(qkv.data_ptr()), C.c_void_p(qkv_bias.data_ptr()),
-                                                 C.c_void_p(table.data_ptr()), C.c_void_p(out.data_ptr()), int(batch),
+        _cabi.check(self.lib.dd_window_attention(self._h, _ptr(qkv), _ptr(qkv_bias), _ptr(table), _ptr(out), int(batch),
                                                  int(hw[0]), int(hw[1]), int(num_heads), int(shift), int(kernel), info,
                                                  C.c_void_p(self._stream())))
         return out, {"work": info[0], "grid": info[1]}
@@ -597,17 +567,14 @@ class DenoiseEngine:
         (dd_factor_attention; 8 heads, crpe windows {3: 2, 5: 3, 7: 3}): qkv [B*H*W, 3C] fp32, crpe_w / crpe_b the three
         crpe.conv_list weights [nh*Ch, 1, k, k] / biases.  Returns (out [B*H*W, C] fp32, {"tpc", "chunks", "hb",
         "grid"})."""
-        def f32(t):
-            return t.detach().to(self.device, torch.float32).contiguous()
-
-        qkv, crpe_w, crpe_b = f32(qkv), [f32(t) for t in crpe_w], [f32(t) for t in crpe_b]
+        qkv = _f32(qkv, self.device)
+        crpe_w, crpe_b = [_f32(t, self.device) for t in crpe_w], [_f32(t, self.device) for t in crpe_b]
         out = torch.empty(qkv.shape[0], qkv.shape[1] // 3, device=self.device, dtype=torch.float32)
         info = (C.c_int32 * 4)()
-        _cabi.check(self.lib.dd_factor_attention(self._h, C.c_void_p(qkv.data_ptr()),
-                                                 (C.c_void_p * 3)(*[t.data_ptr() for t in crpe_w]),
-                                                 (C.c_void_p * 3)(*[t.data_ptr() for t in crpe_b]),
-                                                 C.c_void_p(out.data_ptr()), int(batch), int(hw[0]), int(hw[1]),
-                                                 out.shape[1], info, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_factor_attention(self._h, _ptr(qkv), (C.c_void_p * 3)(*[t.data_ptr() for t in crpe_w]),
+                                                 (C.c_void_p * 3)(*[t.data_ptr() for t in crpe_b]), _ptr(out),
+                                                 int(batch), int(hw[0]), int(hw[1]), out.shape[1], info,
+                                                 C.c_void_p(self._stream())))
         return out, {"tpc": info[0], "chunks": info[1], "hb": info[2], "grid": info[3]}
 
     def depthwise_conv(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, bn=None,
@@ -616,22 +583,16 @@ class DenoiseEngine:
         3], then bn = (weight, bias, running_mean, running_var) folded or `bias`; act 0 / 3 (Hardswish); residual adds x
         (stride 1).  y32 / planes: True allocates the output (planes: fp16 hi / lo at the producers' scale), False skips
         it.  Returns (y32, (hi, lo), {"grid", "work"}) with None for a skipped output."""
-        def f32(t):
-            return None if t is None else t.detach().to(self.device, torch.float32).contiguous()
-
-        def ptr(t):
-            return C.c_void_p(0 if t is None else t.data_ptr())
-
-        x, w, bias = f32(x), f32(w), f32(bias)
-        bn = None if bn is None else [f32(t) for t in bn]
+        x, w, bias = (_f32(t, self.device) for t in (x, w, bias))
+        bn = None if bn is None else [_f32(t, self.device) for t in bn]
         B, H, W, Cc = x.shape
         shape = (B, (H - 1) // stride + 1, (W - 1) // stride + 1, Cc)
         y32 = torch.full(shape, float("nan"), device=self.device) if y32 else None
         planes = tuple(torch.zeros(shape, dtype=torch.float16, device=self.device) for _ in range(2)) if planes else None
         info = (C.c_int32 * 2)()
         bn_ptrs = None if bn is None else (C.c_void_p * 4)(*[t.data_ptr() for t in bn])
-        _cabi.check(self.lib.dd_depthwise_conv(self._h, ptr(x), ptr(w), ptr(bias), bn_ptrs, ptr(y32),
-                                               ptr(planes[0] if planes else None), ptr(planes[1] if planes else None),
+        _cabi.check(self.lib.dd_depthwise_conv(self._h, _ptr(x), _ptr(w), _ptr(bias), bn_ptrs, _ptr(y32),
+                                               _ptr(planes[0] if planes else None), _ptr(planes[1] if planes else None),
                                                B, H, W, Cc, int(stride), int(act), int(residual), info,
                                                C.c_void_p(self._stream())))
         return y32, planes, {"grid": info[0], "work": info[1]}
@@ -639,27 +600,22 @@ class DenoiseEngine:
     def layer_norm(self, x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
         """LayerNorm over the last axis on the MPViT encoders' kernel (dd_layer_norm, C <= 512): x [M, C] fp32 ->
         fp32 [M, C], rebuilt from the kernel's hi / lo planes."""
-        x, gamma, beta = (t.detach().to(self.device, torch.float32).contiguous() for t in (x, gamma, beta))
+        x, gamma, beta = (_f32(t, self.device) for t in (x, gamma, beta))
         out = torch.empty_like(x)
-        _cabi.check(self.lib.dd_layer_norm(self._h, C.c_void_p(x.data_ptr()), C.c_void_p(gamma.data_ptr()),
-                                           C.c_void_p(beta.data_ptr()), C.c_void_p(out.data_ptr()), x.shape[0],
-                                           x.shape[1], float(eps), C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_layer_norm(self._h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), x.shape[0], x.shape[1],
+                                           float(eps), C.c_void_p(self._stream())))
         return out
 
     def bench_conv(self, cin: int, cout: int, iters: int = 20) -> float:
         """Average milliseconds per launch of the (cin -> cout) conv on this engine's latent grid."""
         ms = C.c_float()
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_bench_conv(self._h, cin, cout, iters, C.byref(ms), C.c_void_p(self._aligned(ws)),
-                                           ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_bench_conv(self._h, cin, cout, iters, C.byref(ms), *self._ws_args()))
         return float(ms.value)
 
     def bench_pred_fold(self, iters: int = 20) -> float:
         """Average milliseconds of the Swin step's composed convB -> pred.0 (5x5 conv + ring correction)."""
         ms = C.c_float()
-        ws = self._workspace()
-        _cabi.check(self.lib.dd_bench_pred_fold(self._h, iters, C.byref(ms), C.c_void_p(self._aligned(ws)),
-                                                ws.numel() - 1024, C.c_void_p(self._stream())))
+        _cabi.check(self.lib.dd_bench_pred_fold(self._h, iters, C.byref(ms), *self._ws_args()))
         return float(ms.value)
 
     def bench_gemm(self, M: int, K: int, N: int, mode: int = 0, iters: int = 20) -> float:

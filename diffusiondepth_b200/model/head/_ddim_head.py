@@ -15,7 +15,7 @@ import collections
 import copy
 import threading
 import weakref
-from typing import Dict, Optional, Tuple
+from typing import Dict, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -54,6 +54,28 @@ def collect_tensors(module: nn.Module, prefix: str = "") -> Dict[str, torch.Tens
 
     walk(module, prefix)
     return out
+
+
+class EngineKey(NamedTuple):
+    """What a head's cached engine was created for: geometry, schedule and the creation flags."""
+    batch: int
+    latent_hw: Tuple[int, int]
+    cond_hw: Tuple[int, int]
+    device: str
+    steps: int
+    cuda_graph: bool
+    native: bool                          # neck + FPN on the engine
+    image_hw: Optional[Tuple[int, int]]   # and the backbone (None: not native)
+    step_decode: bool
+    fp8_corr: bool
+    producer_train: bool
+    backward: bool
+    loop_backward: bool
+
+    @property
+    def geometry(self):
+        """What an engine serving the bare operators (denoiser / decode) must match."""
+        return self.batch, self.latent_hw, self.cond_hw, self.device, self.steps
 
 
 def _signature(tensors):
@@ -421,34 +443,35 @@ class DDIMHeadBase(nn.Module):
             return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
                                        loop_backward, producer_train)
 
+    def _engine_key(self, batch, latent_hw, cond_hw, device, native=False, image_hw=None, backward=False,
+                    loop_backward=False) -> EngineKey:
+        return EngineKey(batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)),
+                         self.diffusion_inference_steps, self.use_cuda_graph, native,
+                         tuple(image_hw) if image_hw is not None else None, bool(self.return_intermediates),
+                         bool(self.fp8_corrections), native and bool(self.producer_train_bn), bool(backward),
+                         bool(loop_backward))
+
     def _grad_engine(self, batch, latent_hw, cond_hw, device) -> DenoiseEngine:
         """The engine `denoiser_backward` runs on: the loop-backward engine of this geometry when the head trains through
         the loop or that engine exists (its flag is a superset), else a backward-only one."""
-        loop_key = (batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)), self.diffusion_inference_steps,
-                    self.use_cuda_graph, False, None, bool(self.return_intermediates), bool(self.fp8_corrections),
-                    False, False, True)
-        loop = self.grad_through_loop or loop_key in self._engines
+        loop = self.grad_through_loop or \
+            self._engine_key(batch, latent_hw, cond_hw, device, loop_backward=True) in self._engines
         return self._engine(batch, latent_hw, cond_hw, device, backward=not loop, loop_backward=loop)
 
     def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
                        loop_backward, producer_train=False) -> DenoiseEngine:
         native = feats is not None
-        ptrain_flag = native and bool(self.producer_train_bn)
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
-        key = (batch, tuple(latent_hw), tuple(cond_hw), str(device), self.diffusion_inference_steps,
-               self.use_cuda_graph, native, tuple(image_hw) if image_hw is not None else None,
-               bool(self.return_intermediates), bool(self.fp8_corrections), ptrain_flag, bool(backward),
-               bool(loop_backward))
+        key = self._engine_key(batch, latent_hw, cond_hw, device, native, image_hw, backward, loop_backward)
         eng = self._engines.get(key)
         if eng is None:
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
-            eng = DenoiseEngine(self.variant, batch, latent_hw, cond_hw, self.diffusion_inference_steps, device,
-                                cuda_graph=self.use_cuda_graph, check_range=False,
-                                step_decode=bool(self.return_intermediates), workspace_pool=pool,
-                                fp8_corr=bool(self.fp8_corrections), backward=bool(backward),
-                                loop_backward=bool(loop_backward), producer_train=ptrain_flag)
+            eng = DenoiseEngine(self.variant, batch, latent_hw, cond_hw, key.steps, device, cuda_graph=key.cuda_graph,
+                                check_range=False, step_decode=key.step_decode, workspace_pool=pool,
+                                fp8_corr=key.fp8_corr, backward=key.backward, loop_backward=key.loop_backward,
+                                producer_train=key.producer_train)
             if native:
                 eng.enable_producers(feats[0], feats[1], has_neck=self.has_neck)
             if image_hw is not None:
@@ -508,9 +531,9 @@ class DDIMHeadBase(nn.Module):
     def _any_engine(self, batch, latent_hw, cond_hw, device):
         """An engine of this geometry for the bare operators (denoiser / decode): reuse the forward's engine (same
         packed denoiser + codec weights) instead of packing a second one."""
-        want = (batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)))
+        want = self._engine_key(batch, latent_hw, cond_hw, device)
         for key in reversed(self._engines):
-            if key[:4] == want and key[4] == self.diffusion_inference_steps and self._packed.get(key) is not None:
+            if key.geometry == want.geometry and self._packed.get(key) is not None:
                 tensors, sig, _ = self._packed[key]
                 if _signature(tensors) == sig:
                     self._engines.move_to_end(key)

@@ -92,8 +92,8 @@ def main():
         it[mode].append((time.perf_counter() - t0) * 1e3)
 
     # (a) and (b) on the head's engines, at its own latent, condition map and noise
-    fwd = next(e for k, e in head._engines.items() if k[7] is not None)
-    loop = next(e for k, e in head._engines.items() if k[-1])
+    fwd = next(e for k, e in head._engines.items() if k.image_hw is not None)
+    loop = next(e for k, e in head._engines.items() if k.loop_backward)
     latent, cond = head.last_latent.detach().contiguous(), head.last_cond.detach().contiguous()
     noise = sample["noise"].contiguous()
     d_depth = torch.randn(a.batch, 1, 2 * latent.shape[2], 2 * latent.shape[3], device=dev) * 1e-6

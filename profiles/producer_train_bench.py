@@ -80,7 +80,7 @@ def run_config(name, iters, dev):
         it[mode].append((time.perf_counter() - t0) * 1e3)
 
     head = models[True].depth_head
-    eng = next(e for k, e in head._engines.items() if k[7] is not None and k[10])  # native backbone, flagged
+    eng = next(e for k, e in head._engines.items() if k.image_hw is not None and k.producer_train)
     img = sample["rgb"].contiguous().float()
 
     def chain(train):

@@ -93,7 +93,7 @@ def main():
         caps[mode].append(captures() - before)
 
     # (a) and (b) on the forward engine (native backbone + producers), from the tensors it was last packed with
-    fwd_key = next(k for k in head._engines if k[7] is not None)
+    fwd_key = next(k for k in head._engines if k.image_hw is not None)
     eng, tensors = head._engines[fwd_key], head._packed[fwd_key][0]
     trained = {k: tensors[k] for k in keys}
     res = {"card (name, power limit, max SM clock)": card(), "family": a.family, "batch": a.batch,

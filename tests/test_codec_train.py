@@ -404,7 +404,7 @@ def test_vis_head_applies_T_plus_1_updates_in_reference_order():
     fp, gt, noise = _head_inputs(head)
     r0 = (bn.running_mean.double().cpu().clone(), bn.running_var.double().cpu().clone())
     out = _run_head(head, fp, gt, noise)
-    eng = next(e for k, e in head._engines.items() if k[8])  # the step-decode engine
+    eng = next(e for k, e in head._engines.items() if k.step_decode)
     rec = eng.codec_batch_stats().double().cpu()
     assert rec.shape == (T, 2, 16)
 

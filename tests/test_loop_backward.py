@@ -277,7 +277,7 @@ def test_head_grad_through_loop_reaches_every_parameter():
     for k, p in zip(keys, params):
         assert p.grad is not None and float(p.grad.abs().max()) > 0, k
     # the operator backward of ddim_loss ran on the loop engine: no backward-only engine was created
-    assert not any(key[-2] for key in head._engines)
+    assert not any(key.backward for key in head._engines)
 
 
 @pytest.mark.gpu
