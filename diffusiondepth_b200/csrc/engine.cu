@@ -312,6 +312,7 @@ struct GenLayer {
   bool alt = false;          // cout divisible by 256 and 192: launch_gen picks the width whose last wave wastes least
   CUtensorMap mb_hi_alt, mb_lo_alt;  // for N tiles of 192 columns
   float* zero_shift = nullptr;       // layers deep enough to be split along K (gen_parts): the partial launches' shift
+  int bn = -1;                       // index of its training-mode BatchNorm pack in dd_engine::pt.layers (-1: none)
 };
 
 // K iterations (64-channel chunk x tap, 12 wgmma each) that one fp32 wgmma accumulator of convgen_wgmma_kernel takes.
@@ -472,10 +473,10 @@ struct dd_engine {
   // DD_PRODUCER_TRAIN (dd_set_producer_mode; DD_FLAG_PRODUCER_TRAIN): the producers' BatchNorms on batch statistics.
   // Every BatchNorm'ed producer layer, in evaluation order (ResNet bn1 / bn2 block by block, then per level the neck's
   // lateral / proj / fusion, then the FPN top-down: lateral, conv_up), keeps an unfolded pack of its conv and device
-  // copies of gamma / beta; the scratch below is engine-owned and sized for the largest layer.
+  // copies of gamma / beta; the scratch below is engine-owned and sized for the largest layer.  The eval layer names
+  // its record (GenLayer::bn).
   int producer_mode = DD_PRODUCER_EVAL;
   struct ProdBn {
-    const GenLayer* eval = nullptr;  // the layer's eval (folded) pack, which names it at run time
     GenLayer raw;                    // conv (or ConvT) weights alone: no BatchNorm, zero shift
     float *gamma = nullptr, *beta = nullptr;
     int C = 0;                       // BatchNorm channels
@@ -487,7 +488,6 @@ struct dd_engine {
   };
   struct ProdTrain {
     std::vector<ProdBn> layers;
-    std::map<const GenLayer*, int> index;
     float* U = nullptr;                              // pre-BN conv output, fp32 NHWC
     double *part = nullptr, *sum1 = nullptr;         // pbn_stats_kernel partials [blocks][2][C]; pass-1 sums [C]
     float *s = nullptr, *t = nullptr, *rec = nullptr;  // batch scale / shift [C]; records
@@ -1271,6 +1271,17 @@ int find_bn(dd_engine* e, const std::string& prefix, const float** bn) {
   }
   return DD_OK;
 }
+int copy_param(dd_engine* e, const std::string& key, size_t n, float** out, cudaStream_t st) {
+  const Raw* r = find(e, key);
+  if (!r) return fail(DD_ERR_INVALID, "missing weights: " + key);
+  size_t have = 1;
+  for (int64_t d : r->shape) have *= static_cast<size_t>(d);
+  if (have != n) return fail(DD_ERR_INVALID, "weight shape mismatch: " + key);
+  int rc;
+  if ((rc = dev_alloc(e, reinterpret_cast<void**>(out), n * 4))) return rc;
+  CUDA_TRY(cudaMemcpyAsync(*out, r->ptr, n * 4, cudaMemcpyDeviceToDevice, st));
+  return DD_OK;
+}
 
 // ------------------------------------------------------------------------------------------------ denoiser + codec pack
 // dd_finalize_weights allocates (alloc_pack) and fills (fill_pack) everything; dd_update_weights validates
@@ -1644,10 +1655,20 @@ int pack_gen_weights(dd_engine* e, std::vector<void*>& owned, GenLayer& L, const
   return DD_OK;
 }
 
-// conv weight key `wkey` ([cout][cin][k][k], or ConvT [cin][co][2][2] when transposed); see pack_gen_weights
+// Where a producer layer's BatchNorm runs in DD_PRODUCER_TRAIN: the call (0 dd_run_backbone, 1 dd_build_condition;
+// -1 not at all) and the pixel count of the pre-BN output (a ConvT's: B x 2H x 2W).
+struct TrainBn {
+  int stage = -1;
+  long long n = 0;
+};
+
+// conv weight key `wkey` ([cout][cin][k][k], or ConvT [cin][co][2][2] when transposed); see pack_gen_weights.  With
+// `train` and DD_FLAG_PRODUCER_TRAIN, the BatchNorm `bnkey` also gets its training-mode record in pt.layers (L.bn): the
+// conv packed unfolded (no BatchNorm, no bias, zero shift) and device copies of gamma / beta.
 int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::string& bnkey, int cin, int cout_conv,
              int taps, bool transposed, cudaStream_t st, float* scratch, int cin_pad = 0,
-             const std::string& biaskey = std::string()) {
+             const std::string& biaskey = std::string(), TrainBn train = TrainBn()) {
+  L.bn = -1;  // the Producers' layers outlive a pack: no index from an earlier one may survive
   const Raw* w = find(e, wkey);
   if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
   const int k = taps == 9 ? 3 : (transposed ? 2 : 1);
@@ -1664,8 +1685,23 @@ int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::stri
     if (!b) return fail(DD_ERR_INVALID, "missing weights: " + biaskey);
     bias = b->ptr;
   }
-  return pack_gen_weights(e, e->owned, L, w->ptr, wkey, bnkey.empty() ? nullptr : bn, bias, cin, cout_conv, taps,
-                          transposed, cin_pad, 0, st, scratch);
+  if ((rc = pack_gen_weights(e, e->owned, L, w->ptr, wkey, bnkey.empty() ? nullptr : bn, bias, cin, cout_conv, taps,
+                             transposed, cin_pad, 0, st, scratch)))
+    return rc;
+  if (train.stage < 0 || !(e->cfg.flags & DD_FLAG_PRODUCER_TRAIN)) return DD_OK;
+  dd_engine::ProdBn b;
+  b.C = cout_conv;
+  b.stage = train.stage;
+  b.n = train.n;
+  b.key = bnkey;
+  if ((rc = pack_gen_weights(e, e->owned, b.raw, w->ptr, wkey, nullptr, nullptr, cin, cout_conv, taps, transposed,
+                             cin_pad, 0, st, scratch)))
+    return rc;
+  if ((rc = copy_param(e, bnkey + ".weight", cout_conv, &b.gamma, st))) return rc;
+  if ((rc = copy_param(e, bnkey + ".bias", cout_conv, &b.beta, st))) return rc;
+  L.bn = static_cast<int>(e->pt.layers.size());
+  e->pt.layers.push_back(b);
+  return DD_OK;
 }
 
 // nn.Linear: weight key `wkey` [N][K], bias key `bkey` (empty: none).  run_gemm supplies the activation.
@@ -1680,25 +1716,33 @@ int pack_linear(dd_engine* e, GenLayer& L, const std::string& wkey, const std::s
                           scratch);
 }
 
+// In evaluation order, which is that of the training-mode records: the neck level by level, then the FPN top-down.
 int pack_producers(dd_engine* e, cudaStream_t st, float* scratch) {
   Producers& p = e->prod;
+  const long long B = e->cfg.batch;
   int rc;
-  for (int i = 0; i < p.nlev; ++i) {
+  for (int i = 0; p.neck && i < p.nlev; ++i) {
+    const std::string si = std::to_string(i), h = "hahineck.";
+    const TrainBn bn = {1, B * p.H[i] * p.W[i]};
+    if ((rc = pack_gen(e, p.lat[i], h + "lateral_convs." + si + ".conv.weight", h + "lateral_convs." + si + ".bn",
+                       p.C[i], p.C[i], 1, false, st, scratch, 0, "", bn))) return rc;
+    const std::string pj = i == 0 ? h + "conv_proj.0" : h + "trans_proj." + std::to_string(i - 1);
+    const std::string fs = i == 0 ? h + "conv_fusion.0" : h + "trans_fusion." + std::to_string(i - 1);
+    if ((rc = pack_gen(e, p.proj[i], pj + ".conv.weight", pj + ".bn", p.C[i], 512, 1, false, st, scratch, 0, "", bn)))
+      return rc;
+    if ((rc = pack_gen(e, p.fus[i], fs + ".conv.weight", fs + ".bn", p.C[i] + 512, p.C[i], 9, false, st, scratch, 0, "",
+                       bn))) return rc;
+  }
+  for (int i = p.nlev - 1; i >= 0; --i) {
     const std::string si = std::to_string(i);
-    if (p.neck) {
-      const std::string h = "hahineck.";
-      if ((rc = pack_gen(e, p.lat[i], h + "lateral_convs." + si + ".conv.weight", h + "lateral_convs." + si + ".bn",
-                         p.C[i], p.C[i], 1, false, st, scratch))) return rc;
-      const std::string pj = i == 0 ? h + "conv_proj.0" : h + "trans_proj." + std::to_string(i - 1);
-      const std::string fs = i == 0 ? h + "conv_fusion.0" : h + "trans_fusion." + std::to_string(i - 1);
-      if ((rc = pack_gen(e, p.proj[i], pj + ".conv.weight", pj + ".bn", p.C[i], 512, 1, false, st, scratch))) return rc;
-      if ((rc = pack_gen(e, p.fus[i], fs + ".conv.weight", fs + ".bn", p.C[i] + 512, p.C[i], 9, false, st, scratch))) return rc;
-    }
+    const long long n = B * p.H[i] * p.W[i];
     if ((rc = pack_gen(e, p.fl[i], "conv_lateral." + si + ".0.weight", "conv_lateral." + si + ".1", p.C[i], 256, 9, false,
-                       st, scratch))) return rc;
-    if (i < p.nlev - 1)
-      if ((rc = pack_gen(e, p.fu[i], "conv_up." + si + ".0.weight", "conv_up." + si + ".1", 256, 256, 1, true, st,
-                         scratch))) return rc;
+                       st, scratch, 0, "", {1, n}))) return rc;
+    if (i > 0) {  // the ConvT from level i up to level i - 1
+      const std::string su = std::to_string(i - 1);
+      if ((rc = pack_gen(e, p.fu[i - 1], "conv_up." + su + ".0.weight", "conv_up." + su + ".1", 256, 256, 1, true, st,
+                         scratch, 0, "", {1, 4 * n}))) return rc;
+    }
   }
   p.ready = true;
   return DD_OK;
@@ -1856,97 +1900,16 @@ int launch_gen(dd_engine* e, const GenLayer& L, int act, const GenGrid& g, const
   return DD_OK;
 }
 
-// H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.
-int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
-            float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
-            int ld_out = 0, int ch_off = 0) {
-  return launch_gen(e, L, L.relu, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, y32, add32, out, ld_out, ch_off,
-                    st, 0, nullptr, e->prod.KS);
-}
-
 // ------------------------------------------------------------------------------------------------ producer BatchNorms
-// DD_PRODUCER_TRAIN (producer_train.cuh).  One BatchNorm'ed layer: the unfolded pack of its conv weight `wkey` (as
-// pack_gen reads it, without the BatchNorm), device copies of gamma / beta of `bnkey`, and its pre-BN output size.
-int add_bn_layer(dd_engine* e, const GenLayer& ev, const std::string& wkey, const std::string& bnkey, int cin,
-                 int cout_conv, int taps, bool transposed, int cin_pad, int stage, long long n, cudaStream_t st,
-                 float* scratch) {
-  dd_engine::ProdBn b;
-  b.eval = &ev;
-  b.C = cout_conv;
-  b.stage = stage;
-  b.n = n;
-  b.key = bnkey;
-  const Raw* w = find(e, wkey);
-  if (!w) return fail(DD_ERR_INVALID, "missing weights: " + wkey);
-  const float* bn[4] = {nullptr, nullptr, nullptr, nullptr};
-  int rc;
-  if ((rc = find_bn(e, bnkey, bn))) return rc;
-  if ((rc = pack_gen_weights(e, e->owned, b.raw, w->ptr, wkey, nullptr, nullptr, cin, cout_conv, taps, transposed,
-                             cin_pad, 0, st, scratch)))
-    return rc;
-  b.raw.stride = ev.stride;
-  if ((rc = dev_array(e, &b.gamma, cout_conv))) return rc;
-  if ((rc = dev_array(e, &b.beta, cout_conv))) return rc;
-  CUDA_TRY(cudaMemcpyAsync(b.gamma, bn[0], cout_conv * 4, cudaMemcpyDeviceToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(b.beta, bn[1], cout_conv * 4, cudaMemcpyDeviceToDevice, st));
-  e->pt.layers.push_back(b);
-  return DD_OK;
-}
-
 int pbn_blocks(long long n) { return static_cast<int>((n + dd::PBN_ROWS - 1) / dd::PBN_ROWS); }
 
-// Every BatchNorm'ed producer layer in evaluation order (after pack_producers / pack_resnet), and the scratch for the
-// largest of them.  DD_FLAG_PRODUCER_TRAIN only.
-int pack_prod_train(dd_engine* e, cudaStream_t st, float* scratch) {
-  dd_engine::ProdTrain& pt = e->pt;  // reset by dd_finalize_weights: the previous pack's buffers went with `owned`
-  const long long B = e->cfg.batch;
-  int rc;
-  if (e->rn.enabled) {
-    ResNetW& r = e->rn;
-    for (int s = 0; s < 4; ++s) {
-      const int cprev = s == 0 ? 3 : r.C[s - 1];
-      const long long n = B * r.Hs[s] * r.Ws[s];
-      for (int b = 0; b < r.depths[s]; ++b) {
-        const std::string bp = "backbone.layers." + std::to_string(s) + "." + std::to_string(b) + ".";
-        const int cin = b == 0 ? cprev : r.C[s];
-        const int pad = (cin % dd::GEN_BK) ? dd::GEN_BK : 0;
-        if ((rc = add_bn_layer(e, r.blocks[s][b].c1, bp + "conv1.weight", bp + "bn1", cin, r.C[s], 9, false, pad, 0, n,
-                               st, scratch))) return rc;
-        if ((rc = add_bn_layer(e, r.blocks[s][b].c2, bp + "conv2.weight", bp + "bn2", r.C[s], r.C[s], 9, false, 0, 0, n,
-                               st, scratch))) return rc;
-      }
-    }
-  }
-  if (e->prod.enabled) {
-    Producers& p = e->prod;
-    for (int i = 0; p.neck && i < p.nlev; ++i) {
-      const std::string si = std::to_string(i), h = "hahineck.";
-      const long long n = B * p.H[i] * p.W[i];
-      const std::string pj = i == 0 ? h + "conv_proj.0" : h + "trans_proj." + std::to_string(i - 1);
-      const std::string fs = i == 0 ? h + "conv_fusion.0" : h + "trans_fusion." + std::to_string(i - 1);
-      if ((rc = add_bn_layer(e, p.lat[i], h + "lateral_convs." + si + ".conv.weight", h + "lateral_convs." + si + ".bn",
-                             p.C[i], p.C[i], 1, false, 0, 1, n, st, scratch))) return rc;
-      if ((rc = add_bn_layer(e, p.proj[i], pj + ".conv.weight", pj + ".bn", p.C[i], 512, 1, false, 0, 1, n, st, scratch)))
-        return rc;
-      if ((rc = add_bn_layer(e, p.fus[i], fs + ".conv.weight", fs + ".bn", p.C[i] + 512, p.C[i], 9, false, 0, 1, n, st,
-                             scratch))) return rc;
-    }
-    for (int i = p.nlev - 1; i >= 0; --i) {
-      const std::string si = std::to_string(i);
-      if ((rc = add_bn_layer(e, p.fl[i], "conv_lateral." + si + ".0.weight", "conv_lateral." + si + ".1", p.C[i], 256, 9,
-                             false, 0, 1, B * p.H[i] * p.W[i], st, scratch))) return rc;
-      if (i > 0) {
-        const std::string su = std::to_string(i - 1);
-        if ((rc = add_bn_layer(e, p.fu[i - 1], "conv_up." + su + ".0.weight", "conv_up." + su + ".1", 256, 256, 1, true, 0,
-                               1, 4 * B * p.H[i] * p.W[i], st, scratch))) return rc;
-      }
-    }
-  }
+// DD_FLAG_PRODUCER_TRAIN (producer_train.cuh): the records' offsets, in the order pack_gen appended them, and the
+// scratch for the largest layer.
+int pack_prod_train(dd_engine* e, cudaStream_t st) {
+  dd_engine::ProdTrain& pt = e->pt;
   size_t u_max = 0, part_max = 0;
   int c_max = 0;
-  for (size_t k = 0; k < pt.layers.size(); ++k) {
-    dd_engine::ProdBn& b = pt.layers[k];
-    pt.index[b.eval] = static_cast<int>(k);
+  for (dd_engine::ProdBn& b : pt.layers) {
     b.rec_off = pt.rec_floats;
     pt.rec_floats += 2 * static_cast<size_t>(b.C);
     u_max = std::max(u_max, static_cast<size_t>(b.n) * b.C);
@@ -1954,6 +1917,7 @@ int pack_prod_train(dd_engine* e, cudaStream_t st, float* scratch) {
     c_max = std::max(c_max, b.C);
   }
   if (pt.layers.empty()) return DD_OK;
+  int rc;
   if ((rc = dev_array(e, &pt.U, u_max))) return rc;
   if ((rc = dev_array(e, &pt.part, part_max))) return rc;
   if ((rc = dev_array(e, &pt.sum1, c_max))) return rc;
@@ -1964,19 +1928,23 @@ int pack_prod_train(dd_engine* e, cudaStream_t st, float* scratch) {
   return DD_OK;
 }
 
-// run_gen for a layer followed by a BatchNorm: in DD_PRODUCER_TRAIN the conv on the unfolded pack into pt.U, the
-// batch statistics and fold (record written), then act(s u + t) with the eval layer's addend and outputs; otherwise
-// the eval layer itself.
-int run_bn_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
-               float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0) {
+// H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.  A layer with a training-mode
+// BatchNorm (L.bn) in DD_PRODUCER_TRAIN runs its conv on the unfolded pack into pt.U, then the batch statistics and fold
+// (record written), then act(s u + t) with L's addend and outputs.
+int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
+            float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
+            int ld_out = 0, int ch_off = 0) {
+  if (L.bn < 0 || e->producer_mode != DD_PRODUCER_TRAIN)
+    return launch_gen(e, L, L.relu, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, y32, add32, out, ld_out,
+                      ch_off, st, 0, nullptr, e->prod.KS);
   dd_engine::ProdTrain& pt = e->pt;
-  const auto it = e->producer_mode == DD_PRODUCER_TRAIN ? pt.index.find(&L) : pt.index.end();
-  if (it == pt.index.end()) return run_gen(e, L, a0, c0, a1, c1, H, W, y32, add32, out, st, src_h, src_w);
-  const dd_engine::ProdBn& b = pt.layers[it->second];
+  const dd_engine::ProdBn& b = pt.layers[L.bn];
   const long long n = static_cast<long long>(e->cfg.batch) * H * W * (L.shuffle ? 4 : 1);
   if (n != b.n) return fail(DD_ERR_INVALID, b.key + ": output grid differs from the packed geometry");
+  GenLayer raw = b.raw;  // the unfolded weights; the layer's shape is L's
+  raw.stride = L.stride;
   int rc;
-  if ((rc = launch_gen(e, b.raw, 0, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, pt.U, nullptr, nullptr, 0, 0,
+  if ((rc = launch_gen(e, raw, 0, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, pt.U, nullptr, nullptr, 0, 0,
                        st, 0, nullptr, e->prod.KS)))
     return rc;
   const int C = b.C, nblk = pbn_blocks(n);
@@ -2002,8 +1970,8 @@ int run_bn_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const 
   a.y32 = y32;
   a.out_hi = out ? out->hi : nullptr;
   a.out_lo = out ? out->lo : nullptr;
-  a.ld_out = C;
-  a.ch_off = 0;
+  a.ld_out = ld_out > 0 ? ld_out : C;
+  a.ch_off = ch_off;
   a.split_scale = kProdScale;
   a.status = e->status;
   dd::pbn_apply_kernel<<<grid_of(static_cast<size_t>(n) * C / 8), 256, 0, st>>>(a);
@@ -2030,14 +1998,17 @@ int pack_resnet(dd_engine* e, cudaStream_t st, float* scratch) {
   for (int s = 0; s < 4; ++s) {
     r.blocks[s].assign(r.depths[s], ResBlockW());
     const int cprev = s == 0 ? 3 : r.C[s - 1];
+    const TrainBn bn = {0, static_cast<long long>(e->cfg.batch) * r.Hs[s] * r.Ws[s]};
     for (int b = 0; b < r.depths[s]; ++b) {
       ResBlockW& W = r.blocks[s][b];
       const std::string bp = "backbone.layers." + std::to_string(s) + "." + std::to_string(b) + ".";
       const int cin = b == 0 ? cprev : r.C[s];
       const int pad = (cin % dd::GEN_BK) ? dd::GEN_BK : 0;
-      if ((rc = pack_gen(e, W.c1, bp + "conv1.weight", bp + "bn1", cin, r.C[s], 9, false, st, scratch, pad))) return rc;
+      if ((rc = pack_gen(e, W.c1, bp + "conv1.weight", bp + "bn1", cin, r.C[s], 9, false, st, scratch, pad, "", bn)))
+        return rc;
       W.c1.stride = b == 0 ? 2 : 1;
-      if ((rc = pack_gen(e, W.c2, bp + "conv2.weight", bp + "bn2", r.C[s], r.C[s], 9, false, st, scratch))) return rc;
+      if ((rc = pack_gen(e, W.c2, bp + "conv2.weight", bp + "bn2", r.C[s], r.C[s], 9, false, st, scratch, 0, "", bn)))
+        return rc;
       W.c2.add_first = 1;  // out = relu(bn2(conv2) + skip)
       W.has_ds = (b == 0);
       if (W.has_ds) {
@@ -2073,7 +2044,7 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
       const int k = b & 1;
       const Planes& in = (b == 0) ? src : r.Yp[cur];
       const int in_c = (b == 0) ? src_c : C;
-      if ((rc = run_bn_gen(e, Wt.c1, in, in_c, none, 0, H, W, nullptr, nullptr, &r.T, st, src_h, src_w))) return rc;
+      if ((rc = run_gen(e, Wt.c1, in, in_c, none, 0, H, W, nullptr, nullptr, &r.T, st, src_h, src_w))) return rc;
       const float* skip;
       if (Wt.has_ds) {
         if ((rc = run_gen(e, Wt.ds, in, in_c, none, 0, H, W, r.D32, nullptr, nullptr, st, src_h, src_w))) return rc;
@@ -2082,7 +2053,7 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
         skip = r.Y32[cur];
       }
       const Planes& outp = last ? e->prod.F[s] : r.Yp[k];
-      if ((rc = run_bn_gen(e, Wt.c2, r.T, C, none, 0, H, W, r.Y32[k], skip, &outp, st))) return rc;
+      if ((rc = run_gen(e, Wt.c2, r.T, C, none, 0, H, W, r.Y32[k], skip, &outp, st))) return rc;
       cur = k;
     }
     if (feats_out && feats_out[s]) {
@@ -2100,18 +2071,6 @@ int run_resnet(dd_engine* e, const float* rgb, float* const* feats_out, cudaStre
 // ------------------------------------------------------------------------------------------------ Swin backbone
 constexpr float kTokScale = 16.f;  // fp16-split pre-scale of token activations (LayerNorm / GELU / attention outputs)
 static_assert(kTokScale == kProdScale, "run_gemm reads token planes at the producers' split scale");
-
-int copy_param(dd_engine* e, const std::string& key, size_t n, float** out, cudaStream_t st) {
-  const Raw* r = find(e, key);
-  if (!r) return fail(DD_ERR_INVALID, "missing weights: " + key);
-  size_t have = 1;
-  for (int64_t d : r->shape) have *= static_cast<size_t>(d);
-  if (have != n) return fail(DD_ERR_INVALID, "weight shape mismatch: " + key);
-  int rc;
-  if ((rc = dev_alloc(e, reinterpret_cast<void**>(out), n * 4))) return rc;
-  CUDA_TRY(cudaMemcpyAsync(*out, r->ptr, n * 4, cudaMemcpyDeviceToDevice, st));
-  return DD_OK;
-}
 
 int pack_backbone(dd_engine* e, cudaStream_t st, float* scratch) {
   Backbone& b = e->bb;
@@ -2820,25 +2779,24 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   h->packed = false;
   for (void* p : h->owned) cudaFree(p);
   h->owned.clear();
+  h->pt = dd_engine::ProdTrain();  // pack_gen appends the training-mode records, the ResNet's before the producers'
   int rc;
   if ((rc = alloc_pack(h, encoder, st))) return rc;
   if ((rc = fill_pack(h, st))) return rc;
   float* scratch = h->amax;
+  h->rn.ready = false;
+  if (h->rn.enabled)
+    if ((rc = pack_resnet(h, st, scratch))) return rc;
   h->prod.ready = false;
   if (h->prod.enabled)
     if ((rc = pack_producers(h, st, scratch))) return rc;
   h->bb.ready = false;
   if (h->bb.enabled)
     if ((rc = pack_backbone(h, st, scratch))) return rc;
-  h->rn.ready = false;
-  if (h->rn.enabled)
-    if ((rc = pack_resnet(h, st, scratch))) return rc;
   h->mp.ready = false;
   if (h->mp.enabled)
     if ((rc = pack_mpvit(h, st, scratch))) return rc;
-  h->pt = dd_engine::ProdTrain();
-  if (h->cfg.flags & DD_FLAG_PRODUCER_TRAIN)
-    if ((rc = pack_prod_train(h, st, scratch))) return rc;
+  if ((rc = pack_prod_train(h, st))) return rc;
   // the registered pointers were borrowed for this call only (include/dd_engine.h): wait for the kernels that read them
   // and forget them, so a later finalize cannot read memory the caller has freed in the meantime
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -3294,22 +3252,22 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
       continue;
     }
     // HAHI neck, attention gates off (reference necks/hahi.py:173-176, 226-250, 253-272)
-    if ((rc = run_bn_gen(h, p.lat[i], p.F[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.L[i], s))) return rc;
-    if ((rc = run_bn_gen(h, p.proj[i], p.L[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.P[i], s))) return rc;
+    if ((rc = run_gen(h, p.lat[i], p.F[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.L[i], s))) return rc;
+    if ((rc = run_gen(h, p.proj[i], p.L[i], p.C[i], none, 0, p.H[i], p.W[i], nullptr, nullptr, &p.P[i], s))) return rc;
     if (i == 0) {  // cat([conv_proj(lat), lat])
-      if ((rc = run_bn_gen(h, p.fus[i], p.P[i], 512, p.L[i], p.C[i], p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
+      if ((rc = run_gen(h, p.fus[i], p.P[i], 512, p.L[i], p.C[i], p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
     } else {       // cat([lat, trans_proj(lat)])
-      if ((rc = run_bn_gen(h, p.fus[i], p.L[i], p.C[i], p.P[i], 512, p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
+      if ((rc = run_gen(h, p.fus[i], p.L[i], p.C[i], p.P[i], 512, p.H[i], p.W[i], nullptr, nullptr, &p.O[i], s))) return rc;
     }
   }
   // FPN top-down (reference head :112-122): x_i = relu(bn(conv3x3(O_i))) + relu(bn(convT2x2(x_{i+1})))
   for (int i = p.nlev - 1; i >= 0; --i) {
     const float* add = (i < p.nlev - 1) ? p.UP[i] : nullptr;
-    if ((rc = run_bn_gen(h, p.fl[i], p.O[i], p.C[i], none, 0, p.H[i], p.W[i], p.X[i], add, i > 0 ? &p.XP[i] : nullptr, s)))
+    if ((rc = run_gen(h, p.fl[i], p.O[i], p.C[i], none, 0, p.H[i], p.W[i], p.X[i], add, i > 0 ? &p.XP[i] : nullptr, s)))
       return rc;
     if (i > 0) {
       float* up_raw = p.resample ? p.UPR[i - 1] : p.UP[i - 1];
-      if ((rc = run_bn_gen(h, p.fu[i - 1], p.XP[i], 256, none, 0, p.H[i], p.W[i], up_raw, nullptr, nullptr, s))) return rc;
+      if ((rc = run_gen(h, p.fu[i - 1], p.XP[i], 256, none, 0, p.H[i], p.W[i], up_raw, nullptr, nullptr, s))) return rc;
       if (p.resample) {  // F.adaptive_avg_pool2d(conv_up(pre_x), output_size = lateral size)  (reference head :121)
         const size_t n = static_cast<size_t>(B) * p.H[i - 1] * p.W[i - 1] * 256;
         dd::adaptive_avg_pool_nhwc_kernel<<<grid_of(n), 256, 0, s>>>(up_raw, p.UP[i - 1], B, 2 * p.H[i], 2 * p.W[i],

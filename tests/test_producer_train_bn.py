@@ -110,6 +110,32 @@ def _cond_err(cond, cond64):
     return ((cond.double() - cond64).abs().max() / cond64.abs().max()).item()
 
 
+def _eval_order(neck, res_depths=(), nlev=4):
+    """Producer BatchNorm keys in evaluation order: the ResNet block by block, then the neck level by level (lateral,
+    proj, fusion), then the FPN top-down (lateral, conv_up)."""
+    keys = [f"backbone.layers.{s}.{b}.bn{j}" for s, d in enumerate(res_depths) for b in range(d) for j in (1, 2)]
+    for i in range(nlev if neck else 0):
+        t, j = ("conv", 0) if i == 0 else ("trans", i - 1)
+        keys += [f"hahineck.lateral_convs.{i}.bn", f"hahineck.{t}_proj.{j}.bn", f"hahineck.{t}_fusion.{j}.bn"]
+    for i in reversed(range(nlev)):
+        keys += [f"conv_lateral.{i}.1"] + ([f"conv_up.{i - 1}.1"] if i else [])
+    return keys
+
+
+def _bn_channels(module, prefix=""):
+    return {prefix + n: m.num_features for n, m in module.named_modules() if isinstance(m, nn.BatchNorm2d)}
+
+
+def _check_record_order(eng, keys, channels):
+    """The records are those of `keys`, in that order, each 2 x C floats, back to back from offset 0."""
+    info = eng.producer_bn_keys()
+    assert [k for k, _, _ in info] == keys
+    off = 0
+    for k, c, o in info:
+        assert (c, o) == (channels[k], off), k
+        off += 2 * c
+
+
 # ------------------------------------------------------------------------------------------------ CPU
 def test_repack_plan_defers_producer_running_stats():
     keys = ["model.pred.0.weight", "hahineck.lateral_convs.0.bn.running_mean", "conv_up.0.1.num_batches_tracked",
@@ -158,6 +184,7 @@ def _cond_case(kind, B, sizes, seed, margins):
     margins.append((kind, sizes[0], "cond", err))
     assert err <= COND_BOUND, err
     assert set(rec) == set(stats)
+    _check_record_order(eng, _eval_order("HAHI" in kind), _bn_channels(head))
     _check_stats(rec, stats, margins, kind)
     # determinism: a second call gives the same bits
     cond2 = eng.build_condition(fp, want_cond=True)
@@ -210,6 +237,8 @@ def test_resnet_backbone_train_mode(img):
     print("res", img, "cond", err)
     assert err <= COND_BOUND, err
     assert set(rec) == set(stats) and len(rec) == 16 + 7
+    _check_record_order(eng, _eval_order(False, res_depths=(2, 2, 2, 2)),
+                        {**_bn_channels(head), **_bn_channels(bb, "backbone.")})
     margins = []
     _check_stats(rec, stats, margins, "res")
     print("res", img, "stats", max(m[2] for m in margins), max(m[3] for m in margins))
