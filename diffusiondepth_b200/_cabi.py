@@ -43,6 +43,8 @@ FLAG_CHAIN_PRED, FLAG_PRODUCER_TRAIN = 1024, 2048
 CODEC_EVAL, CODEC_TRAIN = 0, 1
 PRODUCER_EVAL, PRODUCER_TRAIN = 0, 1
 STATUS = {0: "DD_OK", 1: "DD_ERR_INVALID", 2: "DD_ERR_CUDA", 3: "DD_ERR_UNSUPPORTED", 4: "DD_ERR_RANGE"}
+# dd_allgather_fn: (in, out, count, cuda_stream, user) -> 0 on success
+ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p)
 
 # name -> (restype, argtypes); every symbol include/dd_engine.h declares
 SIGNATURES = {
@@ -86,6 +88,7 @@ SIGNATURES = {
     "dd_producer_batch_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.c_void_p]),
     "dd_producer_bn_info": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int32),
                                       C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "dd_set_bn_allgather": (C.c_int, [C.c_void_p, ALLGATHER_FN, C.c_void_p, C.c_int32]),
     "dd_last_launch_count": (C.c_int64, [C.c_void_p]),
     "dd_poll_status": (C.c_int, [C.c_void_p, C.c_void_p]),
     "dd_conv3x3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,

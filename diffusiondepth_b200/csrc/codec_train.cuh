@@ -6,6 +6,9 @@
 // mean rounded to fp32, so the variance is a mean of squared deviations (no E[u^2] - mean^2 cancellation when
 // |mean| >> std) and sum d corrects the rounding of m.  Every reduction writes fixed per-block fp64 partials that a
 // second kernel sums in block order: the statistics, the folded weights and the gradients are bit-reproducible.
+//
+// Across ranks (dd_set_bn_allgather) every total above is gathered with the local item count and summed in rank order
+// (bn_rank_sum_kernel); the kernels then divide by the global count *cnt instead of their own n (cnt null: n).
 #pragma once
 #include "backward.cuh"
 
@@ -128,17 +131,18 @@ struct EncPreBn2 {
 };
 
 // Per-block sums over the block's BNS_PIX items: columns 0..15 sum d, 16..31 sum d^2, d = u - m.  Pass 1: sum1 null,
-// m = 0; pass 2: m = fp32(sum1 / n).
+// m = 0; pass 2: m = fp32(sum1 / N), N = *cnt or n when cnt is null.
 template <class Op>
 __global__ void __launch_bounds__(256) bn_stats_kernel(const Op op, long long n, const double* __restrict__ sum1,
-                                                       double* __restrict__ part) {
+                                                       const double* __restrict__ cnt, double* __restrict__ part) {
   __shared__ __align__(16) float s_op[Op::SMEM];
   __shared__ double s_red[8][BNS_COLS];
   op.load(s_op);
   __syncthreads();
+  const double N = cnt ? *cnt : static_cast<double>(n);
   float m[16];
 #pragma unroll
-  for (int c = 0; c < 16; ++c) m[c] = sum1 ? static_cast<float>(sum1[c] / static_cast<double>(n)) : 0.f;
+  for (int c = 0; c < 16; ++c) m[c] = sum1 ? static_cast<float>(sum1[c] / N) : 0.f;
   float acc[BNS_COLS];
 #pragma unroll
   for (int j = 0; j < BNS_COLS; ++j) acc[j] = 0.f;
@@ -170,14 +174,27 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const Op op, long long n,
   }
 }
 
-// out[c] = sum over blocks, in block order, of part[b * stride + c], c < ncols (one thread per column)
+// out[c] = sum over blocks, in block order, of part[b * stride + c], c < ncols (one thread per column).  count > 0:
+// out[ncols] = count as well, the row a cross-rank gather sends (the launch then covers ncols + 1 threads).
 __global__ void part_colsum_kernel(const double* __restrict__ part, int nblk, int stride, int ncols,
-                                   double* __restrict__ out) {
-  const int c = threadIdx.x;
+                                   double* __restrict__ out, long long count) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c == ncols && count > 0) out[c] = static_cast<double>(count);
   if (c >= ncols) return;
   double s = 0.0;
   for (int b = 0; b < nblk; ++b) s += part[static_cast<size_t>(b) * stride + c];
   out[c] = s;
+}
+
+// out[j] = rows[0][j] + rows[1][j] + ... + rows[R - 1][j], added in rank order, j < cols: the gathered per-rank totals
+// of a cross-rank BatchNorm (count last), so every rank folds the same union-batch statistics, bit for bit.
+__global__ void __launch_bounds__(256) bn_rank_sum_kernel(const double* __restrict__ rows, int R, int cols,
+                                                          double* __restrict__ out) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= cols) return;
+  double s = rows[j];
+  for (int r = 1; r < R; ++r) s += rows[static_cast<size_t>(r) * cols + j];
+  out[j] = s;
 }
 
 // Fold the batch statistics of pass 2 into a copy of one conv's weights:
@@ -190,6 +207,7 @@ struct BnFoldArgs {
   const double* part;  // [nblk][BNS_COLS] pass-2 partials
   int nblk;
   long long n;
+  const double* cnt;   // null, or the global item count across ranks (used instead of n)
   const float *gamma, *beta;
   const float* bias;  // the conv's own bias in front of the BatchNorm, not in the statistics (null: none)
   const float* w;     // unfolded weights, output channel fastest
@@ -208,7 +226,7 @@ __global__ void __launch_bounds__(256) bn_fold_kernel(const BnFoldArgs f) {
       d1 += f.part[static_cast<size_t>(b) * BNS_COLS + c];
       d2 += f.part[static_cast<size_t>(b) * BNS_COLS + 16 + c];
     }
-    const double nn = static_cast<double>(f.n);
+    const double nn = f.cnt ? *f.cnt : static_cast<double>(f.n);
     const double dm = d1 / nn;  // mean of d: the rounding of the shift
     const double mean_conv = static_cast<double>(static_cast<float>(f.sum1[c] / nn)) + dm;
     const double mean = mean_conv + (f.bias ? static_cast<double>(f.bias[c]) : 0.0);
@@ -236,20 +254,22 @@ __global__ void __launch_bounds__(256) bn_fold_kernel(const BnFoldArgs f) {
 // sums[32] their totals over the N output pixels, du becomes s (dv - sum dv / N - xhat sum(dv xhat) / N), xhat = (u -
 // mean) rstd recomputed from the bias-free u in dec_bwd_act_kernel's order (the same xhat); the per-block sums of the
 // new du (the ConvT bias gradient, zero up to rounding) go to part_db [blocks][16].
-// Same block decomposition as dec_bwd_act_kernel.
+// Same block decomposition as dec_bwd_act_kernel.  Across ranks sums are the union batch's and *cnt its pixel count
+// (cnt null: the local N).
 __global__ void __launch_bounds__(256) dec_bwd_bn_kernel(const DecBwdArgs a, const double* __restrict__ sums,
-                                                         double* __restrict__ part_db) {
+                                                         const double* __restrict__ cnt, double* __restrict__ part_db) {
   __shared__ __align__(16) float s_op[DecPreBn::SMEM];
   __shared__ double s_red[8][16];
   const DecPreBn op{a.x, a.wu, a.h, a.w};
   op.load(s_op);
   __syncthreads();
   const long long N = static_cast<long long>(a.B) * 4 * a.h * a.w;
+  const double NN = cnt ? *cnt : static_cast<double>(N);
   float ka[16], kb[16], acc[16];
 #pragma unroll
   for (int c = 0; c < 16; ++c) {
-    ka[c] = static_cast<float>(sums[c] / static_cast<double>(N));
-    kb[c] = static_cast<float>(sums[16 + c] / static_cast<double>(N));
+    ka[c] = static_cast<float>(sums[c] / NN);
+    kb[c] = static_cast<float>(sums[16 + c] / NN);
     acc[c] = 0.f;
   }
   const long long base = static_cast<long long>(blockIdx.x) * DEC_ACT_PIX;

@@ -493,6 +493,16 @@ struct dd_engine {
     float *s = nullptr, *t = nullptr, *rec = nullptr;  // batch scale / shift [C]; records
     size_t rec_floats = 0;
   } pt;
+  // dd_set_bn_allgather: every training-mode BatchNorm takes the statistics of the union of all ranks' batches.  Each
+  // statistics pass sends this rank's totals and pixel count (`row`) through `fn`; the gathered rows are summed in rank
+  // order into tot1 (pass 1, and the decoder backward) or tot2 (pass 2), which the fold kernels read as one block.
+  struct BnSync {
+    dd_allgather_fn fn = nullptr;
+    void* user = nullptr;
+    int world = 1;
+    int cap = 0;  // doubles per row the buffers hold (grown on first use by a wider layer)
+    double *row = nullptr, *rows = nullptr, *tot1 = nullptr, *tot2 = nullptr;  // [cap], [world][cap], [cap], [cap]
+  } sync;
   std::vector<void*> owned;
   // schedule
   std::vector<int64_t> ts;
@@ -642,6 +652,49 @@ int dec_wc_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(
 int dec_wt_blocks(const Geom& g) { return static_cast<int>((static_cast<size_t>(g.B) * g.P + dd::DEC_WT_PIX - 1) / dd::DEC_WT_PIX); }
 // blocks of bn_stats_kernel over n items (the decoder's B x 2h x 2w is the largest codec BatchNorm)
 int codec_stats_blocks(long long n) { return static_cast<int>((n + dd::BNS_PIX - 1) / dd::BNS_PIX); }
+
+void free_bn_sync(dd_engine* e) {
+  dd_engine::BnSync& s = e->sync;
+  for (double* p : {s.row, s.rows, s.tot1, s.tot2})
+    if (p) cudaFree(p);
+  s.row = s.rows = s.tot1 = s.tot2 = nullptr;
+  s.cap = 0;
+}
+
+// Across ranks (dd_set_bn_allgather), before a BatchNorm's first gather: room for rows of `cols` doubles.  The first
+// BatchNorm with wider rows waits for the old buffers' readers and grows them (tot1 / tot2 hold nothing across
+// BatchNorms).
+int bn_sync_reserve(dd_engine* e, int cols, cudaStream_t st) {
+  dd_engine::BnSync& s = e->sync;
+  if (cols > s.cap) {
+    CUDA_TRY(cudaStreamSynchronize(st));
+    free_bn_sync(e);
+    const size_t b = static_cast<size_t>(cols) * sizeof(double);
+    if (cudaMalloc(&s.row, b) != cudaSuccess || cudaMalloc(&s.rows, b * s.world) != cudaSuccess ||
+        cudaMalloc(&s.tot1, b) != cudaSuccess || cudaMalloc(&s.tot2, b) != cudaSuccess) {
+      free_bn_sync(e);
+      return fail(DD_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(cudaGetLastError()));
+    }
+    s.cap = cols;
+  }
+  return DD_OK;
+}
+
+// Across ranks: this rank's totals over nblk partial rows (stride doubles apart, ncols columns) and its item count n go
+// out as one row; tot2 (second) or tot1 [0 .. ncols] = every rank's row summed in rank order (the count last).  The
+// BatchNorm reserved ncols + 1 columns.
+int bn_sync_totals(dd_engine* e, const double* part, int nblk, int stride, int ncols, long long n, bool second,
+                   cudaStream_t st) {
+  dd_engine::BnSync& s = e->sync;
+  const int cols = ncols + 1;
+  int rc;
+  dd::part_colsum_kernel<<<(cols + 255) / 256, 256, 0, st>>>(part, nblk, stride, ncols, s.row, n);
+  if ((rc = launched(e, "part_colsum"))) return rc;
+  const int r = s.fn(s.row, s.rows, cols, st, s.user);
+  if (r != 0) return fail(DD_ERR_CUDA, "BatchNorm statistics all-gather callback failed (returned " + std::to_string(r) + ")");
+  dd::bn_rank_sum_kernel<<<(cols + 255) / 256, 256, 0, st>>>(s.rows, s.world, cols, second ? s.tot2 : s.tot1);
+  return launched(e, "bn_rank_sum");
+}
 
 void drop_graph(dd_engine* e, int which) {
   if (e->graphs[which]) {
@@ -1088,19 +1141,28 @@ template <class Op>
 int run_bn_batch(dd_engine* e, const Op& op, long long n, const float* gb, const float* bias, const float* w, int nw,
                  float* w_out, float* b_out, float* bn_out, float* rec, cudaStream_t st) {
   dd_engine::CodecTrain& ct = e->ct;
+  const dd_engine::BnSync& sy = e->sync;
   const int nblk = codec_stats_blocks(n);
   int rc;
-  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, nullptr, ct.part);
+  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, nullptr, nullptr, ct.part);
   if ((rc = launched(e, "bn_stats"))) return rc;
-  dd::part_colsum_kernel<<<1, 32, 0, st>>>(ct.part, nblk, dd::BNS_COLS, 16, ct.sum1);
-  if ((rc = launched(e, "part_colsum"))) return rc;
-  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, ct.sum1, ct.part);
+  if (sy.fn) {
+    if ((rc = bn_sync_reserve(e, dd::BNS_COLS + 1, st))) return rc;
+    if ((rc = bn_sync_totals(e, ct.part, nblk, dd::BNS_COLS, 16, n, false, st))) return rc;
+  } else {
+    dd::part_colsum_kernel<<<1, 32, 0, st>>>(ct.part, nblk, dd::BNS_COLS, 16, ct.sum1, 0);
+    if ((rc = launched(e, "part_colsum"))) return rc;
+  }
+  const double* sum1 = sy.fn ? sy.tot1 : ct.sum1;
+  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, sum1, sy.fn ? sy.tot1 + 16 : nullptr, ct.part);
   if ((rc = launched(e, "bn_stats"))) return rc;
+  if (sy.fn && (rc = bn_sync_totals(e, ct.part, nblk, dd::BNS_COLS, dd::BNS_COLS, n, true, st))) return rc;
   dd::BnFoldArgs f;
-  f.sum1 = ct.sum1;
-  f.part = ct.part;
-  f.nblk = nblk;
+  f.sum1 = sum1;
+  f.part = sy.fn ? sy.tot2 : ct.part;  // across ranks the union's totals, as one block of partials
+  f.nblk = sy.fn ? 1 : nblk;
   f.n = n;
+  f.cnt = sy.fn ? sy.tot2 + dd::BNS_COLS : nullptr;
   f.gamma = gb;
   f.beta = gb + 16;
   f.bias = bias;
@@ -1949,14 +2011,24 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
     return rc;
   const int C = b.C, nblk = pbn_blocks(n);
   const dim3 grid(nblk, (C + dd::PBN_CH - 1) / dd::PBN_CH), block(dd::PBN_CH, 8);
-  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, nullptr, pt.part);
+  const dd_engine::BnSync& sy = e->sync;
+  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, nullptr, nullptr, pt.part);
   if ((rc = launched(e, "pbn_stats"))) return rc;
-  dd::pbn_colsum_kernel<<<(C + 255) / 256, 256, 0, st>>>(pt.part, nblk, C, pt.sum1);
-  if ((rc = launched(e, "pbn_colsum"))) return rc;
-  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, pt.sum1, pt.part);
+  if (sy.fn) {
+    if ((rc = bn_sync_reserve(e, 2 * C + 1, st))) return rc;
+    if ((rc = bn_sync_totals(e, pt.part, nblk, 2 * C, C, n, false, st))) return rc;
+  } else {
+    dd::pbn_colsum_kernel<<<(C + 255) / 256, 256, 0, st>>>(pt.part, nblk, C, pt.sum1);
+    if ((rc = launched(e, "pbn_colsum"))) return rc;
+  }
+  const double* sum1 = sy.fn ? sy.tot1 : pt.sum1;
+  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, sum1, sy.fn ? sy.tot1 + C : nullptr, pt.part);
   if ((rc = launched(e, "pbn_stats"))) return rc;
-  dd::pbn_fold_kernel<<<(C + 255) / 256, 256, 0, st>>>(pt.sum1, pt.part, nblk, n, C, b.gamma, b.beta, pt.s, pt.t,
-                                                        pt.rec + b.rec_off);
+  if (sy.fn && (rc = bn_sync_totals(e, pt.part, nblk, 2 * C, 2 * C, n, true, st))) return rc;
+  // across ranks the fold reads the union's totals [2][C] as one block of partials
+  dd::pbn_fold_kernel<<<(C + 255) / 256, 256, 0, st>>>(sum1, sy.fn ? sy.tot2 : pt.part, sy.fn ? 1 : nblk, n,
+                                                        sy.fn ? sy.tot2 + 2 * C : nullptr, C, b.gamma, b.beta, pt.s,
+                                                        pt.t, pt.rec + b.rec_off);
   if ((rc = launched(e, "pbn_fold"))) return rc;
   dd::PbnApplyArgs a;
   a.u = pt.U;
@@ -2500,10 +2572,17 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
   a.w = g.w;
   dd::dec_bwd_act_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a);
   if ((rc = launched(e, "dec_bwd_act"))) return rc;
-  if (train) {  // du through the batch mean and variance
-    dd::part_colsum_kernel<<<1, 32, 0, st>>>(l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, e->ct.sums);
-    if ((rc = launched(e, "part_colsum"))) return rc;
-    dd::dec_bwd_bn_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a, e->ct.sums, e->ct.part_db);
+  if (train) {  // du through the batch mean and variance (across ranks: the union batch's sums and count)
+    const dd_engine::BnSync& sy = e->sync;
+    if (sy.fn) {
+      if ((rc = bn_sync_reserve(e, 33, st))) return rc;
+      if ((rc = bn_sync_totals(e, l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, nout, false, st))) return rc;
+    } else {
+      dd::part_colsum_kernel<<<1, 32, 0, st>>>(l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, e->ct.sums, 0);
+      if ((rc = launched(e, "part_colsum"))) return rc;
+    }
+    dd::dec_bwd_bn_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a, sy.fn ? sy.tot1 : e->ct.sums,
+                                                            sy.fn ? sy.tot1 + 32 : nullptr, e->ct.part_db);
     if ((rc = launched(e, "dec_bwd_bn"))) return rc;
   }
   if (dx != nullptr) {
@@ -2614,6 +2693,7 @@ void release(dd_engine* e) {
   cudaSetDevice(e->cfg.device);
   drop_graphs(e);
   for (void* p : e->owned) cudaFree(p);
+  free_bn_sync(e);
   if (e->status_host) cudaFreeHost(e->status_host);
   if (e->stage) cudaFreeHost(e->stage);
   if (e->pack_done) cudaEventDestroy(e->pack_done);
@@ -2867,6 +2947,9 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
   const size_t map_elems = static_cast<size_t>(g.B) * g.P * 4;  // one decoded batch [B][2h][2w]
   const bool steps = depth_steps_out != nullptr;
   const bool train = h->codec_mode == DD_CODEC_TRAIN;  // batch statistics before every decode, one record each
+  if (steps && train && h->sync.fn)
+    return fail(DD_ERR_UNSUPPORTED, "dd_denoise_decode_steps in DD_CODEC_TRAIN does not run with a BatchNorm all-gather "
+                                    "installed (dd_set_bn_allgather)");
   h->ct.nrec = 0;
   auto loop = [&](cudaStream_t s) -> int {
     for (int i = 0; i < T; ++i) {
@@ -3153,6 +3236,18 @@ int dd_codec_batch_stats(dd_handle h, float* dev_out, int32_t capacity, int32_t*
   return DD_OK;
 }
 
+int dd_set_bn_allgather(dd_handle h, dd_allgather_fn fn, void* user, int32_t world_size) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  if (fn && world_size < 1) return fail(DD_ERR_INVALID, "world_size must be at least 1");
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  CUDA_TRY(cudaDeviceSynchronize());  // earlier gathers may still read the buffers
+  free_bn_sync(h);
+  h->sync.fn = fn;
+  h->sync.user = fn ? user : nullptr;
+  h->sync.world = fn ? world_size : 1;
+  return DD_OK;
+}
+
 int dd_set_producer_mode(dd_handle h, int32_t mode) {
   if (!h) return fail(DD_ERR_INVALID, "null handle");
   if (mode != DD_PRODUCER_EVAL && mode != DD_PRODUCER_TRAIN)
@@ -3278,9 +3373,10 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
   }
   return DD_OK;
   };
-  // every pointer of the neck / FPN kernels lives in the workspace -> replayable as a graph
+  // every pointer of the neck / FPN kernels lives in the workspace -> replayable as a graph; with a BatchNorm all-gather
+  // installed the training-mode launches run eagerly (the gathers are host calls)
   const bool train = h->producer_mode == DD_PRODUCER_TRAIN;
-  if (h->cfg.flags & DD_FLAG_CUDA_GRAPH) {
+  if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !(train && h->sync.fn)) {
     if ((rc = graph_run(h, train ? dd_engine::G_COND_TRAIN : dd_engine::G_COND, st, build))) return rc;
   } else if ((rc = build(st))) {
     return rc;
@@ -3402,7 +3498,7 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
   const bool train = resnet && h->producer_mode == DD_PRODUCER_TRAIN;
   bool want_out = false;
   for (int i = 0; feats_out && i < 4; ++i) want_out |= (feats_out[i] != nullptr);
-  if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !want_out) {
+  if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !want_out && !(train && h->sync.fn)) {
     // the graph's kernels read the image from the workspace: stage the caller's batch there first (20 MB at C3)
     const size_t n = static_cast<size_t>(h->cfg.batch) * 3 *
                      (swin ? h->bb.H * h->bb.W : (resnet ? h->rn.H * h->rn.W : h->mp.H * h->mp.W));

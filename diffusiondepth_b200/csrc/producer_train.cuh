@@ -7,6 +7,10 @@
 // Statistics take two passes over u, as codec_train.cuh does: pass 1 sums u, pass 2 sums d = u - m and d^2 with m =
 // the pass-1 mean rounded to fp32, so the variance is a mean of squared deviations and sum d corrects the rounding of
 // m.  Each block writes fixed fp64 partials that are summed in block order: bit-reproducible.
+//
+// Across ranks (dd_set_bn_allgather) the pass totals are gathered with the local pixel count and summed in rank order
+// (bn_rank_sum_kernel), and `cnt` points at the global count: the mean and variance are the union batch's.  cnt null:
+// the local n, as on one GPU.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -16,12 +20,14 @@ constexpr int PBN_ROWS = 512;  // pixels per block of pbn_stats_kernel (64 per t
 constexpr int PBN_CH = 32;     // channels per block (one per lane)
 
 // grid (ceil(n / PBN_ROWS), ceil(C / PBN_CH)), block (32, 8).  part [blocks.x][2][C]: sum d, sum d^2 of the block's
-// pixels, d = u - m with m = 0 (pass 1, sum1 null) or fp32(sum1[c] / n) (pass 2).
+// pixels, d = u - m with m = 0 (pass 1, sum1 null) or fp32(sum1[c] / N) (pass 2), N = *cnt, or n when cnt is null.
 __global__ void __launch_bounds__(256) pbn_stats_kernel(const float* __restrict__ u, long long n, int C,
-                                                        const double* __restrict__ sum1, double* __restrict__ part) {
+                                                        const double* __restrict__ sum1, const double* __restrict__ cnt,
+                                                        double* __restrict__ part) {
   const int c = blockIdx.y * PBN_CH + threadIdx.x;
   const bool ok = c < C;
-  const float m = (sum1 && ok) ? static_cast<float>(sum1[c] / static_cast<double>(n)) : 0.f;
+  const double N = cnt ? *cnt : static_cast<double>(n);
+  const float m = (sum1 && ok) ? static_cast<float>(sum1[c] / N) : 0.f;
   float s = 0.f, q = 0.f;
   const long long base = static_cast<long long>(blockIdx.x) * PBN_ROWS;
   if (ok) {
@@ -56,9 +62,11 @@ __global__ void __launch_bounds__(256) pbn_colsum_kernel(const double* __restric
 }
 
 // From the pass-2 partials: s = gamma / sqrt(var_b + 1e-5) in fp64, rounded once, t = beta - s mean, and the record
-// [2][C] (batch mean, unbiased batch variance) that the caller's running update reads.
+// [2][C] (batch mean, unbiased batch variance) that the caller's running update reads.  The count is *cnt, or n when
+// cnt is null.
 __global__ void __launch_bounds__(256) pbn_fold_kernel(const double* __restrict__ sum1, const double* __restrict__ part,
-                                                       int nblk, long long n, int C, const float* __restrict__ gamma,
+                                                       int nblk, long long n, const double* __restrict__ cnt, int C,
+                                                       const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, float* __restrict__ s_out,
                                                        float* __restrict__ t_out, float* __restrict__ rec) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -68,7 +76,7 @@ __global__ void __launch_bounds__(256) pbn_fold_kernel(const double* __restrict_
     d1 += part[(static_cast<size_t>(b) * 2) * C + c];
     d2 += part[(static_cast<size_t>(b) * 2 + 1) * C + c];
   }
-  const double nn = static_cast<double>(n);
+  const double nn = cnt ? *cnt : static_cast<double>(n);
   const double dm = d1 / nn;  // mean of d: the rounding of the shift
   const double mean = static_cast<double>(static_cast<float>(sum1[c] / nn)) + dm;
   const double var = fmax(d2 / nn - dm * dm, 0.0);
@@ -76,7 +84,7 @@ __global__ void __launch_bounds__(256) pbn_fold_kernel(const double* __restrict_
   s_out[c] = static_cast<float>(sc);
   t_out[c] = static_cast<float>(static_cast<double>(beta[c]) - mean * sc);
   rec[c] = static_cast<float>(mean);
-  rec[C + c] = static_cast<float>(n > 1 ? var * nn / (nn - 1.0) : var);
+  rec[C + c] = static_cast<float>(nn > 1.0 ? var * nn / (nn - 1.0) : var);
 }
 
 // y = act(s u + t) over n pixels of C channels (C % 8 == 0), eight channels per item, with the eval epilogue's addend

@@ -87,6 +87,14 @@ def ddim_coefficients(alphas_cumprod: torch.Tensor, num_inference_steps: int, nu
     return ts, cx, ce
 
 
+class _DeviceDoubles:
+    """`count` fp64 values at device address `ptr`, viewable as a tensor through __cuda_array_interface__."""
+
+    def __init__(self, ptr: int, count: int):
+        self.__cuda_array_interface__ = {"shape": (int(count),), "typestr": "<f8", "data": (int(ptr), False),
+                                         "version": 3, "strides": None}
+
+
 class WorkspacePool:
     """One growing device buffer shared by several engines that never run concurrently (the engines of one head):
     a ragged last batch or a second image size then costs packed weights only, not another workspace (1.3 GB at C3)."""
@@ -142,6 +150,9 @@ class DenoiseEngine:
         self._keep = []  # fp32 contiguous copies handed to dd_set_weight must outlive finalize
         self.producers = None
         self.backbone = None
+        self.bn_allgather_group = None  # the process group set_bn_allgather installed
+        self.bn_allgather_error: Optional[BaseException] = None  # what the last failed gather raised
+        self._allgather = None  # the installed ctypes callback: must outlive its installation
 
     # ---------------------------------------------------------------- setup
     def load_weights(self, tensors: Dict[str, torch.Tensor]):
@@ -469,6 +480,44 @@ class DenoiseEngine:
         n = C.c_int32()
         _cabi.check(self.lib.dd_producer_batch_stats(self._h, _ptr(rec), total, C.byref(n), C.c_void_p(self._stream())))
         return {k: (rec[o:o + c], rec[o + c:o + 2 * c]) for k, c, o, f in info if f}
+
+    def set_bn_allgather(self, group):
+        """Synchronised BatchNorm (dd_set_bn_allgather): with a torch.distributed process group, every BatchNorm this
+        engine runs on batch statistics (`set_codec_mode(True)`, `set_producer_mode(True)`) normalises with the
+        statistics of all the group's ranks' batches together, and every rank gets the same records bit for bit.  Every
+        rank must then make the same engine calls in the same order.  NCCL gathers on the engine's stream, other
+        backends (gloo) through host memory.  None (the default) turns it off.  A gather that raises fails the engine
+        call with EngineError (the exception is kept in `bn_allgather_error`); the engine stays usable."""
+        if group is None:
+            _cabi.check(self.lib.dd_set_bn_allgather(self._h, _cabi.ALLGATHER_FN(), None, 0))
+            self._allgather, self.bn_allgather_group = None, None
+            return
+        import torch.distributed as dist
+        world = dist.get_world_size(group)
+        nccl = dist.get_backend(group) == "nccl"
+        device = self.device
+
+        def gather(inp, out, count, stream, _user):
+            try:
+                src = torch.as_tensor(_DeviceDoubles(inp, count), device=device)
+                dst = torch.as_tensor(_DeviceDoubles(out, world * count), device=device)
+                cur = torch.cuda.current_stream(device)
+                st = cur if cur.cuda_stream == (stream or 0) else torch.cuda.ExternalStream(stream, device=device)
+                with torch.cuda.stream(st):
+                    if nccl:
+                        dist.all_gather_into_tensor(dst, src, group=group)
+                    else:  # synchronous copies through the host, in order on the engine's stream
+                        rows = [torch.empty(count, dtype=torch.float64) for _ in range(world)]
+                        dist.all_gather(rows, src.cpu(), group=group)
+                        dst.copy_(torch.cat(rows))
+                return 0
+            except Exception as e:  # noqa: BLE001 - any failure becomes the engine call's error
+                self.bn_allgather_error = e
+                return 1
+
+        fn = _cabi.ALLGATHER_FN(gather)
+        _cabi.check(self.lib.dd_set_bn_allgather(self._h, fn, None, world))
+        self._allgather, self.bn_allgather_group = fn, group
 
     def decode(self, latent: torch.Tensor, want_logits=False):
         B, (h, w) = self.batch, self.latent_hw

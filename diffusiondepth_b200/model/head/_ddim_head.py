@@ -244,6 +244,13 @@ class DDIMHeadBase(nn.Module):
     # backbone in training mode runs in torch (its BatchNorms are not covered).  Off by default: the producers then run
     # on their running statistics in every mode.
     producer_train_bn = False
+    # Synchronised BatchNorm across ranks (reference src/main.py:128, apex `convert_syncbn_model`): a torch.distributed
+    # process group, or None (the default: each rank's own batch).  When set, every BatchNorm that `codec_train_bn` /
+    # `producer_train_bn` run in training mode normalises with the statistics of all the group's ranks' batches
+    # together, its decoder backward reduces over all of them, and every rank records the same statistics, so the
+    # running statistics stay identical on every rank.  Every rank must run the same forwards.  The *Vis heads do not
+    # support it (their step decodes run inside one CUDA graph).
+    bn_sync_group = None
 
     def __init__(self, in_channels=None, up_scale_factor=1, inference_steps=20, num_train_timesteps=1000,
                  return_indices=None, depth_transform_cfg=None, detach_fp=False, depth_embed_dim=16,
@@ -300,6 +307,9 @@ class DDIMHeadBase(nn.Module):
         memo[id(self)] = new
         for k, v in self.__dict__.items():
             if k in ("_engines", "_packed", "_pools", "_backbone_ref", "_lock", "_stale"):
+                continue
+            if k == "bn_sync_group":  # a process group is shared, not copied
+                new.__dict__[k] = v
                 continue
             new.__dict__[k] = copy.deepcopy(v, memo)
         new.__dict__['_backbone_ref'] = None
@@ -494,6 +504,8 @@ class DDIMHeadBase(nn.Module):
                 self._stale.discard(old_key)
         else:
             self._engines.move_to_end(key)
+        if getattr(eng, "bn_allgather_group", None) is not self.bn_sync_group:  # every engine follows bn_sync_group
+            eng.set_bn_allgather(self.bn_sync_group)
         # Re-pack when a parameter changed.  The ~500 tensors are walked once per pack; per forward only their
         # (data_ptr, _version) pairs are compared (0.3 ms instead of 2.6 ms for a Swin-L model).
         packed = self._packed.get(key)
@@ -654,6 +666,8 @@ class DDIMHeadBase(nn.Module):
         differentiable `cond` to the operator itself, `self.model(noisy, t, cond)`, whose backward also returns d_cond.
         With `grad_through_loop = True`, `pred` and the final latent are differentiable too (denoiser and decoder
         parameters, through every step: `_LoopFunction`)."""
+        if self.bn_sync_group is not None and self.return_intermediates:
+            raise EngineError("bn_sync_group is not supported by the *Vis heads (their step decodes run in one CUDA graph)")
         with_backbone = fp is None
         if with_backbone:
             B, dev, dtype = image.shape[0], image.device, torch.float32

@@ -361,6 +361,22 @@ int dd_producer_batch_stats(dd_handle h, float* dev_out, int64_t capacity, int32
 int dd_producer_bn_info(dd_handle h, int32_t i, char* key, int32_t key_capacity, int32_t* channels, int64_t* offset,
                         int32_t* fresh);
 
+/* Cross-rank all-gather of BatchNorm statistics: fill out[world_size][count] with every rank's in[count], ordered by
+ * rank, in stream order on cuda_stream (in and out are device memory the engine owns); return 0 on success.  Every
+ * rank must make the same sequence of calls with the same counts. */
+typedef int (*dd_allgather_fn)(const double* in, double* out, int64_t count, void* cuda_stream, void* user);
+
+/* Synchronised BatchNorm (as apex's SyncBatchNorm): with fn installed, every BatchNorm that runs on batch statistics
+ * (DD_CODEC_TRAIN, DD_PRODUCER_TRAIN) normalises with the statistics of the union of all world_size ranks' batches,
+ * which may be ragged.  Each statistics pass gathers this rank's fp64 totals with its pixel count and sums the gathered
+ * rows in rank order, so every rank folds and records the same values bit for bit: the mean and variance of the union,
+ * the unbiased variance with N = the union's pixel count.  Gathers per BatchNorm: two in the forward, one in the
+ * decoder backward (its sum dv and sum dv xhat over the union).  While fn is installed the training-mode producer
+ * calls run their launches eagerly instead of from their CUDA graphs, and dd_denoise_decode_steps in DD_CODEC_TRAIN
+ * returns DD_ERR_UNSUPPORTED.  A non-zero return of fn fails the call with DD_ERR_CUDA; the engine stays usable.
+ * fn = NULL (the default) turns it off: nothing changes.  Synchronises the device. */
+int dd_set_bn_allgather(dd_handle h, dd_allgather_fn fn, void* user, int32_t world_size);
+
 /* Synchronise `cuda_stream` and report DD_ERR_RANGE if any activation left the fp16 split's range since the
  * last hot-path call started (DD_OK otherwise).  The hot-path calls themselves never synchronise unless
  * DD_FLAG_CHECK_RANGE is set. */
