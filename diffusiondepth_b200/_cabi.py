@@ -26,7 +26,8 @@ class DDProducerConfig(C.Structure):
 class DDBackboneConfig(C.Structure):
     _fields_ = [("kind", C.c_int32), ("embed_dims", C.c_int32), ("depths", C.c_int32 * 4),
                 ("num_heads", C.c_int32 * 4), ("window", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
-                ("mp_dims", C.c_int32 * 4), ("mp_paths", C.c_int32 * 4), ("mlp_ratio", C.c_int32)]
+                ("mp_dims", C.c_int32 * 4), ("mp_paths", C.c_int32 * 4), ("mlp_ratio", C.c_int32),
+                ("mp_drop_path", C.c_int32 * 4)]
 
 
 class DDGenLayerDesc(C.Structure):
@@ -35,7 +36,7 @@ class DDGenLayerDesc(C.Structure):
                                          "ch_off", "n_tile", "alt_tile")]
 
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
 FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD, FLAG_LOOP_BACKWARD = 64, 128, 256, 512
@@ -85,6 +86,7 @@ SIGNATURES = {
     "dd_set_codec_mode": (C.c_int, [C.c_void_p, C.c_int32]),
     "dd_codec_batch_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
     "dd_set_producer_mode": (C.c_int, [C.c_void_p, C.c_int32]),
+    "dd_set_drop_path": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "dd_producer_batch_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32), C.c_void_p]),
     "dd_producer_bn_info": (C.c_int, [C.c_void_p, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_int32),
                                       C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),

@@ -378,6 +378,8 @@ struct DwLayer {
   int C = 0, K = 3;
   float* w = nullptr;     // [K*K][C], eval-BN scale folded in
   float* bias = nullptr;  // [C]
+  int bn = -1;            // index of its training-mode BatchNorm record in dd_engine::pt.layers (-1: none)
+  float *raw_w = nullptr, *raw_bias = nullptr;  // with a record: the weights unfolded, and a zero bias
 };
 struct MpBlockW {
   float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
@@ -407,6 +409,12 @@ struct MPViTW {
   int Hs[4] = {0, 0, 0, 0}, Ws[4] = {0, 0, 0, 0};
   GenLayer stem0, stem1;
   MpStageW stage[4];
+  // stochastic depth (dd_set_drop_path): bit l of drop_mask[s] marks stage s's encoder layer l (in every path) as having
+  // a DropPath on its two residual branches; drop_blocks counts those blocks.  While drop_on, drop_scales holds
+  // [block][attention, MLP][B] per-sample scales, blocks in stage, path, layer order.
+  int drop_mask[4] = {0, 0, 0, 0}, drop_blocks = 0;
+  bool drop_on = false;
+  float* drop_scales = nullptr;
   // workspace views
   Planes IN, S1, D, EP0, AP, HP, CAT;
   float* XS = nullptr;      // stem output, then each stage's output (fp32 NHWC)
@@ -541,10 +549,11 @@ struct dd_engine {
   // CUDA graphs (DD_FLAG_CUDA_GRAPH), captured on first use and replayed: the T-step loop, the same loop with a decode
   // after every step (dd_denoise_decode_steps), the native backbone, the neck + FPN
   // (G_LOOP_STEPS_TRAIN: the step-decode loop in DD_CODEC_TRAIN, batch statistics before every decode)
-  // (G_BACKBONE_TRAIN, G_COND_TRAIN: the ResNet backbone and the neck + FPN in DD_PRODUCER_TRAIN)
+  // (G_BACKBONE_TRAIN, G_COND_TRAIN: the native backbone and the neck + FPN in DD_PRODUCER_TRAIN; G_BACKBONE_DROP,
+  // G_BACKBONE_TRAIN_DROP: the MPViT backbone with stochastic depth on, in either producer mode)
   enum {
     G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_LOOP_STEPS_TRAIN = 4, G_BACKBONE_TRAIN = 5,
-    G_COND_TRAIN = 6, G_COUNT = 7
+    G_COND_TRAIN = 6, G_BACKBONE_DROP = 7, G_BACKBONE_TRAIN_DROP = 8, G_COUNT = 9
   };
   cudaGraphExec_t graphs[G_COUNT] = {};
   int64_t graph_launches[G_COUNT] = {};  // kernel nodes per graph (added to `launches` per replay)
@@ -1724,6 +1733,22 @@ struct TrainBn {
   long long n = 0;
 };
 
+// Appends the training-mode record `b` of the BatchNorm `bnkey` (C channels; the caller packed its unfolded conv) to
+// pt.layers with device copies of gamma / beta; *index receives its position.
+int push_bn_record(dd_engine* e, dd_engine::ProdBn& b, const std::string& bnkey, int C, TrainBn train, int* index,
+                   cudaStream_t st) {
+  b.C = C;
+  b.stage = train.stage;
+  b.n = train.n;
+  b.key = bnkey;
+  int rc;
+  if ((rc = copy_param(e, bnkey + ".weight", C, &b.gamma, st))) return rc;
+  if ((rc = copy_param(e, bnkey + ".bias", C, &b.beta, st))) return rc;
+  *index = static_cast<int>(e->pt.layers.size());
+  e->pt.layers.push_back(b);
+  return DD_OK;
+}
+
 // conv weight key `wkey` ([cout][cin][k][k], or ConvT [cin][co][2][2] when transposed); see pack_gen_weights.  With
 // `train` and DD_FLAG_PRODUCER_TRAIN, the BatchNorm `bnkey` also gets its training-mode record in pt.layers (L.bn): the
 // conv packed unfolded (no BatchNorm, no bias, zero shift) and device copies of gamma / beta.
@@ -1752,18 +1777,10 @@ int pack_gen(dd_engine* e, GenLayer& L, const std::string& wkey, const std::stri
     return rc;
   if (train.stage < 0 || !(e->cfg.flags & DD_FLAG_PRODUCER_TRAIN)) return DD_OK;
   dd_engine::ProdBn b;
-  b.C = cout_conv;
-  b.stage = train.stage;
-  b.n = train.n;
-  b.key = bnkey;
   if ((rc = pack_gen_weights(e, e->owned, b.raw, w->ptr, wkey, nullptr, nullptr, cin, cout_conv, taps, transposed,
                              cin_pad, 0, st, scratch)))
     return rc;
-  if ((rc = copy_param(e, bnkey + ".weight", cout_conv, &b.gamma, st))) return rc;
-  if ((rc = copy_param(e, bnkey + ".bias", cout_conv, &b.beta, st))) return rc;
-  L.bn = static_cast<int>(e->pt.layers.size());
-  e->pt.layers.push_back(b);
-  return DD_OK;
+  return push_bn_record(e, b, bnkey, cout_conv, train, &L.bn, st);
 }
 
 // nn.Linear: weight key `wkey` [N][K], bias key `bkey` (empty: none).  run_gemm supplies the activation.
@@ -1990,28 +2007,17 @@ int pack_prod_train(dd_engine* e, cudaStream_t st) {
   return DD_OK;
 }
 
-// H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.  A layer with a training-mode
-// BatchNorm (L.bn) in DD_PRODUCER_TRAIN runs its conv on the unfolded pack into pt.U, then the batch statistics and fold
-// (record written), then act(s u + t) with L's addend and outputs.
-int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
-            float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
-            int ld_out = 0, int ch_off = 0) {
-  if (L.bn < 0 || e->producer_mode != DD_PRODUCER_TRAIN)
-    return launch_gen(e, L, L.relu, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, y32, add32, out, ld_out,
-                      ch_off, st, 0, nullptr, e->prod.KS);
+// The training-mode BatchNorm of record b on the pre-BN value in pt.U (b.n pixels): the batch statistics (across ranks
+// with dd_set_bn_allgather) and fold, which write the record, then act(s u + t) (`act` as the eval epilogue's code)
+// with the addend add32 placed as add_first says, into y32 and / or the planes *out (row width ld_out, 0: b.C).
+int run_bn_batch(dd_engine* e, const dd_engine::ProdBn& b, int act, int add_first, const float* add32, float* y32,
+                 const Planes* out, int ld_out, int ch_off, cudaStream_t st) {
   dd_engine::ProdTrain& pt = e->pt;
-  const dd_engine::ProdBn& b = pt.layers[L.bn];
-  const long long n = static_cast<long long>(e->cfg.batch) * H * W * (L.shuffle ? 4 : 1);
-  if (n != b.n) return fail(DD_ERR_INVALID, b.key + ": output grid differs from the packed geometry");
-  GenLayer raw = b.raw;  // the unfolded weights; the layer's shape is L's
-  raw.stride = L.stride;
-  int rc;
-  if ((rc = launch_gen(e, raw, 0, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, pt.U, nullptr, nullptr, 0, 0,
-                       st, 0, nullptr, e->prod.KS)))
-    return rc;
+  const long long n = b.n;
   const int C = b.C, nblk = pbn_blocks(n);
   const dim3 grid(nblk, (C + dd::PBN_CH - 1) / dd::PBN_CH), block(dd::PBN_CH, 8);
   const dd_engine::BnSync& sy = e->sync;
+  int rc;
   dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, nullptr, nullptr, pt.part);
   if ((rc = launched(e, "pbn_stats"))) return rc;
   if (sy.fn) {
@@ -2034,8 +2040,8 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
   a.u = pt.U;
   a.n = n;
   a.C = C;
-  a.relu = L.relu;
-  a.add_first = L.add_first;
+  a.relu = act;
+  a.add_first = add_first;
   a.s = pt.s;
   a.t = pt.t;
   a.add32 = add32;
@@ -2048,6 +2054,28 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
   a.status = e->status;
   dd::pbn_apply_kernel<<<grid_of(static_cast<size_t>(n) * C / 8), 256, 0, st>>>(a);
   return launched(e, "pbn_apply");
+}
+
+// H, W: OUTPUT grid.  With L.stride == 2 the sources live on a (src_h, src_w) grid.  A layer with a training-mode
+// BatchNorm (L.bn) in DD_PRODUCER_TRAIN runs its conv on the unfolded pack into pt.U, then the batch statistics and fold
+// (record written), then act(s u + t) with L's addend and outputs.
+int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Planes& a1, int c1, int H, int W,
+            float* y32, const float* add32, const Planes* out, cudaStream_t st, int src_h = 0, int src_w = 0,
+            int ld_out = 0, int ch_off = 0) {
+  if (L.bn < 0 || e->producer_mode != DD_PRODUCER_TRAIN)
+    return launch_gen(e, L, L.relu, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, y32, add32, out, ld_out,
+                      ch_off, st, 0, nullptr, e->prod.KS);
+  dd_engine::ProdTrain& pt = e->pt;
+  const dd_engine::ProdBn& b = pt.layers[L.bn];
+  const long long n = static_cast<long long>(e->cfg.batch) * H * W * (L.shuffle ? 4 : 1);
+  if (n != b.n) return fail(DD_ERR_INVALID, b.key + ": output grid differs from the packed geometry");
+  GenLayer raw = b.raw;  // the unfolded weights; the layer's shape is L's
+  raw.stride = L.stride;
+  int rc;
+  if ((rc = launch_gen(e, raw, 0, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, pt.U, nullptr, nullptr, 0, 0,
+                       st, 0, nullptr, e->prod.KS)))
+    return rc;
+  return run_bn_batch(e, b, L.relu, L.add_first, add32, y32, out, ld_out, ch_off, st);
 }
 
 // A forward starts (dd_run_backbone, dd_build_condition with feature maps): no record is current.
@@ -2859,7 +2887,7 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   h->packed = false;
   for (void* p : h->owned) cudaFree(p);
   h->owned.clear();
-  h->pt = dd_engine::ProdTrain();  // pack_gen appends the training-mode records, the ResNet's before the producers'
+  h->pt = dd_engine::ProdTrain();  // pack_gen appends the training-mode records, the backbone's before the producers'
   int rc;
   if ((rc = alloc_pack(h, encoder, st))) return rc;
   if ((rc = fill_pack(h, st))) return rc;
@@ -2867,15 +2895,15 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   h->rn.ready = false;
   if (h->rn.enabled)
     if ((rc = pack_resnet(h, st, scratch))) return rc;
+  h->mp.ready = false;
+  if (h->mp.enabled)
+    if ((rc = pack_mpvit(h, st, scratch))) return rc;
   h->prod.ready = false;
   if (h->prod.enabled)
     if ((rc = pack_producers(h, st, scratch))) return rc;
   h->bb.ready = false;
   if (h->bb.enabled)
     if ((rc = pack_backbone(h, st, scratch))) return rc;
-  h->mp.ready = false;
-  if (h->mp.enabled)
-    if ((rc = pack_mpvit(h, st, scratch))) return rc;
   if ((rc = pack_prod_train(h, st))) return rc;
   // the registered pointers were borrowed for this call only (include/dd_engine.h): wait for the kernels that read them
   // and forget them, so a later finalize cannot read memory the caller has freed in the meantime
@@ -3258,6 +3286,25 @@ int dd_set_producer_mode(dd_handle h, int32_t mode) {
   return DD_OK;
 }
 
+int dd_set_drop_path(dd_handle h, const float* dev_scales, int32_t n, void* cuda_stream) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  MPViTW& m = h->mp;
+  if (n == 0) {
+    m.drop_on = false;
+    return DD_OK;
+  }
+  if (!dev_scales) return fail(DD_ERR_INVALID, "null argument");
+  if (!(m.enabled && m.ready)) return fail(DD_ERR_INVALID, "dd_set_drop_path needs a finalized MPViT backbone");
+  if (n != static_cast<int64_t>(m.drop_blocks) * 2 * h->cfg.batch)
+    return fail(DD_ERR_INVALID, "dd_set_drop_path: n must be 0 or 2 x batch x the blocks mp_drop_path marks (" +
+                                    std::to_string(static_cast<int64_t>(m.drop_blocks) * 2 * h->cfg.batch) + ")");
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  CUDA_TRY(cudaMemcpyAsync(m.drop_scales, dev_scales, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice,
+                           static_cast<cudaStream_t>(cuda_stream)));
+  m.drop_on = true;
+  return DD_OK;
+}
+
 int dd_producer_batch_stats(dd_handle h, float* dev_out, int64_t capacity, int32_t* n_out, void* cuda_stream) {
   if (!h || !n_out) return fail(DD_ERR_INVALID, "null argument");
   const dd_engine::ProdTrain& pt = h->pt;
@@ -3432,6 +3479,10 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
       m.layers[s] = bc->depths[s];
       m.paths[s] = bc->mp_paths[s];
       if (m.layers[s] < 1 || m.paths[s] < 1 || m.paths[s] > 3) return fail(DD_ERR_UNSUPPORTED, "MPViT: 1..3 paths, >= 1 layer per stage");
+      m.drop_mask[s] = bc->mp_drop_path[s];
+      if (m.drop_mask[s] < 0 || (m.layers[s] < 31 && (m.drop_mask[s] >> m.layers[s]) != 0))
+        return fail(DD_ERR_INVALID, "MPViT: mp_drop_path marks a layer the stage does not have");
+      m.drop_blocks += m.paths[s] * __builtin_popcount(static_cast<unsigned>(m.drop_mask[s]));
       if (m.dims[s] <= 0 || m.dims[s] % 8 != 0 || m.dims[s] / m.heads > dd::KTV_CH_MAX || m.dims[s] > 512)
         return fail(DD_ERR_UNSUPPORTED, "MPViT: stage widths must be multiples of 8 (8 heads), at most 512");
       hh = (hh - 1) / 2 + 1;  // depthwise 3x3, stride 2, pad 1
@@ -3494,8 +3545,10 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
   if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   if ((rc = start_forward(h, st))) return rc;
   producer_forward_start(h);
-  // the ResNet's BatchNorms follow the producer mode; Swin has none, MPViT's are not covered (always eval)
-  const bool train = resnet && h->producer_mode == DD_PRODUCER_TRAIN;
+  // the ResNet's and MPViT's BatchNorms follow the producer mode (Swin has none); MPViT's stochastic depth is on while
+  // dd_set_drop_path holds scales, in either mode
+  const bool train = (resnet || mpvit) && h->producer_mode == DD_PRODUCER_TRAIN;
+  const bool drop = mpvit && h->mp.drop_on;
   bool want_out = false;
   for (int i = 0; feats_out && i < 4; ++i) want_out |= (feats_out[i] != nullptr);
   if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !want_out && !(train && h->sync.fn)) {
@@ -3503,8 +3556,9 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
     const size_t n = static_cast<size_t>(h->cfg.batch) * 3 *
                      (swin ? h->bb.H * h->bb.W : (resnet ? h->rn.H * h->rn.W : h->mp.H * h->mp.W));
     CUDA_TRY(cudaMemcpyAsync(h->rgb_stage, rgb, n * 4, cudaMemcpyDeviceToDevice, st));
-    if ((rc = graph_run(h, train ? dd_engine::G_BACKBONE_TRAIN : dd_engine::G_BACKBONE, st,
-                        [&](cudaStream_t s) { return run(h->rgb_stage, nullptr, s); })))
+    const int which = train ? (drop ? dd_engine::G_BACKBONE_TRAIN_DROP : dd_engine::G_BACKBONE_TRAIN)
+                            : (drop ? dd_engine::G_BACKBONE_DROP : dd_engine::G_BACKBONE);
+    if ((rc = graph_run(h, which, st, [&](cudaStream_t s) { return run(h->rgb_stage, nullptr, s); })))
       return rc;
   } else if ((rc = run(rgb, feats_out, st))) {
     return rc;

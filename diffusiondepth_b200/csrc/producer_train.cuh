@@ -87,8 +87,8 @@ __global__ void __launch_bounds__(256) pbn_fold_kernel(const double* __restrict_
   rec[C + c] = static_cast<float>(nn > 1.0 ? var * nn / (nn - 1.0) : var);
 }
 
-// y = act(s u + t) over n pixels of C channels (C % 8 == 0), eight channels per item, with the eval epilogue's addend
-// placements: add32 (dense [n][C]) before the ReLU (add_first, ResNet conv2 + skip) or after it (FPN lateral + up).
+// y = act(s u + t) over n pixels of C channels (C % 8 == 0), eight channels per item, act as the eval epilogue's `relu`
+// code (0 none, 1 ReLU, 3 Hardswish), with the eval epilogue's addend placements: add32 (dense [n][C]) before the ReLU (add_first, ResNet conv2 + skip) or after it (FPN lateral + up).
 // Outputs: y32 dense [n][C] and / or fp16 hi / lo planes [n][ld_out] from channel ch_off at split_scale; an output
 // outside the split's range sets bit 0 of *status, as convgen_wgmma_kernel does.
 struct PbnApplyArgs {
@@ -132,7 +132,8 @@ __global__ void __launch_bounds__(256) pbn_apply_kernel(const PbnApplyArgs a) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       if (a.add32 && a.add_first) v[j] += ad[j];
-      if (a.relu) v[j] = fmaxf(v[j], 0.f);
+      if (a.relu == 1) v[j] = fmaxf(v[j], 0.f);
+      else if (a.relu == 3) v[j] = v[j] * fminf(fmaxf(v[j] + 3.f, 0.f), 6.f) * (1.f / 6.f);
       if (a.add32 && !a.add_first) v[j] += ad[j];
     }
     if (a.y32) {
@@ -156,6 +157,57 @@ __global__ void __launch_bounds__(256) pbn_apply_kernel(const PbnApplyArgs a) {
       const size_t po = static_cast<size_t>(p) * a.ld_out + a.ch_off + c0;
       *reinterpret_cast<uint4*>(a.out_hi + po) = *reinterpret_cast<const uint4*>(hi);
       *reinterpret_cast<uint4*>(a.out_lo + po) = *reinterpret_cast<const uint4*>(lo);
+    }
+  }
+  if (overflow) atomicOr(a.status, 1);
+}
+
+// Stochastic depth on a residual branch (MPViT's MHCABlock, reference mpvit.py:432,435): y = x + scale[b] branch over
+// B images of `per_img` rows of C channels (C % 4 == 0), scale[b] = mask / keep.  y goes to y32 (dense [rows][C]; may
+// alias x) or to fp16 hi / lo planes [rows][ld_out] from channel ch_off at split_scale, where an output outside the
+// split's range sets bit 0 of *status, as convgen_wgmma_kernel does.
+struct DropAddArgs {
+  const float* x;
+  const float* branch;
+  const float* scale;
+  long long per_img;
+  int B, C;
+  float* y32;
+  __half *out_hi, *out_lo;
+  int ld_out, ch_off;
+  float split_scale;
+  int* status;
+};
+__global__ void __launch_bounds__(256) drop_path_add_kernel(const DropAddArgs a) {
+  const int c4 = a.C / 4;
+  const long long items = a.per_img * a.B * c4;
+  bool overflow = false;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < items;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long p = i / c4;
+    const int c0 = static_cast<int>(i - p * c4) * 4;
+    const float s = __ldg(a.scale + p / a.per_img);
+    const size_t o = static_cast<size_t>(p) * a.C + c0;
+    const float4 x = __ldg(reinterpret_cast<const float4*>(a.x + o));
+    const float4 r = __ldg(reinterpret_cast<const float4*>(a.branch + o));
+    const float v[4] = {fmaf(s, r.x, x.x), fmaf(s, r.y, x.y), fmaf(s, r.z, x.z), fmaf(s, r.w, x.w)};
+    if (a.y32) *reinterpret_cast<float4*>(a.y32 + o) = make_float4(v[0], v[1], v[2], v[3]);
+    if (a.out_hi) {
+      __align__(8) __half2 hi[2];
+      __align__(8) __half2 lo[2];
+      float amax = 0.f;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const float s0 = v[2 * j] * a.split_scale, s1 = v[2 * j + 1] * a.split_scale;
+        amax = fmaxf(amax, fmaxf(fabsf(s0), fabsf(s1)));
+        hi[j] = __floats2half2_rn(s0, s1);
+        const float2 back = __half22float2(hi[j]);
+        lo[j] = __floats2half2_rn(s0 - back.x, s1 - back.y);
+      }
+      overflow |= !(amax <= 60000.f);  // also catches NaN
+      const size_t po = static_cast<size_t>(p) * a.ld_out + a.ch_off + c0;
+      *reinterpret_cast<uint2*>(a.out_hi + po) = *reinterpret_cast<const uint2*>(hi);
+      *reinterpret_cast<uint2*>(a.out_lo + po) = *reinterpret_cast<const uint2*>(lo);
     }
   }
   if (overflow) atomicOr(a.status, 1);

@@ -211,10 +211,12 @@ class DenoiseEngine:
         self._ws = None
 
     def enable_backbone(self, image_hw, embed_dims=192, depths=(2, 2, 18, 2), num_heads=(6, 12, 24, 48), window=7,
-                        kind="swin", mp_dims=(64, 128, 216, 288), mp_paths=(2, 3, 3, 3), mlp_ratio=4):
+                        kind="swin", mp_dims=(64, 128, 216, 288), mp_paths=(2, 3, 3, 3), mlp_ratio=4,
+                        mp_drop_path=(0, 0, 0, 0)):
         """Run the backbone natively as well (after enable_producers, before load_weights).  kind: 'swin' (Swin-L),
         'resnet' (ResNetForMMBEV BasicBlock stages; only `depths` is used) or 'mpvit' (`depths` = encoder layers per
-        stage, `mp_dims` / `mp_paths` / `mlp_ratio`)."""
+        stage, `mp_dims` / `mp_paths` / `mlp_ratio`; `mp_drop_path[s]` bit l: stage s's encoder layer l has
+        stochastic depth, see `set_drop_path`)."""
         bc = _cabi.DDBackboneConfig()
         bc.kind, bc.embed_dims, bc.window = {"swin": 1, "resnet": 2, "mpvit": 3}[kind], int(embed_dims), int(window)
         bc.height, bc.width = int(image_hw[0]), int(image_hw[1])
@@ -222,6 +224,7 @@ class DenoiseEngine:
         for i in range(4):
             bc.depths[i], bc.num_heads[i] = int(depths[i]), int(num_heads[i])
             bc.mp_dims[i], bc.mp_paths[i] = int(mp_dims[i]), int(mp_paths[i])
+            bc.mp_drop_path[i] = int(mp_drop_path[i])
         _cabi.check(self.lib.dd_enable_backbone(self._h, C.byref(bc)))
         self.backbone = (tuple(image_hw), int(embed_dims))
         self._ws = None
@@ -452,6 +455,18 @@ class DenoiseEngine:
         (the default) for every later run_backbone / build_condition.  The engine never updates running statistics;
         `producer_batch_stats` returns what a caller needs to."""
         _cabi.check(self.lib.dd_set_producer_mode(self._h, _cabi.PRODUCER_TRAIN if training else _cabi.PRODUCER_EVAL))
+
+    def set_drop_path(self, scales: Optional[torch.Tensor]):
+        """Stochastic depth of the MPViT backbone for every later run_backbone (dd_set_drop_path): `scales` (fp32 on
+        the engine's device) = mask / keep of every DropPath branch, [block][attention, MLP][B] for the blocks
+        `enable_backbone(mp_drop_path=...)` marked, in stage, path, layer order; copied on the current stream.  None
+        turns it off."""
+        if scales is None:
+            _cabi.check(self.lib.dd_set_drop_path(self._h, None, 0, C.c_void_p(self._stream())))
+            return
+        if scales.device != self.device or scales.dtype != torch.float32 or not scales.is_contiguous():
+            raise EngineError(f"drop-path scales must be contiguous fp32 on {self.device}")
+        _cabi.check(self.lib.dd_set_drop_path(self._h, _ptr(scales), scales.numel(), C.c_void_p(self._stream())))
 
     def _producer_records(self):
         n = C.c_int32()

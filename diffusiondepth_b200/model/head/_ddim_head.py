@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from diffusiondepth_b200._cabi import EngineError
 from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS, FUSE_KEYS,
                                         DenoiseEngine, WorkspacePool, is_updatable)
-from .._blocks import ConvModule, exact_fp32
+from .._blocks import ConvModule, DropPath, exact_fp32
 from ..diffusers.schedulers.scheduling_ddim import DDIMScheduler
 from ..ops import depth_transform as _codec  # noqa: F401  (registers the codec classes)
 from ..registry import DEPTH_TRANSFORM
@@ -71,6 +71,7 @@ class EngineKey(NamedTuple):
     producer_train: bool
     backward: bool
     loop_backward: bool
+    mpvit_drop: Tuple[int, ...] = ()      # native MPViT with stochastic depth: per stage, the bit mask of its layers
 
     @property
     def geometry(self):
@@ -241,9 +242,16 @@ class DDIMHeadBase(nn.Module):
     # mode) normalise with the statistics of the batch, and every forward applies torch's running-statistic update to
     # their BatchNorm buffers.  Engines are created with DenoiseEngine(producer_train=True).  While they run in training
     # mode those buffer updates do not re-pack; the first eval-mode forward on the engine re-packs once.  An MPViT
-    # backbone in training mode runs in torch (its BatchNorms are not covered).  Off by default: the producers then run
+    # backbone in training mode runs in torch unless `mpvit_native_train` is set.  Off by default: the producers then run
     # on their running statistics in every mode.
     producer_train_bn = False
+    # Training-mode MPViT backbone on the engine (the MPViT head, together with `producer_train_bn`): when True, an MPViT
+    # in training mode runs natively as well — its 29 BatchNorms on batch statistics when all are in training mode (on
+    # running statistics when all are in eval, `norm_eval`; a mix runs in torch), and stochastic depth on every
+    # MHCABlock whose DropPath is in training mode, with the masks drawn on the device in the order torch's forward
+    # draws them, so every later random draw is the same as with the torch backbone.  Off by default: a training-mode
+    # MPViT then runs in torch under `producer_train_bn`.
+    mpvit_native_train = False
     # Synchronised BatchNorm across ranks (reference src/main.py:128, apex `convert_syncbn_model`): a torch.distributed
     # process group, or None (the default: each rank's own batch).  When set, every BatchNorm that `codec_train_bn` /
     # `producer_train_bn` run in training mode normalises with the statistics of all the group's ranks' batches
@@ -408,6 +416,49 @@ class DDIMHeadBase(nn.Module):
         except (AttributeError, IndexError):
             return None
 
+    @staticmethod
+    def mpvit_drop_paths(backbone):
+        """(per-stage bit masks of the encoder layers with stochastic depth, their DropPath modules in torch's draw order:
+        stage, path, layer) of an MPViT module, or None when the layers with a DropPath of rate > 0 differ between the
+        paths of a stage."""
+        masks, mods = [], []
+        for st in backbone.mhca_stages:
+            bits = None
+            for enc in st.mhca_blks:
+                b = 0
+                for l, blk in enumerate(enc.MHCA_layers):
+                    if isinstance(blk.drop_path, DropPath) and blk.drop_path.p > 0.0:
+                        b |= 1 << l
+                        mods.append(blk.drop_path)
+                if bits is not None and b != bits:
+                    return None
+                bits = b
+            masks.append(bits or 0)
+        return tuple(masks), mods
+
+    def _mpvit_drop_scales(self, backbone, batch, device):
+        """Per-sample scales mask / keep of every DropPath branch of a natively run MPViT, [block][attention, MLP][B]
+        (set_drop_path), drawn as torch's forward would (`x.new_empty((B, 1, 1)).bernoulli_(keep)` on the device, one
+        draw per branch of a DropPath in training mode); None when none is in training mode."""
+        _, mods = self.mpvit_drop_paths(backbone)
+        if not any(m.training for m in mods):
+            return None
+        out = []
+        for m in mods:
+            for _ in range(2):  # the attention branch, then the MLP branch (one DropPath module, two calls)
+                if m.training:
+                    keep = 1.0 - m.p
+                    out.append(torch.empty((batch, 1, 1), device=device, dtype=torch.float32).bernoulli_(keep)
+                               .reshape(batch) / keep)
+                else:
+                    out.append(torch.ones(batch, device=device, dtype=torch.float32))
+        return torch.cat(out)
+
+    @staticmethod
+    def _bn_modes(module):
+        """{training flags} of the BatchNorms in `module`."""
+        return {m.training for m in module.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)}
+
     def can_run_backbone(self, backbone, img) -> bool:
         """Native backbone path: CUDA input and an architecture the engine instantiates — Swin-L for the Swin heads,
         BasicBlock ResNetForMMBEV (64/128/256/512, stride 2 per stage) for the Res heads, MPViT for the MPViT head."""
@@ -416,7 +467,11 @@ class DDIMHeadBase(nn.Module):
         name = type(backbone).__name__
         if name == "MPViT":
             if self.producer_train_bn and backbone.training:
-                return False  # its BatchNorms in training mode: torch runs it, the neck and FPN stay native
+                # natively with mpvit_native_train, when its BatchNorms share one mode and its paths one DropPath
+                # layout; otherwise torch runs it and the neck and FPN stay native
+                if not self.mpvit_native_train or len(self._bn_modes(backbone)) > 1 \
+                        or self.mpvit_drop_paths(backbone) is None:
+                    return False
             spec = self.mpvit_spec(backbone)
             if spec is None or self.variant != "swin" or list(self.fpn_in_channels) != list(backbone.out_channels):
                 return False
@@ -454,12 +509,17 @@ class DDIMHeadBase(nn.Module):
                                        loop_backward, producer_train)
 
     def _engine_key(self, batch, latent_hw, cond_hw, device, native=False, image_hw=None, backward=False,
-                    loop_backward=False) -> EngineKey:
+                    loop_backward=False, mpvit_drop=()) -> EngineKey:
         return EngineKey(batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)),
                          self.diffusion_inference_steps, self.use_cuda_graph, native,
                          tuple(image_hw) if image_hw is not None else None, bool(self.return_intermediates),
                          bool(self.fp8_corrections), native and bool(self.producer_train_bn), bool(backward),
-                         bool(loop_backward))
+                         bool(loop_backward), tuple(mpvit_drop))
+
+    def _mpvit_native_train(self, image_hw, backbone):
+        """Whether the engine running this backbone also runs it in training mode (stochastic depth included)."""
+        return (image_hw is not None and self.mpvit_native_train and self.producer_train_bn
+                and type(self._backbone(backbone)).__name__ == "MPViT")
 
     def _grad_engine(self, batch, latent_hw, cond_hw, device) -> DenoiseEngine:
         """The engine `denoiser_backward` runs on: the loop-backward engine of this geometry when the head trains through
@@ -474,7 +534,8 @@ class DDIMHeadBase(nn.Module):
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
-        key = self._engine_key(batch, latent_hw, cond_hw, device, native, image_hw, backward, loop_backward)
+        drop = self.mpvit_drop_paths(self._backbone(backbone))[0] if self._mpvit_native_train(image_hw, backbone) else ()
+        key = self._engine_key(batch, latent_hw, cond_hw, device, native, image_hw, backward, loop_backward, drop)
         eng = self._engines.get(key)
         if eng is None:
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
@@ -487,7 +548,8 @@ class DDIMHeadBase(nn.Module):
             if image_hw is not None:
                 if type(self._backbone(backbone)).__name__ == "MPViT":
                     layers, dims, paths, ratio = self.mpvit_spec(self._backbone(backbone))
-                    eng.enable_backbone(image_hw, depths=layers, kind="mpvit", mp_dims=dims, mp_paths=paths, mlp_ratio=ratio)
+                    eng.enable_backbone(image_hw, depths=layers, kind="mpvit", mp_dims=dims, mp_paths=paths, mlp_ratio=ratio,
+                                        mp_drop_path=key.mpvit_drop or (0, 0, 0, 0))
                 elif self.variant == "swin":
                     eng.enable_backbone(image_hw)
                 else:
@@ -606,13 +668,16 @@ class DDIMHeadBase(nn.Module):
     # ------------------------------------------------------------------------------------------ producer BatchNorms
     def _producer_training(self, backbone=None):
         """(neck + FPN, native backbone) run their BatchNorms on batch statistics in this forward: `producer_train_bn`
-        and the modules in training mode.  `backbone`: the natively run backbone module (None: torch runs it); only the
-        ResNet's BatchNorms are on the engine.  The engine's BatchNorms use eps = 1e-5 and track running statistics."""
+        and the modules in training mode.  `backbone`: the natively run backbone module (None: torch runs it); the
+        ResNet's BatchNorms are on the engine, and the MPViT's under `mpvit_native_train` (all of them in training mode).
+        The engine's BatchNorms use eps = 1e-5 and track running statistics."""
         if not self.producer_train_bn:
             return False, False
         cond_mods = [self._modules[n] for n in ("hahineck", "conv_lateral") if n in self._modules]
         cond = any(m.training for m in cond_mods)
-        bb = backbone is not None and type(backbone).__name__ == "ResNetForMMBEV" and backbone.training
+        name = type(backbone).__name__ if backbone is not None else None
+        bb = (name == "ResNetForMMBEV" and backbone.training) or \
+            (name == "MPViT" and self.mpvit_native_train and self._bn_modes(backbone) == {True})
         mods = ([self._modules[n] for n in ("hahineck", "conv_lateral", "conv_up") if n in self._modules] if cond else []) \
             + ([backbone] if bb else [])
         for m in mods:
@@ -669,10 +734,14 @@ class DDIMHeadBase(nn.Module):
         if self.bn_sync_group is not None and self.return_intermediates:
             raise EngineError("bn_sync_group is not supported by the *Vis heads (their step decodes run in one CUDA graph)")
         with_backbone = fp is None
+        drop_scales = None
         if with_backbone:
             B, dev, dtype = image.shape[0], image.device, torch.float32
             sizes = self.backbone_pyramid(image.shape[-2:], self._backbone(backbone))
             native = True
+            native_train = self._mpvit_native_train(image.shape[-2:], backbone)
+            if native_train:  # drawn first, as the torch backbone's forward would before the head draws x_T
+                drop_scales = self._mpvit_drop_scales(self._backbone(backbone), B, dev)
         else:
             if self.detach_fp is not False and self.detach_fp is not None:
                 idx = self.detach_fp if isinstance(self.detach_fp, (list, tuple, range)) else range(len(fp))
@@ -705,6 +774,8 @@ class DDIMHeadBase(nn.Module):
                                    image_hw=tuple(image.shape[-2:]), backbone=backbone, producer_train=ptrain)
                 if eng.producer_train:
                     eng.set_producer_mode(ptrain_bb)
+                if native_train:
+                    eng.set_drop_path(drop_scales)
                 eng.run_backbone(image.contiguous().float())
                 if eng.producer_train:
                     eng.set_producer_mode(ptrain_cond)

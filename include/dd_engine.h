@@ -53,7 +53,7 @@
 extern "C" {
 #endif
 
-#define DD_ABI_VERSION 1
+#define DD_ABI_VERSION 2
 
 typedef struct dd_engine* dd_handle;
 
@@ -215,6 +215,9 @@ typedef struct dd_backbone_config {
   int32_t mp_dims[4];  /* DD_BACKBONE_MPVIT only: 64, 128, 216, 288 (mpvit_small) */
   int32_t mp_paths[4]; /* 2, 3, 3, 3 */
   int32_t mlp_ratio;   /* 4 */
+  int32_t mp_drop_path[4]; /* DD_BACKBONE_MPVIT only: bit l of entry s set = encoder layer l of stage s (in every path)
+                              has stochastic depth (a DropPath of rate > 0) on its two residual branches; see
+                              dd_set_drop_path.  All zero: none */
 } dd_backbone_config;
 int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc);
 
@@ -341,8 +344,10 @@ int dd_codec_batch_stats(dd_handle h, float* dev_out, int32_t capacity, int32_t*
  * dd_build_condition then run each such layer as the conv on its unfolded pack into engine-owned fp32 scratch (a ConvT
  * pixel-shuffled: its statistics cover all B x 2H x 2W pixels before the FPN's adaptive_avg_pool2d), two statistics
  * passes, a fold s = gamma / sqrt(var + 1e-5), t = beta - s mean, and act(s u + t) with the eval layer's addend and
- * outputs; no host synchronisation, CUDA graphs of their own (the eval graphs are kept).  The Swin and MPViT backbones
- * are not affected.  The engine never writes running statistics: the caller applies the running update from the
+ * outputs; no host synchronisation, CUDA graphs of their own (the eval graphs are kept).  dd_run_backbone (MPViT) does the
+ * same for the stem, the patch embeddings' pointwise convs, InvRes conv1 / conv2, the aggregate and InvRes.norm after
+ * its depthwise conv, with Hardswish where the layer has it (records: stem, then per stage the patch embeddings,
+ * conv1, norm, conv2, aggregate).  The Swin backbone is not affected.  The engine never writes running statistics: the caller applies the running update from the
  * records (dd_producer_batch_stats) and re-packs the eval weights with dd_finalize_weights when it next runs in
  * DD_PRODUCER_EVAL.  The mode is engine state, read by each call. */
 enum dd_producer_mode { DD_PRODUCER_EVAL = 0, DD_PRODUCER_TRAIN = 1 };
@@ -354,6 +359,15 @@ int dd_set_producer_mode(dd_handle h, int32_t mode);
  * synchronisation.  A record is current when the forward that last started (dd_run_backbone, or dd_build_condition
  * with feature maps) evaluated its layer in DD_PRODUCER_TRAIN (dd_producer_bn_info's *fresh). */
 int dd_producer_batch_stats(dd_handle h, float* dev_out, int64_t capacity, int32_t* n_out, void* cuda_stream);
+
+/* Stochastic depth of the MPViT backbone (reference mpvit.py:432,435, timm DropPath in training mode): dev_scales
+ * (device fp32, n of them) holds, for every block dd_backbone_config.mp_drop_path marks, in stage, path, layer order,
+ * the B per-sample scales mask / (1 - rate) of its attention branch, then the B of its MLP branch.  They are copied on
+ * cuda_stream into an engine-owned buffer that every later dd_run_backbone reads (graphs included), in either producer
+ * mode: x = x + scale[b] branch.  n = 0 turns stochastic depth off (the default; dev_scales may be NULL).  DD_ERR_INVALID
+ * when n is neither 0 nor 2 x batch x the marked blocks, or before dd_finalize_weights of an MPViT backbone (which also
+ * turns it off). */
+int dd_set_drop_path(dd_handle h, const float* dev_scales, int32_t n, void* cuda_stream);
 
 /* Record i: the registered key prefix of its BatchNorm (e.g. `hahineck.trans_fusion.1.bn`, `conv_up.0.1`,
  * `backbone.layers.2.0.bn1`; NUL-terminated, truncated to key_capacity), its channels, its offset in floats into
