@@ -36,6 +36,11 @@ class DDGenLayerDesc(C.Structure):
                                          "ch_off", "n_tile", "alt_tile")]
 
 
+class DDConvGnDesc(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("batch", "cin", "cout", "height", "width", "mode", "cond_h", "cond_w",
+                                         "up_qpb")] + [("c_x", C.c_float), ("c_eps", C.c_float)]
+
+
 ABI_VERSION = 2
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
@@ -112,6 +117,9 @@ SIGNATURES = {
                                     C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
     "dd_layer_norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                 C.c_float, C.c_void_p]),
+    "dd_conv_groupnorm": (C.c_int, [C.c_void_p, C.POINTER(DDConvGnDesc), C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p]),
     "dd_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     "dd_bench_conv": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_void_p,
                                 C.c_size_t, C.c_void_p]),

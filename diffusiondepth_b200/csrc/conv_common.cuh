@@ -20,7 +20,7 @@ constexpr int TILE_W = 16;
 constexpr int TILE_M = TILE_H * TILE_W;  // 128
 
 enum EpiMode : int {
-  EPI_F32_STATS = 0,  // y fp32 NHWC + per-(tile, group) sum / sum-of-squares for the consumer GroupNorm
+  EPI_F32_STATS = 0,  // y fp32 NHWC + per-(tile, group) fp64 sum / sum-of-squares for the consumer GroupNorm
   EPI_SPLIT = 1,      // y -> scaled fp16 hi/lo planes (input of the next conv; no norm in between)
   EPI_F32 = 2         // y fp32 NHWC only
 };
@@ -31,7 +31,7 @@ struct ConvArgs {
   const float* bias;       // [COUT]
   float acc_scale;         // 1 / (act_scale * weight_scale): undoes the power-of-two operand scaling
   float* y32;              // [B*H*W][COUT]                       (EPI_F32*)
-  float* stats_partial;    // [num_tiles][4][2]                   (EPI_F32_STATS)
+  double* stats_partial;   // [num_tiles][4][2]                   (EPI_F32_STATS)
   __half* out_hi;          // [B*H*W][COUT]                       (EPI_SPLIT)
   __half* out_lo;
   uint8_t* out_a8;         // non-null (EPI_SPLIT): write the e4m3 planes a8 / l8 instead of the fp16 lo plane

@@ -56,7 +56,7 @@ struct HaloCfg {
   static constexpr int CH = NWG > 1 ? 16 : (NW < 32 ? NW : 32);
   static constexpr int LD = CH + 1;                                  // staging row stride (floats): conflict-free rows
   static constexpr int STAGE_BYTES = NWG * 128 * LD * 4;
-  static constexpr int CTRL_BYTES = 1024;  // barriers, GroupNorm partials [2][4 NWG][4][2]
+  static constexpr int CTRL_BYTES = 1024;  // barriers, GroupNorm partials [2][4 NWG][GPW][2] (fp64)
   static constexpr int BUDGET = 227 * 1024 - 1024 - CTRL_BYTES - STAGE_BYTES - A_SLOTS * A_SLOT;
   static constexpr int B_SLOTS_RAW = BUDGET / B_SLOT;
   // Small layers (16->64, 64->16): all 9 x KC weight tiles fit in shared memory -> fetch them ONCE per CTA instead of
@@ -90,7 +90,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   uint64_t* a_empty = a_full + C::A_SLOTS;
   uint64_t* b_full = a_empty + C::A_SLOTS;
   uint64_t* b_empty = b_full + C::B_SLOTS;
-  float* red = reinterpret_cast<float*>(b_empty + C::B_SLOTS);  // [2][4 NWG][4][2]
+  double* red = reinterpret_cast<double*>(b_empty + C::B_SLOTS);  // [2][4 NWG][GPW][2]
   float* stage = reinterpret_cast<float*>(ctrl + C::CTRL_BYTES);
 
   const int warp = threadIdx.x >> 5;
@@ -249,9 +249,13 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       const size_t pix = (static_cast<size_t>(img) * p.H + y) * p.W + x;
       const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
       const uint32_t row_off = static_cast<uint32_t>(pix * COUT);  // < 2^32 elements for every tensor of the path
-      float tsum[C::GPW], tsq[C::GPW];
+      // E[v^2] - mean^2 cancels (mean / std)^2 of the sums' significant bits, so a group whose mean dominates its
+      // spread loses its variance in plain fp32 sums (rstd off by 1e-2 at mean / std = 1000).  Each thread sums its
+      // pixel's d = v - k in fp32, k = the pixel's first value in the group (|d| ~ the group's spread), and turns the
+      // sums into fp64 sums of v and v^2 once per group.
+      float tk[C::GPW], tsum[C::GPW], tsq[C::GPW];
 #pragma unroll
-      for (int g = 0; g < C::GPW; ++g) tsum[g] = tsq[g] = 0.f;
+      for (int g = 0; g < C::GPW; ++g) tk[g] = tsum[g] = tsq[g] = 0.f;
       bool overflow = false;
 #pragma unroll
       for (int cj = 0; cj < NW / C::CH; ++cj) {
@@ -268,8 +272,10 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 #pragma unroll
             for (int j = 0; j < C::CH; ++j) {
               const int g = (cj * C::CH + j) / C::GROUP_CH;  // compile-time: group within this warpgroup's columns
-              tsum[g] += v[j];
-              tsq[g] = fmaf(v[j], v[j], tsq[g]);
+              if ((cj * C::CH + j) % C::GROUP_CH == 0) tk[g] = v[j];
+              const float d = v[j] - tk[g];
+              tsum[g] += d;
+              tsq[g] = fmaf(d, d, tsq[g]);
             }
           }
         }
@@ -321,32 +327,28 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         // warp tree -> shared memory -> 8 threads combine the consumer warps in fixed order (deterministic)
         const int cw = wg * 4 + q;  // consumer warp index
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int gl = g - (C::NWG > 1 ? wg * C::GPW : 0);  // this warpgroup's local group index
-          float s = 0.f, s2 = 0.f;
-#pragma unroll
-          for (int k = 0; k < C::GPW; ++k)
-            if (k == gl) {
-              s = tsum[k];
-              s2 = tsq[k];
-            }
+        for (int k = 0; k < C::GPW; ++k) {  // this warpgroup's groups
+          const double n = valid ? C::GROUP_CH : 0, kk = tk[k], ds = tsum[k];
+          double s = fma(n, kk, ds), s2 = fma(n * kk, kk, fma(2.0 * kk, ds, static_cast<double>(tsq[k])));
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) {
             s += __shfl_xor_sync(0xffffffffu, s, o);
             s2 += __shfl_xor_sync(0xffffffffu, s2, o);
           }
           if (lane == 0) {
-            red[((par * 4 * C::NWG + cw) * 4 + g) * 2 + 0] = s;
-            red[((par * 4 * C::NWG + cw) * 4 + g) * 2 + 1] = s2;
+            red[((par * 4 * C::NWG + cw) * C::GPW + k) * 2 + 0] = s;
+            red[((par * 4 * C::NWG + cw) * C::GPW + k) * 2 + 1] = s2;
           }
         }
         named_bar_sync(1, 128 * C::NWG);
         const int e = threadIdx.x - 128;
         if (e < 8) {
           const int g = e >> 1, which = e & 1;
-          float tt = 0.f;
+          const int w0 = C::NWG > 1 ? (g / C::GPW) * 4 : 0, k = C::NWG > 1 ? g % C::GPW : g;  // the group's warps
+          double tt = 0.0;
 #pragma unroll
-          for (int w = 0; w < 4 * C::NWG; ++w) tt += red[((par * 4 * C::NWG + w) * 4 + g) * 2 + which];
+          for (int w = 0; w < 4 * C::NWG; ++w)
+            if (C::NWG == 1 || (w >= w0 && w < w0 + 4)) tt += red[((par * 4 * C::NWG + w) * C::GPW + k) * 2 + which];
           p.stats_partial[(static_cast<size_t>(tile) * 4 + g) * 2 + which] = tt;
         }
         par ^= 1;  // double-buffered scratch: one barrier per tile is enough

@@ -517,7 +517,8 @@ struct dd_engine {
   std::vector<float> cx, ce;
   // workspace views
   void* ws = nullptr;
-  float *x32 = nullptr, *Y = nullptr, *cond = nullptr, *stats[4] = {}, *mr[4] = {}, *temb_sel = nullptr;
+  float *x32 = nullptr, *Y = nullptr, *cond = nullptr, *mr[4] = {}, *temb_sel = nullptr;
+  double* stats[4] = {};  // GroupNorm partials [tiles][4][2] of the conv before each norm
   __half *xs_hi = nullptr, *xs_lo = nullptr, *S_hi[2] = {}, *S_lo[2] = {};
   int* status = nullptr;
   struct Bwd {  // dd_denoiser_backward's region (DD_FLAG_BACKWARD): the recomputed forward and the gradient buffers
@@ -760,7 +761,7 @@ size_t carve(dd_engine* e, void* base) {
   }
   v->cond = c.take<float>(static_cast<size_t>(g.B) * e->cfg.cond_h * e->cfg.cond_w * 256);
   for (int i = 0; i < 4; ++i) {
-    v->stats[i] = c.take<float>(static_cast<size_t>(g.tiles_max) * 8);
+    v->stats[i] = c.take<double>(static_cast<size_t>(g.tiles_max) * 8);
     v->mr[i] = c.take<float>(static_cast<size_t>(g.B) * 8);
   }
   v->temb_sel = c.take<float>(static_cast<size_t>(g.B) * 256);
@@ -922,7 +923,7 @@ constexpr int kF8In = 1, kF8Out = 2;
 // so correction products added into the running fp32 sum of the hi * hi product would be lost.
 bool fp8_active(const dd_engine*) { return false; }
 int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, float in_scale, int epi, float* y32,
-             float* stats_partial, __half* out_hi, __half* out_lo, cudaStream_t st, int f8 = 0) {
+             double* stats_partial, __half* out_hi, __half* out_lo, cudaStream_t st, int f8 = 0) {
   const Geom g = geom_of(e->cfg);
   ConvLayer& L = e->L[layer];
   dd::ConvArgs a;
@@ -954,12 +955,32 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
   return launched(e, "conv3x3");
 }
 
-int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st, const float* ring = nullptr, int ring_per_img = 0) {
+int run_finalize(dd_engine* e, int which, int channels, cudaStream_t st, const double* ring = nullptr, int ring_per_img = 0) {
   const Geom g = geom_of(e->cfg);
   const double inv = 1.0 / (static_cast<double>(g.P) * (channels / 4));
   dd::gn_finalize_kernel<<<g.B * 4, 256, 0, st>>>(e->stats[which], e->stats_tiles_img[which], ring, ring_per_img, inv,
                                                    1e-5f, e->mr[which]);
   return launched(e, "gn_finalize");
+}
+
+// The GroupNorm apply kernel of a (C, COND) layer on a's B x H x W grid; up_qpb: quads per block of the bilinear
+// up-add kernel (4, or 1: one 64-thread block per quad).  The caller checks the launch.
+template <int C, int COND>
+void launch_apply(const dd::ApplyArgs& a, int B, int up_qpb, cudaStream_t st) {
+  if (COND == 2 && C == 256) {
+    // one 64-thread block per 2 x 2 output quad (rows 2i-1, 2i; columns 2j-1, 2j)
+    if (up_qpb == 4) {
+      dim3 grid((a.W / 2 + 1 + 3) / 4, a.H / 2 + 1, B);
+      dd::gn_apply_up_split_kernel<4, 4><<<grid, 256, 0, st>>>(a);
+    } else {
+      dim3 grid(a.W / 2 + 1, a.H / 2 + 1, B);
+      dd::gn_apply_up_split_kernel<4, 1><<<grid, 64, 0, st>>>(a);
+    }
+  } else {
+    constexpr int PPB = 256 / (C / 8);
+    dim3 grid((a.H * a.W + PPB - 1) / PPB, B);
+    dd::gn_apply_split_kernel<C, COND><<<grid, 256, 0, st>>>(a);
+  }
 }
 
 template <int C, int COND>
@@ -989,20 +1010,7 @@ int run_apply(dd_engine* e, int which, const float* temb, int temb_bstride, __ha
   }
   a.scale = kActScale;
   a.status = e->status;
-  if (COND == 2 && C == 256) {
-    // one 64-thread block per 2 x 2 output quad (rows 2i-1, 2i; columns 2j-1, 2j)
-    if (e->up_qpb == 4) {
-      dim3 grid((g.w / 2 + 1 + 3) / 4, g.h / 2 + 1, g.B);
-      dd::gn_apply_up_split_kernel<4, 4><<<grid, 256, 0, st>>>(a);
-    } else {
-      dim3 grid(g.w / 2 + 1, g.h / 2 + 1, g.B);
-      dd::gn_apply_up_split_kernel<4, 1><<<grid, 64, 0, st>>>(a);
-    }
-  } else {
-    constexpr int PPB = 256 / (C / 8);
-    dim3 grid((g.P + PPB - 1) / PPB, g.B);
-    dd::gn_apply_split_kernel<C, COND><<<grid, 256, 0, st>>>(a);
-  }
+  launch_apply<C, COND>(a, g.B, e->up_qpb, st);
   return launched(e, "gn_apply");
 }
 
@@ -1057,6 +1065,12 @@ int run_fold(dd_engine* e, cudaStream_t st) {
 }
 
 int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st);
+
+// pred.4's GroupNorm + ReLU fused with the DDIM update over B images of f.P pixels; the caller checks the launch.
+void launch_final(const dd::FinalArgs& f, int B, cudaStream_t st) {
+  dim3 grid((f.P * 4 + 255) / 256, B);
+  dd::gn_relu_ddim_kernel<<<grid, 256, 0, st>>>(f);
+}
 
 // One ScheduledCNNRefine.forward + (optionally) the DDIM update.
 int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float ce, float* eps_out, cudaStream_t st) {
@@ -1123,8 +1137,7 @@ int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st) 
   f.scale = kXScale;
   f.P = g.P;
   f.status = e->status;
-  dim3 grid((g.P * 4 + 255) / 256, g.B);
-  dd::gn_relu_ddim_kernel<<<grid, 256, 0, st>>>(f);
+  launch_final(f, g.B, st);
   return launched(e, "gn_relu_ddim");
 }
 
@@ -3939,6 +3952,145 @@ int dd_layer_norm(dd_handle h, const float* x, const float* gamma, const float* 
   dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
   if ((rc = check_launch("join_planes"))) return rc;
   return call.finish(st, "x or the LayerNorm output");
+}
+
+int dd_conv_groupnorm(dd_handle h, const dd_conv_gn_desc* d, const float* x, const float* w, const float* b,
+                      const float* gamma, const float* beta, const float* cond, const float* temb, float* latent,
+                      float* y32, float* mean_rstd, float* out, void* cuda_stream) {
+  if (!h || !d || !x || !w || !b || !gamma || !beta) return fail(DD_ERR_INVALID, "null argument");
+  const int B = d->batch, cin = d->cin, cout = d->cout, H = d->height, W = d->width, mode = d->mode;
+  const int sid = shape_id(cin, cout);
+  if (sid < 0 || (cin == 256 && cout == 256)) return fail(DD_ERR_UNSUPPORTED, "not a GroupNorm'd conv of the DDIM loop");
+  if (B < 1 || H < 1 || W < 1 || mode < 0 || mode > 3) return fail(DD_ERR_INVALID, "bad conv / GroupNorm descriptor");
+  if ((mode == 0 && cout != 64) || ((mode == 1 || mode == 2) && cout != 256) || (mode == 3 && cout != 16))
+    return fail(DD_ERR_UNSUPPORTED, "the loop applies that mode to another conv shape");
+  if ((mode == 1 || mode == 2) && (!cond || !temb)) return fail(DD_ERR_INVALID, "null condition or time embedding");
+  if (mode == 2 && (d->cond_h < 1 || d->cond_w < 1 || (d->up_qpb != 4 && d->up_qpb != 1)))
+    return fail(DD_ERR_INVALID, "bad up-add geometry");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const int P = H * W;
+  const size_t BP = static_cast<size_t>(B) * P;
+  const size_t nw = static_cast<size_t>(cin) * cout * 9;
+  const int ch = mode == 2 ? d->cond_h : H, cw = mode == 2 ? d->cond_w : W;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  float* scratch = reinterpret_cast<float*>(call.status) + 8;
+  const bool simt = (h->cfg.flags & DD_FLAG_SIMT_CONV) != 0;
+  const int tiles_img = simt ? ((W + dd::TILE_W - 1) / dd::TILE_W) * ((H + dd::TILE_H - 1) / dd::TILE_H)
+                             : ((W + dd::HALO_TW - 1) / dd::HALO_TW) * ((H + dd::HALO_TH - 1) / dd::HALO_TH);
+  float *xn, *yn, *wsimt, *mr, *cn = nullptr, *xl = nullptr, *eps = nullptr;
+  double* partial;
+  Planes xs, wp, o;
+  if ((rc = call.alloc(&xn, BP * cin)) || (rc = call.alloc(&xs.hi, BP * cin)) || (rc = call.alloc(&xs.lo, BP * cin)) ||
+      (rc = call.alloc(&yn, BP * cout)) || (rc = call.alloc(&wp.hi, nw)) || (rc = call.alloc(&wp.lo, nw)) ||
+      (rc = call.alloc(&wsimt, nw)) || (rc = call.alloc(&partial, static_cast<size_t>(B) * tiles_img * 8)) ||
+      (rc = call.alloc(&mr, static_cast<size_t>(B) * 8)) || (rc = call.alloc(&o.hi, BP * cout)) ||
+      (rc = call.alloc(&o.lo, BP * cout)))
+    return rc;
+  // the conv: fp32 NCHW -> NHWC split planes at the loop's scale of that input (the latent's, or the activations'), the
+  // weights at their own power-of-two scale, and the loop's epilogue
+  if ((rc = transpose_in(x, xn, B, cin, P, st))) return rc;
+  const float sx = cin == 16 ? kXScale : kActScale;
+  float sw;
+  if ((rc = split_scale_of(w, nw, scratch, st, &sw))) return rc;
+  if ((rc = split_planes(h, xn, xs.hi, xs.lo, BP * cin, sx, st))) return rc;
+  dd::pack_conv_weight_kernel<<<128, 256, 0, st>>>(w, wp.hi, wp.lo, wsimt, cout, cin, sw);
+  if ((rc = check_launch("pack_conv_weight"))) return rc;
+  dd::ConvArgs a;
+  a.B = B;
+  a.H = H;
+  a.W = W;
+  a.bias = b;
+  a.acc_scale = 1.f / (sx * sw);
+  a.y32 = yn;
+  a.stats_partial = partial;
+  a.out_hi = a.out_lo = nullptr;
+  a.out_a8 = a.out_l8 = nullptr;
+  a.split_scale = 1.f;
+  a.status = call.status;
+  CUtensorMap mb_hi{}, mb_lo{};
+  if (!simt) {
+    if ((rc = make_weight_map(&mb_hi, wp.hi, cout, cin, 9, kHaloBK[sid], cout))) return rc;
+    if ((rc = make_weight_map(&mb_lo, wp.lo, cout, cin, 9, kHaloBK[sid], cout))) return rc;
+  }
+  if ((rc = launch_conv3x3(sid, dd::EPI_F32_STATS, simt, a, xs.hi, xs.lo, sx, wsimt, mb_hi, mb_lo, h->sm_count, st)))
+    return rc;
+  if ((rc = check_launch("conv3x3"))) return rc;
+  dd::gn_finalize_kernel<<<B * 4, 256, 0, st>>>(partial, a.tiles_x * a.tiles_y, nullptr, 0,
+                                                 1.0 / (static_cast<double>(P) * (cout / 4)), 1e-5f, mr);
+  if ((rc = check_launch("gn_finalize"))) return rc;
+  // the apply kernel the loop runs after this conv
+  if (mode == 3) {
+    dd::FinalArgs f;
+    f.y = yn;
+    f.mean_rstd = mr;
+    f.gamma = gamma;
+    f.beta = beta;
+    f.x = nullptr;
+    f.x_hi = o.hi;
+    f.x_lo = o.lo;
+    f.eps_out = nullptr;
+    f.cx = d->c_x;
+    f.ce = d->c_eps;
+    f.scale = kXScale;
+    f.P = P;
+    f.status = call.status;
+    if (latent) {
+      if ((rc = call.alloc(&xl, BP * 16)) || (rc = transpose_in(latent, xl, B, 16, P, st))) return rc;
+      f.x = xl;
+    } else {
+      if ((rc = call.alloc(&eps, BP * 16))) return rc;
+      f.eps_out = eps;
+    }
+    launch_final(f, B, st);
+    if ((rc = check_launch("gn_relu_ddim"))) return rc;
+  } else {
+    dd::ApplyArgs g;
+    g.y = yn;
+    g.mean_rstd = mr;
+    g.gamma = gamma;
+    g.beta = beta;
+    g.cond = nullptr;
+    g.temb = temb;
+    g.temb_bstride = 256;
+    g.H = H;
+    g.W = W;
+    g.ch = ch;
+    g.cw = cw;
+    g.ry = H > 1 ? static_cast<float>(ch - 1) / static_cast<float>(H - 1) : 0.f;
+    g.rx = W > 1 ? static_cast<float>(cw - 1) / static_cast<float>(W - 1) : 0.f;
+    g.out_hi = o.hi;
+    g.out_lo = o.lo;
+    g.out_a8 = g.out_l8 = nullptr;
+    g.scale = kActScale;
+    g.status = call.status;
+    if (mode != 0) {
+      const size_t nc = static_cast<size_t>(B) * ch * cw * 256;
+      if ((rc = call.alloc(&cn, nc)) || (rc = transpose_in(cond, cn, B, 256, ch * cw, st))) return rc;
+      g.cond = cn;
+    }
+    if (mode == 0) launch_apply<64, 0>(g, B, 0, st);
+    else if (mode == 1) launch_apply<256, 1>(g, B, 0, st);
+    else launch_apply<256, 2>(g, B, d->up_qpb, st);
+    if ((rc = check_launch("gn_apply"))) return rc;
+  }
+  // outputs, NCHW
+  if (y32 && (rc = transpose_out(yn, y32, B, cout, P, st))) return rc;
+  if (mean_rstd) CUDA_TRY(cudaMemcpyAsync(mean_rstd, mr, static_cast<size_t>(B) * 32, cudaMemcpyDeviceToDevice, st));
+  if (xl && (rc = transpose_out(xl, latent, B, 16, P, st))) return rc;
+  if (out) {
+    const float* src = eps;
+    if (!eps) {  // the split planes the apply kernel wrote, joined back in place of the conv output
+      dd::join_planes_kernel<<<grid_of(BP * cout), 256, 0, st>>>(o.hi, o.lo, yn, BP * cout,
+                                                                 1.f / (mode == 3 ? kXScale : kActScale));
+      if ((rc = check_launch("join_planes"))) return rc;
+      src = yn;
+    }
+    if ((rc = transpose_out(src, out, B, cout, P, st))) return rc;
+  }
+  return call.finish(st, "x or the GroupNorm'd output");
 }
 
 int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,

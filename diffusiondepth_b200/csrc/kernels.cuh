@@ -160,19 +160,21 @@ __global__ void absmax_kernel(const float* __restrict__ w, int n, float* __restr
 }
 
 // ------------------------------------------------------------------ GroupNorm(4, C) finalize
-// partial [tiles_total][4][2] (fp32 sums over one conv tile) and, optionally, ring [B][ring_per_img][4][2] (the
-// border pixels the composed pred.0 conv leaves to ring_fix_kernel) -> mean/rstd per (image, group).
-// Combined in fp64 in a fixed order (deterministic; SURVEY.md §7.2-4).
-__global__ void gn_finalize_kernel(const float* __restrict__ partial, int tiles_per_img, const float* __restrict__ ring,
+// partial [tiles_total][4][2] (fp64 sums of v and v^2 over one conv tile) and, optionally, ring [B][ring_per_img][4][2]
+// (the border pixels the composed pred.0 conv leaves to ring_fix_kernel) -> mean/rstd per (image, group).
+// Combined in fp64 in a fixed order (deterministic; SURVEY.md §7.2-4).  var = E[v^2] - mean^2 keeps ~53 - 2 log2(mean /
+// std) bits: the producers' sums are fp64 (or fp32 about a per-thread shift, converted per thread), so a group's mean
+// may dominate its spread.
+__global__ void gn_finalize_kernel(const double* __restrict__ partial, int tiles_per_img, const double* __restrict__ ring,
                                    int ring_per_img, double inv_count, float eps,
                                    float* __restrict__ mean_rstd /* [B][4][2] */) {
   const int b = blockIdx.x >> 2, g = blockIdx.x & 3;
   double s = 0.0, s2 = 0.0;
   for (int t = threadIdx.x; t < tiles_per_img + ring_per_img; t += blockDim.x) {
-    const float* q = (t < tiles_per_img ? partial + (static_cast<size_t>(b) * tiles_per_img + t) * 8
+    const double* q = (t < tiles_per_img ? partial + (static_cast<size_t>(b) * tiles_per_img + t) * 8
                                         : ring + (static_cast<size_t>(b) * ring_per_img + t - tiles_per_img) * 8) + g * 2;
-    s += static_cast<double>(q[0]);
-    s2 += static_cast<double>(q[1]);
+    s += q[0];
+    s2 += q[1];
   }
   __shared__ double sh[2][32];
   for (int o = 16; o > 0; o >>= 1) {
@@ -588,7 +590,7 @@ __global__ void __launch_bounds__(256) conv3x3_simt_kernel(const SimtArgs a) {
   constexpr int PXT = TILE_M / PGS;      // pixels per thread (8 or 2)
   __shared__ float s_in[(TILE_H + 2) * (TILE_W + 2)][CK];
   __shared__ float s_w[9][CK][CO_T];
-  __shared__ float s_red[4][2];
+  __shared__ double s_red[4][2];
   const ConvArgs& p = a.c;
   const int tile = blockIdx.x;
   const int co0 = blockIdx.y * CO_T;
@@ -600,7 +602,7 @@ __global__ void __launch_bounds__(256) conv3x3_simt_kernel(const SimtArgs a) {
   for (int i = 0; i < PXT; ++i)
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  if (threadIdx.x < 8) (&s_red[0][0])[threadIdx.x] = 0.f;
+  if (threadIdx.x < 8) (&s_red[0][0])[threadIdx.x] = 0.0;
 
   for (int k0 = 0; k0 < CIN; k0 += CK) {
     __syncthreads();
@@ -638,7 +640,7 @@ __global__ void __launch_bounds__(256) conv3x3_simt_kernel(const SimtArgs a) {
     }
   }
   // epilogue
-  float ls[4] = {0.f, 0.f, 0.f, 0.f}, ls2[4] = {0.f, 0.f, 0.f, 0.f};
+  double ls[4] = {0.0, 0.0, 0.0, 0.0}, ls2[4] = {0.0, 0.0, 0.0, 0.0};  // fp64 per element (check path)
   bool ov = false;
 #pragma unroll
   for (int i = 0; i < PXT; ++i) {
@@ -663,8 +665,9 @@ __global__ void __launch_bounds__(256) conv3x3_simt_kernel(const SimtArgs a) {
         for (int j = 0; j < 4; ++j) {
           const int g = (co0 + cg * 4 + j) / (COUT / 4);
           const int gl = (COUT / 4 >= CO_T) ? 0 : (g - co0 / (COUT / 4));
-          ls[gl] += v[j];
-          ls2[gl] = fmaf(v[j], v[j], ls2[gl]);
+          const double d = v[j];
+          ls[gl] += d;
+          ls2[gl] = fma(d, d, ls2[gl]);
         }
       }
     }

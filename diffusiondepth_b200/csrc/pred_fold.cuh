@@ -65,7 +65,7 @@ struct FoldArgs {
   const float* bias;     // b5 [64]
   float acc_scale;       // 1 / (act_scale * K5 scale)
   float* y32;            // [B*H*W][64]
-  float* stats_partial;  // [num_tiles][4][2], interior pixels only
+  double* stats_partial;  // [num_tiles][4][2] fp64 sums, interior pixels only
 };
 
 __global__ void __launch_bounds__(F5::THREADS, 1)
@@ -80,7 +80,7 @@ conv5x5_fold_kernel(const __grid_constant__ CUtensorMap tmP_hi, const __grid_con
   uint64_t* p_empty = p_full + F5::P_SLOTS;
   uint64_t* w_full = p_empty + F5::P_SLOTS;
   uint64_t* w_empty = w_full + F5::W_SLOTS;
-  float* red = reinterpret_cast<float*>(w_empty + F5::W_SLOTS);  // [2 par][2 wg][4 warps][2]
+  double* red = reinterpret_cast<double*>(w_empty + F5::W_SLOTS);  // [2 par][2 wg][4 warps][2]
   float* stage = reinterpret_cast<float*>(ctrl + F5::CTRL_BYTES);
 
   const int warp = threadIdx.x >> 5;
@@ -214,7 +214,9 @@ conv5x5_fold_kernel(const __grid_constant__ CUtensorMap tmP_hi, const __grid_con
       const int x0 = tx * F5_TW, yw = ty * F5_TH + wg * 8;
       const int co0 = 16 * q + (lane >> 2);  // this thread's output channels: co0 and co0 + 8 (GroupNorm group q)
       const float bias0 = __ldg(p.bias + co0), bias1 = __ldg(p.bias + co0 + 8);
-      float tsum = 0.f, tsq = 0.f;
+      // as conv3x3_halo_kernel sums: d = v - k in fp32, k = this thread's first interior value, then fp64 sums of v, v^2
+      float tk = 0.f, tsum = 0.f, tsq = 0.f;
+      int tn = 0;
 #pragma unroll
       for (int cj = 0; cj < F5_TW / 4; ++cj) {
         named_bar_sync(2 + wg, 128);  // the previous chunk's staging reads are done
@@ -228,8 +230,10 @@ conv5x5_fold_kernel(const __grid_constant__ CUtensorMap tmP_hi, const __grid_con
             const int y = yw + yl;
             const float v = fmaf(acc0[4 * i + e] + acc1[4 * i + e], p.acc_scale, (e >> 1) ? bias1 : bias0);
             if (x > 0 && x < p.W - 1 && y > 0 && y < p.H - 1) {  // interior; ring_fix_kernel sums the ring
-              tsum += v;
-              tsq = fmaf(v, v, tsq);
+              if (tn++ == 0) tk = v;
+              const float d = v - tk;
+              tsum += d;
+              tsq = fmaf(d, d, tsq);
             }
             S[(ii * 8 + yl) * F5::LD + co0 + 8 * (e >> 1)] = v;
           }
@@ -248,14 +252,16 @@ conv5x5_fold_kernel(const __grid_constant__ CUtensorMap tmP_hi, const __grid_con
         }
       }
       // warp q holds exactly GroupNorm group q: warp tree, then the two warpgroups in fixed order
+      const double n = tn, kk = tk, ds = tsum;
+      double s = fma(n, kk, ds), s2 = fma(n * kk, kk, fma(2.0 * kk, ds, static_cast<double>(tsq)));
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
-        tsum += __shfl_xor_sync(0xffffffffu, tsum, o);
-        tsq += __shfl_xor_sync(0xffffffffu, tsq, o);
+        s += __shfl_xor_sync(0xffffffffu, s, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
       }
       if (lane == 0) {
-        red[((par * 2 + wg) * 4 + q) * 2 + 0] = tsum;
-        red[((par * 2 + wg) * 4 + q) * 2 + 1] = tsq;
+        red[((par * 2 + wg) * 4 + q) * 2 + 0] = s;
+        red[((par * 2 + wg) * 4 + q) * 2 + 1] = s2;
       }
       named_bar_sync(1, 256);
       const int e = threadIdx.x - 128;
@@ -283,7 +289,7 @@ constexpr int RING_ABOX = RING_S + 4;  // a(q + d'): 5 x (n + 4) box
 constexpr int RING_JG = 4;
 constexpr int RING_JB = (RING_BOX + RING_JG - 1) / RING_JG;
 constexpr int RING_THREADS = 256 * RING_JG;
-constexpr int RING_SMEM = (5 * RING_ABOX + 3 * RING_BOX + 2) * 256 * 4 + RING_S * 64 * 4;
+constexpr int RING_SMEM = (5 * RING_ABOX + 3 * RING_BOX + 4) * 256 * 4 + RING_S * 64 * 4;
 
 struct RingSide {
   int y0, x0, vert, len;
@@ -320,7 +326,7 @@ struct RingArgs {
   const float* bb;           // convB bias [256]
   const float* wp;           // pred.0 [9][256 cm][64 co] fp32
   float* y32;                // [B][H][W][64]: the composed conv's output, corrected in place on the ring
-  float* ring_partial;       // [B][blocks_per_img][4][2] GroupNorm sums of the corrected ring pixels
+  double* ring_partial;      // [B][blocks_per_img][4][2] GroupNorm fp64 sums of the corrected ring pixels
 };
 
 __device__ __forceinline__ bool inside_img(int y, int x, int H, int W) { return y >= 0 && y < H && x >= 0 && x < W; }
@@ -330,15 +336,15 @@ __global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p
   extern __shared__ float4 ring_smem4[];
   float* abox = reinterpret_cast<float*>(ring_smem4);  // [5][RING_ABOX][256]
   float* bbox = abox + 5 * RING_ABOX * 256;           // [3][RING_BOX][256]
-  float* red = bbox + 3 * RING_BOX * 256;             // [2][256]
-  float* ycor = red + 2 * 256;                        // [RING_S][64] corrected outputs of the segment
+  double* red = reinterpret_cast<double*>(bbox + 3 * RING_BOX * 256);  // [2][256]
+  float* ycor = bbox + (3 * RING_BOX + 4) * 256;      // [RING_S][64] corrected outputs of the segment
   const int img = blockIdx.y, t = threadIdx.x;
   const int H = p.H, W = p.W;
   RingSide sd[4];
   ring_sides(H, W, sd);
   const int s_begin = static_cast<int>(static_cast<long long>(p.nseg) * blockIdx.x / p.blocks_per_img);
   const int s_end = static_cast<int>(static_cast<long long>(p.nseg) * (blockIdx.x + 1) / p.blocks_per_img);
-  float ts = 0.f, tq = 0.f;
+  double ts = 0.0, tq = 0.0;  // fp64 per element: the ring is a few pixels per block
   for (int sg = s_begin; sg < s_end; ++sg) {
     int k = sg, si = 0;
     while (k >= (sd[si].len + RING_S - 1) / RING_S) {
@@ -439,9 +445,9 @@ __global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p
     // GroupNorm sums: thread t < 256 takes every 4th pixel, in the same order whatever RING_THREADS is
     if (t < 256)
       for (int j = t >> 6; j < n; j += 4) {
-        const float v = ycor[j * 64 + co];
+        const double v = ycor[j * 64 + co];
         ts += v;
-        tq = fmaf(v, v, tq);
+        tq = fma(v, v, tq);
       }
   }
   // GroupNorm partials of this block's ring pixels, summed in a fixed order
@@ -452,7 +458,7 @@ __global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p
   __syncthreads();
   if (t < 8) {
     const int g = t >> 1, which = t & 1;
-    float s = 0.f;
+    double s = 0.0;
     for (int pg = 0; pg < 4; ++pg)
       for (int c = 0; c < 16; ++c) s += red[which * 256 + pg * 64 + g * 16 + c];
     p.ring_partial[((static_cast<size_t>(img) * p.blocks_per_img + blockIdx.x) * 4 + g) * 2 + which] = s;

@@ -670,6 +670,30 @@ class DenoiseEngine:
                                            float(eps), C.c_void_p(self._stream())))
         return out
 
+    def conv_groupnorm(self, x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor,
+                       beta: torch.Tensor, mode: int, cond: Optional[torch.Tensor] = None,
+                       temb: Optional[torch.Tensor] = None, latent: Optional[torch.Tensor] = None, c_x: float = 0.0,
+                       c_eps: float = 0.0, up_qpb: int = 4):
+        """One GroupNorm(4, Cout)'d conv of the DDIM loop on the loop's kernels (dd_conv_groupnorm): x [B, Cin, H, W]
+        -> conv -> GroupNorm + ReLU, then mode 0 nothing, 1 + cond [B, 256, H, W] + temb [B, 256], 2 + bilinear
+        up(cond [B, 256, h, w] + temb), 3 the DDIM update (latent [B, 16, H, W] is updated in place; None: eps only).
+        Returns (y32 the conv output, mean_rstd [B, 4, 2], out [B, Cout, H, W])."""
+        dev = self.device
+        x, w, b, gamma, beta, cond, temb = (_f32(t, dev) for t in (x, w, b, gamma, beta, cond, temb))
+        B, cin, H, W = x.shape
+        cout = w.shape[0]
+        d = _cabi.DDConvGnDesc()
+        d.batch, d.cin, d.cout, d.height, d.width, d.mode = B, cin, cout, H, W, int(mode)
+        d.cond_h, d.cond_w = (cond.shape[2], cond.shape[3]) if cond is not None else (0, 0)
+        d.up_qpb, d.c_x, d.c_eps = int(up_qpb), float(c_x), float(c_eps)
+        y32 = torch.full((B, cout, H, W), float("nan"), device=dev)
+        mean_rstd = torch.full((B, 4, 2), float("nan"), device=dev)
+        out = torch.full((B, cout, H, W), float("nan"), device=dev)
+        _cabi.check(self.lib.dd_conv_groupnorm(self._h, C.byref(d), _ptr(x), _ptr(w), _ptr(b), _ptr(gamma), _ptr(beta),
+                                               _ptr(cond), _ptr(temb), _ptr(latent), _ptr(y32), _ptr(mean_rstd),
+                                               _ptr(out), C.c_void_p(self._stream())))
+        return y32, mean_rstd, out
+
     def bench_conv(self, cin: int, cout: int, iters: int = 20) -> float:
         """Average milliseconds per launch of the (cin -> cout) conv on this engine's latent grid."""
         ms = C.c_float()

@@ -492,6 +492,27 @@ int dd_depthwise_conv(dd_handle h, const float* x, const float* w, const float* 
 int dd_layer_norm(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, int32_t tokens,
                   int32_t channels, float eps, void* cuda_stream);
 
+typedef struct dd_conv_gn_desc {
+  int32_t batch, cin, cout, height, width; /* one of the loop's GroupNorm'd convs: 16->64, 64->256, 256->64, 64->16 */
+  int32_t mode;            /* 0 GN + ReLU (Cout 64); 1 + cond (same grid) + temb (Cout 256); 2 + bilinear up(cond + temb),
+                              align_corners=True (Cout 256); 3 GN + ReLU -> the DDIM update (Cout 16) */
+  int32_t cond_h, cond_w;  /* mode 2: the condition's grid */
+  int32_t up_qpb;          /* mode 2: quads per block of the up-add kernel, 4 or 1 */
+  float c_x, c_eps;        /* mode 3 with a latent: x <- c_x x + c_eps eps */
+} dd_conv_gn_desc;
+
+/* Standalone GroupNorm(4, Cout)'d conv of the DDIM loop, through the loop's own kernels: the 3x3 conv (the engine's
+ * choice, DD_FLAG_SIMT_CONV honoured) with its GroupNorm-statistics epilogue, the fp64 finalize and the apply kernel of
+ * `mode`.  x [B][cin][H][W], w [cout][cin][3][3], b / gamma / beta [cout]; cond [B][256][cond grid] and temb [B][256]
+ * (modes 1 and 2); latent [B][16][H][W] (mode 3, nullable: null writes eps, otherwise it is updated in place), all
+ * device fp32.  Outputs, each nullable: y32 [B][cout][H][W] the conv output before the norm, mean_rstd [B][4][2], out
+ * [B][cout][H][W] the layer's output in fp32, rebuilt from the hi/lo planes the apply kernel wrote (mode 3: eps, or
+ * the updated latent's planes).  Allocates and frees its own buffers; synchronises and returns DD_ERR_RANGE as
+ * dd_gen_layer does. */
+int dd_conv_groupnorm(dd_handle h, const dd_conv_gn_desc* d, const float* x, const float* w, const float* b,
+                      const float* gamma, const float* beta, const float* cond, const float* temb, float* latent,
+                      float* y32, float* mean_rstd, float* out, void* cuda_stream);
+
 /* Time the dominant kernel (convA-shaped 256->256 3x3 on the engine's latent grid) `iters` times with
  * CUDA events on `cuda_stream`; returns average milliseconds per launch in *ms_out. */
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,
