@@ -1,21 +1,15 @@
 // Training-mode BatchNorm of the depth codec (dd_set_codec_mode(DD_CODEC_TRAIN)): batch statistics of the pre-BN value,
 // folded on the device into a copy of the weights that the unchanged decoder_kernel / encoder_kernel then run on, and
-// the decoder backward's extra term through the batch mean and variance.
-//
-// Statistics take two passes over the same values: pass 1 sums u, pass 2 sums d = u - m and d^2 with m = the pass-1
-// mean rounded to fp32, so the variance is a mean of squared deviations (no E[u^2] - mean^2 cancellation when
-// |mean| >> std) and sum d corrects the rounding of m.  Every reduction writes fixed per-block fp64 partials that a
-// second kernel sums in block order: the statistics, the folded weights and the gradients are bit-reproducible.
-//
-// Across ranks (dd_set_bn_allgather) every total above is gathered with the local item count and summed in rank order
-// (bn_rank_sum_kernel); the kernels then divide by the global count *cnt instead of their own n (cnt null: n).
+// the decoder backward's extra term through the batch mean and variance.  The two statistics passes, their partials
+// and the cross-rank totals follow bn_stats.cuh.
 #pragma once
 #include "backward.cuh"
+#include "bn_stats.cuh"
 
 namespace dd {
 
-constexpr int BNS_PIX = 1024;  // items per block of bn_stats_kernel (4 per thread)
-constexpr int BNS_COLS = 32;   // partials per block: sum d [16], sum d^2 [16]
+constexpr int BNS_PIX = 1024;     // items per block of bn_stats_kernel (4 per thread)
+constexpr int BNS_COLS = 2 * 16;  // partials per block: [2][16], sum d then sum d^2 of the 16 channels
 
 // The pre-BatchNorm values (16 channels per item) of the codec's three BatchNorms.  load() stages what eval() reads in
 // shared memory (SMEM floats).
@@ -130,8 +124,8 @@ struct EncPreBn2 {
   }
 };
 
-// Per-block sums over the block's BNS_PIX items: columns 0..15 sum d, 16..31 sum d^2, d = u - m.  Pass 1: sum1 null,
-// m = 0; pass 2: m = fp32(sum1 / N), N = *cnt or n when cnt is null.
+// Per-block partials [2][16] over the block's BNS_PIX items: sum d, sum d^2, d = u - m.  Pass 1: sum1 null, m = 0;
+// pass 2: m = fp32(sum1 / N), N = *cnt or n when cnt is null.
 template <class Op>
 __global__ void __launch_bounds__(256) bn_stats_kernel(const Op op, long long n, const double* __restrict__ sum1,
                                                        const double* __restrict__ cnt, double* __restrict__ part) {
@@ -174,40 +168,12 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(const Op op, long long n,
   }
 }
 
-// out[c] = sum over blocks, in block order, of part[b * stride + c], c < ncols (one thread per column).  count > 0:
-// out[ncols] = count as well, the row a cross-rank gather sends (the launch then covers ncols + 1 threads).
-__global__ void part_colsum_kernel(const double* __restrict__ part, int nblk, int stride, int ncols,
-                                   double* __restrict__ out, long long count) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c == ncols && count > 0) out[c] = static_cast<double>(count);
-  if (c >= ncols) return;
-  double s = 0.0;
-  for (int b = 0; b < nblk; ++b) s += part[static_cast<size_t>(b) * stride + c];
-  out[c] = s;
-}
-
-// out[j] = rows[0][j] + rows[1][j] + ... + rows[R - 1][j], added in rank order, j < cols: the gathered per-rank totals
-// of a cross-rank BatchNorm (count last), so every rank folds the same union-batch statistics, bit for bit.
-__global__ void __launch_bounds__(256) bn_rank_sum_kernel(const double* __restrict__ rows, int R, int cols,
-                                                          double* __restrict__ out) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= cols) return;
-  double s = rows[j];
-  for (int r = 1; r < R; ++r) s += rows[static_cast<size_t>(r) * cols + j];
-  out[j] = s;
-}
-
-// Fold the batch statistics of pass 2 into a copy of one conv's weights:
-//   s = gamma / sqrt(var_b + 1e-5) in fp64, rounded once (as the host fold of the running statistics),
+// Fold the batch statistics (bn_batch_stats) into a copy of one conv's weights:
 //   w_out = w s (output channel = index % 16),  b_out = (bias - mean_b) s + beta = beta - mean_conv s,
 // where the statistics were taken of the convolution without its bias (mean_b = mean_conv + bias),
 // and the record of this evaluation: batch mean and unbiased variance.
 struct BnFoldArgs {
-  const double* sum1;  // [16] pass-1 sums
-  const double* part;  // [nblk][BNS_COLS] pass-2 partials
-  int nblk;
-  long long n;
-  const double* cnt;   // null, or the global item count across ranks (used instead of n)
+  BnFoldIn in;  // C = 16
   const float *gamma, *beta;
   const float* bias;  // the conv's own bias in front of the BatchNorm, not in the statistics (null: none)
   const float* w;     // unfolded weights, output channel fastest
@@ -221,27 +187,19 @@ __global__ void __launch_bounds__(256) bn_fold_kernel(const BnFoldArgs f) {
   __shared__ double s_sc[16];
   const int c = threadIdx.x;
   if (c < 16) {
-    double d1 = 0.0, d2 = 0.0;
-    for (int b = 0; b < f.nblk; ++b) {
-      d1 += f.part[static_cast<size_t>(b) * BNS_COLS + c];
-      d2 += f.part[static_cast<size_t>(b) * BNS_COLS + 16 + c];
-    }
-    const double nn = f.cnt ? *f.cnt : static_cast<double>(f.n);
-    const double dm = d1 / nn;  // mean of d: the rounding of the shift
-    const double mean_conv = static_cast<double>(static_cast<float>(f.sum1[c] / nn)) + dm;
-    const double mean = mean_conv + (f.bias ? static_cast<double>(f.bias[c]) : 0.0);
-    const double var = fmax(d2 / nn - dm * dm, 0.0);
-    const double sc = static_cast<double>(f.gamma[c]) / sqrt(var + 1e-5);
-    s_sc[c] = sc;
-    f.b_out[c] = static_cast<float>(static_cast<double>(f.beta[c]) - mean_conv * sc);
+    // read before the statistics: ptxas then keeps 11 partials' loads in flight in their latency-bound sum, not 8
+    const double bias = f.bias ? static_cast<double>(f.bias[c]) : 0.0;
+    const BnBatchStats b = bn_batch_stats(f.in, 16, c, f.gamma);
+    s_sc[c] = b.scale;
+    f.b_out[c] = static_cast<float>(static_cast<double>(f.beta[c]) - b.mean * b.scale);
     if (f.bn_out) {
-      f.bn_out[c] = static_cast<float>(sc);
-      f.bn_out[16 + c] = static_cast<float>(mean_conv);
-      f.bn_out[32 + c] = static_cast<float>(1.0 / sqrt(var + 1e-5));
+      f.bn_out[c] = static_cast<float>(b.scale);
+      f.bn_out[16 + c] = static_cast<float>(b.mean);
+      f.bn_out[32 + c] = static_cast<float>(1.0 / sqrt(b.var + 1e-5));
     }
     if (f.rec) {
-      f.rec[c] = static_cast<float>(mean);
-      f.rec[16 + c] = static_cast<float>(var * nn / (nn - 1.0));
+      f.rec[c] = static_cast<float>(b.mean + bias);
+      f.rec[16 + c] = static_cast<float>(b.var_unbiased);
     }
   }
   __syncthreads();

@@ -473,7 +473,7 @@ struct dd_engine {
     float* zero16 = nullptr;  // [16] zeros: the ConvT bias of the decoder backward's xhat (bn's mean is bias-free)
     float *enc_w1 = nullptr, *enc_w2 = nullptr, *enc_gb = nullptr;  // unfolded encoder; [4][16] gamma1, beta1, gamma2, beta2
     float *enc_w1f = nullptr, *enc_b1f = nullptr, *enc_w2f = nullptr, *enc_b2f = nullptr;  // batch-folded encoder
-    double *part = nullptr, *sum1 = nullptr;     // bn_stats_kernel partials [blocks][32]; pass-1 sums [16]
+    double *part = nullptr, *sum1 = nullptr;     // bn_stats_kernel partials [blocks][2][16]; pass-1 sums [16]
     double *sums = nullptr, *part_db = nullptr;  // decoder backward: [32] sum dv, sum dv xhat; [act blocks][16]
     float* rec = nullptr;                        // [max(T, 2)][2][16] batch mean, unbiased variance
     int nrec = 0;                                // records the last forward entry wrote
@@ -671,39 +671,61 @@ void free_bn_sync(dd_engine* e) {
   s.cap = 0;
 }
 
-// Across ranks (dd_set_bn_allgather), before a BatchNorm's first gather: room for rows of `cols` doubles.  The first
-// BatchNorm with wider rows waits for the old buffers' readers and grows them (tot1 / tot2 hold nothing across
-// BatchNorms).
-int bn_sync_reserve(dd_engine* e, int cols, cudaStream_t st) {
+// What a consumer of batch statistics reads: totals, and the count to divide them by (null: its own item count).
+struct BnTotals {
+  const double* sum;
+  const double* cnt;
+};
+
+// The totals of columns [0, ncols) of nblk block partials (stride doubles apart), summed in block order.  On one GPU
+// they go to `local`.  Across ranks (dd_set_bn_allgather) this rank's totals and its item count n go out as one row,
+// and every rank's row summed in rank order (the count last) lands in tot1 when reserve > 0: the BatchNorm's first
+// gather, which makes room for its widest row of `reserve` columns; or in tot2 when reserve is 0 (its second).
+int bn_totals(dd_engine* e, const double* part, int nblk, int stride, int ncols, long long n, double* local,
+              int reserve, cudaStream_t st, BnTotals* out) {
   dd_engine::BnSync& s = e->sync;
-  if (cols > s.cap) {
+  int rc;
+  if (!s.fn) {
+    dd::part_colsum_kernel<<<(ncols + 255) / 256, 256, 0, st>>>(part, nblk, stride, ncols, local, 0);
+    *out = {local, nullptr};
+    return launched(e, "part_colsum");
+  }
+  if (reserve > s.cap) {  // wait for the old buffers' readers (tot1 / tot2 hold nothing across BatchNorms), then grow
     CUDA_TRY(cudaStreamSynchronize(st));
     free_bn_sync(e);
-    const size_t b = static_cast<size_t>(cols) * sizeof(double);
+    const size_t b = static_cast<size_t>(reserve) * sizeof(double);
     if (cudaMalloc(&s.row, b) != cudaSuccess || cudaMalloc(&s.rows, b * s.world) != cudaSuccess ||
         cudaMalloc(&s.tot1, b) != cudaSuccess || cudaMalloc(&s.tot2, b) != cudaSuccess) {
       free_bn_sync(e);
       return fail(DD_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(cudaGetLastError()));
     }
-    s.cap = cols;
+    s.cap = reserve;
   }
-  return DD_OK;
-}
-
-// Across ranks: this rank's totals over nblk partial rows (stride doubles apart, ncols columns) and its item count n go
-// out as one row; tot2 (second) or tot1 [0 .. ncols] = every rank's row summed in rank order (the count last).  The
-// BatchNorm reserved ncols + 1 columns.
-int bn_sync_totals(dd_engine* e, const double* part, int nblk, int stride, int ncols, long long n, bool second,
-                   cudaStream_t st) {
-  dd_engine::BnSync& s = e->sync;
   const int cols = ncols + 1;
-  int rc;
   dd::part_colsum_kernel<<<(cols + 255) / 256, 256, 0, st>>>(part, nblk, stride, ncols, s.row, n);
   if ((rc = launched(e, "part_colsum"))) return rc;
   const int r = s.fn(s.row, s.rows, cols, st, s.user);
   if (r != 0) return fail(DD_ERR_CUDA, "BatchNorm statistics all-gather callback failed (returned " + std::to_string(r) + ")");
-  dd::bn_rank_sum_kernel<<<(cols + 255) / 256, 256, 0, st>>>(s.rows, s.world, cols, second ? s.tot2 : s.tot1);
+  double* tot = reserve > 0 ? s.tot1 : s.tot2;
+  dd::bn_rank_sum_kernel<<<(cols + 255) / 256, 256, 0, st>>>(s.rows, s.world, cols, tot);
+  *out = {tot, tot + ncols};
   return launched(e, "bn_rank_sum");
+}
+
+// One training-mode BatchNorm over n items of C channels: two statistics passes into the partials part [nblk][2][C]
+// (pass-1 totals on one GPU in sum1_local), then the fold.  stats(sum1, cnt) launches a pass (pass 1: both null);
+// fold(const dd::BnFoldIn&) launches the fold.
+template <class Stats, class Fold>
+int run_bn_passes(dd_engine* e, double* part, int nblk, int C, long long n, double* sum1_local, cudaStream_t st,
+                  const Stats& stats, const Fold& fold) {
+  BnTotals t1, t2;
+  int rc;
+  if ((rc = stats(nullptr, nullptr))) return rc;
+  if ((rc = bn_totals(e, part, nblk, 2 * C, C, n, sum1_local, 2 * C + 1, st, &t1))) return rc;
+  if ((rc = stats(t1.sum, t1.cnt))) return rc;
+  if (!e->sync.fn) return fold(dd::BnFoldIn{t1.sum, part, nblk, n, nullptr});
+  if ((rc = bn_totals(e, part, nblk, 2 * C, 2 * C, n, nullptr, 0, st, &t2))) return rc;
+  return fold(dd::BnFoldIn{t1.sum, t2.sum, 1, n, t2.cnt});
 }
 
 void drop_graph(dd_engine* e, int which) {
@@ -1157,45 +1179,33 @@ int split_planes(dd_engine* e, const float* x, __half* hi, __half* lo, size_t n,
   return check_launch("split_planes");
 }
 
-// Training-mode BatchNorm over n items of op's pre-BN value: two statistics passes, then the fold of (gamma, beta) =
-// gb[0..15], gb[16..31] into w_out / b_out (see dd::BnFoldArgs for the other pointers).
+// A codec BatchNorm in training mode over n items of op's pre-BN value (run_bn_passes): bn_stats_kernel's two passes,
+// then the fold of (gamma, beta) = gb[0..15], gb[16..31] into w_out / b_out (see dd::BnFoldArgs for the other pointers).
 template <class Op>
-int run_bn_batch(dd_engine* e, const Op& op, long long n, const float* gb, const float* bias, const float* w, int nw,
+int run_codec_bn(dd_engine* e, const Op& op, long long n, const float* gb, const float* bias, const float* w, int nw,
                  float* w_out, float* b_out, float* bn_out, float* rec, cudaStream_t st) {
   dd_engine::CodecTrain& ct = e->ct;
-  const dd_engine::BnSync& sy = e->sync;
   const int nblk = codec_stats_blocks(n);
-  int rc;
-  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, nullptr, nullptr, ct.part);
-  if ((rc = launched(e, "bn_stats"))) return rc;
-  if (sy.fn) {
-    if ((rc = bn_sync_reserve(e, dd::BNS_COLS + 1, st))) return rc;
-    if ((rc = bn_sync_totals(e, ct.part, nblk, dd::BNS_COLS, 16, n, false, st))) return rc;
-  } else {
-    dd::part_colsum_kernel<<<1, 32, 0, st>>>(ct.part, nblk, dd::BNS_COLS, 16, ct.sum1, 0);
-    if ((rc = launched(e, "part_colsum"))) return rc;
-  }
-  const double* sum1 = sy.fn ? sy.tot1 : ct.sum1;
-  dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, sum1, sy.fn ? sy.tot1 + 16 : nullptr, ct.part);
-  if ((rc = launched(e, "bn_stats"))) return rc;
-  if (sy.fn && (rc = bn_sync_totals(e, ct.part, nblk, dd::BNS_COLS, dd::BNS_COLS, n, true, st))) return rc;
-  dd::BnFoldArgs f;
-  f.sum1 = sum1;
-  f.part = sy.fn ? sy.tot2 : ct.part;  // across ranks the union's totals, as one block of partials
-  f.nblk = sy.fn ? 1 : nblk;
-  f.n = n;
-  f.cnt = sy.fn ? sy.tot2 + dd::BNS_COLS : nullptr;
-  f.gamma = gb;
-  f.beta = gb + 16;
-  f.bias = bias;
-  f.w = w;
-  f.nw = nw;
-  f.w_out = w_out;
-  f.b_out = b_out;
-  f.bn_out = bn_out;
-  f.rec = rec;
-  dd::bn_fold_kernel<<<1, 256, 0, st>>>(f);
-  return launched(e, "bn_fold");
+  auto stats = [&](const double* sum1, const double* cnt) {
+    dd::bn_stats_kernel<Op><<<nblk, 256, 0, st>>>(op, n, sum1, cnt, ct.part);
+    return launched(e, "bn_stats");
+  };
+  auto fold = [&](const dd::BnFoldIn& in) {
+    dd::BnFoldArgs f;
+    f.in = in;
+    f.gamma = gb;
+    f.beta = gb + 16;
+    f.bias = bias;
+    f.w = w;
+    f.nw = nw;
+    f.w_out = w_out;
+    f.b_out = b_out;
+    f.bn_out = bn_out;
+    f.rec = rec;
+    dd::bn_fold_kernel<<<1, 256, 0, st>>>(f);
+    return launched(e, "bn_fold");
+  };
+  return run_bn_passes(e, ct.part, nblk, 16, n, ct.sum1, st, stats, fold);
 }
 
 // DD_CODEC_TRAIN: the decoder BatchNorm's statistics over the latent in x32, folded into ct.dec_wt / dec_bt / dec_bn
@@ -1204,7 +1214,7 @@ int run_dec_batch_stats(dd_engine* e, float* rec, cudaStream_t st) {
   const Geom g = geom_of(e->cfg);
   const dd::DecPreBn op{e->x32, e->dec_wu, g.h, g.w};
   dd_engine::CodecTrain& ct = e->ct;
-  return run_bn_batch(e, op, static_cast<long long>(g.B) * g.P * 4, ct.dec_gb, e->dec_bu, e->dec_wu, 4096, ct.dec_wt,
+  return run_codec_bn(e, op, static_cast<long long>(g.B) * g.P * 4, ct.dec_gb, e->dec_bu, e->dec_wu, 4096, ct.dec_wt,
                       ct.dec_bt, ct.dec_bn, rec, st);
 }
 
@@ -2020,35 +2030,25 @@ int pack_prod_train(dd_engine* e, cudaStream_t st) {
   return DD_OK;
 }
 
-// The training-mode BatchNorm of record b on the pre-BN value in pt.U (b.n pixels): the batch statistics (across ranks
-// with dd_set_bn_allgather) and fold, which write the record, then act(s u + t) (`act` as the eval epilogue's code)
+// The training-mode BatchNorm of record b on the pre-BN value in pt.U (b.n pixels): pbn_stats_kernel's two passes and
+// the fold (run_bn_passes), which write the record, then act(s u + t) (`act` as the eval epilogue's code)
 // with the addend add32 placed as add_first says, into y32 and / or the planes *out (row width ld_out, 0: b.C).
-int run_bn_batch(dd_engine* e, const dd_engine::ProdBn& b, int act, int add_first, const float* add32, float* y32,
-                 const Planes* out, int ld_out, int ch_off, cudaStream_t st) {
+int run_producer_bn(dd_engine* e, const dd_engine::ProdBn& b, int act, int add_first, const float* add32, float* y32,
+                    const Planes* out, int ld_out, int ch_off, cudaStream_t st) {
   dd_engine::ProdTrain& pt = e->pt;
   const long long n = b.n;
   const int C = b.C, nblk = pbn_blocks(n);
   const dim3 grid(nblk, (C + dd::PBN_CH - 1) / dd::PBN_CH), block(dd::PBN_CH, 8);
-  const dd_engine::BnSync& sy = e->sync;
+  auto stats = [&](const double* sum1, const double* cnt) {
+    dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, sum1, cnt, pt.part);
+    return launched(e, "pbn_stats");
+  };
+  auto fold = [&](const dd::BnFoldIn& in) {
+    dd::pbn_fold_kernel<<<(C + 255) / 256, 256, 0, st>>>(in, C, b.gamma, b.beta, pt.s, pt.t, pt.rec + b.rec_off);
+    return launched(e, "pbn_fold");
+  };
   int rc;
-  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, nullptr, nullptr, pt.part);
-  if ((rc = launched(e, "pbn_stats"))) return rc;
-  if (sy.fn) {
-    if ((rc = bn_sync_reserve(e, 2 * C + 1, st))) return rc;
-    if ((rc = bn_sync_totals(e, pt.part, nblk, 2 * C, C, n, false, st))) return rc;
-  } else {
-    dd::pbn_colsum_kernel<<<(C + 255) / 256, 256, 0, st>>>(pt.part, nblk, C, pt.sum1);
-    if ((rc = launched(e, "pbn_colsum"))) return rc;
-  }
-  const double* sum1 = sy.fn ? sy.tot1 : pt.sum1;
-  dd::pbn_stats_kernel<<<grid, block, 0, st>>>(pt.U, n, C, sum1, sy.fn ? sy.tot1 + C : nullptr, pt.part);
-  if ((rc = launched(e, "pbn_stats"))) return rc;
-  if (sy.fn && (rc = bn_sync_totals(e, pt.part, nblk, 2 * C, 2 * C, n, true, st))) return rc;
-  // across ranks the fold reads the union's totals [2][C] as one block of partials
-  dd::pbn_fold_kernel<<<(C + 255) / 256, 256, 0, st>>>(sum1, sy.fn ? sy.tot2 : pt.part, sy.fn ? 1 : nblk, n,
-                                                        sy.fn ? sy.tot2 + 2 * C : nullptr, C, b.gamma, b.beta, pt.s,
-                                                        pt.t, pt.rec + b.rec_off);
-  if ((rc = launched(e, "pbn_fold"))) return rc;
+  if ((rc = run_bn_passes(e, pt.part, nblk, C, n, pt.sum1, st, stats, fold))) return rc;
   dd::PbnApplyArgs a;
   a.u = pt.U;
   a.n = n;
@@ -2088,7 +2088,7 @@ int run_gen(dd_engine* e, const GenLayer& L, const Planes& a0, int c0, const Pla
   if ((rc = launch_gen(e, raw, 0, {e->cfg.batch, H, W, 0, src_h, src_w}, a0, c0, a1, c1, pt.U, nullptr, nullptr, 0, 0,
                        st, 0, nullptr, e->prod.KS)))
     return rc;
-  return run_bn_batch(e, b, L.relu, L.add_first, add32, y32, out, ld_out, ch_off, st);
+  return run_producer_bn(e, b, L.relu, L.add_first, add32, y32, out, ld_out, ch_off, st);
 }
 
 // A forward starts (dd_run_backbone, dd_build_condition with feature maps): no record is current.
@@ -2614,16 +2614,9 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
   dd::dec_bwd_act_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a);
   if ((rc = launched(e, "dec_bwd_act"))) return rc;
   if (train) {  // du through the batch mean and variance (across ranks: the union batch's sums and count)
-    const dd_engine::BnSync& sy = e->sync;
-    if (sy.fn) {
-      if ((rc = bn_sync_reserve(e, 33, st))) return rc;
-      if ((rc = bn_sync_totals(e, l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, nout, false, st))) return rc;
-    } else {
-      dd::part_colsum_kernel<<<1, 32, 0, st>>>(l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, e->ct.sums, 0);
-      if ((rc = launched(e, "part_colsum"))) return rc;
-    }
-    dd::dec_bwd_bn_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a, sy.fn ? sy.tot1 : e->ct.sums,
-                                                            sy.fn ? sy.tot1 + 32 : nullptr, e->ct.part_db);
+    BnTotals t;
+    if ((rc = bn_totals(e, l.part_act, dec_act_blocks(g), dd::DEC_ACT_N, 32, nout, e->ct.sums, 33, st, &t))) return rc;
+    dd::dec_bwd_bn_kernel<<<dec_act_blocks(g), 256, 0, st>>>(a, t.sum, t.cnt, e->ct.part_db);
     if ((rc = launched(e, "dec_bwd_bn"))) return rc;
   }
   if (dx != nullptr) {
@@ -3633,10 +3626,10 @@ int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, fl
     const long long n = static_cast<long long>(h->cfg.batch) * h->cfg.latent_h * h->cfg.latent_w;
     const dd::EncPreBn1 op1{depth, ct.enc_w1, height, width, h->cfg.latent_h, h->cfg.latent_w};
     int rc;
-    if ((rc = run_bn_batch(h, op1, n, ct.enc_gb, nullptr, ct.enc_w1, 144, ct.enc_w1f, ct.enc_b1f, nullptr, ct.rec, st)))
+    if ((rc = run_codec_bn(h, op1, n, ct.enc_gb, nullptr, ct.enc_w1, 144, ct.enc_w1f, ct.enc_b1f, nullptr, ct.rec, st)))
       return rc;
     const dd::EncPreBn2 op2{depth, ct.enc_w1f, ct.enc_b1f, ct.enc_w2, height, width, h->cfg.latent_h, h->cfg.latent_w};
-    if ((rc = run_bn_batch(h, op2, n, ct.enc_gb + 32, nullptr, ct.enc_w2, 2304, ct.enc_w2f, ct.enc_b2f, nullptr,
+    if ((rc = run_codec_bn(h, op2, n, ct.enc_gb + 32, nullptr, ct.enc_w2, 2304, ct.enc_w2f, ct.enc_b2f, nullptr,
                            ct.rec + 32, st)))
       return rc;
     ct.nrec = 2;

@@ -2,17 +2,12 @@
 // conv_up, the HAHI neck's ConvModules and the ResNet BasicBlocks' bn1 / bn2.  The unchanged convgen_wgmma_kernel runs
 // the layer on an unfolded pack (no BatchNorm, no bias, no activation) and writes the pre-BN value u, fp32 NHWC
 // [n][C]; these kernels then take its per-channel batch statistics, fold them into a scale and shift, and apply
-// act(s u + t) with the eval epilogue's addend placements and outputs.
-//
-// Statistics take two passes over u, as codec_train.cuh does: pass 1 sums u, pass 2 sums d = u - m and d^2 with m =
-// the pass-1 mean rounded to fp32, so the variance is a mean of squared deviations and sum d corrects the rounding of
-// m.  Each block writes fixed fp64 partials that are summed in block order: bit-reproducible.
-//
-// Across ranks (dd_set_bn_allgather) the pass totals are gathered with the local pixel count and summed in rank order
-// (bn_rank_sum_kernel), and `cnt` points at the global count: the mean and variance are the union batch's.  cnt null:
-// the local n, as on one GPU.
+// act(s u + t) with the eval epilogue's addend placements and outputs.  The two statistics passes, their partials and
+// the cross-rank totals follow bn_stats.cuh.
 #pragma once
 #include <cuda_fp16.h>
+
+#include "bn_stats.cuh"
 
 namespace dd {
 
@@ -51,40 +46,18 @@ __global__ void __launch_bounds__(256) pbn_stats_kernel(const float* __restrict_
   }
 }
 
-// sum1[c] = pass-1 partials summed in block order (one thread per channel)
-__global__ void __launch_bounds__(256) pbn_colsum_kernel(const double* __restrict__ part, int nblk, int C,
-                                                         double* __restrict__ sum1) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  double s = 0.0;
-  for (int b = 0; b < nblk; ++b) s += part[static_cast<size_t>(b) * 2 * C + c];
-  sum1[c] = s;
-}
-
-// From the pass-2 partials: s = gamma / sqrt(var_b + 1e-5) in fp64, rounded once, t = beta - s mean, and the record
-// [2][C] (batch mean, unbiased batch variance) that the caller's running update reads.  The count is *cnt, or n when
-// cnt is null.
-__global__ void __launch_bounds__(256) pbn_fold_kernel(const double* __restrict__ sum1, const double* __restrict__ part,
-                                                       int nblk, long long n, const double* __restrict__ cnt, int C,
-                                                       const float* __restrict__ gamma,
+// From the batch statistics (bn_batch_stats): s, t = beta - s mean in fp64, each rounded once, and the record [2][C]
+// (batch mean, unbiased batch variance) that the caller's running update reads.
+__global__ void __launch_bounds__(256) pbn_fold_kernel(const BnFoldIn in, int C, const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, float* __restrict__ s_out,
                                                        float* __restrict__ t_out, float* __restrict__ rec) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  double d1 = 0.0, d2 = 0.0;
-  for (int b = 0; b < nblk; ++b) {
-    d1 += part[(static_cast<size_t>(b) * 2) * C + c];
-    d2 += part[(static_cast<size_t>(b) * 2 + 1) * C + c];
-  }
-  const double nn = cnt ? *cnt : static_cast<double>(n);
-  const double dm = d1 / nn;  // mean of d: the rounding of the shift
-  const double mean = static_cast<double>(static_cast<float>(sum1[c] / nn)) + dm;
-  const double var = fmax(d2 / nn - dm * dm, 0.0);
-  const double sc = static_cast<double>(gamma[c]) / sqrt(var + 1e-5);
-  s_out[c] = static_cast<float>(sc);
-  t_out[c] = static_cast<float>(static_cast<double>(beta[c]) - mean * sc);
-  rec[c] = static_cast<float>(mean);
-  rec[C + c] = static_cast<float>(nn > 1.0 ? var * nn / (nn - 1.0) : var);
+  const BnBatchStats b = bn_batch_stats(in, C, c, gamma);
+  s_out[c] = static_cast<float>(b.scale);
+  t_out[c] = static_cast<float>(static_cast<double>(beta[c]) - b.mean * b.scale);
+  rec[c] = static_cast<float>(b.mean);
+  rec[C + c] = static_cast<float>(b.var_unbiased);
 }
 
 // y = act(s u + t) over n pixels of C channels (C % 8 == 0), eight channels per item, act as the eval epilogue's `relu`
