@@ -117,6 +117,12 @@ SIGNATURES = {
                                     C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
     "dd_layer_norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                 C.c_float, C.c_void_p]),
+    "dd_swin_patch_embed": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "dd_swin_layer_norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "dd_swin_patch_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "dd_conv_groupnorm": (C.c_int, [C.c_void_p, C.POINTER(DDConvGnDesc), C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p]),

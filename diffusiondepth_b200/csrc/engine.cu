@@ -2245,6 +2245,31 @@ int run_ln(dd_engine* e, int C, const float* x, const float* g, const float* b, 
   return launched(e, "ln_split");
 }
 
+// Swin patch embedding: 4x4/s4 conv (3 -> E) + bias + LayerNorm(E), rgb [B][3][H][W] zero-padded right / bottom to a
+// multiple of 4 -> x fp32 [B * ceil(H / 4) * ceil(W / 4)][E]
+int run_patch_embed(dd_engine* e, int E, const float* rgb, const float* w, const float* bias, const float* g,
+                    const float* beta, float* x, int B, int H, int W, cudaStream_t st) {
+  if (E != 192) return fail(DD_ERR_UNSUPPORTED, "patch embedding width not instantiated");
+  const int Hp = (H + 3) / 4, Wp = (W + 3) / 4;
+  const int segs = (Wp + dd::PE_TOK - 1) / dd::PE_TOK;
+  dd::patch_embed_kernel<192><<<segs * Hp * B, 192, 0, st>>>(rgb, w, bias, g, beta, x, B, H, W, Hp, Wp);
+  return launched(e, "patch_embed");
+}
+
+// Swin patch merging: x [B][H][W][C] -> 2x2 unfold (zero pad for odd H / W) + LayerNorm(4C) -> out planes
+// [B * ceil(H / 2) * ceil(W / 2)][4C]
+int run_merge_ln(dd_engine* e, int C, const float* x, const float* g, const float* b, const Planes& out, int B, int H,
+                 int W, cudaStream_t st) {
+  const int grid = (B * ((H + 1) / 2) * ((W + 1) / 2) + 7) / 8;
+  switch (C) {
+    case 192: dd::merge_ln_split_kernel<192><<<grid, 256, 0, st>>>(x, g, b, out.hi, out.lo, kTokScale, B, H, W, e->status); break;
+    case 384: dd::merge_ln_split_kernel<384><<<grid, 256, 0, st>>>(x, g, b, out.hi, out.lo, kTokScale, B, H, W, e->status); break;
+    case 768: dd::merge_ln_split_kernel<768><<<grid, 256, 0, st>>>(x, g, b, out.hi, out.lo, kTokScale, B, H, W, e->status); break;
+    default: return fail(DD_ERR_UNSUPPORTED, "patch merging width not instantiated");
+  }
+  return launched(e, "merge_ln_split");
+}
+
 // Window attention on the fp32 CUDA-core kernel: the check path (DD_FLAG_SIMT_CONV, probes switch) and any odd head
 // count (the wgmma kernel takes heads in pairs).
 bool attn_simt(const dd_engine* e, int nH) {
@@ -2289,13 +2314,8 @@ int launch_attention(dd_engine* e, const float* qkv, const float* qkv_bias, cons
 int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream_t st) {
   Backbone& b = e->bb;
   const int B = e->cfg.batch;
-  {
-    const int segs = (b.Ws[0] + dd::PE_TOK - 1) / dd::PE_TOK;
-    dd::patch_embed_kernel<192><<<segs * b.Hs[0] * B, 192, 0, st>>>(rgb, b.pe_w, b.pe_b, b.pe_g, b.pe_beta, b.X[0], B, b.H,
-                                                                     b.W, b.Hs[0], b.Ws[0]);
-  }
   int rc;
-  if ((rc = launched(e, "patch_embed"))) return rc;
+  if ((rc = run_patch_embed(e, b.E, rgb, b.pe_w, b.pe_b, b.pe_g, b.pe_beta, b.X[0], B, b.H, b.W, st))) return rc;
   for (int s = 0; s < 4; ++s) {
     const int C = b.E << s, H = b.Hs[s], W = b.Ws[s], M = B * H * W, nH = b.heads[s];
     float* x = b.X[s & 1];
@@ -2316,15 +2336,8 @@ int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream
                      H * W, st))) return rc;
     if (s < 3) {
       const int M2 = B * b.Hs[s + 1] * b.Ws[s + 1];
-      const int grid = (M2 + 7) / 8;
       const SwinStageW& S = b.stage[s];
-      switch (C) {
-        case 192: dd::merge_ln_split_kernel<192><<<grid, 256, 0, st>>>(x, S.dn_g, S.dn_b, b.AP.hi, b.AP.lo, kTokScale, B, H, W, e->status); break;
-        case 384: dd::merge_ln_split_kernel<384><<<grid, 256, 0, st>>>(x, S.dn_g, S.dn_b, b.AP.hi, b.AP.lo, kTokScale, B, H, W, e->status); break;
-        case 768: dd::merge_ln_split_kernel<768><<<grid, 256, 0, st>>>(x, S.dn_g, S.dn_b, b.AP.hi, b.AP.lo, kTokScale, B, H, W, e->status); break;
-        default: return fail(DD_ERR_UNSUPPORTED, "patch merging width not instantiated");
-      }
-      if ((rc = launched(e, "merge_ln_split"))) return rc;
+      if ((rc = run_merge_ln(e, C, x, S.dn_g, S.dn_b, b.AP, B, H, W, st))) return rc;
       if ((rc = run_gemm(e, S.reduction, b.AP, M2, 0, b.X[(s + 1) & 1], nullptr, nullptr, st))) return rc;
     }
   }
@@ -3945,6 +3958,57 @@ int dd_layer_norm(dd_handle h, const float* x, const float* gamma, const float* 
   dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
   if ((rc = check_launch("join_planes"))) return rc;
   return call.finish(st, "x or the LayerNorm output");
+}
+
+int dd_swin_patch_embed(dd_handle h, const float* rgb, const float* w, const float* bias, const float* gamma,
+                        const float* beta, float* out, int32_t batch, int32_t height, int32_t width, int32_t embed,
+                        void* cuda_stream) {
+  if (!h || !rgb || !w || !bias || !gamma || !beta || !out) return fail(DD_ERR_INVALID, "null argument");
+  if (batch < 1 || height < 1 || width < 1 || embed < 1) return fail(DD_ERR_INVALID, "bad patch embedding geometry");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  if ((rc = run_patch_embed(h, embed, rgb, w, bias, gamma, beta, out, batch, height, width, st))) return rc;
+  return call.finish(st, "the patch embedding");
+}
+
+int dd_swin_layer_norm(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, float* nchw_out,
+                       int32_t tokens, int32_t channels, int32_t hw, void* cuda_stream) {
+  if (!h || !x || !gamma || !beta || !out) return fail(DD_ERR_INVALID, "null argument");
+  if (tokens < 1 || channels < 1 || (nchw_out && (hw < 1 || tokens % hw != 0)))
+    return fail(DD_ERR_INVALID, "bad LayerNorm geometry");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const size_t n = static_cast<size_t>(tokens) * channels;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  Planes o;
+  if ((rc = call.alloc(&o.hi, n)) || (rc = call.alloc(&o.lo, n))) return rc;
+  if ((rc = run_ln(h, channels, x, gamma, beta, o, tokens, nchw_out, nchw_out ? hw : 0, st))) return rc;
+  dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
+  if ((rc = check_launch("join_planes"))) return rc;
+  return call.finish(st, "x or the LayerNorm output");
+}
+
+int dd_swin_patch_merge(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, int32_t batch,
+                        int32_t height, int32_t width, int32_t channels, void* cuda_stream) {
+  if (!h || !x || !gamma || !beta || !out) return fail(DD_ERR_INVALID, "null argument");
+  if (batch < 1 || height < 1 || width < 1 || channels < 1) return fail(DD_ERR_INVALID, "bad patch merging geometry");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  const size_t n = static_cast<size_t>(batch) * ((height + 1) / 2) * ((width + 1) / 2) * 4 * channels;
+  StandaloneCall call(h);
+  int rc;
+  if ((rc = call.begin(st))) return rc;
+  Planes o;
+  if ((rc = call.alloc(&o.hi, n)) || (rc = call.alloc(&o.lo, n))) return rc;
+  if ((rc = run_merge_ln(h, channels, x, gamma, beta, o, batch, height, width, st))) return rc;
+  dd::join_planes_kernel<<<grid_of(n), 256, 0, st>>>(o.hi, o.lo, out, n, 1.f / kTokScale);
+  if ((rc = check_launch("join_planes"))) return rc;
+  return call.finish(st, "x or the patch merging output");
 }
 
 int dd_conv_groupnorm(dd_handle h, const dd_conv_gn_desc* d, const float* x, const float* w, const float* b,

@@ -14,6 +14,7 @@
 #include <stdint.h>
 
 #include "kernels.cuh"
+#include "swin.cuh"  // warp_sum, warp_ln_centre
 
 namespace dd {
 
@@ -110,32 +111,12 @@ __global__ void __launch_bounds__(256) ln_split_generic_kernel(const float* __re
   if (token >= M) return;
   const float* row = x + static_cast<size_t>(token) * C;
   float v[VMAX];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < VMAX; ++i) {
     const int c = lane + 32 * i;
     v[i] = c < C ? row[c] : 0.f;
-    s += v[i];
   }
-  const float inv_c = 1.f / static_cast<float>(C);
-  // The mean in two parts: the fp32 mean m0, then the mean mc of v - m0.  A row with a large mean and a small spread
-  // (1e3 +- 1e-2) would otherwise lose the spread to m0's rounding (~1e-4 there), and a constant row would come out as
-  // rounding noise times rsqrt(eps) instead of beta; v - m0 is exact for v within a factor 2 of m0.
-  const float m0 = warp_sum(s) * inv_c;
-  float s1 = 0.f;
-#pragma unroll
-  for (int i = 0; i < VMAX; ++i) {
-    v[i] = (lane + 32 * i < C) ? v[i] - m0 : 0.f;
-    s1 += v[i];
-  }
-  const float mc = warp_sum(s1) * inv_c;
-  float s2 = 0.f;
-#pragma unroll
-  for (int i = 0; i < VMAX; ++i) {
-    v[i] = (lane + 32 * i < C) ? v[i] - mc : 0.f;
-    s2 = fmaf(v[i], v[i], s2);
-  }
-  const float rstd = rsqrtf(warp_sum(s2) * inv_c + eps);
+  const float rstd = warp_ln_centre(v, C, eps);  // two-part mean (swin.cuh)
   bool ov = false;
 #pragma unroll
   for (int i = 0; i < VMAX; ++i) {

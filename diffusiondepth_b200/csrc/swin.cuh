@@ -17,6 +17,35 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// LayerNorm statistics of one warp's token: v[i] holds channel lane + 32 i, the first C channels real (the others 0).
+// Centres v in place (the others stay 0) and returns rstd = 1 / sqrt(var + eps).  The mean in two parts: the fp32 mean
+// m0, then the mean mc of v - m0.  A row with a large mean and a small spread (1e3 +- 1e-2) would otherwise lose the
+// spread to m0's rounding (~1e-4 there), and a constant row would come out as rounding noise times rsqrt(eps) instead
+// of beta; v - m0 is exact for v within a factor 2 of m0.
+template <int N>
+__device__ __forceinline__ float warp_ln_centre(float (&v)[N], int C, float eps) {
+  const int lane = threadIdx.x & 31;
+  const float inv_c = 1.f / static_cast<float>(C);
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < N; ++i) s += v[i];
+  const float m0 = warp_sum(s) * inv_c;
+  float s1 = 0.f;
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    v[i] = (lane + 32 * i < C) ? v[i] - m0 : 0.f;
+    s1 += v[i];
+  }
+  const float mc = warp_sum(s1) * inv_c;
+  float s2 = 0.f;
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    v[i] = (lane + 32 * i < C) ? v[i] - mc : 0.f;
+    s2 = fmaf(v[i], v[i], s2);
+  }
+  return rsqrtf(warp_sum(s2) * inv_c + eps);
+}
+
 // ------------------------------------------------------------------ LayerNorm(C) -> scaled fp16 hi/lo planes
 // one warp per token; C = 32 * VPT elements (VPT <= 48).  Optionally also writes fp32 NCHW (stage outputs).
 template <int C>
@@ -30,25 +59,14 @@ __global__ void __launch_bounds__(256) ln_split_kernel(const float* __restrict__
   if (token >= M) return;
   const float* row = x + static_cast<size_t>(token) * C;
   float v[VPT];
-  float s = 0.f;
 #pragma unroll
-  for (int i = 0; i < VPT; ++i) {
-    v[i] = row[lane + 32 * i];
-    s += v[i];
-  }
-  const float mean = warp_sum(s) * (1.f / C);
-  float s2 = 0.f;
-#pragma unroll
-  for (int i = 0; i < VPT; ++i) {
-    const float d = v[i] - mean;
-    s2 = fmaf(d, d, s2);
-  }
-  const float rstd = rsqrtf(warp_sum(s2) * (1.f / C) + 1e-5f);
+  for (int i = 0; i < VPT; ++i) v[i] = row[lane + 32 * i];
+  const float rstd = warp_ln_centre(v, C, 1e-5f);
   bool ov = false;
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int c = lane + 32 * i;
-    const float y = (v[i] - mean) * rstd * gamma[c] + beta[c];
+    const float y = v[i] * rstd * gamma[c] + beta[c];
     __half h, l;
     split_f16(y, scale, h, l, ov);
     hi[static_cast<size_t>(token) * C + c] = h;
@@ -74,7 +92,7 @@ __global__ void __launch_bounds__(E) patch_embed_kernel(const float* __restrict_
                                                         int W, int Hp, int Wp) {
   constexpr int TOK = 8;  // tokens per inner group
   __shared__ __align__(16) float patch[PE_TOK][48];  // [token][c*16 + ky*4 + kx]: read back as broadcast float4s
-  __shared__ float red[2][TOK][E / 32];
+  __shared__ float red[3][TOK][E / 32];  // per-warp sums of v, of v - m0 and of the centred squares
   const int segs = (Wp + PE_TOK - 1) / PE_TOK;
   const int seg = blockIdx.x % segs, py = (blockIdx.x / segs) % Hp, b = blockIdx.x / (segs * Hp);
   const int px0 = seg * PE_TOK;
@@ -115,26 +133,35 @@ __global__ void __launch_bounds__(E) patch_embed_kernel(const float* __restrict_
       if (lane == 0) red[0][tk][warp] = s;
     }
     __syncthreads();
-    float mean[TOK];
+    // the mean in two parts, m0 then the mean of acc - m0, as warp_ln_centre takes it; acc is centred in place
 #pragma unroll
     for (int tk = 0; tk < TOK; ++tk) {
       float s = 0.f;
 #pragma unroll
       for (int wv = 0; wv < E / 32; ++wv) s += red[0][tk][wv];
-      mean[tk] = s * (1.f / E);
-      const float d = acc[tk] - mean[tk];
-      const float s2 = warp_sum(d * d);
-      if (lane == 0) red[1][tk][warp] = s2;
+      acc[tk] -= s * (1.f / E);
+      const float s1 = warp_sum(acc[tk]);
+      if (lane == 0) red[1][tk][warp] = s1;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int tk = 0; tk < TOK; ++tk) {
+      float s1 = 0.f;
+#pragma unroll
+      for (int wv = 0; wv < E / 32; ++wv) s1 += red[1][tk][wv];
+      acc[tk] -= s1 * (1.f / E);
+      const float s2 = warp_sum(acc[tk] * acc[tk]);
+      if (lane == 0) red[2][tk][warp] = s2;
     }
     __syncthreads();
 #pragma unroll
     for (int tk = 0; tk < TOK; ++tk) {
       float s2 = 0.f;
 #pragma unroll
-      for (int wv = 0; wv < E / 32; ++wv) s2 += red[1][tk][wv];
+      for (int wv = 0; wv < E / 32; ++wv) s2 += red[2][tk][wv];
       const float rstd = rsqrtf(s2 * (1.f / E) + 1e-5f);
       const int px = px0 + g0 + tk;
-      if (px < Wp) x[(static_cast<size_t>(b) * Hp * Wp + static_cast<size_t>(py) * Wp + px) * E + e] = (acc[tk] - mean[tk]) * rstd * ga + bt;
+      if (px < Wp) x[(static_cast<size_t>(b) * Hp * Wp + static_cast<size_t>(py) * Wp + px) * E + e] = acc[tk] * rstd * ga + bt;
     }
     __syncthreads();  // red[] is reused by the next group
   }
@@ -156,28 +183,19 @@ __global__ void __launch_bounds__(256) merge_ln_split_kernel(const float* __rest
   if (token >= M2) return;
   const int b = token / (H2 * W2), r = token % (H2 * W2), oy = r / W2, ox = r % W2;
   float v[VPT];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int f = lane + 32 * i;
     const int c = f >> 2, ky = (f >> 1) & 1, kx = f & 1;
     const int yy = 2 * oy + ky, xx = 2 * ox + kx;
     v[i] = (yy < H && xx < W) ? x[((static_cast<size_t>(b) * H + yy) * W + xx) * C + c] : 0.f;
-    s += v[i];
   }
-  const float mean = warp_sum(s) * (1.f / F);
-  float s2 = 0.f;
-#pragma unroll
-  for (int i = 0; i < VPT; ++i) {
-    const float d = v[i] - mean;
-    s2 = fmaf(d, d, s2);
-  }
-  const float rstd = rsqrtf(warp_sum(s2) * (1.f / F) + 1e-5f);
+  const float rstd = warp_ln_centre(v, F, 1e-5f);
   bool ov = false;
 #pragma unroll
   for (int i = 0; i < VPT; ++i) {
     const int f = lane + 32 * i;
-    const float y = (v[i] - mean) * rstd * gamma[f] + beta[f];
+    const float y = v[i] * rstd * gamma[f] + beta[f];
     __half h, l;
     split_f16(y, scale, h, l, ov);
     hi[static_cast<size_t>(token) * F + f] = h;

@@ -670,6 +670,42 @@ class DenoiseEngine:
                                            float(eps), C.c_void_p(self._stream())))
         return out
 
+    def swin_patch_embed(self, rgb: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, gamma: torch.Tensor,
+                         beta: torch.Tensor) -> torch.Tensor:
+        """Swin's patch embedding on the backbone's kernel (dd_swin_patch_embed, E = 192): rgb [B, 3, H, W] fp32, w [E,
+        3, 4, 4] -> 4x4/s4 conv (zero pad right / bottom) + bias + LayerNorm(E) -> fp32 [B * ceil(H/4) * ceil(W/4),
+        E]."""
+        rgb, w, bias, gamma, beta = (_f32(t, self.device) for t in (rgb, w, bias, gamma, beta))
+        B, _, H, W = rgb.shape
+        E = w.shape[0]
+        out = torch.full((B * ((H + 3) // 4) * ((W + 3) // 4), E), float("nan"), device=self.device)
+        _cabi.check(self.lib.dd_swin_patch_embed(self._h, _ptr(rgb), _ptr(w), _ptr(bias), _ptr(gamma), _ptr(beta),
+                                                 _ptr(out), B, H, W, E, C.c_void_p(self._stream())))
+        return out
+
+    def swin_layer_norm(self, x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, hw: int = 0):
+        """Swin's LayerNorm on the backbone's kernel (dd_swin_layer_norm, C in {192, 384, 768, 1536}, eps 1e-5): x
+        [M, C] fp32 -> (out [M, C] fp32 rebuilt from the kernel's hi / lo planes, the stage-output copy [M / hw, C, hw]
+        fp32 when hw > 0, else None)."""
+        x, gamma, beta = (_f32(t, self.device) for t in (x, gamma, beta))
+        M, Cc = x.shape
+        out = torch.empty_like(x)
+        nchw = torch.full((M // hw, Cc, hw), float("nan"), device=self.device) if hw > 0 else None
+        _cabi.check(self.lib.dd_swin_layer_norm(self._h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), _ptr(nchw), M,
+                                                Cc, int(hw), C.c_void_p(self._stream())))
+        return out, nchw
+
+    def swin_patch_merge(self, x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor) -> torch.Tensor:
+        """Swin's patch merging on the backbone's kernel (dd_swin_patch_merge, C in {192, 384, 768}): x [B, H, W, C]
+        fp32 -> 2x2 unfold (zero pad for odd H / W) + LayerNorm(4C) -> fp32 [B * ceil(H/2) * ceil(W/2), 4C], rebuilt
+        from the kernel's hi / lo planes."""
+        x, gamma, beta = (_f32(t, self.device) for t in (x, gamma, beta))
+        B, H, W, Cc = x.shape
+        out = torch.empty(B * ((H + 1) // 2) * ((W + 1) // 2), 4 * Cc, device=self.device)
+        _cabi.check(self.lib.dd_swin_patch_merge(self._h, _ptr(x), _ptr(gamma), _ptr(beta), _ptr(out), B, H, W, Cc,
+                                                 C.c_void_p(self._stream())))
+        return out
+
     def conv_groupnorm(self, x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, gamma: torch.Tensor,
                        beta: torch.Tensor, mode: int, cond: Optional[torch.Tensor] = None,
                        temb: Optional[torch.Tensor] = None, latent: Optional[torch.Tensor] = None, c_x: float = 0.0,

@@ -492,6 +492,30 @@ int dd_depthwise_conv(dd_handle h, const float* x, const float* w, const float* 
 int dd_layer_norm(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, int32_t tokens,
                   int32_t channels, float eps, void* cuda_stream);
 
+/* Standalone patch embedding of the Swin backbone, launched as the backbone does: rgb [B][3][H][W] (device fp32,
+ * zero-padded right / bottom to a multiple of 4), w [E][3][4][4], bias / gamma / beta [E] -> 4x4/s4 conv + bias +
+ * LayerNorm(E) (eps 1e-5) -> out [B * ceil(H / 4) * ceil(W / 4)][E] fp32, written by the kernel itself (not
+ * range-checked).  DD_ERR_UNSUPPORTED for E other than 192.  Allocates and frees its own buffers; synchronises. */
+int dd_swin_patch_embed(dd_handle h, const float* rgb, const float* w, const float* bias, const float* gamma,
+                        const float* beta, float* out, int32_t batch, int32_t height, int32_t width, int32_t embed,
+                        void* cuda_stream);
+
+/* Standalone LayerNorm of the Swin backbone (norm1 / norm2 of every block, the stage-output norms; eps 1e-5): x
+ * [tokens][C] (device fp32), gamma / beta [C] -> out [tokens][C] fp32, rebuilt from the kernel's hi/lo output planes,
+ * and, when nchw_out is not null, the stage-output copy nchw_out [tokens / hw][C][hw] fp32 (tokens a multiple of hw;
+ * hw is ignored otherwise).  DD_ERR_UNSUPPORTED for C outside {192, 384, 768, 1536}.  Allocates and frees its own
+ * buffers; synchronises and returns DD_ERR_RANGE as dd_gen_layer does. */
+int dd_swin_layer_norm(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, float* nchw_out,
+                       int32_t tokens, int32_t channels, int32_t hw, void* cuda_stream);
+
+/* Standalone patch merging of the Swin backbone, launched as the backbone does: x [B][H][W][C] (device fp32) -> 2x2
+ * unfold (feature c * 4 + ky * 2 + kx; zero pad for odd H / W) + LayerNorm(4C) (eps 1e-5) with gamma / beta [4C] ->
+ * out [B * ceil(H / 2) * ceil(W / 2)][4C] fp32, rebuilt from the kernel's hi/lo output planes.  DD_ERR_UNSUPPORTED for
+ * C outside {192, 384, 768}.  Allocates and frees its own buffers; synchronises and returns DD_ERR_RANGE as
+ * dd_gen_layer does. */
+int dd_swin_patch_merge(dd_handle h, const float* x, const float* gamma, const float* beta, float* out, int32_t batch,
+                        int32_t height, int32_t width, int32_t channels, void* cuda_stream);
+
 typedef struct dd_conv_gn_desc {
   int32_t batch, cin, cout, height, width; /* one of the loop's GroupNorm'd convs: 16->64, 64->256, 256->64, 64->16 */
   int32_t mode;            /* 0 GN + ReLU (Cout 64); 1 + cond (same grid) + temb (Cout 256); 2 + bilinear up(cond + temb),
