@@ -409,12 +409,6 @@ struct MPViTW {
   int Hs[4] = {0, 0, 0, 0}, Ws[4] = {0, 0, 0, 0};
   GenLayer stem0, stem1;
   MpStageW stage[4];
-  // stochastic depth (dd_set_drop_path): bit l of drop_mask[s] marks stage s's encoder layer l (in every path) as having
-  // a DropPath on its two residual branches; drop_blocks counts those blocks.  While drop_on, drop_scales holds
-  // [block][attention, MLP][B] per-sample scales, blocks in stage, path, layer order.
-  int drop_mask[4] = {0, 0, 0, 0}, drop_blocks = 0;
-  bool drop_on = false;
-  float* drop_scales = nullptr;
   // workspace views
   Planes IN, S1, D, EP0, AP, HP, CAT;
   float* XS = nullptr;      // stem output, then each stage's output (fp32 NHWC)
@@ -422,6 +416,16 @@ struct MPViTW {
   float* R1 = nullptr;
   float* QKV = nullptr;
   FactorAttBufs fab;
+};
+
+// Stochastic depth of the native backbone (dd_backbone_config.mp_drop_path, dd_set_drop_path).  Bit k of mask[s] marks
+// block k of stage s: an MPViT encoder layer (in every path) or a Swin block, each with two residual branches (attention,
+// then MLP / FFN); blocks counts the marked blocks (MPViT: times the stage's paths).  While on, scales holds
+// [block][branch][B] per-sample scales, blocks in stage(, path), block order.
+struct DropPathState {
+  int mask[4] = {0, 0, 0, 0}, blocks = 0;
+  bool on = false;
+  float* scales = nullptr;
 };
 
 }  // namespace
@@ -545,13 +549,14 @@ struct dd_engine {
   Backbone bb;
   ResNetW rn;
   MPViTW mp;
+  DropPathState drop;  // of whichever of bb / mp is enabled
   bool feats_ready = false;  // dd_run_backbone has filled the neck's input planes
   bool cond_ready = false;  // dd_build_condition has filled `cond` for the next dd_denoise_decode(cond = NULL)
   // CUDA graphs (DD_FLAG_CUDA_GRAPH), captured on first use and replayed: the T-step loop, the same loop with a decode
   // after every step (dd_denoise_decode_steps), the native backbone, the neck + FPN
   // (G_LOOP_STEPS_TRAIN: the step-decode loop in DD_CODEC_TRAIN, batch statistics before every decode)
   // (G_BACKBONE_TRAIN, G_COND_TRAIN: the native backbone and the neck + FPN in DD_PRODUCER_TRAIN; G_BACKBONE_DROP,
-  // G_BACKBONE_TRAIN_DROP: the MPViT backbone with stochastic depth on, in either producer mode)
+  // G_BACKBONE_TRAIN_DROP: the MPViT or Swin backbone with stochastic depth on, in either producer mode)
   enum {
     G_LOOP = 0, G_LOOP_STEPS = 1, G_BACKBONE = 2, G_COND = 3, G_LOOP_STEPS_TRAIN = 4, G_BACKBONE_TRAIN = 5,
     G_COND_TRAIN = 6, G_BACKBONE_DROP = 7, G_BACKBONE_TRAIN_DROP = 8, G_COUNT = 9
@@ -2311,25 +2316,64 @@ int launch_attention(dd_engine* e, const float* qkv, const float* qkv_bias, cons
   return launched(e, "window_attention");
 }
 
+// x (+)= scale[b] branch over B images of n tokens of C channels (drop_path_add_kernel): into y32, or into the planes
+// *out (row width ld_out, channel offset ch_off)
+int run_drop_add(dd_engine* e, const float* x, const float* branch, const float* scale, int B, int n, int C, float* y32,
+                 const Planes* out, int ld_out, int ch_off, cudaStream_t st) {
+  dd::DropAddArgs a;
+  a.x = x;
+  a.branch = branch;
+  a.scale = scale;
+  a.per_img = n;
+  a.B = B;
+  a.C = C;
+  a.y32 = y32;
+  a.out_hi = out ? out->hi : nullptr;
+  a.out_lo = out ? out->lo : nullptr;
+  a.ld_out = ld_out > 0 ? ld_out : C;
+  a.ch_off = ch_off;
+  a.split_scale = kProdScale;
+  a.status = e->status;
+  dd::drop_path_add_kernel<<<grid_of(static_cast<size_t>(B) * n * C / 4), 256, 0, st>>>(a);
+  return launched(e, "drop_path_add");
+}
+
+// With stochastic depth on, a marked block (reference swin.py:412,421) runs proj and ffn2 without the addend into QKV,
+// dead between its attention and the next block's qkv GEMM and 3x the size of the token map, then adds each branch
+// through drop_path_add_kernel; every other block adds them in the GEMM's epilogue.
 int run_swin(dd_engine* e, const float* rgb, float* const* feats_out, cudaStream_t st) {
   Backbone& b = e->bb;
+  const DropPathState& dp = e->drop;
   const int B = e->cfg.batch;
   int rc;
   if ((rc = run_patch_embed(e, b.E, rgb, b.pe_w, b.pe_b, b.pe_g, b.pe_beta, b.X[0], B, b.H, b.W, st))) return rc;
+  int slot = 0;  // marked blocks in stage, block order
   for (int s = 0; s < 4; ++s) {
     const int C = b.E << s, H = b.Hs[s], W = b.Ws[s], M = B * H * W, nH = b.heads[s];
     float* x = b.X[s & 1];
     const int ws = b.window;
     for (int k = 0; k < b.depths[s]; ++k) {
       const SwinBlockW& Wt = b.stage[s].blocks[k];
+      const float* drop = (dp.on && ((dp.mask[s] >> k) & 1)) ? dp.scales + static_cast<size_t>(slot++) * 2 * B
+                                                             : nullptr;  // [attention, FFN][B]
       if ((rc = run_ln(e, C, x, Wt.ln1_g, Wt.ln1_b, b.AP, M, nullptr, 0, st))) return rc;
       if ((rc = run_gemm(e, Wt.qkv, b.AP, M, 0, b.QKV, nullptr, nullptr, st))) return rc;
       if ((rc = launch_attention(e, b.QKV, Wt.qkv.shift, Wt.table, b.AP, B, H, W, C, nH, (k & 1) ? ws / 2 : 0,
                                  attn_simt(e, nH), st))) return rc;
-      if ((rc = run_gemm(e, Wt.proj, b.AP, M, 0, x, x, nullptr, st))) return rc;      // x += proj(attn)
+      if (drop) {
+        if ((rc = run_gemm(e, Wt.proj, b.AP, M, 0, b.QKV, nullptr, nullptr, st))) return rc;
+        if ((rc = run_drop_add(e, x, b.QKV, drop, B, H * W, C, x, nullptr, 0, 0, st))) return rc;  // x += drop(proj(attn))
+      } else if ((rc = run_gemm(e, Wt.proj, b.AP, M, 0, x, x, nullptr, st))) {  // x += proj(attn)
+        return rc;
+      }
       if ((rc = run_ln(e, C, x, Wt.ln2_g, Wt.ln2_b, b.AP, M, nullptr, 0, st))) return rc;
       if ((rc = run_gemm(e, Wt.ffn1, b.AP, M, 2, nullptr, nullptr, &b.HP, st))) return rc;  // GELU(fc1) -> planes
-      if ((rc = run_gemm(e, Wt.ffn2, b.HP, M, 0, x, x, nullptr, st))) return rc;      // x += fc2(...)
+      if (drop) {
+        if ((rc = run_gemm(e, Wt.ffn2, b.HP, M, 0, b.QKV, nullptr, nullptr, st))) return rc;
+        if ((rc = run_drop_add(e, x, b.QKV, drop + B, B, H * W, C, x, nullptr, 0, 0, st))) return rc;  // x += drop(fc2(...))
+      } else if ((rc = run_gemm(e, Wt.ffn2, b.HP, M, 0, x, x, nullptr, st))) {  // x += fc2(...)
+        return rc;
+      }
     }
     // per-stage output norm straight into the neck's input planes (+ NCHW copy on request)
     if ((rc = run_ln(e, C, x, b.stage[s].out_g, b.stage[s].out_b, e->prod.F[s], M, feats_out ? feats_out[s] : nullptr,
@@ -2924,6 +2968,10 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   if (h->bb.enabled)
     if ((rc = pack_backbone(h, st, scratch))) return rc;
   if ((rc = pack_prod_train(h, st))) return rc;
+  h->drop.on = false;  // a new buffer: dd_set_drop_path fills it
+  if (h->drop.blocks > 0 && (h->mp.enabled || h->bb.enabled) &&
+      (rc = dev_array(h, &h->drop.scales, static_cast<size_t>(h->drop.blocks) * 2 * h->cfg.batch)))
+    return rc;
   // the registered pointers were borrowed for this call only (include/dd_engine.h): wait for the kernels that read them
   // and forget them, so a later finalize cannot read memory the caller has freed in the meantime
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -3307,20 +3355,21 @@ int dd_set_producer_mode(dd_handle h, int32_t mode) {
 
 int dd_set_drop_path(dd_handle h, const float* dev_scales, int32_t n, void* cuda_stream) {
   if (!h) return fail(DD_ERR_INVALID, "null handle");
-  MPViTW& m = h->mp;
+  DropPathState& d = h->drop;
   if (n == 0) {
-    m.drop_on = false;
+    d.on = false;
     return DD_OK;
   }
   if (!dev_scales) return fail(DD_ERR_INVALID, "null argument");
-  if (!(m.enabled && m.ready)) return fail(DD_ERR_INVALID, "dd_set_drop_path needs a finalized MPViT backbone");
-  if (n != static_cast<int64_t>(m.drop_blocks) * 2 * h->cfg.batch)
+  if (!((h->mp.enabled && h->mp.ready) || (h->bb.enabled && h->bb.ready)))
+    return fail(DD_ERR_INVALID, "dd_set_drop_path needs a finalized MPViT or Swin backbone");
+  if (n != static_cast<int64_t>(d.blocks) * 2 * h->cfg.batch)
     return fail(DD_ERR_INVALID, "dd_set_drop_path: n must be 0 or 2 x batch x the blocks mp_drop_path marks (" +
-                                    std::to_string(static_cast<int64_t>(m.drop_blocks) * 2 * h->cfg.batch) + ")");
+                                    std::to_string(static_cast<int64_t>(d.blocks) * 2 * h->cfg.batch) + ")");
   CUDA_TRY(cudaSetDevice(h->cfg.device));
-  CUDA_TRY(cudaMemcpyAsync(m.drop_scales, dev_scales, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice,
+  CUDA_TRY(cudaMemcpyAsync(d.scales, dev_scales, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToDevice,
                            static_cast<cudaStream_t>(cuda_stream)));
-  m.drop_on = true;
+  d.on = true;
   return DD_OK;
 }
 
@@ -3456,6 +3505,19 @@ int dd_build_condition(dd_handle h, const float* const* feats, float* cond_out, 
   return DD_OK;
 }
 
+// dd_backbone_config.mp_drop_path of a backbone with depths[s] blocks per stage, each marked block counting per_mark[s]
+// times (MPViT: its paths) -> *d, stochastic depth off
+int drop_marks(const int32_t* marks, const int* depths, const int* per_mark, DropPathState* d) {
+  *d = DropPathState();
+  for (int s = 0; s < 4; ++s) {
+    d->mask[s] = marks[s];
+    if (d->mask[s] < 0 || (depths[s] < 31 && (d->mask[s] >> depths[s]) != 0))
+      return fail(DD_ERR_INVALID, "mp_drop_path marks a block the stage does not have");
+    d->blocks += per_mark[s] * __builtin_popcount(static_cast<unsigned>(d->mask[s]));
+  }
+  return DD_OK;
+}
+
 int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
   if (!h || !bc) return fail(DD_ERR_INVALID, "null argument");
   if (bc->kind == DD_BACKBONE_RESNET) {
@@ -3477,6 +3539,7 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
         return fail(DD_ERR_INVALID, "backbone stage geometry does not match the producer pyramid");
     }
     h->rn = r;
+    h->drop = DropPathState();
     h->bb.enabled = false;
     h->mp.enabled = false;
     invalidate_pack(h);
@@ -3498,10 +3561,6 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
       m.layers[s] = bc->depths[s];
       m.paths[s] = bc->mp_paths[s];
       if (m.layers[s] < 1 || m.paths[s] < 1 || m.paths[s] > 3) return fail(DD_ERR_UNSUPPORTED, "MPViT: 1..3 paths, >= 1 layer per stage");
-      m.drop_mask[s] = bc->mp_drop_path[s];
-      if (m.drop_mask[s] < 0 || (m.layers[s] < 31 && (m.drop_mask[s] >> m.layers[s]) != 0))
-        return fail(DD_ERR_INVALID, "MPViT: mp_drop_path marks a layer the stage does not have");
-      m.drop_blocks += m.paths[s] * __builtin_popcount(static_cast<unsigned>(m.drop_mask[s]));
       if (m.dims[s] <= 0 || m.dims[s] % 8 != 0 || m.dims[s] / m.heads > dd::KTV_CH_MAX || m.dims[s] > 512)
         return fail(DD_ERR_UNSUPPORTED, "MPViT: stage widths must be multiples of 8 (8 heads), at most 512");
       hh = (hh - 1) / 2 + 1;  // depthwise 3x3, stride 2, pad 1
@@ -3515,7 +3574,11 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
       if (m.Hs[s] != h->prod.H[s] || m.Ws[s] != h->prod.W[s] || m.out_dims[s] != h->prod.C[s])
         return fail(DD_ERR_INVALID, "backbone stage geometry does not match the producer pyramid");
     }
+    DropPathState d;
+    int rc;
+    if ((rc = drop_marks(bc->mp_drop_path, m.layers, m.paths, &d))) return rc;
     h->mp = m;
+    h->drop = d;
     h->bb.enabled = false;
     h->rn.enabled = false;
     invalidate_pack(h);
@@ -3544,7 +3607,12 @@ int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc) {
     hh = (hh + 1) / 2;
     ww = (ww + 1) / 2;
   }
+  const int one[4] = {1, 1, 1, 1};
+  DropPathState d;
+  int rc;
+  if ((rc = drop_marks(bc->mp_drop_path, b.depths, one, &d))) return rc;
   h->bb = b;
+  h->drop = d;
   h->rn.enabled = false;
   h->mp.enabled = false;
   invalidate_pack(h);
@@ -3564,10 +3632,10 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
   if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   if ((rc = start_forward(h, st))) return rc;
   producer_forward_start(h);
-  // the ResNet's and MPViT's BatchNorms follow the producer mode (Swin has none); MPViT's stochastic depth is on while
-  // dd_set_drop_path holds scales, in either mode
+  // the ResNet's and MPViT's BatchNorms follow the producer mode (Swin has none); MPViT's and Swin's stochastic depth is
+  // on while dd_set_drop_path holds scales, in either mode
   const bool train = (resnet || mpvit) && h->producer_mode == DD_PRODUCER_TRAIN;
-  const bool drop = mpvit && h->mp.drop_on;
+  const bool drop = (mpvit || swin) && h->drop.on;
   bool want_out = false;
   for (int i = 0; feats_out && i < 4; ++i) want_out |= (feats_out[i] != nullptr);
   if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !want_out && !(train && h->sync.fn)) {

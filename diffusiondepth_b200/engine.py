@@ -215,8 +215,8 @@ class DenoiseEngine:
                         mp_drop_path=(0, 0, 0, 0)):
         """Run the backbone natively as well (after enable_producers, before load_weights).  kind: 'swin' (Swin-L),
         'resnet' (ResNetForMMBEV BasicBlock stages; only `depths` is used) or 'mpvit' (`depths` = encoder layers per
-        stage, `mp_dims` / `mp_paths` / `mlp_ratio`; `mp_drop_path[s]` bit l: stage s's encoder layer l has
-        stochastic depth, see `set_drop_path`)."""
+        stage, `mp_dims` / `mp_paths` / `mlp_ratio`).  `mp_drop_path[s]` bit k (MPViT and Swin): block k of stage s
+        has stochastic depth, see `set_drop_path`."""
         bc = _cabi.DDBackboneConfig()
         bc.kind, bc.embed_dims, bc.window = {"swin": 1, "resnet": 2, "mpvit": 3}[kind], int(embed_dims), int(window)
         bc.height, bc.width = int(image_hw[0]), int(image_hw[1])
@@ -457,10 +457,10 @@ class DenoiseEngine:
         _cabi.check(self.lib.dd_set_producer_mode(self._h, _cabi.PRODUCER_TRAIN if training else _cabi.PRODUCER_EVAL))
 
     def set_drop_path(self, scales: Optional[torch.Tensor]):
-        """Stochastic depth of the MPViT backbone for every later run_backbone (dd_set_drop_path): `scales` (fp32 on
-        the engine's device) = mask / keep of every DropPath branch, [block][attention, MLP][B] for the blocks
-        `enable_backbone(mp_drop_path=...)` marked, in stage, path, layer order; copied on the current stream.  None
-        turns it off."""
+        """Stochastic depth of the MPViT or Swin backbone for every later run_backbone (dd_set_drop_path): `scales`
+        (fp32 on the engine's device) = mask / keep of every DropPath branch, [block][attention, MLP][B] for the blocks
+        `enable_backbone(mp_drop_path=...)` marked, in stage, path, layer order (Swin: stage, block order); copied on
+        the current stream.  None turns it off."""
         if scales is None:
             _cabi.check(self.lib.dd_set_drop_path(self._h, None, 0, C.c_void_p(self._stream())))
             return

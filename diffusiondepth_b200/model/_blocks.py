@@ -42,6 +42,23 @@ class DropPath(nn.Module):
         return x * x.new_empty((x.shape[0],) + (1,) * (x.dim() - 1)).bernoulli_(keep) / keep
 
 
+class MMCVDropPath(nn.Module):
+    """Stochastic depth as mmcv 1.x's DropPath draws it (mmcv/cnn/bricks/drop.py, the Swin backbone's): in training mode
+    at a rate above 0, x / keep * floor(keep + torch.rand((B, 1, ...))); otherwise identity, drawing nothing.  Its draw
+    consumes the generator differently from DropPath's `bernoulli_`, so the two are separate classes."""
+
+    def __init__(self, drop_prob=0.0):
+        super().__init__()
+        self.drop_prob = drop_prob
+
+    def forward(self, x):
+        if self.drop_prob == 0.0 or not self.training:
+            return x
+        keep = 1 - self.drop_prob
+        r = keep + torch.rand((x.shape[0],) + (1,) * (x.dim() - 1), dtype=x.dtype, device=x.device)
+        return x.div(keep) * r.floor()
+
+
 @contextlib.contextmanager
 def exact_fp32():
     """cuDNN/cuBLAS default to TF32 for fp32 convs/matmuls on GPU, which alone breaks the 1e-3 parity bar

@@ -9,6 +9,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from .._blocks import MMCVDropPath
+
 
 class PatchEmbed(nn.Module):
     def __init__(self, cin, dim, patch):
@@ -78,7 +80,7 @@ class ShiftWindowMSA(nn.Module):
         super().__init__()
         self.ws, self.shift = ws, shift
         self.w_msa = WindowMSA(dim, heads, ws)
-        self.drop = nn.Identity()
+        self.drop = MMCVDropPath(0.0)  # stochastic depth of the attention branch (reference :248)
 
     def forward(self, x, hw):
         B, _, C = x.shape
@@ -103,15 +105,16 @@ class ShiftWindowMSA(nn.Module):
 
 
 class FFN(nn.Module):
-    """Keys `layers.0.0.*` / `layers.1.*` as mmcv's FFN lays them out."""
+    """Keys `layers.0.0.*` / `layers.1.*` as mmcv's FFN lays them out; `dropout_layer`: stochastic depth of the branch."""
 
     def __init__(self, dim, hidden):
         super().__init__()
         self.layers = nn.Sequential(nn.Sequential(nn.Linear(dim, hidden), nn.GELU(), nn.Dropout(0.0)),
                                     nn.Linear(hidden, dim), nn.Dropout(0.0))
+        self.dropout_layer = MMCVDropPath(0.0)
 
     def forward(self, x, identity):
-        return identity + self.layers(x)
+        return identity + self.dropout_layer(self.layers(x))
 
 
 class SwinBlock(nn.Module):
@@ -121,6 +124,10 @@ class SwinBlock(nn.Module):
         self.attn = ShiftWindowMSA(dim, heads, ws, ws // 2 if shift else 0)
         self.norm2 = nn.LayerNorm(dim)
         self.ffn = FFN(dim, hidden)
+
+    def set_drop_path_rate(self, rate):
+        """Both branches' stochastic-depth rate (reference :412,421: one rate per block)."""
+        self.attn.drop.drop_prob = self.ffn.dropout_layer.drop_prob = float(rate)
 
     def forward(self, x, hw):
         x = x + self.attn(self.norm1(x), hw)
@@ -143,9 +150,13 @@ class SwinStage(nn.Module):
 
 
 class SwinTransformer(nn.Module):
+    """`drop_path_rate`: stochastic depth in training mode (mmcv DropPath on both residual branches of every block).  The
+    reference class defaults to 0.1; the mirror's factories build at 0, so nothing changes unless a user calls
+    `set_drop_path_rate`."""
+
     def __init__(self, pretrain_img_size=224, in_channels=3, embed_dims=96, patch_size=4, window_size=7,
                  mlp_ratio=4, depths=(2, 2, 6, 2), num_heads=(3, 6, 12, 24), strides=(4, 2, 2, 2),
-                 out_indices=(0, 1, 2, 3), pretrain_style="official", pretrained=None, **unused):
+                 out_indices=(0, 1, 2, 3), pretrain_style="official", pretrained=None, drop_path_rate=0.0, **unused):
         super().__init__()
         self.out_indices = out_indices
         self.patch_embed = PatchEmbed(in_channels, embed_dims, patch_size)
@@ -159,6 +170,17 @@ class SwinTransformer(nn.Module):
         self.num_features = [embed_dims * 2 ** i for i in range(len(depths))]
         for i in out_indices:
             self.add_module(f"norm{i}", nn.LayerNorm(self.num_features[i]))
+        self.set_drop_path_rate(drop_path_rate)
+
+    def set_drop_path_rate(self, rate):
+        """Re-derive every block's stochastic-depth rate from `rate`, as the reference's constructor does (:639-674):
+        linspace(0, rate, sum(depths)) over the blocks in order, so block 0 of stage 0 has rate 0 and the last block has
+        `rate`.  The reference hands stage i `dpr[:depths[i]]` and then advances `dpr = dpr[depths[i]:]`, a running
+        slice.  The rate is the switch: in training mode every block with a rate above 0 draws one mask per branch."""
+        blocks = [blk for st in self.stages for blk in st.blocks]
+        for blk, r in zip(blocks, torch.linspace(0, rate, len(blocks))):
+            blk.set_drop_path_rate(r.item())
+        self.drop_path_rate = float(rate)
 
     def forward(self, x):
         x, hw = self.patch_embed(x)

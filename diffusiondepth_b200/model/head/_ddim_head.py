@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from diffusiondepth_b200._cabi import EngineError
 from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS, FUSE_KEYS,
                                         DenoiseEngine, WorkspacePool, is_updatable)
-from .._blocks import ConvModule, DropPath, exact_fp32
+from .._blocks import ConvModule, DropPath, MMCVDropPath, exact_fp32
 from ..diffusers.schedulers.scheduling_ddim import DDIMScheduler
 from ..ops import depth_transform as _codec  # noqa: F401  (registers the codec classes)
 from ..registry import DEPTH_TRANSFORM
@@ -71,7 +71,8 @@ class EngineKey(NamedTuple):
     producer_train: bool
     backward: bool
     loop_backward: bool
-    mpvit_drop: Tuple[int, ...] = ()      # native MPViT with stochastic depth: per stage, the bit mask of its layers
+    drop_path: Tuple[int, ...] = ()       # native backbone with stochastic depth: per stage, the bit mask of its MPViT
+                                          # layers / Swin blocks (dd_backbone_config.mp_drop_path)
 
     @property
     def geometry(self):
@@ -436,23 +437,56 @@ class DDIMHeadBase(nn.Module):
             masks.append(bits or 0)
         return tuple(masks), mods
 
-    def _mpvit_drop_scales(self, backbone, batch, device):
-        """Per-sample scales mask / keep of every DropPath branch of a natively run MPViT, [block][attention, MLP][B]
-        (set_drop_path), drawn as torch's forward would (`x.new_empty((B, 1, 1)).bernoulli_(keep)` on the device, one
-        draw per branch of a DropPath in training mode); None when none is in training mode."""
-        _, mods = self.mpvit_drop_paths(backbone)
-        if not any(m.training for m in mods):
+    @staticmethod
+    def swin_drop_paths(backbone):
+        """(per-stage bit masks of the blocks with stochastic depth, their MMCVDropPath modules in torch's draw order:
+        stage, block, then the attention branch before the FFN branch) of a Swin module.  A block is marked when one of
+        its two branches has a rate above 0 (the reference gives both the block's rate, swin.py:412,421)."""
+        masks, mods = [], []
+        for st in backbone.stages:
+            bits = 0
+            for k, blk in enumerate(st.blocks):
+                pair = (getattr(blk.attn, "drop", None), getattr(blk.ffn, "dropout_layer", None))
+                if all(isinstance(m, MMCVDropPath) for m in pair) and max(m.drop_prob for m in pair) > 0.0:
+                    bits |= 1 << k
+                    mods += pair
+            masks.append(bits)
+        return tuple(masks), mods
+
+    @staticmethod
+    def _draw_drop_scales(branches, batch, device):
+        """Per-sample scales mask / keep of stochastic-depth branches, [branch][B] (set_drop_path), `branches` holding
+        one DropPath or MMCVDropPath module per branch in torch's draw order.  Each is drawn on the device as its module's
+        forward draws it: DropPath `x.new_empty((B, 1, 1)).bernoulli_(keep)`, MMCVDropPath
+        `floor(keep + torch.rand((B, 1, 1)))`; a module in eval or at rate 0 draws nothing (scale 1).  None when no
+        module draws."""
+        def rate(m):
+            return m.p if isinstance(m, DropPath) else m.drop_prob
+
+        if not any(m.training and rate(m) > 0.0 for m in branches):
             return None
         out = []
-        for m in mods:
-            for _ in range(2):  # the attention branch, then the MLP branch (one DropPath module, two calls)
-                if m.training:
-                    keep = 1.0 - m.p
-                    out.append(torch.empty((batch, 1, 1), device=device, dtype=torch.float32).bernoulli_(keep)
-                               .reshape(batch) / keep)
-                else:
-                    out.append(torch.ones(batch, device=device, dtype=torch.float32))
+        for m in branches:
+            if not (m.training and rate(m) > 0.0):
+                out.append(torch.ones(batch, device=device, dtype=torch.float32))
+                continue
+            keep = 1.0 - rate(m)
+            if isinstance(m, MMCVDropPath):
+                mask = (keep + torch.rand((batch, 1, 1), dtype=torch.float32, device=device)).floor()
+            else:
+                mask = torch.empty((batch, 1, 1), device=device, dtype=torch.float32).bernoulli_(keep)
+            out.append(mask.reshape(batch) / keep)
         return torch.cat(out)
+
+    def _mpvit_drop_scales(self, backbone, batch, device):
+        """The scales of a natively run MPViT, [block][attention, MLP][B]: one DropPath module serves both branches of
+        its block, called twice.  None when none is in training mode."""
+        _, mods = self.mpvit_drop_paths(backbone)
+        return self._draw_drop_scales([m for m in mods for _ in range(2)], batch, device)
+
+    def _swin_drop_scales(self, backbone, batch, device):
+        """The scales of a natively run Swin, [block][attention, FFN][B]; None when no branch draws."""
+        return self._draw_drop_scales(self.swin_drop_paths(backbone)[1], batch, device)
 
     @staticmethod
     def _bn_modes(module):
@@ -509,17 +543,32 @@ class DDIMHeadBase(nn.Module):
                                        loop_backward, producer_train)
 
     def _engine_key(self, batch, latent_hw, cond_hw, device, native=False, image_hw=None, backward=False,
-                    loop_backward=False, mpvit_drop=()) -> EngineKey:
+                    loop_backward=False, drop_path=()) -> EngineKey:
         return EngineKey(batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)),
                          self.diffusion_inference_steps, self.use_cuda_graph, native,
                          tuple(image_hw) if image_hw is not None else None, bool(self.return_intermediates),
                          bool(self.fp8_corrections), native and bool(self.producer_train_bn), bool(backward),
-                         bool(loop_backward), tuple(mpvit_drop))
+                         bool(loop_backward), tuple(drop_path))
 
     def _mpvit_native_train(self, image_hw, backbone):
         """Whether the engine running this backbone also runs it in training mode (stochastic depth included)."""
         return (image_hw is not None and self.mpvit_native_train and self.producer_train_bn
                 and type(self._backbone(backbone)).__name__ == "MPViT")
+
+    def _native_drop_paths(self, image_hw, backbone):
+        """(per-stage marks, scale drawer) of the stochastic depth the engine runs on this backbone, or None: an MPViT
+        under `mpvit_native_train`, or a Swin whose drop-path rate is above 0 (`set_drop_path_rate`; the factories
+        build at 0).  The drawer returns the scales of this forward, or None when no module is in training mode."""
+        if image_hw is None:
+            return None
+        bb = self._backbone(backbone)
+        if self._mpvit_native_train(image_hw, bb):
+            return self.mpvit_drop_paths(bb)[0], lambda B, dev: self._mpvit_drop_scales(bb, B, dev)
+        if type(bb).__name__ == "SwinTransformer":
+            masks = self.swin_drop_paths(bb)[0]
+            if any(masks):
+                return masks, lambda B, dev: self._swin_drop_scales(bb, B, dev)
+        return None
 
     def _grad_engine(self, batch, latent_hw, cond_hw, device) -> DenoiseEngine:
         """The engine `denoiser_backward` runs on: the loop-backward engine of this geometry when the head trains through
@@ -534,8 +583,9 @@ class DDIMHeadBase(nn.Module):
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
-        drop = self.mpvit_drop_paths(self._backbone(backbone))[0] if self._mpvit_native_train(image_hw, backbone) else ()
-        key = self._engine_key(batch, latent_hw, cond_hw, device, native, image_hw, backward, loop_backward, drop)
+        drop = self._native_drop_paths(image_hw, backbone)
+        key = self._engine_key(batch, latent_hw, cond_hw, device, native, image_hw, backward, loop_backward,
+                               drop[0] if drop else ())
         eng = self._engines.get(key)
         if eng is None:
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
@@ -549,9 +599,9 @@ class DDIMHeadBase(nn.Module):
                 if type(self._backbone(backbone)).__name__ == "MPViT":
                     layers, dims, paths, ratio = self.mpvit_spec(self._backbone(backbone))
                     eng.enable_backbone(image_hw, depths=layers, kind="mpvit", mp_dims=dims, mp_paths=paths, mlp_ratio=ratio,
-                                        mp_drop_path=key.mpvit_drop or (0, 0, 0, 0))
+                                        mp_drop_path=key.drop_path or (0, 0, 0, 0))
                 elif self.variant == "swin":
-                    eng.enable_backbone(image_hw)
+                    eng.enable_backbone(image_hw, mp_drop_path=key.drop_path or (0, 0, 0, 0))
                 else:
                     eng.enable_backbone(image_hw, depths=[len(st) for st in self._backbone(backbone).layers], kind="resnet")
             ts, cx, ce = self.scheduler.fused_coefficients(self.diffusion_inference_steps)
@@ -739,9 +789,9 @@ class DDIMHeadBase(nn.Module):
             B, dev, dtype = image.shape[0], image.device, torch.float32
             sizes = self.backbone_pyramid(image.shape[-2:], self._backbone(backbone))
             native = True
-            native_train = self._mpvit_native_train(image.shape[-2:], backbone)
-            if native_train:  # drawn first, as the torch backbone's forward would before the head draws x_T
-                drop_scales = self._mpvit_drop_scales(self._backbone(backbone), B, dev)
+            drop = self._native_drop_paths(image.shape[-2:], backbone)
+            if drop is not None:  # drawn first, as the torch backbone's forward would before the head draws x_T
+                drop_scales = drop[1](B, dev)
         else:
             if self.detach_fp is not False and self.detach_fp is not None:
                 idx = self.detach_fp if isinstance(self.detach_fp, (list, tuple, range)) else range(len(fp))
@@ -774,7 +824,7 @@ class DDIMHeadBase(nn.Module):
                                    image_hw=tuple(image.shape[-2:]), backbone=backbone, producer_train=ptrain)
                 if eng.producer_train:
                     eng.set_producer_mode(ptrain_bb)
-                if native_train:
+                if drop is not None:
                     eng.set_drop_path(drop_scales)
                 eng.run_backbone(image.contiguous().float())
                 if eng.producer_train:

@@ -215,9 +215,10 @@ typedef struct dd_backbone_config {
   int32_t mp_dims[4];  /* DD_BACKBONE_MPVIT only: 64, 128, 216, 288 (mpvit_small) */
   int32_t mp_paths[4]; /* 2, 3, 3, 3 */
   int32_t mlp_ratio;   /* 4 */
-  int32_t mp_drop_path[4]; /* DD_BACKBONE_MPVIT only: bit l of entry s set = encoder layer l of stage s (in every path)
-                              has stochastic depth (a DropPath of rate > 0) on its two residual branches; see
-                              dd_set_drop_path.  All zero: none */
+  int32_t mp_drop_path[4]; /* DD_BACKBONE_MPVIT and DD_BACKBONE_SWIN: bit k of entry s set = block k of stage s has
+                              stochastic depth (a DropPath of rate > 0) on its two residual branches, attention then
+                              MLP / FFN; see dd_set_drop_path.  MPViT: encoder layer k in every path of the stage;
+                              Swin: SwinBlock k.  All zero: none.  Ignored by DD_BACKBONE_RESNET */
 } dd_backbone_config;
 int dd_enable_backbone(dd_handle h, const dd_backbone_config* bc);
 
@@ -360,13 +361,14 @@ int dd_set_producer_mode(dd_handle h, int32_t mode);
  * with feature maps) evaluated its layer in DD_PRODUCER_TRAIN (dd_producer_bn_info's *fresh). */
 int dd_producer_batch_stats(dd_handle h, float* dev_out, int64_t capacity, int32_t* n_out, void* cuda_stream);
 
-/* Stochastic depth of the MPViT backbone (reference mpvit.py:432,435, timm DropPath in training mode): dev_scales
- * (device fp32, n of them) holds, for every block dd_backbone_config.mp_drop_path marks, in stage, path, layer order,
- * the B per-sample scales mask / (1 - rate) of its attention branch, then the B of its MLP branch.  They are copied on
- * cuda_stream into an engine-owned buffer that every later dd_run_backbone reads (graphs included), in either producer
- * mode: x = x + scale[b] branch.  n = 0 turns stochastic depth off (the default; dev_scales may be NULL).  DD_ERR_INVALID
- * when n is neither 0 nor 2 x batch x the marked blocks, or before dd_finalize_weights of an MPViT backbone (which also
- * turns it off). */
+/* Stochastic depth of the MPViT backbone (reference mpvit.py:432,435, timm DropPath in training mode) or of the Swin
+ * backbone (reference swin.py:412,421, mmcv DropPath in training mode): dev_scales (device fp32, n of them) holds, for
+ * every block dd_backbone_config.mp_drop_path marks, the B per-sample scales mask / (1 - rate) of its attention branch,
+ * then the B of its MLP / FFN branch; blocks in stage, path, layer order (MPViT) or stage, block order (Swin).  They are
+ * copied on cuda_stream into an engine-owned buffer that every later dd_run_backbone reads (graphs included), in either
+ * producer mode: x = x + scale[b] branch.  n = 0 turns stochastic depth off (the default; dev_scales may be NULL).
+ * DD_ERR_INVALID when n is neither 0 nor 2 x batch x the marked blocks, or before dd_finalize_weights of an MPViT or
+ * Swin backbone (which also turns it off). */
 int dd_set_drop_path(dd_handle h, const float* dev_scales, int32_t n, void* cuda_stream);
 
 /* Record i: the registered key prefix of its BatchNorm (e.g. `hahineck.trans_fusion.1.bn`, `conv_up.0.1`,
