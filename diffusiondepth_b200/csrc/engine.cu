@@ -433,11 +433,6 @@ struct DropPathState {
 struct dd_engine {
   dd_config cfg;
   int sm_count = 0;
-  int up_qpb = 4;      // quads per block in gn_apply_up_split_kernel; DD_PROBES build: DD_UP_QPB=1 -> one 64-thread block per quad (A/B: equal)
-  bool f8_ne3 = true;  // DD_PROBES build: DD_F8_NE3=0 keeps noise_embedding.3 on the 3-pass split (A/B timing)
-  // tuning switches: read from the environment ONCE in dd_create, and only in a -DDD_PROBES build; a product build
-  // ignores the variables altogether
-  int attn_simt = 0;     // DD_ATTN_SIMT=1 (probes build): window attention on the fp32 CUDA-core kernel
   bool weights_ready = false;
   bool packed = false;  // a dd_finalize_weights has completed and its buffers are intact (dd_update_weights needs that)
   std::map<std::string, Raw> raw;
@@ -943,14 +938,8 @@ size_t carve(dd_engine* e, void* base) {
 }
 
 // One convolution on the engine's latent grid.  in planes have `cin` channels (scale in_scale).
-// f8 bit 0: the INPUT planes are hi / a8 / l8 (in_lo = base of the e4m3 pair: a8, then l8 B*P*cin bytes further) and the
-// conv runs with fp8 correction products; bit 1: the OUTPUT planes are written as hi / a8 / l8 (out_lo = their base).
-constexpr int kF8In = 1, kF8Out = 2;
-// DD_FLAG_FP8_CORR is accepted and runs the exact 3-pass split: Hopper's e4m3 wgmma accumulates with reduced precision,
-// so correction products added into the running fp32 sum of the hi * hi product would be lost.
-bool fp8_active(const dd_engine*) { return false; }
 int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, float in_scale, int epi, float* y32,
-             double* stats_partial, __half* out_hi, __half* out_lo, cudaStream_t st, int f8 = 0) {
+             double* stats_partial, __half* out_hi, __half* out_lo, cudaStream_t st) {
   const Geom g = geom_of(e->cfg);
   ConvLayer& L = e->L[layer];
   dd::ConvArgs a;
@@ -963,17 +952,9 @@ int run_conv(dd_engine* e, int layer, const __half* in_hi, const __half* in_lo, 
   a.stats_partial = stats_partial;
   a.out_hi = out_hi;
   a.out_lo = out_lo;
-  a.out_a8 = a.out_l8 = nullptr;
-  if (f8 & kF8Out) {
-    a.out_a8 = reinterpret_cast<uint8_t*>(out_lo);
-    a.out_l8 = a.out_a8 + static_cast<size_t>(g.B) * g.P * kShapes[L.sid].cout;
-  }
   a.split_scale = kActScale;
   a.status = e->status;
   const bool simt = (e->cfg.flags & DD_FLAG_SIMT_CONV) != 0;
-  if (f8)
-    return fail(DD_ERR_INVALID, simt ? "fp8-correction planes need the tensor-core kernel"
-                                     : "fp8-correction planes are not supported by the sm_90a kernels");
   int rc;
   if ((rc = launch_conv3x3(L.sid, epi, simt, a, in_hi, in_lo, in_scale, L.w_simt, L.mh_hi, L.mh_lo, e->sm_count, st)))
     return rc;
@@ -1012,7 +993,7 @@ void launch_apply(const dd::ApplyArgs& a, int B, int up_qpb, cudaStream_t st) {
 
 template <int C, int COND>
 int run_apply(dd_engine* e, int which, const float* temb, int temb_bstride, __half* out_hi, __half* out_lo,
-              cudaStream_t st, bool out_f8 = false, const float* y = nullptr) {
+              cudaStream_t st, const float* y = nullptr) {
   const Geom g = geom_of(e->cfg);
   dd::ApplyArgs a;
   a.y = y != nullptr ? y : e->Y;
@@ -1030,14 +1011,9 @@ int run_apply(dd_engine* e, int which, const float* temb, int temb_bstride, __ha
   a.rx = g.w > 1 ? static_cast<float>(a.cw - 1) / static_cast<float>(g.w - 1) : 0.f;
   a.out_hi = out_hi;
   a.out_lo = out_lo;
-  a.out_a8 = a.out_l8 = nullptr;
-  if (out_f8) {  // hi + e4m3 a8 / l8 planes; the e4m3 pair shares the fp16 lo plane's storage
-    a.out_a8 = reinterpret_cast<uint8_t*>(out_lo);
-    a.out_l8 = a.out_a8 + static_cast<size_t>(g.B) * g.P * C;
-  }
   a.scale = kActScale;
   a.status = e->status;
-  launch_apply<C, COND>(a, g.B, e->up_qpb, st);
+  launch_apply<C, COND>(a, g.B, 4, st);
   return launched(e, "gn_apply");
 }
 
@@ -1106,29 +1082,24 @@ int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float 
   // noise_embedding.0 : x (16) -> 64, GN stats
   if ((rc = run_conv(e, 0, e->xs_hi, e->xs_lo, kXScale, dd::EPI_F32_STATS, e->Y, e->stats[0], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 0, 64, st))) return rc;
-  // with DD_FLAG_FP8_CORR noise_embedding.3 takes hi / a8 / l8 planes too (fp16 hi*hi + two e4m3 correction products)
-  const bool f8_ne3 = fp8_active(e) && e->f8_ne3;
-  if ((rc = run_apply<64, 0>(e, 0, nullptr, 0, e->S_hi[0], e->S_lo[0], st, f8_ne3))) return rc;
+  if ((rc = run_apply<64, 0>(e, 0, nullptr, 0, e->S_hi[0], e->S_lo[0], st))) return rc;
   // noise_embedding.3 : 64 -> 256, GN stats
-  if ((rc = run_conv(e, 1, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_F32_STATS, e->Y, e->stats[1], nullptr, nullptr, st,
-                     f8_ne3 ? kF8In : 0))) return rc;
+  if ((rc = run_conv(e, 1, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_F32_STATS, e->Y, e->stats[1], nullptr, nullptr, st)))
+    return rc;
   if ((rc = run_finalize(e, 1, 256, st))) return rc;
   const __half *p_hi, *p_lo;
   if (e->cfg.variant == DD_VARIANT_SWIN) {
     // feat = up(cond + temb) + relu(gn(y2));  convA ; convB   (UpSample_add)
-    // with DD_FLAG_FP8_CORR convA and convB take hi / a8 / l8 planes (fp8 correction products); convB's output feeds the
-    // swapped-operand pred.0 kernel and stays fp16 hi / lo
-    const bool f8 = fp8_active(e);
-    if ((rc = run_apply<256, 2>(e, 1, temb, temb_bstride, e->S_hi[1], e->S_lo[1], st, f8))) return rc;
-    if ((rc = run_conv(e, 2, e->S_hi[1], e->S_lo[1], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[0], e->S_lo[0], st,
-                       f8 ? (kF8In | kF8Out) : 0))) return rc;
+    if ((rc = run_apply<256, 2>(e, 1, temb, temb_bstride, e->S_hi[1], e->S_lo[1], st))) return rc;
+    if ((rc = run_conv(e, 2, e->S_hi[1], e->S_lo[1], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[0], e->S_lo[0], st)))
+      return rc;
     if (fold_active(e)) {  // convB + pred.0 as one composed conv + its ring correction
       if ((rc = run_fold(e, st))) return rc;
       if ((rc = run_finalize(e, 2, 64, st, e->stats[3], ring_blocks_per_img(g)))) return rc;
       return run_tail(e, cx, ce, eps_out, st);
     }
-    if ((rc = run_conv(e, 3, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[1], e->S_lo[1], st,
-                       f8 ? kF8In : 0))) return rc;
+    if ((rc = run_conv(e, 3, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[1], e->S_lo[1], st)))
+      return rc;
     p_hi = e->S_hi[1];
     p_lo = e->S_lo[1];
   } else {
@@ -1273,9 +1244,7 @@ int poll_status(dd_engine* h, cudaStream_t st) {
   CUDA_TRY(cudaMemcpyAsync(h->status_host, h->status, 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   if (*h->status_host & 1)
-    return fail(DD_ERR_RANGE, "an activation exceeded the operand split's range (16 |v| > 6e4; with fp8 corrections, "
-                              "DD_FLAG_FP8_CORR, 16 |v| > 1792: create the engine without that flag / set "
-                              "head.fp8_corrections = False)");
+    return fail(DD_ERR_RANGE, "an activation exceeded the operand split's range (16 |v| > 6e4)");
   return DD_OK;
 }
 
@@ -2275,10 +2244,10 @@ int run_merge_ln(dd_engine* e, int C, const float* x, const float* g, const floa
   return launched(e, "merge_ln_split");
 }
 
-// Window attention on the fp32 CUDA-core kernel: the check path (DD_FLAG_SIMT_CONV, probes switch) and any odd head
-// count (the wgmma kernel takes heads in pairs).
+// Window attention on the fp32 CUDA-core kernel: the check path (DD_FLAG_SIMT_CONV) and any odd head count (the wgmma
+// kernel takes heads in pairs).
 bool attn_simt(const dd_engine* e, int nH) {
-  return (e->cfg.flags & DD_FLAG_SIMT_CONV) || (nH & 1) || e->attn_simt;
+  return (e->cfg.flags & DD_FLAG_SIMT_CONV) || (nH & 1);
 }
 
 // One (shifted-)window attention launch (7 x 7 windows, head_dim 32): qkv fp32 [B*H*W][3C] (padded tokens carry
@@ -2568,19 +2537,19 @@ int run_recompute(dd_engine* e, const float* temb, int temb_bstride, cudaStream_
   int rc;
   if ((rc = run_conv(e, 0, e->xs_hi, e->xs_lo, kXScale, dd::EPI_F32_STATS, b.y1, e->stats[0], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 0, 64, st))) return rc;
-  if ((rc = run_apply<64, 0>(e, 0, nullptr, 0, b.a1.hi, b.a1.lo, st, false, b.y1))) return rc;
+  if ((rc = run_apply<64, 0>(e, 0, nullptr, 0, b.a1.hi, b.a1.lo, st, b.y1))) return rc;
   if ((rc = run_conv(e, 1, b.a1.hi, b.a1.lo, kActScale, dd::EPI_F32_STATS, b.y2, e->stats[1], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 1, 256, st))) return rc;
   if (e->cfg.variant == DD_VARIANT_SWIN) {
-    if ((rc = run_apply<256, 2>(e, 1, temb, temb_bstride, b.f0.hi, b.f0.lo, st, false, b.y2))) return rc;
+    if ((rc = run_apply<256, 2>(e, 1, temb, temb_bstride, b.f0.hi, b.f0.lo, st, b.y2))) return rc;
     if ((rc = run_conv(e, 2, b.f0.hi, b.f0.lo, kActScale, dd::EPI_SPLIT, nullptr, nullptr, b.fa.hi, b.fa.lo, st))) return rc;
     if ((rc = run_conv(e, 3, b.fa.hi, b.fa.lo, kActScale, dd::EPI_SPLIT, nullptr, nullptr, b.fp.hi, b.fp.lo, st))) return rc;
-  } else if ((rc = run_apply<256, 1>(e, 1, temb, temb_bstride, b.fp.hi, b.fp.lo, st, false, b.y2))) {
+  } else if ((rc = run_apply<256, 1>(e, 1, temb, temb_bstride, b.fp.hi, b.fp.lo, st, b.y2))) {
     return rc;
   }
   if ((rc = run_conv(e, 4, b.fp.hi, b.fp.lo, kActScale, dd::EPI_F32_STATS, b.y5, e->stats[2], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 2, 64, st))) return rc;
-  if ((rc = run_apply<64, 0>(e, 2, nullptr, 0, b.a5.hi, b.a5.lo, st, false, b.y5))) return rc;
+  if ((rc = run_apply<64, 0>(e, 2, nullptr, 0, b.a5.hi, b.a5.lo, st, b.y5))) return rc;
   if ((rc = run_conv(e, 5, b.a5.hi, b.a5.lo, kActScale, dd::EPI_F32_STATS, b.y6, e->stats[3], nullptr, nullptr, st))) return rc;
   return run_finalize(e, 3, 16, st);
 }
@@ -2866,11 +2835,6 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
   dd_engine* e = new dd_engine();
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
-#ifdef DD_PROBES
-  if (const char* v = getenv("DD_ATTN_SIMT")) e->attn_simt = atoi(v);
-  if (const char* v = getenv("DD_F8_NE3")) e->f8_ne3 = atoi(v) != 0;
-  if (const char* v = getenv("DD_UP_QPB")) e->up_qpb = atoi(v);
-#endif
   if (cudaMallocHost(&e->status_host, 64) != cudaSuccess ||
       cudaMallocHost(&e->stage, sizeof(PackStage)) != cudaSuccess ||
       cudaEventCreateWithFlags(&e->pack_done, cudaEventDisableTiming) != cudaSuccess ||
@@ -3781,7 +3745,6 @@ int dd_conv3x3(dd_handle h, const float* x, const float* w, const float* b, floa
   a.stats_partial = nullptr;
   a.out_hi = nullptr;
   a.out_lo = nullptr;
-  a.out_a8 = a.out_l8 = nullptr;
   a.split_scale = 1.f;
   a.status = v.status;
   const bool simt = (h->cfg.flags & DD_FLAG_SIMT_CONV) != 0;
@@ -4132,7 +4095,6 @@ int dd_conv_groupnorm(dd_handle h, const dd_conv_gn_desc* d, const float* x, con
   a.y32 = yn;
   a.stats_partial = partial;
   a.out_hi = a.out_lo = nullptr;
-  a.out_a8 = a.out_l8 = nullptr;
   a.split_scale = 1.f;
   a.status = call.status;
   CUtensorMap mb_hi{}, mb_lo{};
@@ -4188,7 +4150,6 @@ int dd_conv_groupnorm(dd_handle h, const dd_conv_gn_desc* d, const float* x, con
     g.rx = W > 1 ? static_cast<float>(cw - 1) / static_cast<float>(W - 1) : 0.f;
     g.out_hi = o.hi;
     g.out_lo = o.lo;
-    g.out_a8 = g.out_l8 = nullptr;
     g.scale = kActScale;
     g.status = call.status;
     if (mode != 0) {
@@ -4242,13 +4203,12 @@ int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* 
     if (h->L[i].sid >= 0 && kShapes[h->L[i].sid].cin == cin && kShapes[h->L[i].sid].cout == cout) layer = i;
   if (layer < 0) return fail(DD_ERR_UNSUPPORTED, "no packed layer with that shape in this engine variant");
   const bool split_out = (cin == 256 && cout == 256);
-  const int f8 = ((split_out || (cin == 64 && cout == 256 && h->f8_ne3)) && fp8_active(h)) ? kF8In : 0;  // time the kernel the loop actually runs
   // whatever the planes currently hold is fine for timing: MMA time is data independent
   const __half* in_hi = cin == 16 ? h->xs_hi : h->S_hi[1];
   const __half* in_lo = cin == 16 ? h->xs_lo : h->S_lo[1];
   return time_per_call(st, 2, iters, ms_out, [&]() {
     return run_conv(h, layer, in_hi, in_lo, kActScale, split_out ? dd::EPI_SPLIT : dd::EPI_F32_STATS, h->Y, h->stats[0],
-                    h->S_hi[0], h->S_lo[0], st, f8);
+                    h->S_hi[0], h->S_lo[0], st);
   });
 }
 

@@ -80,49 +80,7 @@ __global__ void join_planes_kernel(const __half* __restrict__ hi, const __half* 
     x[i] = (__half2float(hi[i]) + __half2float(lo[i])) * inv_scale;
 }
 
-// fp32 NHWC -> fp16 hi plane + e4m3 a8 / l8 planes (standalone-layer path of the fp8-correction kernel)
-__global__ void split_planes8_kernel(const float* __restrict__ x, __half* __restrict__ hi, uint8_t* __restrict__ a8,
-                                     uint8_t* __restrict__ l8, size_t n8, float scale, int* status) {
-  bool ov = false;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n8;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const float4 u0 = reinterpret_cast<const float4*>(x)[2 * i], u1 = reinterpret_cast<const float4*>(x)[2 * i + 1];
-    const float v[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
-    __align__(16) __half h[8];
-    __align__(8) uint16_t pa[4];
-    __align__(8) uint16_t pl[4];
-#pragma unroll
-    for (int j = 0; j < 8; j += 2) {
-      const float s0 = v[j] * scale, s1 = v[j + 1] * scale;
-      ov |= (fabsf(s0) > kF8ActMax) | (fabsf(s1) > kF8ActMax);
-      h[j] = __float2half_rn(s0);
-      h[j + 1] = __float2half_rn(s1);
-      pa[j >> 1] = e4m3x2(s0 * kF8ActDiv, s1 * kF8ActDiv);
-      pl[j >> 1] = e4m3x2((s0 - __half2float(h[j])) * kF8LoMul, (s1 - __half2float(h[j + 1])) * kF8LoMul);
-    }
-    reinterpret_cast<uint4*>(hi)[i] = *reinterpret_cast<const uint4*>(h);
-    reinterpret_cast<uint2*>(a8)[i] = *reinterpret_cast<const uint2*>(pa);
-    reinterpret_cast<uint2*>(l8)[i] = *reinterpret_cast<const uint2*>(pl);
-  }
-  if (ov) atomicOr(status, 1);
-}
-
 // ------------------------------------------------------------------ weight pre-pack
-// fp8-correction weight planes [tap][COUT][CIN] bytes: w8 = e4m3(t w / 512) (partner of the activation l8, scaled by
-// 512), lw8 = e4m3((t w - fp16(t w)) * 4) (partner of a8, scaled by 1/4); t = the layer's fp16 weight scale
-__global__ void pack_conv_weight8_kernel(const float* __restrict__ w, uint8_t* __restrict__ w8, uint8_t* __restrict__ lw8,
-                                         int cout, int cin, float scale) {
-  const int n = cout * cin * 9;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int tap = i % 9, ci = (i / 9) % cin, co = i / (9 * cin);
-    const float s = w[i] * scale;
-    const float h = __half2float(__float2half_rn(s));
-    const size_t o = (static_cast<size_t>(tap) * cout + co) * cin + ci;
-    w8[o] = static_cast<uint8_t>(e4m3x2(s * (1.f / kF8LoMul), 0.f) & 0xff);
-    lw8[o] = static_cast<uint8_t>(e4m3x2((s - h) * (1.f / kF8ActDiv), 0.f) & 0xff);
-  }
-}
-
 // w [COUT][CIN][3][3] fp32 -> hi/lo fp16 [tap][COUT][CIN] (scaled) and fp32 [tap][CIN][COUT] (SIMT path)
 __global__ void pack_conv_weight_kernel(const float* __restrict__ w, __half* __restrict__ hi, __half* __restrict__ lo,
                                         float* __restrict__ w_simt, int cout, int cin, float scale) {
@@ -217,38 +175,19 @@ struct ApplyArgs {
   float ry, rx;            // (ch-1)/(H-1), (cw-1)/(W-1) in fp32 as ATen computes them
   __half* out_hi;
   __half* out_lo;
-  uint8_t* out_a8;         // non-null: the consumer uses fp8 corrections -> write e4m3 planes a8 / l8 instead of fp16 lo
-  uint8_t* out_l8;
   float scale;
   int* status;
 };
 
-// 8 consecutive channels of one pixel -> operand planes (fp16 hi + fp16 lo, or fp16 hi + e4m3 a8 + e4m3 l8)
+// 8 consecutive channels of one pixel -> fp16 hi / lo operand planes
 __device__ __forceinline__ void store_planes8(const float (&v)[8], float scale, __half* out_hi, __half* out_lo,
-                                              uint8_t* out_a8, uint8_t* out_l8, size_t off, bool& ov) {
+                                              size_t off, bool& ov) {
   __align__(16) __half h[8];
-  if (out_a8 != nullptr) {
-    __align__(8) uint16_t a8[4];
-    __align__(8) uint16_t l8[4];
+  __align__(16) __half l[8];
 #pragma unroll
-    for (int j = 0; j < 8; j += 2) {
-      const float s0 = v[j] * scale, s1 = v[j + 1] * scale;
-      ov |= (fabsf(s0) > kF8ActMax) | (fabsf(s1) > kF8ActMax);
-      h[j] = __float2half_rn(s0);
-      h[j + 1] = __float2half_rn(s1);
-      a8[j >> 1] = e4m3x2(s0 * kF8ActDiv, s1 * kF8ActDiv);
-      l8[j >> 1] = e4m3x2((s0 - __half2float(h[j])) * kF8LoMul, (s1 - __half2float(h[j + 1])) * kF8LoMul);
-    }
-    *reinterpret_cast<uint4*>(out_hi + off) = *reinterpret_cast<const uint4*>(h);
-    *reinterpret_cast<uint2*>(out_a8 + off) = *reinterpret_cast<const uint2*>(a8);
-    *reinterpret_cast<uint2*>(out_l8 + off) = *reinterpret_cast<const uint2*>(l8);
-  } else {
-    __align__(16) __half l[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) split_f16(v[j], scale, h[j], l[j], ov);
-    *reinterpret_cast<uint4*>(out_hi + off) = *reinterpret_cast<const uint4*>(h);
-    *reinterpret_cast<uint4*>(out_lo + off) = *reinterpret_cast<const uint4*>(l);
-  }
+  for (int j = 0; j < 8; ++j) split_f16(v[j], scale, h[j], l[j], ov);
+  *reinterpret_cast<uint4*>(out_hi + off) = *reinterpret_cast<const uint4*>(h);
+  *reinterpret_cast<uint4*>(out_lo + off) = *reinterpret_cast<const uint4*>(l);
 }
 
 template <int C, int COND>
@@ -324,7 +263,7 @@ __global__ void __launch_bounds__(256) gn_apply_split_kernel(const ApplyArgs a) 
   }
 
   bool ov = false;
-  store_planes8(v, a.scale, a.out_hi, a.out_lo, a.out_a8, a.out_l8, off, ov);
+  store_planes8(v, a.scale, a.out_hi, a.out_lo, off, ov);
   if (ov) atomicOr(a.status, 1);
 }
 
@@ -340,13 +279,13 @@ __global__ void __launch_bounds__(256) gn_apply_split_kernel(const ApplyArgs a) 
 // the time embedding and the weights (exact), and the time embedding enters once (interp(cond + te) == interp(cond) + te *
 // (sum of the weights), which is 1 within 2 ulp).
 
-// V (4 or 8) consecutive channels of one pixel, ALREADY multiplied by the operand scale -> planes; `mx` collects max |s|
+// V (4 or 8) consecutive channels of one pixel, ALREADY multiplied by the operand scale -> fp16 hi / lo planes; `mx`
+// collects max |s|
 template <int V>
-__device__ __forceinline__ void store_planes_scaled(const float (&s)[V], __half* out_hi, __half* out_lo, uint8_t* out_a8,
-                                                    uint8_t* out_l8, size_t off, float& mx) {
+__device__ __forceinline__ void store_planes_scaled(const float (&s)[V], __half* out_hi, __half* out_lo, size_t off,
+                                                    float& mx) {
   static_assert(V == 4 || V == 8, "4 or 8 channels per thread");
   using VH = typename std::conditional<V == 8, uint4, uint2>::type;  // V fp16 values
-  using VB = typename std::conditional<V == 8, uint2, uint32_t>::type;  // V e4m3 values
   __align__(16) __half2 h[V / 2];
 #pragma unroll
   for (int j = 0; j < V / 2; ++j) {
@@ -354,26 +293,13 @@ __device__ __forceinline__ void store_planes_scaled(const float (&s)[V], __half*
     mx = fmaxf(mx, fmaxf(fabsf(s[2 * j]), fabsf(s[2 * j + 1])));
   }
   *reinterpret_cast<VH*>(out_hi + off) = *reinterpret_cast<const VH*>(h);
-  if (out_a8 != nullptr) {
-    __align__(8) uint16_t a8[V / 2];
-    __align__(8) uint16_t l8[V / 2];
+  __align__(16) __half2 l[V / 2];
 #pragma unroll
-    for (int j = 0; j < V / 2; ++j) {
-      const float2 hf = __half22float2(h[j]);
-      a8[j] = e4m3x2(s[2 * j] * kF8ActDiv, s[2 * j + 1] * kF8ActDiv);
-      l8[j] = e4m3x2((s[2 * j] - hf.x) * kF8LoMul, (s[2 * j + 1] - hf.y) * kF8LoMul);
-    }
-    *reinterpret_cast<VB*>(out_a8 + off) = *reinterpret_cast<const VB*>(a8);
-    *reinterpret_cast<VB*>(out_l8 + off) = *reinterpret_cast<const VB*>(l8);
-  } else {
-    __align__(16) __half2 l[V / 2];
-#pragma unroll
-    for (int j = 0; j < V / 2; ++j) {
-      const float2 hf = __half22float2(h[j]);
-      l[j] = __floats2half2_rn(s[2 * j] - hf.x, s[2 * j + 1] - hf.y);
-    }
-    *reinterpret_cast<VH*>(out_lo + off) = *reinterpret_cast<const VH*>(l);
+  for (int j = 0; j < V / 2; ++j) {
+    const float2 hf = __half22float2(h[j]);
+    l[j] = __floats2half2_rn(s[2 * j] - hf.x, s[2 * j + 1] - hf.y);
   }
+  *reinterpret_cast<VH*>(out_lo + off) = *reinterpret_cast<const VH*>(l);
 }
 
 __device__ __forceinline__ void ld4(const float* p, float (&v)[4]) {
@@ -510,10 +436,10 @@ __global__ void __launch_bounds__(QPB * 256 / V, 12 / QPB) gn_apply_up_split_ker
         }
       }
       const size_t off = (static_cast<size_t>(b) * P + static_cast<size_t>(oy[r]) * a.W + ox[c]) * C + c0;
-      store_planes_scaled<V>(sv, a.out_hi, a.out_lo, a.out_a8, a.out_l8, off, mx);
+      store_planes_scaled<V>(sv, a.out_hi, a.out_lo, off, mx);
     }
   }
-  if (mx > (a.out_a8 != nullptr ? kF8ActMax : 60000.f)) atomicOr(a.status, 1);
+  if (mx > 60000.f) atomicOr(a.status, 1);
 }
 
 // ------------------------------------------------------------------ last GN + ReLU (C = 16) fused with the DDIM update

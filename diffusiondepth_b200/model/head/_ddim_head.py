@@ -67,7 +67,6 @@ class EngineKey(NamedTuple):
     native: bool                          # neck + FPN on the engine
     image_hw: Optional[Tuple[int, int]]   # and the backbone (None: not native)
     step_decode: bool
-    fp8_corr: bool
     producer_train: bool
     backward: bool
     loop_backward: bool
@@ -285,9 +284,8 @@ class DDIMHeadBase(nn.Module):
         self.incremental_repack = True   # after an optimizer step re-pack only the changed denoiser / codec tensors, in
         #                                  place (DenoiseEngine.update_weights; bit-identical); False: always the full pack
         self.native_backbone = True      # Swin-L backbone on the engine's GEMM/attention path (needs native_producers)
-        self.fp8_corrections = True      # Swin heads: correction products of convA / convB as e4m3 MMAs (DD_FLAG_FP8_CORR;
-        #                                  ~1.5x on the dominant kernel, max |dz| 3.4e-4 of the 1e-3 budget on config 3).
-        #                                  False = the exact 3-pass fp16 split everywhere.
+        self.fp8_corrections = True      # accepted and selects nothing on sm_90a: every conv runs the exact 3-pass fp16
+        #                                  split (Hopper's e4m3 wgmma accumulates at reduced precision; DESIGN.md §3)
         self.__dict__['_backbone_ref'] = None  # weakref to the model's depth_backbone (Diffusion_DCbase_Model passes the
         #                                        backbone with every call; this is the fallback for direct head calls)
         self.capture_cond = False        # tests: keep the NCHW condition map of the last forward
@@ -547,8 +545,7 @@ class DDIMHeadBase(nn.Module):
         return EngineKey(batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)),
                          self.diffusion_inference_steps, self.use_cuda_graph, native,
                          tuple(image_hw) if image_hw is not None else None, bool(self.return_intermediates),
-                         bool(self.fp8_corrections), native and bool(self.producer_train_bn), bool(backward),
-                         bool(loop_backward), tuple(drop_path))
+                         native and bool(self.producer_train_bn), bool(backward), bool(loop_backward), tuple(drop_path))
 
     def _mpvit_native_train(self, image_hw, backbone):
         """Whether the engine running this backbone also runs it in training mode (stochastic depth included)."""
@@ -591,8 +588,7 @@ class DDIMHeadBase(nn.Module):
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
             eng = DenoiseEngine(self.variant, batch, latent_hw, cond_hw, key.steps, device, cuda_graph=key.cuda_graph,
                                 check_range=False, step_decode=key.step_decode, workspace_pool=pool,
-                                fp8_corr=key.fp8_corr, backward=key.backward, loop_backward=key.loop_backward,
-                                producer_train=key.producer_train)
+                                backward=key.backward, loop_backward=key.loop_backward, producer_train=key.producer_train)
             if native:
                 eng.enable_producers(feats[0], feats[1], has_neck=self.has_neck)
             if image_hw is not None:
