@@ -446,6 +446,7 @@ struct dd_engine {
     float* src[2] = {nullptr, nullptr};  // convB's and pred.0's weights as registered: an update of one composes with the other
     double* k5 = nullptr;                // [64][256][25] the composition in fp64, and its magnitudes for the scale
     float* k5_abs = nullptr;
+    float* edge = nullptr;               // the ring correction's edge kernels (dd::EDGE_ELEMS)
   } fold;
   float* w_flip[6] = {};       // data-gradient layer 6 + i: layer i's weights flipped and transposed, before the split
   float* amax = nullptr;       // [16] abs-max words of the pack (PackStage::amax)
@@ -1058,9 +1059,7 @@ int run_fold(dd_engine* e, cudaStream_t st) {
   r.a_hi = e->S_hi[0];
   r.a_lo = e->S_lo[0];
   r.a_inv_scale = 1.f / kActScale;
-  r.wb = e->L[3].w_simt;
-  r.bb = e->L[3].bias;
-  r.wp = e->L[4].w_simt;
+  r.edge = e->fold.edge;
   r.y32 = e->Y;
   r.ring_partial = e->stats[3];
   dd::ring_fix_kernel<<<dim3(r.blocks_per_img, g.B), dd::RING_THREADS, dd::RING_SMEM, st>>>(r);
@@ -1404,6 +1403,7 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
     if ((rc = dev_array(h, &h->fold.src[1], 64 * 256 * 9))) return rc;
     if ((rc = dev_array(h, &h->fold.k5, n5))) return rc;
     if ((rc = dev_array(h, &h->fold.k5_abs, n5))) return rc;
+    if ((rc = dev_array(h, &h->fold.edge, dd::EDGE_ELEMS))) return rc;
   }
   for (int i = 0; i < 4; ++i) {
     if ((rc = dev_array(h, &h->gn_gamma[i], kGnCh[i]))) return rc;
@@ -1521,6 +1521,8 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     dd::compose_fold_kernel<<<256, 256, 0, st>>>(h->fold.src[1], h->L[4].bias, h->fold.src[0], h->L[3].bias, h->fold.k5,
                                                  h->fold.k5_abs, h->fold.bias);
     if ((rc = check_launch("compose_fold"))) return rc;
+    dd::compose_edge_kernel<<<256, 256, 0, st>>>(h->fold.src[1], h->fold.src[0], h->L[3].bias, h->fold.edge);
+    if ((rc = check_launch("compose_edge"))) return rc;
     dd::absmax_kernel<<<absmax_grid(64 * 256 * 25), 256, 0, st>>>(h->fold.k5_abs, 64 * 256 * 25, h->amax + 12);
     if ((rc = check_launch("absmax"))) return rc;
   }

@@ -9,8 +9,8 @@
 // The composition is exact where neither conv pads.  conv5x5_fold_kernel runs K5 on zero-padded a; at a pixel p next
 // to the border it then also counts pred.0 taps that land on positions q outside the image, where the chain has zeros:
 //   corr(p) = sum_{d: p + d outside} Wp0[d] b_ext(p + d),   b_ext(q) = bB + sum_{d': q + d' inside} WB[d'] a(q + d')
-// ring_fix_kernel subtracts corr on the one-pixel ring (fp32 CUDA cores; ~1.2 GMAC per step at B = 4, 176 x 608) and
-// writes the ring's GroupNorm partials; the composed kernel's partials cover the interior only.
+// ring_fix_kernel subtracts corr on the one-pixel ring (fp32 CUDA cores, as composed 1-D edge convs: ~0.5 GMAC per step
+// at B = 4, 176 x 608) and writes the ring's GroupNorm partials; the composed kernel's partials cover the interior only.
 #pragma once
 #include "conv_common.cuh"
 
@@ -276,20 +276,33 @@ conv5x5_fold_kernel(const __grid_constant__ CUtensorMap tmP_hi, const __grid_con
 }
 
 // ---------------------------------------------------------------------------------------------- ring correction
-// The ring (pixels with a 3 x 3 neighbour outside the image) is cut into straight sides, each counted once: top and
-// bottom rows, then the left and right columns between them; a latent with h <= 2 (or w <= 2) is all ring and is cut
-// into its rows (columns).  Sides are split into segments of at most RING_S pixels.
+// corr(p) cut by the side that each outside position q = p + d lies on.  Above the image (q in row -1) only convB taps
+// with d'y = +1 reach an inside pixel, all in row 0, so for p in row 0 the top share is a 1-D 5-tap 256 -> 64 conv of
+// a's row 0, zero-padded along the row:
+//   T(x) = cT + sum_{D = -2..2} ET[D] a(0, x + D),   ET[D] = sum_{dx + d'x = D} Wp0[-1][dx] WB[+1][d'x],
+//   cT = sum_dx Wp0[-1][dx] bB
+// and the same for the bottom row (B), the left column (L, along y) and the right column (R).  T and B own every d whose
+// row is outside; L and R own only the d whose row is inside, so their zero-padded column convs count the four corner
+// positions once too often and a corner fix-up removes that: at p = (0, 0) the left conv's d = (-1, -1) term is
+// Wp0[-1][-1] (bB + WB[+1][+1] a(0, 0)), and likewise at the other corners (Wp0[d] WB[-d] a(p) + Wp0[d] bB).  Hence
+//   corr(p) = [y = 0] T(x) + [y = h-1] B(x) + [x = 0] (L(y) - [y = 0] C_TL - [y = h-1] C_BL)
+//                                            + [x = w-1] (R(y) - [y = 0] C_TR - [y = h-1] C_BR),
+// which holds for any h, w >= 1.  The edge kernels and constants are composed in fp64 next to K5 (compose_edge_kernel):
+// about 0.5 GMAC per step at B = 4, 176 x 608, against 1.5 for building b_ext at every outside position.
+//
+// ring_fix_kernel cuts the ring into straight sides, each counted once: top and bottom rows, then the left and right
+// columns between them; a latent with h <= 2 (or w <= 2) is all ring and is cut into its rows (columns).  Sides are
+// split into segments of at most RING_S pixels.  A segment's own sides (T / B for a row, L / R for a column) are one
+// GEMM [pixels x 1280] . [1280 x 64] on a's line under the segment; the few end pixels that also lie on a crossing side
+// or a corner add those terms afterwards.
 constexpr int RING_S = 16;
-constexpr int RING_BOX = RING_S + 2;   // outside positions q of a segment: 3 x (n + 2) box around it
-constexpr int RING_ABOX = RING_S + 4;  // a(q + d'): 5 x (n + 4) box
-// Each convB output channel cm of b_ext is worked by RING_JG threads, one per slice of RING_JB box columns: the 156 KB
-// of boxes allow one block per SM, and with one thread per cm its 8 warps, each waiting on L2 for its weights every 4
-// input channels, ran the kernel at ~3 TFLOP/s.  Every sum keeps its operand order, so the result does not depend on
-// RING_JG.
-constexpr int RING_JG = 4;
-constexpr int RING_JB = (RING_BOX + RING_JG - 1) / RING_JG;
-constexpr int RING_THREADS = 256 * RING_JG;
-constexpr int RING_SMEM = (5 * RING_ABOX + 3 * RING_BOX + 4) * 256 * 4 + RING_S * 64 * 4;
+constexpr int RING_LINE = RING_S + 4;  // a along a segment and its 2-pixel halo
+constexpr int RING_THREADS = 256;
+constexpr int RING_KQ = 5 * 256 / 4;  // K rows per quarter of the own-side GEMM
+constexpr int RING_SMEM = RING_LINE * 256 * 4 + 4 * RING_S * 64 * 4 + 4 * 64 * 4 + 2 * 256 * 8;
+constexpr int EDGE_E = 5 * 256 * 64;  // one side's kernel [tap][ci][co]
+constexpr int EDGE_C = 256 * 64;      // one corner's [ci][co]
+constexpr int EDGE_ELEMS = 4 * EDGE_E + 4 * EDGE_C + 8 * 64;  // T, B, L, R; TL, TR, BL, BR; their constants [8][64]
 
 struct RingSide {
   int y0, x0, vert, len;
@@ -322,28 +335,36 @@ struct RingArgs {
   const __half* a_hi;        // convA output planes [B][H][W][256], value = (hi + lo) * a_inv_scale
   const __half* a_lo;
   float a_inv_scale;
-  const float* wb;           // convB [9][256 ci][256 cm] fp32
-  const float* bb;           // convB bias [256]
-  const float* wp;           // pred.0 [9][256 cm][64 co] fp32
+  const float* edge;         // EDGE_ELEMS fp32 (compose_edge_kernel)
   float* y32;                // [B][H][W][64]: the composed conv's output, corrected in place on the ring
   double* ring_partial;      // [B][blocks_per_img][4][2] GroupNorm fp64 sums of the corrected ring pixels
 };
 
 __device__ __forceinline__ bool inside_img(int y, int x, int H, int W) { return y >= 0 && y < H && x >= 0 && x < W; }
+// side s (0 T, 1 B, 2 L, 3 R) holds pixel (y, x)
+__device__ __forceinline__ bool on_side(int s, int y, int x, int H, int W) {
+  return s == 0 ? y == 0 : s == 1 ? y == H - 1 : s == 2 ? x == 0 : x == W - 1;
+}
 
 // grid (blocks_per_img, B), RING_THREADS threads
 __global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p) {
   extern __shared__ float4 ring_smem4[];
-  float* abox = reinterpret_cast<float*>(ring_smem4);  // [5][RING_ABOX][256]
-  float* bbox = abox + 5 * RING_ABOX * 256;           // [3][RING_BOX][256]
-  double* red = reinterpret_cast<double*>(bbox + 3 * RING_BOX * 256);  // [2][256]
-  float* ycor = bbox + (3 * RING_BOX + 4) * 256;      // [RING_S][64] corrected outputs of the segment
+  float* line = reinterpret_cast<float*>(ring_smem4);  // [RING_LINE][256]
+  float* corr = line + RING_LINE * 256;                // [RING_S][64]
+  float* part = corr + RING_S * 64;                    // [3][RING_S][64]: K quarters 1 .. 3, then the corrected outputs
+  float* xred = part + 3 * RING_S * 64;                // [4][64] ci-slice sums of an end pixel's extra terms
+  double* red = reinterpret_cast<double*>(xred + 4 * 64);  // [2][256]
   const int img = blockIdx.y, t = threadIdx.x;
   const int H = p.H, W = p.W;
+  const float* cst = p.edge + 4 * EDGE_E + 4 * EDGE_C;  // [8][64]
   RingSide sd[4];
   ring_sides(H, W, sd);
   const int s_begin = static_cast<int>(static_cast<long long>(p.nseg) * blockIdx.x / p.blocks_per_img);
   const int s_end = static_cast<int>(static_cast<long long>(p.nseg) * (blockIdx.x + 1) / p.blocks_per_img);
+  auto a_at = [&](int y, int x, int ci) {
+    const size_t o = ((static_cast<size_t>(img) * H + y) * W + x) * 256 + ci;
+    return (__half2float(p.a_hi[o]) + __half2float(p.a_lo[o])) * p.a_inv_scale;
+  };
   double ts = 0.0, tq = 0.0;  // fp64 per element: the ring is a few pixels per block
   for (int sg = s_begin; sg < s_end; ++sg) {
     int k = sg, si = 0;
@@ -352,15 +373,14 @@ __global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p
       ++si;
     }
     const int n = min(RING_S, sd[si].len - k * RING_S);
-    const int ly = sd[si].vert, lx = 1 - ly;  // along the segment (box coordinate c)
-    const int ay = lx, ax = ly;               // across it (box coordinate r)
+    const int ly = sd[si].vert, lx = 1 - ly;  // along the segment
     const int oy = sd[si].y0 + k * RING_S * ly, ox = sd[si].x0 + k * RING_S * lx;
+    const int s0 = 2 * ly;                    // the segment's own sides: T / B for a row, L / R for a column
     __syncthreads();  // the previous segment's shared-memory reads are done
-    // a on the 5 x (n + 4) box, zero outside the image, reconstructed from the split planes as the convs read it
-    for (int i = t; i < 5 * RING_ABOX * 32; i += RING_THREADS) {
+    // a along the segment, positions -2 .. RING_S + 1, zero outside the image and past the segment's halo
+    for (int i = t; i < RING_LINE * 32; i += RING_THREADS) {
       const int c8 = i & 31, pos = i >> 5;
-      const int r = pos / RING_ABOX - 2, c = pos % RING_ABOX - 2;
-      const int y = oy + r * ay + c * ly, x = ox + r * ax + c * lx;
+      const int c = pos - 2, y = oy + c * ly, x = ox + c * lx;
       float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
       if (c <= n + 1 && inside_img(y, x, H, W)) {
         const size_t o = ((static_cast<size_t>(img) * H + y) * W + x) * 256 + c8 * 8;
@@ -371,90 +391,121 @@ __global__ void __launch_bounds__(RING_THREADS) ring_fix_kernel(const RingArgs p
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = (__half2float(hh[j]) + __half2float(ll[j])) * p.a_inv_scale;
       }
-      float4* d = reinterpret_cast<float4*>(abox + pos * 256 + c8 * 8);
+      float4* d = reinterpret_cast<float4*>(line + pos * 256 + c8 * 8);
       d[0] = make_float4(v[0], v[1], v[2], v[3]);
       d[1] = make_float4(v[4], v[5], v[6], v[7]);
     }
     __syncthreads();
-    // b_ext at the box's outside positions, one box row at a time; thread = (convB output channel cm, box columns
-    // [j0, j0 + RING_JB))
-    const int cm = t & 255, j0 = (t >> 8) * RING_JB;
-    for (int r = -1; r <= 1; ++r) {
-      uint32_t omask = 0;
-      for (int j = j0; j < min(n + 2, j0 + RING_JB); ++j)
-        if (!inside_img(oy + r * ay + (j - 1) * ly, ox + r * ax + (j - 1) * lx, H, W)) omask |= 1u << (j - j0);
-      if (omask == 0) continue;
-      float acc[RING_JB];
+    // own sides: thread = (K quarter kq, pixels [4 pg, 4 pg + 4), channels [4 cg, 4 cg + 4)), K = 5 taps x 256 in
+    // order.  The L2 latency of the weight loads bounds the kernel, so segments are short and K is split four ways:
+    // more blocks in flight, each with a shorter serial K loop (32-pixel segments and K halves took 1.5x as long)
+    {
+      const int kq = t >> 6, cg = t & 15, pg = (t >> 4) & 3;
+      float acc[4][4];
 #pragma unroll
-      for (int j = 0; j < RING_JB; ++j) acc[j] = 0.f;
-      for (int tp = 0; tp < 9; ++tp) {
-        const int rr = tp / 3 - 1, cc = tp % 3 - 1;  // box offset (across, along)
-        uint32_t vmask = 0;
-        for (int j = 0; j < RING_JB; ++j) {
-          const int jb = j0 + j;
-          if (((omask >> j) & 1u) && inside_img(oy + (r + rr) * ay + (jb - 1 + cc) * ly, ox + (r + rr) * ax + (jb - 1 + cc) * lx, H, W))
-            vmask |= 1u << j;
-        }
-        if (vmask == 0) continue;
-        const int dy = rr * ay + cc * ly, dx = rr * ax + cc * lx;
-        const float* wt = p.wb + static_cast<size_t>((dy + 1) * 3 + (dx + 1)) * 65536 + cm;
-        const float* arow = abox + ((r + rr + 2) * RING_ABOX + j0 + cc + 1) * 256;  // box column of j = j0
-#pragma unroll 4
-        for (int ci = 0; ci < 256; ci += 4) {
-          const float w0 = __ldg(wt + (ci + 0) * 256), w1 = __ldg(wt + (ci + 1) * 256);
-          const float w2 = __ldg(wt + (ci + 2) * 256), w3 = __ldg(wt + (ci + 3) * 256);
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
-          for (int j = 0; j < RING_JB; ++j)
-            if ((vmask >> j) & 1u) {
-              const float4 av = *reinterpret_cast<const float4*>(arow + j * 256 + ci);
-              acc[j] = fmaf(w3, av.w, fmaf(w2, av.z, fmaf(w1, av.y, fmaf(w0, av.x, acc[j]))));
-            }
+        for (int c = 0; c < 4; ++c) acc[i][c] = 0.f;
+      for (int s = s0; s < s0 + 2; ++s) {
+        if (!on_side(s, oy, ox, H, W)) continue;  // every pixel of a segment is on the same own sides
+        const float* E = p.edge + s * EDGE_E + 4 * cg;
+#pragma unroll 2
+        for (int kk = kq * RING_KQ; kk < (kq + 1) * RING_KQ; kk += 4) {
+          const int tap = kk >> 8, ci = kk & 255;
+          float4 w[4];
+#pragma unroll
+          for (int r = 0; r < 4; ++r) w[r] = __ldg(reinterpret_cast<const float4*>(E + (kk + r) * 64));
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float4 av = *reinterpret_cast<const float4*>(line + (4 * pg + i + tap) * 256 + ci);
+            acc[i][0] = fmaf(av.w, w[3].x, fmaf(av.z, w[2].x, fmaf(av.y, w[1].x, fmaf(av.x, w[0].x, acc[i][0]))));
+            acc[i][1] = fmaf(av.w, w[3].y, fmaf(av.z, w[2].y, fmaf(av.y, w[1].y, fmaf(av.x, w[0].y, acc[i][1]))));
+            acc[i][2] = fmaf(av.w, w[3].z, fmaf(av.z, w[2].z, fmaf(av.y, w[1].z, fmaf(av.x, w[0].z, acc[i][2]))));
+            acc[i][3] = fmaf(av.w, w[3].w, fmaf(av.z, w[2].w, fmaf(av.y, w[1].w, fmaf(av.x, w[0].w, acc[i][3]))));
+          }
         }
       }
-      const float bias = __ldg(p.bb + cm);
+      if (kq > 0)
 #pragma unroll
-      for (int j = 0; j < RING_JB; ++j)
-        if ((omask >> j) & 1u) bbox[((r + 1) * RING_BOX + j0 + j) * 256 + cm] = acc[j] + bias;
+        for (int i = 0; i < 4; ++i)
+          *reinterpret_cast<float4*>(part + ((kq - 1) * RING_S + 4 * pg + i) * 64 + 4 * cg) =
+              make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+      __syncthreads();
+      if (kq == 0) {
+        float c0[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int s = s0; s < s0 + 2; ++s)
+          if (on_side(s, oy, ox, H, W))
+#pragma unroll
+            for (int c = 0; c < 4; ++c) c0[c] += cst[s * 64 + 4 * cg + c];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          float v[4] = {acc[i][0], acc[i][1], acc[i][2], acc[i][3]};
+#pragma unroll
+          for (int q = 0; q < 3; ++q) {
+            const float4 h = *reinterpret_cast<const float4*>(part + (q * RING_S + 4 * pg + i) * 64 + 4 * cg);
+            v[0] += h.x;
+            v[1] += h.y;
+            v[2] += h.z;
+            v[3] += h.w;
+          }
+          *reinterpret_cast<float4*>(corr + (4 * pg + i) * 64 + 4 * cg) =
+              make_float4(v[0] + c0[0], v[1] + c0[1], v[2] + c0[2], v[3] + c0[3]);
+        }
+      }
     }
     __syncthreads();
-    // y(p) -= sum over pred.0 taps that land outside; thread = (output channel, every RING_THREADS / 64-th pixel)
-    const int co = t & 63;
-    for (int j = t >> 6; j < n; j += RING_THREADS / 64) {
+    // end pixels that also lie on a crossing side: its 5-tap conv across the segment's line, minus the corner terms;
+    // thread = (channel co, input-channel slice of 64), slices summed in order
+    for (int e = 0; e < 2; ++e) {
+      const int j = e == 0 ? (ly ? -oy : -ox) : (ly ? H - 1 - oy : W - 1 - ox);
+      if (j < 0 || j >= n || (e == 1 && j == (ly ? -oy : -ox))) continue;
       const int y = oy + j * ly, x = ox + j * lx;
-      float corr = 0.f;
-      for (int tp = 0; tp < 9; ++tp) {
-        const int rr = tp / 3 - 1, cc = tp % 3 - 1;
-        const int dy = rr * ay + cc * ly, dx = rr * ax + cc * lx;
-        if (inside_img(y + dy, x + dx, H, W)) continue;
-        const float* bq = bbox + ((rr + 1) * RING_BOX + j + cc + 1) * 256;
-        const float* wt = p.wp + static_cast<size_t>((dy + 1) * 3 + (dx + 1)) * 256 * 64 + co;
-        for (int c = 0; c < 256; c += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(bq + c);
-          corr = fmaf(__ldg(wt + (c + 0) * 64), b4.x, corr);
-          corr = fmaf(__ldg(wt + (c + 1) * 64), b4.y, corr);
-          corr = fmaf(__ldg(wt + (c + 2) * 64), b4.z, corr);
-          corr = fmaf(__ldg(wt + (c + 3) * 64), b4.w, corr);
+      const int co = t & 63, c0 = (t >> 6) * 64;
+      float v = 0.f, cv = 0.f;
+      for (int s = 2 - s0; s < 4 - s0; ++s) {
+        if (!on_side(s, y, x, H, W)) continue;
+        if (t < 64) cv += cst[s * 64 + co];
+        const int ay = s >= 2, ax = s < 2;  // direction of side s
+        for (int tap = 0; tap < 5; ++tap) {
+          const int yy = y + (tap - 2) * ay, xx = x + (tap - 2) * ax;
+          if (!inside_img(yy, xx, H, W)) continue;
+          const float* E = p.edge + s * EDGE_E + tap * 256 * 64 + co;
+          for (int ci = c0; ci < c0 + 64; ++ci) v = fmaf(a_at(yy, xx, ci), __ldg(E + ci * 64), v);
         }
       }
-      float* yp = p.y32 + ((static_cast<size_t>(img) * H + y) * W + x) * 64 + co;
-      const float v = *yp - corr;
+      for (int cn = 0; cn < 4; ++cn) {  // TL, TR, BL, BR
+        if (y != ((cn >> 1) ? H - 1 : 0) || x != ((cn & 1) ? W - 1 : 0)) continue;
+        if (t < 64) cv -= cst[(4 + cn) * 64 + co];
+        const float* C = p.edge + 4 * EDGE_E + cn * EDGE_C + co;
+        for (int ci = c0; ci < c0 + 64; ++ci) v = fmaf(-a_at(y, x, ci), __ldg(C + ci * 64), v);
+      }
+      xred[t] = v;
+      __syncthreads();
+      if (t < 64) corr[j * 64 + co] += xred[co] + xred[64 + co] + xred[128 + co] + xred[192 + co] + cv;
+      __syncthreads();
+    }
+    // y(p) -= corr(p)
+    for (int i = t; i < n * 64; i += RING_THREADS) {
+      const int j = i >> 6, co = i & 63;
+      float* yp = p.y32 + ((static_cast<size_t>(img) * H + oy + j * ly) * W + ox + j * lx) * 64 + co;
+      const float v = *yp - corr[i];
       *yp = v;
-      ycor[j * 64 + co] = v;
+      part[i] = v;
     }
     __syncthreads();
-    // GroupNorm sums: thread t < 256 takes every 4th pixel, in the same order whatever RING_THREADS is
-    if (t < 256)
+    // GroupNorm sums: thread t takes every 4th pixel of channel t % 64
+    {
+      const int co = t & 63;
       for (int j = t >> 6; j < n; j += 4) {
-        const double v = ycor[j * 64 + co];
+        const double v = part[j * 64 + co];
         ts += v;
         tq = fma(v, v, tq);
       }
+    }
   }
   // GroupNorm partials of this block's ring pixels, summed in a fixed order
-  if (t < 256) {
-    red[t] = ts;
-    red[256 + t] = tq;
-  }
+  red[t] = ts;
+  red[256 + t] = tq;
   __syncthreads();
   if (t < 8) {
     const int g = t >> 1, which = t & 1;
@@ -495,6 +546,45 @@ __global__ void compose_fold_kernel(const float* __restrict__ wp, const float* _
         for (int k = 0; k < 9; ++k) b += static_cast<double>(wp[(co * 256 + cm) * 9 + k]) * static_cast<double>(bb[cm]);
       b5[co] = static_cast<float>(b);
     }
+  }
+}
+// The ring correction's edge kernels, corners and constants (EDGE_ELEMS, ring_fix_kernel's layout) in fp64 from the
+// same weights, rounded once to fp32.  Side s pairs pred.0's outer tap row / column with convB's opposite one:
+// T = (ky 0, ey 2), B = (ky 2, ey 0), L = (kx 0, ex 2), R = (kx 2, ex 0); tap D + 2 = k + e along the side.  Corner
+// (dy, dx) pairs Wp0[d] with WB[-d].
+__global__ void compose_edge_kernel(const float* __restrict__ wp, const float* __restrict__ wb,
+                                    const float* __restrict__ bb, float* __restrict__ edge) {
+  auto P = [&](int co, int cm, int ky, int kx) { return static_cast<double>(wp[((co * 256 + cm) * 3 + ky) * 3 + kx]); };
+  auto Q = [&](int cm, int ci, int ey, int ex) { return static_cast<double>(wb[((cm * 256 + ci) * 3 + ey) * 3 + ex]); };
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < EDGE_ELEMS; i += gridDim.x * blockDim.x) {
+    const int co = i & 63;
+    double s = 0.0;
+    if (i < 4 * EDGE_E) {
+      const int ci = (i >> 6) & 255, tap = (i >> 14) % 5, side = i / EDGE_E;
+      const int o = (side & 1) ? 2 : 0;  // pred.0's outer row / column; convB's is 2 - o
+      for (int cm = 0; cm < 256; ++cm)
+        for (int k = 0; k < 3; ++k) {
+          const int e = tap - k;
+          if (e < 0 || e > 2) continue;
+          s += side < 2 ? P(co, cm, o, k) * Q(cm, ci, 2 - o, e) : P(co, cm, k, o) * Q(cm, ci, e, 2 - o);
+        }
+    } else if (i < 4 * EDGE_E + 4 * EDGE_C) {
+      const int j = i - 4 * EDGE_E, ci = (j >> 6) & 255, cn = j / EDGE_C;
+      const int ky = (cn >> 1) * 2, kx = (cn & 1) * 2;
+      for (int cm = 0; cm < 256; ++cm) s += P(co, cm, ky, kx) * Q(cm, ci, 2 - ky, 2 - kx);
+    } else {
+      const int c = (i - 4 * EDGE_E - 4 * EDGE_C) >> 6;  // sides T, B, L, R, then corners TL, TR, BL, BR
+      for (int cm = 0; cm < 256; ++cm) {
+        const double b = bb[cm];
+        if (c < 4) {
+          const int o = (c & 1) ? 2 : 0;
+          for (int k = 0; k < 3; ++k) s += (c < 2 ? P(co, cm, o, k) : P(co, cm, k, o)) * b;
+        } else {
+          s += P(co, cm, ((c - 4) >> 1) * 2, ((c - 4) & 1) * 2) * b;
+        }
+      }
+    }
+    edge[i] = static_cast<float>(s);
   }
 }
 // K5 * scale -> fp16 hi / lo in conv5x5_fold_kernel's packed order
