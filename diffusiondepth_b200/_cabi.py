@@ -88,6 +88,8 @@ SIGNATURES = {
     "dd_decode_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
                                      C.c_void_p, C.c_size_t, C.c_void_p]),
     "dd_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "dd_encode_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p),
+                                     C.c_void_p, C.c_size_t, C.c_void_p]),
     "dd_set_codec_mode": (C.c_int, [C.c_void_p, C.c_int32]),
     "dd_codec_batch_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
     "dd_set_producer_mode": (C.c_int, [C.c_void_p, C.c_int32]),

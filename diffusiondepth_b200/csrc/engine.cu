@@ -292,6 +292,7 @@ struct PackStage {
   float wt_f[4 * 4 * 16 * 16], bt_f[16], wc_f[9 * 16], wu[4 * 4 * 16 * 16], bn[3 * 16];
   float f1[144], t1[16], f2[2304], t2[16];
   float e1u[144], e2u[2304], enc_gb[4][16];  // unfolded encoder for DD_CODEC_TRAIN: [tap][co], [tap][ci][co]; gamma / beta
+  float enc_bn[2][3][16];                     // the encoder backward's running-statistics BatchNorms: s, mean, rstd
 };
 
 struct Raw {
@@ -463,6 +464,7 @@ struct dd_engine {
   float* dec_bu = nullptr;  // [16] unfolded ConvT bias
   float* dec_bn = nullptr;  // [3][16] BatchNorm scale gamma * rstd, running mean, rstd
   float *enc_w1 = nullptr, *enc_b1 = nullptr, *enc_w2 = nullptr, *enc_b2 = nullptr;  // folded encoder (optional)
+  float* enc_bn = nullptr;  // [2][3][16] encoder BatchNorms 1, 2 on running statistics: s = gamma rstd, mean, rstd
   // DD_CODEC_TRAIN (dd_set_codec_mode): the codec's BatchNorms on batch statistics.  The unfolded parameters (filled
   // with the pack), the batch-folded copies decoder_kernel / encoder_kernel run on, and the statistics' scratch; all
   // engine-owned, so the workspace size does not depend on the mode.
@@ -473,6 +475,7 @@ struct dd_engine {
     float* zero16 = nullptr;  // [16] zeros: the ConvT bias of the decoder backward's xhat (bn's mean is bias-free)
     float *enc_w1 = nullptr, *enc_w2 = nullptr, *enc_gb = nullptr;  // unfolded encoder; [4][16] gamma1, beta1, gamma2, beta2
     float *enc_w1f = nullptr, *enc_b1f = nullptr, *enc_w2f = nullptr, *enc_b2f = nullptr;  // batch-folded encoder
+    float* enc_bn = nullptr;  // [2][3][16] the encoder backward's batch s, mean, rstd (layout of dd_engine::enc_bn)
     double *part = nullptr, *sum1 = nullptr;     // bn_stats_kernel partials [blocks][2][16]; pass-1 sums [16]
     double *sums = nullptr, *part_db = nullptr;  // decoder backward: [32] sum dv, sum dv xhat; [act blocks][16]
     float* rec = nullptr;                        // [max(T, 2)][2][16] batch mean, unbiased variance
@@ -1439,6 +1442,8 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
     if ((rc = dev_array(h, &h->enc_b1, 16))) return rc;
     if ((rc = dev_array(h, &h->enc_w2, 2304))) return rc;
     if ((rc = dev_array(h, &h->enc_b2, 16))) return rc;
+    if ((rc = dev_array(h, &h->enc_bn, 2 * 3 * 16))) return rc;
+    if ((rc = dev_array(h, &ct.enc_bn, 2 * 3 * 16))) return rc;
     if ((rc = dev_array(h, &ct.enc_w1, 144))) return rc;
     if ((rc = dev_array(h, &ct.enc_w2, 2304))) return rc;
     if ((rc = dev_array(h, &ct.enc_gb, 4 * 16))) return rc;
@@ -1633,10 +1638,18 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
       sg->enc_gb[1][co] = sg->enc_bn1[1][co];
       sg->enc_gb[2][co] = sg->enc_bn2[0][co];
       sg->enc_gb[3][co] = sg->enc_bn2[1][co];
+      for (int k = 0; k < 2; ++k) {  // the backward's eval BatchNorms, as dec_bn
+        const float(*bn)[16] = k == 0 ? sg->enc_bn1 : sg->enc_bn2;  // weight, bias, running_mean, running_var
+        const double rstd = 1.0 / sqrt(static_cast<double>(bn[3][co]) + 1e-5);
+        sg->enc_bn[k][0][co] = static_cast<float>(static_cast<double>(bn[0][co]) * rstd);
+        sg->enc_bn[k][1][co] = bn[2][co];
+        sg->enc_bn[k][2][co] = static_cast<float>(rstd);
+      }
     }
     CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w1, sg->e1u, sizeof(sg->e1u), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w2, sg->e2u, sizeof(sg->e2u), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(h->ct.enc_gb, sg->enc_gb, sizeof(sg->enc_gb), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(h->enc_bn, sg->enc_bn, sizeof(sg->enc_bn), cudaMemcpyHostToDevice, st));
   }
   CUDA_TRY(cudaEventRecord(h->pack_done, st));
   if (loop_stale) drop_graph(h, dd_engine::G_LOOP);
@@ -3695,6 +3708,102 @@ int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, fl
   dim3 grid((a.w + 15) / 16, (a.h + 15) / 16, h->cfg.batch);
   dd::encoder_kernel<<<grid, 256, 0, st>>>(a);
   return check_launch("encoder");
+}
+
+// The encoder backward's weight partials fit the smallest wgrad partials region: one chunk of a 256 -> 256 conv.
+static_assert(dd::ENC_WG_BLOCKS * dd::ENC_WG_COLS <= 256 * 256 * 9, "encoder weight partials exceed bw.wg_part");
+
+// Reverse mode of dd_encode in the current codec mode: d_latent NCHW [B][16][h][w] -> the six encoder gradients
+// dp[0..5] (each nullable), in ENCODER_KEYS order without the running statistics.  Its planes and partials live in the
+// operator backward's region (bw.g[0], bw.g[1], bw.wg_part), which no other call uses while this one runs.
+int run_encode_bwd(dd_engine* e, const float* depth, int H, int W, const float* d_latent, float* const* dp, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  const long long N = static_cast<long long>(g.B) * g.P;
+  const bool train = e->codec_mode == DD_CODEC_TRAIN;
+  dd_engine::CodecTrain& ct = e->ct;
+  int rc;
+  if (train) {  // dd_encode's two batch statistics, the same kernels in the same order; no record
+    const dd::EncPreBn1 op1{depth, ct.enc_w1, H, W, g.h, g.w};
+    if ((rc = run_codec_bn(e, op1, N, ct.enc_gb, nullptr, ct.enc_w1, 144, ct.enc_w1f, ct.enc_b1f, ct.enc_bn, nullptr, st)))
+      return rc;
+    const dd::EncPreBn2 op2{depth, ct.enc_w1f, ct.enc_b1f, ct.enc_w2, H, W, g.h, g.w};
+    if ((rc = run_codec_bn(e, op2, N, ct.enc_gb + 32, nullptr, ct.enc_w2, 2304, ct.enc_w2f, ct.enc_b2f, ct.enc_bn + 48,
+                           nullptr, st)))
+      return rc;
+  }
+  const float* bn = train ? ct.enc_bn : e->enc_bn;
+  const size_t plane = static_cast<size_t>(N) * 16;
+  const int nb_pix = static_cast<int>((N + dd::ENC_PIX - 1) / dd::ENC_PIX);
+  const int nb_w = static_cast<int>(std::min<long long>(dd::ENC_WG_BLOCKS, (N + 1023) / 1024));
+  const int per_block = static_cast<int>((N + nb_w - 1) / nb_w);
+  dd::EncBwdArgs a;
+  a.depth = depth;
+  a.w1f = train ? ct.enc_w1f : e->enc_w1;
+  a.b1f = train ? ct.enc_b1f : e->enc_b1;
+  a.w2f = train ? ct.enc_w2f : e->enc_w2;
+  a.b2f = train ? ct.enc_b2f : e->enc_b2;
+  a.w1u = ct.enc_w1;
+  a.w2u = ct.enc_w2;
+  a.bn1 = bn;
+  a.bn2 = bn + 48;
+  a.dlat = d_latent;
+  a.a1 = e->bw.g[0];
+  a.x1 = e->bw.g[0] + plane;
+  a.x2 = e->bw.g[0] + 2 * plane;
+  a.dz = e->bw.g[0] + 3 * plane;
+  a.part2 = reinterpret_cast<double*>(e->bw.g[1]);
+  a.part1 = a.part2 + static_cast<size_t>(nb_pix) * 32;
+  a.part_w = e->bw.wg_part;
+  a.B = g.B;
+  a.H = H;
+  a.W = W;
+  a.h = g.h;
+  a.w = g.w;
+  dd::enc_bwd_mid_kernel<<<nb_pix, 256, 0, st>>>(a);
+  if ((rc = launched(e, "enc_bwd_mid"))) return rc;
+  dd::enc_bwd_out_kernel<<<nb_pix, 256, 0, st>>>(a);
+  if ((rc = launched(e, "enc_bwd_out"))) return rc;
+  // each BatchNorm's du through its statistics (training mode: the two backward sums, across ranks the union batch's)
+  auto bn_bwd = [&](float* d, const float* xhat, const float* bnk, const double* part) -> int {
+    BnTotals t{nullptr, nullptr};
+    int r;
+    if (train && (r = bn_totals(e, part, nb_pix, 32, 32, N, ct.sums, 33, st, &t))) return r;
+    dd::enc_bwd_bn_kernel<<<grid_of(plane), 256, 0, st>>>(d, xhat, bnk, t.sum, t.cnt, N);
+    return launched(e, "enc_bwd_bn");
+  };
+  if ((rc = bn_bwd(a.dz, a.x2, a.bn2, a.part2))) return rc;
+  dd::enc_bwd_mid_grad_kernel<<<nb_pix, 256, 0, st>>>(a);
+  if ((rc = launched(e, "enc_bwd_mid_grad"))) return rc;
+  if ((rc = bn_bwd(a.x2, a.x1, a.bn1, a.part1))) return rc;
+  dd::enc_bwd_wgrad_kernel<<<nb_w, 160, 0, st>>>(a, per_block);
+  if ((rc = launched(e, "enc_bwd_wgrad"))) return rc;
+  dd::EncFinishArgs f;
+  f.part1 = a.part1;
+  f.part2 = a.part2;
+  f.part_w = a.part_w;
+  f.nb_pix = nb_pix;
+  f.nb_w = nb_w;
+  for (int i = 0; i < 6; ++i) f.out[i] = dp[i];
+  dd::enc_bwd_finish_kernel<<<(dd::ENC_GRAD_N + 255) / 256, 256, 0, st>>>(f);
+  return launched(e, "enc_bwd_finish");
+}
+
+int dd_encode_backward(dd_handle h, const float* depth, int32_t height, int32_t width, const float* d_latent,
+                       float* const* d_enc_params, void* workspace, size_t workspace_bytes, void* cuda_stream) {
+  if (!h || !depth || !d_latent) return fail(DD_ERR_INVALID, "null argument");
+  int rc;
+  if ((rc = check_operator_bwd_call(h, "dd_encode_backward"))) return rc;
+  if (!h->enc_w1) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
+  if ((height + 1) / 2 != h->cfg.latent_h || (width + 1) / 2 != h->cfg.latent_w)
+    return fail(DD_ERR_INVALID, "depth map size does not match the engine's latent grid");
+  if (h->codec_mode == DD_CODEC_TRAIN && static_cast<long long>(h->cfg.batch) * h->cfg.latent_h * h->cfg.latent_w < 2)
+    return fail(DD_ERR_INVALID, "training-mode BatchNorm needs more than 1 value per channel (batch x latent = 1)");
+  if (static_cast<long long>(h->cfg.batch) * height * width > static_cast<long long>(INT32_MAX))
+    return fail(DD_ERR_UNSUPPORTED, "depth map too large for one encoder backward call");
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
+  float* none[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  return run_encode_bwd(h, depth, height, width, d_latent, d_enc_params ? d_enc_params : none,
+                        static_cast<cudaStream_t>(cuda_stream));
 }
 
 int64_t dd_last_launch_count(dd_handle h) { return h ? h->launches : 0; }

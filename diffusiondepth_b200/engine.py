@@ -24,6 +24,10 @@ ENCODER_KEYS = (
     "depth_transform.conv_transform.0.1.running_var", "depth_transform.conv_transform.1.0.weight",
     "depth_transform.conv_transform.1.1.weight", "depth_transform.conv_transform.1.1.bias",
     "depth_transform.conv_transform.1.1.running_mean", "depth_transform.conv_transform.1.1.running_var")
+# the encoder's parameters (ENCODER_KEYS without the running statistics): the order of dd_encode_backward's d_enc_params
+ENCODER_PARAM_KEYS = tuple(k for k in ENCODER_KEYS if "running" not in k)
+_ENCODER_SHAPES = {"depth_transform.conv_transform.0.0.weight": (16, 1, 3, 3),
+                   "depth_transform.conv_transform.1.0.weight": (16, 16, 3, 3)}
 # shapes of the denoiser's parameters (reference ScheduledCNNRefine, head :336-359) in DENOISER_KEYS + FUSE_KEYS order
 _PARAM_SHAPES = {
     "model.noise_embedding.0.weight": (64, 16, 3, 3), "model.noise_embedding.0.bias": (64,),
@@ -433,6 +437,22 @@ class DenoiseEngine:
         out = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32)
         _cabi.check(self.lib.dd_encode(self._h, _ptr(depth), H, W, _ptr(out), C.c_void_p(self._stream())))
         return out
+
+    def encode_backward(self, depth: torch.Tensor, d_latent: torch.Tensor, want_params=True) -> Dict[str, torch.Tensor]:
+        """Gradients of latent = encode(depth) given d_latent [B,16,h,w], in the current codec mode (engine created with
+        backward=True or loop_backward=True): {encoder key relative to `depth_head.`: gradient} (ENCODER_PARAM_KEYS;
+        empty without `want_params`).  In training mode it differentiates through the batch statistics and records
+        nothing: `codec_batch_stats` still reports the last forward.  No gradient with respect to depth."""
+        if not self.backward:
+            raise EngineError("engine was created without backward=True or loop_backward=True")
+        B, (h, w) = self.batch, self.latent_hw
+        H, W = depth.shape[-2:]
+        self._check_in(depth, (B, 1, H, W))
+        self._check_in(d_latent, (B, 16, h, w))
+        grads, ptrs = self._grad_buffers(ENCODER_PARAM_KEYS if want_params else (), _ENCODER_SHAPES, (16,))
+        _cabi.check(self.lib.dd_encode_backward(self._h, _ptr(depth), H, W, _ptr(d_latent),
+                                                ptrs if want_params else None, *self._ws_args()))
+        return grads
 
     def set_codec_mode(self, training: bool):
         """The depth codec's BatchNorms on batch statistics (`training`, as torch's BatchNorm2d in training mode) or on

@@ -22,8 +22,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from diffusiondepth_b200._cabi import EngineError
-from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS, FUSE_KEYS,
-                                        DenoiseEngine, WorkspacePool, is_updatable)
+from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS,
+                                        ENCODER_PARAM_KEYS, FUSE_KEYS, DenoiseEngine, WorkspacePool, is_updatable)
 from .._blocks import ConvModule, DropPath, MMCVDropPath, exact_fp32
 from ..diffusers.schedulers.scheduling_ddim import DDIMScheduler
 from ..ops import depth_transform as _codec  # noqa: F401  (registers the codec classes)
@@ -205,6 +205,29 @@ class _LoopFunction(torch.autograd.Function):
         return (None,) * 6 + (d_cond, d_noise) + tuple(grads[k] if need[8 + i] else None for i, k in enumerate(ctx.keys))
 
 
+class _EncodeFunction(torch.autograd.Function):
+    """gt_map_t = depth_transform.t(depth) as an autograd node over (depth, *encoder parameters).  The forward is the
+    head's plain `encode` call on `eng`, in the codec mode the caller set (gt_map_t bit-identical to the no-grad path),
+    and keeps depth and that mode; the backward runs `dd_encode_backward` in the same mode on the engine the denoiser
+    backward runs on, which recomputes the forward from depth.  Ground truth gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, head, eng, keys, codec_train, depth, *params):
+        latent = eng.encode(depth)
+        ctx.save_for_backward(depth)
+        ctx.head, ctx.keys, ctx.codec_train, ctx.cond_hw = head, keys, codec_train, eng.cond_hw
+        return latent
+
+    @staticmethod
+    def backward(ctx, d_latent):
+        depth, = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        eng = ctx.head._grad_engine(depth.shape[0], d_latent.shape[-2:], ctx.cond_hw, depth.device)
+        eng.set_codec_mode(ctx.codec_train)  # differentiate the encoder the forward ran
+        grads = eng.encode_backward(depth, d_latent.contiguous().float(), want_params=any(need[5:]))
+        return (None,) * 5 + tuple(grads[k] if need[5 + i] else None for i, k in enumerate(ctx.keys))
+
+
 def bn_running_update(bn: nn.BatchNorm2d, mean: torch.Tensor, var: torch.Tensor):
     """The running-statistic update torch's training-mode BatchNorm (F.batch_norm) makes after one batch with mean `mean`
     and UNBIASED variance `var`: num_batches_tracked += 1, then running = (1 - f) running + f batch with f = momentum,
@@ -231,6 +254,12 @@ class DDIMHeadBase(nn.Module):
     # decoder (native dd_denoise_backward), so the L1 / L2 depth losses train the head and `ddim_loss` also reaches the
     # loop through its re-noised latent.  Off by default: it changes what `ddim_loss.backward()` costs and computes.
     grad_through_loop = False
+    # Training the depth encoder through `gt_map_t`: when True, grad is enabled and an encoder parameter
+    # (`depth_transform.conv_transform.*`) requires grad, `gt_map_t` (= `pred_init` = `blur_depth_t`) is the engine's
+    # encoding as an autograd node (native dd_encode_backward, in the codec's BatchNorm mode), so `ddim_loss_gt` trains
+    # the encoder as well as the denoiser.  Without native producers the engine then encodes too, instead of torch's
+    # `t()` under no_grad.  Off by default: `gt_map_t` then carries no gradient.
+    grad_through_encoder = False
     # Training-mode BatchNorm in the depth codec (reference `net.train()`): when True and `depth_transform.training`, the
     # engine's encoder and decoder normalise with the statistics of the batch they see, the decoder's gradients flow
     # through those statistics, and every forward applies torch's running-statistic update to the codec's BatchNorm
@@ -798,9 +827,15 @@ class DDIMHeadBase(nn.Module):
         Hd, Wd = gt_depth_map.shape[-2:]
         latent_hw = ((Hd + 1) // 2, (Wd + 1) // 2)  # shape of depth_transform.t(gt): conv3x3 stride 2 pad 1
         gt_map_t = None
+        enc_grad = None  # (keys, parameters) when gt_map_t is differentiable
+        if self.grad_through_encoder and torch.is_grad_enabled():
+            enc_grad = self._encoder_params()
+            if not any(p.requires_grad for p in enc_grad[1]):
+                enc_grad = None
         if not native:
             with torch.no_grad(), exact_fp32():
-                gt_map_t = self.depth_transform.t(gt_depth_map)
+                if enc_grad is None:
+                    gt_map_t = self.depth_transform.t(gt_depth_map)
                 cond = self._condition(self._neck(fp)).contiguous()
         else:
             cond = None
@@ -833,13 +868,16 @@ class DDIMHeadBase(nn.Module):
                 cond = eng.build_condition(fp, want_cond=want_cond)
             if ptrain:
                 bn_updates += self._producer_records(eng, bb_mod)
-            eng.set_codec_mode(codec_train)
-            gt_map_t = eng.encode(gt_depth_map.contiguous().float())  # returned as pred_init / gt_map_t only
+            gt_map_t = self._encode(eng, gt_depth_map, codec_train, enc_grad)  # returned as pred_init / gt_map_t only
             if codec_train:
                 bn_updates += self._codec_records(eng, (enc_bn1, enc_bn2))
             loop_cond = None
         else:
             eng = self._engine(B, latent_hw, tuple(cond.shape[-2:]), dev)
+            if enc_grad is not None:
+                gt_map_t = self._encode(eng, gt_depth_map, codec_train, enc_grad)
+                if codec_train:
+                    bn_updates += self._codec_records(eng, (enc_bn1, enc_bn2))
             loop_cond = cond
         inter = None
         loop_keys, loop_params = None, None
@@ -878,6 +916,33 @@ class DDIMHeadBase(nn.Module):
         return {'pred': refined_depth, 'pred_init': gt_map_t, 'blur_depth_t': gt_map_t, 'ddim_loss': ddim_loss,
                 'gt_map_t': gt_map_t, 'pred_uncertainty': None, 'pred_inter': inter, 'weight_map': None,
                 'guidance': None, 'offset': None, 'aff': None, 'gamma': None, 'confidence': None}
+
+    def _encoder_params(self):
+        """The encoder's parameters in ENCODER_PARAM_KEYS order: the order of dd_encode_backward's gradients."""
+        return ENCODER_PARAM_KEYS, [self.get_submodule(k.rpartition(".")[0]).get_parameter(k.rpartition(".")[2])
+                                    for k in ENCODER_PARAM_KEYS]
+
+    def _encode(self, eng, gt_depth_map, codec_train, enc_grad):
+        """depth_transform.t(gt_depth_map) on `eng` in the codec mode `codec_train`; through `_EncodeFunction` when
+        `enc_grad` = (keys, parameters) is given."""
+        eng.set_codec_mode(codec_train)
+        depth = gt_depth_map.contiguous().float()
+        if enc_grad is None:
+            return eng.encode(depth)
+        return _EncodeFunction.apply(self, eng, enc_grad[0], codec_train, depth, *enc_grad[1])
+
+    def ddim_loss_gt(self, gt_depth, refine_module_inputs, blur_depth_t, weight, **kwargs):
+        """Reference head :225-240: the diffusion objective on the encoded ground truth `gt_depth` (the forward's
+        `gt_map_t`), re-noised at a random timestep per image; `self.model(noisy, t, *refine_module_inputs)` must
+        predict the noise.  Random draws in the reference's order: the noise on the CPU, then the timesteps on the
+        device.  `blur_depth_t` and `weight` are unused, as in the reference.  The denoiser's parameters (and `cond`,
+        when it requires grad) are trained through `_DenoiserFunction`; with `grad_through_encoder` the encoder too,
+        through `gt_depth`."""
+        noise = torch.randn(gt_depth.shape).to(gt_depth.device)
+        timesteps = torch.randint(0, self.scheduler.num_train_timesteps, (gt_depth.shape[0],),
+                                  device=gt_depth.device).long()
+        noisy = self.scheduler.add_noise(gt_depth, noise, timesteps)
+        return F.mse_loss(self.model(noisy, timesteps, *refine_module_inputs), noise)
 
     def _ddim_loss(self, cond, latent):
         """Reference head :207-223 — one extra denoiser call on a re-noised latent; RNG-dependent."""

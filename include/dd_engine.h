@@ -34,6 +34,8 @@
  *   dd_decode                     <- `depth_transform.inv_t(latent)` alone (the *Vis heads call it
  *                                    per step, ..._swin_addHAHI_vis.py)
  *   dd_decode_backward            <- reverse-mode differentiation of `inv_t` (eval BatchNorm)
+ *   dd_encode_backward            <- reverse-mode differentiation of `t` with respect to the encoder's parameters
+ *                                    (the heads' `ddim_loss_gt`, head :225-240, trains the encoder through `gt_map_t`)
  *
  * Conventions (inherited from the reference, SURVEY.md §8b): every tensor is fp32, NCHW, contiguous,
  * resident on the engine's CUDA device; no autograd.  Ownership: the caller (PyTorch's allocator)
@@ -317,13 +319,25 @@ int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, f
  * latent_out [B,16,ceil(height/2),ceil(width/2)].  Needs the optional keys `depth_transform.conv_transform.*`. */
 int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, void* cuda_stream);
 
+/* Backward of dd_encode in the current codec mode: d_latent [B,16,ceil(height/2),ceil(width/2)] -> d_enc_params[0..5]
+ * = the gradients of conv_transform.0.0.weight [16,1,3,3], .0.1.weight, .0.1.bias, .1.0.weight [16,16,3,3],
+ * .1.1.weight, .1.1.bias (the array and every entry nullable).  It recomputes the forward from depth; in DD_CODEC_TRAIN
+ * it recomputes the two batch statistics as dd_encode does (bit-identical) and differentiates through them, across
+ * ranks with each BatchNorm's backward sums gathered once.  It records nothing (dd_codec_batch_stats still reports the
+ * last forward).  No gradient with respect to depth.  Bit-identical run to run; no synchronisation.  Its scratch
+ * aliases the operator backward's region of the workspace.  DD_ERR_INVALID without DD_FLAG_BACKWARD or
+ * DD_FLAG_LOOP_BACKWARD, before dd_finalize_weights, without encoder weights, for a size that does not match the
+ * latent grid, for a NULL depth or d_latent, and in DD_CODEC_TRAIN when batch x latent is 1. */
+int dd_encode_backward(dd_handle h, const float* depth, int32_t height, int32_t width, const float* d_latent,
+                       float* const* d_enc_params, void* workspace, size_t workspace_bytes, void* cuda_stream);
+
 /* How the depth codec's BatchNorms normalise.  DD_CODEC_EVAL (the default): running statistics, folded into the
  * weights at dd_finalize_weights.  DD_CODEC_TRAIN: as BatchNorm2d in training mode, the statistics of the batch
  * each call sees (biased variance, eps 1e-5), computed and folded on the device without synchronising:
  *   dd_decode, dd_denoise_decode           one batch-statistics decode                      (1 record)
  *   dd_denoise_decode_steps                one per step, inside a CUDA graph of its own      (T records)
  *   dd_encode                              both BatchNorms, the second after the first       (2 records)
- *   dd_decode_backward, dd_denoise_backward  differentiate through the batch mean and variance
+ *   dd_decode_backward, dd_denoise_backward, dd_encode_backward  differentiate through the batch mean and variance
  * The backward's recompute and the steps variant's extra logit decode record nothing.  The engine never writes running
  * statistics: the caller applies the running update from the records and registers the new buffers with
  * dd_update_weights.  In DD_CODEC_TRAIN dd_encode returns DD_ERR_INVALID when batch x latent is 1 (one value per
