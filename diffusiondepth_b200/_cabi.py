@@ -47,6 +47,9 @@ FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NAR
 FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD, FLAG_LOOP_BACKWARD = 64, 128, 256, 512
 FLAG_CHAIN_PRED, FLAG_PRODUCER_TRAIN = 1024, 2048
 CODEC_EVAL, CODEC_TRAIN = 0, 1
+# dd_codec_kind, carried in the flags at FLAG_CODEC_SHIFT
+CODEC_UP2, CODEC_UP2_1X1, CODEC_UP4, CODEC_FULL = 0, 1, 2, 3
+FLAG_CODEC_SHIFT = 12
 PRODUCER_EVAL, PRODUCER_TRAIN = 0, 1
 STATUS = {0: "DD_OK", 1: "DD_ERR_INVALID", 2: "DD_ERR_CUDA", 3: "DD_ERR_UNSUPPORTED", 4: "DD_ERR_RANGE"}
 # dd_allgather_fn: (in, out, count, cuda_stream, user) -> 0 on success
@@ -133,6 +136,8 @@ SIGNATURES = {
                                 C.c_size_t, C.c_void_p]),
     "dd_bench_pred_fold": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float), C.c_void_p, C.c_size_t,
                                      C.c_void_p]),
+    "dd_bench_decoder": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_float), C.c_void_p, C.c_size_t,
+                                   C.c_void_p]),
 }
 
 

@@ -23,6 +23,7 @@
 #include "backward.cuh"
 #include "codec_train.cuh"
 #include "producer_train.cuh"
+#include "codec_kinds.cuh"
 
 namespace {
 
@@ -252,6 +253,14 @@ cudaError_t configure_all_kernels() {
                                 dd::WAU_SMEM)) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(dd::decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::DEC_SMEM)) != cudaSuccess)
     return e;
+  if ((e = cudaFuncSetAttribute(dd::encoder_x4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::E4_SMEM)) !=
+      cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::encoder_full_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::EF_SMEM)) !=
+      cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::decoder_x4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::D4_SMEM)) !=
+      cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(dd::decoder_full_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dd::DF_SMEM)) !=
+      cudaSuccess) return e;
   if ((e = configure_halo_all_epi<16, 64, 16>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<64, 256, 32>()) != cudaSuccess) return e;
   if ((e = configure_halo_all_epi<256, 256, 32>()) != cudaSuccess) return e;
@@ -280,6 +289,10 @@ struct ConvLayer {
   CUtensorMap mh_hi, mh_lo;  // box for the halo kernel's K chunk
 };
 
+// PackStage::xraw: the codec kinds' registered tensors, the encoder's from 0, the decoder's from kXDecRaw (largest:
+// the UP4 encoder, 3 conv_bn_relu = 4944 floats, and the UP4 decoder, 2 ConvT + BatchNorm + final conv = 8433 floats;
+// kind_keys_fit checks every table against these bounds).
+constexpr size_t kXDecRaw = 8192, kXRawFloats = kXDecRaw + 12288;
 // Pinned host side of the denoiser / codec pack, so that its copies are asynchronous and one synchronisation serves a
 // whole pack: the abs-max words of the conv weights, the decoder's and encoder's raw tensors as last registered (an
 // update re-reads only the registered ones; the BatchNorm folds need all of them), and what the host folds produce.
@@ -293,6 +306,10 @@ struct PackStage {
   float f1[144], t1[16], f2[2304], t2[16];
   float e1u[144], e2u[2304], enc_gb[4][16];  // unfolded encoder for DD_CODEC_TRAIN: [tap][co], [tap][ci][co]; gamma / beta
   float enc_bn[2][3][16];                     // the encoder backward's running-statistics BatchNorms: s, mean, rstd
+  // codec kinds other than DD_CODEC_UP2 (codec_kinds.cuh): their registered tensors at kind_keys' offsets, and the
+  // folded parameter blocks of their kernels (encoder, decoder)
+  float xraw[kXRawFloats];
+  float xenc[dd::CK_E4_N], xdec[dd::CK_D4_N];
 };
 
 struct Raw {
@@ -465,6 +482,7 @@ struct dd_engine {
   float* dec_bn = nullptr;  // [3][16] BatchNorm scale gamma * rstd, running mean, rstd
   float *enc_w1 = nullptr, *enc_b1 = nullptr, *enc_w2 = nullptr, *enc_b2 = nullptr;  // folded encoder (optional)
   float* enc_bn = nullptr;  // [2][3][16] encoder BatchNorms 1, 2 on running statistics: s = gamma rstd, mean, rstd
+  float *xenc = nullptr, *xdec = nullptr;  // codec kinds 1..3: folded encoder (optional) / decoder (UP4, FULL) blocks
   // DD_CODEC_TRAIN (dd_set_codec_mode): the codec's BatchNorms on batch statistics.  The unfolded parameters (filled
   // with the pack), the batch-folded copies decoder_kernel / encoder_kernel run on, and the statistics' scratch; all
   // engine-owned, so the workspace size does not depend on the mode.
@@ -648,6 +666,27 @@ size_t wgrad_partial_elems(int cout, int cin, int B, int H, int W) {
                                             : wgrad_plan(cout, cin, static_cast<long long>(B) * H * W).chunks;
   return static_cast<size_t>(chunks) * cout * cin * 9;
 }
+// The depth codec (dd_codec_kind in the flags) and the upsampling u of its decoder: the decoded map is u h x u w.
+int codec_kind(const dd_config& c) { return (c.flags >> DD_FLAG_CODEC_SHIFT) & 3; }
+int codec_up(const dd_config& c) {
+  static const int u[4] = {2, 2, 4, 1};
+  return u[codec_kind(c)];
+}
+const char* codec_name(int kind) {
+  static const char* const n[4] = {"DeepDepthTransformWithUpsampling", "DeepDepthTransformWithUpsampling1x1",
+                                   "DeepDepthTransformWithUpsamplingX4", "DeepDepthTransform"};
+  return n[kind];
+}
+// One side of the latent grid for a depth map side n: ceil(n / 2) (one stride-2 conv or pool), ceil(ceil(n / 2) / 2)
+// (two), n (none).
+int codec_latent(int kind, int n) {
+  return kind == DD_CODEC_UP4 ? ((n + 1) / 2 + 1) / 2 : kind == DD_CODEC_FULL ? n : (n + 1) / 2;
+}
+// elements of one decoded batch [B][u h][u w]
+size_t codec_map_elems(const dd_config& c) {
+  const size_t u = static_cast<size_t>(codec_up(c));
+  return static_cast<size_t>(c.batch) * (u * c.latent_h) * (u * c.latent_w);
+}
 // DD_FLAG_LOOP_BACKWARD implies DD_FLAG_BACKWARD
 bool has_backward(const dd_config& c) { return (c.flags & (DD_FLAG_BACKWARD | DD_FLAG_LOOP_BACKWARD)) != 0; }
 // Elements of the denoiser's parameters in dd_denoiser_backward's order (time_embedding dense); offsets into lp.acc.
@@ -792,7 +831,7 @@ size_t carve(dd_engine* e, void* base) {
   }
   v->temb_sel = c.take<float>(static_cast<size_t>(g.B) * 256);
   if (e->cfg.flags & DD_FLAG_STEP_DECODE)
-    v->inter = c.take<float>(static_cast<size_t>(e->cfg.num_inference_steps) * BP * 4);
+    v->inter = c.take<float>(static_cast<size_t>(e->cfg.num_inference_steps) * codec_map_elems(e->cfg));
   if (e->rn.enabled || e->bb.enabled || e->mp.enabled)
     v->rgb_stage = c.take<float>(static_cast<size_t>(g.B) * 3 *
                                  (e->rn.enabled ? e->rn.H * e->rn.W : (e->mp.enabled ? e->mp.H * e->mp.W : e->bb.H * e->bb.W)));
@@ -1196,8 +1235,31 @@ int run_dec_batch_stats(dd_engine* e, float* rec, cudaStream_t st) {
                       ct.dec_bt, ct.dec_bn, rec, st);
 }
 
-// decoder_kernel on the running-statistics fold, or in DD_CODEC_TRAIN on the batch fold of the last run_dec_batch_stats
+// The UP4 / FULL decoders (codec_kinds.cuh) on their folded block: x32 -> [B][u h][u w]
+int run_kind_decoder(dd_engine* e, float* logit, float* depth, cudaStream_t st) {
+  const Geom g = geom_of(e->cfg);
+  dd::CodecKindArgs a{};
+  a.in = e->x32;
+  a.p = e->xdec;
+  a.out = depth;
+  a.logit = logit;
+  a.h = g.h;
+  a.w = g.w;
+  a.eps = 1e-6f;
+  if (codec_kind(e->cfg) == DD_CODEC_UP4) {
+    dim3 grid((4 * g.w + dd::D4_TW - 1) / dd::D4_TW, (4 * g.h + dd::D4_TH - 1) / dd::D4_TH, g.B);
+    dd::decoder_x4_kernel<<<grid, 256, dd::D4_SMEM, st>>>(a);
+    return launched(e, "decoder_x4");
+  }
+  dim3 grid((g.w + dd::DF_TW - 1) / dd::DF_TW, (g.h + dd::DF_TH - 1) / dd::DF_TH, g.B);
+  dd::decoder_full_kernel<<<grid, 256, dd::DF_SMEM, st>>>(a);
+  return launched(e, "decoder_full");
+}
+
+// The codec's decoder: decoder_kernel on the running-statistics fold, or in DD_CODEC_TRAIN on the batch fold of the
+// last run_dec_batch_stats; the UP4 / FULL kinds' own kernels
 int run_decoder(dd_engine* e, float* logit, float* depth, cudaStream_t st) {
+  if (codec_kind(e->cfg) >= DD_CODEC_UP4) return run_kind_decoder(e, logit, depth, st);
   const Geom g = geom_of(e->cfg);
   const bool train = e->codec_mode == DD_CODEC_TRAIN;
   dd::DecoderArgs a;
@@ -1383,6 +1445,141 @@ size_t numel(const std::vector<int64_t>& s) {
   return n;
 }
 
+// Codec kinds other than DD_CODEC_UP2: the keys their own pack reads and where PackStage::xraw holds them (encoders
+// from 0, decoders from kXDecRaw).  DD_CODEC_UP2_1X1's decoder is the default one (kDecKeys); the FULL encoder has the
+// default encoder's keys but its own kernel and pack.
+struct KindKey {
+  std::string name;
+  std::vector<int64_t> shape;
+  size_t off;
+};
+std::vector<KindKey> make_kind_keys(int kind, bool enc) {
+  std::vector<std::pair<std::string, std::vector<int64_t>>> k;
+  auto conv_bn = [&](const std::string& p, int64_t ci, int64_t co) {  // conv_bn_relu: conv `p0`, BatchNorm `p1`
+    k.push_back({p + "0.weight", {co, ci, 3, 3}});
+    for (const char* leaf : {"1.weight", "1.bias", "1.running_mean", "1.running_var"}) k.push_back({p + leaf, {co}});
+  };
+  const std::string E = "conv_transform.", D = "conv_inv_transform.";
+  if (enc && kind == DD_CODEC_UP2_1X1) {
+    k.push_back({E + "0.weight", {16, 1, 1, 1}});
+    k.push_back({E + "1.weight", {16, 16, 1, 1}});
+  }
+  if (enc && kind == DD_CODEC_UP4) {
+    conv_bn(E + "0.", 1, 16);
+    conv_bn(E + "1.", 16, 16);
+    conv_bn(E + "2.", 16, 16);
+  }
+  if (enc && kind == DD_CODEC_FULL) {
+    conv_bn(E + "0.", 1, 16);
+    conv_bn(E + "1.", 16, 16);
+  }
+  if (!enc && kind == DD_CODEC_UP4) {
+    k.push_back({D + "0.weight", {16, 16, 4, 4}});
+    k.push_back({D + "0.bias", {16}});
+    k.push_back({D + "1.weight", {16, 16, 4, 4}});
+    k.push_back({D + "1.bias", {16}});
+    for (const char* leaf : {"2.weight", "2.bias", "2.running_mean", "2.running_var"}) k.push_back({D + leaf, {16}});
+    k.push_back({D + "4.0.weight", {1, 16, 3, 3}});
+    k.push_back({D + "4.0.bias", {1}});
+  }
+  if (!enc && kind == DD_CODEC_FULL) {
+    conv_bn(D + "0.", 16, 16);
+    conv_bn(D + "1.", 16, 1);
+  }
+  std::vector<KindKey> out;
+  size_t off = enc ? 0 : kXDecRaw;
+  for (auto& kv : k) {
+    out.push_back({"depth_transform." + kv.first, kv.second, off});
+    off += numel(kv.second);
+  }
+  return out;
+}
+const std::vector<KindKey>& kind_keys(int kind, bool enc) {
+  static const std::vector<KindKey> t[2][4] = {
+      {make_kind_keys(0, false), make_kind_keys(1, false), make_kind_keys(2, false), make_kind_keys(3, false)},
+      {make_kind_keys(0, true), make_kind_keys(1, true), make_kind_keys(2, true), make_kind_keys(3, true)}};
+  return t[enc ? 1 : 0][kind];
+}
+// Every codec kind's tables fit their PackStage::xraw region (encoder [0, kXDecRaw), decoder [kXDecRaw, kXRawFloats)).
+bool kind_keys_fit() {
+  for (int kind = 0; kind < 4; ++kind)
+    for (bool enc : {true, false})
+      for (const KindKey& k : kind_keys(kind, enc))
+        if (k.off + numel(k.shape) > (enc ? kXDecRaw : kXRawFloats)) return false;
+  return true;
+}
+const KindKey* find_kind_key(int kind, const std::string& name) {
+  for (bool enc : {true, false})
+    for (const KindKey& k : kind_keys(kind, enc))
+      if (k.name == name) return &k;
+  return nullptr;
+}
+
+// Fold the staged tensors of codec kind `kind` (PackStage::xraw) into its encoder (PackStage::xenc) or decoder
+// (xdec) block, in fp64 on the host like the default codec's folds; layouts in codec_kinds.cuh.
+void fold_kind(PackStage* sg, int kind, bool enc) {
+  auto R = [&](const std::string& leaf) -> const float* {
+    for (const KindKey& k : kind_keys(kind, enc))
+      if (k.name == "depth_transform." + leaf) return sg->xraw + k.off;
+    return nullptr;
+  };
+  // conv_bn_relu `p` (ci -> co, 3x3) with its BatchNorm folded: w [9][ci][co], b [co]
+  auto conv_bn = [&](const std::string& p, int ci, int co, float* w, float* b) {
+    const float* raw = R(p + "0.weight");
+    const float* bn[4] = {R(p + "1.weight"), R(p + "1.bias"), R(p + "1.running_mean"), R(p + "1.running_var")};
+    float sc[16], sh[16];
+    bn_fold_host(bn, co, sc, sh);
+    for (int o = 0; o < co; ++o) {
+      b[o] = sh[o];
+      for (int i = 0; i < ci; ++i)
+        for (int tap = 0; tap < 9; ++tap)
+          w[(tap * ci + i) * co + o] = static_cast<float>(static_cast<double>(raw[(o * ci + i) * 9 + tap]) * sc[o]);
+    }
+  };
+  const std::string E = "conv_transform.", D = "conv_inv_transform.";
+  if (enc) {
+    float* x = sg->xenc;
+    if (kind == DD_CODEC_UP2_1X1) {
+      const float *w1 = R(E + "0.weight"), *w2 = R(E + "1.weight");
+      for (int co = 0; co < 16; ++co) {
+        double k = 0.0;
+        for (int ci = 0; ci < 16; ++ci) k += static_cast<double>(w2[co * 16 + ci]) * w1[ci];
+        x[dd::CK_E1_K + co] = static_cast<float>(k);
+      }
+      return;
+    }
+    conv_bn(E + "0.", 1, 16, x + dd::CK_E4_W1, x + dd::CK_E4_B1);
+    conv_bn(E + "1.", 16, 16, x + dd::CK_E4_W2, x + dd::CK_E4_B2);
+    if (kind == DD_CODEC_UP4) conv_bn(E + "2.", 16, 16, x + dd::CK_E4_W3, x + dd::CK_E4_B3);
+    return;
+  }
+  float* x = sg->xdec;
+  if (kind == DD_CODEC_FULL) {
+    conv_bn(D + "0.", 16, 16, x + dd::CK_DF_W1, x + dd::CK_DF_B1);
+    conv_bn(D + "1.", 16, 1, x + dd::CK_DF_WC, x + dd::CK_DF_BC);
+    for (int i = 1; i < 4; ++i) x[dd::CK_DF_BC + i] = 0.f;
+    return;
+  }
+  const float *t1 = R(D + "0.weight"), *b1 = R(D + "0.bias"), *t2 = R(D + "1.weight"), *b2 = R(D + "1.bias");
+  const float *g = R(D + "2.weight"), *be = R(D + "2.bias"), *mu = R(D + "2.running_mean"), *var = R(D + "2.running_var");
+  const float *wc = R(D + "4.0.weight"), *bc = R(D + "4.0.bias");
+  for (int co = 0; co < 16; ++co) {
+    const double sc = static_cast<double>(g[co]) / sqrt(static_cast<double>(var[co]) + 1e-5);
+    x[dd::CK_D4_B1 + co] = b1[co];
+    x[dd::CK_D4_B2 + co] = static_cast<float>((static_cast<double>(b2[co]) - mu[co]) * sc + be[co]);
+    for (int ci = 0; ci < 16; ++ci)
+      for (int k = 0; k < 16; ++k) {  // ConvTranspose2d weight layout: [Cin][Cout][kh][kw] -> [ky][kx][ci][co]
+        x[dd::CK_D4_T1 + (k * 16 + ci) * 16 + co] = t1[(ci * 16 + co) * 16 + k];
+        x[dd::CK_D4_T2 + (k * 16 + ci) * 16 + co] = static_cast<float>(static_cast<double>(t2[(ci * 16 + co) * 16 + k]) * sc);
+      }
+  }
+  for (int ci = 0; ci < 16; ++ci)
+    for (int tap = 0; tap < 9; ++tap) x[dd::CK_D4_WC + tap * 16 + ci] = wc[ci * 9 + tap];
+  x[dd::CK_D4_BC] = bc[0];
+  for (int i = 1; i < 4; ++i) x[dd::CK_D4_BC + i] = 0.f;
+}
+
+// `encoder`: the codec kind's encoder keys are registered (its pack is optional, as dd_encode is).
 int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
   const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
   int rc;
@@ -1436,8 +1633,12 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
   if ((rc = dev_array(h, &ct.part_db, static_cast<size_t>(dec_act_blocks(g)) * 16))) return rc;
   if ((rc = dev_array(h, &ct.rec, static_cast<size_t>(std::max(h->cfg.num_inference_steps, 2)) * 32))) return rc;
   ct.nrec = 0;
+  const int kind = codec_kind(h->cfg);
+  h->xenc = h->xdec = nullptr;
+  if (kind != DD_CODEC_UP2 && encoder && (rc = dev_array(h, &h->xenc, dd::CK_E4_N))) return rc;
+  if (kind >= DD_CODEC_UP4 && (rc = dev_array(h, &h->xdec, dd::CK_D4_N))) return rc;
   h->enc_w1 = nullptr;
-  if (encoder) {
+  if (encoder && kind == DD_CODEC_UP2) {
     if ((rc = dev_array(h, &h->enc_w1, 144))) return rc;
     if ((rc = dev_array(h, &h->enc_b1, 16))) return rc;
     if ((rc = dev_array(h, &h->enc_w2, 2304))) return rc;
@@ -1466,9 +1667,14 @@ int check_update(dd_engine* h) {
   }
   for (int i = 0; i < 4; ++i) want[std::string(kGnKey[i]) + ".weight"] = want[std::string(kGnKey[i]) + ".bias"] = {kGnCh[i]};
   want["model.time_embedding.weight"] = {DD_TIME_ROWS, 256};
-  for (const CodecKey& k : kDecKeys) want[kDecPrefix + k.leaf] = k.shape;
+  const int kind = codec_kind(h->cfg);
+  if (kind <= DD_CODEC_UP2_1X1)
+    for (const CodecKey& k : kDecKeys) want[kDecPrefix + k.leaf] = k.shape;
   if (h->enc_w1)
     for (const CodecKey& k : kEncKeys) want[kEncPrefix + k.leaf] = k.shape;
+  for (bool enc : {true, false})
+    if (kind != DD_CODEC_UP2 && (!enc || h->xenc))
+      for (const KindKey& k : kind_keys(kind, enc)) want[k.name] = k.shape;
   for (const auto& kv : h->raw) {
     const std::string& name = kv.first;
     for (const char* p : {"hahineck.", "conv_lateral.", "conv_up.", "backbone."})
@@ -1539,9 +1745,16 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
   }
   if (const float* t = W("model.time_embedding.weight"))
     CUDA_TRY(cudaMemcpyAsync(h->temb, t, DD_TIME_ROWS * 256 * 4, cudaMemcpyDeviceToDevice, st));
-  bool dec = false, enc = false;
+  const int kind = codec_kind(h->cfg);
+  bool dec = false, enc = false, xenc = false, xdec = false;
+  for (bool e : {true, false})
+    for (const KindKey& k : kind_keys(kind, e))
+      if (const float* p = W(k.name)) {
+        CUDA_TRY(cudaMemcpyAsync(sg->xraw + k.off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
+        (e ? xenc : xdec) = true;
+      }
   for (const CodecKey& k : kDecKeys)
-    if (const float* p = W(kDecPrefix + k.leaf)) {
+    if (const float* p = kind <= DD_CODEC_UP2_1X1 ? W(kDecPrefix + k.leaf) : nullptr) {
       CUDA_TRY(cudaMemcpyAsync(sg_f + k.host_off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
       dec = true;
     }
@@ -1650,6 +1863,14 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w2, sg->e2u, sizeof(sg->e2u), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(h->ct.enc_gb, sg->enc_gb, sizeof(sg->enc_gb), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(h->enc_bn, sg->enc_bn, sizeof(sg->enc_bn), cudaMemcpyHostToDevice, st));
+  }
+  if (xenc) {
+    fold_kind(sg, kind, true);
+    CUDA_TRY(cudaMemcpyAsync(h->xenc, sg->xenc, sizeof(sg->xenc), cudaMemcpyHostToDevice, st));
+  }
+  if (xdec) {  // the UP4 / FULL decoders read every constant from this block, so no graph holds one by value
+    fold_kind(sg, kind, false);
+    CUDA_TRY(cudaMemcpyAsync(h->xdec, sg->xdec, sizeof(sg->xdec), cudaMemcpyHostToDevice, st));
   }
   CUDA_TRY(cudaEventRecord(h->pack_done, st));
   if (loop_stale) drop_graph(h, dd_engine::G_LOOP);
@@ -2836,6 +3057,11 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
     return fail(DD_ERR_INVALID, "bad geometry");
   if (cfg->variant == DD_VARIANT_RES && (cfg->cond_h != cfg->latent_h || cfg->cond_w != cfg->latent_w))
     return fail(DD_ERR_INVALID, "Res variant needs the condition map at latent resolution");
+  if (!kind_keys_fit()) return fail(DD_ERR_INVALID, "codec key tables exceed the pack's host staging buffer");
+  if (codec_kind(*cfg) != DD_CODEC_UP2 && (cfg->flags & DD_FLAG_LOOP_BACKWARD))
+    return fail(DD_ERR_UNSUPPORTED, std::string("DD_FLAG_LOOP_BACKWARD: the loop backward differentiates through the "
+                                                "DeepDepthTransformWithUpsampling decoder only, not ") +
+                                        codec_name(codec_kind(*cfg)));
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(DD_ERR_UNSUPPORTED, "no CUDA device: libddengine has no CPU path");
@@ -2884,10 +3110,17 @@ int dd_set_weight(dd_handle h, const char* name, const float* dev_ptr, const int
   if (!h || !name || !dev_ptr || ndim < 0 || ndim > 4) return fail(DD_ERR_INVALID, "bad argument");
   bool known = strncmp(name, "hahineck.", 9) == 0 || strncmp(name, "conv_lateral.", 13) == 0 ||
                strncmp(name, "conv_up.", 8) == 0 ||  // step-invariant producers (optional, dd_enable_producers)
-               strncmp(name, "backbone.", 9) == 0 ||  // native backbone (optional, dd_enable_backbone)
-               strncmp(name, "depth_transform.conv_transform.", 31) == 0;  // encoder t() (optional, dd_encode)
-  for (const char* k : kKeys) known |= (strcmp(k, name) == 0);
-  if (!known) return fail(DD_ERR_INVALID, std::string("unknown weight key: ") + name);
+               strncmp(name, "backbone.", 9) == 0;  // native backbone (optional, dd_enable_backbone)
+  const int kind = codec_kind(h->cfg);
+  // the codec's keys: the default encoder t() (optional, dd_encode) and decoder, or those of this engine's codec kind
+  // (UP2_1X1 keeps the default decoder)
+  known |= kind == DD_CODEC_UP2 && strncmp(name, "depth_transform.conv_transform.", 31) == 0;
+  for (const char* k : kKeys)
+    known |= strcmp(k, name) == 0 && (kind <= DD_CODEC_UP2_1X1 || strncmp(k, "depth_transform.", 16) != 0);
+  known |= find_kind_key(kind, name) != nullptr;
+  if (!known)
+    return fail(DD_ERR_INVALID, std::string("unknown weight key: ") + name +
+                                    (strncmp(name, "depth_transform.", 16) == 0 ? std::string(" (codec ") + codec_name(kind) + ")" : ""));
   Raw r;
   r.ptr = dev_ptr;
   r.shape.assign(shape, shape + ndim);
@@ -2901,23 +3134,36 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CUDA_TRY(cudaSetDevice(h->cfg.device));
   const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
+  const int kind = codec_kind(h->cfg);
+  const bool default_dec = kind <= DD_CODEC_UP2_1X1;
   std::string missing;
   for (const char* k : kKeys) {
     if (!swin && strstr(k, "upsample_fuse")) continue;
+    if (!default_dec && strncmp(k, "depth_transform.", 16) == 0) continue;
     if (!find(h, k)) missing += std::string(missing.empty() ? "" : ", ") + k;
   }
+  for (const KindKey& k : kind_keys(kind, false))
+    if (!find(h, k.name)) missing += (missing.empty() ? "" : ", ") + k.name;
   if (!missing.empty()) return fail(DD_ERR_INVALID, "missing weights: " + missing);
   auto expect = [&](const char* k, std::vector<int64_t> s) { return find(h, k)->shape == s; };
   if (!expect("model.noise_embedding.0.weight", {64, 16, 3, 3}) || !expect("model.noise_embedding.3.weight", {256, 64, 3, 3}) ||
       !expect("model.pred.0.weight", {64, 256, 3, 3}) || !expect("model.pred.3.weight", {16, 64, 3, 3}) ||
       !expect("model.time_embedding.weight", {DD_TIME_ROWS, 256}) ||
-      !expect("depth_transform.conv_inv_transform.0.weight", {16, 16, 4, 4}) ||
-      !expect("depth_transform.conv_inv_transform.3.0.weight", {1, 16, 3, 3}) ||
+      (default_dec && (!expect("depth_transform.conv_inv_transform.0.weight", {16, 16, 4, 4}) ||
+                       !expect("depth_transform.conv_inv_transform.3.0.weight", {1, 16, 3, 3}))) ||
       (swin && (!expect("model.upsample_fuse.convA.conv.weight", {256, 256, 3, 3}) ||
                 !expect("model.upsample_fuse.convB.conv.weight", {256, 256, 3, 3}))))
     return fail(DD_ERR_INVALID, "weight shape mismatch with the reference architecture");
-  const bool encoder = find(h, kEncPrefix + "0.0.weight") != nullptr;
-  if (encoder) {
+  bool encoder = kind == DD_CODEC_UP2 && find(h, kEncPrefix + "0.0.weight") != nullptr;
+  for (const KindKey& k : kind_keys(kind, true)) encoder |= find(h, k.name) != nullptr;
+  for (bool enc : {true, false})  // the codec kind's keys: all of the encoder's when one is registered, shapes
+    for (const KindKey& k : kind_keys(kind, enc)) {
+      if (enc && !encoder) break;
+      const Raw* r = find(h, k.name);
+      if (!r) return fail(DD_ERR_INVALID, "missing weights: " + k.name);
+      if (r->shape != k.shape) return fail(DD_ERR_INVALID, k.name + ": weight shape mismatch with " + codec_name(kind));
+    }
+  if (encoder && kind == DD_CODEC_UP2) {
     const Raw *w1 = find(h, kEncPrefix + "0.0.weight"), *w2 = find(h, kEncPrefix + "1.0.weight");
     if (!w2 || w1->shape != std::vector<int64_t>{16, 1, 3, 3} || w2->shape != std::vector<int64_t>{16, 16, 3, 3})
       return fail(DD_ERR_INVALID, "encoder weights missing / wrong shape");
@@ -3018,7 +3264,7 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
   if ((rc = split_planes(h, h->x32, h->xs_hi, h->xs_lo, static_cast<size_t>(g.B) * g.P * 16, kXScale, st))) return rc;
   h->launches += 2;
   const int T = h->cfg.num_inference_steps;
-  const size_t map_elems = static_cast<size_t>(g.B) * g.P * 4;  // one decoded batch [B][2h][2w]
+  const size_t map_elems = codec_map_elems(h->cfg);  // one decoded batch [B][u h][u w]
   const bool steps = depth_steps_out != nullptr;
   const bool train = h->codec_mode == DD_CODEC_TRAIN;  // batch statistics before every decode, one record each
   if (steps && train && h->sync.fn)
@@ -3261,6 +3507,8 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
 int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, float* d_latent_out,
                        float* const* d_dec_params, void* workspace, size_t workspace_bytes, void* cuda_stream) {
   if (!h || !latent || !d_depth) return fail(DD_ERR_INVALID, "null argument");
+  if (codec_kind(h->cfg) != DD_CODEC_UP2)
+    return fail(DD_ERR_UNSUPPORTED, std::string("dd_decode_backward: no decoder backward for ") + codec_name(codec_kind(h->cfg)));
   if (!(h->cfg.flags & DD_FLAG_LOOP_BACKWARD))
     return fail(DD_ERR_INVALID, "dd_decode_backward needs an engine created with DD_FLAG_LOOP_BACKWARD");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
@@ -3293,6 +3541,9 @@ int dd_decode(dd_handle h, const float* latent, float* logit_out, float* depth_o
 int dd_set_codec_mode(dd_handle h, int32_t mode) {
   if (!h) return fail(DD_ERR_INVALID, "null handle");
   if (mode != DD_CODEC_EVAL && mode != DD_CODEC_TRAIN) return fail(DD_ERR_INVALID, "codec mode must be DD_CODEC_EVAL or DD_CODEC_TRAIN");
+  if (mode == DD_CODEC_TRAIN && codec_kind(h->cfg) != DD_CODEC_UP2)
+    return fail(DD_ERR_UNSUPPORTED, std::string("DD_CODEC_TRAIN: no batch-statistics BatchNorms for ") +
+                                        codec_name(codec_kind(h->cfg)));
   h->codec_mode = mode;
   return DD_OK;
 }
@@ -3670,8 +3921,44 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
   });
 }
 
+// dd_encode for the codec kinds other than DD_CODEC_UP2 (eval BatchNorm only: dd_set_codec_mode refuses DD_CODEC_TRAIN)
+static int encode_kind(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, cudaStream_t st) {
+  const int kind = codec_kind(h->cfg);
+  if (!h->weights_ready || !h->xenc)
+    return fail(DD_ERR_INVALID, std::string("encoder weights (depth_transform.conv_transform.* of ") + codec_name(kind) +
+                                    ") not registered");
+  if (codec_latent(kind, height) != h->cfg.latent_h || codec_latent(kind, width) != h->cfg.latent_w)
+    return fail(DD_ERR_INVALID, "depth map size " + std::to_string(height) + " x " + std::to_string(width) +
+                                    " does not match the engine's latent grid under " + codec_name(kind));
+  CUDA_TRY(cudaSetDevice(h->cfg.device));
+  h->ct.nrec = 0;
+  dd::CodecKindArgs a{};
+  a.in = depth;
+  a.p = h->xenc;
+  a.out = latent_out;
+  a.H = height;
+  a.W = width;
+  a.h = h->cfg.latent_h;
+  a.w = h->cfg.latent_w;
+  if (kind == DD_CODEC_UP2_1X1) {
+    dim3 grid(static_cast<unsigned>((static_cast<long long>(a.h) * a.w + 255) / 256), h->cfg.batch);
+    dd::encoder_1x1_kernel<<<grid, 256, 0, st>>>(a);
+    return check_launch("encoder_1x1");
+  }
+  if (kind == DD_CODEC_UP4) {
+    dim3 grid((a.w + dd::E4_T - 1) / dd::E4_T, (a.h + dd::E4_T - 1) / dd::E4_T, h->cfg.batch);
+    dd::encoder_x4_kernel<<<grid, 256, dd::E4_SMEM, st>>>(a);
+    return check_launch("encoder_x4");
+  }
+  dim3 grid((a.w + dd::EF_T - 1) / dd::EF_T, (a.h + dd::EF_T - 1) / dd::EF_T, h->cfg.batch);
+  dd::encoder_full_kernel<<<grid, 256, dd::EF_SMEM, st>>>(a);
+  return check_launch("encoder_full");
+}
+
 int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, void* cuda_stream) {
   if (!h || !depth || !latent_out) return fail(DD_ERR_INVALID, "null argument");
+  if (codec_kind(h->cfg) != DD_CODEC_UP2)
+    return encode_kind(h, depth, height, width, latent_out, static_cast<cudaStream_t>(cuda_stream));
   if (!h->weights_ready || !h->enc_w1) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
   if ((height + 1) / 2 != h->cfg.latent_h || (width + 1) / 2 != h->cfg.latent_w)
     return fail(DD_ERR_INVALID, "depth map size does not match the engine's latent grid");
@@ -3791,6 +4078,8 @@ int run_encode_bwd(dd_engine* e, const float* depth, int H, int W, const float* 
 int dd_encode_backward(dd_handle h, const float* depth, int32_t height, int32_t width, const float* d_latent,
                        float* const* d_enc_params, void* workspace, size_t workspace_bytes, void* cuda_stream) {
   if (!h || !depth || !d_latent) return fail(DD_ERR_INVALID, "null argument");
+  if (codec_kind(h->cfg) != DD_CODEC_UP2)
+    return fail(DD_ERR_UNSUPPORTED, std::string("dd_encode_backward: no encoder backward for ") + codec_name(codec_kind(h->cfg)));
   int rc;
   if ((rc = check_operator_bwd_call(h, "dd_encode_backward"))) return rc;
   if (!h->enc_w1) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
@@ -4300,6 +4589,17 @@ int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspac
   if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
   // whatever the planes currently hold is fine for timing: MMA time is data independent
   return time_per_call(st, 2, iters, ms_out, [&]() { return run_fold(h, st); });
+}
+
+int dd_bench_decoder(dd_handle h, float* depth_out, int32_t iters, float* ms_out, void* workspace,
+                     size_t workspace_bytes, void* cuda_stream) {
+  if (!h || !depth_out || !ms_out || iters < 1) return fail(DD_ERR_INVALID, "bad argument");
+  if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  int rc;
+  if ((rc = enter_workspace(h, workspace, workspace_bytes))) return rc;
+  // the latent the workspace holds (the last call's) is decoded: the kernel's time does not depend on it
+  return time_per_call(st, 3, iters, ms_out, [&]() { return run_decoder(h, nullptr, depth_out, st); });
 }
 
 int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* ms_out, void* workspace,

@@ -52,6 +52,24 @@ DECODER_PARAM_KEYS = tuple(k for k in DECODER_KEYS if "running" not in k)
 _DECODER_SHAPES = {"depth_transform.conv_inv_transform.0.weight": (16, 16, 4, 4),
                    "depth_transform.conv_inv_transform.3.0.weight": (1, 16, 3, 3),
                    "depth_transform.conv_inv_transform.3.0.bias": (1,)}
+
+def _conv_bn_keys(prefix):
+    return (prefix + "0.weight",) + tuple(prefix + "1." + leaf for leaf in ("weight", "bias", "running_mean", "running_var"))
+
+
+# The codec's keys per dd_codec_kind (the `ENGINE_KIND` of the depth_transform classes): (encoder, decoder).  Kind 0 is
+# the default codec's ENCODER_KEYS / DECODER_KEYS.
+_T, _IT = "depth_transform.conv_transform.", "depth_transform.conv_inv_transform."
+CODEC_KEYS = {
+    0: (ENCODER_KEYS, DECODER_KEYS),
+    1: ((_T + "0.weight", _T + "1.weight"), DECODER_KEYS),
+    2: (_conv_bn_keys(_T + "0.") + _conv_bn_keys(_T + "1.") + _conv_bn_keys(_T + "2."),
+        (_IT + "0.weight", _IT + "0.bias", _IT + "1.weight", _IT + "1.bias") +
+        tuple(_IT + "2." + leaf for leaf in ("weight", "bias", "running_mean", "running_var")) +
+        (_IT + "4.0.weight", _IT + "4.0.bias")),
+    3: (ENCODER_KEYS, _conv_bn_keys(_IT + "0.") + _conv_bn_keys(_IT + "1.")),
+}
+CODEC_UP = {0: 2, 1: 2, 2: 4, 3: 1}  # the decoder's upsampling: decoded map [B, 1, u h, u w]
 # keys `DenoiseEngine.update_weights` re-packs in place (the denoiser and the depth codec); the neck, FPN and backbone
 # packs are rebuilt by `load_weights` only
 UPDATABLE_PREFIXES = ("model.", "depth_transform.conv_inv_transform.", "depth_transform.conv_transform.")
@@ -122,7 +140,7 @@ class DenoiseEngine:
                  simt_conv: bool = False, check_range: bool = False, halo_conv: bool = True,
                  swap_narrow: bool = True, pair_wide: bool = True, step_decode: bool = False, workspace_pool=None,
                  fp8_corr: bool = True, backward: bool = False, loop_backward: bool = False,
-                 chain_pred: bool = False, producer_train: bool = False):
+                 chain_pred: bool = False, producer_train: bool = False, codec_kind: int = 0):
         self.lib = _cabi.load_library()
         device = torch.device(device)
         if device.type != "cuda":
@@ -137,6 +155,11 @@ class DenoiseEngine:
                 (_cabi.FLAG_STEP_DECODE if step_decode else 0) | (_cabi.FLAG_FP8_CORR if fp8_corr else 0) | \
                 (_cabi.FLAG_BACKWARD if backward else 0) | (_cabi.FLAG_LOOP_BACKWARD if loop_backward else 0) | \
                 (_cabi.FLAG_CHAIN_PRED if chain_pred else 0) | (_cabi.FLAG_PRODUCER_TRAIN if producer_train else 0)
+        if codec_kind not in CODEC_KEYS:
+            raise EngineError(f"unknown codec kind {codec_kind}")
+        flags |= int(codec_kind) << _cabi.FLAG_CODEC_SHIFT
+        self.codec_kind = int(codec_kind)
+        self.up = CODEC_UP[self.codec_kind]  # decoded map [B, 1, up h, up w]
         self.producer_train = bool(producer_train)
         self.fp8_corr = bool(fp8_corr)
         self.backward = bool(backward or loop_backward)  # the loop backward includes the operator's
@@ -160,9 +183,10 @@ class DenoiseEngine:
 
     # ---------------------------------------------------------------- setup
     def load_weights(self, tensors: Dict[str, torch.Tensor]):
-        keys = DENOISER_KEYS + DECODER_KEYS + (FUSE_KEYS if self.variant == "swin" else ())
-        if all(k in tensors for k in ENCODER_KEYS):
-            keys = keys + ENCODER_KEYS
+        enc_keys, dec_keys = CODEC_KEYS[self.codec_kind]
+        keys = DENOISER_KEYS + dec_keys + (FUSE_KEYS if self.variant == "swin" else ())
+        if all(k in tensors for k in enc_keys):
+            keys = keys + enc_keys
         if self.backbone is not None:
             keys = keys + tuple(k for k in tensors if k.startswith("backbone.") and tensors[k].is_floating_point())
         if self.producers is not None:
@@ -182,7 +206,7 @@ class DenoiseEngine:
         changed, all of them `is_updatable`.  Buffers, TMA descriptors and CUDA graphs are kept (a loop graph is
         captured again only when a conv's power-of-two weight scale changed); the result is bit-identical to a
         `load_weights` of the whole model.  On EngineError the previous pack is intact."""
-        known = DENOISER_KEYS + FUSE_KEYS + DECODER_KEYS + ENCODER_KEYS
+        known = DENOISER_KEYS + FUSE_KEYS + sum(CODEC_KEYS[self.codec_kind], ())
         for k, v in tensors.items():  # what dd_set_weight would reject, before anything is registered
             if not (k in known or k.startswith(("hahineck.", "conv_lateral.", "conv_up.", "backbone."))) or v.dim() > 4:
                 raise EngineError(f"unknown weight key: {k}")
@@ -293,13 +317,13 @@ class DenoiseEngine:
         return cond
 
     def denoise_decode(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False, want_logits=False):
-        """cond [B,256,hc,wc] (or None right after build_condition), noise [B,16,h,w] -> depth [B,1,2h,2w]
-        (+ latent [B,16,h,w], logits)."""
-        B, (h, w) = self.batch, self.latent_hw
+        """cond [B,256,hc,wc] (or None right after build_condition), noise [B,16,h,w] -> depth [B,1,u h,u w]
+        (u = `self.up`, the codec's upsampling; + latent [B,16,h,w], logits)."""
+        B, (h, w), u = self.batch, self.latent_hw, self.up
         if cond is not None:
             self._check_in(cond, (B, 256, *self.cond_hw))
         self._check_in(noise, (B, 16, h, w))
-        depth = torch.empty(B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32)
+        depth = torch.empty(B, 1, u * h, u * w, device=self.device, dtype=torch.float32)
         latent = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32) if want_latent else None
         logits = torch.empty_like(depth) if want_logits else None
         _cabi.check(self.lib.dd_denoise_decode(self._h, _ptr(cond), _ptr(noise), _ptr(latent), _ptr(logits), _ptr(depth),
@@ -309,16 +333,16 @@ class DenoiseEngine:
     def denoise_decode_steps(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False,
                              want_logits=False):
         """As `denoise_decode`, additionally decoding the latent after every step inside the captured graph (the *Vis
-        heads' `pred_inter`): returns (depth_steps [T,B,1,2h,2w], latent, logits of the final step)."""
+        heads' `pred_inter`): returns (depth_steps [T,B,1,u h,u w], latent, logits of the final step)."""
         if not self.step_decode:
             raise EngineError("engine was created without step_decode=True")
-        B, (h, w) = self.batch, self.latent_hw
+        B, (h, w), u = self.batch, self.latent_hw, self.up
         if cond is not None:
             self._check_in(cond, (B, 256, *self.cond_hw))
         self._check_in(noise, (B, 16, h, w))
-        steps = torch.empty(self.steps, B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32)
+        steps = torch.empty(self.steps, B, 1, u * h, u * w, device=self.device, dtype=torch.float32)
         latent = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32) if want_latent else None
-        logits = torch.empty(B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32) if want_logits else None
+        logits = torch.empty(B, 1, u * h, u * w, device=self.device, dtype=torch.float32) if want_logits else None
         _cabi.check(self.lib.dd_denoise_decode_steps(self._h, _ptr(cond), _ptr(noise), _ptr(latent), _ptr(logits),
                                                      _ptr(steps), *self._ws_args()))
         return steps, latent, logits
@@ -400,7 +424,7 @@ class DenoiseEngine:
             self._check_in(cond, (B, 256, *self.cond_hw))
         self._check_in(noise, (B, 16, h, w))
         if d_depth is not None:
-            self._check_in(d_depth, (B, 1, 2 * h, 2 * w))
+            self._check_in(d_depth, (B, 1, self.up * h, self.up * w))
         if d_latent is not None:
             self._check_in(d_latent, (B, 16, h, w))
         d_cond = torch.empty(B, 256, *self.cond_hw, device=self.device) if want_cond else None
@@ -422,7 +446,7 @@ class DenoiseEngine:
             raise EngineError("engine was created without loop_backward=True")
         B, (h, w) = self.batch, self.latent_hw
         self._check_in(latent, (B, 16, h, w))
-        self._check_in(d_depth, (B, 1, 2 * h, 2 * w))
+        self._check_in(d_depth, (B, 1, self.up * h, self.up * w))
         d_latent = torch.empty_like(latent) if want_latent else None
         grads, ptrs = self._grad_buffers(DECODER_PARAM_KEYS if want_params else (), _DECODER_SHAPES, (16,))
         _cabi.check(self.lib.dd_decode_backward(self._h, _ptr(latent), _ptr(d_depth), _ptr(d_latent),
@@ -430,7 +454,8 @@ class DenoiseEngine:
         return d_latent, grads
 
     def encode(self, depth: torch.Tensor) -> torch.Tensor:
-        """latent = depth_transform.t(depth): [B,1,H,W] -> [B,16,ceil(H/2),ceil(W/2)]."""
+        """latent = depth_transform.t(depth): [B,1,H,W] -> [B,16,h,w], the codec's latent grid of H x W (the default
+        codec: ceil(H/2) x ceil(W/2))."""
         B, (h, w) = self.batch, self.latent_hw
         H, W = depth.shape[-2:]
         self._check_in(depth, (B, 1, H, W))
@@ -555,9 +580,9 @@ class DenoiseEngine:
         self._allgather, self.bn_allgather_group = fn, group
 
     def decode(self, latent: torch.Tensor, want_logits=False):
-        B, (h, w) = self.batch, self.latent_hw
+        B, (h, w), u = self.batch, self.latent_hw, self.up
         self._check_in(latent, (B, 16, h, w))
-        depth = torch.empty(B, 1, 2 * h, 2 * w, device=self.device, dtype=torch.float32)
+        depth = torch.empty(B, 1, u * h, u * w, device=self.device, dtype=torch.float32)
         logits = torch.empty_like(depth) if want_logits else None
         _cabi.check(self.lib.dd_decode(self._h, _ptr(latent), _ptr(logits), _ptr(depth), *self._ws_args()))
         return depth, logits
@@ -754,6 +779,15 @@ class DenoiseEngine:
         """Average milliseconds per launch of the (cin -> cout) conv on this engine's latent grid."""
         ms = C.c_float()
         _cabi.check(self.lib.dd_bench_conv(self._h, cin, cout, iters, C.byref(ms), *self._ws_args()))
+        return float(ms.value)
+
+    def bench_decoder(self, iters: int = 20) -> float:
+        """Average milliseconds per launch of the codec's decoder kernel alone (CUDA events), on the latent the
+        workspace holds from the last call."""
+        B, (h, w), u = self.batch, self.latent_hw, self.up
+        depth = torch.empty(B, 1, u * h, u * w, device=self.device, dtype=torch.float32)
+        ms = C.c_float()
+        _cabi.check(self.lib.dd_bench_decoder(self._h, _ptr(depth), iters, C.byref(ms), *self._ws_args()))
         return float(ms.value)
 
     def bench_pred_fold(self, iters: int = 20) -> float:

@@ -22,7 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from diffusiondepth_b200._cabi import EngineError
-from diffusiondepth_b200.engine import (DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS,
+from diffusiondepth_b200.engine import (CODEC_KEYS, DECODER_KEYS, DECODER_PARAM_KEYS, DENOISER_KEYS, ENCODER_KEYS,
                                         ENCODER_PARAM_KEYS, FUSE_KEYS, DenoiseEngine, WorkspacePool, is_updatable)
 from .._blocks import ConvModule, DropPath, MMCVDropPath, exact_fp32
 from ..diffusers.schedulers.scheduling_ddim import DDIMScheduler
@@ -72,11 +72,12 @@ class EngineKey(NamedTuple):
     loop_backward: bool
     drop_path: Tuple[int, ...] = ()       # native backbone with stochastic depth: per stage, the bit mask of its MPViT
                                           # layers / Swin blocks (dd_backbone_config.mp_drop_path)
+    codec_kind: int = 0                   # the depth codec's dd_codec_kind (`depth_transform.ENGINE_KIND`)
 
     @property
     def geometry(self):
         """What an engine serving the bare operators (denoiser / decode) must match."""
-        return self.batch, self.latent_hw, self.cond_hw, self.device, self.steps
+        return self.batch, self.latent_hw, self.cond_hw, self.device, self.steps, self.codec_kind
 
 
 def _signature(tensors):
@@ -363,11 +364,39 @@ class DDIMHeadBase(nn.Module):
     # ------------------------------------------------------------------------------------------ engine bridge
     def _engine_tensors(self):
         sd = {}
-        for k in DENOISER_KEYS + DECODER_KEYS + ENCODER_KEYS + (FUSE_KEYS if self.variant == "swin" else ()):
+        enc_keys, dec_keys = CODEC_KEYS[self._codec_kind()]
+        for k in DENOISER_KEYS + dec_keys + enc_keys + (FUSE_KEYS if self.variant == "swin" else ()):
             mod, _, leaf = k.rpartition(".")
             obj = self.get_submodule(mod)
             sd[k] = getattr(obj, leaf)
         return sd
+
+    def _codec_kind(self) -> int:
+        """The engine's dd_codec_kind for `depth_transform`: one of the four learned codecs, with hidden = 16 (the
+        denoiser's `channels_noise`)."""
+        dt = self.depth_transform
+        kind = getattr(dt, "ENGINE_KIND", None)
+        if kind is None:
+            raise EngineError(f"{type(dt).__name__} has no engine codec: the DDIM heads denoise a 16-channel latent "
+                              "of a learned depth transform")
+        hidden = next(m.out_channels for m in dt.conv_transform.modules() if isinstance(m, nn.Conv2d))
+        if hidden != 16:
+            raise EngineError(f"{type(dt).__name__}(hidden={hidden}): the engine's latent has 16 channels (the "
+                              "denoiser's channels_noise)")
+        return kind
+
+    def _check_codec_trains(self):
+        """Training the codec on the engine (batch-statistics BatchNorms, encoder / decoder backward) exists for the
+        default codec only."""
+        if self._codec_kind() == 0:
+            return
+        name = type(self.depth_transform).__name__
+        if self.grad_through_loop:
+            raise EngineError(f"grad_through_loop: no decoder backward for {name} on the engine")
+        if self.grad_through_encoder:
+            raise EngineError(f"grad_through_encoder: no encoder backward for {name} on the engine")
+        if self.codec_train_bn and getattr(self.depth_transform, "training", False):
+            raise EngineError(f"codec_train_bn: no batch-statistics BatchNorms for {name} on the engine")
 
     def _producer_tensors(self):
         sd = {}
@@ -574,7 +603,8 @@ class DDIMHeadBase(nn.Module):
         return EngineKey(batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)),
                          self.diffusion_inference_steps, self.use_cuda_graph, native,
                          tuple(image_hw) if image_hw is not None else None, bool(self.return_intermediates),
-                         native and bool(self.producer_train_bn), bool(backward), bool(loop_backward), tuple(drop_path))
+                         native and bool(self.producer_train_bn), bool(backward), bool(loop_backward), tuple(drop_path),
+                         self._codec_kind())
 
     def _mpvit_native_train(self, image_hw, backbone):
         """Whether the engine running this backbone also runs it in training mode (stochastic depth included)."""
@@ -614,10 +644,14 @@ class DDIMHeadBase(nn.Module):
                                drop[0] if drop else ())
         eng = self._engines.get(key)
         if eng is None:
+            if key.codec_kind != 0 and self.variant == "res" and tuple(cond_hw) != tuple(latent_hw):
+                raise EngineError(f"{type(self.depth_transform).__name__}: the Res denoiser adds the condition map "
+                                  f"{tuple(cond_hw)} to the latent {tuple(latent_hw)} without resampling")
             pool = self._pools.setdefault(str(device), WorkspacePool(device))
             eng = DenoiseEngine(self.variant, batch, latent_hw, cond_hw, key.steps, device, cuda_graph=key.cuda_graph,
                                 check_range=False, step_decode=key.step_decode, workspace_pool=pool,
-                                backward=key.backward, loop_backward=key.loop_backward, producer_train=key.producer_train)
+                                backward=key.backward, loop_backward=key.loop_backward, producer_train=key.producer_train,
+                                codec_kind=key.codec_kind)
             if native:
                 eng.enable_producers(feats[0], feats[1], has_neck=self.has_neck)
             if image_hw is not None:
@@ -806,6 +840,7 @@ class DDIMHeadBase(nn.Module):
         differentiable `cond` to the operator itself, `self.model(noisy, t, cond)`, whose backward also returns d_cond.
         With `grad_through_loop = True`, `pred` and the final latent are differentiable too (denoiser and decoder
         parameters, through every step: `_LoopFunction`)."""
+        self._check_codec_trains()
         if self.bn_sync_group is not None and self.return_intermediates:
             raise EngineError("bn_sync_group is not supported by the *Vis heads (their step decodes run in one CUDA graph)")
         with_backbone = fp is None
@@ -824,8 +859,7 @@ class DDIMHeadBase(nn.Module):
             fp = [f.contiguous().float() for f in fp]
             B, dev, dtype = fp[0].shape[0], fp[0].device, fp[0].dtype
             native = self.native_producers and fp[0].is_cuda and self._pyramid_ok(fp)
-        Hd, Wd = gt_depth_map.shape[-2:]
-        latent_hw = ((Hd + 1) // 2, (Wd + 1) // 2)  # shape of depth_transform.t(gt): conv3x3 stride 2 pad 1
+        latent_hw = tuple(self.depth_transform.latent_hw(gt_depth_map.shape[-2:]))  # shape of depth_transform.t(gt)
         gt_map_t = None
         enc_grad = None  # (keys, parameters) when gt_map_t is differentiable
         if self.grad_through_encoder and torch.is_grad_enabled():

@@ -101,11 +101,27 @@ enum dd_flags {
                                    an engine without the flag. */
 };
 
+/* The depth codec (`depth_transform_cfg` of the reference heads, src/model/ops/depth_transform.py), carried in flag bits
+ * DD_FLAG_CODEC_SHIFT .. +1 (kind << DD_FLAG_CODEC_SHIFT).  It fixes the latent grid of an H x W depth map and the
+ * upsampling u of the decoder (decoded map [B,1,u h,u w]):
+ *   DD_CODEC_UP2      DeepDepthTransformWithUpsampling (:10-35)     latent ceil(H/2) x ceil(W/2),           u = 2
+ *   DD_CODEC_UP2_1X1  DeepDepthTransformWithUpsampling1x1 (:38-64)  latent ceil(H/2) x ceil(W/2),           u = 2
+ *   DD_CODEC_UP4      DeepDepthTransformWithUpsamplingX4 (:67-94)   latent ceil(ceil(H/2)/2) (each side),   u = 4
+ *   DD_CODEC_FULL     DeepDepthTransform (:97-117)                  latent H x W,                           u = 1
+ * dd_set_weight takes the kind's `depth_transform.*` keys and rejects the other kinds'; dd_finalize_weights needs the
+ * decoder's, the encoder's stay optional.  Kinds other than DD_CODEC_UP2 run with eval-mode BatchNorm only: they
+ * answer dd_set_codec_mode(DD_CODEC_TRAIN), dd_encode_backward and dd_decode_backward with DD_ERR_UNSUPPORTED, and
+ * dd_create refuses them with DD_FLAG_LOOP_BACKWARD.  dd_denoiser_forward / dd_denoiser_backward do not involve the
+ * codec. */
+enum dd_codec_kind { DD_CODEC_UP2 = 0, DD_CODEC_UP2_1X1 = 1, DD_CODEC_UP4 = 2, DD_CODEC_FULL = 3 };
+#define DD_FLAG_CODEC_SHIFT 12
+
 typedef struct dd_config {
   int32_t abi_version;          /* must be DD_ABI_VERSION */
   int32_t variant;              /* enum dd_variant */
   int32_t batch;                /* images per call on this device */
-  int32_t latent_h, latent_w;   /* h = ceil(H/2), w = ceil(W/2): shape of depth_transform.t(gt) */
+  int32_t latent_h, latent_w;   /* shape of depth_transform.t(gt): h = ceil(H/2), w = ceil(W/2) for the default
+                                   codec (dd_codec_kind: ceil(ceil(H/2)/2) for DD_CODEC_UP4, H for DD_CODEC_FULL) */
   int32_t cond_h, cond_w;       /* spatial size of the FPN condition map x (256 channels) */
   int32_t num_inference_steps;  /* T */
   int32_t device;               /* CUDA ordinal */
@@ -233,14 +249,15 @@ int dd_run_backbone(dd_handle h, const float* rgb, float* const* feats_out, void
 size_t dd_workspace_bytes(dd_handle h);
 
 /* cond [B,256,cond_h,cond_w], noise [B,16,h,w] -> latent_out [B,16,h,w] (nullable),
- * logit_out [B,1,2h,2w] (nullable; the decoder's pre-sigmoid z), depth_out [B,1,2h,2w].
+ * logit_out [B,1,u h,u w] (nullable; the decoder's pre-sigmoid z), depth_out [B,1,u h,u w]; u = 2 for the default
+ * codec (dd_codec_kind).
  * cond may be NULL right after dd_build_condition. */
 int dd_denoise_decode(dd_handle h, const float* cond, const float* noise, float* latent_out, float* logit_out,
                       float* depth_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* The *Vis heads' variant (reference src/model/head/ddim_depth_estimate_res_swin_addHAHI_vis.py:130-149, pipeline
  * :289-304 `image_list`): same loop, and `inv_t` of the latent after EVERY step, all inside the captured graph.
- * depth_steps_out [T][B,1,2h,2w] (slice T-1 is the final `pred`); latent_out / logit_out (nullable) refer to the
+ * depth_steps_out [T][B,1,u h,u w] (slice T-1 is the final `pred`); latent_out / logit_out (nullable) refer to the
  * final step.  Needs DD_FLAG_STEP_DECODE at dd_create. */
 int dd_denoise_decode_steps(dd_handle h, const float* cond, const float* noise, float* latent_out, float* logit_out,
                             float* depth_steps_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
@@ -306,7 +323,7 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
                         float* d_cond_out, float* d_noise_out, float* const* d_params, float* const* d_dec_params,
                         float* latents_out, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
-/* depth = inv_t(latent): latent [B,16,h,w] -> logit_out (nullable), depth_out [B,1,2h,2w]. */
+/* depth = inv_t(latent): latent [B,16,h,w] -> logit_out (nullable), depth_out [B,1,u h,u w] (dd_codec_kind). */
 int dd_decode(dd_handle h, const float* latent, float* logit_out, float* depth_out, void* workspace,
               size_t workspace_bytes, void* cuda_stream);
 
@@ -316,7 +333,8 @@ int dd_decode_backward(dd_handle h, const float* latent, const float* d_depth, f
                        float* const* d_dec_params, void* workspace, size_t workspace_bytes, void* cuda_stream);
 
 /* latent = depth_transform.t(depth) (reference src/model/ops/depth_transform.py:29-31): depth [B,1,height,width] ->
- * latent_out [B,16,ceil(height/2),ceil(width/2)].  Needs the optional keys `depth_transform.conv_transform.*`. */
+ * latent_out [B,16,ceil(height/2),ceil(width/2)] (other codec kinds: their latent grid, dd_codec_kind).  Needs the
+ * optional keys `depth_transform.conv_transform.*`. */
 int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, void* cuda_stream);
 
 /* Backward of dd_encode in the current codec mode: d_latent [B,16,ceil(height/2),ceil(width/2)] -> d_enc_params[0..5]
@@ -562,6 +580,12 @@ int dd_bench_conv(dd_handle h, int32_t cin, int32_t cout, int32_t iters, float* 
  * CUDA events; average milliseconds per pair in *ms_out.  DD_ERR_UNSUPPORTED when the engine runs the chain. */
 int dd_bench_pred_fold(dd_handle h, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,
                        void* cuda_stream);
+
+/* Time the codec's decoder kernel alone (decoder_kernel, or the UP4 / FULL kind's own) `iters` times with CUDA events
+ * on `cuda_stream`, decoding the latent the workspace holds from the last call into depth_out [B,1,u h,u w]; average
+ * milliseconds per launch in *ms_out. */
+int dd_bench_decoder(dd_handle h, float* depth_out, int32_t iters, float* ms_out, void* workspace, size_t workspace_bytes,
+                     void* cuda_stream);
 
 /* Tuning aid: average milliseconds per launch of the GEMM-mode kernel (tokens [M,K] x weights [N,K]^T) on
  * synthetic operands.  mode 0: fp32 out, 1: fp32 out + residual add, 2: GELU -> fp16 planes, 3: no output. */
