@@ -41,7 +41,7 @@ class DDConvGnDesc(C.Structure):
                                          "up_qpb")] + [("c_x", C.c_float), ("c_eps", C.c_float)]
 
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 VARIANT_RES, VARIANT_SWIN = 0, 1
 FLAG_CUDA_GRAPH, FLAG_SIMT_CONV, FLAG_CHECK_RANGE, FLAG_HALO_CONV, FLAG_SWAP_NARROW, FLAG_PAIR_WIDE = 1, 2, 4, 8, 16, 32
 FLAG_STEP_DECODE, FLAG_FP8_CORR, FLAG_BACKWARD, FLAG_LOOP_BACKWARD = 64, 128, 256, 512
@@ -67,6 +67,9 @@ SIGNATURES = {
     "dd_graph_capture_count": (C.c_int64, [C.c_void_p]),
     "dd_set_schedule": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_double),
                                   C.POINTER(C.c_double), C.c_int32]),
+    "dd_set_schedule_eta": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_double),
+                                      C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int32]),
+    "dd_set_step_io": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "dd_workspace_bytes": (C.c_size_t, [C.c_void_p]),
     "dd_enable_producers": (C.c_int, [C.c_void_p, C.POINTER(DDProducerConfig)]),
     "dd_enable_backbone": (C.c_int, [C.c_void_p, C.POINTER(DDBackboneConfig)]),

@@ -535,7 +535,13 @@ struct dd_engine {
   std::vector<void*> owned;
   // schedule
   std::vector<int64_t> ts;
-  std::vector<float> cx, ce;
+  std::vector<float> cx, ce, sg;  // sg: sigma_t of a stochastic schedule (dd_set_schedule_eta), all 0 for eta = 0
+  bool stochastic = false;        // some sg[i] != 0
+  // dd_set_step_io's borrowed pointers for the next dd_denoise_decode(_steps), and the device slot the noise kernel
+  // reads the noise base from (engine-owned, outside `owned`: it survives a re-pack)
+  const float* z_host = nullptr;
+  float* lat_steps = nullptr;
+  const float** z_slot = nullptr;
   // workspace views
   void* ws = nullptr;
   float *x32 = nullptr, *Y = nullptr, *cond = nullptr, *mr[4] = {}, *temb_sel = nullptr;
@@ -1108,7 +1114,7 @@ int run_fold(dd_engine* e, cudaStream_t st) {
   return launched(e, "ring_fix");
 }
 
-int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st);
+int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st, float sg = 0.f, size_t z_off = 0);
 
 // pred.4's GroupNorm + ReLU fused with the DDIM update over B images of f.P pixels; the caller checks the launch.
 void launch_final(const dd::FinalArgs& f, int B, cudaStream_t st) {
@@ -1116,8 +1122,10 @@ void launch_final(const dd::FinalArgs& f, int B, cudaStream_t st) {
   dd::gn_relu_ddim_kernel<<<grid, 256, 0, st>>>(f);
 }
 
-// One ScheduledCNNRefine.forward + (optionally) the DDIM update.
-int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float ce, float* eps_out, cudaStream_t st) {
+// One ScheduledCNNRefine.forward + (optionally) the DDIM update; sg != 0: plus sg times the [B][16][P] slice at z_off of
+// the noise e->z_slot points to.
+int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float ce, float* eps_out, cudaStream_t st,
+             float sg = 0.f, size_t z_off = 0) {
   const Geom g = geom_of(e->cfg);
   int rc;
   // noise_embedding.0 : x (16) -> 64, GN stats
@@ -1137,7 +1145,7 @@ int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float 
     if (fold_active(e)) {  // convB + pred.0 as one composed conv + its ring correction
       if ((rc = run_fold(e, st))) return rc;
       if ((rc = run_finalize(e, 2, 64, st, e->stats[3], ring_blocks_per_img(g)))) return rc;
-      return run_tail(e, cx, ce, eps_out, st);
+      return run_tail(e, cx, ce, eps_out, st, sg, z_off);
     }
     if ((rc = run_conv(e, 3, e->S_hi[0], e->S_lo[0], kActScale, dd::EPI_SPLIT, nullptr, nullptr, e->S_hi[1], e->S_lo[1], st)))
       return rc;
@@ -1151,11 +1159,11 @@ int run_step(dd_engine* e, const float* temb, int temb_bstride, float cx, float 
   // pred.0 : 256 -> 64, GN stats
   if ((rc = run_conv(e, 4, p_hi, p_lo, kActScale, dd::EPI_F32_STATS, e->Y, e->stats[2], nullptr, nullptr, st))) return rc;
   if ((rc = run_finalize(e, 2, 64, st))) return rc;
-  return run_tail(e, cx, ce, eps_out, st);
+  return run_tail(e, cx, ce, eps_out, st, sg, z_off);
 }
 
 // pred.0's GroupNorm + ReLU, pred.3 and its GroupNorm + ReLU, and the DDIM update (Y holds pred.0's output).
-int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st) {
+int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st, float sg, size_t z_off) {
   const Geom g = geom_of(e->cfg);
   int rc;
   if ((rc = run_apply<64, 0>(e, 2, nullptr, 0, e->S_hi[0], e->S_lo[0], st))) return rc;
@@ -1176,8 +1184,12 @@ int run_tail(dd_engine* e, float cx, float ce, float* eps_out, cudaStream_t st) 
   f.scale = kXScale;
   f.P = g.P;
   f.status = e->status;
-  launch_final(f, g.B, st);
-  return launched(e, "gn_relu_ddim");
+  if (sg == 0.f) {
+    launch_final(f, g.B, st);
+    return launched(e, "gn_relu_ddim");
+  }
+  dd::gn_relu_ddim_noise_kernel<<<dim3((f.P * 4 + 255) / 256, g.B), 256, 0, st>>>(f, e->z_slot, z_off, sg);
+  return launched(e, "gn_relu_ddim_noise");
 }
 
 // The layout changes and the latent split leave counting their launch to their callers.
@@ -2989,6 +3001,7 @@ void release(dd_engine* e) {
   cudaSetDevice(e->cfg.device);
   drop_graphs(e);
   for (void* p : e->owned) cudaFree(p);
+  if (e->z_slot) cudaFree(e->z_slot);
   free_bn_sync(e);
   if (e->status_host) cudaFreeHost(e->status_host);
   if (e->stage) cudaFreeHost(e->stage);
@@ -3222,18 +3235,49 @@ int dd_update_weights(dd_handle h, void* cuda_stream) {
 
 int64_t dd_graph_capture_count(dd_handle h) { return h ? h->graph_captures : 0; }
 
-int dd_set_schedule(dd_handle h, const int64_t* timesteps, const double* c_x, const double* c_eps, int32_t n) {
+int dd_set_schedule_eta(dd_handle h, const int64_t* timesteps, const double* c_x, const double* c_eps,
+                        const double* sigma, int32_t n) {
   if (!h || !timesteps || !c_x || !c_eps) return fail(DD_ERR_INVALID, "null argument");
   if (n != h->cfg.num_inference_steps) return fail(DD_ERR_INVALID, "schedule length != num_inference_steps");
+  bool stochastic = false;
+  for (int i = 0; i < n; ++i) {
+    if (timesteps[i] < 0 || timesteps[i] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
+    if (sigma && !(sigma[i] >= 0.0 && isfinite(sigma[i]))) return fail(DD_ERR_INVALID, "sigma must be finite and >= 0");
+    stochastic = stochastic || (sigma && static_cast<float>(sigma[i]) != 0.f);
+  }
+  if (stochastic && (h->cfg.flags & DD_FLAG_LOOP_BACKWARD))
+    return fail(DD_ERR_UNSUPPORTED, "a schedule with sigma != 0 (eta > 0) on a DD_FLAG_LOOP_BACKWARD engine: the loop "
+                                    "backward does not differentiate a stochastic sample");
+  if (stochastic && !h->z_slot) {
+    if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(DD_ERR_CUDA, "cudaSetDevice failed");
+    const cudaError_t err = cudaMalloc(reinterpret_cast<void**>(&h->z_slot), sizeof(float*));
+    if (err != cudaSuccess) {
+      h->z_slot = nullptr;
+      return fail(DD_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(err));
+    }
+  }
   h->ts.assign(timesteps, timesteps + n);
   h->cx.resize(n);
   h->ce.resize(n);
+  h->sg.assign(n, 0.f);
   for (int i = 0; i < n; ++i) {
-    if (timesteps[i] < 0 || timesteps[i] >= DD_TIME_ROWS) return fail(DD_ERR_INVALID, "timestep outside time_embedding");
     h->cx[i] = static_cast<float>(c_x[i]);
     h->ce[i] = static_cast<float>(c_eps[i]);
+    if (sigma) h->sg[i] = static_cast<float>(sigma[i]);
   }
+  h->stochastic = stochastic;
   drop_graphs(h);
+  return DD_OK;
+}
+
+int dd_set_schedule(dd_handle h, const int64_t* timesteps, const double* c_x, const double* c_eps, int32_t n) {
+  return dd_set_schedule_eta(h, timesteps, c_x, c_eps, nullptr, n);
+}
+
+int dd_set_step_io(dd_handle h, const float* variance_noise, float* latent_steps_out) {
+  if (!h) return fail(DD_ERR_INVALID, "null handle");
+  h->z_host = variance_noise;
+  h->lat_steps = latent_steps_out;
   return DD_OK;
 }
 
@@ -3244,7 +3288,15 @@ size_t dd_workspace_bytes(dd_handle h) { return h ? carve(h, nullptr) : 0; }
 static int denoise_impl(dd_handle h, const float* cond, const float* noise, float* latent_out, float* logit_out,
                         float* depth_out, float* depth_steps_out, void* workspace, size_t workspace_bytes,
                         void* cuda_stream) {
-  if (!h || !noise || (!depth_out && !depth_steps_out)) return fail(DD_ERR_INVALID, "null argument");
+  if (!h) return fail(DD_ERR_INVALID, "null argument");
+  // dd_set_step_io's pointers serve this call only
+  const float* z = h->z_host;
+  float* lat_steps = h->lat_steps;
+  h->z_host = nullptr;
+  h->lat_steps = nullptr;
+  if (!noise || (!depth_out && !depth_steps_out)) return fail(DD_ERR_INVALID, "null argument");
+  if (h->stochastic && !z)
+    return fail(DD_ERR_INVALID, "the schedule has sigma != 0 (eta > 0) but no variance noise was given (dd_set_step_io)");
   if (!cond && !h->cond_ready) return fail(DD_ERR_INVALID, "cond is NULL but dd_build_condition has not run");
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   if (static_cast<int>(h->ts.size()) != h->cfg.num_inference_steps) return fail(DD_ERR_INVALID, "dd_set_schedule has not been called");
@@ -3271,16 +3323,26 @@ static int denoise_impl(dd_handle h, const float* cond, const float* noise, floa
     return fail(DD_ERR_UNSUPPORTED, "dd_denoise_decode_steps in DD_CODEC_TRAIN does not run with a BatchNorm all-gather "
                                     "installed (dd_set_bn_allgather)");
   h->ct.nrec = 0;
+  const size_t nx = static_cast<size_t>(g.B) * 16 * g.P;  // one latent / one step's noise
+  if (h->stochastic) {  // the kernels read the noise's base from z_slot: set it, in stream order, before the loop runs
+    dd::set_ptr_kernel<<<1, 1, 0, st>>>(h->z_slot, z);
+    if ((rc = launched(h, "set_ptr"))) return rc;
+  }
   auto loop = [&](cudaStream_t s) -> int {
     for (int i = 0; i < T; ++i) {
-      int r = run_step(h, h->temb + h->ts[i] * 256, 0, h->cx[i], h->ce[i], nullptr, s);
+      int r = run_step(h, h->temb + h->ts[i] * 256, 0, h->cx[i], h->ce[i], nullptr, s, h->sg[i], i * nx);
       if (r == DD_OK && steps && train) r = run_dec_batch_stats(h, h->ct.rec + i * 32, s);
       if (r == DD_OK && steps) r = run_decoder(h, nullptr, h->inter + i * map_elems, s);
+      if (r == DD_OK && lat_steps) {
+        r = transpose_out(h->x32, lat_steps + i * nx, g.B, 16, g.P, s);
+        h->launches++;
+      }
       if (r != DD_OK) return r;
     }
     return DD_OK;
   };
-  if (h->cfg.flags & DD_FLAG_CUDA_GRAPH) {
+  // every latent out to a caller buffer: launched eagerly (a graph holds no caller pointer)
+  if ((h->cfg.flags & DD_FLAG_CUDA_GRAPH) && !lat_steps) {
     const int which = steps ? (train ? dd_engine::G_LOOP_STEPS_TRAIN : dd_engine::G_LOOP_STEPS) : dd_engine::G_LOOP;
     if ((rc = graph_run(h, which, st, loop))) return rc;
   } else if ((rc = loop(st))) {
@@ -3412,6 +3474,7 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
   if (!h->weights_ready) return fail(DD_ERR_INVALID, "dd_finalize_weights has not been called");
   const int T = h->cfg.num_inference_steps;
   if (static_cast<int>(h->ts.size()) != T) return fail(DD_ERR_INVALID, "dd_set_schedule has not been called");
+  if (h->stochastic) return fail(DD_ERR_UNSUPPORTED, "dd_denoise_backward: the schedule has sigma != 0 (eta > 0)");
   const Geom g = geom_of(h->cfg);
   if (static_cast<size_t>(g.B) * g.P * 256 > static_cast<size_t>(INT32_MAX))
     return fail(DD_ERR_UNSUPPORTED, "batch x latent too large for one backward call");

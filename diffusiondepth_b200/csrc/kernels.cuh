@@ -446,6 +446,7 @@ __global__ void __launch_bounds__(QPB * 256 / V, 12 / QPB) gn_apply_up_split_ker
 // eps = relu(gn(y6));  x <- c_x * x + c_eps * eps   (reference scheduling_ddim.py:285-326 with eta = 0,
 // collapsed; SURVEY.md §3.3).  Also refreshes the fp16 planes of x for the next step's first conv.
 // If eps_out != nullptr, only eps is written (bare denoiser call) and x is left untouched.
+// gn_relu_ddim_noise_kernel is the eta > 0 step: x <- c_x * x + c_eps * eps + sigma * z, z the caller's variance noise.
 struct FinalArgs {
   const float* y;          // [B][P][16]
   const float* mean_rstd;  // [B][4][2]
@@ -459,7 +460,8 @@ struct FinalArgs {
   int P;
   int* status;
 };
-__global__ void __launch_bounds__(256) gn_relu_ddim_kernel(const FinalArgs a) {
+template <bool NOISE>
+__device__ __forceinline__ void gn_relu_ddim(const FinalArgs& a, const float* z, float sigma) {
   const int b = blockIdx.y;
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;  // float4 index within image
   if (i >= static_cast<size_t>(a.P) * 4) return;
@@ -482,18 +484,34 @@ __global__ void __launch_bounds__(256) gn_relu_ddim_kernel(const FinalArgs a) {
   }
   const float4 xv = reinterpret_cast<const float4*>(a.x)[o4];
   float xn[4] = {xv.x, xv.y, xv.z, xv.w};
+  float zn[4];
+  if constexpr (NOISE) {  // z is NCHW [B][16][P]: channel 4g + j of pixel i / 4, coalesced across the warp's pixels
+    const float* zp = z + (static_cast<size_t>(b) * 16 + 4 * g) * a.P + (i >> 2);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) zn[j] = __ldcs(zp + static_cast<size_t>(j) * a.P);
+  }
   bool ov = false;
   __align__(8) __half h[4];
   __align__(8) __half l[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     xn[j] = a.cx * xn[j] + a.ce * e[j];
+    if constexpr (NOISE) xn[j] = fmaf(sigma, zn[j], xn[j]);
     split_f16(xn[j], a.scale, h[j], l[j], ov);
   }
   reinterpret_cast<float4*>(a.x)[o4] = make_float4(xn[0], xn[1], xn[2], xn[3]);
   reinterpret_cast<uint2*>(a.x_hi)[o4] = *reinterpret_cast<const uint2*>(h);
   reinterpret_cast<uint2*>(a.x_lo)[o4] = *reinterpret_cast<const uint2*>(l);
   if (ov) atomicOr(a.status, 1);
+}
+__global__ void __launch_bounds__(256) gn_relu_ddim_kernel(const FinalArgs a) { gn_relu_ddim<false>(a, nullptr, 0.f); }
+// One pointer into device memory, written in stream order (the noise slot below).
+__global__ void set_ptr_kernel(const float** slot, const float* p) { *slot = p; }
+// z_slot: device memory holding the base of the caller's [T][B][16][P] noise, written by the call before the (possibly
+// graph-captured) loop runs; z_off selects this step's [B][16][P] slice.
+__global__ void __launch_bounds__(256) gn_relu_ddim_noise_kernel(const FinalArgs a, const float* const* z_slot,
+                                                                 size_t z_off, float sigma) {
+  gn_relu_ddim<true>(a, *z_slot + z_off, sigma);
 }
 
 // ------------------------------------------------------------------ fp32 CUDA-core 3x3 conv (validation / DD_FLAG_SIMT_CONV)

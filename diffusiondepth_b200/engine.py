@@ -257,10 +257,15 @@ class DenoiseEngine:
         self.backbone = (tuple(image_hw), int(embed_dims))
         self._ws = None
 
-    def set_schedule(self, timesteps, c_x, c_eps):
+    def set_schedule(self, timesteps, c_x, c_eps, sigma=None):
+        """The loop's timesteps and fp64 step coefficients (`DDIMScheduler.fused_coefficients`); `sigma` (per step,
+        optional) makes it the stochastic step of eta > 0, which needs `variance_noise` on every denoise call."""
         n = len(timesteps)
-        _cabi.check(self.lib.dd_set_schedule(self._h, (C.c_int64 * n)(*[int(t) for t in timesteps]),
-                                             (C.c_double * n)(*c_x), (C.c_double * n)(*c_eps), n))
+        ts, cx, ce = (C.c_int64 * n)(*[int(t) for t in timesteps]), (C.c_double * n)(*c_x), (C.c_double * n)(*c_eps)
+        if sigma is None:
+            _cabi.check(self.lib.dd_set_schedule(self._h, ts, cx, ce, n))
+        else:
+            _cabi.check(self.lib.dd_set_schedule_eta(self._h, ts, cx, ce, (C.c_double * n)(*sigma), n))
 
     # ---------------------------------------------------------------- calls
     def _stream(self) -> int:
@@ -316,9 +321,21 @@ class DenoiseEngine:
         _cabi.check(self.lib.dd_build_condition(self._h, ptrs, _ptr(cond), *self._ws_args()))
         return cond
 
-    def denoise_decode(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False, want_logits=False):
+    def _step_io(self, variance_noise: Optional[torch.Tensor], latent_steps: Optional[torch.Tensor]):
+        """dd_set_step_io for the next denoise call: the [T,B,16,h,w] noise of a stochastic schedule and / or the
+        buffer that receives the latent after every step."""
+        shape = (self.steps, self.batch, 16, *self.latent_hw)
+        for t in (variance_noise, latent_steps):
+            if t is not None:
+                self._check_in(t, shape)
+        _cabi.check(self.lib.dd_set_step_io(self._h, _ptr(variance_noise), _ptr(latent_steps)))
+
+    def denoise_decode(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False, want_logits=False,
+                       variance_noise: Optional[torch.Tensor] = None, latent_steps: Optional[torch.Tensor] = None):
         """cond [B,256,hc,wc] (or None right after build_condition), noise [B,16,h,w] -> depth [B,1,u h,u w]
-        (u = `self.up`, the codec's upsampling; + latent [B,16,h,w], logits)."""
+        (u = `self.up`, the codec's upsampling; + latent [B,16,h,w], logits).  `variance_noise` [T,B,16,h,w]: z_t of
+        every step, required by a schedule set with sigma (eta > 0); `latent_steps` [T,B,16,h,w] (optional) receives
+        the latent after every step (the call then runs without its CUDA graph)."""
         B, (h, w), u = self.batch, self.latent_hw, self.up
         if cond is not None:
             self._check_in(cond, (B, 256, *self.cond_hw))
@@ -326,12 +343,13 @@ class DenoiseEngine:
         depth = torch.empty(B, 1, u * h, u * w, device=self.device, dtype=torch.float32)
         latent = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32) if want_latent else None
         logits = torch.empty_like(depth) if want_logits else None
+        self._step_io(variance_noise, latent_steps)
         _cabi.check(self.lib.dd_denoise_decode(self._h, _ptr(cond), _ptr(noise), _ptr(latent), _ptr(logits), _ptr(depth),
                                                *self._ws_args()))
         return depth, latent, logits
 
     def denoise_decode_steps(self, cond: Optional[torch.Tensor], noise: torch.Tensor, want_latent=False,
-                             want_logits=False):
+                             want_logits=False, variance_noise: Optional[torch.Tensor] = None):
         """As `denoise_decode`, additionally decoding the latent after every step inside the captured graph (the *Vis
         heads' `pred_inter`): returns (depth_steps [T,B,1,u h,u w], latent, logits of the final step)."""
         if not self.step_decode:
@@ -343,6 +361,7 @@ class DenoiseEngine:
         steps = torch.empty(self.steps, B, 1, u * h, u * w, device=self.device, dtype=torch.float32)
         latent = torch.empty(B, 16, h, w, device=self.device, dtype=torch.float32) if want_latent else None
         logits = torch.empty(B, 1, u * h, u * w, device=self.device, dtype=torch.float32) if want_logits else None
+        self._step_io(variance_noise, None)
         _cabi.check(self.lib.dd_denoise_decode_steps(self._h, _ptr(cond), _ptr(noise), _ptr(latent), _ptr(logits),
                                                      _ptr(steps), *self._ws_args()))
         return steps, latent, logits

@@ -66,8 +66,11 @@ class DDIMScheduler:
         a_t, a_prev = self._alpha_pair(timestep, prev_timestep)
         return ((1 - a_prev) / (1 - a_t)) * (1 - a_t / a_prev)
 
-    def fused_coefficients(self, num_inference_steps=None):
-        """(timesteps, c_x, c_eps) for eta = 0 / epsilon prediction / no clipping, fp64 from the fp32 table."""
+    def fused_coefficients(self, num_inference_steps=None, eta=None):
+        """(timesteps, c_x, c_eps) for eta = 0 / epsilon prediction / no clipping, fp64 from the fp32 table.  With
+        `eta` given, (timesteps, c_x, c_eps, sigma) of `step(..., eta, use_clipped_model_output=True)` collapsed to
+        x_{t-1} = c_x x_t + c_eps eps + sigma z:  sigma = eta sqrt(variance), c_eps = sqrt(1 - a_prev - sigma^2) -
+        sqrt(a_prev (1 - a_t) / a_t); at eta = 0 the first three lists are those of the call without eta."""
         if num_inference_steps is not None:
             self.set_timesteps(num_inference_steps)
         if self._cfg["prediction_type"] != "epsilon" or self._cfg["clip_sample"]:
@@ -75,13 +78,18 @@ class DDIMScheduler:
                                       "(prediction_type='epsilon', clip_sample=False)")
         stride = self._cfg["num_train_timesteps"] // self.num_inference_steps
         acp = self.alphas_cumprod.to("cpu", torch.float64)
-        ts, cx, ce = [int(t) for t in self.timesteps.tolist()], [], []
+        ts, cx, ce, sg = [int(t) for t in self.timesteps.tolist()], [], [], []
+        e = float(eta or 0.0)
+        if e < 0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
         for t in ts:
             a_t = float(acp[t])
             a_p = float(acp[t - stride]) if t - stride >= 0 else float(self.final_alpha_cumprod)
+            s = e * math.sqrt((1.0 - a_p) / (1.0 - a_t) * (1.0 - a_t / a_p))
             cx.append(math.sqrt(a_p / a_t))
-            ce.append(math.sqrt(1.0 - a_p) - math.sqrt(a_p * (1.0 - a_t) / a_t))
-        return ts, cx, ce
+            ce.append((math.sqrt(1.0 - a_p) if e == 0 else math.sqrt(1.0 - a_p - s * s)) - math.sqrt(a_p * (1.0 - a_t) / a_t))
+            sg.append(s)
+        return (ts, cx, ce) if eta is None else (ts, cx, ce, sg)
 
     # -- one reverse step (torch; API parity with the reference, not on the CUDA hot path) -----------------
     def step(self, model_output, timestep, sample, eta=0.0, use_clipped_model_output=False, generator=None,

@@ -15,7 +15,7 @@ import collections
 import copy
 import threading
 import weakref
-from typing import Dict, NamedTuple, Optional, Tuple
+from typing import Dict, NamedTuple, Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
@@ -73,6 +73,7 @@ class EngineKey(NamedTuple):
     drop_path: Tuple[int, ...] = ()       # native backbone with stochastic depth: per stage, the bit mask of its MPViT
                                           # layers / Swin blocks (dd_backbone_config.mp_drop_path)
     codec_kind: int = 0                   # the depth codec's dd_codec_kind (`depth_transform.ENGINE_KIND`)
+    eta: float = 0.0                      # the DDIM step's eta (> 0: `pipeline(eta=...)`, the stochastic schedule)
 
     @property
     def geometry(self):
@@ -361,6 +362,15 @@ class DDIMHeadBase(nn.Module):
         replica.__dict__['_backbone_ref'] = None
         return replica
 
+    @property
+    def pipeline(self) -> "CNNDDIMPipiline":
+        """The reference's sampler object (`self.pipeline = CNNDDIMPipiline(self.model, self.scheduler)`, head :49),
+        built on each access: it holds nothing but this head's `model` and `scheduler`, so deep copies and DataParallel
+        replicas get their own."""
+        pipe = CNNDDIMPipiline(self.model, self.scheduler, image_list=self.return_intermediates)
+        pipe._head = self
+        return pipe
+
     # ------------------------------------------------------------------------------------------ engine bridge
     def _engine_tensors(self):
         sd = {}
@@ -588,23 +598,24 @@ class DDIMHeadBase(nn.Module):
         return tensors
 
     def _engine(self, batch, latent_hw, cond_hw, device, feats=None, image_hw=None, backbone=None,
-                backward=False, loop_backward=False, producer_train=False) -> DenoiseEngine:
+                backward=False, loop_backward=False, producer_train=False, steps=None, eta=0.0) -> DenoiseEngine:
         """feats: backbone feature maps, or a (channels, sizes) pyramid spec -> native neck/FPN;
         image_hw: additionally run the backbone natively (`backbone`: the module holding its parameters);
         backward: an engine that also serves `denoiser_backward`; loop_backward: one that also serves
         `denoise_backward` / `decode_backward` (and `denoiser_backward`); producer_train: this forward runs a producer
-        BatchNorm in training mode (the eval producer pack may then lag behind their running statistics)."""
+        BatchNorm in training mode (the eval producer pack may then lag behind their running statistics); steps, eta:
+        the schedule (default: the head's own steps, eta = 0)."""
         with self._lock:
             return self._engine_locked(batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
-                                       loop_backward, producer_train)
+                                       loop_backward, producer_train, steps, eta)
 
     def _engine_key(self, batch, latent_hw, cond_hw, device, native=False, image_hw=None, backward=False,
-                    loop_backward=False, drop_path=()) -> EngineKey:
+                    loop_backward=False, drop_path=(), steps=None, eta=0.0) -> EngineKey:
         return EngineKey(batch, tuple(latent_hw), tuple(cond_hw), str(torch.device(device)),
-                         self.diffusion_inference_steps, self.use_cuda_graph, native,
+                         int(steps or self.diffusion_inference_steps), self.use_cuda_graph, native,
                          tuple(image_hw) if image_hw is not None else None, bool(self.return_intermediates),
                          native and bool(self.producer_train_bn), bool(backward), bool(loop_backward), tuple(drop_path),
-                         self._codec_kind())
+                         self._codec_kind(), float(eta))
 
     def _mpvit_native_train(self, image_hw, backbone):
         """Whether the engine running this backbone also runs it in training mode (stochastic depth included)."""
@@ -634,14 +645,14 @@ class DDIMHeadBase(nn.Module):
         return self._engine(batch, latent_hw, cond_hw, device, backward=not loop, loop_backward=loop)
 
     def _engine_locked(self, batch, latent_hw, cond_hw, device, feats, image_hw, backbone, backward,
-                       loop_backward, producer_train=False) -> DenoiseEngine:
+                       loop_backward, producer_train=False, steps=None, eta=0.0) -> DenoiseEngine:
         native = feats is not None
         if native and not isinstance(feats, tuple):
             feats = ([f.shape[1] for f in feats], [tuple(f.shape[-2:]) for f in feats])
         device = torch.device(device)
         drop = self._native_drop_paths(image_hw, backbone)
         key = self._engine_key(batch, latent_hw, cond_hw, device, native, image_hw, backward, loop_backward,
-                               drop[0] if drop else ())
+                               drop[0] if drop else (), steps, eta)
         eng = self._engines.get(key)
         if eng is None:
             if key.codec_kind != 0 and self.variant == "res" and tuple(cond_hw) != tuple(latent_hw):
@@ -663,8 +674,10 @@ class DDIMHeadBase(nn.Module):
                     eng.enable_backbone(image_hw, mp_drop_path=key.drop_path or (0, 0, 0, 0))
                 else:
                     eng.enable_backbone(image_hw, depths=[len(st) for st in self._backbone(backbone).layers], kind="resnet")
-            ts, cx, ce = self.scheduler.fused_coefficients(self.diffusion_inference_steps)
-            eng.set_schedule(ts, cx, ce)
+            if key.eta > 0:
+                eng.set_schedule(*self.scheduler.fused_coefficients(key.steps, eta=key.eta))
+            else:
+                eng.set_schedule(*self.scheduler.fused_coefficients(key.steps))
             self._engines[key] = eng
             self._packed.pop(key, None)
             self._stale.discard(key)
@@ -986,3 +999,64 @@ class DDIMHeadBase(nn.Module):
         return F.mse_loss(self.denoiser(noisy, t, cond), noise)  # == self.model(noisy, t, cond, None, None, None)
 
     ddim_loss = _ddim_loss
+
+
+class CNNDDIMPipiline:
+    """The reference's DDIM sampler (head :244-303; the *Vis heads' copy also returns `image_list`, ..._vis.py:254-306):
+    `pipeline(batch_size, device, dtype, shape, input_args, generator, eta, num_inference_steps, return_dict)` ->
+    `(latent,)` or `{'images': latent}` (Vis: `(latent, image_list)` / `{'images', 'image_list'}`, the latent after
+    every step).  It draws x_T = randn((batch_size, *shape)), then, only when eta > 0, one randn of that shape per step
+    (the reference scheduler's `variance_noise`, the last step's included), each with `generator` when given, and runs
+    the T steps of `scheduler.step(..., eta, use_clipped_model_output=True)` on the head's engine in one call: the
+    condition map `input_args[0]` must be a CUDA tensor and `model` the head's ScheduledCNNRefine.  It returns the
+    latent; decoding it (`depth_transform.inv_t`) is the caller's.  No gradient: under autograd, with the condition
+    map or a denoiser / decoder parameter requiring grad, eta > 0 raises, as does eta = 0 on a head set to
+    `grad_through_loop` (the head's forward is the differentiable path); otherwise the result carries no graph."""
+
+    def __init__(self, model, scheduler, image_list=False):
+        self.model = model
+        self.scheduler = scheduler
+        self.image_list = image_list
+        self._head = None
+
+    def __call__(self, batch_size, device, dtype, shape, input_args, generator: Optional[torch.Generator] = None,
+                 eta: float = 0.0, num_inference_steps: int = 50, return_dict: bool = True,
+                 **kwargs) -> Union[Dict, Tuple]:
+        head = self._head if self._head is not None else (self.model._bridge() if self.model._bridge else None)
+        cond = input_args[0]
+        if head is None or head.model is not self.model or not (torch.is_tensor(cond) and cond.is_cuda):
+            raise EngineError("CNNDDIMPipiline runs on the head's CUDA engine: `model` must be the head's "
+                              "ScheduledCNNRefine and input_args[0] a CUDA condition map")
+        eta = float(eta)
+        if eta < 0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        if torch.is_grad_enabled():
+            _, params = head._denoiser_params()
+            if cond.requires_grad or any(p.requires_grad for p in params):
+                if eta > 0:
+                    raise EngineError(f"CNNDDIMPipiline(eta={eta}) has no backward: a stochastic sample (eta > 0) is "
+                                      "not differentiated; run it under torch.no_grad()")
+                if head.grad_through_loop:
+                    raise EngineError("CNNDDIMPipiline has no backward: with grad_through_loop, train through the "
+                                      "head's forward, or run the pipeline under torch.no_grad()")
+        image_shape = (batch_size, *shape)
+        image = torch.randn(image_shape, generator=generator, device=device, dtype=dtype)
+        self.scheduler.set_timesteps(num_inference_steps)
+        T = len(self.scheduler.timesteps)
+        z = None
+        if eta > 0:
+            z = torch.stack([torch.randn(image_shape, generator=generator, device=device, dtype=dtype)
+                             for _ in range(T)]).float()
+        x_T = image.detach().float().contiguous()
+        eng = head._engine(batch_size, tuple(shape[-2:]), tuple(cond.shape[-2:]), cond.device, steps=T, eta=eta)
+        eng.set_codec_mode(False)
+        steps = torch.empty(T, *x_T.shape, device=x_T.device) if self.image_list else None
+        _, latent, _ = eng.denoise_decode(cond.detach().contiguous().float(), x_T, want_latent=True, variance_noise=z,
+                                          latent_steps=steps)
+        if head.check_range:
+            eng.poll_status()
+        image = latent.to(dtype)
+        if self.image_list:
+            image_list = [s.to(dtype) for s in steps.unbind(0)]
+            return (image, image_list) if not return_dict else {'images': image, 'image_list': image_list}
+        return (image,) if not return_dict else {'images': image}

@@ -16,6 +16,11 @@
  *                                    `DDIMScheduler.step` (src/model/diffusers/schedulers/
  *                                    scheduling_ddim.py:215-229, 285-326) collapsed to
  *                                    x_{t-1} = c_x * x_t + c_eps * eps
+ *   dd_set_schedule_eta           <- the same with `eta` > 0: `DDIMScheduler.step(..., eta,
+ *                                    use_clipped_model_output=True)` (scheduling_ddim.py:285-350) collapsed to
+ *                                    x_{t-1} = c_x * x_t + c_eps * eps + sigma_t * z_t
+ *   dd_set_step_io                <- the per-step `randn` draws of that `step` (:336-345) passed in as
+ *                                    `variance_noise`, and the Vis pipeline's `image_list` (..._vis.py:289-306)
  *   dd_denoise_decode             <- `CNNDDIMPipiline.__call__` (head :254-303) = T x
  *                                    {`ScheduledCNNRefine.forward` (:361-382 / res.py:324-344),
  *                                    `DDIMScheduler.step`} followed by
@@ -55,7 +60,7 @@
 extern "C" {
 #endif
 
-#define DD_ABI_VERSION 2
+#define DD_ABI_VERSION 3
 
 typedef struct dd_engine* dd_handle;
 
@@ -181,6 +186,28 @@ int64_t dd_graph_capture_count(dd_handle h);
 /* Per-step timesteps (descending, as DDIMScheduler.set_timesteps produces) and the collapsed DDIM
  * coefficients; n must equal num_inference_steps. */
 int dd_set_schedule(dd_handle h, const int64_t* timesteps, const double* c_x, const double* c_eps, int32_t n);
+
+/* As dd_set_schedule, for the reference's stochastic DDIM step (`CNNDDIMPipiline.__call__(eta=...)`, head :254-303,
+ * calling `DDIMScheduler.step(..., eta, use_clipped_model_output=True)`, scheduling_ddim.py:285-350, clip_sample
+ * False, epsilon prediction): step i runs x <- c_x[i] x + c_eps[i] eps + sigma[i] z_i with
+ *   sigma = eta sqrt((1 - a_prev) / (1 - a_t) (1 - a_t / a_prev)),
+ *   c_eps = sqrt(1 - a_prev - sigma^2) - sqrt(a_prev (1 - a_t) / a_t),   c_x = sqrt(a_prev / a_t),
+ * computed by the caller in fp64 (DDIMScheduler.fused_coefficients(eta=...)).  sigma NULL or all zero: exactly
+ * dd_set_schedule (the eta = 0 kernels and graphs).  A schedule with a non-zero sigma makes every dd_denoise_decode(_steps)
+ * need the noise of dd_set_step_io (DD_ERR_INVALID without it).  DD_ERR_UNSUPPORTED on an engine created with
+ * DD_FLAG_LOOP_BACKWARD (a stochastic sample is not differentiated); DD_ERR_INVALID for a negative or non-finite sigma.
+ * Either setter drops the loop graphs: the next call captures them again. */
+int dd_set_schedule_eta(dd_handle h, const int64_t* timesteps, const double* c_x, const double* c_eps,
+                        const double* sigma, int32_t n);
+
+/* Borrowed for the next dd_denoise_decode or dd_denoise_decode_steps call only, which then forgets both (NULL: none):
+ *   variance_noise    [T][B,16,h,w] device fp32: z_i of step i (the reference's `variance_noise`, one `randn(shape)`
+ *                     per step in step order, the last step's included); read in place by the loop's kernels, through
+ *                     an engine-owned device slot the call writes before the loop (or its CUDA graph) runs.  Ignored
+ *                     by a schedule without sigma.
+ *   latent_steps_out  [T][B,16,h,w] device fp32: the latent after every step (the Vis pipeline's `image_list`); the
+ *                     call then runs its loop without a CUDA graph. */
+int dd_set_step_io(dd_handle h, const float* variance_noise, float* latent_steps_out);
 
 /* Optional: also run the step-invariant condition producers natively — HAHI neck (attention gates off, as
  * the shipped heads configure it: src/model/necks/hahi.py:165-276) and the FPN (head :112-122) — on the same
