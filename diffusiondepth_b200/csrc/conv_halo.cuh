@@ -17,9 +17,13 @@
 //
 // Roles: warpgroup 0 = producers (warp 0: A strips, warp 1: B weight tiles; one elected lane issues the copies),
 // warpgroups 1 .. NWG = consumers.  Consumer warpgroup w owns all 128 pixels of the tile and output channels
-// [w NW, (w + 1) NW) as two 64-row wgmma accumulators in registers; after the K loop it drains them chunk by chunk
-// through a shared-memory staging tile so that thread t holds row (pixel) t of the chunk for the epilogue (bias,
-// GroupNorm partial sums, fp32 / split-plane stores).
+// [w NW, (w + 1) NW) as two 64-row wgmma accumulators in registers.  After the K loop each consumer warp applies
+// scale and bias (and the fp16 hi/lo split) to its fragments in registers, writes them once into its own store buffer
+// laid out as the NHWC output box (16 pixels x up to 32 channels), and one lane hands the box to a TMA tensor store,
+// which clips it at the image's right and bottom edges.  The warps only wait until a buffer has been read out before
+// writing it again, never on global memory, and need no warpgroup barrier, so the next tile's MMAs start while the
+// stores drain.  GroupNorm partials are summed per pixel from the staged fp32 chunks in column order, then combined
+// in a fixed order (bit-reproducible).
 // Replaces: the nn.Conv2d calls inside ScheduledCNNRefine (reference
 // src/model/head/ddim_depth_estimate_res_swin_addHAHI.py:339-359, UpSample_add :321-333).
 #pragma once
@@ -29,6 +33,8 @@ namespace dd {
 
 constexpr int HALO_TH = 16;  // output tile: 16 rows x 8 columns = 128 pixels
 constexpr int HALO_TW = 8;
+// output channels per TMA store box of the epilogue (the output maps are built with the same box)
+constexpr int halo_out_box_c(int cout) { return cout < 32 ? cout : 32; }
 
 template <int CIN, int COUT, int BK>
 struct HaloCfg {
@@ -50,12 +56,15 @@ struct HaloCfg {
   static constexpr int NWG = COUT > 128 ? 2 : 1;
   static constexpr int NW = COUT / NWG;
   static constexpr int THREADS = 128 * (1 + NWG);
-  // accumulator columns per epilogue chunk.  The two-warpgroup (256-wide) layers drain 16 at a time: the smaller
-  // staging tile (17 KB instead of 33 KB) leaves room for a third weight slot, so the producer runs two taps ahead of
-  // the MMAs instead of one.
-  static constexpr int CH = NWG > 1 ? 16 : (NW < 32 ? NW : 32);
-  static constexpr int LD = CH + 1;                                  // staging row stride (floats): conflict-free rows
-  static constexpr int STAGE_BYTES = NWG * 128 * LD * 4;
+  // Epilogue: each consumer warp stores its 16 fragment rows (two image rows of 8 pixels) in boxes of OC channels,
+  // OUT_BUFS buffers per warp.  A buffer holds one box as fp32, or as the fp16 hi plane followed by the lo plane; a
+  // box row (OC channels of one pixel) is the swizzle span.  The two-warpgroup (256-wide) layers get one buffer per
+  // warp (16 KB in all), which leaves room for a third weight slot, so the producer runs two taps ahead of the MMAs.
+  static constexpr int OC = halo_out_box_c(COUT);
+  static constexpr int OBUF = 16 * OC * 4;
+  static constexpr int OUT_BUFS = NWG > 1 ? 1 : 4;
+  static_assert(NW % OC == 0 && OC % 8 == 0, "a warp's columns are whole store boxes of whole fragment blocks");
+  static constexpr int STAGE_BYTES = NWG * 4 * OUT_BUFS * OBUF;
   static constexpr int CTRL_BYTES = 1024;  // barriers, GroupNorm partials [2][4 NWG][GPW][2] (fp64)
   static constexpr int BUDGET = 227 * 1024 - 1024 - CTRL_BYTES - STAGE_BYTES - A_SLOTS * A_SLOT;
   static constexpr int B_SLOTS_RAW = BUDGET / B_SLOT;
@@ -78,6 +87,7 @@ template <int CIN, int COUT, int BK, int EPI>
 __global__ void __launch_bounds__((HaloCfg<CIN, COUT, BK>::THREADS), 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                     const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
+                    const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1,
                     const ConvArgs p) {
   using C = HaloCfg<CIN, COUT, BK>;
   constexpr int NW = C::NW;
@@ -91,7 +101,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   uint64_t* b_full = a_empty + C::A_SLOTS;
   uint64_t* b_empty = b_full + C::B_SLOTS;
   double* red = reinterpret_cast<double*>(b_empty + C::B_SLOTS);  // [2][4 NWG][GPW][2]
-  float* stage = reinterpret_cast<float*>(ctrl + C::CTRL_BYTES);
+  uint8_t* stage = ctrl + C::CTRL_BYTES;  // [consumer warp][OUT_BUFS] store buffers
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -101,6 +111,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
     tma_prefetch_desc(&tmA_lo);
     tma_prefetch_desc(&tmB_hi);
     tma_prefetch_desc(&tmB_lo);
+    tma_prefetch_desc(&tmO0);
+    if (EPI == EPI_SPLIT) tma_prefetch_desc(&tmO1);
     // full: one arrive.expect_tx by the producer; empty: one arrive per consumer warpgroup
     for (int s = 0; s < C::A_SLOTS; ++s) {
       mbar_init(&a_full[s], 1);
@@ -116,9 +128,10 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 
   // setmaxnreg sits at the top of each role's branch and the branches only meet again at the exit.  With a merge point
   // after it (one if / else, then the role dispatch) ptxas ignored setmaxnreg (C7507) and the consumers' accumulators
-  // spilled at the 168-register launch bound.
+  // spilled at the 168-register launch bound.  The two producer warps need few registers; 24 leave the consumers 240,
+  // which the 256-wide statistics epilogue needs to hold its 128 accumulator registers without spilling.
   if (warp < 4) {
-    if constexpr (C::NWG > 1) setmaxnreg_dec<40>();
+    if constexpr (C::NWG > 1) setmaxnreg_dec<24>();
     if (warp == 0) {
       // ---------------------------------------------------------------- TMA producer (A strips).  The WHOLE warp walks
       // the loop (barrier waits and coordinates stay warp-uniform) and one elected lane issues the copies.
@@ -172,17 +185,17 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       }
     }
   } else {
-    if constexpr (C::NWG > 1) setmaxnreg_inc<232>();
+    if constexpr (C::NWG > 1) setmaxnreg_inc<240>();
     // ------------------------------------------------------------------ consumers: MMA + epilogue
     const int wg = (warp >> 2) - 1;  // consumer warpgroup
     const int t = threadIdx.x & 127;
     const int q = t >> 5;
     const bool signal = (t == 0);    // the thread that releases ring slots for its warpgroup
-    float* S = stage + wg * 128 * C::LD;
-    const int m = t;                 // epilogue: this thread's row (pixel) of the tile
+    uint8_t* obufs = stage + wg * 4 * C::OUT_BUFS * C::OBUF;  // this warpgroup's, [warp][OUT_BUFS]
+    const int m = t;                 // epilogue statistics: this thread's row (pixel) of the tile
     const int r = m >> 3, c = m & 7;
     const uint32_t b_off = static_cast<uint32_t>(wg * NW);  // first weight row of this warpgroup
-    int sa = 0, sb = 0, par = 0;
+    int sa = 0, sb = 0, par = 0, ob = 0;
     uint32_t pa = 0, pb = 0;
     float acc[2][NW / 2];
 
@@ -243,83 +256,88 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       retire_prev();  // the producers refill the rings while this warpgroup drains its accumulators
 
       // ---------------------------------------------------------------- epilogue
+      // Warp q holds fragment rows 64 h + 16 q + [0, 16) of accumulator h: image rows y0 + 8 h + 2 q + {0, 1}, all 8
+      // columns.  Per OC-column chunk it applies scale + bias (+ the hi/lo split) in registers, writes the chunk once
+      // into a store buffer laid out as the NHWC box {OC, 8, 2} (swizzled as the output map), and lane 0 stores it
+      // with one TMA tensor store per plane.  The box is clipped to the image, and nobody waits on the global write:
+      // before a buffer is written again, lane 0 only waits until the store that last used it has read it out.
       const int tx = tile % p.tiles_x, ty = (tile / p.tiles_x) % p.tiles_y, img = tile / (p.tiles_x * p.tiles_y);
-      const int x = tx * HALO_TW + c, y = ty * HALO_TH + r;
-      const bool valid = (x < p.W) && (y < p.H);
-      const size_t pix = (static_cast<size_t>(img) * p.H + y) * p.W + x;
-      const uint32_t vmask = __ballot_sync(0xffffffffu, valid);
-      const uint32_t row_off = static_cast<uint32_t>(pix * COUT);  // < 2^32 elements for every tensor of the path
+      const int x0 = tx * HALO_TW, y0 = ty * HALO_TH;
+      const bool valid = (x0 + c < p.W) && (y0 + r < p.H);
       // E[v^2] - mean^2 cancels (mean / std)^2 of the sums' significant bits, so a group whose mean dominates its
       // spread loses its variance in plain fp32 sums (rstd off by 1e-2 at mean / std = 1000).  Each thread sums its
       // pixel's d = v - k in fp32, k = the pixel's first value in the group (|d| ~ the group's spread), and turns the
-      // sums into fp64 sums of v and v^2 once per group.
+      // sums into fp64 sums of v and v^2 once per group.  Thread m reads its pixel back from the staged chunks, in
+      // column order.
       float tk[C::GPW], tsum[C::GPW], tsq[C::GPW];
 #pragma unroll
       for (int g = 0; g < C::GPW; ++g) tk[g] = tsum[g] = tsq[g] = 0.f;
       bool overflow = false;
+      constexpr int SPAN = C::OC * (EPI == EPI_SPLIT ? 2 : 4);  // bytes per box row
+      auto swz = [](int a) { return a ^ (((a >> 7) & (SPAN / 16 - 1)) << 4); };  // TMA swizzle of byte offset a
+      const int fc = 2 * (lane & 3), fr = lane >> 2;  // fragment column pair within an 8-column block, row within 8
+      uint8_t* wbufs = obufs + q * C::OUT_BUFS * C::OBUF;
 #pragma unroll
-      for (int cj = 0; cj < NW / C::CH; ++cj) {
-        const int ch0 = wg * NW + cj * C::CH;
-        named_bar_sync(2 + wg, 128);  // the previous chunk's staging reads are done
-        stage_acc_cols<NW, C::CH, C::LD>(acc[0], S, 0, cj * C::CH / 8);
-        stage_acc_cols<NW, C::CH, C::LD>(acc[1], S, 64, cj * C::CH / 8);
-        named_bar_sync(2 + wg, 128);
-        float v[C::CH];
+      for (int h = 0; h < 2; ++h) {
+        const int yb = y0 + 8 * h + 2 * q;
 #pragma unroll
-        for (int j = 0; j < C::CH; ++j) v[j] = fmaf(S[m * C::LD + j], p.acc_scale, __ldg(p.bias + ch0 + j));
-        if constexpr (EPI == EPI_F32_STATS) {
-          if (valid) {
-#pragma unroll
-            for (int j = 0; j < C::CH; ++j) {
-              const int g = (cj * C::CH + j) / C::GROUP_CH;  // compile-time: group within this warpgroup's columns
-              if ((cj * C::CH + j) % C::GROUP_CH == 0) tk[g] = v[j];
-              const float d = v[j] - tk[g];
-              tsum[g] += d;
-              tsq[g] = fmaf(d, d, tsq[g]);
-            }
-          }
-        }
-        if constexpr (EPI == EPI_F32_STATS || EPI == EPI_F32) {
-          // thread = row; go back through the staging tile so that lanes = columns and every store instruction writes
-          // whole row segments (row-per-thread stores write 32 partial lines per instruction)
-#pragma unroll
-          for (int j = 0; j < C::CH; ++j) S[m * C::LD + j] = v[j];
+        for (int cc = 0; cc < NW / C::OC; ++cc) {
+          const int ch0 = wg * NW + cc * C::OC;
+          uint8_t* O = wbufs + ob * C::OBUF;
+          if (lane == 0) bulk_wait_group_read<C::OUT_BUFS - 1>();  // the store that last used O has read it
+          // one buffer per warp: every thread has also read its statistics out of the buffers
+          if constexpr (EPI == EPI_F32_STATS && C::OUT_BUFS == 1) named_bar_sync(2 + wg, 128);
           __syncwarp();
-          if constexpr (C::CH == 32) {
-#pragma unroll 8
-            for (int rw = 0; rw < 32; ++rw) {
-              const uint32_t o = __shfl_sync(0xffffffffu, row_off, rw) + ch0 + lane;
-              if ((vmask >> rw) & 1u) p.y32[o] = S[(q * 32 + rw) * C::LD + lane];
-            }
-          } else {
-            constexpr int RPI = 32 / C::CH;  // rows per store instruction
-            const int hsel = lane / C::CH, cl = lane % C::CH;
-#pragma unroll 8
-            for (int i = 0; i < 32 / RPI; ++i) {
-              const int rw = RPI * i + hsel;
-              const uint32_t o = __shfl_sync(0xffffffffu, row_off, rw) + ch0 + cl;
-              if ((vmask >> rw) & 1u) p.y32[o] = S[(q * 32 + rw) * C::LD + cl];
+#pragma unroll
+          for (int b = 0; b < C::OC / 8; ++b) {
+            const int blk = cc * C::OC / 8 + b;
+            const float b0 = __ldg(p.bias + ch0 + 8 * b + fc), b1 = __ldg(p.bias + ch0 + 8 * b + fc + 1);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {  // fragment rows fr and fr + 8 (stage_acc_cols' layout): image row yb + e
+              const float v0 = fmaf(acc[h][4 * blk + 2 * e], p.acc_scale, b0);
+              const float v1 = fmaf(acc[h][4 * blk + 2 * e + 1], p.acc_scale, b1);
+              const int o = (8 * e + fr) * C::OC + 8 * b + fc;  // element of the box
+              if constexpr (EPI == EPI_SPLIT) {
+                const float s0 = v0 * p.split_scale, s1 = v1 * p.split_scale;
+                const bool rv = (x0 + fr < p.W) && (yb + e < p.H);
+                overflow |= rv && (fabsf(s0) > 60000.f || fabsf(s1) > 60000.f);
+                const __half h0 = __float2half_rn(s0), h1 = __float2half_rn(s1);
+                const __half l0 = __float2half_rn(s0 - __half2float(h0)), l1 = __float2half_rn(s1 - __half2float(h1));
+                *reinterpret_cast<__half2*>(O + swz(2 * o)) = __halves2half2(h0, h1);
+                *reinterpret_cast<__half2*>(O + C::OBUF / 2 + swz(2 * o)) = __halves2half2(l0, l1);  // lo plane
+              } else {
+                *reinterpret_cast<float2*>(O + swz(4 * o)) = make_float2(v0, v1);
+              }
             }
           }
-        } else if (valid) {
-          {
-            __align__(16) __half hi[C::CH];
-            __align__(16) __half lo[C::CH];
+          fence_proxy_async();  // this thread's buffer writes become visible to the TMA store
+          __syncwarp();
+          if (lane == 0) {
+            tma_store_4d(&tmO0, O, ch0, x0, yb, img);
+            if constexpr (EPI == EPI_SPLIT) tma_store_4d(&tmO1, O + C::OBUF / 2, ch0, x0, yb, img);
+            bulk_commit_group();
+          }
+          if constexpr (EPI == EPI_F32_STATS) {
+            named_bar_sync(2 + wg, 128);  // every warp's chunk is staged
+            if (valid && (m >> 6) == h) {
+              const uint8_t* src = obufs + (((m & 63) >> 4) * C::OUT_BUFS + ob) * C::OBUF;  // the warp that holds m
 #pragma unroll
-            for (int j = 0; j < C::CH; ++j) {
-              const float s = v[j] * p.split_scale;
-              overflow |= (fabsf(s) > 60000.f);
-              hi[j] = __float2half_rn(s);
-              lo[j] = __float2half_rn(s - __half2float(hi[j]));
-            }
-            uint4* dh = reinterpret_cast<uint4*>(p.out_hi + pix * COUT + ch0);
-            uint4* dl = reinterpret_cast<uint4*>(p.out_lo + pix * COUT + ch0);
+              for (int u = 0; u < C::OC / 4; ++u) {
+                const float4 f = *reinterpret_cast<const float4*>(src + swz(((m & 15) * C::OC + 4 * u) * 4));
+                const float vv[4] = {f.x, f.y, f.z, f.w};
 #pragma unroll
-            for (int j = 0; j < C::CH / 8; ++j) {
-              dh[j] = reinterpret_cast<const uint4*>(hi)[j];
-              dl[j] = reinterpret_cast<const uint4*>(lo)[j];
+                for (int i = 0; i < 4; ++i) {
+                  const int col = cc * C::OC + 4 * u + i;
+                  const int g = col / C::GROUP_CH;  // compile-time: group within this warpgroup's columns
+                  if (col % C::GROUP_CH == 0) tk[g] = vv[i];
+                  const float d = vv[i] - tk[g];
+                  tsum[g] += d;
+                  tsq[g] = fmaf(d, d, tsq[g]);
+                }
+              }
             }
           }
+          if (++ob == C::OUT_BUFS) ob = 0;
         }
       }
 
@@ -357,6 +375,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         if (overflow) atomicOr(p.status, 1);
       }
     }
+    if (lane == 0) bulk_wait_group<0>();  // each warp's store buffers stay valid until its last stores have completed
   }
 }
 

@@ -100,12 +100,12 @@ CUtensorMapSwizzle swizzle_for(int bk) {
   return bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-// The one cuTensorMapEncodeTiled call: an fp16 tensor of `rank` dims (innermost first; strides in bytes of dims 1..),
-// no interleave, out-of-bounds elements read as zero.  `what` names the map in the error message.
-int encode_map(CUtensorMap* m, const char* what, cuuint32_t rank, const __half* base, const cuuint64_t* dims,
+// The one cuTensorMapEncodeTiled call: an fp16 (or `dtype`) tensor of `rank` dims (innermost first; strides in bytes
+// of dims 1..), no interleave, out-of-bounds elements read as zero.  `what` names the map in the error message.
+int encode_map(CUtensorMap* m, const char* what, cuuint32_t rank, const void* base, const cuuint64_t* dims,
                const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swizzle,
-               CUtensorMapL2promotion l2) {
-  const CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<__half*>(base), dims, strides, box, estr,
+               CUtensorMapL2promotion l2, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16) {
+  const CUresult r = g_encode(m, dtype, rank, const_cast<void*>(base), dims, strides, box, estr,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail(DD_ERR_CUDA, std::string("cuTensorMapEncodeTiled(") + what + ") failed: " + std::to_string((int)r));
@@ -131,6 +131,17 @@ int make_nhwc_map(CUtensorMap* m, const char* what, const __half* base, int B, i
 int make_act_map(CUtensorMap* m, const __half* base, int B, int H, int W, int C, int bk, int stride = 1, int ld = 0) {
   return make_nhwc_map(m, "activation", base, B, H, W, C, bk, dd::TILE_W * stride, dd::TILE_H * stride, swizzle_for(bk),
                        stride, ld);
+}
+// output of the halo kernel: NHWC [B][H][W][C] fp32 (y32) or fp16 (split planes), stored by each consumer warp in
+// boxes of {halo_out_box_c(C) channels, 8, 2, 1}; a box row is the swizzle span
+int make_out_map(CUtensorMap* m, const void* base, bool f32, int B, int H, int W, int C) {
+  const int es = f32 ? 4 : 2, box_c = dd::halo_out_box_c(C);
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)C * es, (cuuint64_t)W * C * es, (cuuint64_t)H * W * C * es};
+  const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)dd::HALO_TW, 2, 1};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  return encode_map(m, "output", 4, base, dims, strides, box, estr, swizzle_for(box_c * es / 2),
+                    CU_TENSOR_MAP_L2_PROMOTION_NONE, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
 }
 // halo patch of conv5x5_fold_kernel: the NHWC [B][H][W][256] fp16 plane seen as {8 ch, y, x, channel group, image};
 // box = {8, 20, 36, 2, 1} lands in shared memory as [channel group][x][y][8 ch], no swizzle
@@ -168,7 +179,7 @@ int shape_id(int cin, int cout) {
 constexpr int kHaloBK[5] = {16, 32, 32, 32, 32};  // K chunk of the halo kernel per shape id
 
 // One 3x3 conv kernel: conv3x3_simt_kernel (fp32 CUDA cores, reads sa) or the persistent conv3x3_halo_kernel (reads
-// the strip maps m[0..1] of the input planes and the weight maps m[2..3]).
+// the strip maps m[0..1] of the input planes and the weight maps m[2..3], stores through the output maps m[4..5]).
 template <int CIN, int COUT, int BK, int EPI>
 void conv3x3_kernel(bool simt, const dd::SimtArgs& sa, const CUtensorMap* m, const dd::ConvArgs& a, int sm_count,
                     cudaStream_t st) {
@@ -178,7 +189,8 @@ void conv3x3_kernel(bool simt, const dd::SimtArgs& sa, const CUtensorMap* m, con
   } else {
     using C = dd::HaloCfg<CIN, COUT, BK>;
     const int grid = a.num_tiles < sm_count ? a.num_tiles : sm_count;
-    dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(m[0], m[1], m[2], m[3], a);
+    dd::conv3x3_halo_kernel<CIN, COUT, BK, EPI><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(m[0], m[1], m[2], m[3], m[4],
+                                                                                         m[5], a);
   }
 }
 template <int CIN, int COUT, int BK>
@@ -199,7 +211,7 @@ int launch_conv3x3(int sid, int epi, bool simt, dd::ConvArgs& a, const __half* i
   a.tiles_x = (a.W + tw - 1) / tw;
   a.tiles_y = (a.H + th - 1) / th;
   a.num_tiles = a.tiles_x * a.tiles_y * a.B;
-  CUtensorMap m[4] = {{}, {}, w_hi, w_lo};
+  CUtensorMap m[6] = {{}, {}, w_hi, w_lo, {}, {}};
   dd::SimtArgs sa{};
   if (simt) {
     sa.in_hi = in_hi;
@@ -214,6 +226,13 @@ int launch_conv3x3(int sid, int epi, bool simt, dd::ConvArgs& a, const __half* i
       return rc;
     if ((rc = make_nhwc_map(&m[1], "strip", in_lo, a.B, a.H, a.W, cin, bk, dd::HALO_TW, dd::HALO_TH + 2, swizzle_for(bk))))
       return rc;
+    const int cout = kShapes[sid].cout;
+    if (epi == dd::EPI_SPLIT) {
+      if ((rc = make_out_map(&m[4], a.out_hi, false, a.B, a.H, a.W, cout))) return rc;
+      if ((rc = make_out_map(&m[5], a.out_lo, false, a.B, a.H, a.W, cout))) return rc;
+    } else if ((rc = make_out_map(&m[4], a.y32, true, a.B, a.H, a.W, cout))) {
+      return rc;
+    }
   }
   switch (sid) {
     case 0: conv3x3_epi<16, 64, kHaloBK[0]>(epi, simt, sa, m, a, sm_count, st); break;
