@@ -308,27 +308,23 @@ struct ConvLayer {
   CUtensorMap mh_hi, mh_lo;  // box for the halo kernel's K chunk
 };
 
-// PackStage::xraw: the codec kinds' registered tensors, the encoder's from 0, the decoder's from kXDecRaw (largest:
-// the UP4 encoder, 3 conv_bn_relu = 4944 floats, and the UP4 decoder, 2 ConvT + BatchNorm + final conv = 8433 floats;
-// kind_keys_fit checks every table against these bounds).
-constexpr size_t kXDecRaw = 8192, kXRawFloats = kXDecRaw + 12288;
+// The default codec's (DD_CODEC_UP2; UP2_1X1 shares its decoder) host-written device blocks, in floats.  Encoder: the
+// folded convs at the CK_E4 offsets the FULL encoder uses, then for DD_CODEC_TRAIN and the backward the unfolded
+// weights ([tap][co], [tap][ci][co]), gamma1 / beta1 / gamma2 / beta2, and both BatchNorms on running statistics
+// ([2][3][16]: s = gamma rstd, mean, rstd).  Decoder: folded ConvT [ky][kx][ci][co], its bias, the final conv
+// [tap][ci]; unfolded ConvT and bias, the BatchNorm on running statistics ([3][16]), gamma / beta.
+constexpr int kEncW1u = dd::CK_E4_W3, kEncW2u = kEncW1u + 144, kEncGb = kEncW2u + 2304, kEncBn = kEncGb + 64,
+              kEncN = kEncBn + 96;
+constexpr int kDecWt = 0, kDecBt = 4096, kDecWc = 4112, kDecWu = 4256, kDecBu = 8352, kDecBn = 8368, kDecGb = 8416,
+              kDecN = 8448;
 // Pinned host side of the denoiser / codec pack, so that its copies are asynchronous and one synchronisation serves a
-// whole pack: the abs-max words of the conv weights, the decoder's and encoder's raw tensors as last registered (an
-// update re-reads only the registered ones; the BatchNorm folds need all of them), and what the host folds produce.
+// whole pack: the abs-max words of the conv weights, the folded encoder and decoder blocks, and after the struct
+// (raw()) the codec's tensors as last registered, at their PackKey::off (an update re-reads only the registered ones;
+// the BatchNorm folds need all of them).
 struct PackStage {
   float amax[16];  // slot i: conv layer i (0..5), 6 + i: its data-gradient layer, 12: the composed 5x5 conv
-  // device -> host
-  float dec_wt[16 * 16 * 16], dec_bt[16], dec_g[16], dec_be[16], dec_mu[16], dec_var[16], dec_wc[16 * 9], dec_bc[1];
-  float enc_w1[144], enc_bn1[4][16], enc_w2[2304], enc_bn2[4][16];
-  // host -> device
-  float wt_f[4 * 4 * 16 * 16], bt_f[16], wc_f[9 * 16], wu[4 * 4 * 16 * 16], bn[3 * 16];
-  float f1[144], t1[16], f2[2304], t2[16];
-  float e1u[144], e2u[2304], enc_gb[4][16];  // unfolded encoder for DD_CODEC_TRAIN: [tap][co], [tap][ci][co]; gamma / beta
-  float enc_bn[2][3][16];                     // the encoder backward's running-statistics BatchNorms: s, mean, rstd
-  // codec kinds other than DD_CODEC_UP2 (codec_kinds.cuh): their registered tensors at kind_keys' offsets, and the
-  // folded parameter blocks of their kernels (encoder, decoder)
-  float xraw[kXRawFloats];
-  float xenc[dd::CK_E4_N], xdec[dd::CK_D4_N];
+  float enc[std::max(kEncN, dd::CK_E4_N)], dec[std::max(kDecN, dd::CK_D4_N)];
+  float* raw() { return reinterpret_cast<float*>(this + 1); }
 };
 
 struct Raw {
@@ -492,6 +488,9 @@ struct dd_engine {
   float* gn_gamma[4] = {nullptr, nullptr, nullptr, nullptr};  // ne.1, ne.4, pred.1, pred.4
   float* gn_beta[4] = {nullptr, nullptr, nullptr, nullptr};
   float* temb = nullptr;    // [1280][256]
+  // the codec's host-written blocks: folded encoder (null: no encoder registered) and decoder, laid out as
+  // codec_kinds.cuh for its kinds and as kEnc* / kDec* for the default codec, whose named views follow
+  float *xenc = nullptr, *xdec = nullptr;
   float* dec_wt = nullptr;  // [4][4][16][16] folded
   float* dec_bt = nullptr;  // [16]
   float* dec_wc = nullptr;  // [9][16]
@@ -499,12 +498,11 @@ struct dd_engine {
   float* dec_wu = nullptr;  // [4][4][16][16] unfolded ConvT weights, [ky][kx][ci][co]
   float* dec_bu = nullptr;  // [16] unfolded ConvT bias
   float* dec_bn = nullptr;  // [3][16] BatchNorm scale gamma * rstd, running mean, rstd
-  float *enc_w1 = nullptr, *enc_b1 = nullptr, *enc_w2 = nullptr, *enc_b2 = nullptr;  // folded encoder (optional)
+  float *enc_w1 = nullptr, *enc_b1 = nullptr, *enc_w2 = nullptr, *enc_b2 = nullptr;  // folded encoder
   float* enc_bn = nullptr;  // [2][3][16] encoder BatchNorms 1, 2 on running statistics: s = gamma rstd, mean, rstd
-  float *xenc = nullptr, *xdec = nullptr;  // codec kinds 1..3: folded encoder (optional) / decoder (UP4, FULL) blocks
-  // DD_CODEC_TRAIN (dd_set_codec_mode): the codec's BatchNorms on batch statistics.  The unfolded parameters (filled
-  // with the pack), the batch-folded copies decoder_kernel / encoder_kernel run on, and the statistics' scratch; all
-  // engine-owned, so the workspace size does not depend on the mode.
+  // DD_CODEC_TRAIN (dd_set_codec_mode): the codec's BatchNorms on batch statistics.  The unfolded parameters (views of
+  // the pack's blocks), the batch-folded copies decoder_kernel / encoder_kernel run on, and the statistics' scratch;
+  // all engine-owned, so the workspace size does not depend on the mode.
   int codec_mode = DD_CODEC_EVAL;
   struct CodecTrain {
     float *dec_gb = nullptr;                                  // [2][16] decoder BatchNorm weight, bias
@@ -659,11 +657,10 @@ Geom geom_of(const dd_config& c) {
 
 // ---- backward (DD_FLAG_BACKWARD)
 constexpr int kBwdSlots = 16;  // gradient splits per dd_denoiser_backward call (at most 6 are used)
-// conv layer i: reference key prefix, Cout, Cin
-const char* const kConvKey[6] = {"model.noise_embedding.0", "model.noise_embedding.3", "model.upsample_fuse.convA.conv",
-                                 "model.upsample_fuse.convB.conv", "model.pred.0", "model.pred.3"};
+// conv layer i (ne.0, ne.3, convA, convB, pred.0, pred.3): Cout, Cin; GroupNorm i (ne.1, ne.4, pred.1, pred.4): channels
 constexpr int kConvCout[6] = {64, 256, 256, 256, 64, 16};
 constexpr int kConvCin[6] = {16, 64, 256, 256, 256, 64};
+constexpr int kGnCh[4] = {64, 256, 64, 16};
 // Split-K plan of wgrad_simt_kernel: about 16 blocks per SM in all, each chunk a multiple of the fp32 flush interval.
 struct WgPlan {
   int chunks, chunk;
@@ -714,14 +711,111 @@ size_t codec_map_elems(const dd_config& c) {
 }
 // DD_FLAG_LOOP_BACKWARD implies DD_FLAG_BACKWARD
 bool has_backward(const dd_config& c) { return (c.flags & (DD_FLAG_BACKWARD | DD_FLAG_LOOP_BACKWARD)) != 0; }
-// Elements of the denoiser's parameters in dd_denoiser_backward's order (time_embedding dense); offsets into lp.acc.
-constexpr size_t kParamNumel[21] = {64 * 16 * 9, 64, 64, 64, 256 * 64 * 9, 256, 256, 256, DD_TIME_ROWS * 256,
-                                    64 * 256 * 9, 64, 64, 64, 16 * 64 * 9, 16, 16, 16,
-                                    256 * 256 * 9, 256, 256 * 256 * 9, 256};
+size_t numel(const std::vector<int64_t>& s) {
+  size_t n = 1;
+  for (int64_t d : s) n *= static_cast<size_t>(d);
+  return n;
+}
+
+// ---- the keys of the denoiser + codec pack: what dd_set_weight takes besides the producers' and the backbone's, what
+// dd_finalize_weights requires and shape-checks, what dd_update_weights re-packs
+enum PackGroup { PK_DENOISER, PK_FUSE, PK_ENC, PK_DEC };  // PK_FUSE: convA / convB, packed on Swin only
+struct PackKey {
+  std::string name;
+  std::vector<int64_t> shape;
+  PackGroup group;
+  unsigned kinds;  // bit k: codec kind k packs the key
+  size_t off;      // PK_ENC / PK_DEC: floats into PackStage::raw()
+};
+struct PackTable {
+  // the denoiser's keys first, in DENOISER_KEYS + FUSE_KEYS order (dd_denoiser_backward's gradient order); the
+  // default decoder's in DECODER_KEYS order
+  std::vector<PackKey> keys;
+  int conv[6], gn[4];  // index of conv layer i's and GroupNorm i's weight; its bias follows
+  size_t raw_floats = 0;
+};
+PackTable make_pack_table() {
+  PackTable t;
+  auto add = [&](PackGroup g, unsigned kinds, const std::string& name, std::vector<int64_t> shape) {
+    t.keys.push_back({name, shape, g, kinds, g >= PK_ENC ? t.raw_floats : 0});
+    if (g >= PK_ENC) t.raw_floats += numel(shape);
+  };
+  const unsigned all = 15, k0 = 1u << DD_CODEC_UP2, k1 = 1u << DD_CODEC_UP2_1X1, k2 = 1u << DD_CODEC_UP4,
+                 k3 = 1u << DD_CODEC_FULL;
+  auto conv = [&](PackGroup g, const std::string& p, int i) {
+    t.conv[i] = static_cast<int>(t.keys.size());
+    add(g, all, p + ".weight", {kConvCout[i], kConvCin[i], 3, 3});
+    add(g, all, p + ".bias", {kConvCout[i]});
+  };
+  auto gn = [&](const std::string& p, int i) {
+    t.gn[i] = static_cast<int>(t.keys.size());
+    add(PK_DENOISER, all, p + ".weight", {kGnCh[i]});
+    add(PK_DENOISER, all, p + ".bias", {kGnCh[i]});
+  };
+  conv(PK_DENOISER, "model.noise_embedding.0", 0);
+  gn("model.noise_embedding.1", 0);
+  conv(PK_DENOISER, "model.noise_embedding.3", 1);
+  gn("model.noise_embedding.4", 1);
+  add(PK_DENOISER, all, "model.time_embedding.weight", {DD_TIME_ROWS, 256});
+  conv(PK_DENOISER, "model.pred.0", 4);
+  gn("model.pred.1", 2);
+  conv(PK_DENOISER, "model.pred.3", 5);
+  gn("model.pred.4", 3);
+  conv(PK_FUSE, "model.upsample_fuse.convA.conv", 2);
+  conv(PK_FUSE, "model.upsample_fuse.convB.conv", 3);
+  auto bn = [&](PackGroup g, unsigned kinds, const std::string& p, int64_t c) {
+    for (const char* leaf : {"weight", "bias", "running_mean", "running_var"}) add(g, kinds, p + leaf, {c});
+  };
+  auto conv_bn = [&](PackGroup g, unsigned kinds, const std::string& p, int64_t ci, int64_t co) {  // conv_bn_relu
+    add(g, kinds, p + "0.weight", {co, ci, 3, 3});
+    bn(g, kinds, p + "1.", co);
+  };
+  const std::string E = "depth_transform.conv_transform.", D = "depth_transform.conv_inv_transform.";
+  add(PK_DEC, k0 | k1, D + "0.weight", {16, 16, 4, 4});
+  add(PK_DEC, k0 | k1, D + "0.bias", {16});
+  bn(PK_DEC, k0 | k1, D + "1.", 16);
+  add(PK_DEC, k0 | k1, D + "3.0.weight", {1, 16, 3, 3});
+  add(PK_DEC, k0 | k1, D + "3.0.bias", {1});
+  add(PK_DEC, k2, D + "0.weight", {16, 16, 4, 4});
+  add(PK_DEC, k2, D + "0.bias", {16});
+  add(PK_DEC, k2, D + "1.weight", {16, 16, 4, 4});
+  add(PK_DEC, k2, D + "1.bias", {16});
+  bn(PK_DEC, k2, D + "2.", 16);
+  add(PK_DEC, k2, D + "4.0.weight", {1, 16, 3, 3});
+  add(PK_DEC, k2, D + "4.0.bias", {1});
+  conv_bn(PK_DEC, k3, D + "0.", 16, 16);
+  conv_bn(PK_DEC, k3, D + "1.", 16, 1);
+  conv_bn(PK_ENC, k0 | k3, E + "0.", 1, 16);  // the FULL encoder has the default one's keys, not its pack
+  conv_bn(PK_ENC, k0 | k3, E + "1.", 16, 16);
+  add(PK_ENC, k1, E + "0.weight", {16, 1, 1, 1});
+  add(PK_ENC, k1, E + "1.weight", {16, 16, 1, 1});
+  conv_bn(PK_ENC, k2, E + "0.", 1, 16);
+  conv_bn(PK_ENC, k2, E + "1.", 16, 16);
+  conv_bn(PK_ENC, k2, E + "2.", 16, 16);
+  return t;
+}
+const PackTable& pack_table() {
+  static const PackTable t = make_pack_table();
+  return t;
+}
+bool in_kind(const PackKey& k, int kind) { return (k.kinds >> kind & 1) != 0; }
+// The key `name` of codec kind `kind`'s engines (null: not a pack key of that kind).
+const PackKey* find_pack_key(int kind, const std::string& name) {
+  for (const PackKey& k : pack_table().keys)
+    if (in_kind(k, kind) && k.name == name) return &k;
+  return nullptr;
+}
+// The engine packs `k`: a key of its codec kind, the fuse convs on Swin only, the encoder's when it has one.
+bool packs(const dd_config& c, const PackKey& k, bool encoder) {
+  if (!in_kind(k, codec_kind(c))) return false;
+  return k.group == PK_FUSE ? c.variant == DD_VARIANT_SWIN : k.group != PK_ENC || encoder;
+}
 int param_count(const dd_config& c) { return c.variant == DD_VARIANT_SWIN ? 21 : 17; }
+// Elements of denoiser parameter i in dd_denoiser_backward's order (time_embedding dense), and its offset into lp.acc.
+size_t param_numel(int i) { return numel(pack_table().keys[i].shape); }
 size_t param_offset(int i) {
   size_t o = 0;
-  for (int k = 0; k < i; ++k) o += kParamNumel[k];
+  for (int k = 0; k < i; ++k) o += param_numel(k);
   return o;
 }
 // block counts of the decoder backward's reductions
@@ -1449,127 +1543,60 @@ int copy_param(dd_engine* e, const std::string& key, size_t n, float** out, cuda
 // ------------------------------------------------------------------------------------------------ denoiser + codec pack
 // dd_finalize_weights allocates (alloc_pack) and fills (fill_pack) everything; dd_update_weights validates
 // (check_update) and fills what depends on the registered keys, at the same addresses.
-const char* const kGnKey[4] = {"model.noise_embedding.1", "model.noise_embedding.4", "model.pred.1", "model.pred.4"};
-constexpr int kGnCh[4] = {64, 256, 64, 16};
-const std::string kDecPrefix = "depth_transform.conv_inv_transform.";
-const std::string kEncPrefix = "depth_transform.conv_transform.";
-struct CodecKey {
-  const char* leaf;
-  size_t host_off;  // floats from the start of PackStage
-  std::vector<int64_t> shape;
-};
-#define DD_STAGE_OFF(m) (offsetof(PackStage, m) / sizeof(float))
-const CodecKey kDecKeys[8] = {{"0.weight", DD_STAGE_OFF(dec_wt), {16, 16, 4, 4}}, {"0.bias", DD_STAGE_OFF(dec_bt), {16}},
-                              {"1.weight", DD_STAGE_OFF(dec_g), {16}},            {"1.bias", DD_STAGE_OFF(dec_be), {16}},
-                              {"1.running_mean", DD_STAGE_OFF(dec_mu), {16}},     {"1.running_var", DD_STAGE_OFF(dec_var), {16}},
-                              {"3.0.weight", DD_STAGE_OFF(dec_wc), {1, 16, 3, 3}}, {"3.0.bias", DD_STAGE_OFF(dec_bc), {1}}};
-const CodecKey kEncKeys[10] = {
-    {"0.0.weight", DD_STAGE_OFF(enc_w1), {16, 1, 3, 3}},        {"0.1.weight", DD_STAGE_OFF(enc_bn1[0]), {16}},
-    {"0.1.bias", DD_STAGE_OFF(enc_bn1[1]), {16}},               {"0.1.running_mean", DD_STAGE_OFF(enc_bn1[2]), {16}},
-    {"0.1.running_var", DD_STAGE_OFF(enc_bn1[3]), {16}},        {"1.0.weight", DD_STAGE_OFF(enc_w2), {16, 16, 3, 3}},
-    {"1.1.weight", DD_STAGE_OFF(enc_bn2[0]), {16}},             {"1.1.bias", DD_STAGE_OFF(enc_bn2[1]), {16}},
-    {"1.1.running_mean", DD_STAGE_OFF(enc_bn2[2]), {16}},       {"1.1.running_var", DD_STAGE_OFF(enc_bn2[3]), {16}}};
-#undef DD_STAGE_OFF
-size_t numel(const std::vector<int64_t>& s) {
-  size_t n = 1;
-  for (int64_t d : s) n *= static_cast<size_t>(d);
-  return n;
+// conv weight w [co][ci][3][3] -> [tap][ci][co], times s[co] in fp64 (s null: as registered)
+void conv_taps(const float* w, int ci, int co, const float* s, float* out) {
+  for (int o = 0; o < co; ++o)
+    for (int i = 0; i < ci; ++i)
+      for (int tap = 0; tap < 9; ++tap) {
+        const float v = w[(o * ci + i) * 9 + tap];
+        out[(tap * ci + i) * co + o] = s ? static_cast<float>(static_cast<double>(v) * s[o]) : v;
+      }
+}
+// ConvTranspose2d weight w [16][16][4][4] ([ci][co][ky][kx]) -> [ky][kx][ci][co], times s[co] (s null: as registered)
+void convt_taps(const float* w, const double* s, float* out) {
+  for (int ci = 0; ci < 16; ++ci)
+    for (int co = 0; co < 16; ++co)
+      for (int k = 0; k < 16; ++k) {
+        const float v = w[(ci * 16 + co) * 16 + k];
+        out[(k * 16 + ci) * 16 + co] = s ? static_cast<float>(static_cast<double>(v) * s[co]) : v;
+      }
 }
 
-// Codec kinds other than DD_CODEC_UP2: the keys their own pack reads and where PackStage::xraw holds them (encoders
-// from 0, decoders from kXDecRaw).  DD_CODEC_UP2_1X1's decoder is the default one (kDecKeys); the FULL encoder has the
-// default encoder's keys but its own kernel and pack.
-struct KindKey {
-  std::string name;
-  std::vector<int64_t> shape;
-  size_t off;
-};
-std::vector<KindKey> make_kind_keys(int kind, bool enc) {
-  std::vector<std::pair<std::string, std::vector<int64_t>>> k;
-  auto conv_bn = [&](const std::string& p, int64_t ci, int64_t co) {  // conv_bn_relu: conv `p0`, BatchNorm `p1`
-    k.push_back({p + "0.weight", {co, ci, 3, 3}});
-    for (const char* leaf : {"1.weight", "1.bias", "1.running_mean", "1.running_var"}) k.push_back({p + leaf, {co}});
-  };
-  const std::string E = "conv_transform.", D = "conv_inv_transform.";
-  if (enc && kind == DD_CODEC_UP2_1X1) {
-    k.push_back({E + "0.weight", {16, 1, 1, 1}});
-    k.push_back({E + "1.weight", {16, 16, 1, 1}});
-  }
-  if (enc && kind == DD_CODEC_UP4) {
-    conv_bn(E + "0.", 1, 16);
-    conv_bn(E + "1.", 16, 16);
-    conv_bn(E + "2.", 16, 16);
-  }
-  if (enc && kind == DD_CODEC_FULL) {
-    conv_bn(E + "0.", 1, 16);
-    conv_bn(E + "1.", 16, 16);
-  }
-  if (!enc && kind == DD_CODEC_UP4) {
-    k.push_back({D + "0.weight", {16, 16, 4, 4}});
-    k.push_back({D + "0.bias", {16}});
-    k.push_back({D + "1.weight", {16, 16, 4, 4}});
-    k.push_back({D + "1.bias", {16}});
-    for (const char* leaf : {"2.weight", "2.bias", "2.running_mean", "2.running_var"}) k.push_back({D + leaf, {16}});
-    k.push_back({D + "4.0.weight", {1, 16, 3, 3}});
-    k.push_back({D + "4.0.bias", {1}});
-  }
-  if (!enc && kind == DD_CODEC_FULL) {
-    conv_bn(D + "0.", 16, 16);
-    conv_bn(D + "1.", 16, 1);
-  }
-  std::vector<KindKey> out;
-  size_t off = enc ? 0 : kXDecRaw;
-  for (auto& kv : k) {
-    out.push_back({"depth_transform." + kv.first, kv.second, off});
-    off += numel(kv.second);
-  }
-  return out;
-}
-const std::vector<KindKey>& kind_keys(int kind, bool enc) {
-  static const std::vector<KindKey> t[2][4] = {
-      {make_kind_keys(0, false), make_kind_keys(1, false), make_kind_keys(2, false), make_kind_keys(3, false)},
-      {make_kind_keys(0, true), make_kind_keys(1, true), make_kind_keys(2, true), make_kind_keys(3, true)}};
-  return t[enc ? 1 : 0][kind];
-}
-// Every codec kind's tables fit their PackStage::xraw region (encoder [0, kXDecRaw), decoder [kXDecRaw, kXRawFloats)).
-bool kind_keys_fit() {
-  for (int kind = 0; kind < 4; ++kind)
-    for (bool enc : {true, false})
-      for (const KindKey& k : kind_keys(kind, enc))
-        if (k.off + numel(k.shape) > (enc ? kXDecRaw : kXRawFloats)) return false;
-  return true;
-}
-const KindKey* find_kind_key(int kind, const std::string& name) {
-  for (bool enc : {true, false})
-    for (const KindKey& k : kind_keys(kind, enc))
-      if (k.name == name) return &k;
-  return nullptr;
-}
-
-// Fold the staged tensors of codec kind `kind` (PackStage::xraw) into its encoder (PackStage::xenc) or decoder
-// (xdec) block, in fp64 on the host like the default codec's folds; layouts in codec_kinds.cuh.
-void fold_kind(PackStage* sg, int kind, bool enc) {
-  auto R = [&](const std::string& leaf) -> const float* {
-    for (const KindKey& k : kind_keys(kind, enc))
-      if (k.name == "depth_transform." + leaf) return sg->xraw + k.off;
-    return nullptr;
+// Fold the staged tensors (PackStage::raw()) of codec kind `kind`'s encoder or decoder into its block (PackStage::enc,
+// dec), in fp64 on the host; layouts in codec_kinds.cuh and at kEncN / kDecN.
+void fold_codec(PackStage* sg, int kind, bool enc) {
+  auto R = [&](const std::string& leaf) { return sg->raw() + find_pack_key(kind, "depth_transform." + leaf)->off; };
+  // BatchNorm `p` on running statistics, unfolded: [3][16] s = gamma rstd, mean, rstd
+  auto bn_rstd = [&](const std::string& p, float* out) {
+    const float *g = R(p + "weight"), *mu = R(p + "running_mean"), *var = R(p + "running_var");
+    for (int c = 0; c < 16; ++c) {
+      const double rstd = 1.0 / sqrt(static_cast<double>(var[c]) + 1e-5);
+      out[c] = static_cast<float>(static_cast<double>(g[c]) * rstd);
+      out[16 + c] = mu[c];
+      out[32 + c] = static_cast<float>(rstd);
+    }
   };
   // conv_bn_relu `p` (ci -> co, 3x3) with its BatchNorm folded: w [9][ci][co], b [co]
   auto conv_bn = [&](const std::string& p, int ci, int co, float* w, float* b) {
-    const float* raw = R(p + "0.weight");
     const float* bn[4] = {R(p + "1.weight"), R(p + "1.bias"), R(p + "1.running_mean"), R(p + "1.running_var")};
-    float sc[16], sh[16];
-    bn_fold_host(bn, co, sc, sh);
-    for (int o = 0; o < co; ++o) {
-      b[o] = sh[o];
-      for (int i = 0; i < ci; ++i)
-        for (int tap = 0; tap < 9; ++tap)
-          w[(tap * ci + i) * co + o] = static_cast<float>(static_cast<double>(raw[(o * ci + i) * 9 + tap]) * sc[o]);
+    float sc[16];
+    bn_fold_host(bn, co, sc, b);
+    conv_taps(R(p + "0.weight"), ci, co, sc, w);
+  };
+  // ConvTranspose2d `t` (16 -> 16, 4x4) and the BatchNorm `p` after it, folded: w [ky][kx][ci][co], b [co]
+  auto convt_bn = [&](const std::string& t, const std::string& p, float* w, float* b) {
+    const float *bt = R(t + "bias"), *g = R(p + "weight"), *be = R(p + "bias"), *mu = R(p + "running_mean"),
+                *var = R(p + "running_var");
+    double sc[16];
+    for (int co = 0; co < 16; ++co) {
+      sc[co] = static_cast<double>(g[co]) / sqrt(static_cast<double>(var[co]) + 1e-5);
+      b[co] = static_cast<float>((static_cast<double>(bt[co]) - mu[co]) * sc[co] + be[co]);
     }
+    convt_taps(R(t + "weight"), sc, w);
   };
   const std::string E = "conv_transform.", D = "conv_inv_transform.";
   if (enc) {
-    float* x = sg->xenc;
+    float* x = sg->enc;
     if (kind == DD_CODEC_UP2_1X1) {
       const float *w1 = R(E + "0.weight"), *w2 = R(E + "1.weight");
       for (int co = 0; co < 16; ++co) {
@@ -1582,33 +1609,43 @@ void fold_kind(PackStage* sg, int kind, bool enc) {
     conv_bn(E + "0.", 1, 16, x + dd::CK_E4_W1, x + dd::CK_E4_B1);
     conv_bn(E + "1.", 16, 16, x + dd::CK_E4_W2, x + dd::CK_E4_B2);
     if (kind == DD_CODEC_UP4) conv_bn(E + "2.", 16, 16, x + dd::CK_E4_W3, x + dd::CK_E4_B3);
+    if (kind == DD_CODEC_UP2) {
+      conv_taps(R(E + "0.0.weight"), 1, 16, nullptr, x + kEncW1u);
+      conv_taps(R(E + "1.0.weight"), 16, 16, nullptr, x + kEncW2u);
+      const char* gb[4] = {"0.1.weight", "0.1.bias", "1.1.weight", "1.1.bias"};
+      for (int i = 0; i < 4; ++i) memcpy(x + kEncGb + 16 * i, R(E + gb[i]), 16 * 4);
+      bn_rstd(E + "0.1.", x + kEncBn);
+      bn_rstd(E + "1.1.", x + kEncBn + 48);
+    }
     return;
   }
-  float* x = sg->xdec;
+  float* x = sg->dec;
   if (kind == DD_CODEC_FULL) {
     conv_bn(D + "0.", 16, 16, x + dd::CK_DF_W1, x + dd::CK_DF_B1);
     conv_bn(D + "1.", 16, 1, x + dd::CK_DF_WC, x + dd::CK_DF_BC);
     for (int i = 1; i < 4; ++i) x[dd::CK_DF_BC + i] = 0.f;
     return;
   }
-  const float *t1 = R(D + "0.weight"), *b1 = R(D + "0.bias"), *t2 = R(D + "1.weight"), *b2 = R(D + "1.bias");
-  const float *g = R(D + "2.weight"), *be = R(D + "2.bias"), *mu = R(D + "2.running_mean"), *var = R(D + "2.running_var");
-  const float *wc = R(D + "4.0.weight"), *bc = R(D + "4.0.bias");
-  for (int co = 0; co < 16; ++co) {
-    const double sc = static_cast<double>(g[co]) / sqrt(static_cast<double>(var[co]) + 1e-5);
-    x[dd::CK_D4_B1 + co] = b1[co];
-    x[dd::CK_D4_B2 + co] = static_cast<float>((static_cast<double>(b2[co]) - mu[co]) * sc + be[co]);
-    for (int ci = 0; ci < 16; ++ci)
-      for (int k = 0; k < 16; ++k) {  // ConvTranspose2d weight layout: [Cin][Cout][kh][kw] -> [ky][kx][ci][co]
-        x[dd::CK_D4_T1 + (k * 16 + ci) * 16 + co] = t1[(ci * 16 + co) * 16 + k];
-        x[dd::CK_D4_T2 + (k * 16 + ci) * 16 + co] = static_cast<float>(static_cast<double>(t2[(ci * 16 + co) * 16 + k]) * sc);
-      }
+  if (kind == DD_CODEC_UP4) {
+    convt_taps(R(D + "0.weight"), nullptr, x + dd::CK_D4_T1);
+    memcpy(x + dd::CK_D4_B1, R(D + "0.bias"), 16 * 4);
+    convt_bn(D + "1.", D + "2.", x + dd::CK_D4_T2, x + dd::CK_D4_B2);
+    conv_taps(R(D + "4.0.weight"), 16, 1, nullptr, x + dd::CK_D4_WC);
+    x[dd::CK_D4_BC] = R(D + "4.0.bias")[0];
+    for (int i = 1; i < 4; ++i) x[dd::CK_D4_BC + i] = 0.f;
+    return;
   }
-  for (int ci = 0; ci < 16; ++ci)
-    for (int tap = 0; tap < 9; ++tap) x[dd::CK_D4_WC + tap * 16 + ci] = wc[ci * 9 + tap];
-  x[dd::CK_D4_BC] = bc[0];
-  for (int i = 1; i < 4; ++i) x[dd::CK_D4_BC + i] = 0.f;
+  convt_bn(D + "0.", D + "1.", x + kDecWt, x + kDecBt);
+  conv_taps(R(D + "3.0.weight"), 16, 1, nullptr, x + kDecWc);
+  convt_taps(R(D + "0.weight"), nullptr, x + kDecWu);
+  memcpy(x + kDecBu, R(D + "0.bias"), 16 * 4);
+  bn_rstd(D + "1.", x + kDecBn);
+  memcpy(x + kDecGb, R(D + "1.weight"), 16 * 4);
+  memcpy(x + kDecGb + 16, R(D + "1.bias"), 16 * 4);
 }
+// floats of codec kind `kind`'s encoder and decoder blocks
+size_t enc_block(int kind) { return kind == DD_CODEC_UP2 ? kEncN : dd::CK_E4_N; }
+size_t dec_block(int kind) { return kind <= DD_CODEC_UP2_1X1 ? kDecN : dd::CK_D4_N; }
 
 // `encoder`: the codec kind's encoder keys are registered (its pack is optional, as dd_encode is).
 int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
@@ -1641,15 +1678,21 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
     if ((rc = dev_array(h, &h->gn_beta[i], kGnCh[i]))) return rc;
   }
   if ((rc = dev_array(h, &h->temb, DD_TIME_ROWS * 256))) return rc;
-  if ((rc = dev_array(h, &h->dec_wt, 4 * 4 * 16 * 16))) return rc;
-  if ((rc = dev_array(h, &h->dec_bt, 16))) return rc;
-  if ((rc = dev_array(h, &h->dec_wc, 9 * 16))) return rc;
-  // the decoder backward and DD_CODEC_TRAIN need the BatchNorm unfolded
-  if ((rc = dev_array(h, &h->dec_wu, 4 * 4 * 16 * 16))) return rc;
-  if ((rc = dev_array(h, &h->dec_bu, 16))) return rc;
-  if ((rc = dev_array(h, &h->dec_bn, 3 * 16))) return rc;
+  const int kind = codec_kind(h->cfg);
+  h->xenc = nullptr;
+  if (encoder && (rc = dev_array(h, &h->xenc, enc_block(kind)))) return rc;
+  if ((rc = dev_array(h, &h->xdec, dec_block(kind)))) return rc;
   dd_engine::CodecTrain& ct = h->ct;
-  if ((rc = dev_array(h, &ct.dec_gb, 2 * 16))) return rc;
+  if (kind <= DD_CODEC_UP2_1X1) {  // the default decoder's block
+    float* x = h->xdec;
+    h->dec_wt = x + kDecWt;
+    h->dec_bt = x + kDecBt;
+    h->dec_wc = x + kDecWc;
+    h->dec_wu = x + kDecWu;
+    h->dec_bu = x + kDecBu;
+    h->dec_bn = x + kDecBn;
+    ct.dec_gb = x + kDecGb;
+  }
   if ((rc = dev_array(h, &ct.dec_wt, 4 * 4 * 16 * 16))) return rc;
   if ((rc = dev_array(h, &ct.dec_bt, 16))) return rc;
   if ((rc = dev_array(h, &ct.dec_bn, 3 * 16))) return rc;
@@ -1664,21 +1707,17 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
   if ((rc = dev_array(h, &ct.part_db, static_cast<size_t>(dec_act_blocks(g)) * 16))) return rc;
   if ((rc = dev_array(h, &ct.rec, static_cast<size_t>(std::max(h->cfg.num_inference_steps, 2)) * 32))) return rc;
   ct.nrec = 0;
-  const int kind = codec_kind(h->cfg);
-  h->xenc = h->xdec = nullptr;
-  if (kind != DD_CODEC_UP2 && encoder && (rc = dev_array(h, &h->xenc, dd::CK_E4_N))) return rc;
-  if (kind >= DD_CODEC_UP4 && (rc = dev_array(h, &h->xdec, dd::CK_D4_N))) return rc;
-  h->enc_w1 = nullptr;
-  if (encoder && kind == DD_CODEC_UP2) {
-    if ((rc = dev_array(h, &h->enc_w1, 144))) return rc;
-    if ((rc = dev_array(h, &h->enc_b1, 16))) return rc;
-    if ((rc = dev_array(h, &h->enc_w2, 2304))) return rc;
-    if ((rc = dev_array(h, &h->enc_b2, 16))) return rc;
-    if ((rc = dev_array(h, &h->enc_bn, 2 * 3 * 16))) return rc;
+  if (h->xenc && kind == DD_CODEC_UP2) {  // the default encoder's block, and the batch-folded copies
+    float* x = h->xenc;
+    h->enc_w1 = x + dd::CK_E4_W1;
+    h->enc_b1 = x + dd::CK_E4_B1;
+    h->enc_w2 = x + dd::CK_E4_W2;
+    h->enc_b2 = x + dd::CK_E4_B2;
+    h->enc_bn = x + kEncBn;
+    ct.enc_w1 = x + kEncW1u;
+    ct.enc_w2 = x + kEncW2u;
+    ct.enc_gb = x + kEncGb;
     if ((rc = dev_array(h, &ct.enc_bn, 2 * 3 * 16))) return rc;
-    if ((rc = dev_array(h, &ct.enc_w1, 144))) return rc;
-    if ((rc = dev_array(h, &ct.enc_w2, 2304))) return rc;
-    if ((rc = dev_array(h, &ct.enc_gb, 4 * 16))) return rc;
     if ((rc = dev_array(h, &ct.enc_w1f, 144))) return rc;
     if ((rc = dev_array(h, &ct.enc_b1f, 16))) return rc;
     if ((rc = dev_array(h, &ct.enc_w2f, 2304))) return rc;
@@ -1689,31 +1728,14 @@ int alloc_pack(dd_engine* h, bool encoder, cudaStream_t st) {
 
 // Every key registered for dd_update_weights belongs to the denoiser / codec pack and has the packed shape.
 int check_update(dd_engine* h) {
-  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
-  std::map<std::string, std::vector<int64_t>> want;
-  for (int i = 0; i < 6; ++i) {
-    if (!swin && (i == 2 || i == 3)) continue;
-    want[std::string(kConvKey[i]) + ".weight"] = {kConvCout[i], kConvCin[i], 3, 3};
-    want[std::string(kConvKey[i]) + ".bias"] = {kConvCout[i]};
-  }
-  for (int i = 0; i < 4; ++i) want[std::string(kGnKey[i]) + ".weight"] = want[std::string(kGnKey[i]) + ".bias"] = {kGnCh[i]};
-  want["model.time_embedding.weight"] = {DD_TIME_ROWS, 256};
-  const int kind = codec_kind(h->cfg);
-  if (kind <= DD_CODEC_UP2_1X1)
-    for (const CodecKey& k : kDecKeys) want[kDecPrefix + k.leaf] = k.shape;
-  if (h->enc_w1)
-    for (const CodecKey& k : kEncKeys) want[kEncPrefix + k.leaf] = k.shape;
-  for (bool enc : {true, false})
-    if (kind != DD_CODEC_UP2 && (!enc || h->xenc))
-      for (const KindKey& k : kind_keys(kind, enc)) want[k.name] = k.shape;
   for (const auto& kv : h->raw) {
     const std::string& name = kv.first;
     for (const char* p : {"hahineck.", "conv_lateral.", "conv_up.", "backbone."})
       if (name.compare(0, strlen(p), p) == 0)
         return fail(DD_ERR_UNSUPPORTED, name + ": the neck, FPN and backbone are re-packed by dd_finalize_weights only");
-    auto it = want.find(name);
-    if (it == want.end()) return fail(DD_ERR_INVALID, name + " is not part of this engine's pack");
-    if (kv.second.shape != it->second) return fail(DD_ERR_INVALID, name + ": shape differs from the packed tensor");
+    const PackKey* k = find_pack_key(codec_kind(h->cfg), name);
+    if (!k || !packs(h->cfg, *k, h->xenc != nullptr)) return fail(DD_ERR_INVALID, name + " is not part of this engine's pack");
+    if (kv.second.shape != k->shape) return fail(DD_ERR_INVALID, name + ": shape differs from the packed tensor");
   }
   return DD_OK;
 }
@@ -1727,7 +1749,7 @@ bool loop_reads_wscale(const dd_engine* e, int layer) { return !(fold_active(e) 
 int fill_pack(dd_engine* h, cudaStream_t st) {
   const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
   PackStage* sg = h->stage;
-  float* sg_f = reinterpret_cast<float*>(sg);
+  const PackTable& T = pack_table();
   auto W = [&](const std::string& k) -> const float* {
     const Raw* r = find(h, k);
     return r ? r->ptr : nullptr;
@@ -1741,8 +1763,8 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     if (!swin && (i == 2 || i == 3)) continue;
     const int co = kConvCout[i], ci = kConvCin[i];
     const int n = co * ci * 9;
-    w[i] = W(std::string(kConvKey[i]) + ".weight");
-    const float* b = W(std::string(kConvKey[i]) + ".bias");
+    w[i] = W(T.keys[T.conv[i]].name);
+    const float* b = W(T.keys[T.conv[i] + 1].name);
     if (b) CUDA_TRY(cudaMemcpyAsync(h->L[i].bias, b, co * 4, cudaMemcpyDeviceToDevice, st));
     if (w[i]) {
       dd::absmax_kernel<<<absmax_grid(n), 256, 0, st>>>(w[i], n, h->amax + i);
@@ -1769,31 +1791,20 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     if ((rc = check_launch("absmax"))) return rc;
   }
   for (int i = 0; i < 4; ++i) {
-    if (const float* g = W(std::string(kGnKey[i]) + ".weight"))
+    if (const float* g = W(T.keys[T.gn[i]].name))
       CUDA_TRY(cudaMemcpyAsync(h->gn_gamma[i], g, kGnCh[i] * 4, cudaMemcpyDeviceToDevice, st));
-    if (const float* b = W(std::string(kGnKey[i]) + ".bias"))
+    if (const float* b = W(T.keys[T.gn[i] + 1].name))
       CUDA_TRY(cudaMemcpyAsync(h->gn_beta[i], b, kGnCh[i] * 4, cudaMemcpyDeviceToDevice, st));
   }
   if (const float* t = W("model.time_embedding.weight"))
     CUDA_TRY(cudaMemcpyAsync(h->temb, t, DD_TIME_ROWS * 256 * 4, cudaMemcpyDeviceToDevice, st));
   const int kind = codec_kind(h->cfg);
-  bool dec = false, enc = false, xenc = false, xdec = false;
-  for (bool e : {true, false})
-    for (const KindKey& k : kind_keys(kind, e))
+  bool enc = false, dec = false;
+  for (const PackKey& k : T.keys)
+    if (k.group >= PK_ENC && in_kind(k, kind))
       if (const float* p = W(k.name)) {
-        CUDA_TRY(cudaMemcpyAsync(sg->xraw + k.off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
-        (e ? xenc : xdec) = true;
-      }
-  for (const CodecKey& k : kDecKeys)
-    if (const float* p = kind <= DD_CODEC_UP2_1X1 ? W(kDecPrefix + k.leaf) : nullptr) {
-      CUDA_TRY(cudaMemcpyAsync(sg_f + k.host_off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
-      dec = true;
-    }
-  if (h->enc_w1)
-    for (const CodecKey& k : kEncKeys)
-      if (const float* p = W(kEncPrefix + k.leaf)) {
-        CUDA_TRY(cudaMemcpyAsync(sg_f + k.host_off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
-        enc = true;
+        CUDA_TRY(cudaMemcpyAsync(sg->raw() + k.off, p, numel(k.shape) * 4, cudaMemcpyDeviceToHost, st));
+        (k.group == PK_ENC ? enc : dec) = true;
       }
   CUDA_TRY(cudaMemcpyAsync(sg->amax, h->amax, 16 * 4, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -1824,84 +1835,18 @@ int fill_pack(dd_engine* h, cudaStream_t st) {
     dd::pack_fold_kernel<<<256, 256, 0, st>>>(h->fold.k5, h->fold.w, static_cast<double>(h->fold.wscale));
     if ((rc = check_launch("pack_fold"))) return rc;
   }
-  if (dec) {  // fold eval-BN into the transposed conv (tiny: on the host in fp64)
-    for (int co = 0; co < 16; ++co) {
-      const double sc = static_cast<double>(sg->dec_g[co]) / sqrt(static_cast<double>(sg->dec_var[co]) + 1e-5);
-      sg->bt_f[co] = static_cast<float>((static_cast<double>(sg->dec_bt[co]) - sg->dec_mu[co]) * sc + sg->dec_be[co]);
-      for (int ci = 0; ci < 16; ++ci)
-        for (int ky = 0; ky < 4; ++ky)
-          for (int kx = 0; kx < 4; ++kx)  // ConvTranspose2d weight layout: [Cin][Cout][kh][kw]
-            sg->wt_f[((ky * 4 + kx) * 16 + ci) * 16 + co] =
-                static_cast<float>(static_cast<double>(sg->dec_wt[((ci * 16 + co) * 4 + ky) * 4 + kx]) * sc);
+  if (dec) {  // every decoder reads its constants from this block but the default one's final bias, a kernel argument
+    fold_codec(sg, kind, false);
+    CUDA_TRY(cudaMemcpyAsync(h->xdec, sg->dec, dec_block(kind) * 4, cudaMemcpyHostToDevice, st));
+    if (kind <= DD_CODEC_UP2_1X1) {
+      const float bc = sg->raw()[find_pack_key(kind, "depth_transform.conv_inv_transform.3.0.bias")->off];
+      steps_stale |= bc != h->dec_bc;
+      h->dec_bc = bc;
     }
-    for (int ci = 0; ci < 16; ++ci)
-      for (int tap = 0; tap < 9; ++tap) sg->wc_f[tap * 16 + ci] = sg->dec_wc[ci * 9 + tap];
-    CUDA_TRY(cudaMemcpyAsync(h->dec_wt, sg->wt_f, sizeof(sg->wt_f), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->dec_bt, sg->bt_f, sizeof(sg->bt_f), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->dec_wc, sg->wc_f, sizeof(sg->wc_f), cudaMemcpyHostToDevice, st));
-    steps_stale |= sg->dec_bc[0] != h->dec_bc;
-    h->dec_bc = sg->dec_bc[0];
-    for (int co = 0; co < 16; ++co) {  // unfolded: the decoder backward and DD_CODEC_TRAIN
-      const double rstd = 1.0 / sqrt(static_cast<double>(sg->dec_var[co]) + 1e-5);
-      sg->bn[co] = static_cast<float>(static_cast<double>(sg->dec_g[co]) * rstd);
-      sg->bn[16 + co] = sg->dec_mu[co];
-      sg->bn[32 + co] = static_cast<float>(rstd);
-      for (int ci = 0; ci < 16; ++ci)
-        for (int k = 0; k < 16; ++k) sg->wu[(k * 16 + ci) * 16 + co] = sg->dec_wt[(ci * 16 + co) * 16 + k];
-    }
-    CUDA_TRY(cudaMemcpyAsync(h->dec_wu, sg->wu, sizeof(sg->wu), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->dec_bu, sg->dec_bt, sizeof(sg->dec_bt), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->dec_bn, sg->bn, sizeof(sg->bn), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->ct.dec_gb, sg->dec_g, 16 * 4, cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->ct.dec_gb + 16, sg->dec_be, 16 * 4, cudaMemcpyHostToDevice, st));
   }
   if (enc) {
-    float s1[16], s2[16];
-    const float* bn1[4] = {sg->enc_bn1[0], sg->enc_bn1[1], sg->enc_bn1[2], sg->enc_bn1[3]};
-    const float* bn2[4] = {sg->enc_bn2[0], sg->enc_bn2[1], sg->enc_bn2[2], sg->enc_bn2[3]};
-    bn_fold_host(bn1, 16, s1, sg->t1);
-    bn_fold_host(bn2, 16, s2, sg->t2);
-    for (int co = 0; co < 16; ++co)
-      for (int tap = 0; tap < 9; ++tap)
-        sg->f1[tap * 16 + co] = static_cast<float>(static_cast<double>(sg->enc_w1[co * 9 + tap]) * s1[co]);
-    for (int co = 0; co < 16; ++co)
-      for (int ci = 0; ci < 16; ++ci)
-        for (int tap = 0; tap < 9; ++tap)
-          sg->f2[(tap * 16 + ci) * 16 + co] =
-              static_cast<float>(static_cast<double>(sg->enc_w2[(co * 16 + ci) * 9 + tap]) * s2[co]);
-    CUDA_TRY(cudaMemcpyAsync(h->enc_w1, sg->f1, sizeof(sg->f1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_b1, sg->t1, sizeof(sg->t1), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_w2, sg->f2, sizeof(sg->f2), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_b2, sg->t2, sizeof(sg->t2), cudaMemcpyHostToDevice, st));
-    for (int co = 0; co < 16; ++co) {  // unfolded, for DD_CODEC_TRAIN
-      for (int tap = 0; tap < 9; ++tap) {
-        sg->e1u[tap * 16 + co] = sg->enc_w1[co * 9 + tap];
-        for (int ci = 0; ci < 16; ++ci) sg->e2u[(tap * 16 + ci) * 16 + co] = sg->enc_w2[(co * 16 + ci) * 9 + tap];
-      }
-      sg->enc_gb[0][co] = sg->enc_bn1[0][co];
-      sg->enc_gb[1][co] = sg->enc_bn1[1][co];
-      sg->enc_gb[2][co] = sg->enc_bn2[0][co];
-      sg->enc_gb[3][co] = sg->enc_bn2[1][co];
-      for (int k = 0; k < 2; ++k) {  // the backward's eval BatchNorms, as dec_bn
-        const float(*bn)[16] = k == 0 ? sg->enc_bn1 : sg->enc_bn2;  // weight, bias, running_mean, running_var
-        const double rstd = 1.0 / sqrt(static_cast<double>(bn[3][co]) + 1e-5);
-        sg->enc_bn[k][0][co] = static_cast<float>(static_cast<double>(bn[0][co]) * rstd);
-        sg->enc_bn[k][1][co] = bn[2][co];
-        sg->enc_bn[k][2][co] = static_cast<float>(rstd);
-      }
-    }
-    CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w1, sg->e1u, sizeof(sg->e1u), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->ct.enc_w2, sg->e2u, sizeof(sg->e2u), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->ct.enc_gb, sg->enc_gb, sizeof(sg->enc_gb), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(h->enc_bn, sg->enc_bn, sizeof(sg->enc_bn), cudaMemcpyHostToDevice, st));
-  }
-  if (xenc) {
-    fold_kind(sg, kind, true);
-    CUDA_TRY(cudaMemcpyAsync(h->xenc, sg->xenc, sizeof(sg->xenc), cudaMemcpyHostToDevice, st));
-  }
-  if (xdec) {  // the UP4 / FULL decoders read every constant from this block, so no graph holds one by value
-    fold_kind(sg, kind, false);
-    CUDA_TRY(cudaMemcpyAsync(h->xdec, sg->xdec, sizeof(sg->xdec), cudaMemcpyHostToDevice, st));
+    fold_codec(sg, kind, true);
+    CUDA_TRY(cudaMemcpyAsync(h->xenc, sg->enc, enc_block(kind) * 4, cudaMemcpyHostToDevice, st));
   }
   CUDA_TRY(cudaEventRecord(h->pack_done, st));
   if (loop_stale) drop_graph(h, dd_engine::G_LOOP);
@@ -2937,8 +2882,6 @@ int run_decode_bwd(dd_engine* e, const float* d_depth, float* dx, float* const* 
   return launched(e, "dec_bwd_finish");
 }
 
-constexpr size_t kDecGradNumel[6] = {16 * 16 * 4 * 4, 16, 16, 16, 16 * 9, 1};
-
 // Checks of an entry that recomputes one denoiser call on the backward's region (dd_denoiser_backward,
 // dd_denoiser_relu_inputs), after its own null-pointer checks.
 int check_operator_bwd_call(const dd_engine* h, const char* entry) {
@@ -3089,7 +3032,6 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
     return fail(DD_ERR_INVALID, "bad geometry");
   if (cfg->variant == DD_VARIANT_RES && (cfg->cond_h != cfg->latent_h || cfg->cond_w != cfg->latent_w))
     return fail(DD_ERR_INVALID, "Res variant needs the condition map at latent resolution");
-  if (!kind_keys_fit()) return fail(DD_ERR_INVALID, "codec key tables exceed the pack's host staging buffer");
   if (codec_kind(*cfg) != DD_CODEC_UP2 && (cfg->flags & DD_FLAG_LOOP_BACKWARD))
     return fail(DD_ERR_UNSUPPORTED, std::string("DD_FLAG_LOOP_BACKWARD: the loop backward differentiates through the "
                                                 "DeepDepthTransformWithUpsampling decoder only, not ") +
@@ -3109,7 +3051,7 @@ int dd_create(const dd_config* cfg, dd_handle* out) {
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
   if (cudaMallocHost(&e->status_host, 64) != cudaSuccess ||
-      cudaMallocHost(&e->stage, sizeof(PackStage)) != cudaSuccess ||
+      cudaMallocHost(&e->stage, sizeof(PackStage) + pack_table().raw_floats * 4) != cudaSuccess ||
       cudaEventCreateWithFlags(&e->pack_done, cudaEventDisableTiming) != cudaSuccess ||
       cudaStreamCreateWithFlags(&e->cap_stream, cudaStreamNonBlocking) != cudaSuccess ||
       configure_all_kernels() != cudaSuccess) {
@@ -3126,30 +3068,13 @@ int dd_destroy(dd_handle h) {
   return DD_OK;
 }
 
-static const char* kKeys[] = {
-    "model.noise_embedding.0.weight", "model.noise_embedding.0.bias", "model.noise_embedding.1.weight",
-    "model.noise_embedding.1.bias", "model.noise_embedding.3.weight", "model.noise_embedding.3.bias",
-    "model.noise_embedding.4.weight", "model.noise_embedding.4.bias", "model.upsample_fuse.convA.conv.weight",
-    "model.upsample_fuse.convA.conv.bias", "model.upsample_fuse.convB.conv.weight",
-    "model.upsample_fuse.convB.conv.bias", "model.time_embedding.weight", "model.pred.0.weight", "model.pred.0.bias",
-    "model.pred.1.weight", "model.pred.1.bias", "model.pred.3.weight", "model.pred.3.bias", "model.pred.4.weight",
-    "model.pred.4.bias", "depth_transform.conv_inv_transform.0.weight", "depth_transform.conv_inv_transform.0.bias",
-    "depth_transform.conv_inv_transform.1.weight", "depth_transform.conv_inv_transform.1.bias",
-    "depth_transform.conv_inv_transform.1.running_mean", "depth_transform.conv_inv_transform.1.running_var",
-    "depth_transform.conv_inv_transform.3.0.weight", "depth_transform.conv_inv_transform.3.0.bias"};
-
 int dd_set_weight(dd_handle h, const char* name, const float* dev_ptr, const int64_t* shape, int32_t ndim) {
   if (!h || !name || !dev_ptr || ndim < 0 || ndim > 4) return fail(DD_ERR_INVALID, "bad argument");
-  bool known = strncmp(name, "hahineck.", 9) == 0 || strncmp(name, "conv_lateral.", 13) == 0 ||
-               strncmp(name, "conv_up.", 8) == 0 ||  // step-invariant producers (optional, dd_enable_producers)
-               strncmp(name, "backbone.", 9) == 0;  // native backbone (optional, dd_enable_backbone)
   const int kind = codec_kind(h->cfg);
-  // the codec's keys: the default encoder t() (optional, dd_encode) and decoder, or those of this engine's codec kind
-  // (UP2_1X1 keeps the default decoder)
-  known |= kind == DD_CODEC_UP2 && strncmp(name, "depth_transform.conv_transform.", 31) == 0;
-  for (const char* k : kKeys)
-    known |= strcmp(k, name) == 0 && (kind <= DD_CODEC_UP2_1X1 || strncmp(k, "depth_transform.", 16) != 0);
-  known |= find_kind_key(kind, name) != nullptr;
+  const bool known = strncmp(name, "hahineck.", 9) == 0 || strncmp(name, "conv_lateral.", 13) == 0 ||
+                     strncmp(name, "conv_up.", 8) == 0 ||  // step-invariant producers (optional, dd_enable_producers)
+                     strncmp(name, "backbone.", 9) == 0 ||  // native backbone (optional, dd_enable_backbone)
+                     find_pack_key(kind, name) != nullptr;
   if (!known)
     return fail(DD_ERR_INVALID, std::string("unknown weight key: ") + name +
                                     (strncmp(name, "depth_transform.", 16) == 0 ? std::string(" (codec ") + codec_name(kind) + ")" : ""));
@@ -3165,43 +3090,18 @@ int dd_finalize_weights(dd_handle h, void* cuda_stream) {
   if (!h) return fail(DD_ERR_INVALID, "null handle");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   CUDA_TRY(cudaSetDevice(h->cfg.device));
-  const bool swin = h->cfg.variant == DD_VARIANT_SWIN;
+  // the encoder is optional (dd_encode), and all or nothing
   const int kind = codec_kind(h->cfg);
-  const bool default_dec = kind <= DD_CODEC_UP2_1X1;
+  bool encoder = false;
+  for (const PackKey& k : pack_table().keys) encoder |= k.group == PK_ENC && in_kind(k, kind) && find(h, k.name);
   std::string missing;
-  for (const char* k : kKeys) {
-    if (!swin && strstr(k, "upsample_fuse")) continue;
-    if (!default_dec && strncmp(k, "depth_transform.", 16) == 0) continue;
-    if (!find(h, k)) missing += std::string(missing.empty() ? "" : ", ") + k;
-  }
-  for (const KindKey& k : kind_keys(kind, false))
-    if (!find(h, k.name)) missing += (missing.empty() ? "" : ", ") + k.name;
+  for (const PackKey& k : pack_table().keys)
+    if (packs(h->cfg, k, encoder) && !find(h, k.name)) missing += (missing.empty() ? "" : ", ") + k.name;
   if (!missing.empty()) return fail(DD_ERR_INVALID, "missing weights: " + missing);
-  auto expect = [&](const char* k, std::vector<int64_t> s) { return find(h, k)->shape == s; };
-  if (!expect("model.noise_embedding.0.weight", {64, 16, 3, 3}) || !expect("model.noise_embedding.3.weight", {256, 64, 3, 3}) ||
-      !expect("model.pred.0.weight", {64, 256, 3, 3}) || !expect("model.pred.3.weight", {16, 64, 3, 3}) ||
-      !expect("model.time_embedding.weight", {DD_TIME_ROWS, 256}) ||
-      (default_dec && (!expect("depth_transform.conv_inv_transform.0.weight", {16, 16, 4, 4}) ||
-                       !expect("depth_transform.conv_inv_transform.3.0.weight", {1, 16, 3, 3}))) ||
-      (swin && (!expect("model.upsample_fuse.convA.conv.weight", {256, 256, 3, 3}) ||
-                !expect("model.upsample_fuse.convB.conv.weight", {256, 256, 3, 3}))))
-    return fail(DD_ERR_INVALID, "weight shape mismatch with the reference architecture");
-  bool encoder = kind == DD_CODEC_UP2 && find(h, kEncPrefix + "0.0.weight") != nullptr;
-  for (const KindKey& k : kind_keys(kind, true)) encoder |= find(h, k.name) != nullptr;
-  for (bool enc : {true, false})  // the codec kind's keys: all of the encoder's when one is registered, shapes
-    for (const KindKey& k : kind_keys(kind, enc)) {
-      if (enc && !encoder) break;
-      const Raw* r = find(h, k.name);
-      if (!r) return fail(DD_ERR_INVALID, "missing weights: " + k.name);
-      if (r->shape != k.shape) return fail(DD_ERR_INVALID, k.name + ": weight shape mismatch with " + codec_name(kind));
-    }
-  if (encoder && kind == DD_CODEC_UP2) {
-    const Raw *w1 = find(h, kEncPrefix + "0.0.weight"), *w2 = find(h, kEncPrefix + "1.0.weight");
-    if (!w2 || w1->shape != std::vector<int64_t>{16, 1, 3, 3} || w2->shape != std::vector<int64_t>{16, 16, 3, 3})
-      return fail(DD_ERR_INVALID, "encoder weights missing / wrong shape");
-    for (const CodecKey& k : kEncKeys)
-      if (!find(h, kEncPrefix + k.leaf)) return fail(DD_ERR_INVALID, "missing weights: " + kEncPrefix + k.leaf);
-  }
+  for (const PackKey& k : pack_table().keys)
+    if (packs(h->cfg, k, encoder) && find(h, k.name)->shape != k.shape)
+      return fail(DD_ERR_INVALID, k.name + ": weight shape mismatch with the reference architecture (" +
+                                      codec_name(kind) + ")");
   // drop any previous pack
   drop_graphs(h);
   h->packed = false;
@@ -3530,9 +3430,11 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
     if ((rc = run_decode_bwd(h, d_depth, h->bw.g[1], d_dec_params, st))) return rc;
     dd::latent_grad_step_kernel<<<grid_of(nx), 256, 0, st>>>(l.gl, h->bw.g[1], nullptr, 1.f, nx);
     if ((rc = launched(h, "latent_grad_step"))) return rc;
-  } else if (d_dec_params) {  // the depth does not enter the loss: zero decoder gradients
-    for (int i = 0; i < 6; ++i)
-      if (d_dec_params[i]) CUDA_TRY(cudaMemsetAsync(d_dec_params[i], 0, kDecGradNumel[i] * 4, st));
+  } else if (d_dec_params) {  // the depth does not enter the loss: zero decoder gradients (DECODER_PARAM_KEYS)
+    int i = 0;
+    for (const PackKey& k : pack_table().keys)
+      if (k.group == PK_DEC && in_kind(k, DD_CODEC_UP2) && k.name.find(".running_") == std::string::npos)
+        if (float* d = d_dec_params[i++]) CUDA_TRY(cudaMemsetAsync(d, 0, numel(k.shape) * 4, st));
   }
   // 3. walk back: step s maps x_s -> x_{s+1} = c_x x_s + c_eps eps(x_s)
   float* P[21] = {};
@@ -3558,7 +3460,7 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
       return rc;
     for (int i = 0; i < npar; ++i) {
       if (!P[i]) continue;
-      dd::acc_add_kernel<<<grid_of(kParamNumel[i]), 256, 0, st>>>(l.acc + param_offset(i), P[i], nullptr, kParamNumel[i]);
+      dd::acc_add_kernel<<<grid_of(param_numel(i)), 256, 0, st>>>(l.acc + param_offset(i), P[i], nullptr, param_numel(i));
       if ((rc = launched(h, "acc_add"))) return rc;
     }
     if (want_dtemb) {
@@ -3574,7 +3476,7 @@ int dd_denoise_backward(dd_handle h, const float* cond, const float* noise, cons
   if (d_noise_out && (rc = transpose_out(l.gl, d_noise_out, g.B, 16, g.P, st))) return rc;
   for (int i = 0; i < npar && d_params; ++i) {
     if (!d_params[i]) continue;
-    dd::acc_store_kernel<<<grid_of(kParamNumel[i]), 256, 0, st>>>(l.acc + param_offset(i), d_params[i], kParamNumel[i]);
+    dd::acc_store_kernel<<<grid_of(param_numel(i)), 256, 0, st>>>(l.acc + param_offset(i), d_params[i], param_numel(i));
     if ((rc = launched(h, "acc_store"))) return rc;
   }
   if (d_cond_out) {  // fp32 NHWC in a backward buffer of at least that size, then NCHW
@@ -4006,9 +3908,6 @@ int dd_bench_gemm(dd_handle h, int32_t M, int32_t K, int32_t N, int32_t mode, in
 // dd_encode for the codec kinds other than DD_CODEC_UP2 (eval BatchNorm only: dd_set_codec_mode refuses DD_CODEC_TRAIN)
 static int encode_kind(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, cudaStream_t st) {
   const int kind = codec_kind(h->cfg);
-  if (!h->weights_ready || !h->xenc)
-    return fail(DD_ERR_INVALID, std::string("encoder weights (depth_transform.conv_transform.* of ") + codec_name(kind) +
-                                    ") not registered");
   if (codec_latent(kind, height) != h->cfg.latent_h || codec_latent(kind, width) != h->cfg.latent_w)
     return fail(DD_ERR_INVALID, "depth map size " + std::to_string(height) + " x " + std::to_string(width) +
                                     " does not match the engine's latent grid under " + codec_name(kind));
@@ -4039,9 +3938,11 @@ static int encode_kind(dd_handle h, const float* depth, int32_t height, int32_t 
 
 int dd_encode(dd_handle h, const float* depth, int32_t height, int32_t width, float* latent_out, void* cuda_stream) {
   if (!h || !depth || !latent_out) return fail(DD_ERR_INVALID, "null argument");
+  if (!h->weights_ready || !h->xenc)
+    return fail(DD_ERR_INVALID, std::string("encoder weights (depth_transform.conv_transform.* of ") +
+                                    codec_name(codec_kind(h->cfg)) + ") not registered");
   if (codec_kind(h->cfg) != DD_CODEC_UP2)
     return encode_kind(h, depth, height, width, latent_out, static_cast<cudaStream_t>(cuda_stream));
-  if (!h->weights_ready || !h->enc_w1) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
   if ((height + 1) / 2 != h->cfg.latent_h || (width + 1) / 2 != h->cfg.latent_w)
     return fail(DD_ERR_INVALID, "depth map size does not match the engine's latent grid");
   const bool train = h->codec_mode == DD_CODEC_TRAIN;
@@ -4164,7 +4065,7 @@ int dd_encode_backward(dd_handle h, const float* depth, int32_t height, int32_t 
     return fail(DD_ERR_UNSUPPORTED, std::string("dd_encode_backward: no encoder backward for ") + codec_name(codec_kind(h->cfg)));
   int rc;
   if ((rc = check_operator_bwd_call(h, "dd_encode_backward"))) return rc;
-  if (!h->enc_w1) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
+  if (!h->xenc) return fail(DD_ERR_INVALID, "encoder weights (depth_transform.conv_transform.*) not registered");
   if ((height + 1) / 2 != h->cfg.latent_h || (width + 1) / 2 != h->cfg.latent_w)
     return fail(DD_ERR_INVALID, "depth map size does not match the engine's latent grid");
   if (h->codec_mode == DD_CODEC_TRAIN && static_cast<long long>(h->cfg.batch) * h->cfg.latent_h * h->cfg.latent_w < 2)

@@ -114,7 +114,7 @@ enum dd_flags {
  *   DD_CODEC_UP4      DeepDepthTransformWithUpsamplingX4 (:67-94)   latent ceil(ceil(H/2)/2) (each side),   u = 4
  *   DD_CODEC_FULL     DeepDepthTransform (:97-117)                  latent H x W,                           u = 1
  * dd_set_weight takes the kind's `depth_transform.*` keys and rejects the other kinds'; dd_finalize_weights needs the
- * decoder's, the encoder's stay optional.  Kinds other than DD_CODEC_UP2 run with eval-mode BatchNorm only: they
+ * decoder's, the encoder's stay optional (all of them or none).  Kinds other than DD_CODEC_UP2 run with eval-mode BatchNorm only: they
  * answer dd_set_codec_mode(DD_CODEC_TRAIN), dd_encode_backward and dd_decode_backward with DD_ERR_UNSUPPORTED, and
  * dd_create refuses them with DD_FLAG_LOOP_BACKWARD.  dd_denoiser_forward / dd_denoiser_backward do not involve the
  * codec. */
@@ -153,7 +153,8 @@ int dd_destroy(dd_handle h);
 int dd_set_weight(dd_handle h, const char* name, const float* dev_ptr, const int64_t* shape, int32_t ndim);
 
 /* Pre-pack: fold eval-BatchNorm into the decoder, repack conv weights tap-major, split them into
- * scaled fp16 hi/lo planes for the 3-pass tensor-core product.  Fails listing any missing key. */
+ * scaled fp16 hi/lo planes for the 3-pass tensor-core product.  Fails listing any missing key, and on any key of the
+ * denoiser or codec whose shape is not the reference's (DD_ERR_INVALID). */
 int dd_finalize_weights(dd_handle h, void* cuda_stream);
 
 /* After an optimizer step: re-pack, in place, what depends on the tensors registered with dd_set_weight since the
